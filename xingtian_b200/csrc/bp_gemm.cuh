@@ -107,20 +107,28 @@ __device__ __forceinline__ void fence_regs(float* d) {
 #pragma unroll
   for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+// emits nothing: tells the compiler the accumulators' old values are dead before a scale-d 0 wgmma overwrites them (its
+// "+f" operands would otherwise keep them live, e.g. through the epilogue that reads them last)
+template <int R>
+__device__ __forceinline__ void discard_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "=f"(d[i]));
+}
 
 // D[64 x n] (+)= A[64 x 16] B[16 x n], bf16 operands from shared memory, fp32 accumulators d[n / 2] in the wgmma
-// register layout; TA / TB = 1: operand is MN-major ("transposed").  Always accumulates: callers zero d first.
+// register layout; TA / TB = 1: operand is MN-major ("transposed").  scale_d = 1: D += A B; scale_d = 0: D = A B, which
+// starts an accumulator without register writes between wgmma instructions (those make ptxas serialize them, C7515).
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n16(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]),
         "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
@@ -128,10 +136,10 @@ __device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b) {
         "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
         "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n48(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n48(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
@@ -141,10 +149,10 @@ __device__ __forceinline__ void wgmma_n48(float* d, uint64_t a, uint64_t b) {
         "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
         "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
@@ -156,10 +164,10 @@ __device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b) {
         "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
         "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n96(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n96(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n\t}"
@@ -175,10 +183,10 @@ __device__ __forceinline__ void wgmma_n96(float* d, uint64_t a, uint64_t b) {
         "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]),
         "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n128(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
@@ -198,17 +206,17 @@ __device__ __forceinline__ void wgmma_n128(float* d, uint64_t a, uint64_t b) {
         "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
         "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+      : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 template <int N, int TA, int TB>
-__device__ __forceinline__ void wgmma(float* d, uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma(float* d, uint64_t a, uint64_t b, uint32_t scale_d = 1) {
   static_assert(N == 16 || N == 32 || N == 48 || N == 64 || N == 96 || N == 128, "wgmma width");
-  if constexpr (N == 16) wgmma_n16<TA, TB>(d, a, b);
-  else if constexpr (N == 32) wgmma_n32<TA, TB>(d, a, b);
-  else if constexpr (N == 48) wgmma_n48<TA, TB>(d, a, b);
-  else if constexpr (N == 64) wgmma_n64<TA, TB>(d, a, b);
-  else if constexpr (N == 96) wgmma_n96<TA, TB>(d, a, b);
-  else wgmma_n128<TA, TB>(d, a, b);
+  if constexpr (N == 16) wgmma_n16<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_n32<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 48) wgmma_n48<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 64) wgmma_n64<TA, TB>(d, a, b, scale_d);
+  else if constexpr (N == 96) wgmma_n96<TA, TB>(d, a, b, scale_d);
+  else wgmma_n128<TA, TB>(d, a, b, scale_d);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
@@ -441,7 +449,6 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
     // ================= consumers: wgmma on the ring stages, epilogue from the accumulator registers =================
     constexpr int ACC = CAT ? 2 * N : N;                 // accumulator columns
     constexpr int NCH = N >> 3;                          // output feature chunks of a tile
-    float acc[ACC / 2];
     float dbacc[N / 4];                                  // data gradient: column sums of this thread's columns
 #pragma unroll
     for (int j = 0; j < N / 4; j++) dbacc[j] = 0.f;
@@ -473,69 +480,84 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
     const uint64_t b_const = w_res ? wdesc : bdesc;
     if (w_res) mbar_wait(wbar, 0);
     int stage = 0; uint32_t phase = 0;
+    int held = -1;                                       // ring slot whose wgmma group may still be reading
+    // this warpgroup's 64 rows of batch tile bt all lie at or beyond B: no MMAs and no epilogue for that tile
+    auto idle = [&](int bt) { return bt * 128 + wg * 64 >= Bsz; };
+
+    // One K stage into accumulator bank acc; the first stage of a tile starts the bank with scale-d 0.  Every value that
+    // steers a branch or a trip count between wgmma_fence and wgmma_wait must be provably warp-uniform (kernel
+    // parameters, shuffle results and what derives from them): ptxas otherwise serializes the wgmma instructions (C7520),
+    // one MMA in flight at a time.  An idle warpgroup still waits on the full barrier and frees the slot, so the producer
+    // protocol does not change.
+    auto mma_stage = [&](float* acc, const StageDesc& d, bool first, bool skip) {
+      mbar_wait(full0 + 8 * stage, phase);
+      const uint32_t sA = stage0 + (uint32_t)stage * stage_bytes;
+      uint32_t a_lo32 = (sA >> 4) + a_row_add;
+      uint32_t b_lo32 = w_res ? (wres + d.w_off) >> 4 : (sA + RW_STAGE_A) >> 4;
+      const int ksteps = __shfl_sync(0xffffffffu, skip ? 0 : (int)d.nch >> 1, 0);
+      uint32_t sd = first ? 0u : 1u;
+      wgmma_fence();
+      // the a_split test stays outside the issue loops: a branch between wgmma instructions makes ptxas serialize them
+      if (a_split) {
+        for (int j = 0; j < ksteps; j++) {
+          const uint64_t ah = adesc | a_lo32, bh = b_const | b_lo32, al = adesc | (a_lo32 + a_lo_add);
+          if (KIND != 2) {
+            wgmma<2 * N, 0, 1>(acc, ah, bh, sd);                                   // A_hi x [W_hi | W_lo]
+            wgmma<N, 0, 1>(acc, al, bh);                                           // A_lo x W_hi
+          } else {
+            wgmma<N, 0, 0>(acc, ah, bh, sd);
+            wgmma<N, 0, 0>(acc, ah, b_const | (b_lo32 + b_lo_add));
+            wgmma<N, 0, 0>(acc, al, bh);
+          }
+          a_lo32 += a_step; b_lo32 += b_step; sd = 1u;
+        }
+      } else {
+        for (int j = 0; j < ksteps; j++) {
+          const uint64_t ah = adesc | a_lo32, bh = b_const | b_lo32;
+          if (KIND != 2) {
+            wgmma<2 * N, 0, 1>(acc, ah, bh, sd);
+          } else {
+            wgmma<N, 0, 0>(acc, ah, bh, sd);
+            wgmma<N, 0, 0>(acc, ah, b_const | (b_lo32 + b_lo_add));
+          }
+          a_lo32 += a_step; b_lo32 += b_step; sd = 1u;
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                   // all earlier groups are complete: free the slot they read
+      if (held >= 0 && lane == 0) mbar_arrive(empty0 + 8 * held);
+      held = stage;
+      if (++stage == n_stages) { stage = 0; phase ^= 1; }
+    };
+
+    int tile = blockIdx.x;
     int u = (int)blockIdx.x / nbt, bt = (int)blockIdx.x - u * nbt;
     TileWalk tw; tw.setup(a, stages_sm, units_sm);
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    // issue the first stage of tile (u, bt) into bank acc; false if the unit has no stages
+    auto start_tile = [&](float* acc) {
       tw.init<KIND>(u);
-#pragma unroll
-      for (int j = 0; j < ACC / 2; j++) acc[j] = 0.f;
-      int held = -1;                                     // ring slot whose wgmma group may still be reading
-      for (int s = 0; s < tw.ns; s++) {
-        const StageDesc d = tw.get(s);
-        mbar_wait(full0 + 8 * stage, phase);
-        const uint32_t sA = stage0 + (uint32_t)stage * stage_bytes;
-        uint32_t a_lo32 = (sA >> 4) + a_row_add;
-        uint32_t b_lo32 = w_res ? (wres + d.w_off) >> 4 : (sA + RW_STAGE_A) >> 4;
-        const int ksteps = (int)d.nch >> 1;
-        wgmma_fence();
-        // the a_split test stays outside the issue loops: a branch between wgmma instructions makes ptxas serialize them
-        if (a_split) {
-          for (int j = 0; j < ksteps; j++) {
-            const uint64_t ah = adesc | a_lo32, bh = b_const | b_lo32, al = adesc | (a_lo32 + a_lo_add);
-            if (KIND != 2) {
-              wgmma<2 * N, 0, 1>(acc, ah, bh);                                       // A_hi x [W_hi | W_lo]
-              wgmma<N, 0, 1>(acc, al, bh);                                           // A_lo x W_hi
-            } else {
-              wgmma<N, 0, 0>(acc, ah, bh);
-              wgmma<N, 0, 0>(acc, ah, b_const | (b_lo32 + b_lo_add));
-              wgmma<N, 0, 0>(acc, al, bh);
-            }
-            a_lo32 += a_step; b_lo32 += b_step;
-          }
-        } else {
-          for (int j = 0; j < ksteps; j++) {
-            const uint64_t ah = adesc | a_lo32, bh = b_const | b_lo32;
-            if (KIND != 2) {
-              wgmma<2 * N, 0, 1>(acc, ah, bh);
-            } else {
-              wgmma<N, 0, 0>(acc, ah, bh);
-              wgmma<N, 0, 0>(acc, ah, b_const | (b_lo32 + b_lo_add));
-            }
-            a_lo32 += a_step; b_lo32 += b_step;
-          }
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                                 // the previous stage's group has finished reading its slot
-        if (held >= 0 && lane == 0) mbar_arrive(empty0 + 8 * held);
-        held = stage;
-        if (++stage == n_stages) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      fence_regs<ACC / 2>(acc);
-      if (held >= 0 && lane == 0) mbar_arrive(empty0 + 8 * held);
+      tw.ns = __shfl_sync(0xffffffffu, tw.ns, 0);
+      if (tw.ns == 0) return false;
+      discard_regs<ACC / 2>(acc);
+      mma_stage(acc, tw.get(0), true, idle(bt));
+      return true;
+    };
 
-      const int btile0 = bt * 128;
+    // epilogue of tile (cu, cbt) from bank cur: bias / activation / ReLU mask, batch-planar and fp32 stores
+    auto epilogue = [&](const float* cur, int cu, int cbt, bool empty) {
+      const int btile0 = cbt * 128;
       int oc0, z = 0;                          // first output chunk of the unit
-      if (mode == 2) { const int nt = u % n_nt; z = u / n_nt; oc0 = nt * NCH; }
-      else oc0 = u * NCH;
+      if (mode == 2) { const int nt = cu % n_nt; z = cu / n_nt; oc0 = nt * NCH; }
+      else oc0 = cu * NCH;
 #pragma unroll
       for (int h = 0; h < 2; h++) {
         const int b = btile0 + row_in_tile + 8 * h;
 #pragma unroll
         for (int i = 0; i < NCH; i++) {
           const int c = 8 * i + 2 * q;           // column inside the tile
-          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-          if (CAT) { v0 += acc[4 * (i + NCH) + 2 * h]; v1 += acc[4 * (i + NCH) + 2 * h + 1]; }
+          float v0 = cur[4 * i + 2 * h], v1 = cur[4 * i + 2 * h + 1];
+          if (CAT) { v0 += cur[4 * (i + NCH) + 2 * h]; v1 += cur[4 * (i + NCH) + 2 * h + 1]; }
+          if (empty) { v0 = 0.f; v1 = 0.f; }
           if (KIND == 0) {
             if (b < Bsz) {
               const int f = oc0 * 8 + c;
@@ -593,8 +615,38 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
           }
         }
       }
-      u += du; bt += dbt;
+    };
+
+    // Tile loop, software-pipelined over two accumulator banks: the remaining stages of the current tile go into cur,
+    // then the first stage of the next tile into nxt, and the current tile's epilogue (global loads and stores) runs
+    // while that group is on the tensor pipe.  The wgmma_wait<1> of that first stage is what completes cur's groups.
+    // Registers cannot be indexed at run time, so the loop is unrolled by two: even tiles in acc0, odd tiles in acc1.
+    // The forward at N = 64 (2 x 64 accumulators per bank) does not fit both banks and the epilogue in the 168 registers
+    // per thread of a 288-thread CTA: it starts the next tile after the epilogue instead, one bank live at a time.
+    constexpr bool OVERLAP = !(KIND == 0 && N == 64);
+    auto finish_tile = [&](float* cur, float* nxt) {
+      for (int s = 1; s < tw.ns; s++) mma_stage(cur, tw.get(s), false, idle(bt));
+      // a unit without stages (a data-gradient pixel that no filter tap reaches) stores zeros: its bank was never
+      // written, and zeroing it here would put register writes between wgmma instructions
+      const bool empty = tw.ns == 0;
+      const int cu = u, cbt = bt;
+      tile += gridDim.x; u += du; bt += dbt;
       if (bt >= nbt) { bt -= nbt; u++; }
+      if (!(OVERLAP && tile < total && start_tile(nxt))) {
+        wgmma_wait<0>();
+        if (held >= 0 && lane == 0) mbar_arrive(empty0 + 8 * held);
+        held = -1;
+      }
+      fence_regs<ACC / 2>(cur);
+      if (!idle(cbt)) epilogue(cur, cu, cbt, empty);
+      if (!OVERLAP && tile < total) start_tile(nxt);
+    };
+    float acc0[ACC / 2], acc1[ACC / 2];
+    if (tile < total) start_tile(acc0);
+    while (tile < total) {
+      finish_tile(acc0, acc1);
+      if (tile >= total) break;
+      finish_tile(acc1, acc0);
     }
     if (KIND == 2 && a.db_part) {
       // column sums of this CTA: the 8 row lanes of a column -> one row per consumer warp -> fixed-order sum over warps
@@ -755,8 +807,9 @@ bp_wgrad_kernel(const __grid_constant__ WgradArgs a) {
       int held = -1;
       for (int kc = kc0; kc < n_kc; kc += kc_step) {
         const int opix = conv ? kc / a.n_bsub : 0, bs = conv ? kc - opix * a.n_bsub : kc;
-        if (!WgWalk::get(a, tab_sm, opix, r_conv, rt).valid) continue;
-        const int ksteps = ((min(WG_KB, a.B - bs * WG_KB) + 15) & ~15) >> 4;
+        // the skip and the trip count steer the wgmma issue: warp-uniform through a shuffle (see bp_rows_kernel)
+        if (!__shfl_sync(0xffffffffu, (int)WgWalk::get(a, tab_sm, opix, r_conv, rt).valid, 0)) continue;
+        const int ksteps = __shfl_sync(0xffffffffu, ((min(WG_KB, a.B - bs * WG_KB) + 15) & ~15) >> 4, 0);
         mbar_wait(full0 + 8 * stage, phase);
         const uint32_t sA = stage0 + (uint32_t)stage * WG_STAGE;
         uint32_t x32 = (sA >> 4) + x_row_add, g32 = (sA + WG_STAGE_A) >> 4;
