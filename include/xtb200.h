@@ -205,11 +205,15 @@ int xtb_adam_set_lr(xtb_adam* opt, float lr);
 int xtb_opt_use_rmsprop(xtb_adam* opt, float* mean_grad, float decay, float epsilon);
 
 /* ---- fused learner loops -------------------------------------------------------- */
+/* use_graph != 0 (xtb_ppo_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer and the predict calls
+ * built on it): the call's launches are captured once as a CUDA graph and replayed.  A graph is keyed on every
+ * argument plus the kernel-path mode (xtb_set_tc_mode), the fused-heads mode (xtb_set_fuse_heads) and the installed
+ * communicator (xtb_set_grad_comm), so a mode change takes effect at the next call.  It is dropped when its net,
+ * target net, optimiser or communicator is destroyed, or when its net is rebound (xtb_net_bind). */
 /* PPO.train (xt/model/ppo/ppo.py:111-132): for every minibatch slice of `perm`
  * (device int32 [n_epoch*n_sample], the host-generated np.random.shuffle order) run
  * forward, loss, backward, clip, Adam.  loss_per_step: device float [n_epoch*ceil(N/B)].
- * All launches go to `stream` (capturable into a CUDA graph; the library caches one per
- * (n_sample, batch) when use_graph != 0). */
+ * All launches go to `stream`. */
 typedef struct xtb_ppo_rollout {
   const void* obs;            /* [N, H,W,C] uint8 / float */
   const int32_t* action;      /* [N] */
@@ -241,7 +245,7 @@ int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs,
  * obs[step_idx[t*n_env+e]], NULL = rows t*n_env..), sample actions with Philox(seed, *offset_dev + t), and
  * write action/logp/value time-major [n_step, n_env]; finally *offset_dev += n_step.  This is the batched
  * replacement of the per-explorer batch-1 PPO.predict calls (xt/agent/ppo/ppo.py:35-45,
- * xt/algorithm/ppo/ppo.py:87-95); use_graph caches one CUDA graph per (buffers, n_env, n_step). */
+ * xt/algorithm/ppo/ppo.py:87-95). */
 int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
                           int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
                           int32_t* action, float* logp, float* value, int use_graph, void* stream);
@@ -292,7 +296,7 @@ int xtb_net_bench_layer(xtb_net* net, int layer, int which, const void* obs, con
  * 0 = fp32 CUDA-core kernels only (also XTB_TC=0 in the environment).  For A/B parity tests. */
 int xtb_set_tc_mode(int mode);
 /* 1 (default): xtb_ppo_train evaluates both heads, the loss and their backward in one fused kernel;
- * 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Affects graphs captured after the call. */
+ * 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call. */
 int xtb_set_fuse_heads(int on);
 int xtb_get_tc_mode(void);
 /* Self-test of the wgmma GEMM core on plain fp32 matrices (sizes multiples of 8):

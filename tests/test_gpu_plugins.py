@@ -542,6 +542,109 @@ def test_fused_heads_equals_unfused():
     assert l2_rel(outs[0][2], outs[1][2]) < 1e-3
 
 
+def test_rollout_infer_graph_follows_fuse_heads_mode():
+    """The fused-heads mode is part of a rollout-inference graph's key: after xtb_set_fuse_heads(0) a graphed call on
+    the same buffers launches what an eager layer-by-layer call launches, not the fused graph captured before."""
+    import xingtian_b200 as xb
+    from xingtian_b200 import capi
+    lib = capi.lib()
+    m = xb.alg_builder("PPO", ppo_cnn_info(), alg_cfg()).actor
+    E, T = 8, 2
+    obs = torch.from_numpy(np.random.default_rng(0).integers(0, 256, (E * T, 84, 84, 4), dtype=np.uint8)).cuda()
+    act = torch.empty(T, E, dtype=torch.int32, device="cuda"); lp = torch.empty(T, E, device="cuda"); val = torch.empty(T, E, device="cuda")
+
+    def launches(use_graph):
+        m.use_graph = use_graph
+        n0, r0 = lib.xtb_launch_count(), lib.xtb_graph_replay_count()
+        m.rollout_infer_device(obs, None, E, T, act, lp, val)
+        torch.cuda.synchronize()
+        assert lib.xtb_graph_replay_count() - r0 == int(use_graph)
+        return lib.xtb_launch_count() - n0
+
+    try:
+        lib.xtb_set_fuse_heads(1)
+        fused = launches(True)
+        lib.xtb_set_fuse_heads(0)
+        graphed = launches(True)
+        eager = launches(False)
+    finally:
+        lib.xtb_set_fuse_heads(1)
+    assert fused != eager, (fused, eager)
+    assert graphed == eager, (graphed, eager)
+
+
+def test_dqn_graph_is_keyed_on_scratch_and_discount_buffers():
+    """A graphed xtb_dqn_train call that differs from a captured one only in its qn_t or disc buffer uses the new
+    buffer: the old scratch keeps what the host wrote into it, and the loss is that of an eager call."""
+    import xingtian_b200 as xb
+    from xingtian_b200 import capi
+    from xingtian_b200.engine import _ptr, stream_ptr
+    info = {"actor": {"model_name": "DqnCnn", "state_dim": [84, 84, 4], "action_dim": 4, "model_config": {"LR": 0.00015, "init_seed": 5}}}
+    alg = xb.alg_builder("DQN", info, alg_cfg(instance_num=1, learning_starts=8, BUFFER_SIZE=64, BATCH_SIZE=32))
+    m, tgt = alg.actor, alg.target_actor
+    m.opt.set_lr(0.0)        # the weights stay put: every call below sees the same network
+    lib = m.net.lib
+    n, A = 32, 4
+    rng = np.random.default_rng(2)
+    obs = torch.from_numpy(rng.integers(0, 256, (n, 84, 84, 4), dtype=np.uint8)).cuda()
+    next_obs = torch.from_numpy(rng.integers(0, 256, (n, 84, 84, 4), dtype=np.uint8)).cuda()
+    action = torch.from_numpy(rng.integers(0, A, n).astype(np.int32)).cuda()
+    reward = torch.zeros(n, device="cuda"); done = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    disc_gamma = torch.full((n,), 0.99, device="cuda"); disc_zero = torch.zeros(n, device="cuda")
+    qn_t1 = torch.empty(n, A, device="cuda"); qn_t2 = torch.empty(n, A, device="cuda")
+    loss = torch.zeros(1, device="cuda")
+
+    def step(qn_t, disc, use_graph):
+        loss.zero_()
+        capi.check(lib.xtb_dqn_train(m.net.handle, tgt.net.handle, m.opt.handle, _ptr(obs), _ptr(next_obs), None, _ptr(action),
+                                     _ptr(reward), _ptr(done), _ptr(disc), n, 0.99, 0.0, m.net.tid[m.q_name], _ptr(qn_t), None,
+                                     _ptr(loss), use_graph, stream_ptr()))
+        return float(loss.cpu()[0])
+
+    step(qn_t1, disc_gamma, 1)                       # captured on qn_t1 and disc_gamma
+    ref_gamma, ref_zero = step(qn_t2, disc_gamma, 0), step(qn_t2, disc_zero, 0)
+    assert abs(ref_gamma - ref_zero) > 0.1 * max(abs(ref_gamma), abs(ref_zero)), (ref_gamma, ref_zero)
+    disc_gamma.fill_(12345.0)
+    got = step(qn_t1, disc_zero, 1)                  # another disc buffer
+    assert abs(got - ref_zero) < 5e-3 * abs(ref_zero), (got, ref_zero)
+    qn_t1.fill_(12345.0)
+    got = step(qn_t2, disc_zero, 1)                  # another qn_t buffer
+    assert bool((qn_t1 == 12345.0).all())
+    assert abs(got - ref_zero) < 5e-3 * abs(ref_zero), (got, ref_zero)
+
+
+def test_rebinding_a_net_drops_its_graphs():
+    """xtb_net_bind_stream on a live handle drops the graphs captured with the old buffers: the next graphed training
+    call updates the new parameter buffer and leaves the old one alone."""
+    import ctypes as C
+    import xingtian_b200 as xb
+    from xingtian_b200 import capi
+    from xingtian_b200.engine import _ptr, stream_ptr
+    alg = xb.alg_builder("PPO", ppo_cnn_info(batch=24, iters=1), alg_cfg())
+    net = alg.actor.net
+    lib = net.lib
+    trajs = make_trajs(4, 16, seed=3)
+
+    def train():
+        for tr in trajs:
+            alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "adv", "old_value", "target_value")})
+        np.random.seed(5)
+        alg.train()
+
+    r0 = lib.xtb_graph_replay_count()
+    train()
+    old_p, old_g = net.params, net.grads
+    new_p, new_g = old_p.clone(), torch.zeros_like(old_g)
+    capi.check(lib.xtb_net_bind_stream(net.handle, _ptr(new_p), _ptr(new_g), C.c_void_p(net._ws_base),
+                                       lib.xtb_net_workspace_bytes(net.handle), stream_ptr()))
+    net.params, net.grads = new_p, new_g
+    old_snap, new_snap = old_p.clone(), new_p.clone()
+    train()
+    assert lib.xtb_graph_replay_count() - r0 == 2
+    assert torch.equal(old_p, old_snap)
+    assert not torch.equal(new_p, new_snap)
+
+
 def test_staged_h2d_copy_is_exact():
     """xtb_copy_h2d_staged (threaded pinned-ring staging of pageable arrays) is a byte-exact copy for empty,
     sub-chunk, chunk-boundary and larger-than-ring sizes, back to back on one stream and across two streams."""

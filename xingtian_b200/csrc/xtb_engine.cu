@@ -461,7 +461,6 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
 }
 
 static void drop_graphs_of(const void* obj);
-static void drop_step_graphs_of(const void* obj);
 extern "C" void xtb_net_destroy(xtb_net* net) {
   if (!net) return;
   drop_graphs_of(net);
@@ -496,6 +495,7 @@ extern "C" int xtb_net_sync_weights(xtb_net* net, void* stream);
 extern "C" int xtb_net_bind_stream(xtb_net* net, float* params, float* grads, void* workspace, size_t workspace_bytes, void* stream) {
   if (!net || !params || !workspace) return fail(XTB_ERR_ARG, "xtb_net_bind: null pointer");
   if (workspace_bytes < net->ws_bytes) return fail(XTB_ERR_ARG, "workspace too small: %zu < %zu", workspace_bytes, net->ws_bytes);
+  drop_graphs_of(net);                     // captured graphs baked the old buffers in
   net->params = params; net->grads = grads; net->ws = (char*)workspace;
   cudaStream_t st = S(stream);
   { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
@@ -1516,19 +1516,6 @@ struct StreamScope {
     return XTB_OK;
   }
 };
-static std::atomic<long long> g_graph_replays{0};
-extern "C" long long xtb_graph_replay_count(void) { return g_graph_replays.load(); }
-
-// A captured graph bakes every kernel argument: the key carries everything that can change them.
-struct GraphKey {
-  const void* net; const void* opt; const void* obs; const void* perm; const void* loss; int n, b, e;
-  const void* ro[5]; float hp[4]; int pi_t, v_t, fuse, tc; const void* ws; const void* comm;
-  bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
-};
-struct GraphVal { cudaGraphExec_t exec; long long kernels; };
-static constexpr size_t kMaxCachedGraphs = 256;   // per cache; beyond it the cache is emptied (keys are buffer addresses)
-static std::map<GraphKey, GraphVal> g_graphs;
-
 static int g_fuse_heads = [] { const char* e = getenv("XTB_FUSE_HEADS"); return e ? atoi(e) : 1; }();
 extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 static xtb_grad_hook g_grad_hook = nullptr;
@@ -1536,6 +1523,85 @@ static void* g_grad_hook_user = nullptr;
 extern "C" int xtb_set_grad_hook(xtb_grad_hook hook, void* user) {
   g_grad_hook = hook; g_grad_hook_user = user;
   return XTB_OK;
+}
+
+// ---- CUDA-graph cache of the fused entry points ------------------------------------------------
+// A captured graph bakes in every kernel argument, so its key holds everything the capture reads.  capture_key()
+// zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
+// modes, which every capture reads.  Keys are compared bytewise.
+enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer };
+struct CaptureKey {
+  uint64_t tag;          // entry point
+  const void* own[4];    // net, target, opt, comm: destroying one, or rebinding a net, drops the graph
+  uint64_t mode[2];      // kernel-path and fused-heads modes
+  uint64_t arg[18];      // every pointer and scalar argument; floats by bit pattern
+  bool operator<(const CaptureKey& o) const { return memcmp(this, &o, sizeof(CaptureKey)) < 0; }
+};
+template <class T> static uint64_t key_word(T v) {
+  if constexpr (std::is_same_v<T, float>) { uint32_t u; memcpy(&u, &v, sizeof u); return u; }
+  else if constexpr (std::is_pointer_v<T>) return (uint64_t)(uintptr_t)v;
+  else return (uint64_t)v;
+}
+template <class... A>
+static CaptureKey capture_key(GraphTag tag, const void* net, const void* target, const void* opt, A... args) {
+  static_assert(sizeof...(A) <= sizeof(CaptureKey::arg) / sizeof(uint64_t), "CaptureKey::arg too small");
+  CaptureKey k;
+  memset(&k, 0, sizeof k);
+  k.tag = tag; k.own[0] = net; k.own[1] = target; k.own[2] = opt;
+  const uint64_t w[] = {key_word(args)...};
+  memcpy(k.arg, w, sizeof w);
+  return k;
+}
+struct GraphVal { cudaGraphExec_t exec; long long kernels; };
+static constexpr size_t kMaxCachedGraphs = 256;   // beyond it the cache is emptied (keys are buffer addresses)
+static std::map<CaptureKey, GraphVal> g_graphs;
+static std::atomic<long long> g_graph_replays{0};
+extern "C" long long xtb_graph_replay_count(void) { return g_graph_replays.load(); }
+
+// cached graphs hold raw pointers into their owners: they die with the object (a later object may be allocated at
+// the same address) and with a net's binding
+static void drop_graphs_of(const void* obj) {
+  for (auto it = g_graphs.begin(); it != g_graphs.end();) {
+    const auto& own = it->first.own;
+    if (std::find(std::begin(own), std::end(own), obj) != std::end(own)) { cudaGraphExecDestroy(it->second.exec); it = g_graphs.erase(it); } else ++it;
+  }
+}
+
+// use_graph == 0: launch(stream) runs eagerly.  Otherwise the launches are captured once per key, with the global
+// state every capture reads added to it, and the graph is replayed.
+template <class F>
+static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
+  if (!use_graph) return launch(stream);
+  key.own[3] = g_comm; key.mode[0] = g_tc_mode; key.mode[1] = g_fuse_heads;
+  StreamScope sc;
+  int src = sc.begin(stream, true);
+  if (src) return src;
+  auto it = g_graphs.find(key);
+  if (it == g_graphs.end()) {
+    cudaStream_t st = sc.st;
+    long long before = g_launches.load();
+    CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    int rc = launch((void*)st);
+    cudaGraph_t graph = nullptr;
+    cudaError_t e = cudaStreamEndCapture(st, &graph);
+    long long captured = g_launches.load() - before;
+    g_launches.store(before);   // captured, not launched yet
+    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+    cudaGraphExec_t exec = nullptr;
+    e = cudaGraphInstantiate(&exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
+    if (g_graphs.size() >= kMaxCachedGraphs) {     // callers that pass fresh buffers every call must not leak executables
+      for (auto& kv : g_graphs) cudaGraphExecDestroy(kv.second.exec);
+      g_graphs.clear();
+    }
+    it = g_graphs.emplace(key, GraphVal{exec, captured}).first;
+  }
+  CUDA_TRY(cudaGraphLaunch(it->second.exec, sc.st));
+  g_launches.fetch_add(it->second.kernels, std::memory_order_relaxed);
+  g_graph_replays.fetch_add(1, std::memory_order_relaxed);
+  return sc.end();
 }
 
 static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
@@ -1651,94 +1717,17 @@ extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout*
     if (rc > 0) world = rc;
     inv_world = 1.f / world;
   }
-  if (!use_graph || (g_grad_hook && !g_comm))
-    return ppo_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, loss_per_step, inv_world, stream);
-  StreamScope sc;
-  int src = sc.begin(stream, true);
-  if (src) return src;
-  GraphKey key;
-  memset(&key, 0, sizeof key);
-  key.net = net; key.opt = opt; key.obs = ro->obs; key.perm = perm; key.loss = loss_per_step;
-  key.n = n_sample; key.b = batch_size; key.e = n_epoch;
-  key.ro[0] = ro->action; key.ro[1] = ro->old_logp; key.ro[2] = ro->adv; key.ro[3] = ro->old_v; key.ro[4] = ro->target_v;
-  key.hp[0] = hp->clip_ratio; key.hp[1] = hp->ent_coef; key.hp[2] = hp->vf_clip; key.hp[3] = hp->critic_coef;
-  key.pi_t = pi_tensor; key.v_t = v_tensor; key.fuse = g_fuse_heads; key.tc = g_tc_mode; key.ws = net->ws; key.comm = g_comm;
-  auto it = g_graphs.find(key);
-  if (it == g_graphs.end()) {
-    cudaStream_t st = sc.st;
-    long long before = g_launches.load();
-    CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = ppo_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, loss_per_step, inv_world, (void*)st);
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    long long captured = g_launches.load() - before;
-    g_launches.store(before);   // captured, not launched yet
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t exec = nullptr;
-    e = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-    if (g_graphs.size() >= kMaxCachedGraphs) {
-      for (auto& kv : g_graphs) cudaGraphExecDestroy(kv.second.exec);
-      g_graphs.clear();
-    }
-    it = g_graphs.emplace(key, GraphVal{exec, captured}).first;
-  }
-  CUDA_TRY(cudaGraphLaunch(it->second.exec, sc.st));
-  g_launches.fetch_add(it->second.kernels, std::memory_order_relaxed);
-  g_graph_replays.fetch_add(1, std::memory_order_relaxed);
-  return sc.end();
+  return run_graph(capture_key(kPpoTrain, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v,
+                               perm, loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
+                               hp->critic_coef, pi_tensor, v_tensor),
+                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
+    return ppo_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, loss_per_step, inv_world, st);
+  });
 }
 
 // ------------------------------------------------------------------------------------------
 // fused IMPALA / DQN learner steps (graph-captured like xtb_ppo_train; gradients all-reduced when a communicator is set)
 // ------------------------------------------------------------------------------------------
-struct StepKey {
-  const void* p[12]; int i[8]; float f[4];
-  bool operator<(const StepKey& o) const { return memcmp(this, &o, sizeof(StepKey)) < 0; }
-};
-static std::map<StepKey, GraphVal> g_step_graphs;
-
-static void drop_step_graphs_of(const void* obj) {
-  for (auto it = g_step_graphs.begin(); it != g_step_graphs.end();) {
-    if (it->first.p[0] == obj || it->first.p[1] == obj || it->first.p[10] == obj || it->first.p[11] == obj) { cudaGraphExecDestroy(it->second.exec); it = g_step_graphs.erase(it); } else ++it;
-  }
-}
-
-template <class F>
-static int run_step_graph(const StepKey& key, int use_graph, void* stream, F&& launch) {
-  if (!use_graph) return launch(stream);
-  StreamScope sc;
-  int src = sc.begin(stream, true);
-  if (src) return src;
-  auto it = g_step_graphs.find(key);
-  if (it == g_step_graphs.end()) {
-    cudaStream_t st = sc.st;
-    long long before = g_launches.load();
-    CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = launch((void*)st);
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    long long captured = g_launches.load() - before;
-    g_launches.store(before);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t exec = nullptr;
-    e = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-    if (g_step_graphs.size() >= kMaxCachedGraphs) {     // callers that pass fresh buffers every step must not leak executables
-      for (auto& kv : g_step_graphs) cudaGraphExecDestroy(kv.second.exec);
-      g_step_graphs.clear();
-    }
-    it = g_step_graphs.emplace(key, GraphVal{exec, captured}).first;
-  }
-  CUDA_TRY(cudaGraphLaunch(it->second.exec, sc.st));
-  g_launches.fetch_add(it->second.kernels, std::memory_order_relaxed);
-  g_graph_replays.fetch_add(1, std::memory_order_relaxed);
-  return sc.end();
-}
 
 // ImpalaCnnOpt.train (xt/model/impala/impala_cnn_opt.py:251-265): forward over n = k * step_len env-major samples,
 // V-trace + summed losses (vtrace_kernel), backward, clip + Adam.  With a communicator the losses are sums over the
@@ -1754,13 +1743,9 @@ extern "C" int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, co
   if (n_sample <= 0 || n_sample > net->max_batch || step_len < 2 || n_sample % step_len) return fail(XTB_ERR_ARG, "xtb_impala_train: bad sizes");
   const int adim = net->tsize[logit_tensor];
   if (adim > MAX_ADIM) return fail(XTB_ERR_ARG, "xtb_impala_train: action dim too large");
-  StepKey key;
-  memset(&key, 0, sizeof key);
-  key.p[0] = net; key.p[1] = opt; key.p[2] = obs; key.p[3] = gather_idx; key.p[4] = bp_logits; key.p[5] = action; key.p[6] = done;
-  key.p[7] = reward; key.p[8] = loss_out; key.p[9] = net->ws; key.p[10] = g_comm;
-  key.i[0] = n_sample; key.i[1] = step_len; key.i[2] = logit_tensor; key.i[3] = base_tensor; key.i[4] = g_tc_mode; key.i[5] = 1;
-  key.f[0] = gamma;
-  return run_step_graph(key, use_graph, stream, [&](void* st) -> int {
+  return run_graph(capture_key(kImpalaTrain, net, nullptr, opt, obs, gather_idx, bp_logits, action, done, reward, loss_out,
+                               n_sample, step_len, gamma, logit_tensor, base_tensor),
+                   use_graph, stream, [&](void* st) -> int {
     int rc = net_forward_impl(net, nullptr, obs, gather_idx, n_sample, st, 0u, (1u << logit_tensor) | (1u << base_tensor));
     if (rc) return rc;
     rc = xtb_vtrace_loss_grad(xtb_net_tensor(net, logit_tensor), xtb_net_tensor(net, base_tensor), bp_logits, action, done, reward,
@@ -1789,14 +1774,10 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
   if (q_tensor < 1 || q_tensor > nl || (int)target->L.size() != nl) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad head tensor");
   if (n_sample <= 0 || n_sample > net->max_batch || n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad batch");
   const int adim = net->tsize[q_tensor];
-  StepKey key;
-  memset(&key, 0, sizeof key);
-  key.p[0] = net; key.p[1] = opt; key.p[2] = obs; key.p[3] = next_obs; key.p[4] = idx; key.p[5] = action; key.p[6] = reward;
-  key.p[7] = done; key.p[8] = loss_out; key.p[9] = net->ws; key.p[10] = g_comm; key.p[11] = target;
-  key.i[0] = n_sample; key.i[1] = q_tensor; key.i[2] = qn_o ? 1 : 0; key.i[3] = disc ? 1 : 0; key.i[4] = g_tc_mode; key.i[5] = 2;
-  key.f[0] = gamma; key.f[1] = huber_delta;
   const float inv_world = g_comm ? 1.f / g_comm->world : 1.f;
-  return run_step_graph(key, use_graph, stream, [&](void* st) -> int {
+  return run_graph(capture_key(kDqnTrain, net, target, opt, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
+                               n_sample, gamma, huber_delta, q_tensor),
+                   use_graph, stream, [&](void* st) -> int {
     const size_t qbytes = (size_t)n_sample * adim * sizeof(float);
     int rc = net_forward_impl(target, nullptr, next_obs, idx, n_sample, st, 0u, 1u << q_tensor);
     if (rc) return rc;
@@ -1821,24 +1802,6 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
 // ------------------------------------------------------------------------------------------
 // rollout inference: T batched policy evaluations over the E stacked observations
 // ------------------------------------------------------------------------------------------
-struct InferKey {
-  const void* net; const void* obs; const void* idx; const void* act; const void* logp; const void* val; const void* ctr;
-  const void* ws; unsigned long long seed; int e, t, pi_t, v_t, tc;
-  bool operator<(const InferKey& o) const { return memcmp(this, &o, sizeof(InferKey)) < 0; }
-};
-static std::map<InferKey, GraphVal> g_infer_graphs;
-// cached graphs hold raw pointers into a network / optimiser: they die with the object (a later object may
-// be allocated at the same address)
-static void drop_graphs_of(const void* obj) {
-  for (auto it = g_graphs.begin(); it != g_graphs.end();) {
-    if (it->first.net == obj || it->first.opt == obj || it->first.comm == obj) { cudaGraphExecDestroy(it->second.exec); it = g_graphs.erase(it); } else ++it;
-  }
-  for (auto it = g_infer_graphs.begin(); it != g_infer_graphs.end();) {
-    if (it->first.net == obj) { cudaGraphExecDestroy(it->second.exec); it = g_infer_graphs.erase(it); } else ++it;
-  }
-  drop_step_graphs_of(obj);
-}
-
 static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* step_idx, int E, int T, int pi_t, int v_t,
                                 uint64_t seed, unsigned long long* offset_dev, int32_t* action, float* logp, float* value,
                                 void* stream) {
@@ -1882,37 +1845,11 @@ extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_
   if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_rollout_infer: bad sizes");
   if (pi_tensor < 1 || pi_tensor > nl || v_tensor < 1 || v_tensor > nl || net->tsize[v_tensor] != 1 || net->tsize[pi_tensor] > MAX_ADIM)
     return fail(XTB_ERR_ARG, "xtb_ppo_rollout_infer: bad head tensors");
-  if (!use_graph)
-    return rollout_infer_launch(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, seed, offset_dev, action, logp, value, stream);
-  StreamScope sc;
-  int src = sc.begin(stream, true);
-  if (src) return src;
-  InferKey key;
-  memset(&key, 0, sizeof key);
-  key.net = net; key.obs = obs; key.idx = step_idx; key.act = action; key.logp = logp; key.val = value; key.ctr = offset_dev;
-  key.ws = net->ws; key.seed = seed; key.e = n_env; key.t = n_step; key.pi_t = pi_tensor; key.v_t = v_tensor; key.tc = g_tc_mode;
-  auto it = g_infer_graphs.find(key);
-  if (it == g_infer_graphs.end()) {
-    cudaStream_t st = sc.st;
-    long long before = g_launches.load();
-    CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = rollout_infer_launch(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, seed, offset_dev, action, logp, value, (void*)st);
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    long long captured = g_launches.load() - before;
-    g_launches.store(before);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t exec = nullptr;
-    e = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
-    it = g_infer_graphs.emplace(key, GraphVal{exec, captured}).first;
-  }
-  CUDA_TRY(cudaGraphLaunch(it->second.exec, sc.st));
-  g_launches.fetch_add(it->second.kernels, std::memory_order_relaxed);
-  g_graph_replays.fetch_add(1, std::memory_order_relaxed);
-  return sc.end();
+  return run_graph(capture_key(kRolloutInfer, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value, n_env, n_step,
+                               pi_tensor, v_tensor, seed),
+                   use_graph, stream, [&](void* st) {
+    return rollout_infer_launch(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, seed, offset_dev, action, logp, value, st);
+  });
 }
 
 // ------------------------------------------------------------------------------------------
