@@ -81,6 +81,21 @@ long long xtb_net_param_count(const xtb_net* net);
 /* offsets (in floats) of layer `layer`'s kernel and bias inside the flat buffer, and K,N */
 int xtb_net_layer_params(const xtb_net* net, int layer, long long* kernel_off, long long* bias_off,
                          int* k_rows, int* n_cols);
+/* How xtb_net_create planned layer `layer` (read-only; changes nothing that runs).  Every field but `kind` is 0 for a
+ * layer on the fp32 CUDA-core kernels.  A layer planned onto the tensor cores runs there while xtb_get_tc_mode() is 1. */
+typedef struct xtb_layer_plan {
+  int32_t kind;           /* xtb_layer_kind after planning: a VALID conv whose window covers the whole map is dense */
+  int32_t tc;             /* 1: the wgmma (tensor-core) kernels run this layer */
+  int32_t s2d;            /* first layer run as a stride-1 conv over the space-to-depth canvas of uint8 frames */
+  int32_t w_res;          /* conv: the weight blob stays resident in shared memory; 0: it streams through the ring */
+  int32_t n_fwd, n_dg;    /* accumulator columns of a forward / data-gradient tile */
+  int32_t R;              /* conv: weight-gradient accumulators (filter row x 128-feature tile) */
+  int32_t fwd_stages;     /* ring stages of the forward launch */
+  int32_t dg_stages;      /* ring stages of the data-gradient launch */
+  int32_t dg_empty_units; /* conv: input pixels that no filter tap reaches (their data gradient is zero) */
+  int32_t k_slices;       /* K slices (split-K) of a dense forward at max_batch samples; 1 for a conv */
+} xtb_layer_plan;
+int xtb_net_layer_plan(const xtb_net* net, int layer, xtb_layer_plan* out);
 /* floats per sample of tensor `t` (0 = observation) */
 int xtb_net_tensor_size(const xtb_net* net, int t);
 size_t xtb_net_workspace_bytes(const xtb_net* net);

@@ -25,6 +25,12 @@ class NetDesc(C.Structure):
                 ("in_c", C.c_int32), ("n_layers", C.c_int32), ("layers", LayerDesc * XTB_MAX_LAYERS)]
 
 
+class LayerPlan(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("tc", C.c_int32), ("s2d", C.c_int32), ("w_res", C.c_int32), ("n_fwd", C.c_int32),
+                ("n_dg", C.c_int32), ("R", C.c_int32), ("fwd_stages", C.c_int32), ("dg_stages", C.c_int32),
+                ("dg_empty_units", C.c_int32), ("k_slices", C.c_int32)]
+
+
 class PpoHyper(C.Structure):
     _fields_ = [("clip_ratio", C.c_float), ("ent_coef", C.c_float), ("vf_clip", C.c_float),
                 ("critic_coef", C.c_float)]
@@ -47,6 +53,7 @@ _SIGS = {
     "xtb_net_param_count": (C.c_longlong, [_P]),
     "xtb_net_layer_params": (C.c_int, [_P, C.c_int, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong),
                                        C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "xtb_net_layer_plan": (C.c_int, [_P, C.c_int, C.POINTER(LayerPlan)]),
     "xtb_net_tensor_size": (C.c_int, [_P, C.c_int]),
     "xtb_net_workspace_bytes": (C.c_size_t, [_P]),
     "xtb_net_bind": (C.c_int, [_P, _P, _P, _P, C.c_size_t]),

@@ -166,10 +166,11 @@ struct LayerPlan {
 // The K-stage walk of every unit of a conv layer (see bp_rows_kernel): forward = per filter row the taps inside the
 // image are one contiguous feature run, cut into stages of <= 64 elements; data gradient = one stage per filter tap
 // whose output position exists.  Weight gradient: per (output pixel, accumulator) the first X chunk and which of the
-// 16 chunks of the M tile are real.
-static void build_conv_tables(LayerPlan& lp) {
+// 16 chunks of the M tile are real.  Returns the largest stage count of any unit (a UnitEnt holds at most 255).
+static uint32_t build_conv_tables(LayerPlan& lp) {
   const ConvGeom& q = lp.q;
   const int Cout = lp.N;
+  uint32_t max_count = 0;
   for (int oy = 0; oy < q.OH; oy++)
     for (int ox = 0; ox < q.OW; ox++) {
       uint32_t first = (uint32_t)lp.fwd_st.size(), count = 0;
@@ -186,6 +187,7 @@ static void build_conv_tables(LayerPlan& lp) {
         }
       }
       lp.fwd_un.push_back(first | (count << 24));
+      max_count = std::max(max_count, count);
     }
   for (int iy = 0; iy < q.H; iy++)
     for (int ix = 0; ix < q.W; ix++) {
@@ -200,6 +202,7 @@ static void build_conv_tables(LayerPlan& lp) {
         count++;
       }
       lp.dg_un.push_back(first | (count << 24));
+      max_count = std::max(max_count, count);
     }
   for (int oy = 0; oy < q.OH; oy++)
     for (int ox = 0; ox < q.OW; ox++)
@@ -219,6 +222,7 @@ static void build_conv_tables(LayerPlan& lp) {
         }
         lp.wg_tab.push_back(e);
       }
+  return max_count;
 }
 
 struct PendingRed { bp::RedSeg s; };
@@ -270,6 +274,47 @@ static inline const bp::bf16* blob_hi(const xtb_net* n, const LayerPlan& lp) { r
 static inline bool use_tc(const LayerPlan& lp) { return g_tc_mode && lp.tc; }
 
 static int pick_tile(int n) { return n % 64 == 0 ? 64 : (n % 32 == 0 ? 32 : (n % 16 == 0 ? 16 : 0)); }
+
+// Dynamic shared memory of the tensor-core launches.  xtb_net_create plans with the same arithmetic as launch_rows /
+// launch_wgrad, so a layer it puts on the tensor cores always gets a launch that fits.
+// bp_rows_kernel: [resident weight blob][ring of n_stages stages][conv stage-walk table]
+struct RowsSmem { int wres_bytes, stage_bytes, tab_bytes, n_stages; };
+static RowsSmem rows_smem(bool w_res, int w_res_chunks, int w_pitch, int mode, size_t n_stage_ents, size_t n_units) {
+  RowsSmem r;
+  r.wres_bytes = w_res ? (int)align_up((size_t)2 * w_res_chunks * w_pitch * 16, 128) : 0;
+  r.stage_bytes = bp::RW_STAGE_A + (w_res ? 0 : bp::RW_STAGE_B);
+  const size_t tab = mode == 2 ? 0 : align_up(n_stage_ents * sizeof(bp::StageEnt) + n_units * sizeof(bp::UnitEnt), 128);
+  r.tab_bytes = (int)std::min(tab, (size_t)kMaxDynSmem + 1);
+  r.n_stages = std::max(0, std::min(bp::RW_MAX_STAGES, (kMaxDynSmem - 128 - r.wres_bytes - r.tab_bytes) / r.stage_bytes));
+  return r;
+}
+// bp_wgrad_kernel: [WG_STAGES stages][conv (output pixel, accumulator) table]
+static size_t wgrad_smem(int mode, int n_opix, int R) {
+  return 128 + bp::WG_STAGES * bp::WG_STAGE + (mode == 0 ? align_up((size_t)n_opix * R * sizeof(bp::WgEnt), 128) : 0);
+}
+// K slices of a dense forward over `tiles` output tiles: as many as fit in ONE wave of CTAs (rounding up instead left a
+// few CTAs with two slices: twice the latency), each a whole number of 64-element stages
+static int dense_k_slices(int kchunks, int tiles, int* kc_split) {
+  *kc_split = kchunks;
+  if (tiles < kSMs && kchunks >= 32) {
+    const int want = std::min(kSMs / tiles, kchunks / 8);
+    if (want > 1) {
+      *kc_split = ((kchunks + want - 1) / want + 7) / 8 * 8;
+      return (kchunks + *kc_split - 1) / *kc_split;
+    }
+  }
+  return 1;
+}
+// A conv layer stays on the tensor cores only if its stage tables fit: the forward and data-gradient launches get at
+// least two ring stages beside their table, the weight-gradient table fits beside the WG_STAGES stages, and no unit
+// needs more stages than a UnitEnt counts.  Otherwise it runs on the fp32 kernels.
+static bool conv_tables_fit(const LayerPlan& lp, uint32_t max_unit_stages) {
+  const ConvGeom& q = lp.q;
+  if (max_unit_stages > 255 || lp.fwd_st.size() >= (1u << 24) || lp.dg_st.size() >= (1u << 24)) return false;
+  if (rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size()).n_stages < 2) return false;
+  if (rows_smem(lp.w_res, lp.N / 8, lp.K, 1, lp.dg_st.size(), lp.dg_un.size()).n_stages < 2) return false;
+  return wgrad_smem(0, q.OH * q.OW, lp.R) <= (size_t)kMaxDynSmem;
+}
 
 extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net** out) {
   if (!desc || !out || max_batch <= 0) return fail(XTB_ERR_ARG, "xtb_net_create: null/invalid argument");
@@ -386,6 +431,15 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     net->L.push_back(lp);
   }
   net->n_params = off;
+  // a tensor-core layer reads its source in batch-planar form: features must come in chunks of 8 (always true for
+  // the shapes accepted above; a dense layer after an uncovered odd-width layer falls back)
+  for (auto& lp : net->L) if (lp.tc && lp.d.src != 0 && net->tsize[lp.d.src] % 8) lp.tc = false;
+  // stage tables of the tensor-core conv layers; a layer whose tables do not fit in shared memory falls back
+  for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_CONV) {
+    if (conv_tables_fit(lp, build_conv_tables(lp))) continue;
+    lp.tc = lp.s2d = false;
+    lp.fwd_st.clear(); lp.fwd_un.clear(); lp.dg_st.clear(); lp.dg_un.clear(); lp.wg_tab.clear();
+  }
   {   // one observation canvas serves every tensor-core first layer: they must agree on its geometry
     const LayerPlan* f = nullptr; bool agree = true;
     for (auto& lp : net->L) if (lp.s2d) {
@@ -396,9 +450,6 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     if (f) { net->H4 = f->q.H; net->W4 = f->q.W; }
     net->obs_feats = net->H4 * net->W4 * 64;
   }
-  // a tensor-core layer reads its source in batch-planar form: features must come in chunks of 8 (always true for
-  // the shapes accepted above; a dense layer after an uncovered odd-width layer falls back)
-  for (auto& lp : net->L) if (lp.tc && lp.d.src != 0 && net->tsize[lp.d.src] % 8) lp.tc = false;
   // workspace
   size_t w = 0;
   const int nt = desc->n_layers + 1;
@@ -434,7 +485,6 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     lp.dbpart_off = w; w += align_up((size_t)kSMs * 64 * sizeof(float), 256);
   }
   for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_CONV) {
-    build_conv_tables(lp);
     auto place = [&](size_t bytes) { size_t o = w; w += align_up(bytes, 256); return o; };
     lp.fwd_st_off = place(lp.fwd_st.size() * sizeof(bp::StageEnt)); lp.fwd_un_off = place(lp.fwd_un.size() * sizeof(bp::UnitEnt));
     lp.dg_st_off = place(lp.dg_st.size() * sizeof(bp::StageEnt)); lp.dg_un_off = place(lp.dg_un.size() * sizeof(bp::UnitEnt));
@@ -480,6 +530,27 @@ extern "C" int xtb_net_layer_params(const xtb_net* net, int layer, long long* ke
   if (bias_off) *bias_off = lp.b_off;
   if (k_rows) *k_rows = lp.K;
   if (n_cols) *n_cols = lp.N;
+  return XTB_OK;
+}
+
+extern "C" int xtb_net_layer_plan(const xtb_net* net, int layer, xtb_layer_plan* out) {
+  if (!net || !out || layer < 0 || layer >= (int)net->L.size()) return fail(XTB_ERR_ARG, "xtb_net_layer_plan: bad argument");
+  const LayerPlan& lp = net->L[layer];
+  memset(out, 0, sizeof *out);
+  out->kind = lp.d.kind;
+  if (!lp.tc) return XTB_OK;
+  out->tc = 1; out->s2d = lp.s2d; out->w_res = lp.w_res;
+  out->n_fwd = lp.n_fwd; out->n_dg = lp.n_dg; out->R = lp.R;
+  if (lp.d.kind == XTB_CONV) {
+    out->fwd_stages = rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size()).n_stages;
+    out->dg_stages = rows_smem(lp.w_res, lp.N / 8, lp.K, 1, lp.dg_st.size(), lp.dg_un.size()).n_stages;
+    for (bp::UnitEnt u : lp.dg_un) out->dg_empty_units += (u >> 24) == 0;
+    out->k_slices = 1;
+  } else {
+    out->fwd_stages = out->dg_stages = rows_smem(false, 0, lp.K, 2, 0, 0).n_stages;
+    int kc_split;
+    out->k_slices = dense_k_slices(lp.K / 8, (lp.N / lp.n_fwd) * ((net->max_batch + 127) / 128), &kc_split);
+  }
   return XTB_OK;
 }
 
@@ -609,15 +680,12 @@ static cudaError_t launch_rows(bp::RowsArgs& a, cudaStream_t st) {
     default: return cudaErrorInvalidValue;
   }
   { cudaError_t e0 = ensure_kernel_attrs(); if (e0 != cudaSuccess) return e0; }
-  const int wres_bytes = a.w_res ? (int)align_up((size_t)2 * a.w_res_chunks * a.w_pitch * 16, 128) : 0;
-  const int stage_bytes = bp::RW_STAGE_A + (a.w_res ? 0 : bp::RW_STAGE_B);
-  const int tab_bytes = a.mode == 2 ? 0 : (int)align_up((size_t)a.n_stage_ents * sizeof(bp::StageEnt) + (size_t)a.n_units * sizeof(bp::UnitEnt), 128);
-  int n_stages = std::min(bp::RW_MAX_STAGES, (kMaxDynSmem - 128 - wres_bytes - tab_bytes) / stage_bytes);
-  if (n_stages < 2) return cudaErrorInvalidConfiguration;
-  const int smem = 128 + wres_bytes + n_stages * stage_bytes + tab_bytes;
+  const RowsSmem m = rows_smem(a.w_res != 0, a.w_res_chunks, a.w_pitch, a.mode, (size_t)a.n_stage_ents, (size_t)a.n_units);
+  if (m.n_stages < 2) return cudaErrorInvalidConfiguration;
+  const int smem = 128 + m.wres_bytes + m.n_stages * m.stage_bytes + m.tab_bytes;
   const int total = a.n_units * a.n_btiles;
   const int grid = std::min(total, kSMs);
-  XLAUNCH(kern, grid, bp::RW_THREADS, smem, st, a, n_stages, stage_bytes, wres_bytes);
+  XLAUNCH(kern, grid, bp::RW_THREADS, smem, st, a, m.n_stages, m.stage_bytes, m.wres_bytes);
   return cudaPeekAtLastError();
 }
 
@@ -632,8 +700,9 @@ static cudaError_t launch_wgrad(const bp::WgradArgs& a, int grid, cudaStream_t s
     default: return cudaErrorInvalidValue;
   }
   { cudaError_t e0 = ensure_kernel_attrs(); if (e0 != cudaSuccess) return e0; }
-  const int smem = 128 + bp::WG_STAGES * bp::WG_STAGE + (a.mode == 0 ? (int)align_up((size_t)a.n_opix * a.R * sizeof(bp::WgEnt), 128) : 0);
-  XLAUNCH(kern, grid, bp::WG_THREADS, smem, st, a);
+  const size_t smem = wgrad_smem(a.mode, a.n_opix, a.R);
+  if (smem > (size_t)kMaxDynSmem) return cudaErrorInvalidConfiguration;
+  XLAUNCH(kern, grid, bp::WG_THREADS, (int)smem, st, a);
   return cudaPeekAtLastError();
 }
 
@@ -664,17 +733,7 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   }
   a.mode = 2;
   a.kchunks = lp.K / 8; a.n_ntiles = lp.N / lp.n_fwd;
-  const int tiles = a.n_ntiles * a.n_btiles;
-  int nz = 1;
-  a.kc_split = a.kchunks;
-  if (tiles < kSMs && a.kchunks >= 32) {
-    // as many K slices as fit in ONE wave of CTAs (rounding up instead left a few CTAs with two slices: twice the latency)
-    int want = std::min(kSMs / tiles, a.kchunks / 8);
-    if (want > 1) {
-      a.kc_split = ((a.kchunks + want - 1) / want + 7) / 8 * 8;     // whole 64-element stages per split
-      nz = (a.kchunks + a.kc_split - 1) / a.kc_split;
-    }
-  }
+  const int nz = dense_k_slices(a.kchunks, a.n_ntiles * a.n_btiles, &a.kc_split);
   a.n_units = a.n_ntiles * nz;
   if (nz == 1) return launch_rows<0>(a, st);
   a.part = (float*)(net->ws + net->splitk_off);

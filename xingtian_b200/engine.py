@@ -116,6 +116,18 @@ class Net(object):
             torch.cuda.current_stream().synchronize()
             self._create(batch)
 
+    def layer_plan(self, i):
+        """How the library planned layer i (xtb_net_layer_plan): kind ("conv" / "dense", after a VALID conv that
+        covers the whole map became dense), tc, s2d, w_res, n_fwd, n_dg, R, fwd_stages, dg_stages, dg_empty_units,
+        k_slices."""
+        p = capi.LayerPlan()
+        check(self.lib.xtb_net_layer_plan(self.handle, int(i), C.byref(p)))
+        out = {name: int(getattr(p, name)) for name, _ in capi.LayerPlan._fields_}
+        out["kind"] = "conv" if p.kind == capi.CONV else "dense"
+        for k in ("tc", "s2d", "w_res"):
+            out[k] = bool(out[k])
+        return out
+
     def _shapes(self):
         shapes = {"obs": tuple(self.arch["state_dim"])}
         for name, kind, src, sp in self.arch["layers"]:
