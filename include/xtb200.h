@@ -34,7 +34,7 @@ enum xtb_status {
   XTB_ERR_NOMEM = -4
 };
 
-enum xtb_layer_kind { XTB_CONV = 0, XTB_DENSE = 1 };
+enum xtb_layer_kind { XTB_CONV = 0, XTB_DENSE = 1, XTB_DUELING = 2 };
 enum xtb_act { XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2 };
 
 #define XTB_MAX_LAYERS 16
@@ -43,7 +43,14 @@ enum xtb_act { XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2 };
  * conv : Conv2D(cout, (k,k), strides=(stride,stride), padding = pad_same ? 'same' : 'valid')
  *        NHWC activations, HWIO kernel  (xt/model/model_utils.py:91-97,
  *        xt/model/impala/impala_cnn_opt.py:120-137, xt/model/dqn/dqn_cnn.py:49-51)
- * dense: Dense(n) on the HWC-flattened source (model_utils.py:83-88, :63-65) */
+ * dense: Dense(n) on the HWC-flattened source (model_utils.py:83-88, :63-65)
+ * dueling: the dueling Q combine of DqnCnn / DqnMlp with model_config {dueling: True} (xt/model/dqn/dqn_cnn.py:55-58,
+ *        dqn_mlp.py:51-54,80-87): Q = adv + (value - mean over actions of value).  No parameters and no activation
+ *        (act must be XTB_ACT_NONE).  `src` is the A-wide "value" tensor and `k` holds the tensor id of the 1-wide "adv"
+ *        tensor (the only layer kind with a second input); both must be outputs of earlier layers, never the
+ *        observation, and different tensors.  The output is A wide.  xtb_net_layer_params reports 0 rows and 0 columns
+ *        for it.  xtb_dqn_train runs a dueling q_tensor in one fused kernel when both streams are linear dense layers
+ *        on one hidden tensor (see xtb_dqn_train). */
 typedef struct xtb_layer_desc {
   int32_t kind;      /* xtb_layer_kind */
   int32_t src;       /* tensor id of the input: 0 = observation, i+1 = output of layer i */
@@ -250,7 +257,11 @@ int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t
 /* DQN.train (xt/algorithm/dqn/dqn.py:61-103) as one captured step over rows idx[0..n_sample) of a device replay ring:
  * target forward on next_obs, optional double-DQN online forward (qn_o != NULL), online forward on obs, TD target +
  * loss gradient (see xtb_dqn_td_loss_grad for disc / huber_delta), backward, per-tensor clip + Adam.
- * qn_t, qn_o: scratch [n_sample, adim].  *loss_out += loss. */
+ * qn_t, qn_o: scratch [n_sample, adim].  *loss_out += loss.
+ * When q_tensor is an XTB_DUELING layer whose two streams are linear dense layers reading the same hidden tensor (not
+ * the observation), the hidden width K is a multiple of 32 with A <= 8 and K <= 256, or A <= 4 and K <= 512, and the
+ * fused-heads mode is on (xtb_set_fuse_heads), the online forward of both streams, the combine, TD target, loss and
+ * the streams' backward run as one kernel; the target and double-DQN forwards, and every other shape, go layer by layer. */
 int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
                   const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                   const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
@@ -310,8 +321,8 @@ int xtb_net_bench_layer(xtb_net* net, int layer, int which, const void* obs, con
 /* Kernel-path selection: 1 (default) = wgmma tensor-core kernels wherever the shape is covered,
  * 0 = fp32 CUDA-core kernels only (also XTB_TC=0 in the environment).  For A/B parity tests. */
 int xtb_set_tc_mode(int mode);
-/* 1 (default): xtb_ppo_train evaluates both heads, the loss and their backward in one fused kernel;
- * 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call. */
+/* 1 (default): xtb_ppo_train (and xtb_dqn_train on a dueling head) evaluates both heads, the loss and their backward
+ * in one fused kernel; 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call. */
 int xtb_set_fuse_heads(int on);
 int xtb_get_tc_mode(void);
 /* Self-test of the wgmma GEMM core on plain fp32 matrices (sizes multiples of 8):

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("XTB_LIB_PATH") or os.path.join(HERE, "lib", "libxtb200.so")   # override: experiment builds (scripts/)
 
 XTB_MAX_LAYERS = 16
-CONV, DENSE = 0, 1
+CONV, DENSE, DUELING = 0, 1, 2
 ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2}
 CLIP_NONE, CLIP_GLOBAL_NORM, CLIP_PER_TENSOR = 0, 1, 2
 

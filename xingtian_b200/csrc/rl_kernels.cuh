@@ -435,6 +435,8 @@ __global__ void nstep_kernel(const float* __restrict__ reward, const uint8_t* __
 //   dWpi,dbpi,dWv,dbv += ...   (atomics into the flat gradient bucket)
 //   g(h) = (dlogits @ Wpi^T [+ dv * Wv^T]) * act'(h)         -> gradient wrt the hidden pre-activation
 // One warp per sample, lane owns hidden units lane, lane+32, ...  (K <= 32*HEAD_KPL, A <= HEAD_AMAX)
+// The same kernel runs the dueling DQN TD step: the K x A head is the "value" stream, the K x 1 head the "adv" stream
+// (xt/model/dqn/dqn_cnn.py:53-58); only the per-sample loss differs, so it is the LOSS template policy.
 // ------------------------------------------------------------------------------------------
 // template: HEAD_KPL hidden units per lane (K <= 32*HEAD_KPL), HEAD_AMAX >= A
 
@@ -453,10 +455,125 @@ struct PpoHeadsArgs {
   float* logits_out; float* v_out;
   int B, K, A, act_pi, act_v, shared;
   PpoHyperDev hp; float inv_count;
+  // dueling TD step (DuelingTdLoss): as dqn_loss_kernel, with q = the combine of the two heads; action / reward / done /
+  // disc are indexed through idx.  loss_in: the loss already accumulated (added once, by sample 0, so the ordered
+  // reduction of the loss slot writes loss_in + this step's loss).
+  const float* qn_t; const float* qn_o; const float* reward; const uint8_t* done; const float* disc; const float* loss_in;
+  float gamma, huber;
 };
 
-template <int HEAD_KPL, int HEAD_AMAX>
-__global__ void __launch_bounds__(256) ppo_heads_kernel(PpoHeadsArgs a) {
+// Per-sample loss policies of heads_kernel.  acc[0..A) = h . W_pi (no bias), acc[HEAD_AMAX] = h . W_v; every lane holds
+// the same values.  Fill dl[i] = dloss/d(pi head output i), dv = dloss/d(v head output) (0 for i >= A) and, on lane 0,
+// add the sample's loss to lsum and the bias gradients to dbp / dbv.
+// PPO: categorical actor loss with entropy + clipped critic loss (xt/model/ppo/__init__.py:4-25).
+struct PpoLoss {
+  template <int HEAD_AMAX>
+  static __device__ __forceinline__ void sample(const PpoHeadsArgs& a, int b, int lane, const float (&acc)[HEAD_AMAX + 1],
+                                                float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
+                                                float& dbv) {
+    const int A = a.A;
+    float lg[HEAD_AMAX]; float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) { lg[i] = (i < A) ? acc[i] + a.b_pi[i] : -INFINITY; mx = fmaxf(mx, lg[i]); }
+    float vv = acc[HEAD_AMAX] + a.b_v[0];
+    float z = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) z += expf(lg[i] - mx);
+    float lz = logf(z), H = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) { float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
+    int r = a.idx ? a.idx[b] : b;
+    int ac = a.action[r];
+    float logp_a = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) logp_a = lg[i] - mx - lz;
+    float ratio = expf(logp_a - a.old_logp[r]);
+    float ad = a.adv[r];
+    float s1 = ratio * ad;
+    float s2 = fminf(fmaxf(ratio, 1.f - a.hp.clip_ratio), 1.f + a.hp.clip_ratio) * ad;
+    float surr = fminf(s1, s2);
+    float dsurr = (s1 <= s2) ? ratio * ad
+                             : ((ratio >= 1.f - a.hp.clip_ratio && ratio <= 1.f + a.hp.clip_ratio) ? ratio * ad : 0.f);
+    float R = a.target_v[r], ov = a.old_v[r];
+    float l1 = (vv - R) * (vv - R);
+    float vc = ov + fminf(fmaxf(vv - ov, -a.hp.vf_clip), a.hp.vf_clip);
+    float l2 = (vc - R) * (vc - R);
+    float dvl = (l1 >= l2) ? 2.f * (vv - R)
+                           : ((vv - ov >= -a.hp.vf_clip && vv - ov <= a.hp.vf_clip) ? 2.f * (vc - R) : 0.f);
+    dv = a.hp.critic_coef * 0.5f * dvl * a.inv_count;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) {
+      dl[i] = 0.f;
+      if (i < A) {
+        float rl = lg[i] - mx, p = expf(rl) / z;
+        dl[i] = (-dsurr * (((i == ac) ? 1.f : 0.f) - p) + a.hp.ent_coef * p * (rl - lz + H)) * a.inv_count;
+      }
+    }
+    if (lane == 0) {
+      lsum += (-surr - a.hp.ent_coef * H + a.hp.critic_coef * 0.5f * fmaxf(l1, l2)) * a.inv_count;
+      if (a.logits_out) for (int i = 0; i < A; i++) a.logits_out[(long long)b * A + i] = lg[i];
+      if (a.v_out) a.v_out[b] = vv;
+      dbv += dv;
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) dbp[i] += dl[i];
+    }
+  }
+};
+
+// Dueling DQN TD step: value = pi head [A], adv = v head [1], q = adv + (value - mean_a value) (xt/model/dqn/dqn_mlp.py:80-87),
+// then the TD target, loss and d(loss)/dq of dqn_loss_kernel.  Only the taken action carries gradient, g = c e_a, so
+// dvalue = c (e_a - 1/A) and dadv = c.
+struct DuelingTdLoss {
+  template <int HEAD_AMAX>
+  static __device__ __forceinline__ void sample(const PpoHeadsArgs& a, int b, int lane, const float (&acc)[HEAD_AMAX + 1],
+                                                float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
+                                                float& dbv) {
+    const int A = a.A;
+    float val[HEAD_AMAX], s = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) { val[i] = (i < A) ? acc[i] + a.b_pi[i] : 0.f; s += val[i]; }
+    const float adv = acc[HEAD_AMAX] + a.b_v[0], mean = s / A;
+    const int r = a.idx ? a.idx[b] : b;
+    const int ac = a.action[r];
+    float q_a = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) q_a = adv + (val[i] - mean);
+    const float* t = a.qn_t + (long long)b * A;
+    float mq;
+    if (a.qn_o) {
+      const float* o = a.qn_o + (long long)b * A;
+      float best = o[0]; int bi = 0;
+      for (int i = 1; i < A; i++) if (o[i] > best) { best = o[i]; bi = i; }
+      mq = t[bi];
+    } else {
+      mq = t[0];
+      for (int i = 1; i < A; i++) mq = fmaxf(mq, t[i]);
+    }
+    const float g = a.disc ? a.disc[r] : a.gamma;
+    const float y = a.done[r] ? a.reward[r] : a.reward[r] + g * mq;
+    const float diff = q_a - y;
+    float grad, l;
+    if (a.huber > 0.f) {
+      const float ad = fabsf(diff);
+      l = ad <= a.huber ? 0.5f * diff * diff : a.huber * (ad - 0.5f * a.huber);
+      grad = fminf(fmaxf(diff, -a.huber), a.huber);
+    } else { l = diff * diff; grad = 2.f * diff; }
+    const float c = grad * a.inv_count, cm = c / A;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? ((i == ac) ? c : 0.f) - cm : 0.f;
+    dv = c;
+    if (lane == 0) {
+      lsum += l * a.inv_count;
+      if (b == 0) lsum += *a.loss_in;
+      dbv += dv;
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) dbp[i] += dl[i];
+    }
+  }
+};
+
+template <class LOSS, int HEAD_KPL, int HEAD_AMAX>
+__global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
   pdl_wait(); pdl_trigger();
   extern __shared__ float sh_dw[];          // [nwarp][nacc] per-warp partial sums in slab layout
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
@@ -501,53 +618,9 @@ __global__ void __launch_bounds__(256) ppo_heads_kernel(PpoHeadsArgs a) {
     }
 #pragma unroll
     for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
-    // ---- loss + d(logits), d(v): every lane computes the same values
-    float lg[HEAD_AMAX]; float mx = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) { lg[i] = (i < A) ? acc[i] + a.b_pi[i] : -INFINITY; mx = fmaxf(mx, lg[i]); }
-    float vv = acc[HEAD_AMAX] + a.b_v[0];
-    float z = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) z += expf(lg[i] - mx);
-    float lz = logf(z), H = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) { float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
-    int r = a.idx ? a.idx[b] : b;
-    int ac = a.action[r];
-    float logp_a = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) logp_a = lg[i] - mx - lz;
-    float ratio = expf(logp_a - a.old_logp[r]);
-    float ad = a.adv[r];
-    float s1 = ratio * ad;
-    float s2 = fminf(fmaxf(ratio, 1.f - a.hp.clip_ratio), 1.f + a.hp.clip_ratio) * ad;
-    float surr = fminf(s1, s2);
-    float dsurr = (s1 <= s2) ? ratio * ad
-                             : ((ratio >= 1.f - a.hp.clip_ratio && ratio <= 1.f + a.hp.clip_ratio) ? ratio * ad : 0.f);
-    float R = a.target_v[r], ov = a.old_v[r];
-    float l1 = (vv - R) * (vv - R);
-    float vc = ov + fminf(fmaxf(vv - ov, -a.hp.vf_clip), a.hp.vf_clip);
-    float l2 = (vc - R) * (vc - R);
-    float dvl = (l1 >= l2) ? 2.f * (vv - R)
-                           : ((vv - ov >= -a.hp.vf_clip && vv - ov <= a.hp.vf_clip) ? 2.f * (vc - R) : 0.f);
-    float dv = a.hp.critic_coef * 0.5f * dvl * a.inv_count;
-    float dl[HEAD_AMAX];
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) {
-      dl[i] = 0.f;
-      if (i < A) {
-        float rl = lg[i] - mx, p = expf(rl) / z;
-        dl[i] = (-dsurr * (((i == ac) ? 1.f : 0.f) - p) + a.hp.ent_coef * p * (rl - lz + H)) * a.inv_count;
-      }
-    }
-    if (lane == 0) {
-      lsum += (-surr - a.hp.ent_coef * H + a.hp.critic_coef * 0.5f * fmaxf(l1, l2)) * a.inv_count;
-      if (a.logits_out) for (int i = 0; i < A; i++) a.logits_out[(long long)b * A + i] = lg[i];
-      if (a.v_out) a.v_out[b] = vv;
-      dbv += dv;
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) dbp[i] += dl[i];
-    }
+    // ---- loss + d(head outputs): every lane computes the same values
+    float dl[HEAD_AMAX], dv;
+    LOSS::template sample<HEAD_AMAX>(a, b, lane, acc, dl, dv, lsum, dbp, dbv);
     // ---- head weight gradients (registers) and gradient wrt the hidden units
 #pragma unroll
     for (int j = 0; j < HEAD_KPL; j++) {
@@ -609,6 +682,42 @@ __global__ void __launch_bounds__(256) ppo_heads_kernel(PpoHeadsArgs a) {
     float t = sh_dw[e];
     for (int w = 1; w < nwarp; w++) t += sh_dw[(size_t)w * nacc + e];
     out[e] = t;
+  }
+}
+
+// Dueling combine layer (XTB_DUELING), one warp per sample: q = adv + (value - mean_a value) (xt/model/dqn/dqn_mlp.py:80-87)
+__global__ void __launch_bounds__(256) dueling_fwd_kernel(const float* __restrict__ value, const float* __restrict__ adv, int B, int A,
+                                                          float* __restrict__ q) {
+  pdl_wait(); pdl_trigger();
+  const int lane = threadIdx.x & 31, b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const float* v = value + (long long)b * A;
+  float s = 0.f;
+  for (int i = lane; i < A; i += 32) s += v[i];
+  const float mean = warp_sum(s) / A, ad = adv[b];
+  for (int i = lane; i < A; i += 32) q[(long long)b * A + i] = ad + (v[i] - mean);
+}
+// Its data gradient, g = dloss/dq: gvalue = (g - mean_a g) * act'(value), gadv = sum_a g * act'(adv), written or, when
+// acc_v / acc_a is set, added to what another consumer of that tensor already wrote.
+__global__ void __launch_bounds__(256) dueling_dgrad_kernel(const float* __restrict__ g, const float* __restrict__ value,
+                                                            const float* __restrict__ adv, int B, int A, int act_v, int act_a,
+                                                            int acc_v, int acc_a, float* __restrict__ gvalue, float* __restrict__ gadv) {
+  pdl_wait(); pdl_trigger();
+  const int lane = threadIdx.x & 31, b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const float* gr = g + (long long)b * A;
+  float s = 0.f;
+  for (int i = lane; i < A; i += 32) s += gr[i];
+  s = warp_sum(s);
+  const float mean = s / A;
+  for (int i = lane; i < A; i += 32) {
+    const long long e = (long long)b * A + i;
+    const float r = (gr[i] - mean) * act_grad_from_out(act_v, value[e]);
+    gvalue[e] = acc_v ? gvalue[e] + r : r;
+  }
+  if (lane == 0) {
+    const float r = s * act_grad_from_out(act_a, adv[b]);
+    gadv[b] = acc_a ? gadv[b] + r : r;
   }
 }
 

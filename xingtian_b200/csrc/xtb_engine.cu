@@ -142,6 +142,7 @@ struct LayerPlan {
   int K = 0, N = 0;      // weight matrix [K,N]
   long long w_off = 0, b_off = 0;
   int src_act = 0;       // activation of the producing layer of the source tensor
+  int adv_act = 0;       // dueling: activation of the producing layer of the 1-wide stream (tensor d.k)
   // device tables (conv, fp32 path)
   int* koff = nullptr; int* kyx = nullptr;            // forward / wgrad, indexed by k=(ky,kx,ci)
   int* dkyx = nullptr; int* dco = nullptr; int* wk = nullptr;  // dgrad, indexed by k=(ky,kx,co)
@@ -162,6 +163,9 @@ struct LayerPlan {
   std::vector<bp::StageEnt> fwd_st, dg_st; std::vector<bp::UnitEnt> fwd_un, dg_un; std::vector<bp::WgEnt> wg_tab;
   size_t fwd_st_off = 0, fwd_un_off = 0, dg_st_off = 0, dg_un_off = 0, wg_off = 0;
 };
+
+// layer `lp` reads tensor t: through src, or as the second (1-wide) input of a dueling layer
+static inline bool reads(const LayerPlan& lp, int t) { return lp.d.src == t || (lp.d.kind == XTB_DUELING && lp.d.k == t); }
 
 // The K-stage walk of every unit of a conv layer (see bp_rows_kernel): forward = per filter row the taps inside the
 // image are one contiguous feature run, cut into stages of <= 64 elements; data gradient = one stage per filter tap
@@ -335,6 +339,21 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     lp.d = desc->layers[i];
     const auto& d = lp.d;
     if (d.src < 0 || d.src > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: bad src %d", i, d.src); }
+    if (d.kind == XTB_DUELING) {
+      // combine of two earlier layers: src = the A-wide stream, k = the 1-wide stream; no parameters
+      if (d.src == 0 || d.k == 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer cannot read the observation", i); }
+      if (d.k < 0 || d.k > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling 1-wide input %d is not an earlier layer", i, d.k); }
+      if (d.k == d.src) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling inputs must be two different tensors", i); }
+      if (net->tsize[d.k] != 1) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling input %d is %d wide, not 1", i, d.k, net->tsize[d.k]); }
+      if (d.act != XTB_ACT_NONE) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer has no activation", i); }
+      lp.in_size = lp.out_size = net->tsize[d.src];
+      lp.src_act = tact[d.src]; lp.adv_act = tact[d.k];
+      shp[i + 1] = {1, 1, lp.out_size};
+      net->tsize[i + 1] = lp.out_size;
+      lp.w_off = lp.b_off = off;
+      net->L.push_back(lp);
+      continue;
+    }
     Shape is = shp[d.src];
     lp.in_size = is.h * is.w * is.c;
     lp.src_act = tact[d.src];
@@ -660,10 +679,11 @@ static cudaError_t ensure_kernel_attrs() {
       (const void*)bp::bp_wgrad_kernel<64>};
   for (const void* k : gemms)
     if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(xtb::ppo_heads_kernel<2, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(xtb::ppo_heads_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(xtb::ppo_heads_kernel<8, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(xtb::ppo_heads_kernel<16, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
+  for (const void* k : {(const void*)heads_kernel<PpoLoss, 2, 8>, (const void*)heads_kernel<PpoLoss, 8, 4>,
+                        (const void*)heads_kernel<PpoLoss, 8, 8>, (const void*)heads_kernel<PpoLoss, 16, 4>,
+                        (const void*)heads_kernel<DuelingTdLoss, 2, 8>, (const void*)heads_kernel<DuelingTdLoss, 8, 4>,
+                        (const void*)heads_kernel<DuelingTdLoss, 8, 8>, (const void*)heads_kernel<DuelingTdLoss, 16, 4>})
+    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
   done = true;
   return cudaSuccess;
 }
@@ -1022,6 +1042,16 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
   float* out = (float*)(net->ws + net->out_off[t]);
   const float* w = P + lp.w_off;
   const float* b = P + lp.b_off;
+  if (lp.d.kind == XTB_DUELING) {
+    int rc = ensure_f32(net, lp.d.src, B, false, st);
+    if (!rc) rc = ensure_f32(net, lp.d.k, B, false, st);
+    if (rc) return rc;
+    XLAUNCH(dueling_fwd_kernel, (B + 7) / 8, 256, 0, st, (const float*)(net->ws + net->out_off[lp.d.src]),
+            (const float*)(net->ws + net->out_off[lp.d.k]), B, lp.out_size, out);
+    LAUNCH_CHECK();
+    net->f32_ok[t] = 1; net->bp_ok[t] = 0;
+    return XTB_OK;
+  }
   if (tc_allowed && use_tc(lp)) {
     int rc = lp.d.src == 0 ? op_decode(net, obs, idx, B, st) : ensure_bp(net, lp.d.src, B, false, st);
     if (rc) return rc;
@@ -1055,6 +1085,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
 
 static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, int B, cudaStream_t st, bool bias_done = false) {
   const LayerPlan& lp = net->L[i];
+  if (lp.d.kind == XTB_DUELING) return XTB_OK;   // no parameters
   int t = i + 1;
   float* dw = net->grads + lp.w_off;
   float* db = net->grads + lp.b_off;
@@ -1111,9 +1142,24 @@ static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, in
 
 // data gradient of layer i into its source tensor (gradient wrt the source's pre-activation)
 // fuse_db: the epilogue also produces the bias gradient of the layer behind the source tensor (ordered partial sums)
-static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool fuse_db = false) {
+static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool fuse_db = false, int acc2 = 0) {
   const LayerPlan& lp = net->L[i];
   int t = i + 1, s = lp.d.src;
+  if (lp.d.kind == XTB_DUELING) {   // both inputs; acc2: accumulate into the 1-wide input (tensor d.k)
+    const int s2 = lp.d.k;
+    int rc = ensure_f32(net, t, B, true, st);
+    if (!rc) rc = ensure_f32(net, s, B, false, st);
+    if (!rc) rc = ensure_f32(net, s2, B, false, st);
+    if (!rc && acc) rc = ensure_f32(net, s, B, true, st);
+    if (!rc && acc2) rc = ensure_f32(net, s2, B, true, st);
+    if (rc) return rc;
+    XLAUNCH(dueling_dgrad_kernel, (B + 7) / 8, 256, 0, st, (const float*)(net->ws + net->gout_off[t]),
+            (const float*)(net->ws + net->out_off[s]), (const float*)(net->ws + net->out_off[s2]), B, lp.out_size, lp.src_act,
+            lp.adv_act, acc, acc2, (float*)(net->ws + net->gout_off[s]), (float*)(net->ws + net->gout_off[s2]));
+    LAUNCH_CHECK();
+    net->gf32_ok[s] = net->gf32_ok[s2] = 1; net->gbp_ok[s] = net->gbp_ok[s2] = 0;
+    return XTB_OK;
+  }
   if (use_tc(lp)) {
     int rc = ensure_bp(net, t, B, true, st);
     if (rc) return rc;
@@ -1204,7 +1250,7 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
     // ... or when a layer outside the tensor-core path consumes it (exact fp32 instead of hi + lo)
     if (lp.d.kind == XTB_DENSE)
       for (int j = i + 1; j < nl; j++)
-        if (net->L[j].d.src == i + 1 && !(skip_mask & (1u << j)) && !(tc_allowed && use_tc(net->L[j]))) direct = true;
+        if (reads(net->L[j], i + 1) && !(skip_mask & (1u << j)) && !(tc_allowed && use_tc(net->L[j]))) direct = true;
     int rc = op_forward(net, i, P, tc_allowed, obs, gather_idx, batch, direct, st);
     if (rc) return rc;
   }
@@ -1250,7 +1296,7 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
     if (bias_done_tensors & (1u << s)) { fuse_bias[s] = 2; continue; }
     const LayerPlan& ps = net->L[s - 1];
     int consumers = 0, cj = -1;
-    for (int j = 0; j < nl; j++) if (net->L[j].d.src == s && !(skip_mask & (1u << j))) { consumers++; cj = j; }
+    for (int j = 0; j < nl; j++) if (reads(net->L[j], s) && !(skip_mask & (1u << j))) { consumers++; cj = j; }
     if (consumers != 1) continue;
     const LayerPlan& c = net->L[cj];
     if (!use_tc(c)) continue;
@@ -1270,7 +1316,12 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
       rc = comm_fork_allreduce(comm, net->grads + early_off, early_cnt, st);
       if (rc) return rc;
     }
-    if (lp.d.src != 0) {
+    if (lp.d.kind == XTB_DUELING) {
+      const int s = lp.d.src, s2 = lp.d.k;
+      rc = op_dgrad(net, i, written[s] ? 1 : 0, batch, st, false, written[s2] ? 1 : 0);
+      if (rc) return rc;
+      written[s] = written[s2] = 1; has_grad[s] = has_grad[s2] = 1;
+    } else if (lp.d.src != 0) {
       int s = lp.d.src;
       rc = op_dgrad(net, i, written[s] ? 1 : 0, batch, st, fuse_bias[s] == 1);
       if (rc) return rc;
@@ -1663,6 +1714,20 @@ static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
   return sc.end();
 }
 
+// heads_kernel instantiations: K hidden units (K % 32 == 0) and A actions, A <= 8 with K <= 256 or A <= 4 with K <= 512
+static bool heads_fit(int K, int A) {
+  const int kpl = K / 32;
+  return K % 32 == 0 && A <= 8 && (kpl <= 8 || (kpl <= 16 && A <= 4));
+}
+template <class LOSS>
+static void launch_heads(const PpoHeadsArgs& a, int blocks, size_t shb, cudaStream_t st) {
+  const int kpl = a.K / 32;
+  if (kpl <= 2) XLAUNCH((heads_kernel<LOSS, 2, 8>), blocks, 256, shb, st, a);
+  else if (kpl <= 8 && a.A <= 4) XLAUNCH((heads_kernel<LOSS, 8, 4>), blocks, 256, shb, st, a);
+  else if (kpl <= 8) XLAUNCH((heads_kernel<LOSS, 8, 8>), blocks, 256, shb, st, a);
+  else XLAUNCH((heads_kernel<LOSS, 16, 4>), blocks, 256, shb, st, a);
+}
+
 static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
                             const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t,
                             float* loss_per_step, float inv_world, void* stream) {
@@ -1673,10 +1738,8 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* 
   // fused heads: both heads are linear dense layers on hidden tensors of equal width
   const LayerPlan& lpi = net->L[pi_t - 1];
   const LayerPlan& lv = net->L[v_t - 1];
-  int kpl = lpi.K / 32;
   bool fuse = g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
-              lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && lpi.K % 32 == 0 && adim <= 8 &&
-              (kpl <= 8 || (kpl <= 16 && adim <= 4));
+              lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && heads_fit(lpi.K, adim);
   unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
   int step = 0;
   for (int e = 0; e < E; e++) {
@@ -1701,7 +1764,7 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* 
         a.pitch = net->pitch;
         a.w_pi = net->params + lpi.w_off; a.b_pi = net->params + lpi.b_off; a.w_v = net->params + lv.w_off; a.b_v = net->params + lv.b_off;
         // the hidden layers' bias gradients (column sums of g) when they are dense and only feed the heads
-        auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (net->L[j].d.src == tsr && !(skip & (1u << j))) return false; return true; };
+        auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], tsr) && !(skip & (1u << j))) return false; return true; };
         bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src);
         bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src);
         unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
@@ -1714,10 +1777,7 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* 
         a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
         size_t shb = (size_t)8 * nacc * sizeof(float);
         { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
-        if (kpl <= 2) XLAUNCH((ppo_heads_kernel<2, 8>), blocks, 256, shb, S(stream), a);
-        else if (kpl <= 8 && adim <= 4) XLAUNCH((ppo_heads_kernel<8, 4>), blocks, 256, shb, S(stream), a);
-        else if (kpl <= 8) XLAUNCH((ppo_heads_kernel<8, 8>), blocks, 256, shb, S(stream), a);
-        else XLAUNCH((ppo_heads_kernel<16, 4>), blocks, 256, shb, S(stream), a);
+        launch_heads<PpoLoss>(a, blocks, shb, S(stream));
         LAUNCH_CHECK();
         {   // ordered reduction of the per-block slabs (queued; runs with the other partial sums at the end of backward)
           auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
@@ -1818,6 +1878,68 @@ extern "C" int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, co
   });
 }
 
+// Dueling head that the fused TD step covers: q_tensor combines two linear dense layers that read the same hidden
+// (non-observation) tensor, within the heads_kernel limits, and the fused-heads mode is on.
+static bool dueling_fusable(const xtb_net* net, int q_tensor) {
+  const LayerPlan& lq = net->L[q_tensor - 1];
+  if (!g_fuse_heads || lq.d.kind != XTB_DUELING) return false;
+  const LayerPlan& lv = net->L[lq.d.src - 1];
+  const LayerPlan& la = net->L[lq.d.k - 1];
+  return lv.d.kind == XTB_DENSE && la.d.kind == XTB_DENSE && lv.d.act == 0 && la.d.act == 0 && lv.d.src != 0 &&
+         lv.d.src == la.d.src && heads_fit(lv.K, lv.N);
+}
+
+// The online half of the dueling TD step in one heads_kernel launch: both streams' forward, the combine, TD target and
+// loss, the streams' backward and the gradient wrt the hidden tensor (straight into its planes when its layer runs on
+// the tensor cores); then the backward pass of the layers below, with the slab reductions queued like ppo_train_launch's.
+static int dueling_td_fused(xtb_net* net, const void* obs, const int32_t* idx, const int32_t* action, const float* reward,
+                            const uint8_t* done, const float* disc, int n, float gamma, float huber, int q_tensor,
+                            const float* qn_t, const float* qn_o, float inv_count, float* loss_out, cudaStream_t st) {
+  const LayerPlan& lq = net->L[q_tensor - 1];
+  const LayerPlan& lv = net->L[lq.d.src - 1];
+  const LayerPlan& la = net->L[lq.d.k - 1];
+  const int h = lv.d.src, K = lv.K, A = lv.N;
+  const unsigned skip = (1u << (q_tensor - 1)) | (1u << (lq.d.src - 1)) | (1u << (lq.d.k - 1));
+  int rc = net_forward_impl(net, nullptr, obs, idx, n, st, skip, 1u << h);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), st));
+  net->pending.clear();
+  PpoHeadsArgs a;
+  memset(&a, 0, sizeof a);
+  a.h_pi = a.h_v = (const float*)(net->ws + net->out_off[h]);
+  a.g_pi = a.g_v = (float*)(net->ws + net->gout_off[h]);
+  const bool bp = use_tc(net->L[h - 1]) && net->plane_elems[h] > 0;
+  a.gp_hi = a.gv_hi = bp ? gout_bp(net, h).hi : nullptr; a.gp_lo = a.gv_lo = net->plane_elems[h];
+  a.pitch = net->pitch;
+  a.w_pi = net->params + lv.w_off; a.b_pi = net->params + lv.b_off; a.w_v = net->params + la.w_off; a.b_v = net->params + la.b_off;
+  bool bh_ok = net->L[h - 1].d.kind == XTB_DENSE;   // the hidden layer's bias gradient, when h feeds nothing but the streams
+  for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], h) && !(skip & (1u << j))) bh_ok = false;
+  a.idx = idx; a.action = action; a.reward = reward; a.done = done; a.disc = disc; a.qn_t = qn_t; a.qn_o = qn_o; a.loss_in = loss_out;
+  a.B = n; a.K = K; a.A = A; a.act_pi = a.act_v = lv.src_act; a.shared = 1;
+  a.gamma = gamma; a.huber = huber; a.inv_count = inv_count;
+  const int blocks = std::max(1, std::min(kSMs, (n + 7) / 8));
+  const int nacc = K * A + 3 * K + A + 2;
+  a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
+  { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
+  launch_heads<DuelingTdLoss>(a, blocks, (size_t)8 * nacc * sizeof(float), st);
+  LAUNCH_CHECK();
+  auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
+    bp::RedSeg r;
+    memset(&r, 0, sizeof r);
+    r.part = a.part + off; r.n_slabs = blocks; r.slab = a.slab; r.count = count; r.kind = 1;
+    r.dst_off = dst_off; r.alpha = 1.f; r.dst_ptr = dst_ptr;
+    net->pending.push_back(r);
+  };
+  seg(0, K * A, lv.w_off, nullptr);
+  seg(K * A, K, la.w_off, nullptr);
+  if (bh_ok) seg(K * A + K, K, net->L[h - 1].b_off, nullptr);
+  seg(K * A + 3 * K, A, lv.b_off, nullptr);
+  seg(K * A + 3 * K + A, 1, la.b_off, nullptr);
+  seg(K * A + 3 * K + A + 1, 1, 0, loss_out);
+  int heads[1] = {h};
+  return net_backward_impl(net, obs, idx, n, heads, 1, st, skip, false, bh_ok ? (1u << h) : 0u, bp ? (1u << h) : 0u, g_comm);
+}
+
 // DQN.train (xt/algorithm/dqn/dqn.py:61-103) on a device replay ring: rows idx[0..n) of (obs, next_obs, action, reward,
 // done[, disc]); target-network forward on s', optional double-DQN online forward on s', online forward on s, TD target +
 // loss gradient, backward, clip + Adam.  qn_t / qn_o: scratch [n, adim] (qn_o NULL = plain DQN).  Reference mode:
@@ -1834,6 +1956,7 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
   if (n_sample <= 0 || n_sample > net->max_batch || n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad batch");
   const int adim = net->tsize[q_tensor];
   const float inv_world = g_comm ? 1.f / g_comm->world : 1.f;
+  const bool fuse = dueling_fusable(net, q_tensor);
   return run_graph(capture_key(kDqnTrain, net, target, opt, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
                                n_sample, gamma, huber_delta, q_tensor),
                    use_graph, stream, [&](void* st) -> int {
@@ -1846,14 +1969,21 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
       if (rc) return rc;
       CUDA_TRY(cudaMemcpyAsync(qn_o, xtb_net_tensor(net, q_tensor), qbytes, cudaMemcpyDeviceToDevice, S(st)));
     }
-    rc = net_forward_impl(net, nullptr, obs, idx, n_sample, st, 0u, 1u << q_tensor);
-    if (rc) return rc;
-    rc = xtb_dqn_td_loss_grad(xtb_net_tensor(net, q_tensor), qn_t, qn_o, idx, action, reward, done, disc, n_sample, adim, gamma,
-                              huber_delta, inv_world / ((float)n_sample * adim), xtb_net_tensor_grad(net, q_tensor), nullptr, loss_out, st);
-    if (rc) return rc;
-    int heads[1] = {q_tensor};
-    rc = net_backward_impl(net, obs, idx, n_sample, heads, 1, st, 0u, true, 0u, 0u, g_comm);
-    if (rc) return rc;
+    const float inv_count = inv_world / ((float)n_sample * adim);
+    if (fuse) {
+      rc = dueling_td_fused(net, obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor, qn_t, qn_o,
+                            inv_count, loss_out, S(st));
+      if (rc) return rc;
+    } else {
+      rc = net_forward_impl(net, nullptr, obs, idx, n_sample, st, 0u, 1u << q_tensor);
+      if (rc) return rc;
+      rc = xtb_dqn_td_loss_grad(xtb_net_tensor(net, q_tensor), qn_t, qn_o, idx, action, reward, done, disc, n_sample, adim, gamma,
+                                huber_delta, inv_count, xtb_net_tensor_grad(net, q_tensor), nullptr, loss_out, st);
+      if (rc) return rc;
+      int heads[1] = {q_tensor};
+      rc = net_backward_impl(net, obs, idx, n_sample, heads, 1, st, 0u, true, 0u, 0u, g_comm);
+      if (rc) return rc;
+    }
     return xtb_adam_step_net(opt, net, 1.f, st);
   });
 }

@@ -35,7 +35,10 @@ def require_cuda():
 
 
 class Net(object):
-    """One network (layers = list of (name, kind, src_name, spec)) living in device memory."""
+    """One network (layers = list of (name, kind, src_name, spec)) living in device memory.
+
+    kind "dueling": (name, "dueling", (value_src, adv_src), {}) combines an A-wide and a 1-wide earlier tensor into
+    Q = adv + (value - mean(value)); it has no parameters."""
 
     def __init__(self, arch, max_batch, device="cuda:0"):
         require_cuda()
@@ -55,6 +58,9 @@ class Net(object):
             raise ValueError("too many layers")
         for i, (name, kind, src, sp) in enumerate(arch["layers"]):
             ld = desc.layers[i]
+            if kind == "dueling":
+                ld.kind, ld.src, ld.k, ld.act = capi.DUELING, self.tid[src[0]], self.tid[src[1]], capi.ACT[None]
+                continue
             ld.kind = capi.CONV if kind == "conv" else capi.DENSE
             ld.src = self.tid[src]
             ld.act = capi.ACT[sp.get("act")]
@@ -71,6 +77,8 @@ class Net(object):
         self.ptable = OrderedDict()
         in_shapes = self._shapes()
         for i, (name, kind, src, sp) in enumerate(arch["layers"]):
+            if kind == "dueling":
+                continue
             ko, bo, kr, nc = C.c_longlong(), C.c_longlong(), C.c_int(), C.c_int()
             check(self.lib.xtb_net_layer_params(self.handle, i, C.byref(ko), C.byref(bo), C.byref(kr), C.byref(nc)))
             if kind == "conv":
@@ -117,13 +125,13 @@ class Net(object):
             self._create(batch)
 
     def layer_plan(self, i):
-        """How the library planned layer i (xtb_net_layer_plan): kind ("conv" / "dense", after a VALID conv that
+        """How the library planned layer i (xtb_net_layer_plan): kind ("conv" / "dense" / "dueling", after a VALID conv that
         covers the whole map became dense), tc, s2d, w_res, n_fwd, n_dg, R, fwd_stages, dg_stages, dg_empty_units,
         k_slices."""
         p = capi.LayerPlan()
         check(self.lib.xtb_net_layer_plan(self.handle, int(i), C.byref(p)))
         out = {name: int(getattr(p, name)) for name, _ in capi.LayerPlan._fields_}
-        out["kind"] = "conv" if p.kind == capi.CONV else "dense"
+        out["kind"] = {capi.CONV: "conv", capi.DENSE: "dense", capi.DUELING: "dueling"}[p.kind]
         for k in ("tc", "s2d", "w_res"):
             out[k] = bool(out[k])
         return out
@@ -131,6 +139,9 @@ class Net(object):
     def _shapes(self):
         shapes = {"obs": tuple(self.arch["state_dim"])}
         for name, kind, src, sp in self.arch["layers"]:
+            if kind == "dueling":
+                shapes[name] = shapes[src[0]]
+                continue
             ish = shapes[src]
             if kind == "conv":
                 h, w, _ = ish

@@ -73,8 +73,16 @@ def impala_cnn(state_dim, action_dim):
                 outputs=[sc + "conv2d_3", sc + "dense"])
 
 
-def dqn_cnn(state_dim, action_dim):
-    """DqnCnn.create_model, xt/model/dqn/dqn_cnn.py:45-54."""
+def _dueling(layers, value, adv_name):
+    """The dueling head (xt/model/dqn/dqn_cnn.py:55-58): adv = Dense(1) on the value stream's input, then the
+    parameter-free combine Q = adv + (value - mean(value)) as the output."""
+    layers.append((adv_name, "dense", layers[-1][2], dict(n=1, act=None)))
+    layers.append(("dueling", "dueling", (value, adv_name), {}))
+    return "dueling"
+
+
+def dqn_cnn(state_dim, action_dim, dueling=False):
+    """DqnCnn.create_model, xt/model/dqn/dqn_cnn.py:45-58."""
     layers = [
         ("conv2d", "conv", "obs", _conv(32, 8, 4, "valid", "relu")),
         ("conv2d_1", "conv", "conv2d", _conv(64, 4, 2, "valid", "relu")),
@@ -82,17 +90,20 @@ def dqn_cnn(state_dim, action_dim):
         ("dense", "dense", "conv2d_2", dict(n=256, act="relu")),
         ("dense_1", "dense", "dense", dict(n=action_dim, act=None)),
     ]
+    out = _dueling(layers, "dense_1", "dense_2") if dueling else "dense_1"
     return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0, layers=layers,
-                outputs=["dense_1"])
+                outputs=[out])
 
 
-def dqn_mlp(state_dim, action_dim, hidden_size, num_layers):
+def dqn_mlp(state_dim, action_dim, hidden_size, num_layers, dueling=False):
     """DqnMlp.create_model, xt/model/dqn/dqn_mlp.py:43-60."""
     layers, src = [], "obs"
     for i in range(num_layers):
         name = "dense" if i == 0 else "dense_{}".format(i)
         layers.append((name, "dense", src, dict(n=hidden_size, act="relu")))
         src = name
-    layers.append(("dense_{}".format(num_layers), "dense", src, dict(n=action_dim, act=None)))
+    value = "dense_{}".format(num_layers)
+    layers.append((value, "dense", src, dict(n=action_dim, act=None)))
+    out = _dueling(layers, value, "dense_{}".format(num_layers + 1)) if dueling else value
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
-                outputs=["dense_{}".format(num_layers)])
+                outputs=[out])

@@ -24,11 +24,9 @@ class _DqnBase(XTModel):
         self.state_dim = model_info["state_dim"]
         self.action_dim = model_info["action_dim"]
         self.learning_rate = LR
-        self.dueling = model_config.get("dueling", False)
+        self.dueling = bool(model_config.get("dueling", False))
         self._init_seed = model_config.get("init_seed")
         self.use_graph = bool(model_config.get("use_cuda_graph", True))
-        if self.dueling:
-            raise NotImplementedError("dueling head (dqn_cnn.py:55-58) is not on the benchmarked path")
         super().__init__(model_info)
 
     def build_arch(self):
@@ -43,7 +41,7 @@ class _DqnBase(XTModel):
         mode = capi.CLIP_PER_TENSOR if self.clipnorm else capi.CLIP_NONE
         # keras Adam: epsilon = K.epsilon() = 1e-7
         self.opt = Adam(self.net, self.learning_rate, eps=1e-7, clip_mode=mode, clip=float(self.clipnorm or 0.0))
-        self.q_name = arch["outputs"][0]
+        self.q_name = arch["outputs"][0]   # the dueling combine layer when model_config has dueling: True
         self._obs_dt = torch.uint8 if arch["input_dtype"] == "uint8" else torch.float32
         self._np_dt = np.uint8 if arch["input_dtype"] == "uint8" else np.float32
         self._bufs = {}
@@ -113,17 +111,17 @@ class _DqnBase(XTModel):
 
 @Registers.model
 class DqnCnn(_DqnBase):
-    """conv32/64/64 -> 256 -> A; Adam(lr, clipnorm=10) (dqn_cnn.py:45-61)."""
+    """conv32/64/64 -> 256 -> A (dueling: + 1, combined); Adam(lr, clipnorm=10) (dqn_cnn.py:45-61)."""
     clipnorm = 10.0
 
     def build_arch(self):
-        return archs.dqn_cnn(self.state_dim, self.action_dim)
+        return archs.dqn_cnn(self.state_dim, self.action_dim, dueling=self.dueling)
 
 
 @Registers.model
 class DqnMlp(_DqnBase):
-    """Dense(HIDDEN_SIZE) x NUM_LAYERS -> A; Adam(lr) (dqn_mlp.py:43-60)."""
+    """Dense(HIDDEN_SIZE) x NUM_LAYERS -> A (dueling: + 1, combined); Adam(lr) (dqn_mlp.py:43-60)."""
     clipnorm = None
 
     def build_arch(self):
-        return archs.dqn_mlp(self.state_dim, self.action_dim, HIDDEN_SIZE, NUM_LAYERS)
+        return archs.dqn_mlp(self.state_dim, self.action_dim, HIDDEN_SIZE, NUM_LAYERS, dueling=self.dueling)
