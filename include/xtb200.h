@@ -201,6 +201,17 @@ int xtb_nstep_returns(const float* reward, const uint8_t* done, int n_env, int n
  * xt/model/dqn/dqn_cnn.py:60-61): loss = mean over B*A of (q-y)^2, dq = 2*(q-y)*inv_count. */
 int xtb_mse_loss_grad(const float* q, const float* y, int batch, int adim, float inv_count, float* dq,
                       float* loss_out, void* stream);
+/* probs[b] = softmax(logits[b]) (the `output_actions` softmax of ImpalaMlp / ImpalaCnn.predict). */
+int xtb_softmax(const float* logits, int batch, int adim, float* probs, void* stream);
+/* Keras loss of ImpalaMlp / ImpalaCnn (impala_loss + value_weight * mse) on p = softmax(logits[b]) and v[b], data row
+ * r = idx[b] (NULL: b) of action_mat / adv / target_v:
+ *   l_b = mean_i [adv_r (-y_ri log(p_i + 1e-10)) - ent_coef (-p_i log(p_i + 1e-10))] + value_weight (v_b - target_v_r)^2
+ * dlogits / dv: gradient of mean_b l_b, through log(p + 1e-10) and the softmax Jacobian.  *loss_out += loss_scale *
+ * sum_b l_b, summed in a fixed order (one block, no atomics).  adim <= 32. */
+int xtb_impala_keras_loss_grad(const float* logits, const float* v, const int32_t* idx, const float* action_mat,
+                               const float* adv, const float* target_v, int batch, int adim, float ent_coef,
+                               float value_weight, float loss_scale, float* dlogits, float* dv, float* loss_out,
+                               void* stream);
 
 /* ---- optimiser: replaces tf.train.AdamOptimizer + clip_by_global_norm
  *      (xt/model/ppo/ppo.py:97-102, impala_cnn_opt.py:198-217) and Keras
@@ -220,6 +231,10 @@ int xtb_adam_step(xtb_adam* opt, float* params, const float* grads, float grad_s
 int xtb_adam_step_net(xtb_adam* opt, xtb_net* net, float grad_scale, void* stream);
 const float* xtb_adam_grad_norm(const xtb_adam* opt);
 int xtb_adam_set_lr(xtb_adam* opt, float lr);
+/* Keras OptimizerV2 `decay` (xt/model/impala/impala_cnn.py: Adam(lr, clipnorm=40, decay=5.12e-9)): every later Adam step
+ * uses lr / (1 + decay * iterations), iterations = the steps this optimiser took before it.  Device-resident like the
+ * learning rate; 0 (the default) leaves the step exactly as without it. */
+int xtb_adam_set_decay(xtb_adam* opt, float decay);
 /* Switch the optimiser handle to tf.train.RMSPropOptimizer(lr, decay, epsilon, centered=True) (momentum 0), the
  * `opt_type: rmsprop` branch of xt/model/impala/impala_cnn_opt.py:205-206: the `m` buffer of xtb_adam_create becomes the
  * mean-square slot and `mean_grad` (count floats) the mean-gradient slot; this call sets them to ones / zeros as TF
@@ -266,6 +281,34 @@ int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs,
                   const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                   const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
                   float* qn_o, float* loss_out, int use_graph, void* stream);
+
+/* IMPALA with the Keras learner (xt/algorithm/impala/impala.py, xt/model/impala/impala_mlp.py, impala_cnn.py).  The
+ * policy head `logit_tensor` is the linear `output_actions` layer; its softmax is evaluated in the kernels.
+ * ImpalaMlp/ImpalaCnn.train = one Keras fit epoch (batch_size fit_batch, shuffle): minibatch k holds rows
+ * order[k*fit_batch ...] (device int32 [n], the host-drawn np.random.shuffle order) of obs / action_mat [n, A] (one-hot
+ * y_true) / adv [n] / target_v [n]; per minibatch forward, the Keras loss (see xtb_impala_keras_loss_grad, value weight
+ * 0.5), backward and the optimiser step.  *loss_out = the epoch loss: per-row loss summed over the n rows, over n.
+ * Both calls return XTB_ERR_STATE, launching nothing, while a gradient hook or communicator is installed. */
+int xtb_impala_keras_fit(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* order, const float* action_mat,
+                         const float* adv, const float* target_v, int n, int fit_batch, int logit_tensor, int v_tensor,
+                         float ent_coef, float* loss_out, int use_graph, void* stream);
+/* IMPALA.train: n_traj trajectories of ep_len steps, stored trajectory by trajectory. */
+typedef struct xtb_impala_traj {
+  const void* obs;            /* [n_traj*(ep_len+1), ...] states, the last of each trajectory its bootstrap state */
+  const float* behav_prob;    /* [n_traj*ep_len, A] behaviour policy probabilities */
+  const float* action_mat;    /* [n_traj*ep_len, A] one-hot actions */
+  const float* reward;        /* [n_traj*ep_len] */
+  const uint8_t* done;        /* [n_traj*ep_len] */
+} xtb_impala_traj;
+/* 1. forward of every state with the current weights; 2. the V-trace variant of impala.py:124-184 into pg_adv and
+ * target_v ([n_traj*ep_len] device scratch the caller may read); 3. for every `slice`-row slice of the training rows,
+ * in order, one fit epoch as xtb_impala_keras_fit with adv = pg_adv.  order: [n_traj*ep_len] training rows, slice by
+ * slice (each slice a permutation of its own rows); training row i reads state row i + i / ep_len (obs_idx: scratch of
+ * the same size).  loss_per_slice[k] = the epoch loss of slice k.  n_traj*(ep_len+1) must not exceed max_batch. */
+int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_impala_traj* tr, int n_traj, int ep_len, int slice,
+                           int fit_batch, const int32_t* order, int32_t* obs_idx, float gamma, float ent_coef,
+                           int logit_tensor, int v_tensor, float* pg_adv, float* target_v, float* loss_per_slice,
+                           int use_graph, void* stream);
 
 /* Rollout inference: for t in [0,n_step): forward over n_env observations (row e of step t is
  * obs[step_idx[t*n_env+e]], NULL = rows t*n_env..), sample actions with Philox(seed, *offset_dev + t), and

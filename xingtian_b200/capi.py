@@ -41,6 +41,11 @@ class PpoRollout(C.Structure):
                 ("old_v", C.c_void_p), ("target_v", C.c_void_p)]
 
 
+class ImpalaTraj(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("behav_prob", C.c_void_p), ("action_mat", C.c_void_p), ("reward", C.c_void_p),
+                ("done", C.c_void_p)]
+
+
 _P = C.c_void_p
 GRAD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
 _SIGS = {
@@ -79,6 +84,13 @@ _SIGS = {
     "xtb_dqn_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_int, _P, _P, _P,
                                C.c_int, _P]),
     "xtb_mse_loss_grad": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
+    "xtb_softmax": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
+    "xtb_impala_keras_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
+                                             _P, _P, _P, _P]),
+    "xtb_impala_keras_fit": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _P,
+                                       C.c_int, _P]),
+    "xtb_impala_keras_train": (C.c_int, [_P, _P, C.POINTER(ImpalaTraj), C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
+                                         C.c_float, C.c_float, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P]),
     "xtb_adam_create": (C.c_int, [C.c_longlong, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int,
                                   C.c_float, C.POINTER(C.c_longlong), C.c_int, _P, _P, C.POINTER(_P)]),
     "xtb_adam_destroy": (None, [_P]),
@@ -86,6 +98,7 @@ _SIGS = {
     "xtb_adam_step_net": (C.c_int, [_P, _P, C.c_float, _P]),
     "xtb_adam_grad_norm": (_P, [_P]),
     "xtb_adam_set_lr": (C.c_int, [_P, C.c_float]),
+    "xtb_adam_set_decay": (C.c_int, [_P, C.c_float]),
     "xtb_opt_use_rmsprop": (C.c_int, [_P, _P, C.c_float, C.c_float]),
     "xtb_ppo_train": (C.c_int, [_P, _P, C.POINTER(PpoRollout), C.c_int, C.c_int, C.c_int, _P,
                                 C.POINTER(PpoHyper), C.c_int, C.c_int, _P, C.c_int, _P]),

@@ -21,14 +21,19 @@ constexpr int OPT_THREADS = 256;
 
 struct AdamState {          // lives in device memory
   float beta1_pow, beta2_pow, lr_t, grad_norm;
+  unsigned int iterations;  // steps taken (Keras `iterations`, read by the `decay` schedule)
 };
-struct AdamHyper {          // lives in device memory too: a captured CUDA graph must see xtb_adam_set_lr
+struct AdamHyper {          // lives in device memory too: a captured CUDA graph must see xtb_adam_set_lr / _set_decay
   float lr, beta1, beta2, eps, clip;
+  float decay;              // Keras OptimizerV2 `decay`: lr / (1 + decay * iterations); 0 = constant lr
 };
 
 __device__ __forceinline__ void adam_prep(AdamState* st, const AdamHyper* hyp, double* norm_sq, float* seg_scale, int n_seg,
                                           int clip_mode, float grad_scale) {
-  const float clip = hyp->clip, lr = hyp->lr, beta1 = hyp->beta1, beta2 = hyp->beta2;
+  const float clip = hyp->clip, beta1 = hyp->beta1, beta2 = hyp->beta2;
+  float lr = hyp->lr;
+  if (hyp->decay != 0.f) lr = lr / (1.f + hyp->decay * (float)st->iterations);   // iterations counted before the step
+  st->iterations += 1;
   double tot = 0.0;
   for (int s = 0; s < n_seg; s++) tot += norm_sq[s];
   float gs = fabsf(grad_scale);

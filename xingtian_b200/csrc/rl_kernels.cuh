@@ -783,6 +783,131 @@ ppo_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// IMPALA (xt/algorithm/impala/impala.py + xt/model/impala/impala_mlp.py, impala_cnn.py): the learner-side V-trace
+// variant and the Keras softmax policy-gradient loss.
+// ------------------------------------------------------------------------------------------
+// probs = softmax(logits) row by row (the `output_actions` softmax of predict)
+__global__ void softmax_rows_kernel(const float* __restrict__ logits, int B, int A, float* __restrict__ probs) {
+  pdl_wait(); pdl_trigger();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const float* l = logits + (long long)b * A;
+  float mx, lz;
+  softmax_stats(l, A, mx, lz);
+  for (int i = 0; i < A; i++) probs[(long long)b * A + i] = expf(l[i] - mx - lz);
+}
+
+// rho_t = min(1, exp(log(sum p_target y + 1e-10) - log(sum p_behav y + 1e-10)))   (impala.py:150-155, 186-189)
+__device__ inline float keras_rho(const float* tl, const float* bp, const float* y, int A) {
+  float mx, lz;
+  softmax_stats(tl, A, mx, lz);
+  float pt = 0.f, pb = 0.f;
+  for (int i = 0; i < A; i++) { pt += expf(tl[i] - mx - lz) * y[i]; pb += bp[i] * y[i]; }
+  return fminf(1.f, expf(logf(pt + 1e-10f) - logf(pb + 1e-10f)));
+}
+
+// IMPALA._train_proc (impala.py:124-184), one warp per trajectory of L steps and L+1 states:
+//   delta_t = rho_t (r_t + disc_t V_{t+1} - V_t),  disc_t = (1 - done_t) gamma
+//   adv_t   = delta_t + disc_{t+1} rho_{t+1} adv_{t+1},  adv_{L-1} = delta_{L-1}   (coefficients of the NEXT step)
+//   tv_t    = V_t + adv_t;   pg_t = rho_t (r_t + disc_t tv_{t+1} - V_t),  tv_L = V_L (the bootstrap value)
+// logits / value: the target head over the L+1 states of each trajectory; behav / amat / reward / done: the L steps.
+// Lanes own consecutive time chunks; the affine maps adv_in -> a adv_in + b are scanned as in gae_kernel.
+__global__ void impala_keras_vtrace_kernel(const float* __restrict__ logits, const float* __restrict__ value,
+                                           const float* __restrict__ behav, const float* __restrict__ amat,
+                                           const float* __restrict__ reward, const uint8_t* __restrict__ done, int n_traj,
+                                           int L, int A, float gamma, float* __restrict__ pg_adv, float* __restrict__ tv) {
+  pdl_wait(); pdl_trigger();
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= n_traj) return;
+  const long long sb = (long long)warp * (L + 1), tb = (long long)warp * L;   // first state row / first step row
+  auto rho = [&](int t) { return keras_rho(logits + (sb + t) * A, behav + (tb + t) * A, amat + (tb + t) * A, A); };
+  auto disc = [&](int t) { return done[tb + t] ? 0.f : gamma; };
+  const int chunk = (L + 31) / 32, t0 = lane * chunk, t1 = min(L, t0 + chunk);
+  // coefficient of adv_{t1} in adv_{t1-1}: disc_{t1} rho_{t1}, or 0 at the end of the trajectory
+  const float c_edge = (t0 < t1 && t1 < L) ? disc(t1) * rho(t1) : 0.f;
+  float a = 1.f, b = 0.f, c = c_edge;
+  for (int t = t1 - 1; t >= t0; --t) {
+    const float r = rho(t), d = disc(t);
+    const float delta = r * (reward[tb + t] + d * value[sb + t + 1] - value[sb + t]);
+    b = delta + c * b;
+    a = c * a;
+    c = d * r;
+  }
+  float fa = a, fb = b;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float oa = __shfl_down_sync(0xffffffffu, fa, o), ob = __shfl_down_sync(0xffffffffu, fb, o);
+    if (lane + o < 32) { fb = fa * ob + fb; fa = fa * oa; }
+  }
+  float incoming = __shfl_down_sync(0xffffffffu, fb, 1);   // adv_{t1}
+  if (lane == 31 || t1 >= L) incoming = 0.f;
+  float adv_next = incoming, tv_next = value[sb + t1] + incoming;   // t1 == L: tv_L = V_L
+  c = c_edge;
+  for (int t = t1 - 1; t >= t0; --t) {
+    const float r = rho(t), d = disc(t), V = value[sb + t], rw = reward[tb + t];
+    const float adv = r * (rw + d * value[sb + t + 1] - V) + c * adv_next;
+    const float tvt = V + adv;
+    pg_adv[tb + t] = r * (rw + d * tv_next - V);
+    tv[tb + t] = tvt;
+    adv_next = adv; tv_next = tvt; c = d * r;
+  }
+}
+
+// state row of training row i (the bootstrap state of every trajectory is skipped): i + i / L
+__global__ void impala_keras_rows_kernel(const int32_t* __restrict__ order, int n, int L, int32_t* __restrict__ obs_idx) {
+  pdl_wait(); pdl_trigger();
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) { const int i = order[k]; obs_idx[k] = i + i / L; }
+}
+
+// Keras loss of ImpalaMlp / ImpalaCnn on softmax(logits) and the value head, minibatch rows b (data rows idx[b]):
+//   l_b = mean_i [adv (-y_i log(p_i + 1e-10)) - ent (-p_i log(p_i + 1e-10))] + vw (v - tv)^2
+// (impala_loss with loss weight 1, 'mse' with loss weight vw = 0.5).  The minibatch loss is mean_b l_b; the gradient
+// goes through log(p + 1e-10) and the softmax Jacobian: dz_j = p_j (g_j - sum_i p_i g_i) / B with g_i = dl/dp_i.
+// *loss_out += loss_scale * sum_b l_b.  One block: rows are summed in a fixed order, so the loss is reproducible.
+constexpr int KERAS_LOSS_THREADS = 256;
+__global__ void __launch_bounds__(KERAS_LOSS_THREADS)
+impala_keras_loss_kernel(const float* __restrict__ logits, const float* __restrict__ v, const int32_t* __restrict__ idx,
+                         const float* __restrict__ y, const float* __restrict__ adv, const float* __restrict__ tv, int B, int A,
+                         float ent, float vw, float loss_scale, float* __restrict__ dlogits, float* __restrict__ dv,
+                         float* __restrict__ loss_out) {
+  pdl_wait(); pdl_trigger();
+  __shared__ float red[KERAS_LOSS_THREADS / 32];
+  const float inv_b = 1.f / B, inv_a = 1.f / A;
+  float lsum = 0.f;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const int r = idx ? idx[b] : b;
+    const float* l = logits + (long long)b * A;
+    const float* yr = y + (long long)r * A;
+    float mx, lz;
+    softmax_stats(l, A, mx, lz);
+    const float ad = adv[r];
+    float f = 0.f, pg = 0.f;
+    for (int i = 0; i < A; i++) {
+      const float p = expf(l[i] - mx - lz), lp = logf(p + 1e-10f);
+      f += ad * (-yr[i] * lp) - ent * (-p * lp);
+      pg += p * (-ad * yr[i] / (p + 1e-10f) + ent * (lp + p / (p + 1e-10f)));
+    }
+    for (int i = 0; i < A; i++) {
+      const float p = expf(l[i] - mx - lz), lp = logf(p + 1e-10f);
+      const float g = -ad * yr[i] / (p + 1e-10f) + ent * (lp + p / (p + 1e-10f));
+      dlogits[(long long)b * A + i] = p * (g - pg) * inv_a * inv_b;
+    }
+    const float dd = v[b] - tv[r];
+    dv[b] = 2.f * vw * dd * inv_b;
+    lsum += f * inv_a + vw * dd * dd;
+  }
+  lsum = warp_sum(lsum);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = lsum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += red[w];
+    *loss_out += loss_scale * s;
+  }
+}
+
 // Keras train_on_batch(states, y) with loss='mse': mean over B*A of (q-y)^2
 __global__ void mse_loss_kernel(const float* __restrict__ q, const float* __restrict__ y, long long n,
                                 float inv_count, float* __restrict__ dq, float* __restrict__ loss_out) {

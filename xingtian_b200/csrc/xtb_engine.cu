@@ -1457,6 +1457,26 @@ extern "C" int xtb_nstep_returns(const float* reward, const uint8_t* done, int n
   return XTB_OK;
 }
 
+extern "C" int xtb_softmax(const float* logits, int batch, int adim, float* probs, void* stream) {
+  if (!logits || !probs || batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_softmax: bad argument");
+  XLAUNCH(softmax_rows_kernel, (batch + 127) / 128, 128, 0, S(stream), logits, batch, adim, probs);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_impala_keras_loss_grad(const float* logits, const float* v, const int32_t* idx, const float* action_mat,
+                                          const float* adv, const float* target_v, int batch, int adim, float ent_coef,
+                                          float value_weight, float loss_scale, float* dlogits, float* dv, float* loss_out,
+                                          void* stream) {
+  if (!logits || !v || !action_mat || !adv || !target_v || !dlogits || !dv || !loss_out)
+    return fail(XTB_ERR_ARG, "xtb_impala_keras_loss_grad: null pointer");
+  if (batch <= 0 || adim <= 0 || adim > MAX_ADIM) return fail(XTB_ERR_ARG, "xtb_impala_keras_loss_grad: batch/adim out of range");
+  XLAUNCH(impala_keras_loss_kernel, 1, KERAS_LOSS_THREADS, 0, S(stream), logits, v, idx, action_mat, adv, target_v, batch, adim,
+          ent_coef, value_weight, loss_scale, dlogits, dv, loss_out);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
 extern "C" int xtb_mse_loss_grad(const float* q, const float* y, int batch, int adim, float inv_count, float* dq,
                                  float* loss_out, void* stream) {
   if (!q || !y || !dq || !loss_out || batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_mse_loss_grad: bad argument");
@@ -1500,7 +1520,7 @@ extern "C" int xtb_adam_create(long long count, float lr, float beta1, float bet
       bseg.push_back(s); bbeg.push_back(b); blen.push_back((int)std::min<long long>(OPT_CHUNK, seg[s + 1] - b));
     }
   o->n_blk = (int)bseg.size();
-  AdamState init{1.f, 1.f, 0.f, 0.f};
+  AdamState init{1.f, 1.f, 0.f, 0.f, 0u};
   cudaError_t e = cudaSuccess;
   auto chk = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
   chk(cudaMalloc(&o->blk_seg, o->n_blk * sizeof(int)));
@@ -1518,7 +1538,7 @@ extern "C" int xtb_adam_create(long long count, float lr, float beta1, float bet
     chk(cudaMemset(o->norm_sq, 0, o->n_seg * sizeof(double)));
     chk(cudaMemcpy(o->st, &init, sizeof init, cudaMemcpyHostToDevice));
     chk(cudaMemset(o->ticket, 0, sizeof(unsigned int)));
-    AdamHyper hy{lr, beta1, beta2, eps, clip};
+    AdamHyper hy{lr, beta1, beta2, eps, clip, 0.f};
     chk(cudaMemcpy(o->hyp, &hy, sizeof hy, cudaMemcpyHostToDevice));
     chk(cudaMemset(m, 0, count * sizeof(float)));
     chk(cudaMemset(v, 0, count * sizeof(float)));
@@ -1589,6 +1609,13 @@ extern "C" int xtb_adam_set_lr(xtb_adam* o, float lr) {
   CUDA_TRY(cudaMemcpy(&o->hyp->lr, &lr, sizeof lr, cudaMemcpyHostToDevice));
   return XTB_OK;
 }
+extern "C" int xtb_adam_set_decay(xtb_adam* o, float decay) {
+  if (!o) return fail(XTB_ERR_ARG, "null optimiser");
+  if (!(decay >= 0.f)) return fail(XTB_ERR_ARG, "xtb_adam_set_decay: decay must be >= 0");
+  CUDA_TRY(cudaDeviceSynchronize());      // device-resident, like the learning rate
+  CUDA_TRY(cudaMemcpy(&o->hyp->decay, &decay, sizeof decay, cudaMemcpyHostToDevice));
+  return XTB_OK;
+}
 
 // ------------------------------------------------------------------------------------------
 // fused PPO learner loop
@@ -1639,7 +1666,7 @@ extern "C" int xtb_set_grad_hook(xtb_grad_hook hook, void* user) {
 // A captured graph bakes in every kernel argument, so its key holds everything the capture reads.  capture_key()
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
-enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer };
+enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[4];    // net, target, opt, comm: destroying one, or rebinding a net, drops the graph
@@ -1875,6 +1902,98 @@ extern "C" int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, co
     rc = net_backward_impl(net, obs, gather_idx, n_sample, heads, 2, st, 0u, true, 0u, 0u, g_comm);
     if (rc) return rc;
     return xtb_adam_step_net(opt, net, 1.f, st);
+  });
+}
+
+// ---- IMPALA with the Keras learner (xt/algorithm/impala/impala.py, xt/model/impala/impala_mlp.py, impala_cnn.py) --------
+// One Keras fit epoch (training_arrays.fit_loop, batch_size = fit_batch, shuffle = True) over n rows in a given order:
+// minibatch k holds rows row_idx[k*fit_batch ...] (observation rows obs_idx[...]); per minibatch forward, the Keras
+// loss (impala_keras_loss_kernel, ragged last batch included), backward and the optimiser step.  *loss_out = the
+// epoch loss Keras reports: sum over the rows of the per-row loss / n.
+static int keras_fit_launch(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* obs_idx, const int32_t* row_idx,
+                            const float* y, const float* adv, const float* tv, int n, int fit_batch, int lt, int vt, float ent,
+                            float* loss_out, void* stream) {
+  CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), S(stream)));
+  const int adim = net->tsize[lt];
+  int heads[2] = {lt, vt};
+  for (int s0 = 0; s0 < n; s0 += fit_batch) {
+    const int mb = std::min(fit_batch, n - s0);
+    int rc = net_forward_impl(net, nullptr, obs, obs_idx + s0, mb, stream, 0u, (1u << lt) | (1u << vt));
+    if (rc) return rc;
+    rc = xtb_impala_keras_loss_grad(xtb_net_tensor(net, lt), xtb_net_tensor(net, vt), row_idx + s0, y, adv, tv, mb, adim, ent,
+                                    0.5f, 1.f / n, xtb_net_tensor_grad(net, lt), xtb_net_tensor_grad(net, vt), loss_out, stream);
+    if (rc) return rc;
+    rc = net_backward_impl(net, obs, obs_idx + s0, mb, heads, 2, stream, 0u, true);
+    if (rc) return rc;
+    rc = xtb_adam_step_net(opt, net, 1.f, stream);
+    if (rc) return rc;
+  }
+  return XTB_OK;
+}
+
+// arguments both IMPALA entry points share; data-parallel training is not supported by them
+static int keras_check(const char* fn, xtb_net* net, int lt, int vt) {
+  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
+  if (g_comm || g_grad_hook) return fail(XTB_ERR_STATE, "%s: data-parallel training (gradient hook / communicator) is not supported", fn);
+  const int nl = (int)net->L.size();
+  if (lt < 1 || lt > nl || vt < 1 || vt > nl || lt == vt || net->tsize[vt] != 1) return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
+  if (net->tsize[lt] > MAX_ADIM) return fail(XTB_ERR_ARG, "%s: action dim %d > %d", fn, net->tsize[lt], MAX_ADIM);
+  return XTB_OK;
+}
+
+extern "C" int xtb_impala_keras_fit(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* order, const float* action_mat,
+                                    const float* adv, const float* target_v, int n, int fit_batch, int logit_tensor, int v_tensor,
+                                    float ent_coef, float* loss_out, int use_graph, void* stream) {
+  if (!net || !opt || !obs || !order || !action_mat || !adv || !target_v || !loss_out)
+    return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: null pointer");
+  if (int rc = keras_check("xtb_impala_keras_fit", net, logit_tensor, v_tensor)) return rc;
+  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: optimiser/net size mismatch");
+  if (n <= 0 || fit_batch <= 0) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: bad sizes");
+  if (std::min(n, fit_batch) > net->max_batch) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: batch exceeds net max_batch");
+  return run_graph(capture_key(kImpalaKerasFit, net, nullptr, opt, obs, order, action_mat, adv, target_v, n, fit_batch, logit_tensor,
+                               v_tensor, ent_coef, loss_out),
+                   use_graph, stream, [&](void* st) {
+    return keras_fit_launch(net, opt, obs, order, order, action_mat, adv, target_v, n, fit_batch, logit_tensor, v_tensor, ent_coef,
+                            loss_out, st);
+  });
+}
+
+extern "C" int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_impala_traj* tr, int n_traj, int ep_len, int slice,
+                                      int fit_batch, const int32_t* order, int32_t* obs_idx, float gamma, float ent_coef,
+                                      int logit_tensor, int v_tensor, float* pg_adv, float* target_v, float* loss_per_slice,
+                                      int use_graph, void* stream) {
+  if (!net || !opt || !tr || !tr->obs || !tr->behav_prob || !tr->action_mat || !tr->reward || !tr->done || !order || !obs_idx ||
+      !pg_adv || !target_v || !loss_per_slice)
+    return fail(XTB_ERR_ARG, "xtb_impala_keras_train: null pointer");
+  if (int rc = keras_check("xtb_impala_keras_train", net, logit_tensor, v_tensor)) return rc;
+  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: optimiser/net size mismatch");
+  if (n_traj <= 0 || ep_len <= 0 || slice <= 0 || fit_batch <= 0) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: bad sizes");
+  const long long n_state = (long long)n_traj * (ep_len + 1), n_train = (long long)n_traj * ep_len;
+  if (n_state > net->max_batch) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: %lld states exceed net max_batch", n_state);
+  const xtb_impala_traj t = *tr;
+  return run_graph(capture_key(kImpalaKerasTrain, net, nullptr, opt, t.obs, t.behav_prob, t.action_mat, t.reward, t.done, n_traj,
+                               ep_len, slice, fit_batch, order, obs_idx, gamma, ent_coef, logit_tensor, v_tensor, pg_adv, target_v,
+                               loss_per_slice),
+                   use_graph, stream, [&](void* st) -> int {
+    // 1. target probabilities and values of every state with the weights before this call's updates
+    int rc = net_forward_impl(net, nullptr, t.obs, nullptr, (int)n_state, st, 0u, (1u << logit_tensor) | (1u << v_tensor));
+    if (rc) return rc;
+    // 2. V-trace into pg_adv / target_v
+    XLAUNCH(impala_keras_vtrace_kernel, (n_traj * 32 + 127) / 128, 128, 0, S(st), (const float*)xtb_net_tensor(net, logit_tensor),
+            (const float*)xtb_net_tensor(net, v_tensor), t.behav_prob, t.action_mat, t.reward, t.done, n_traj, ep_len,
+            net->tsize[logit_tensor], gamma, pg_adv, target_v);
+    LAUNCH_CHECK();
+    // 3. observation row of every training row of the shuffled slices
+    XLAUNCH(impala_keras_rows_kernel, (unsigned)((n_train + 255) / 256), 256, 0, S(st), order, (int)n_train, ep_len, obs_idx);
+    LAUNCH_CHECK();
+    // 4. one Keras fit per BATCH_SIZE slice, in order
+    for (long long s0 = 0, k = 0; s0 < n_train; s0 += slice, k++) {
+      const int n = (int)std::min<long long>(slice, n_train - s0);
+      rc = keras_fit_launch(net, opt, t.obs, obs_idx + s0, order + s0, t.action_mat, pg_adv, target_v, n, fit_batch, logit_tensor,
+                            v_tensor, ent_coef, loss_per_slice + k, st);
+      if (rc) return rc;
+    }
+    return XTB_OK;
   });
 }
 

@@ -253,6 +253,10 @@ class Adam(object):
     def set_lr(self, lr):
         check(self.lib.xtb_adam_set_lr(self.handle, float(lr)))
 
+    def set_decay(self, decay):
+        """Keras OptimizerV2 `decay`: later steps use lr / (1 + decay * steps taken before them)."""
+        check(self.lib.xtb_adam_set_decay(self.handle, float(decay)))
+
     def step(self, grad_scale=1.0):
         check(self.lib.xtb_adam_step_net(self.handle, self.net.handle, float(grad_scale), stream_ptr()))
 

@@ -107,3 +107,27 @@ def dqn_mlp(state_dim, action_dim, hidden_size, num_layers, dueling=False):
     out = _dueling(layers, value, "dense_{}".format(num_layers + 1)) if dueling else value
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
                 outputs=[out])
+
+
+def _impala_heads(layers, action_dim):
+    """output_actions = Dense(A, softmax), output_value = Dense(1) on the last hidden tensor (impala_mlp.py:49-50,
+    impala_cnn.py:55-56); the softmax is evaluated by the engine's kernels, so the layer itself is linear."""
+    src = layers[-1][0]
+    layers.append(("output_actions", "dense", src, dict(n=action_dim, act=None)))
+    layers.append(("output_value", "dense", src, dict(n=1, act=None)))
+
+
+def impala_keras_cnn(state_dim, action_dim):
+    """ImpalaCnn.create_model, xt/model/impala/impala_cnn.py:44-59: DqnCnn's trunk, then the two heads."""
+    layers = dqn_cnn(state_dim, action_dim)["layers"][:4]
+    _impala_heads(layers, action_dim)
+    return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0, layers=layers,
+                outputs=["output_actions", "output_value"])
+
+
+def impala_mlp(state_dim, action_dim, hidden_size, num_layers):
+    """ImpalaMlp.create_model, xt/model/impala/impala_mlp.py:39-55: DqnMlp's trunk, then the two heads."""
+    layers = dqn_mlp(state_dim, action_dim, hidden_size, num_layers)["layers"][:num_layers]
+    _impala_heads(layers, action_dim)
+    return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
+                outputs=["output_actions", "output_value"])
