@@ -34,7 +34,7 @@ enum xtb_status {
   XTB_ERR_NOMEM = -4
 };
 
-enum xtb_layer_kind { XTB_CONV = 0, XTB_DENSE = 1, XTB_DUELING = 2 };
+enum xtb_layer_kind { XTB_CONV = 0, XTB_DENSE = 1, XTB_DUELING = 2, XTB_LOGSTD = 3 };
 enum xtb_act { XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2 };
 
 #define XTB_MAX_LAYERS 16
@@ -50,7 +50,13 @@ enum xtb_act { XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2 };
  *        tensor (the only layer kind with a second input); both must be outputs of earlier layers, never the
  *        observation, and different tensors.  The output is A wide.  xtb_net_layer_params reports 0 rows and 0 columns
  *        for it.  xtb_dqn_train runs a dueling q_tensor in one fused kernel when both streams are linear dense layers
- *        on one hidden tensor (see xtb_dqn_train). */
+ *        on one hidden tensor (see xtb_dqn_train).
+ * logstd: the state-independent `pi_logstd` variable of PPO with action_type DiagGaussian (xt/model/ppo/ppo.py:75-78:
+ *        tf.get_variable('pi_logstd', shape=(1, A), initializer=zeros)).  A parameter-only layer: it owns `cout` = A
+ *        floats, reads no tensor (src must be 0) and produces none (its tensor is 0 wide, so no layer may read it and it
+ *        cannot be a backward head); act must be XTB_ACT_NONE and 1 <= cout <= 32.  xtb_net_layer_params reports 1 row
+ *        and A columns with bias_off = kernel_off + A (it has no bias).  It takes part in clipping, the optimiser and
+ *        the gradient bucket like every other parameter; the PPO Gaussian entry points below read it by offset. */
 typedef struct xtb_layer_desc {
   int32_t kind;      /* xtb_layer_kind */
   int32_t src;       /* tensor id of the input: 0 = observation, i+1 = output of layer i */
@@ -242,8 +248,8 @@ int xtb_adam_set_decay(xtb_adam* opt, float decay);
 int xtb_opt_use_rmsprop(xtb_adam* opt, float* mean_grad, float decay, float epsilon);
 
 /* ---- fused learner loops -------------------------------------------------------- */
-/* use_graph != 0 (xtb_ppo_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer and the predict calls
- * built on it): the call's launches are captured once as a CUDA graph and replayed.  A graph is keyed on every
+/* use_graph != 0 (xtb_ppo_train, xtb_ppo_gauss_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer,
+ * xtb_ppo_gauss_rollout_infer and the predict calls built on them): the call's launches are captured once as a CUDA graph and replayed.  A graph is keyed on every
  * argument plus the kernel-path mode (xtb_set_tc_mode), the fused-heads mode (xtb_set_fuse_heads) and the installed
  * communicator (xtb_set_grad_comm), so a mode change takes effect at the next call.  It is dropped when its net,
  * target net, optimiser or communicator is destroyed, or when its net is rebound (xtb_net_bind). */
@@ -334,6 +340,64 @@ int xtb_actor_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes,
                            int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
                            float* out_dev, float* out_host, float* logits_host, int use_graph, void* stream);
 
+/* ---- PPO with a diagonal Gaussian policy (action_type DiagGaussian): replaces DiagGaussianDist
+ *      (xt/model/tf_dist.py:49-86) as PPO.build_graph wires it (xt/model/ppo/ppo.py:62-95) --------------
+ * mean = the linear pi_latent head [B, A], log_std = the A floats of an XTB_LOGSTD layer, std = exp(log_std).
+ *   neglog_prob(x) = 0.5 log(2 pi) A + 0.5 sum_i ((x_i - mean_i) / std_i)^2 + sum_i log_std_i,  logp = -neglog_prob
+ *   entropy        = sum_i (log_std_i + 0.5 (log(2 pi) + 1))   (state independent)
+ * Actions are unbounded floats: no clipping or squashing, as in the reference. */
+/* DiagGaussianDist.sample + log_prob (tf_dist.py:85-86, ppo.py:82-83): action = mean + std * n, logp computed from
+ * the action.  n from `normals` [batch, adim] if non-NULL, else standard normals drawn with Philox4x32-10(seed, offset)
+ * and Box-Muller: sample b, dimension group g = i / 4 uses counter (b, g, offset_lo, offset_hi) and key (seed_lo,
+ * seed_hi); its four words give uniforms u0..u3 = (x >> 8) 2^-24 + 2^-25 (never 0 or 1, as xtb_categorical_sample) and
+ *   n_{4g}   = sqrt(-2 log u0) cos(2 pi u1),  n_{4g+1} = sqrt(-2 log u0) sin(2 pi u1),
+ *   n_{4g+2} = sqrt(-2 log u2) cos(2 pi u3),  n_{4g+3} = sqrt(-2 log u2) sin(2 pi u3).
+ * action [batch, adim] f32, logp [batch] f32.  adim <= 32. */
+int xtb_diag_gaussian_sample(const float* mean, const float* log_std, int batch, int adim, const float* normals,
+                             uint64_t seed, uint64_t offset, float* action, float* logp, void* stream);
+/* actor_loss_with_entropy + critic_loss (xt/model/ppo/__init__.py:4-25, ppo.py:87-92) on the Gaussian head: as
+ * xtb_ppo_loss_grad with logp = log_prob(action) of the float behaviour action [N, A] (indexed through gather_idx) and
+ * the entropy above.  Writes dmean [B, A], dv [B] and dlog_std [A] (overwritten: the gradient of this minibatch's loss
+ * summed over its samples in a fixed order), adds the loss to *loss_out.  One block: the step is reproducible. */
+int xtb_ppo_gauss_loss_grad(const float* mean, const float* v, const float* log_std, const int32_t* gather_idx,
+                            const float* action, const float* old_logp, const float* adv, const float* old_v,
+                            const float* target_v, int batch, int adim, const xtb_ppo_hyper* hp, float inv_count,
+                            float* dmean, float* dv, float* dlog_std, float* loss_out, void* stream);
+/* PPO.train (ppo.py:111-132) with a Gaussian actor: the loop of xtb_ppo_train (same perm, minibatches, clip, Adam and
+ * data-parallel handling) over the rollout below; logstd_tensor names the XTB_LOGSTD layer (its layer index + 1), whose
+ * width must equal pi_tensor's.  Under the fused-heads conditions of xtb_ppo_train (both heads linear dense layers on
+ * hidden tensors of equal width K, K a multiple of 32 with A <= 8 and K <= 256 or A <= 4 and K <= 512, fused-heads mode
+ * on) both heads, the loss and their backward run in one kernel whose per-block partial sums, the log_std gradient's
+ * included, are reduced in block order: with tensor-core trunk layers the step is bitwise reproducible.  Otherwise every
+ * minibatch runs forward, xtb_ppo_gauss_loss_grad (log_std gradient straight into its slot of the bound gradient
+ * buffer), backward and the optimiser step. */
+typedef struct xtb_ppo_gauss_rollout {
+  const void* obs;            /* [N, H,W,C] uint8 / float */
+  const float* action;        /* [N, A] behaviour actions */
+  const float* old_logp;      /* [N] */
+  const float* adv;           /* [N] */
+  const float* old_v;         /* [N] */
+  const float* target_v;      /* [N] */
+} xtb_ppo_gauss_rollout;
+int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int n_sample, int batch_size,
+                        int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor,
+                        int logstd_tensor, float* loss_per_step, int use_graph, void* stream);
+/* xtb_ppo_rollout_infer for a Gaussian actor: action [n_step, n_env, A] f32 drawn with Philox(seed, *offset_dev + t)
+ * as xtb_diag_gaussian_sample; logp / value [n_step, n_env]; finally *offset_dev += n_step.  Within the fused-inference
+ * limits of xtb_ppo_rollout_infer (linear dense heads on hidden tensors of equal width K, K a multiple of 32, K <= 512,
+ * A <= 8, fused-heads mode on) one kernel evaluates both heads and the sample; otherwise the layer-by-layer forward is
+ * followed by the sampling kernel.  The draws are the same either way. */
+int xtb_ppo_gauss_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
+                                int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
+                                unsigned long long* offset_dev, float* action, float* logp, float* value, int use_graph,
+                                void* stream);
+/* xtb_ppo_predict_host for a Gaussian actor (PPO.predict, ppo.py:104-109): the packed block is
+ * out_dev = [action n_env*A | logp n_env | value n_env] floats, copied to out_host before the synchronise. */
+int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
+                               int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
+                               unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
+                               void* stream);
+
 /* Data-parallel hook (SURVEY 8(e)): called between backward and the optimiser with the flat
  * gradient bucket; must SUM it over ranks on `stream` (e.g. ncclAllReduce).  Called once with
  * grads == NULL before the loop: must return the world size.  While a hook is installed the
@@ -365,7 +429,8 @@ int xtb_net_bench_layer(xtb_net* net, int layer, int which, const void* obs, con
  * 0 = fp32 CUDA-core kernels only (also XTB_TC=0 in the environment).  For A/B parity tests. */
 int xtb_set_tc_mode(int mode);
 /* 1 (default): xtb_ppo_train (and xtb_dqn_train on a dueling head) evaluates both heads, the loss and their backward
- * in one fused kernel; 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call. */
+ * in one fused kernel; 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call.  The same mode
+ * selects the fused heads of xtb_ppo_gauss_train and of the rollout-inference calls. */
 int xtb_set_fuse_heads(int on);
 int xtb_get_tc_mode(void);
 /* Self-test of the wgmma GEMM core on plain fp32 matrices (sizes multiples of 8):

@@ -66,7 +66,8 @@ class PPO(Algorithm):
             ro.obs[sl].copy_(ring["obs"][t0:t0 + n, e], non_blocking=True)
         else:
             self._stage(ro.obs[sl], np.asarray(train_data["cur_state"]), obs_np)
-        self._stage(ro.action[sl], train_data["action"], np.int32)
+        # int32 [n] actions, or float32 [n, A] for a DiagGaussian actor
+        self._stage(ro.action[sl], train_data["action"], np.float32 if ro.action.dim() == 2 else np.int32)
         self._stage(ro.old_logp[sl], train_data["logp"], np.float32)
         if "adv" in train_data:
             self._stage(ro.adv[sl], train_data["adv"], np.float32)

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("XTB_LIB_PATH") or os.path.join(HERE, "lib", "libxtb200.so")   # override: experiment builds (scripts/)
 
 XTB_MAX_LAYERS = 16
-CONV, DENSE, DUELING = 0, 1, 2
+CONV, DENSE, DUELING, LOGSTD = 0, 1, 2, 3
 ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2}
 CLIP_NONE, CLIP_GLOBAL_NORM, CLIP_PER_TENSOR = 0, 1, 2
 
@@ -39,6 +39,11 @@ class PpoHyper(C.Structure):
 class PpoRollout(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("old_logp", C.c_void_p), ("adv", C.c_void_p),
                 ("old_v", C.c_void_p), ("target_v", C.c_void_p)]
+
+
+class PpoGaussRollout(C.Structure):
+    """xtb_ppo_gauss_rollout: as PpoRollout, with float behaviour actions [N, A]."""
+    _fields_ = PpoRollout._fields_
 
 
 class ImpalaTraj(C.Structure):
@@ -105,6 +110,15 @@ _SIGS = {
     "xtb_ppo_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_ppo_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, C.c_int, _P]),
     "xtb_actor_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_diag_gaussian_sample": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "xtb_ppo_gauss_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(PpoHyper), C.c_float,
+                                          _P, _P, _P, _P, _P]),
+    "xtb_ppo_gauss_train": (C.c_int, [_P, _P, C.POINTER(PpoGaussRollout), C.c_int, C.c_int, C.c_int, _P, C.POINTER(PpoHyper),
+                                      C.c_int, C.c_int, C.c_int, _P, C.c_int, _P]),
+    "xtb_ppo_gauss_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P,
+                                              _P, C.c_int, _P]),
+    "xtb_ppo_gauss_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P,
+                                             _P, C.c_int, _P]),
     "xtb_set_grad_hook": (C.c_int, [GRAD_HOOK, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

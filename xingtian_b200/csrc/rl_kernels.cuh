@@ -448,8 +448,8 @@ struct PpoHeadsArgs {
   const float* w_pi; const float* b_pi; const float* w_v; const float* b_v;
   // Parameter-gradient partial sums, one slab of `slab` floats per block, reduced afterwards in block order by
   // bp::grad_reduce_kernel (no atomics: the step is bitwise reproducible).  Slab layout (K hidden units, A actions):
-  // [dW_pi K*A | dW_v K | dbh_pi K | dbh_v K | db_pi A | db_v 1 | loss 1]; dbh_* = bias gradients of the layers that
-  // produced h_pi / h_v (column sums of g).
+  // [dW_pi K*A | dW_v K | dbh_pi K | dbh_v K | db_pi A | db_v 1 | loss 1 (| dlog_std A: LOSS::kLogStd)]; dbh_* = bias
+  // gradients of the layers that produced h_pi / h_v (column sums of g).
   float* part; int slab;
   const int32_t* idx; const int32_t* action; const float* old_logp; const float* adv; const float* old_v; const float* target_v;
   float* logits_out; float* v_out;
@@ -460,17 +460,21 @@ struct PpoHeadsArgs {
   // reduction of the loss slot writes loss_in + this step's loss).
   const float* qn_t; const float* qn_o; const float* reward; const uint8_t* done; const float* disc; const float* loss_in;
   float gamma, huber;
+  // Gaussian PPO (PpoGaussLoss): float behaviour actions [N, A] indexed through idx, and the A floats of pi_logstd
+  const float* action_f; const float* log_std;
 };
 
 // Per-sample loss policies of heads_kernel.  acc[0..A) = h . W_pi (no bias), acc[HEAD_AMAX] = h . W_v; every lane holds
 // the same values.  Fill dl[i] = dloss/d(pi head output i), dv = dloss/d(v head output) (0 for i >= A) and, on lane 0,
-// add the sample's loss to lsum and the bias gradients to dbp / dbv.
+// add the sample's loss to lsum and the bias gradients to dbp / dbv.  A policy with kLogStd also adds, on lane 0, the
+// gradient wrt the state-independent log_std to dls (an extra A slab floats); the others leave dls alone.
 // PPO: categorical actor loss with entropy + clipped critic loss (xt/model/ppo/__init__.py:4-25).
 struct PpoLoss {
+  static constexpr bool kLogStd = false;
   template <int HEAD_AMAX>
   static __device__ __forceinline__ void sample(const PpoHeadsArgs& a, int b, int lane, const float (&acc)[HEAD_AMAX + 1],
                                                 float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
-                                                float& dbv) {
+                                                float& dbv, float (&)[HEAD_AMAX]) {
     const int A = a.A;
     float lg[HEAD_AMAX]; float mx = -INFINITY;
 #pragma unroll
@@ -524,10 +528,11 @@ struct PpoLoss {
 // then the TD target, loss and d(loss)/dq of dqn_loss_kernel.  Only the taken action carries gradient, g = c e_a, so
 // dvalue = c (e_a - 1/A) and dadv = c.
 struct DuelingTdLoss {
+  static constexpr bool kLogStd = false;
   template <int HEAD_AMAX>
   static __device__ __forceinline__ void sample(const PpoHeadsArgs& a, int b, int lane, const float (&acc)[HEAD_AMAX + 1],
                                                 float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
-                                                float& dbv) {
+                                                float& dbv, float (&)[HEAD_AMAX]) {
     const int A = a.A;
     float val[HEAD_AMAX], s = 0.f;
 #pragma unroll
@@ -578,7 +583,7 @@ __global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
   extern __shared__ float sh_dw[];          // [nwarp][nacc] per-warp partial sums in slab layout
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   const int K = a.K, A = a.A, kpl = K / 32;
-  const int nacc = K * A + 3 * K + A + 2;
+  const int nacc = K * A + 3 * K + A + 2 + (LOSS::kLogStd ? A : 0);
   float wpi[HEAD_KPL][HEAD_AMAX], wv[HEAD_KPL];
   float dwp[HEAD_KPL][HEAD_AMAX], dwv[HEAD_KPL];
 #pragma unroll
@@ -593,12 +598,12 @@ __global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
       for (int i = 0; i < HEAD_AMAX; i++) if (i < A) wpi[j][i] = a.w_pi[k * A + i];
     }
   }
-  float dbp[HEAD_AMAX]; float dbv = 0.f, lsum = 0.f;
+  float dbp[HEAD_AMAX], dls[HEAD_AMAX]; float dbv = 0.f, lsum = 0.f;
   float bh_pi[HEAD_KPL], bh_v[HEAD_KPL];
 #pragma unroll
   for (int j = 0; j < HEAD_KPL; j++) { bh_pi[j] = 0.f; bh_v[j] = 0.f; }
 #pragma unroll
-  for (int i = 0; i < HEAD_AMAX; i++) dbp[i] = 0.f;
+  for (int i = 0; i < HEAD_AMAX; i++) { dbp[i] = 0.f; dls[i] = 0.f; }
   for (int b = blockIdx.x * nwarp + warp; b < a.B; b += gridDim.x * nwarp) {
     float hp_[HEAD_KPL], hv_[HEAD_KPL];
     float acc[HEAD_AMAX + 1];
@@ -620,7 +625,7 @@ __global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
     for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
     // ---- loss + d(head outputs): every lane computes the same values
     float dl[HEAD_AMAX], dv;
-    LOSS::template sample<HEAD_AMAX>(a, b, lane, acc, dl, dv, lsum, dbp, dbv);
+    LOSS::template sample<HEAD_AMAX>(a, b, lane, acc, dl, dv, lsum, dbp, dbv, dls);
     // ---- head weight gradients (registers) and gradient wrt the hidden units
 #pragma unroll
     for (int j = 0; j < HEAD_KPL; j++) {
@@ -675,6 +680,10 @@ __global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
     for (int i = 0; i < HEAD_AMAX; i++) if (i < A) row[K * A + 3 * K + i] = dbp[i];
     row[K * A + 3 * K + A] = dbv;
     row[K * A + 3 * K + A + 1] = lsum;
+    if (LOSS::kLogStd) {
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) if (i < A) row[K * A + 3 * K + A + 2 + i] = dls[i];
+    }
   }
   __syncthreads();
   float* out = a.part + (size_t)blockIdx.x * a.slab;
@@ -778,6 +787,239 @@ ppo_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__
       for (int i = 0; i < HEAD_AMAX; i++) if (i == bi) la = lg[i];
       action[b] = bi;
       logp[b] = la - mx - lz;
+      v_out[b] = acc[HEAD_AMAX] + b_v[0];
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Diagonal Gaussian policy of PPO (xt/model/tf_dist.py:49-86, xt/model/ppo/ppo.py:75-83): mean = pi_latent [B, A],
+// log_std = the A floats of the pi_logstd variable, std = exp(log_std).
+// ------------------------------------------------------------------------------------------
+constexpr float kHalfLog2Pi = 0.918938533204672742f;     // 0.5 log(2 pi)
+constexpr float kGaussEntConst = 1.418938533204672742f;  // 0.5 (log(2 pi) + 1)
+
+// standard normals n[0..4) of sample b, dimensions 4g..4g+3: one Philox call (counter (b, g, offset), the uniform
+// mapping of sample_kernel, never 0 or 1) and Box-Muller on the two pairs of its words
+__device__ inline void gauss_normals4(int b, int g, uint64_t seed, uint64_t offset, float (&n)[4]) {
+  uint32_t c[4] = {(uint32_t)b, (uint32_t)g, (uint32_t)(offset & 0xffffffffu), (uint32_t)(offset >> 32)};
+  philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
+#pragma unroll
+  for (int p = 0; p < 2; p++) {
+    const float u0 = (float)(c[2 * p] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
+    const float u1 = (float)(c[2 * p + 1] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
+    const float r = sqrtf(-2.f * logf(u0));
+    float s, co;
+    sincospif(2.f * u1, &s, &co);
+    n[2 * p] = r * co; n[2 * p + 1] = r * s;
+  }
+}
+
+// DiagGaussianDist.sample + log_prob, one thread per sample: x = mean + std n, logp = -neglog_prob(x) computed from x
+// (tf_dist.py:63-66, 85-86).  normals != NULL: n from it; else Philox with offset (or *offset_dev + t_add when
+// offset_dev is set: the device-resident counter of rollout inference).  v_out != NULL: the value head is copied out.
+__global__ void gauss_sample_kernel(const float* __restrict__ mean, const float* __restrict__ log_std, int B, int A,
+                                    const float* __restrict__ normals, uint64_t seed, uint64_t offset,
+                                    const unsigned long long* __restrict__ offset_dev, int t_add, float* __restrict__ action,
+                                    float* __restrict__ logp, const float* __restrict__ v_in, float* __restrict__ v_out) {
+  pdl_wait(); pdl_trigger();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
+  const float* m = mean + (long long)b * A;
+  float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = 0; i < A; i++) {
+    float n;
+    if (normals) {
+      n = normals[(long long)b * A + i];
+    } else {
+      if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
+      n = (i & 3) == 0 ? n4[0] : (i & 3) == 1 ? n4[1] : (i & 3) == 2 ? n4[2] : n4[3];
+    }
+    const float ls = log_std[i], sd = expf(ls);
+    const float x = m[i] + sd * n;
+    const float z = (x - m[i]) / sd;
+    q += z * z; sls += ls;
+    action[(long long)b * A + i] = x;
+  }
+  logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+  if (v_out) v_out[b] = v_in[b];
+}
+
+// actor_loss_with_entropy + critic_loss (xt/model/ppo/__init__.py:4-25) on the Gaussian head, one block, a thread per
+// sample.  With z_i = (x_i - mean_i) / std_i (x = the behaviour action of row idx[b]):
+//   dlogp/dmean_i = z_i / std_i,  dlogp/dlog_std_i = z_i^2 - 1,  dH/dlog_std_i = 1
+// dmean / dv per sample; dlog_std and the loss are summed over the samples in a fixed order (warp butterflies, then the
+// warps in order), so the result is reproducible.  AMAX >= A.
+constexpr int GAUSS_LOSS_THREADS = 256;
+template <int AMAX>
+__global__ void __launch_bounds__(GAUSS_LOSS_THREADS)
+ppo_gauss_loss_kernel(const float* __restrict__ mean, const float* __restrict__ v, const float* __restrict__ log_std,
+                      const int32_t* __restrict__ idx, const float* __restrict__ action, const float* __restrict__ old_logp,
+                      const float* __restrict__ adv, const float* __restrict__ old_v, const float* __restrict__ target_v,
+                      int B, int A, PpoHyperDev hp, float inv_count, float* __restrict__ dmean, float* __restrict__ dv,
+                      float* __restrict__ dlog_std, float* __restrict__ loss_out) {
+  pdl_wait(); pdl_trigger();
+  __shared__ float red[GAUSS_LOSS_THREADS / 32][AMAX + 1];
+  float ls[AMAX], sd[AMAX], acc[AMAX];
+  float H = 0.f, sls = 0.f;
+#pragma unroll
+  for (int i = 0; i < AMAX; i++) {
+    ls[i] = i < A ? log_std[i] : 0.f;
+    sd[i] = expf(ls[i]);
+    acc[i] = 0.f;
+    if (i < A) { H += ls[i] + kGaussEntConst; sls += ls[i]; }
+  }
+  float lsum = 0.f;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const int r = idx ? idx[b] : b;
+    const float* m = mean + (long long)b * A;
+    const float* x = action + (long long)r * A;
+    float z[AMAX], q = 0.f;
+#pragma unroll
+    for (int i = 0; i < AMAX; i++) {
+      z[i] = 0.f;
+      if (i < A) { z[i] = (x[i] - m[i]) / sd[i]; q += z[i] * z[i]; }
+    }
+    const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+    const float ratio = expf(logp_a - old_logp[r]);
+    const float ad = adv[r];
+    const float s1 = ratio * ad;
+    const float s2 = fminf(fmaxf(ratio, 1.f - hp.clip_ratio), 1.f + hp.clip_ratio) * ad;
+    const float surr = fminf(s1, s2);
+    const float dsurr = (s1 <= s2) ? ratio * ad
+                                   : ((ratio >= 1.f - hp.clip_ratio && ratio <= 1.f + hp.clip_ratio) ? ratio * ad : 0.f);
+    const float vv = v[b], R = target_v[r], ov = old_v[r];
+    const float l1 = (vv - R) * (vv - R);
+    const float vc = ov + fminf(fmaxf(vv - ov, -hp.vf_clip), hp.vf_clip);
+    const float l2 = (vc - R) * (vc - R);
+    const float dvl = (l1 >= l2) ? 2.f * (vv - R) : ((vv - ov >= -hp.vf_clip && vv - ov <= hp.vf_clip) ? 2.f * (vc - R) : 0.f);
+    lsum += (-surr - hp.ent_coef * H + hp.critic_coef * 0.5f * fmaxf(l1, l2)) * inv_count;
+    dv[b] = hp.critic_coef * 0.5f * dvl * inv_count;
+#pragma unroll
+    for (int i = 0; i < AMAX; i++) {
+      if (i < A) {
+        dmean[(long long)b * A + i] = -dsurr * (z[i] / sd[i]) * inv_count;
+        acc[i] += (-dsurr * (z[i] * z[i] - 1.f) - hp.ent_coef) * inv_count;
+      }
+    }
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  lsum = warp_sum(lsum);
+  if (lane == 0) red[w][AMAX] = lsum;
+#pragma unroll
+  for (int i = 0; i < AMAX; i++) {
+    const float s = warp_sum(acc[i]);
+    if (lane == 0) red[w][i] = s;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x <= AMAX && ((int)threadIdx.x < A || (int)threadIdx.x == AMAX)) {
+    float s = 0.f;
+    for (int k = 0; k < (int)(blockDim.x >> 5); k++) s += red[k][threadIdx.x];
+    if ((int)threadIdx.x == AMAX) *loss_out += s;
+    else dlog_std[threadIdx.x] = s;
+  }
+}
+
+// heads_kernel policy of the Gaussian PPO step: the loss of ppo_gauss_loss_kernel on mean = h . W_pi + b_pi and
+// v = h . W_v + b_v; the per-sample log_std gradient goes to dls (the extra A slab floats, reduced in block order).
+struct PpoGaussLoss {
+  static constexpr bool kLogStd = true;
+  template <int HEAD_AMAX>
+  static __device__ __forceinline__ void sample(const PpoHeadsArgs& a, int b, int lane, const float (&acc)[HEAD_AMAX + 1],
+                                                float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
+                                                float& dbv, float (&dls)[HEAD_AMAX]) {
+    const int A = a.A;
+    const int r = a.idx ? a.idx[b] : b;
+    const float* x = a.action_f + (long long)r * A;
+    float mean[HEAD_AMAX], sd[HEAD_AMAX], z[HEAD_AMAX], q = 0.f, sls = 0.f, H = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) {
+      mean[i] = 0.f; sd[i] = 1.f; z[i] = 0.f;
+      if (i < A) {
+        const float ls = a.log_std[i];
+        mean[i] = acc[i] + a.b_pi[i];
+        sd[i] = expf(ls);
+        z[i] = (x[i] - mean[i]) / sd[i];
+        q += z[i] * z[i]; sls += ls; H += ls + kGaussEntConst;
+      }
+    }
+    const float vv = acc[HEAD_AMAX] + a.b_v[0];
+    const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+    const float ratio = expf(logp_a - a.old_logp[r]);
+    const float ad = a.adv[r];
+    const float s1 = ratio * ad;
+    const float s2 = fminf(fmaxf(ratio, 1.f - a.hp.clip_ratio), 1.f + a.hp.clip_ratio) * ad;
+    const float surr = fminf(s1, s2);
+    const float dsurr = (s1 <= s2) ? ratio * ad
+                                   : ((ratio >= 1.f - a.hp.clip_ratio && ratio <= 1.f + a.hp.clip_ratio) ? ratio * ad : 0.f);
+    const float R = a.target_v[r], ov = a.old_v[r];
+    const float l1 = (vv - R) * (vv - R);
+    const float vc = ov + fminf(fmaxf(vv - ov, -a.hp.vf_clip), a.hp.vf_clip);
+    const float l2 = (vc - R) * (vc - R);
+    const float dvl = (l1 >= l2) ? 2.f * (vv - R)
+                                 : ((vv - ov >= -a.hp.vf_clip && vv - ov <= a.hp.vf_clip) ? 2.f * (vc - R) : 0.f);
+    dv = a.hp.critic_coef * 0.5f * dvl * a.inv_count;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? -dsurr * (z[i] / sd[i]) * a.inv_count : 0.f;
+    if (lane == 0) {
+      lsum += (-surr - a.hp.ent_coef * H + a.hp.critic_coef * 0.5f * fmaxf(l1, l2)) * a.inv_count;
+      if (a.v_out) a.v_out[b] = vv;
+      dbv += dv;
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) {
+        if (a.logits_out && i < A) a.logits_out[(long long)b * A + i] = mean[i];
+        dbp[i] += dl[i];
+        if (i < A) dls[i] += (-dsurr * (z[i] * z[i] - 1.f) - a.hp.ent_coef) * a.inv_count;
+      }
+    }
+  }
+};
+
+// Gaussian inference heads: mean / value of both dense heads and the sample of gauss_sample_kernel (Philox offset
+// *offset_dev + t_add) in one kernel, one warp per sample; the Gaussian counterpart of ppo_infer_heads_kernel.
+template <int HEAD_KPL, int HEAD_AMAX>
+__global__ void __launch_bounds__(256)
+gauss_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v, const float* __restrict__ w_pi,
+                         const float* __restrict__ b_pi, const float* __restrict__ w_v, const float* __restrict__ b_v,
+                         const float* __restrict__ log_std, int B, int K, int A, uint64_t seed,
+                         const unsigned long long* __restrict__ offset_dev, int t_add, float* __restrict__ action,
+                         float* __restrict__ logp, float* __restrict__ v_out, float* __restrict__ mean_out) {
+  pdl_wait(); pdl_trigger();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  const int kpl = K / 32;
+  const uint64_t offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
+  for (int b = blockIdx.x * nwarp + warp; b < B; b += gridDim.x * nwarp) {
+    float acc[HEAD_AMAX + 1];
+#pragma unroll
+    for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = 0.f;
+#pragma unroll
+    for (int j = 0; j < HEAD_KPL; j++) {
+      if (j < kpl) {
+        int k = lane + 32 * j;
+        float hp = h_pi[(long long)b * K + k], hv = h_v[(long long)b * K + k];
+#pragma unroll
+        for (int i = 0; i < HEAD_AMAX; i++) if (i < A) acc[i] = fmaf(hp, w_pi[k * A + i], acc[i]);
+        acc[HEAD_AMAX] = fmaf(hv, w_v[k], acc[HEAD_AMAX]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
+    if (lane == 0) {
+      float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) {
+        if (i < A) {
+          if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
+          const float m = acc[i] + b_pi[i], ls = log_std[i], sd = expf(ls);
+          const float x = m + sd * n4[i & 3];
+          const float z = (x - m) / sd;
+          q += z * z; sls += ls;
+          action[(long long)b * A + i] = x;
+          if (mean_out) mean_out[(long long)b * A + i] = m;
+        }
+      }
+      logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
       v_out[b] = acc[HEAD_AMAX] + b_v[0];
     }
   }

@@ -339,6 +339,24 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     lp.d = desc->layers[i];
     const auto& d = lp.d;
     if (d.src < 0 || d.src > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: bad src %d", i, d.src); }
+    if (d.kind == XTB_LOGSTD) {
+      // parameter-only: A floats (pi_logstd), no input, no output tensor
+      if (d.src != 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a logstd layer reads no tensor (src must be 0)", i); }
+      if (d.cout < 1 || d.cout > MAX_ADIM) { delete net; return fail(XTB_ERR_ARG, "layer %d: logstd width %d not in [1, %d]", i, d.cout, MAX_ADIM); }
+      if (d.act != XTB_ACT_NONE) { delete net; return fail(XTB_ERR_ARG, "layer %d: a logstd layer has no activation", i); }
+      lp.K = 1; lp.N = d.cout;
+      shp[i + 1] = {1, 1, 0};
+      net->tsize[i + 1] = 0;
+      lp.w_off = off; off += lp.N;
+      lp.b_off = off;
+      net->L.push_back(lp);
+      continue;
+    }
+    {   // no layer reads the (0-wide) tensor of a logstd layer
+      const bool bad_src = d.src > 0 && desc->layers[d.src - 1].kind == XTB_LOGSTD;
+      const bool bad_k = d.kind == XTB_DUELING && d.k > 0 && d.k <= i && desc->layers[d.k - 1].kind == XTB_LOGSTD;
+      if (bad_src || bad_k) { delete net; return fail(XTB_ERR_ARG, "layer %d: reads the tensor of a logstd layer", i); }
+    }
     if (d.kind == XTB_DUELING) {
       // combine of two earlier layers: src = the A-wide stream, k = the 1-wide stream; no parameters
       if (d.src == 0 || d.k == 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer cannot read the observation", i); }
@@ -682,7 +700,9 @@ static cudaError_t ensure_kernel_attrs() {
   for (const void* k : {(const void*)heads_kernel<PpoLoss, 2, 8>, (const void*)heads_kernel<PpoLoss, 8, 4>,
                         (const void*)heads_kernel<PpoLoss, 8, 8>, (const void*)heads_kernel<PpoLoss, 16, 4>,
                         (const void*)heads_kernel<DuelingTdLoss, 2, 8>, (const void*)heads_kernel<DuelingTdLoss, 8, 4>,
-                        (const void*)heads_kernel<DuelingTdLoss, 8, 8>, (const void*)heads_kernel<DuelingTdLoss, 16, 4>})
+                        (const void*)heads_kernel<DuelingTdLoss, 8, 8>, (const void*)heads_kernel<DuelingTdLoss, 16, 4>,
+                        (const void*)heads_kernel<PpoGaussLoss, 2, 8>, (const void*)heads_kernel<PpoGaussLoss, 8, 4>,
+                        (const void*)heads_kernel<PpoGaussLoss, 8, 8>, (const void*)heads_kernel<PpoGaussLoss, 16, 4>})
     if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
   done = true;
   return cudaSuccess;
@@ -1042,6 +1062,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
   float* out = (float*)(net->ws + net->out_off[t]);
   const float* w = P + lp.w_off;
   const float* b = P + lp.b_off;
+  if (lp.d.kind == XTB_LOGSTD) return XTB_OK;   // parameter-only: no output tensor
   if (lp.d.kind == XTB_DUELING) {
     int rc = ensure_f32(net, lp.d.src, B, false, st);
     if (!rc) rc = ensure_f32(net, lp.d.k, B, false, st);
@@ -1085,7 +1106,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
 
 static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, int B, cudaStream_t st, bool bias_done = false) {
   const LayerPlan& lp = net->L[i];
-  if (lp.d.kind == XTB_DUELING) return XTB_OK;   // no parameters
+  if (lp.d.kind == XTB_DUELING || lp.d.kind == XTB_LOGSTD) return XTB_OK;   // no parameters / none fed by a tensor
   int t = i + 1;
   float* dw = net->grads + lp.w_off;
   float* db = net->grads + lp.b_off;
@@ -1255,7 +1276,7 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
     if (rc) return rc;
   }
   for (int t = 1; t <= nl; t++) {
-    if (!((want_f32_mask >> t) & 1u) || (skip_mask & (1u << (t - 1)))) continue;
+    if (!((want_f32_mask >> t) & 1u) || (skip_mask & (1u << (t - 1))) || net->tsize[t] == 0) continue;
     int rc = ensure_f32(net, t, batch, false, st);
     if (rc) return rc;
   }
@@ -1283,7 +1304,7 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
   if (zero_grads) net->pending.clear();      // a fused loss kernel (zero_grads == false) has queued its own reductions
   for (int h = 0; h < n_heads; h++) {
     int t = head_tensors[h];
-    if (t < 1 || t > nl) return fail(XTB_ERR_ARG, "bad head tensor %d", t);
+    if (t < 1 || t > nl || net->tsize[t] == 0) return fail(XTB_ERR_ARG, "bad head tensor %d", t);
     has_grad[t] = 1; written[t] = 1;
     if ((heads_bp_mask >> t) & 1u) net->gbp_ok[t] = 1; else net->gf32_ok[t] = 1;
   }
@@ -1410,6 +1431,34 @@ extern "C" int xtb_ppo_loss_grad(const float* logits, const float* v, const int3
   PpoHyperDev h{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef};
   XLAUNCH(ppo_loss_kernel, (batch + 127) / 128, 128, 0, S(stream), logits, v, gather_idx, action, old_logp, adv, old_v,
                                                               target_v, batch, adim, h, inv_count, dlogits, dv, loss_out);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_diag_gaussian_sample(const float* mean, const float* log_std, int batch, int adim, const float* normals,
+                                        uint64_t seed, uint64_t offset, float* action, float* logp, void* stream) {
+  if (!mean || !log_std || !action || !logp || batch <= 0 || adim <= 0 || adim > MAX_ADIM)
+    return fail(XTB_ERR_ARG, "xtb_diag_gaussian_sample: bad argument");
+  XLAUNCH(gauss_sample_kernel, (batch + 127) / 128, 128, 0, S(stream), mean, log_std, batch, adim, normals, seed, offset,
+          (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_ppo_gauss_loss_grad(const float* mean, const float* v, const float* log_std, const int32_t* gather_idx,
+                                       const float* action, const float* old_logp, const float* adv, const float* old_v,
+                                       const float* target_v, int batch, int adim, const xtb_ppo_hyper* hp, float inv_count,
+                                       float* dmean, float* dv, float* dlog_std, float* loss_out, void* stream) {
+  if (!mean || !v || !log_std || !action || !old_logp || !adv || !old_v || !target_v || !hp || !dmean || !dv || !dlog_std || !loss_out)
+    return fail(XTB_ERR_ARG, "xtb_ppo_gauss_loss_grad: null pointer");
+  if (batch <= 0 || adim <= 0 || adim > MAX_ADIM) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_loss_grad: batch/adim out of range");
+  PpoHyperDev h{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef};
+  if (adim <= 8)
+    XLAUNCH(ppo_gauss_loss_kernel<8>, 1, GAUSS_LOSS_THREADS, 0, S(stream), mean, v, log_std, gather_idx, action, old_logp, adv, old_v,
+            target_v, batch, adim, h, inv_count, dmean, dv, dlog_std, loss_out);
+  else
+    XLAUNCH(ppo_gauss_loss_kernel<MAX_ADIM>, 1, GAUSS_LOSS_THREADS, 0, S(stream), mean, v, log_std, gather_idx, action, old_logp, adv,
+            old_v, target_v, batch, adim, h, inv_count, dmean, dv, dlog_std, loss_out);
   LAUNCH_CHECK();
   return XTB_OK;
 }
@@ -1666,12 +1715,13 @@ extern "C" int xtb_set_grad_hook(xtb_grad_hook hook, void* user) {
 // A captured graph bakes in every kernel argument, so its key holds everything the capture reads.  capture_key()
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
-enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain };
+enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kPpoGaussTrain,
+                kGaussRolloutInfer };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[4];    // net, target, opt, comm: destroying one, or rebinding a net, drops the graph
   uint64_t mode[2];      // kernel-path and fused-heads modes
-  uint64_t arg[18];      // every pointer and scalar argument; floats by bit pattern
+  uint64_t arg[21];      // every pointer and scalar argument; floats by bit pattern
   bool operator<(const CaptureKey& o) const { return memcmp(this, &o, sizeof(CaptureKey)) < 0; }
 };
 template <class T> static uint64_t key_word(T v) {
@@ -1755,85 +1805,20 @@ static void launch_heads(const PpoHeadsArgs& a, int blocks, size_t shb, cudaStre
   else XLAUNCH((heads_kernel<LOSS, 16, 4>), blocks, 256, shb, st, a);
 }
 
-static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
-                            const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t,
-                            float* loss_per_step, float inv_world, void* stream) {
+// The epoch x minibatch loop of PPO.train (xt/model/ppo/ppo.py:111-132): minibatch k of epoch e holds rows
+// perm[e*N + k*B ...] (the last one ragged).  minibatch(idx, mb, loss) enqueues its forward, loss and backward; the
+// gradient hook and the optimiser step follow.
+template <class STEP>
+static int ppo_epoch_loop(xtb_net* net, xtb_adam* opt, int N, int B, int E, const int32_t* perm, float* loss_per_step,
+                          void* stream, STEP&& minibatch) {
   int steps_per_epoch = (N + B - 1) / B;
   CUDA_TRY(cudaMemsetAsync(loss_per_step, 0, sizeof(float) * E * steps_per_epoch, S(stream)));
-  int heads[2] = {pi_t, v_t};
-  int adim = net->tsize[pi_t];
-  // fused heads: both heads are linear dense layers on hidden tensors of equal width
-  const LayerPlan& lpi = net->L[pi_t - 1];
-  const LayerPlan& lv = net->L[v_t - 1];
-  bool fuse = g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
-              lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && heads_fit(lpi.K, adim);
-  unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
   int step = 0;
   for (int e = 0; e < E; e++) {
     for (int s0 = 0; s0 < N; s0 += B, step++) {
       int mb = std::min(B, N - s0);
-      const int32_t* idx = perm + (long long)e * N + s0;
-      // fp32 row-major copies: the hidden tensors the fused heads read, or the head outputs the loss kernel reads
-      unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
-      int rc = net_forward_impl(net, nullptr, ro->obs, idx, mb, stream, skip, want);
+      int rc = minibatch(perm + (long long)e * N + s0, mb, loss_per_step + step);
       if (rc) return rc;
-      if (fuse) {
-        CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
-        net->pending.clear();
-        PpoHeadsArgs a;
-        a.h_pi = (const float*)(net->ws + net->out_off[lpi.d.src]); a.h_v = (const float*)(net->ws + net->out_off[lv.d.src]);
-        a.g_pi = (float*)(net->ws + net->gout_off[lpi.d.src]); a.g_v = (float*)(net->ws + net->gout_off[lv.d.src]);
-        // hidden-layer gradients go straight into batch-planar planes when the hidden layer runs on tensor cores
-        const bool bp_pi = use_tc(net->L[lpi.d.src - 1]) && net->plane_elems[lpi.d.src] > 0;
-        const bool bp_v = use_tc(net->L[lv.d.src - 1]) && net->plane_elems[lv.d.src] > 0;
-        a.gp_hi = bp_pi ? gout_bp(net, lpi.d.src).hi : nullptr; a.gp_lo = net->plane_elems[lpi.d.src];
-        a.gv_hi = bp_v ? gout_bp(net, lv.d.src).hi : nullptr; a.gv_lo = net->plane_elems[lv.d.src];
-        a.pitch = net->pitch;
-        a.w_pi = net->params + lpi.w_off; a.b_pi = net->params + lpi.b_off; a.w_v = net->params + lv.w_off; a.b_v = net->params + lv.b_off;
-        // the hidden layers' bias gradients (column sums of g) when they are dense and only feed the heads
-        auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], tsr) && !(skip & (1u << j))) return false; return true; };
-        bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src);
-        bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src);
-        unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
-        a.idx = idx; a.action = ro->action; a.old_logp = ro->old_logp; a.adv = ro->adv; a.old_v = ro->old_v; a.target_v = ro->target_v;
-        a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
-        a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = lpi.src_act; a.act_v = lv.src_act; a.shared = lpi.d.src == lv.d.src ? 1 : 0;
-        a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
-        int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
-        const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2;
-        a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
-        size_t shb = (size_t)8 * nacc * sizeof(float);
-        { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
-        launch_heads<PpoLoss>(a, blocks, shb, S(stream));
-        LAUNCH_CHECK();
-        {   // ordered reduction of the per-block slabs (queued; runs with the other partial sums at the end of backward)
-          auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
-            bp::RedSeg r;
-            memset(&r, 0, sizeof r);
-            r.part = a.part + off; r.n_slabs = blocks; r.slab = a.slab; r.count = count; r.kind = 1;
-            r.dst_off = dst_off; r.alpha = 1.f; r.dst_ptr = dst_ptr;
-            net->pending.push_back(r);
-          };
-          seg(0, HK * adim, lpi.w_off, nullptr);
-          seg(HK * adim, HK, lv.w_off, nullptr);
-          if (bh_pi_ok) seg(HK * adim + HK, HK, net->L[lpi.d.src - 1].b_off, nullptr);
-          if (!a.shared && bh_v_ok) seg(HK * adim + 2 * HK, HK, net->L[lv.d.src - 1].b_off, nullptr);
-          seg(HK * adim + 3 * HK, adim, lpi.b_off, nullptr);
-          seg(HK * adim + 3 * HK + adim, 1, lv.b_off, nullptr);
-          seg(HK * adim + 3 * HK + adim + 1, 1, 0, loss_per_step + step);
-        }
-        int srcs[2] = {lpi.d.src, lv.d.src};
-        unsigned hbp = (bp_pi ? (1u << lpi.d.src) : 0u) | (bp_v ? (1u << lv.d.src) : 0u);   // the fused kernel wrote planes there
-        rc = net_backward_impl(net, ro->obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm);
-        if (rc) return rc;
-      } else {
-        rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, ro->action, ro->old_logp,
-                               ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
-                               xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), loss_per_step + step, stream);
-        if (rc) return rc;
-        rc = net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, true, 0u, 0u, g_comm);
-        if (rc) return rc;
-      }
       if (g_grad_hook && !g_comm) {
         rc = g_grad_hook(g_grad_hook_user, net->grads, net->n_params, stream);
         if (rc) return fail(XTB_ERR_STATE, "gradient hook failed with %d", rc);
@@ -1842,6 +1827,160 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* 
       if (rc) return rc;
     }
   }
+  return XTB_OK;
+}
+
+// loss / gradient scale of the PPO loops: 1 / world when data parallel (communicator or gradient hook), else 1
+static float ppo_inv_world() {
+  if (g_comm) return 1.f / g_comm->world;
+  if (g_grad_hook) {   // the hook sums gradients over ranks; every rank holds B/world samples
+    int rc = g_grad_hook(g_grad_hook_user, nullptr, 0, nullptr);   // query: returns world size when grads == NULL
+    return 1.f / (rc > 0 ? rc : 1);
+  }
+  return 1.f;
+}
+
+// Fused PPO heads of tensors pi_t / v_t: both heads are linear dense layers on hidden (non-observation) tensors of equal
+// width within the heads_kernel limits, and the fused-heads mode is on
+static bool ppo_heads_fusable(const xtb_net* net, int pi_t, int v_t) {
+  const LayerPlan& lpi = net->L[pi_t - 1];
+  const LayerPlan& lv = net->L[v_t - 1];
+  return g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
+         lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && heads_fit(lpi.K, net->tsize[pi_t]);
+}
+
+// One fused PPO minibatch after the forward of the layers below the heads: heads_kernel<LOSS> evaluates both heads, the
+// loss and their backward, writes the gradient wrt the hidden tensors (straight into their planes when the hidden layer
+// runs on tensor cores), and its per-block slabs are queued for the ordered reduction at the end of the backward pass of
+// the layers below.  `a` carries the loss inputs (idx, rollout arrays, hyper-parameters); ls_off >= 0: the offset of
+// the log_std floats whose gradient the policy adds to the slab (LOSS::kLogStd).
+template <class LOSS>
+static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, int pi_t, int v_t, unsigned skip,
+                           long long ls_off, float* step_loss, void* stream) {
+  const LayerPlan& lpi = net->L[pi_t - 1];
+  const LayerPlan& lv = net->L[v_t - 1];
+  const int adim = net->tsize[pi_t];
+  const int32_t* idx = a.idx;
+  CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
+  net->pending.clear();
+  a.h_pi = (const float*)(net->ws + net->out_off[lpi.d.src]); a.h_v = (const float*)(net->ws + net->out_off[lv.d.src]);
+  a.g_pi = (float*)(net->ws + net->gout_off[lpi.d.src]); a.g_v = (float*)(net->ws + net->gout_off[lv.d.src]);
+  // hidden-layer gradients go straight into batch-planar planes when the hidden layer runs on tensor cores
+  const bool bp_pi = use_tc(net->L[lpi.d.src - 1]) && net->plane_elems[lpi.d.src] > 0;
+  const bool bp_v = use_tc(net->L[lv.d.src - 1]) && net->plane_elems[lv.d.src] > 0;
+  a.gp_hi = bp_pi ? gout_bp(net, lpi.d.src).hi : nullptr; a.gp_lo = net->plane_elems[lpi.d.src];
+  a.gv_hi = bp_v ? gout_bp(net, lv.d.src).hi : nullptr; a.gv_lo = net->plane_elems[lv.d.src];
+  a.pitch = net->pitch;
+  a.w_pi = net->params + lpi.w_off; a.b_pi = net->params + lpi.b_off; a.w_v = net->params + lv.w_off; a.b_v = net->params + lv.b_off;
+  // the hidden layers' bias gradients (column sums of g) when they are dense and only feed the heads
+  auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], tsr) && !(skip & (1u << j))) return false; return true; };
+  bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src);
+  bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src);
+  unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
+  a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
+  a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = lpi.src_act; a.act_v = lv.src_act; a.shared = lpi.d.src == lv.d.src ? 1 : 0;
+  int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
+  const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2 + (LOSS::kLogStd ? adim : 0);
+  a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
+  size_t shb = (size_t)8 * nacc * sizeof(float);
+  { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
+  launch_heads<LOSS>(a, blocks, shb, S(stream));
+  LAUNCH_CHECK();
+  {   // ordered reduction of the per-block slabs (queued; runs with the other partial sums at the end of backward)
+    auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
+      bp::RedSeg r;
+      memset(&r, 0, sizeof r);
+      r.part = a.part + off; r.n_slabs = blocks; r.slab = a.slab; r.count = count; r.kind = 1;
+      r.dst_off = dst_off; r.alpha = 1.f; r.dst_ptr = dst_ptr;
+      net->pending.push_back(r);
+    };
+    seg(0, HK * adim, lpi.w_off, nullptr);
+    seg(HK * adim, HK, lv.w_off, nullptr);
+    if (bh_pi_ok) seg(HK * adim + HK, HK, net->L[lpi.d.src - 1].b_off, nullptr);
+    if (!a.shared && bh_v_ok) seg(HK * adim + 2 * HK, HK, net->L[lv.d.src - 1].b_off, nullptr);
+    seg(HK * adim + 3 * HK, adim, lpi.b_off, nullptr);
+    seg(HK * adim + 3 * HK + adim, 1, lv.b_off, nullptr);
+    seg(HK * adim + 3 * HK + adim + 1, 1, 0, step_loss);
+    if (LOSS::kLogStd) seg(HK * adim + 3 * HK + adim + 2, adim, ls_off, nullptr);
+  }
+  int srcs[2] = {lpi.d.src, lv.d.src};
+  unsigned hbp = (bp_pi ? (1u << lpi.d.src) : 0u) | (bp_v ? (1u << lv.d.src) : 0u);   // the fused kernel wrote planes there
+  return net_backward_impl(net, obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm);
+}
+
+static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
+                            const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t,
+                            float* loss_per_step, float inv_world, void* stream) {
+  int heads[2] = {pi_t, v_t};
+  int adim = net->tsize[pi_t];
+  const LayerPlan& lpi = net->L[pi_t - 1];
+  const LayerPlan& lv = net->L[v_t - 1];
+  const bool fuse = ppo_heads_fusable(net, pi_t, v_t);
+  unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
+  return ppo_epoch_loop(net, opt, N, B, E, perm, loss_per_step, stream, [&](const int32_t* idx, int mb, float* step_loss) -> int {
+      // fp32 row-major copies: the hidden tensors the fused heads read, or the head outputs the loss kernel reads
+      unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
+      int rc = net_forward_impl(net, nullptr, ro->obs, idx, mb, stream, skip, want);
+      if (rc) return rc;
+      if (fuse) {
+        PpoHeadsArgs a;
+        memset(&a, 0, sizeof a);
+        a.idx = idx; a.action = ro->action; a.old_logp = ro->old_logp; a.adv = ro->adv; a.old_v = ro->old_v; a.target_v = ro->target_v;
+        a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
+        return ppo_heads_fused<PpoLoss>(net, ro->obs, a, mb, pi_t, v_t, skip, -1, step_loss, stream);
+      }
+      rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, ro->action, ro->old_logp,
+                             ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
+                             xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), step_loss, stream);
+      if (rc) return rc;
+      return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, true, 0u, 0u, g_comm);
+  });
+}
+
+// The Gaussian policy: under the fused-heads conditions of xtb_ppo_train one heads_kernel<PpoGaussLoss> launch per
+// minibatch (the log_std gradient is A more slab floats, reduced in block order into its slot); otherwise layer by
+// layer: forward, xtb_ppo_gauss_loss_grad (the log_std gradient straight into its slot of the zeroed gradient bucket),
+// then the backward pass of the network, which keeps that slot.
+static int ppo_gauss_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int N, int B, int E,
+                                  const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t,
+                                  float* loss_per_step, float inv_world, void* stream) {
+  int heads[2] = {pi_t, v_t};
+  const int adim = net->tsize[pi_t];
+  const long long ls_off = net->L[ls_t - 1].w_off;
+  const LayerPlan& lpi = net->L[pi_t - 1];
+  const LayerPlan& lv = net->L[v_t - 1];
+  const bool fuse = ppo_heads_fusable(net, pi_t, v_t);
+  const unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
+  return ppo_epoch_loop(net, opt, N, B, E, perm, loss_per_step, stream, [&](const int32_t* idx, int mb, float* step_loss) -> int {
+    const unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
+    int rc = net_forward_impl(net, nullptr, ro->obs, idx, mb, stream, skip, want);
+    if (rc) return rc;
+    if (fuse) {
+      PpoHeadsArgs a;
+      memset(&a, 0, sizeof a);
+      a.idx = idx; a.action_f = ro->action; a.log_std = net->params + ls_off; a.old_logp = ro->old_logp; a.adv = ro->adv;
+      a.old_v = ro->old_v; a.target_v = ro->target_v;
+      a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
+      return ppo_heads_fused<PpoGaussLoss>(net, ro->obs, a, mb, pi_t, v_t, skip, ls_off, step_loss, stream);
+    }
+    CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
+    rc = xtb_ppo_gauss_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), net->params + ls_off, idx, ro->action,
+                                 ro->old_logp, ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
+                                 xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), net->grads + ls_off, step_loss,
+                                 stream);
+    if (rc) return rc;
+    return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, false, 0u, 0u, g_comm);
+  });
+}
+
+// head tensors of the Gaussian entry points: mean (pi_t), value (v_t, 1 wide) and the logstd layer's tensor (ls_t) of
+// the same width as the mean
+static int gauss_heads_check(const char* fn, const xtb_net* net, int pi_t, int v_t, int ls_t) {
+  const int nl = (int)net->L.size();
+  if (pi_t < 1 || pi_t > nl || v_t < 1 || v_t > nl || ls_t < 1 || ls_t > nl || net->tsize[v_t] != 1)
+    return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
+  const LayerPlan& ls = net->L[ls_t - 1];
+  if (ls.d.kind != XTB_LOGSTD || ls.N != net->tsize[pi_t]) return fail(XTB_ERR_ARG, "%s: tensor %d is not a logstd layer of the mean's width", fn, ls_t);
   return XTB_OK;
 }
 
@@ -1855,19 +1994,33 @@ extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout*
   int nl = (int)net->L.size();
   if (pi_tensor < 1 || pi_tensor > nl || v_tensor < 1 || v_tensor > nl || net->tsize[v_tensor] != 1)
     return fail(XTB_ERR_ARG, "xtb_ppo_train: bad head tensors");
-  float inv_world = 1.f;
-  if (g_comm) inv_world = 1.f / g_comm->world;
-  else if (g_grad_hook) {   // data-parallel: the hook sums gradients over ranks; every rank holds B/world samples
-    int world = 1;
-    int rc = g_grad_hook(g_grad_hook_user, nullptr, 0, nullptr);   // query: returns world size when grads == NULL
-    if (rc > 0) world = rc;
-    inv_world = 1.f / world;
-  }
+  const float inv_world = ppo_inv_world();
   return run_graph(capture_key(kPpoTrain, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v,
                                perm, loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
                                hp->critic_coef, pi_tensor, v_tensor),
                    use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
     return ppo_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, loss_per_step, inv_world, st);
+  });
+}
+
+extern "C" int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int n_sample, int batch_size,
+                                   int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor,
+                                   int logstd_tensor, float* loss_per_step, int use_graph, void* stream) {
+  if (!net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v || !perm || !hp ||
+      !loss_per_step)
+    return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: null pointer");
+  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_ppo_gauss_train: net not bound");
+  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: optimiser/net size mismatch");
+  if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: bad sizes");
+  if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
+  if (int rc = gauss_heads_check("xtb_ppo_gauss_train", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
+  const float inv_world = ppo_inv_world();
+  return run_graph(capture_key(kPpoGaussTrain, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v,
+                               ro->target_v, perm, loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef,
+                               hp->vf_clip, hp->critic_coef, pi_tensor, v_tensor, logstd_tensor),
+                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
+    return ppo_gauss_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, logstd_tensor,
+                                  loss_per_step, inv_world, st);
   });
 }
 
@@ -2160,6 +2313,59 @@ extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_
   });
 }
 
+// Gaussian actor: per step the forward of the layers below the heads and gauss_infer_heads_kernel (both heads and the
+// sample) within the fused-inference limits of xtb_ppo_rollout_infer; otherwise every layer, then gauss_sample_kernel
+extern "C" int xtb_ppo_gauss_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
+                                           int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
+                                           unsigned long long* offset_dev, float* action, float* logp, float* value, int use_graph,
+                                           void* stream) {
+  if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_rollout_infer: null pointer");
+  if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_rollout_infer: bad sizes");
+  if (int rc = gauss_heads_check("xtb_ppo_gauss_rollout_infer", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
+  return run_graph(capture_key(kGaussRolloutInfer, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value, n_env, n_step,
+                               pi_tensor, v_tensor, logstd_tensor, seed),
+                   use_graph, stream, [&](void* st) -> int {
+    const int adim = net->tsize[pi_tensor];
+    const float* log_std = net->params + net->L[logstd_tensor - 1].w_off;
+    const LayerPlan& lpi = net->L[pi_tensor - 1];
+    const LayerPlan& lv = net->L[v_tensor - 1];
+    const int kpl = lpi.K / 32;
+    // the fused-inference limits of rollout_infer_launch: both heads in gauss_infer_heads_kernel
+    const bool fuse = g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
+                      lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && lpi.K % 32 == 0 && adim <= 8 && kpl <= 16;
+    const unsigned skip = fuse ? ((1u << (pi_tensor - 1)) | (1u << (v_tensor - 1))) : 0u;
+    const unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_tensor) | (1u << v_tensor));
+    // step_idx NULL: step t reads observation rows t*n_env .. (t+1)*n_env - 1
+    const size_t row_bytes = (size_t)net->tsize[0] * (net->desc.input_u8 ? 1 : sizeof(float));
+    for (int t = 0; t < n_step; t++) {
+      const void* obs_t = step_idx ? obs : (const void*)((const char*)obs + (size_t)t * n_env * row_bytes);
+      int rc = net_forward_impl(net, nullptr, obs_t, step_idx ? step_idx + (long long)t * n_env : nullptr, n_env, st, skip, want);
+      if (rc) return rc;
+      float* a_t = action + (long long)t * n_env * adim; float* lp_t = logp + (long long)t * n_env; float* v_o = value + (long long)t * n_env;
+      if (fuse) {
+        const float* hp = (const float*)(net->ws + net->out_off[lpi.d.src]);
+        const float* hv = (const float*)(net->ws + net->out_off[lv.d.src]);
+        const float *wp = net->params + lpi.w_off, *bp = net->params + lpi.b_off, *wv = net->params + lv.w_off, *bv = net->params + lv.b_off;
+        const int blocks = std::max(1, std::min(kSMs, (n_env + 7) / 8));
+        const unsigned long long* od = offset_dev;
+        float* mean_out = xtb_net_tensor(net, pi_tensor);
+        if (kpl <= 2) XLAUNCH((gauss_infer_heads_kernel<2, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
+        else if (kpl <= 8 && adim <= 4) XLAUNCH((gauss_infer_heads_kernel<8, 4>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
+        else if (kpl <= 8) XLAUNCH((gauss_infer_heads_kernel<8, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
+        else XLAUNCH((gauss_infer_heads_kernel<16, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
+      } else {
+        XLAUNCH(gauss_sample_kernel, (n_env + 127) / 128, 128, 0, S(st), (const float*)xtb_net_tensor(net, pi_tensor), log_std, n_env,
+                adim, (const float*)nullptr, seed, (uint64_t)0, (const unsigned long long*)offset_dev, t, a_t, lp_t,
+                (const float*)xtb_net_tensor(net, v_tensor), v_o);
+      }
+      LAUNCH_CHECK();
+    }
+    XLAUNCH(bump_counter_kernel, 1, 1, 0, S(st), offset_dev, n_step);
+    LAUNCH_CHECK();
+    return XTB_OK;
+  });
+}
+
 // ------------------------------------------------------------------------------------------
 // staging helpers
 // ------------------------------------------------------------------------------------------
@@ -2204,6 +2410,24 @@ extern "C" int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t o
                                     float* out_dev, float* out_host, int use_graph, void* stream) {
   return xtb_actor_predict_host(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, seed, offset_dev, out_dev, out_host,
                                 nullptr, use_graph, stream);
+}
+extern "C" int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
+                                          int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
+                                          unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
+                                          void* stream) {
+  if (!net || !obs_host || !obs_dev || !out_dev || !out_host) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_predict_host: null pointer");
+  if (int rc = gauss_heads_check("xtb_ppo_gauss_predict_host", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
+  const size_t adim = (size_t)net->tsize[pi_tensor];
+  StreamScope sc;
+  int src = sc.begin(stream, use_graph != 0);
+  if (src) return src;
+  CUDA_TRY(xtb::Stager::instance().stage_h2d(obs_dev, obs_host, obs_bytes, sc.st));
+  int rc = xtb_ppo_gauss_rollout_infer(net, obs_dev, nullptr, n_env, 1, pi_tensor, v_tensor, logstd_tensor, seed, offset_dev, out_dev,
+                                       out_dev + adim * n_env, out_dev + (adim + 1) * n_env, use_graph, (void*)sc.st);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(out_host, out_dev, sizeof(float) * (adim + 2) * (size_t)n_env, cudaMemcpyDeviceToHost, sc.st));
+  CUDA_TRY(cudaStreamSynchronize(sc.st));
+  return sc.end();
 }
 extern "C" int xtb_copy_d2h(void* dst, const void* src, size_t bytes, void* stream) {
   CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S(stream)));

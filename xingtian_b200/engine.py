@@ -38,7 +38,9 @@ class Net(object):
     """One network (layers = list of (name, kind, src_name, spec)) living in device memory.
 
     kind "dueling": (name, "dueling", (value_src, adv_src), {}) combines an A-wide and a 1-wide earlier tensor into
-    Q = adv + (value - mean(value)); it has no parameters."""
+    Q = adv + (value - mean(value)); it has no parameters.
+    kind "logstd": (name, "logstd", None, dict(n=A)) is a parameter-only layer (PPO's pi_logstd): A floats under the
+    weight name `name` with shape (1, A); it reads and produces no tensor."""
 
     def __init__(self, arch, max_batch, device="cuda:0"):
         require_cuda()
@@ -61,6 +63,9 @@ class Net(object):
             if kind == "dueling":
                 ld.kind, ld.src, ld.k, ld.act = capi.DUELING, self.tid[src[0]], self.tid[src[1]], capi.ACT[None]
                 continue
+            if kind == "logstd":
+                ld.kind, ld.src, ld.cout, ld.act = capi.LOGSTD, 0, sp["n"], capi.ACT[None]
+                continue
             ld.kind = capi.CONV if kind == "conv" else capi.DENSE
             ld.src = self.tid[src]
             ld.act = capi.ACT[sp.get("act")]
@@ -81,6 +86,9 @@ class Net(object):
                 continue
             ko, bo, kr, nc = C.c_longlong(), C.c_longlong(), C.c_int(), C.c_int()
             check(self.lib.xtb_net_layer_params(self.handle, i, C.byref(ko), C.byref(bo), C.byref(kr), C.byref(nc)))
+            if kind == "logstd":
+                self.ptable[name] = (ko.value, (kr.value, nc.value))
+                continue
             if kind == "conv":
                 kshape = (sp["k"], sp["k"], in_shapes[src][-1], sp["cout"])
             else:
@@ -131,7 +139,7 @@ class Net(object):
         p = capi.LayerPlan()
         check(self.lib.xtb_net_layer_plan(self.handle, int(i), C.byref(p)))
         out = {name: int(getattr(p, name)) for name, _ in capi.LayerPlan._fields_}
-        out["kind"] = {capi.CONV: "conv", capi.DENSE: "dense", capi.DUELING: "dueling"}[p.kind]
+        out["kind"] = {capi.CONV: "conv", capi.DENSE: "dense", capi.DUELING: "dueling", capi.LOGSTD: "logstd"}[p.kind]
         for k in ("tc", "s2d", "w_res"):
             out[k] = bool(out[k])
         return out
@@ -141,6 +149,8 @@ class Net(object):
         for name, kind, src, sp in self.arch["layers"]:
             if kind == "dueling":
                 shapes[name] = shapes[src[0]]
+                continue
+            if kind == "logstd":
                 continue
             ish = shapes[src]
             if kind == "conv":

@@ -34,23 +34,30 @@ def _towers(state_dim, hidden_sizes, activation, share, filters):
     return layers, tails
 
 
-def ppo_cnn(state_dim, action_dim, hidden_sizes, activation, vf_share_layers):
-    """get_cnn_backbone, xt/model/model_utils.py:49-80."""
+def _ppo_heads(layers, tails, action_dim, diag_gaussian):
+    layers.append(("pi_latent", "dense", tails.get("shared", tails.get("pi")), dict(n=action_dim, act=None)))
+    layers.append(("output_value", "dense", tails.get("shared", tails.get("v")), dict(n=1, act=None)))
+    if diag_gaussian:
+        # tf.get_variable('pi_logstd', (1, A)) is created after the Keras model (xt/model/ppo/ppo.py:75-78), so it is
+        # the last variable TFVariables lists
+        layers.append(("pi_logstd", "logstd", None, dict(n=action_dim)))
+
+
+def ppo_cnn(state_dim, action_dim, hidden_sizes, activation, vf_share_layers, diag_gaussian=False):
+    """get_cnn_backbone, xt/model/model_utils.py:49-80; diag_gaussian appends the pi_logstd variable."""
     key = tuple(state_dim[:2])
     if len(state_dim) != 3 or key not in _FILTERS_PPO:
         raise ValueError("Without default architecture for obs shape {}".format(list(state_dim)))
     layers, tails = _towers(state_dim, hidden_sizes, activation, vf_share_layers, _FILTERS_PPO[key])
-    layers.append(("pi_latent", "dense", tails.get("shared", tails.get("pi")), dict(n=action_dim, act=None)))
-    layers.append(("output_value", "dense", tails.get("shared", tails.get("v")), dict(n=1, act=None)))
+    _ppo_heads(layers, tails, action_dim, diag_gaussian)
     return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0, layers=layers,
                 outputs=["pi_latent", "output_value"])
 
 
-def ppo_mlp(state_dim, action_dim, hidden_sizes, activation, vf_share_layers):
-    """get_mlp_backbone, xt/model/model_utils.py:22-46."""
+def ppo_mlp(state_dim, action_dim, hidden_sizes, activation, vf_share_layers, diag_gaussian=False):
+    """get_mlp_backbone, xt/model/model_utils.py:22-46; diag_gaussian appends the pi_logstd variable."""
     layers, tails = _towers(state_dim, hidden_sizes, activation, vf_share_layers, None)
-    layers.append(("pi_latent", "dense", tails.get("shared", tails.get("pi")), dict(n=action_dim, act=None)))
-    layers.append(("output_value", "dense", tails.get("shared", tails.get("v")), dict(n=1, act=None)))
+    _ppo_heads(layers, tails, action_dim, diag_gaussian)
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
                 outputs=["pi_latent", "output_value"])
 

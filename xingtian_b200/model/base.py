@@ -11,10 +11,10 @@ from ..engine import Net, require_cuda
 
 
 def glorot_uniform_(net, rng):
-    """Keras default initialisation: glorot_uniform kernels, zero biases."""
+    """Keras default initialisation: glorot_uniform kernels, zero biases (and zero pi_logstd, ppo.py:77)."""
     host = np.zeros(net.n_params, np.float32)
     for name, (off, shape) in net.ptable.items():
-        if name.endswith("/bias"):
+        if not name.endswith("/kernel"):
             continue
         if len(shape) == 4:
             rf = shape[0] * shape[1]

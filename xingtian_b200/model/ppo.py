@@ -40,23 +40,30 @@ def minibatch_order(nbatch, num_sgd_iter):
 
 
 class DeviceRollout(object):
-    """Device-resident PPO rollout (grow-only, so CUDA-graph pointers stay valid)."""
+    """Device-resident PPO rollout (grow-only, so CUDA-graph pointers stay valid).  With `action_dim` (a DiagGaussian
+    actor) the behaviour actions are float32 [N, action_dim], else int32 [N]."""
 
     FIELDS = (("action", torch.int32), ("old_logp", torch.float32), ("adv", torch.float32),
               ("old_v", torch.float32), ("target_v", torch.float32))
 
-    def __init__(self, state_dim, obs_dtype, device):
+    def __init__(self, state_dim, obs_dtype, device, action_dim=None):
         self.state_dim, self.obs_dtype, self.device = tuple(state_dim), obs_dtype, device
+        self.action_dim = action_dim
         self.capacity = 0
         self.obs = None
         self.n = 0
+
+    def _field(self, key, dt, cap):
+        if key == "action" and self.action_dim is not None:
+            return torch.empty((cap, self.action_dim), dtype=torch.float32, device=self.device)
+        return torch.empty(cap, dtype=dt, device=self.device)
 
     def reserve(self, n):
         if n <= self.capacity:
             return
         cap = max(n, int(self.capacity * 1.5))
         obs = torch.empty((cap,) + self.state_dim, dtype=self.obs_dtype, device=self.device)
-        new = {k: torch.empty(cap, dtype=dt, device=self.device) for k, dt in self.FIELDS}
+        new = {k: self._field(k, dt, cap) for k, dt in self.FIELDS}
         if self.n:
             obs[:self.n].copy_(self.obs[:self.n])
             for k, _ in self.FIELDS:
@@ -67,8 +74,9 @@ class DeviceRollout(object):
         self.capacity = cap
 
     def as_struct(self):
-        return capi.PpoRollout(self.obs.data_ptr(), self.action.data_ptr(), self.old_logp.data_ptr(),
-                               self.adv.data_ptr(), self.old_v.data_ptr(), self.target_v.data_ptr())
+        cls = capi.PpoRollout if self.action_dim is None else capi.PpoGaussRollout
+        return cls(self.obs.data_ptr(), self.action.data_ptr(), self.old_logp.data_ptr(),
+                   self.adv.data_ptr(), self.old_v.data_ptr(), self.target_v.data_ptr())
 
 
 @Registers.model
@@ -93,10 +101,11 @@ class PPO(XTModel):
         self.vf_clip = model_config.get("VF_CLIP", VF_CLIP)
         self.use_graph = bool(model_config.get("use_cuda_graph", True))
         self._init_seed = model_config.get("init_seed")
-        if self.action_type != "Categorical":
-            # DiagGaussian (tf_dist.py:49-86) is not on the Atari/CartPole path BASELINE.json names
+        if self.action_type not in ("Categorical", "DiagGaussian"):
             raise NotImplementedError(
                 "action type: {} not match any implemented distributions.".format(self.action_type))
+        # DiagGaussian (tf_dist.py:49-86, ppo.py:73-78): mean = pi_latent, log_std = the trainable pi_logstd (1, A)
+        self.gaussian = self.action_type == "DiagGaussian"
         super().__init__(model_info)
 
     # -- graph construction ------------------------------------------------------------------
@@ -113,7 +122,7 @@ class PPO(XTModel):
         self.opt = Adam(self.net, self._lr, eps=1e-8, clip_mode=capi.CLIP_GLOBAL_NORM, clip=self._max_grad_norm)
         self.hyper = capi.PpoHyper(self.clip_ratio, self.ent_coef, self.vf_clip, self.critic_loss_coef)
         obs_dt = torch.uint8 if self.input_dtype == "uint8" else torch.float32
-        self.rollout = DeviceRollout(self.state_dim, obs_dt, self.device)
+        self.rollout = DeviceRollout(self.state_dim, obs_dt, self.device, self.action_dim if self.gaussian else None)
         self._obs_dt = obs_dt
         self._perm_dev = None
         self._perm_host = None
@@ -124,6 +133,7 @@ class PPO(XTModel):
         self._sample_offset = 0
         self.pi_t = self.net.tid["pi_latent"]
         self.v_t = self.net.tid["output_value"]
+        self.ls_t = self.net.tid["pi_logstd"] if self.gaussian else None
         return self.net
 
     # -- inference ---------------------------------------------------------------------------
@@ -131,15 +141,17 @@ class PPO(XTModel):
         b = self._pred_bufs.get(batch)
         if b is None:
             dev = self.device
-            b = dict(obs=torch.empty((batch,) + tuple(self.state_dim), dtype=self._obs_dt, device=dev),
-                     action=torch.empty(batch, dtype=torch.int32, device=dev),
+            action = torch.empty((batch, self.action_dim), dtype=torch.float32, device=dev) if self.gaussian else \
+                torch.empty(batch, dtype=torch.int32, device=dev)
+            b = dict(obs=torch.empty((batch,) + tuple(self.state_dim), dtype=self._obs_dt, device=dev), action=action,
                      logp=torch.empty(batch, dtype=torch.float32, device=dev))
             self._pred_bufs[batch] = b
         return b
 
-    def predict_device(self, obs_dev, batch, uniforms=None, out_action=None, out_logp=None, idx=None):
+    def predict_device(self, obs_dev, batch, uniforms=None, out_action=None, out_logp=None, idx=None, normals=None):
         """Batched inference on device-resident observations (row b = obs_dev[idx[b]] when idx is
-        given); returns device views (action[B] i32, logp[B] f32, v[B,1] f32)."""
+        given); returns device views (action[B] i32, logp[B] f32, v[B,1] f32).  A DiagGaussian actor returns
+        action [B, A] f32; `normals` [B, A] (device) then replaces the Philox draws, as `uniforms` does for Categorical."""
         net = self.net
         done = 0
         bufs = self._pred_buffers(batch) if out_action is None else None
@@ -152,10 +164,17 @@ class PPO(XTModel):
                 net.forward(obs_dev[done:done + mb], mb)
             else:
                 net.forward(obs_dev, mb, idx=idx[done:done + mb])
-            u = None if uniforms is None else uniforms[done:done + mb]
-            check(net.lib.xtb_categorical_sample(_ptr(net.tensor("pi_latent")), mb, self.action_dim, _ptr(u),
-                                                 C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset),
-                                                 _ptr(action[done:done + mb]), _ptr(logp[done:done + mb]), stream_ptr()))
+            if self.gaussian:
+                n = None if normals is None else normals[done:done + mb]
+                check(net.lib.xtb_diag_gaussian_sample(_ptr(net.tensor("pi_latent")), _ptr(net.view("pi_logstd")), mb,
+                                                       self.action_dim, _ptr(n), C.c_uint64(self._sample_seed),
+                                                       C.c_uint64(self._sample_offset), _ptr(action[done:done + mb]),
+                                                       _ptr(logp[done:done + mb]), stream_ptr()))
+            else:
+                u = None if uniforms is None else uniforms[done:done + mb]
+                check(net.lib.xtb_categorical_sample(_ptr(net.tensor("pi_latent")), mb, self.action_dim, _ptr(u),
+                                                     C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset),
+                                                     _ptr(action[done:done + mb]), _ptr(logp[done:done + mb]), stream_ptr()))
             self._sample_offset += 1
             if vout is not None:
                 vout[done:done + mb].copy_(net.tensor("output_value")[:mb])
@@ -165,10 +184,16 @@ class PPO(XTModel):
 
     def rollout_infer_device(self, obs_dev, step_idx, n_env, n_step, action, logp, value):
         """T batched policy evaluations on device-resident observations (one CUDA graph): time-major
-        outputs action/logp/value [n_step, n_env]."""
+        outputs action/logp/value [n_step, n_env] (a DiagGaussian actor: action f32 [n_step, n_env, A])."""
         if getattr(self, "_offset_dev", None) is None:
             self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.net.ensure_batch(n_env)
+        if self.gaussian:
+            check(self.net.lib.xtb_ppo_gauss_rollout_infer(
+                self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step), self.pi_t, self.v_t, self.ls_t,
+                C.c_uint64(self._sample_seed), _ptr(self._offset_dev), _ptr(action), _ptr(logp), _ptr(value),
+                1 if self.use_graph else 0, stream_ptr()))
+            return
         check(self.net.lib.xtb_ppo_rollout_infer(self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step),
                                                  self.pi_t, self.v_t, C.c_uint64(self._sample_seed), _ptr(self._offset_dev),
                                                  _ptr(action), _ptr(logp), _ptr(value), 1 if self.use_graph else 0, stream_ptr()))
@@ -180,26 +205,30 @@ class PPO(XTModel):
         if io is None:
             dev = self.device
             shape = (batch,) + tuple(self.state_dim)
-            out_dev = torch.empty(3, batch, dtype=torch.float32, device=dev)
+            # DiagGaussian: [action batch*A | logp batch | value batch] floats, as one [A + 2, batch] block
+            rows = self.action_dim + 2 if self.gaussian else 3
+            out_dev = torch.empty(rows, batch, dtype=torch.float32, device=dev)
             io = dict(obs=torch.empty(shape, dtype=self._obs_dt, device=dev), out_dev=out_dev,
-                      act=out_dev[0].view(torch.int32), logp=out_dev[1], val=out_dev[2],
-                      pin_out=torch.empty(3, batch, dtype=torch.float32).pin_memory())
+                      act=out_dev[0].view(torch.int32), logp=out_dev[rows - 2], val=out_dev[rows - 1],
+                      pin_out=torch.empty(rows, batch, dtype=torch.float32).pin_memory())
             io["obs_ptr"], io["out_dev_ptr"], io["pin_out_ptr"] = _ptr(io["obs"]), _ptr(out_dev), _ptr(io["pin_out"])
             io["pin_out_np"] = io["pin_out"].numpy()
             self._pred_bufs[("io", batch)] = io
         return io
 
-    def predict(self, state, uniforms=None):
-        """xt/model/ppo/ppo.py:104-109: (action [B] int32, logp [B,1], v [B,1])."""
+    def predict(self, state, uniforms=None, normals=None):
+        """xt/model/ppo/ppo.py:104-109: (action [B] int32, logp [B,1], v [B,1]); a DiagGaussian actor returns action
+        [B, A] float32 (`normals` [B, A] then replaces the Philox draws)."""
         state = np.ascontiguousarray(state, dtype=np.uint8 if self.input_dtype == "uint8" else np.float32)
         batch = state.shape[0]
-        if uniforms is not None or batch > self.net.max_batch:
+        noise = normals if self.gaussian else uniforms
+        if noise is not None or batch > self.net.max_batch:
             bufs = self._pred_buffers(batch)
             bufs["obs"].copy_(torch.from_numpy(state), non_blocking=True)
-            u = None
-            if uniforms is not None:
-                u = torch.from_numpy(np.ascontiguousarray(uniforms, np.float32)).to(self.device)
-            action, logp, v = self.predict_device(bufs["obs"], batch, u)
+            if noise is not None:
+                noise = torch.from_numpy(np.ascontiguousarray(noise, np.float32)).to(self.device)
+            action, logp, v = self.predict_device(bufs["obs"], batch, None if self.gaussian else noise,
+                                                  normals=noise if self.gaussian else None)
             return (action.cpu().numpy(), logp.cpu().numpy().reshape(batch, 1), v.cpu().numpy().reshape(batch, 1))
         io = self._predict_io(batch)
         if getattr(self, "_offset_dev", None) is None:
@@ -207,15 +236,24 @@ class PPO(XTModel):
         self.net.ensure_batch(batch)
         ring = self._obs_ring
         # staged H2D -> graphed forward + sampling -> packed D2H -> stream sync, in one native call
-        check(self.net.lib.xtb_ppo_predict_host(self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch,
-                                                self.pi_t, self.v_t, C.c_uint64(self._sample_seed), _ptr(self._offset_dev),
-                                                io["out_dev_ptr"], io["pin_out_ptr"], 1 if self.use_graph else 0, stream_ptr()))
+        if self.gaussian:
+            check(self.net.lib.xtb_ppo_gauss_predict_host(
+                self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch, self.pi_t, self.v_t, self.ls_t,
+                C.c_uint64(self._sample_seed), _ptr(self._offset_dev), io["out_dev_ptr"], io["pin_out_ptr"],
+                1 if self.use_graph else 0, stream_ptr()))
+        else:
+            check(self.net.lib.xtb_ppo_predict_host(self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch,
+                                                    self.pi_t, self.v_t, C.c_uint64(self._sample_seed), _ptr(self._offset_dev),
+                                                    io["out_dev_ptr"], io["pin_out_ptr"], 1 if self.use_graph else 0, stream_ptr()))
         if ring is not None and batch == ring["E"]:
             # learner-side batched inference: the frames just uploaded ARE the rollout's cur_state -- keep them on the
             # device (time-major ring) so prepare_data can take them from here instead of a second H2D copy
             ring["obs"][ring["t"] % ring["T"]].copy_(io["obs"], non_blocking=True)
             ring["t"] += 1
         out = io["pin_out_np"]
+        if self.gaussian:
+            A = self.action_dim
+            return (out[:A].reshape(batch, A).copy(), out[A].reshape(batch, 1).copy(), out[A + 1].reshape(batch, 1).copy())
         return (out[0].view(np.int32).copy(), out[1].reshape(batch, 1).copy(), out[2].reshape(batch, 1).copy())
 
     def keep_predict_obs(self, env_num, steps):
@@ -244,10 +282,16 @@ class PPO(XTModel):
         self._perm_host[:perm.size].copy_(torch.from_numpy(perm))
         self._perm_dev[:perm.size].copy_(self._perm_host[:perm.size], non_blocking=True)
         ro = self.rollout.as_struct()
-        check(self.net.lib.xtb_ppo_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs,
-                                         int(self.num_sgd_iter), _ptr(self._perm_dev), C.byref(self.hyper),
-                                         self.pi_t, self.v_t, _ptr(self._loss_dev), 1 if self.use_graph else 0,
-                                         stream_ptr()))
+        if self.gaussian:
+            check(self.net.lib.xtb_ppo_gauss_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs,
+                                                   int(self.num_sgd_iter), _ptr(self._perm_dev), C.byref(self.hyper),
+                                                   self.pi_t, self.v_t, self.ls_t, _ptr(self._loss_dev),
+                                                   1 if self.use_graph else 0, stream_ptr()))
+        else:
+            check(self.net.lib.xtb_ppo_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs,
+                                             int(self.num_sgd_iter), _ptr(self._perm_dev), C.byref(self.hyper),
+                                             self.pi_t, self.v_t, _ptr(self._loss_dev), 1 if self.use_graph else 0,
+                                             stream_ptr()))
         losses = self._loss_dev[:steps].cpu().numpy()
         self.last_losses = losses
         return float(np.mean(losses))
@@ -259,14 +303,19 @@ class PPO(XTModel):
         ro.reserve(nbatch)
         np_obs = np.ascontiguousarray(state[0], dtype=np.uint8 if self.input_dtype == "uint8" else np.float32)
         ro.obs[:nbatch].copy_(torch.from_numpy(np_obs), non_blocking=True)
-        ro.action[:nbatch].copy_(torch.from_numpy(np.ascontiguousarray(label[0], np.int32).reshape(-1)))
+        if self.gaussian:
+            act = np.ascontiguousarray(label[0], np.float32).reshape(nbatch, self.action_dim)
+        else:
+            act = np.ascontiguousarray(label[0], np.int32).reshape(-1)
+        ro.action[:nbatch].copy_(torch.from_numpy(act))
         for key, arr in zip(("old_logp", "adv", "old_v", "target_v"), label[1:5]):
             getattr(ro, key)[:nbatch].copy_(torch.from_numpy(np.ascontiguousarray(arr, np.float32).reshape(-1)))
         ro.n = nbatch
         return nbatch
 
     def train(self, state, label):
-        """xt/model/ppo/ppo.py:111-132.  state=[obs], label=[action, old_logp, adv, old_v, target_v]."""
+        """xt/model/ppo/ppo.py:111-132.  state=[obs], label=[action, old_logp, adv, old_v, target_v]; action is float
+        [N, A] for a DiagGaussian actor."""
         nbatch = self.upload_rollout(state, label)
         return self.train_device(nbatch)
 
@@ -287,7 +336,8 @@ class PpoCnn(PPO):
     def build_arch(self):
         if self.input_dtype not in ("uint8", "float32"):
             raise ValueError("dtype: {} not supported automatically, please implement it yourself".format(self.input_dtype))
-        arch = archs.ppo_cnn(self.state_dim, self.action_dim, self.hidden_sizes, self.activation, self.vf_share_layers)
+        arch = archs.ppo_cnn(self.state_dim, self.action_dim, self.hidden_sizes, self.activation, self.vf_share_layers,
+                             diag_gaussian=self.gaussian)
         if self.input_dtype == "float32":
             arch["input_dtype"], arch["scale"] = "float32", 1.0
         return arch
@@ -309,4 +359,5 @@ class PpoMlp(PPO):
     def build_arch(self):
         if self.input_dtype != "float32":
             raise ValueError("dtype: {} not supported automatically, please implement it yourself".format(self.input_dtype))
-        return archs.ppo_mlp(self.state_dim, self.action_dim, self.hidden_sizes, self.activation, self.vf_share_layers)
+        return archs.ppo_mlp(self.state_dim, self.action_dim, self.hidden_sizes, self.activation, self.vf_share_layers,
+                             diag_gaussian=self.gaussian)
