@@ -35,7 +35,26 @@ enum xtb_status {
 };
 
 enum xtb_layer_kind { XTB_CONV = 0, XTB_DENSE = 1, XTB_DUELING = 2, XTB_LOGSTD = 3 };
-enum xtb_act { XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2 };
+/* Hidden-layer activations: the keys of ACTIVATION_MAP (xt/model/model_utils.py:8-19) with TF 1.15's semantics, plus
+ * NONE (linear).  xtb_net_create rejects any other value with XTB_ERR_ARG.
+ *   SIGMOID    1 / (1 + e^-x)                                   tf.math.sigmoid
+ *   SOFTSIGN   x / (1 + |x|)                                    tf.nn.softsign
+ *   SOFTPLUS   log(1 + e^x) = max(x, 0) + log1p(e^-|x|)         tf.nn.softplus
+ *   LEAKY_RELU x > 0 ? x : 0.2 x                                tf.nn.leaky_relu (default alpha 0.2)
+ *   ELU        x > 0 ? x : e^x - 1                              tf.nn.elu (alpha 1)
+ *   SELU       1.0507009873554805 * (x > 0 ? x : 1.6732632423543772 (e^x - 1))   tf.nn.selu
+ *   SWISH      x * sigmoid(x)                                   tf.nn.swish
+ *   GELU       0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))  the reference's tanh form, xt/model/tf_utils.py:157-166
+ * The GEMM epilogues apply RELU, TANH and NONE.  A layer with one of the others runs its GEMM linear into fp32 and one
+ * elementwise launch applies the activation; the backward sums the gradients of its consumers wrt its output and one
+ * elementwise launch multiplies by the derivative.  That derivative is taken from the output y, except for SOFTSIGN,
+ * SWISH and GELU, which y does not determine well (or at all): their layers keep the pre-activation in a workspace
+ * buffer of their own, written by every forward (xtb_net_workspace_bytes includes it).  A dueling layer reads only
+ * RELU / TANH / NONE tensors. */
+enum xtb_act {
+  XTB_ACT_NONE = 0, XTB_ACT_RELU = 1, XTB_ACT_TANH = 2, XTB_ACT_SIGMOID = 3, XTB_ACT_SOFTSIGN = 4, XTB_ACT_SOFTPLUS = 5,
+  XTB_ACT_LEAKY_RELU = 6, XTB_ACT_ELU = 7, XTB_ACT_SELU = 8, XTB_ACT_SWISH = 9, XTB_ACT_GELU = 10
+};
 
 #define XTB_MAX_LAYERS 16
 

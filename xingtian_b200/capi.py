@@ -11,7 +11,9 @@ LIB_PATH = os.environ.get("XTB_LIB_PATH") or os.path.join(HERE, "lib", "libxtb20
 
 XTB_MAX_LAYERS = 16
 CONV, DENSE, DUELING, LOGSTD = 0, 1, 2, 3
-ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2}
+# enum xtb_act: the keys of the reference's ACTIVATION_MAP plus linear / None
+ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "sigmoid": 3, "softsign": 4, "softplus": 5, "leaky_relu": 6, "elu": 7,
+       "selu": 8, "swish": 9, "gelu": 10}
 CLIP_NONE, CLIP_GLOBAL_NORM, CLIP_PER_TENSOR = 0, 1, 2
 
 

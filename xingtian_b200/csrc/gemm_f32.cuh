@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/xtb200.h"
 #include "launch.cuh"
 
 namespace xtb {
@@ -60,6 +61,93 @@ __device__ inline float act_grad_from_out(int act, float y) {
   if (act == 1) return y > 0.f ? 1.f : 0.f;
   if (act == 2) return 1.f - y * y;
   return 1.f;
+}
+
+// ------------------------------------------------------------------------------------------
+// The activations past tanh (enum xtb_act, include/xtb200.h).  The GEMM epilogues above and in bp_gemm.cuh apply only
+// relu / tanh / linear: code for the others in their unrolled bodies slowed every network (instruction fetch, register
+// pressure).  A layer with one of these runs its GEMM linear into fp32 and act_fwd_kernel applies the activation; the
+// data gradients into its tensor are taken wrt its output y, and act_bwd_kernel turns their sum into the gradient wrt
+// the pre-activation before the layer's own backward.
+// ------------------------------------------------------------------------------------------
+constexpr float kLeakyAlpha = 0.2f;
+constexpr float kSeluScale = 1.0507009873554805f, kSeluAlpha = 1.6732632423543772f;
+constexpr float kGeluC = 0.7978845608028654f, kGeluA = 0.044715f;   // sqrt(2/pi)
+
+__host__ __device__ inline bool act_is_ext(int act) { return act > XTB_ACT_TANH; }
+// the activations whose derivative is taken from the retained pre-activation z: y does not determine it (swish, gelu)
+// or determines it badly near saturation (softsign)
+__host__ __device__ inline bool act_keeps_z(int act) {
+  return act == XTB_ACT_SOFTSIGN || act == XTB_ACT_SWISH || act == XTB_ACT_GELU;
+}
+
+__device__ inline float act_apply_ext(int act, float x) {
+  switch (act) {
+    case XTB_ACT_SIGMOID: return 1.f / (1.f + expf(-x));
+    case XTB_ACT_SOFTSIGN: return x / (1.f + fabsf(x));
+    case XTB_ACT_SOFTPLUS: return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x)));
+    case XTB_ACT_LEAKY_RELU: return x > 0.f ? x : kLeakyAlpha * x;
+    case XTB_ACT_ELU: return x > 0.f ? x : expm1f(x);
+    case XTB_ACT_SELU: return kSeluScale * (x > 0.f ? x : kSeluAlpha * expm1f(x));
+    case XTB_ACT_SWISH: return x / (1.f + expf(-x));
+    case XTB_ACT_GELU: return 0.5f * x * (1.f + tanhf(kGeluC * (x + kGeluA * x * x * x)));
+    default: return x;
+  }
+}
+// derivative from u = the pre-activation z where act_keeps_z(act), the output y otherwise
+__device__ inline float act_grad_ext(int act, float u) {
+  switch (act) {
+    case XTB_ACT_SIGMOID: return u * (1.f - u);
+    case XTB_ACT_SOFTSIGN: { const float d = 1.f + fabsf(u); return 1.f / (d * d); }
+    case XTB_ACT_SOFTPLUS: return -expm1f(-u);
+    case XTB_ACT_LEAKY_RELU: return u > 0.f ? 1.f : kLeakyAlpha;
+    case XTB_ACT_ELU: return u > 0.f ? 1.f : u + 1.f;
+    case XTB_ACT_SELU: return u > 0.f ? kSeluScale : u + kSeluScale * kSeluAlpha;
+    case XTB_ACT_SWISH: { const float s = 1.f / (1.f + expf(-u)); return s * (1.f + u * (1.f - s)); }
+    case XTB_ACT_GELU: {
+      const float t = tanhf(kGeluC * (u + kGeluA * u * u * u));
+      return 0.5f * (1.f + t) + 0.5f * u * (1.f - t * t) * kGeluC * (1.f + 3.f * kGeluA * u * u);
+    }
+    default: return 1.f;
+  }
+}
+
+// y[i] = act(pre[i]) over n floats (pre may be y itself)
+__global__ void act_fwd_kernel(const float* pre, long long n, int act, float* y) {
+  pdl_wait(); pdl_trigger();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    y[i] = act_apply_ext(act, pre[i]);
+}
+// g *= act'(u) over rows x N (u: z or y, act_grad_ext): the gradient wrt the output becomes the gradient wrt the
+// pre-activation.  Also the layer's bias gradient, without atomics: block b takes a fixed run of rows, its row lanes
+// add in a fixed order, and part[b][N] is left for the ordered reduction (bp::grad_reduce_kernel).
+constexpr int ACT_BWD_BLOCKS = 132, ACT_BWD_THREADS = 256;
+__global__ void __launch_bounds__(ACT_BWD_THREADS) act_bwd_kernel(float* __restrict__ g, const float* __restrict__ u, int rows,
+                                                                  int N, int act, float* __restrict__ part) {
+  pdl_wait(); pdl_trigger();
+  __shared__ float red[ACT_BWD_THREADS];
+  const int rpb = (rows + gridDim.x - 1) / gridDim.x, r0 = blockIdx.x * rpb, r1 = min(rows, r0 + rpb);
+  const int W = min(N, ACT_BWD_THREADS), R = ACT_BWD_THREADS / W;      // columns per pass, row lanes
+  const int rr = threadIdx.x / W;
+  for (int c0 = 0; c0 < N; c0 += W) {
+    const int c = c0 + threadIdx.x % W;
+    float s = 0.f;
+    if (rr < R && c < N)
+      for (int r = r0 + rr; r < r1; r += R) {
+        const long long e = (long long)r * N + c;
+        const float v = g[e] * act_grad_ext(act, u[e]);
+        g[e] = v;
+        s += v;
+      }
+    red[threadIdx.x] = s;
+    __syncthreads();
+    if (rr == 0 && c < N) {
+      float t = red[threadIdx.x];
+      for (int k = 1; k < R; k++) t += red[k * W + threadIdx.x];
+      part[(long long)blockIdx.x * N + c] = t;
+    }
+    __syncthreads();
+  }
 }
 
 // ------------------------------------------------------------------------------------------

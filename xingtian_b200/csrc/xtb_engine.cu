@@ -159,6 +159,7 @@ struct LayerPlan {
   int n_fwd = 0, n_dg = 0;  // accumulator columns: forward (Cout / dense N tile), data gradient (Cin / dense K tile)
   int run_chunks = 0, mts = 0, R = 0;   // conv weight gradient: chunks per filter row, M tiles per row, accumulators
   size_t part_off = 0, dbpart_off = 0;  // workspace offsets of the partial-sum areas
+  size_t act_part_off = 0;              // act_is_ext layers: act_bwd_kernel's bias partial sums [ACT_BWD_BLOCKS][N]
   // host-built stage walks of the tensor-core kernels (conv layers) and their workspace offsets
   std::vector<bp::StageEnt> fwd_st, dg_st; std::vector<bp::UnitEnt> fwd_un, dg_un; std::vector<bp::WgEnt> wg_tab;
   size_t fwd_st_off = 0, fwd_un_off = 0, dg_st_off = 0, dg_un_off = 0, wg_off = 0;
@@ -240,6 +241,7 @@ struct xtb_net {
   size_t ws_bytes = 0;
   std::vector<size_t> out_off, gout_off;  // byte offsets in workspace per tensor (fp32 row-major)
   std::vector<size_t> obp_off, gbp_off;   // byte offsets of the batch-planar hi planes (lo plane follows at plane_elems)
+  std::vector<size_t> z_off;              // byte offset of the retained pre-activation (fp32 row-major), 0 = none
   std::vector<long long> plane_elems;     // elements per plane of tensor t = tsize * pitch
   size_t obs_bp_off = 0; int obs_feats = 0;            // decoded-frame plane (space-to-depth canvas)
   int H4 = 0, W4 = 0;
@@ -274,6 +276,11 @@ static inline bp::BpT out_bp(const xtb_net* n, int t) { return bp::BpT{(bp::bf16
 static inline bp::BpT gout_bp(const xtb_net* n, int t) { return bp::BpT{(bp::bf16*)(n->ws + n->gbp_off[t]), n->plane_elems[t], n->pitch}; }
 static inline bp::BpT obs_bp(const xtb_net* n) { return bp::BpT{(bp::bf16*)(n->ws + n->obs_bp_off), 0, n->pitch}; }
 static inline bp::BpT no_bp() { return bp::BpT{nullptr, 0, 0}; }
+// retained pre-activation of tensor t, [max_batch][tsize] fp32; NULL unless its layer's activation keeps it (act_keeps_z)
+static inline float* z_buf(const xtb_net* n, int t) { return n->z_off[t] ? (float*)(n->ws + n->z_off[t]) : nullptr; }
+// where the GEMM of a layer with an activation past tanh (act_is_ext) writes its pre-activation: the retained buffer, or
+// the fp32 output that act_fwd_kernel then overwrites in place
+static inline float* pre_buf(const xtb_net* n, int t) { float* z = z_buf(n, t); return z ? z : (float*)(n->ws + n->out_off[t]); }
 static inline const bp::bf16* blob_hi(const xtb_net* n, const LayerPlan& lp) { return (const bp::bf16*)(n->ws + n->blob_off) + lp.blob_off; }
 static inline bool use_tc(const LayerPlan& lp) { return g_tc_mode && lp.tc; }
 
@@ -339,6 +346,7 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     lp.d = desc->layers[i];
     const auto& d = lp.d;
     if (d.src < 0 || d.src > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: bad src %d", i, d.src); }
+    if (d.act < XTB_ACT_NONE || d.act > XTB_ACT_GELU) { delete net; return fail(XTB_ERR_ARG, "layer %d: unknown activation %d", i, d.act); }
     if (d.kind == XTB_LOGSTD) {
       // parameter-only: A floats (pi_logstd), no input, no output tensor
       if (d.src != 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a logstd layer reads no tensor (src must be 0)", i); }
@@ -364,6 +372,8 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
       if (d.k == d.src) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling inputs must be two different tensors", i); }
       if (net->tsize[d.k] != 1) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling input %d is %d wide, not 1", i, d.k, net->tsize[d.k]); }
       if (d.act != XTB_ACT_NONE) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer has no activation", i); }
+      if (act_is_ext(tact[d.src]) || act_is_ext(tact[d.k]))
+        { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer reads relu / tanh / linear tensors only", i); }
       lp.in_size = lp.out_size = net->tsize[d.src];
       lp.src_act = tact[d.src]; lp.adv_act = tact[d.k];
       shp[i + 1] = {1, 1, lp.out_size};
@@ -491,7 +501,7 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   size_t w = 0;
   const int nt = desc->n_layers + 1;
   net->out_off.assign(nt, 0); net->gout_off.assign(nt, 0);
-  net->obp_off.assign(nt, 0); net->gbp_off.assign(nt, 0);
+  net->obp_off.assign(nt, 0); net->gbp_off.assign(nt, 0); net->z_off.assign(nt, 0);
   net->plane_elems.assign(nt, 0);
   for (int t = 1; t < nt; t++) {
     size_t bytes = align_up((size_t)max_batch * net->tsize[t] * sizeof(float), 256);
@@ -504,6 +514,8 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
       net->obp_off[t] = w; w += pbytes;
       net->gbp_off[t] = w; w += pbytes;
     }
+    const LayerPlan& lt = net->L[t - 1];
+    if ((lt.d.kind == XTB_CONV || lt.d.kind == XTB_DENSE) && act_keeps_z(lt.d.act)) { net->z_off[t] = w; w += bytes; }
   }
   net->obs_bp_off = w; w += align_up((size_t)net->obs_feats * net->pitch * sizeof(uint16_t) + 256, 256);
   long long be = 0;
@@ -537,6 +549,10 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     }
     w += align_up(need + 256, 256);
   }
+  for (auto& lp : net->L)
+    if ((lp.d.kind == XTB_CONV || lp.d.kind == XTB_DENSE) && act_is_ext(lp.d.act)) {
+      lp.act_part_off = w; w += align_up((size_t)ACT_BWD_BLOCKS * lp.N * sizeof(float), 256);
+    }
   net->zeros_off = w; w += 4096;
   // per-block parameter-gradient slabs of the fused PPO heads kernel (K <= 512 hidden units, A <= 8 actions)
   net->heads_part_off = w; w += align_up((size_t)kSMs * (512 * 8 + 3 * 512 + 16) * sizeof(float), 256);
@@ -756,12 +772,13 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   a.a_split = lp.d.src != 0;
   a.w_hi = blob_hi(net, lp); a.w_lo = a.w_hi + net->blob_elems; a.w_pitch = lp.K;
   a.B = B; a.n_btiles = (B + 127) / 128; a.N = lp.n_fwd;
-  a.out = want_bp ? out_bp(net, t) : no_bp();
-  a.out_f32 = want_f32 ? (float*)(net->ws + net->out_off[t]) : nullptr;
+  const bool ext = act_is_ext(lp.d.act);      // linear into fp32; act_fwd_kernel follows (op_forward)
+  a.out = want_bp && !ext ? out_bp(net, t) : no_bp();
+  a.out_f32 = ext ? pre_buf(net, t) : (want_f32 ? (float*)(net->ws + net->out_off[t]) : nullptr);
   a.ld_f32 = net->tsize[t];
   a.bias = net->params + lp.b_off;
   a.alpha = lp.d.src == 0 ? net->desc.scale : 1.f;
-  a.act = lp.d.act;
+  a.act = ext ? 0 : lp.d.act;
   *launches = 1;
   if (lp.d.kind == XTB_CONV) {
     a.mode = 0;
@@ -783,10 +800,14 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   if (e != cudaSuccess) return e;
   long long pieces = (long long)(lp.N / 8) * b_pad * bp::FIN_ZL;
   XLAUNCH(bp::bp_splitk_finish_kernel, (unsigned)((pieces + 127) / 128), 128, 0, st, (const float*)a.part, nz, a.part_z, B, lp.N,
-          a.bias, lp.d.act, a.out_f32, a.out);
+          a.bias, a.act, a.out_f32, a.out);
   *launches = 2;
   return cudaPeekAtLastError();
 }
+
+// the activation whose derivative a data-gradient epilogue applies: none for the activations past tanh, whose tensors
+// collect the gradient wrt their output until act_backward
+static inline int dgrad_act(const LayerPlan& lp) { return act_is_ext(lp.src_act) ? 0 : lp.src_act; }
 
 // data gradient of tensor-core layer i into the planes of its source tensor
 static cudaError_t tc_dgrad(xtb_net* net, int i, int B, int accumulate, float* db_part, cudaStream_t st) {
@@ -797,7 +818,7 @@ static cudaError_t tc_dgrad(xtb_net* net, int i, int B, int accumulate, float* d
   a.a = gout_bp(net, t); a.a_split = 1;
   a.w_hi = blob_hi(net, lp); a.w_lo = a.w_hi + net->blob_elems; a.w_pitch = lp.K;
   a.B = B; a.n_btiles = (B + 127) / 128; a.N = lp.n_dg;
-  a.out = gout_bp(net, s); a.src = out_bp(net, s); a.src_act = lp.src_act; a.accumulate = accumulate; a.db_part = db_part;
+  a.out = gout_bp(net, s); a.src = out_bp(net, s); a.src_act = dgrad_act(lp); a.accumulate = accumulate; a.db_part = db_part;
   if (lp.d.kind == XTB_CONV) {
     a.mode = 1;
     a.stages = (const bp::StageEnt*)(net->ws + lp.dg_st_off); a.units = (const bp::UnitEnt*)(net->ws + lp.dg_un_off);
@@ -985,7 +1006,7 @@ static void conv_fwd(const LayerPlan& lp, const T* x, const int32_t* idx, const 
                      float alpha, float* out, int B, cudaStream_t st) {
   int M = B * lp.g.P;
   BRowMajor bl{w, lp.N};
-  EpiBiasAct ep{out, b, alpha, lp.d.act, lp.N, nullptr, 0};
+  EpiBiasAct ep{out, b, alpha, act_is_ext(lp.d.act) ? 0 : lp.d.act, lp.N, nullptr, 0};
   if (lp.pad) { AIm2col<T, true> al{x, idx, lp.g, lp.koff, lp.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
   else { AIm2col<T, false> al{x, idx, lp.g, lp.koff, lp.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
 }
@@ -994,7 +1015,7 @@ static void dense_fwd(const LayerPlan& lp, const T* x, const int32_t* idx, const
                       float alpha, float* out, int B, cudaStream_t st) {
   ADense<T> al{x, idx, lp.K};
   BRowMajor bl{w, lp.N};
-  EpiBiasAct ep{out, b, alpha, lp.d.act, lp.N, nullptr, 0};
+  EpiBiasAct ep{out, b, alpha, act_is_ext(lp.d.act) ? 0 : lp.d.act, lp.N, nullptr, 0};
   launch_gemm(al, bl, ep, B, lp.N, lp.K, false, st);
 }
 template <typename T>
@@ -1039,6 +1060,35 @@ __global__ void colsum_kernel(const float* __restrict__ dy, int M, int N, float*
 // ------------------------------------------------------------------------------------------
 // per-layer operations (tensor-core kernel when the shape is covered, fp32 kernel otherwise)
 // ------------------------------------------------------------------------------------------
+// the activation past tanh of tensor t's layer, after its GEMM wrote the pre-activation to pre_buf: fp32 output
+static int act_forward(xtb_net* net, int t, int B, cudaStream_t st) {
+  const long long n = (long long)B * net->tsize[t];
+  const unsigned blocks = (unsigned)std::min<long long>((n + 255) / 256, 8LL * kSMs);
+  XLAUNCH(act_fwd_kernel, blocks, 256, 0, st, (const float*)pre_buf(net, t), n, net->L[t - 1].d.act, (float*)(net->ws + net->out_off[t]));
+  LAUNCH_CHECK();
+  net->f32_ok[t] = 1; net->bp_ok[t] = 0;
+  return XTB_OK;
+}
+// ... and in the backward pass: the gradient wrt its output, summed over its consumers, becomes the gradient wrt its
+// pre-activation (act' from the retained pre-activation, or from the output); the layer's bias gradient is queued for
+// the ordered reduction
+static int act_backward(xtb_net* net, int t, int B, cudaStream_t st) {
+  int rc = ensure_f32(net, t, B, true, st);
+  if (rc) return rc;
+  const LayerPlan& lp = net->L[t - 1];
+  const float* u = z_buf(net, t) ? z_buf(net, t) : (const float*)(net->ws + net->out_off[t]);
+  float* part = (float*)(net->ws + lp.act_part_off);
+  XLAUNCH(act_bwd_kernel, ACT_BWD_BLOCKS, ACT_BWD_THREADS, 0, st, (float*)(net->ws + net->gout_off[t]), u,
+          (int)((long long)B * net->tsize[t] / lp.N), lp.N, lp.d.act, part);
+  LAUNCH_CHECK();
+  bp::RedSeg r;
+  memset(&r, 0, sizeof r);
+  r.part = part; r.n_slabs = ACT_BWD_BLOCKS; r.slab = lp.N; r.count = lp.N; r.kind = 1; r.dst_off = lp.b_off; r.alpha = 1.f;
+  net->pending.push_back(r);
+  net->gf32_ok[t] = 1; net->gbp_ok[t] = 0;
+  return XTB_OK;
+}
+
 // uint8 frame decode (+ minibatch gather) into the space-to-depth observation canvas
 static int op_decode(xtb_net* net, const void* obs, const int32_t* idx, int B, cudaStream_t st) {
   if (net->obs_bp_ok) return XTB_OK;
@@ -1060,6 +1110,8 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
   const LayerPlan& lp = net->L[i];
   const int t = i + 1;
   float* out = (float*)(net->ws + net->out_off[t]);
+  const bool ext = act_is_ext(lp.d.act);
+  float* pre = ext ? pre_buf(net, t) : out;      // the fp32 kernels write the activation, or the pre-activation (ext)
   const float* w = P + lp.w_off;
   const float* b = P + lp.b_off;
   if (lp.d.kind == XTB_LOGSTD) return XTB_OK;   // parameter-only: no output tensor
@@ -1080,26 +1132,28 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
     cudaError_t te = tc_forward(net, i, B, want_f32, true, st, &nl);
     if (te != cudaSuccess) return fail(XTB_ERR_CUDA, "tensor-core forward launch (layer %d): %s", i, cudaGetErrorString(te));
     g_launches.fetch_add(nl, std::memory_order_relaxed);
+    if (ext) return act_forward(net, t, B, st);
     net->bp_ok[t] = 1; net->f32_ok[t] = want_f32 ? 1 : 0;
     return XTB_OK;
   }
   if (lp.d.src == 0) {
     float alpha = net->desc.scale;
     if (net->desc.input_u8) {
-      if (lp.d.kind == XTB_CONV) conv_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, out, B, st);
-      else dense_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, out, B, st);
+      if (lp.d.kind == XTB_CONV) conv_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
+      else dense_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
     } else {
-      if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, out, B, st);
-      else dense_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, out, B, st);
+      if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, pre, B, st);
+      else dense_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, pre, B, st);
     }
   } else {
     int rc = ensure_f32(net, lp.d.src, B, false, st);
     if (rc) return rc;
     const float* x = (const float*)(net->ws + net->out_off[lp.d.src]);
-    if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, x, nullptr, w, b, 1.f, out, B, st);
-    else dense_fwd<float>(lp, x, nullptr, w, b, 1.f, out, B, st);
+    if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, x, nullptr, w, b, 1.f, pre, B, st);
+    else dense_fwd<float>(lp, x, nullptr, w, b, 1.f, pre, B, st);
   }
   LAUNCH_CHECK();
+  if (ext) return act_forward(net, t, B, st);
   net->f32_ok[t] = 1; net->bp_ok[t] = 0;
   return XTB_OK;
 }
@@ -1184,7 +1238,7 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
   if (use_tc(lp)) {
     int rc = ensure_bp(net, t, B, true, st);
     if (rc) return rc;
-    if (lp.src_act != 0) { rc = ensure_bp(net, s, B, false, st); if (rc) return rc; }
+    if (dgrad_act(lp) != 0) { rc = ensure_bp(net, s, B, false, st); if (rc) return rc; }
     if (acc) { rc = ensure_bp(net, s, B, true, st); if (rc) return rc; }
     float* dbp = fuse_db ? (float*)(net->ws + lp.dbpart_off) : nullptr;
     cudaError_t te = tc_dgrad(net, i, B, acc, dbp, st);
@@ -1213,12 +1267,12 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
   if (lp.d.kind == XTB_CONV) {
     ADgrad al{dy, lp.g, lp.dkyx, lp.dco, lp.sshift};
     BConvDgrad bl{w, lp.wk, lp.N};
-    EpiDgrad ep{gsrc, x, lp.src_act, lp.g.C, acc, nullptr, 0};
+    EpiDgrad ep{gsrc, x, dgrad_act(lp), lp.g.C, acc, nullptr, 0};
     launch_gemm(al, bl, ep, B * lp.g.H * lp.g.W, lp.g.C, lp.Kd, false, st);
   } else {
     ADense<float> al{dy, nullptr, lp.N};
     BTransposed bl{w, lp.N};
-    EpiDgrad ep{gsrc, x, lp.src_act, lp.K, acc, nullptr, 0};
+    EpiDgrad ep{gsrc, x, dgrad_act(lp), lp.K, acc, nullptr, 0};
     launch_gemm(al, bl, ep, B, lp.K, lp.N, false, st);
   }
   LAUNCH_CHECK();
@@ -1285,27 +1339,30 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
 
 static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                              const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
-                             unsigned bias_done_tensors = 0u, unsigned heads_bp_mask = 0u, xtb_comm* comm = nullptr);
+                             unsigned bias_done_tensors = 0u, unsigned heads_bp_mask = 0u, xtb_comm* comm = nullptr,
+                             unsigned heads_dy_mask = 0u);
 extern "C" int xtb_net_backward(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                                 const int32_t* head_tensors, int n_heads, void* stream) {
   return net_backward_impl(net, obs, gather_idx, batch, head_tensors, n_heads, stream, 0u, true);
 }
-// head_tensors: tensors whose gradient was filled by the caller: fp32 row-major, or (bit set in heads_bp_mask) planes
+// head_tensors: tensors whose gradient was filled by the caller: fp32 row-major, or (bit set in heads_bp_mask) planes;
+// wrt the pre-activation, or (bit set in heads_dy_mask, a layer with an activation past tanh) wrt the output
 static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                              const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
-                             unsigned bias_done_tensors, unsigned heads_bp_mask, xtb_comm* comm) {
+                             unsigned bias_done_tensors, unsigned heads_bp_mask, xtb_comm* comm, unsigned heads_dy_mask) {
   if (!net || !net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_net_backward: net not bound (grads required)");
   if (batch <= 0 || batch > net->max_batch) return fail(XTB_ERR_ARG, "batch out of range");
   cudaStream_t st = S(stream);
   const int nl = (int)net->L.size();
   std::vector<char> has_grad(nl + 1, 0), written(nl + 1, 0);
+  std::vector<char> dy(nl + 1, 0);          // the gradient is wrt the output of an act_is_ext layer: act_backward pending
   long long early_off = 0, early_cnt = 0;
   for (int t = 1; t <= nl; t++) net->gf32_ok[t] = net->gbp_ok[t] = 0;
   if (zero_grads) net->pending.clear();      // a fused loss kernel (zero_grads == false) has queued its own reductions
   for (int h = 0; h < n_heads; h++) {
     int t = head_tensors[h];
     if (t < 1 || t > nl || net->tsize[t] == 0) return fail(XTB_ERR_ARG, "bad head tensor %d", t);
-    has_grad[t] = 1; written[t] = 1;
+    has_grad[t] = 1; written[t] = 1; dy[t] = (heads_dy_mask >> t) & 1u;
     if ((heads_bp_mask >> t) & 1u) net->gbp_ok[t] = 1; else net->gf32_ok[t] = 1;
   }
   if (zero_grads) CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), st));
@@ -1316,6 +1373,7 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
   for (int s = 1; s <= nl; s++) {
     if (bias_done_tensors & (1u << s)) { fuse_bias[s] = 2; continue; }
     const LayerPlan& ps = net->L[s - 1];
+    if (act_is_ext(ps.d.act)) continue;       // the column sums would be of the gradient wrt the output
     int consumers = 0, cj = -1;
     for (int j = 0; j < nl; j++) if (reads(net->L[j], s) && !(skip_mask & (1u << j))) { consumers++; cj = j; }
     if (consumers != 1) continue;
@@ -1328,7 +1386,9 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
     const LayerPlan& lp = net->L[i];
     int t = i + 1;
     if (!has_grad[t]) continue;   // tensor does not influence the loss
-    int rc = op_wgrad(net, i, obs, gather_idx, batch, st, fuse_bias[t] != 0);
+    const bool act_bwd = dy[t] && act_is_ext(lp.d.act);      // act_backward also queues the bias gradient
+    if (act_bwd) { int rc = act_backward(net, t, batch, st); if (rc) return rc; }
+    int rc = op_wgrad(net, i, obs, gather_idx, batch, st, fuse_bias[t] != 0 || act_bwd);
     if (rc) return rc;
     // data parallel: a large dense weight gradient is final here (direct store) -- start summing it over ranks now, on
     // the communicator's side stream, while the rest of the backward pass runs
@@ -1346,7 +1406,7 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
       int s = lp.d.src;
       rc = op_dgrad(net, i, written[s] ? 1 : 0, batch, st, fuse_bias[s] == 1);
       if (rc) return rc;
-      written[s] = 1; has_grad[s] = 1;
+      written[s] = 1; has_grad[s] = 1; dy[s] = 1;
     }
   }
   int rc = flush_reductions(net, st);
@@ -1866,19 +1926,21 @@ static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int m
   a.h_pi = (const float*)(net->ws + net->out_off[lpi.d.src]); a.h_v = (const float*)(net->ws + net->out_off[lv.d.src]);
   a.g_pi = (float*)(net->ws + net->gout_off[lpi.d.src]); a.g_v = (float*)(net->ws + net->gout_off[lv.d.src]);
   // hidden-layer gradients go straight into batch-planar planes when the hidden layer runs on tensor cores
-  const bool bp_pi = use_tc(net->L[lpi.d.src - 1]) && net->plane_elems[lpi.d.src] > 0;
-  const bool bp_v = use_tc(net->L[lv.d.src - 1]) && net->plane_elems[lv.d.src] > 0;
+  // (a hidden layer with an activation past tanh gets the gradient wrt its output, in fp32, and act_backward follows)
+  const bool ext_pi = act_is_ext(lpi.src_act), ext_v = act_is_ext(lv.src_act);
+  const bool bp_pi = use_tc(net->L[lpi.d.src - 1]) && net->plane_elems[lpi.d.src] > 0 && !ext_pi;
+  const bool bp_v = use_tc(net->L[lv.d.src - 1]) && net->plane_elems[lv.d.src] > 0 && !ext_v;
   a.gp_hi = bp_pi ? gout_bp(net, lpi.d.src).hi : nullptr; a.gp_lo = net->plane_elems[lpi.d.src];
   a.gv_hi = bp_v ? gout_bp(net, lv.d.src).hi : nullptr; a.gv_lo = net->plane_elems[lv.d.src];
   a.pitch = net->pitch;
   a.w_pi = net->params + lpi.w_off; a.b_pi = net->params + lpi.b_off; a.w_v = net->params + lv.w_off; a.b_v = net->params + lv.b_off;
   // the hidden layers' bias gradients (column sums of g) when they are dense and only feed the heads
   auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], tsr) && !(skip & (1u << j))) return false; return true; };
-  bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src);
-  bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src);
+  bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src) && !ext_pi;
+  bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src) && !ext_v;
   unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
   a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
-  a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = lpi.src_act; a.act_v = lv.src_act; a.shared = lpi.d.src == lv.d.src ? 1 : 0;
+  a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = dgrad_act(lpi); a.act_v = dgrad_act(lv); a.shared = lpi.d.src == lv.d.src ? 1 : 0;
   int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
   const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2 + (LOSS::kLogStd ? adim : 0);
   a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
@@ -1905,7 +1967,8 @@ static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int m
   }
   int srcs[2] = {lpi.d.src, lv.d.src};
   unsigned hbp = (bp_pi ? (1u << lpi.d.src) : 0u) | (bp_v ? (1u << lv.d.src) : 0u);   // the fused kernel wrote planes there
-  return net_backward_impl(net, obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm);
+  unsigned hdy = (ext_pi ? (1u << lpi.d.src) : 0u) | (ext_v ? (1u << lv.d.src) : 0u);
+  return net_backward_impl(net, obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm, hdy);
 }
 
 static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
@@ -2158,7 +2221,7 @@ static bool dueling_fusable(const xtb_net* net, int q_tensor) {
   const LayerPlan& lv = net->L[lq.d.src - 1];
   const LayerPlan& la = net->L[lq.d.k - 1];
   return lv.d.kind == XTB_DENSE && la.d.kind == XTB_DENSE && lv.d.act == 0 && la.d.act == 0 && lv.d.src != 0 &&
-         lv.d.src == la.d.src && heads_fit(lv.K, lv.N);
+         lv.d.src == la.d.src && heads_fit(lv.K, lv.N) && !act_is_ext(lv.src_act);
 }
 
 // The online half of the dueling TD step in one heads_kernel launch: both streams' forward, the combine, TD target and

@@ -24,7 +24,7 @@ VF_CLIP = 5.0
 CNN_SHARE_LAYERS = True
 MLP_SHARE_LAYERS = False
 
-_SUPPORTED_ACT = ("relu", "tanh", "linear", None)
+_SUPPORTED_ACT = tuple(capi.ACT)
 
 
 def minibatch_order(nbatch, num_sgd_iter):
