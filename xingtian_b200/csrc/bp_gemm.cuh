@@ -82,6 +82,13 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// shared-memory load in the shared state space: a generic load could alias the global stores around it, which would
+// pin it behind them.  Volatile keeps it after the mbarrier wait that makes the data visible.
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 // one lane of a converged warp issues the bulk copies with warp-uniform operands
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -280,6 +287,13 @@ constexpr int RW_A_PLANE = 2048;                 // 128 rows x 16 B
 constexpr int RW_STAGE_A = 2 * 8 * RW_A_PLANE;   // hi + lo, 8 chunks (64 K elements)
 constexpr int RW_STAGE_B = 16384;
 constexpr int RW_MAX_STAGES = 4;
+constexpr int RW_EPI_BANKS = 2;                  // data-gradient epilogue operand buffers (one per accumulator bank)
+
+// Planes the data-gradient epilogue reads besides its accumulator: the source activation for act' (relu: hi; tanh: hi
+// and lo) and, when it accumulates, the output planes (hi and lo).  The producer warp prefetches them into shared memory.
+__host__ __device__ inline int dgrad_epi_planes(int src_act, int accumulate) {
+  return (src_act == 1 ? 1 : (src_act == 2 ? 2 : 0)) + (accumulate ? 2 : 0);
+}
 
 struct StageEnt {            // one K stage of a conv unit (8 bytes; the tables are copied to shared memory at kernel start)
   uint32_t a_chunk;          // first operand feature chunk of the stage
@@ -341,16 +355,22 @@ struct TileWalk {
   }
 };
 
-// N = accumulator columns per plane (16, 32, 48 or 64)
+// N = accumulator columns per plane (16, 32, 48 or 64).  epi_banks: data-gradient epilogue buffers (0 when the epilogue
+// reads nothing but its accumulator, else 1 or 2; see rows_smem)
 template <int KIND, int N>
 __global__ void __launch_bounds__(RW_THREADS, 1)
-bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes, int wres_bytes) {
+bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes, int wres_bytes, int epi_banks) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
-  // stage-walk tables live behind the stage ring: [stages : n_stage_ents x 8 B][units : n_units x 4 B]
-  uint2* stages_sm = reinterpret_cast<uint2*>(smem + wres_bytes + n_stages * stage_bytes);
+  constexpr int NCH = N >> 3;                            // feature chunks of an accumulator tile
+  // data-gradient epilogue operands behind the stage ring: per bank [plane][chunk][128 rows][16 B]
+  const int epi_planes = KIND == 2 ? dgrad_epi_planes(a.src_act, a.accumulate) : 0;
+  const int epi_bank_bytes = epi_planes * NCH * RW_A_PLANE;
+  uint8_t* epi_sm = smem + wres_bytes + n_stages * stage_bytes;
+  // stage-walk tables behind those: [stages : n_stage_ents x 8 B][units : n_units x 4 B]
+  uint2* stages_sm = reinterpret_cast<uint2*>(epi_sm + epi_banks * epi_bank_bytes);
   uint32_t* units_sm = reinterpret_cast<uint32_t*>(stages_sm + a.n_stage_ents);
-  __shared__ __align__(8) uint64_t bars[2 * RW_MAX_STAGES + 1];
+  __shared__ __align__(8) uint64_t bars[2 * RW_MAX_STAGES + 1 + 2 * RW_EPI_BANKS];
   __shared__ float red_sh[BP_CONSUMER_WARPS][64];
   __shared__ float bias_sh[64];
 
@@ -358,9 +378,11 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
   // not serialize the wgmma instructions behind them
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[RW_MAX_STAGES]), wbar = smem_u32(&bars[2 * RW_MAX_STAGES]);
+  const uint32_t efull0 = wbar + 8, eempty0 = efull0 + 8 * RW_EPI_BANKS;
   if (tid == 0) {
     for (int s = 0; s < RW_MAX_STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, BP_CONSUMER_WARPS); }
     mbar_init(wbar, 1);
+    for (int k = 0; k < RW_EPI_BANKS; k++) { mbar_init(efull0 + 8 * k, 1); mbar_init(eempty0 + 8 * k, BP_CONSUMER_WARPS); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -404,6 +426,14 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
     int u = (int)blockIdx.x / nbt, bt = (int)blockIdx.x - u * nbt;
     const int Bsz = a.B;
     TileWalk tw; tw.setup(a, stages_sm, units_sm);
+    // data-gradient epilogue operands: source planes (act'), then output planes (accumulate)
+    const int src_act = a.src_act, accumulate = a.accumulate;
+    const char* s_hi = reinterpret_cast<const char*>(a.src.hi);
+    const char* s_lo = s_hi + a.src.lo_off * 2;
+    const char* o_hi = reinterpret_cast<const char*>(a.out.hi);
+    const char* o_lo = o_hi + a.out.lo_off * 2;
+    const uint32_t s_ps = (uint32_t)a.src.pitch * 16u, o_ps = (uint32_t)a.out.pitch * 16u;
+    int ebank = 0; uint32_t ephase = 0;
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const int b0 = bt * 128, nr = min(128, Bsz - b0);
       const uint32_t a_bytes = (uint32_t)nr * 16u, row_off = (uint32_t)b0 * 16u;
@@ -442,13 +472,33 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
         __syncwarp();
         if (++stage == n_stages) { stage = 0; phase ^= 1; }
       }
+      // The tile's epilogue operands, issued behind its K stages: the epilogue runs only after the first stage of the
+      // next tile, so the copies have a tile's MMAs to land, and the ring is never held up by the bank still in use by
+      // the epilogue before.  Rows [b0, b0 + nr) of the unit's NCH output chunks, per plane.
+      if (KIND == 2 && epi_planes) {
+        mbar_wait(eempty0 + 8 * ebank, ephase ^ 1);
+        if (elect_one()) {
+          const uint32_t fb = efull0 + 8 * ebank;
+          mbar_expect_tx(fb, a_bytes * (uint32_t)(NCH * epi_planes));
+          const uint32_t oc0 = (uint32_t)((tw.mode == 2 ? u % tw.n_ntiles : u) * NCH);
+          uint32_t dst = smem_u32(epi_sm) + (uint32_t)(ebank * epi_bank_bytes);
+          auto plane = [&](const char* base, uint32_t ps) {
+            const char* src = base + oc0 * ps + row_off;
+            for (int c = 0; c < NCH; c++, dst += RW_A_PLANE) bulk_g2s(dst, src + (uint32_t)c * ps, a_bytes, fb);
+          };
+          if (src_act == 1 || src_act == 2) plane(s_hi, s_ps);
+          if (src_act == 2) plane(s_lo, s_ps);
+          if (accumulate) { plane(o_hi, o_ps); plane(o_lo, o_ps); }
+        }
+        __syncwarp();
+        if (++ebank == epi_banks) { ebank = 0; ephase ^= 1; }
+      }
       u += du; bt += dbt;
       if (bt >= nbt) { bt -= nbt; u++; }
     }
   } else if (warp < BP_P_WARP) {
     // ================= consumers: wgmma on the ring stages, epilogue from the accumulator registers =================
     constexpr int ACC = CAT ? 2 * N : N;                 // accumulator columns
-    constexpr int NCH = N >> 3;                          // output feature chunks of a tile
     float dbacc[N / 4];                                  // data gradient: column sums of this thread's columns
 #pragma unroll
     for (int j = 0; j < N / 4; j++) dbacc[j] = 0.f;
@@ -463,9 +513,14 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
     bf16* const out_hi = a.out.hi; const long long out_lo = a.out.lo_off;
     float* const out_f32 = a.out_f32; const float* const bias_g = a.bias;
     float* const part = a.part; const long long part_z = a.part_z;
-    const bf16* const src_hi = a.src.hi; const long long src_lo = a.src.lo_off, src_pstride = (long long)a.src.pitch * 8;
     const long long out_pstride = (long long)a.out.pitch * 8;      // elements between feature chunks
     const int b_pad = (Bsz + 15) & ~15;
+    // data-gradient epilogue operands in shared memory: this thread's word of (plane p, chunk i, tile row r) lies at
+    // epi_thr + bank * epi_bank_bytes + (p * NCH + i) * RW_A_PLANE + 16 * (r - row_in_tile); the output planes follow
+    // the source planes
+    const uint32_t epi_thr = smem_u32(epi_sm) + (uint32_t)(row_in_tile * 16 + 4 * q);
+    const int epi_out_plane = epi_planes - (accumulate ? 2 : 0);
+    int ebank = 0; uint32_t ephase = 0;
     // descriptor constant parts; the low 14 bits hold (shared address >> 4) and are advanced by plain adds
     const uint64_t adesc = make_desc(0, RW_A_PLANE, 128);
     const uint64_t bdesc = (KIND == 2) ? make_desc(0, (uint32_t)N * 16, 128) : make_desc(0, 128, 1024);
@@ -543,8 +598,9 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
       return true;
     };
 
-    // epilogue of tile (cu, cbt) from bank cur: bias / activation / ReLU mask, batch-planar and fp32 stores
-    auto epilogue = [&](const float* cur, int cu, int cbt, bool empty) {
+    // epilogue of tile (cu, cbt) from bank cur: bias / activation / ReLU mask, batch-planar and fp32 stores.  The data
+    // gradient reads act' and the accumulated planes from the epilogue buffer at shared address eb (this thread's word)
+    auto epilogue = [&](const float* cur, int cu, int cbt, bool empty, uint32_t eb) {
       const int btile0 = cbt * 128;
       int oc0, z = 0;                          // first output chunk of the unit
       if (mode == 2) { const int nt = cu % n_nt; z = cu / n_nt; oc0 = nt * NCH; }
@@ -584,23 +640,24 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
           } else {
             bf16* p = out_hi + (long long)(oc0 + i) * out_pstride + (long long)b * 8 + 2 * q;
             if (b < Bsz) {
-              const bf16* sp = src_hi + (long long)(oc0 + i) * src_pstride + (long long)b * 8 + 2 * q;
+              const uint32_t e = eb + (uint32_t)(i * RW_A_PLANE + 128 * h);        // plane 0, chunk i, row b
               if (src_act == 1) {
                 float s0, s1;
-                unpack2(*reinterpret_cast<const uint32_t*>(sp), s0, s1);
+                unpack2(lds_u32(e), s0, s1);
                 v0 = s0 > 0.f ? v0 : 0.f; v1 = s1 > 0.f ? v1 : 0.f;
               } else if (src_act == 2) {
                 float s0, s1, t0, t1;
-                unpack2(*reinterpret_cast<const uint32_t*>(sp), s0, s1);
-                unpack2(*reinterpret_cast<const uint32_t*>(sp + src_lo), t0, t1);
+                unpack2(lds_u32(e), s0, s1);
+                unpack2(lds_u32(e + NCH * RW_A_PLANE), t0, t1);
                 const float y0 = s0 + t0, y1 = s1 + t1;
                 v0 *= 1.f - y0 * y0; v1 *= 1.f - y1 * y1;
               }
               dbacc[2 * i] += v0; dbacc[2 * i + 1] += v1;
               if (accumulate) {
+                const uint32_t eo = e + (uint32_t)(epi_out_plane * NCH * RW_A_PLANE);
                 float s0, s1, t0, t1;
-                unpack2(*reinterpret_cast<const uint32_t*>(p), s0, s1);
-                unpack2(*reinterpret_cast<const uint32_t*>(p + out_lo), t0, t1);
+                unpack2(lds_u32(eo), s0, s1);
+                unpack2(lds_u32(eo + NCH * RW_A_PLANE), t0, t1);
                 v0 += s0 + t0; v1 += s1 + t1;
               }
               uint32_t hi, lo;
@@ -618,8 +675,8 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
     };
 
     // Tile loop, software-pipelined over two accumulator banks: the remaining stages of the current tile go into cur,
-    // then the first stage of the next tile into nxt, and the current tile's epilogue (global loads and stores) runs
-    // while that group is on the tensor pipe.  The wgmma_wait<1> of that first stage is what completes cur's groups.
+    // then the first stage of the next tile into nxt, and the current tile's epilogue runs while that group is on the
+    // tensor pipe (its operands are in shared memory).  The wgmma_wait<1> of that first stage completes cur's groups.
     // Registers cannot be indexed at run time, so the loop is unrolled by two: even tiles in acc0, odd tiles in acc1.
     // The forward at N = 64 (2 x 64 accumulators per bank) does not fit both banks and the epilogue in the 168 registers
     // per thread of a 288-thread CTA: it starts the next tile after the epilogue instead, one bank live at a time.
@@ -638,7 +695,16 @@ bp_rows_kernel(const __grid_constant__ RowsArgs a, int n_stages, int stage_bytes
         held = -1;
       }
       fence_regs<ACC / 2>(cur);
-      if (!idle(cbt)) epilogue(cur, cu, cbt, empty);
+      // every consumer warp waits for the tile's epilogue operands, idle ones included (the producer copies them for
+      // every tile): a wait loop inside the idle branch, with the next tile's wgmma group in flight, makes ptxas
+      // serialize the kernel's wgmma instructions (C7518)
+      if (KIND == 2 && epi_planes) mbar_wait(efull0 + 8 * ebank, ephase);
+      if (!idle(cbt)) epilogue(cur, cu, cbt, empty, epi_thr + (uint32_t)(ebank * epi_bank_bytes));
+      if (KIND == 2 && epi_planes) {       // every consumer warp frees the bank
+        __syncwarp();
+        if (lane == 0) mbar_arrive(eempty0 + 8 * ebank);
+        if (++ebank == epi_banks) { ebank = 0; ephase ^= 1; }
+      }
       if (!OVERLAP && tile < total) start_tile(nxt);
     };
     float acc0[ACC / 2], acc1[ACC / 2];

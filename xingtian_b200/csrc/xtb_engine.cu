@@ -288,16 +288,33 @@ static int pick_tile(int n) { return n % 64 == 0 ? 64 : (n % 32 == 0 ? 32 : (n %
 
 // Dynamic shared memory of the tensor-core launches.  xtb_net_create plans with the same arithmetic as launch_rows /
 // launch_wgrad, so a layer it puts on the tensor cores always gets a launch that fits.
-// bp_rows_kernel: [resident weight blob][ring of n_stages stages][conv stage-walk table]
-struct RowsSmem { int wres_bytes, stage_bytes, tab_bytes, n_stages; };
-static RowsSmem rows_smem(bool w_res, int w_res_chunks, int w_pitch, int mode, size_t n_stage_ents, size_t n_units) {
+// bp_rows_kernel: [resident weight blob][ring of n_stages stages][epilogue banks][conv stage-walk table]
+// epi_planes: planes the data-gradient epilogue prefetches (bp::dgrad_epi_planes; 0 for the forward kernels), each
+// N / 8 chunks x 128 rows x 16 B per bank.  Two banks let the producer fill one tile's operands while the epilogue of
+// the tile before reads the other; when two banks would leave fewer than two ring stages it runs with one.
+struct RowsSmem { int wres_bytes, stage_bytes, epi_bank_bytes, epi_banks, tab_bytes, n_stages; };
+static RowsSmem rows_smem(bool w_res, int w_res_chunks, int w_pitch, int mode, size_t n_stage_ents, size_t n_units, int N,
+                          int epi_planes) {
   RowsSmem r;
   r.wres_bytes = w_res ? (int)align_up((size_t)2 * w_res_chunks * w_pitch * 16, 128) : 0;
   r.stage_bytes = bp::RW_STAGE_A + (w_res ? 0 : bp::RW_STAGE_B);
+  r.epi_bank_bytes = epi_planes * (N / 8) * bp::RW_A_PLANE;
   const size_t tab = mode == 2 ? 0 : align_up(n_stage_ents * sizeof(bp::StageEnt) + n_units * sizeof(bp::UnitEnt), 128);
   r.tab_bytes = (int)std::min(tab, (size_t)kMaxDynSmem + 1);
-  r.n_stages = std::max(0, std::min(bp::RW_MAX_STAGES, (kMaxDynSmem - 128 - r.wres_bytes - r.tab_bytes) / r.stage_bytes));
+  const int room = kMaxDynSmem - 128 - r.wres_bytes - r.tab_bytes;
+  auto stages = [&](int banks) { return std::max(0, std::min(bp::RW_MAX_STAGES, (room - banks * r.epi_bank_bytes) / r.stage_bytes)); };
+  r.epi_banks = epi_planes ? bp::RW_EPI_BANKS : 0;
+  r.n_stages = stages(r.epi_banks);
+  if (r.n_stages < 2 && r.epi_banks > 1) { r.epi_banks = 1; r.n_stages = stages(1); }
   return r;
+}
+// the activation whose derivative a data-gradient epilogue applies: none for the activations past tanh, whose tensors
+// collect the gradient wrt their output until act_backward
+static inline int dgrad_act(const LayerPlan& lp) { return act_is_ext(lp.src_act) ? 0 : lp.src_act; }
+// shared memory of a conv layer's data-gradient launch; accumulate: into a source tensor with another consumer
+static RowsSmem conv_dgrad_smem(const LayerPlan& lp, bool accumulate) {
+  return rows_smem(lp.w_res, lp.N / 8, lp.K, 1, lp.dg_st.size(), lp.dg_un.size(), lp.n_dg,
+                   bp::dgrad_epi_planes(dgrad_act(lp), accumulate));
 }
 // bp_wgrad_kernel: [WG_STAGES stages][conv (output pixel, accumulator) table]
 static size_t wgrad_smem(int mode, int n_opix, int R) {
@@ -317,13 +334,14 @@ static int dense_k_slices(int kchunks, int tiles, int* kc_split) {
   return 1;
 }
 // A conv layer stays on the tensor cores only if its stage tables fit: the forward and data-gradient launches get at
-// least two ring stages beside their table, the weight-gradient table fits beside the WG_STAGES stages, and no unit
-// needs more stages than a UnitEnt counts.  Otherwise it runs on the fp32 kernels.
+// least two ring stages beside their table (the data gradient with the epilogue buffers of an accumulating launch, the
+// largest it can need), the weight-gradient table fits beside the WG_STAGES stages, and no unit needs more stages than
+// a UnitEnt counts.  Otherwise it runs on the fp32 kernels.
 static bool conv_tables_fit(const LayerPlan& lp, uint32_t max_unit_stages) {
   const ConvGeom& q = lp.q;
   if (max_unit_stages > 255 || lp.fwd_st.size() >= (1u << 24) || lp.dg_st.size() >= (1u << 24)) return false;
-  if (rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size()).n_stages < 2) return false;
-  if (rows_smem(lp.w_res, lp.N / 8, lp.K, 1, lp.dg_st.size(), lp.dg_un.size()).n_stages < 2) return false;
+  if (rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size(), lp.n_fwd, 0).n_stages < 2) return false;
+  if (conv_dgrad_smem(lp, true).n_stages < 2) return false;
   return wgrad_smem(0, q.OH * q.OW, lp.R) <= (size_t)kMaxDynSmem;
 }
 
@@ -595,12 +613,13 @@ extern "C" int xtb_net_layer_plan(const xtb_net* net, int layer, xtb_layer_plan*
   out->tc = 1; out->s2d = lp.s2d; out->w_res = lp.w_res;
   out->n_fwd = lp.n_fwd; out->n_dg = lp.n_dg; out->R = lp.R;
   if (lp.d.kind == XTB_CONV) {
-    out->fwd_stages = rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size()).n_stages;
-    out->dg_stages = rows_smem(lp.w_res, lp.N / 8, lp.K, 1, lp.dg_st.size(), lp.dg_un.size()).n_stages;
+    out->fwd_stages = rows_smem(lp.w_res, lp.N / 8, lp.K, 0, lp.fwd_st.size(), lp.fwd_un.size(), lp.n_fwd, 0).n_stages;
+    out->dg_stages = conv_dgrad_smem(lp, false).n_stages;
     for (bp::UnitEnt u : lp.dg_un) out->dg_empty_units += (u >> 24) == 0;
     out->k_slices = 1;
   } else {
-    out->fwd_stages = out->dg_stages = rows_smem(false, 0, lp.K, 2, 0, 0).n_stages;
+    out->fwd_stages = rows_smem(false, 0, lp.K, 2, 0, 0, lp.n_fwd, 0).n_stages;
+    out->dg_stages = rows_smem(false, 0, lp.K, 2, 0, 0, lp.n_dg, bp::dgrad_epi_planes(dgrad_act(lp), 0)).n_stages;
     int kc_split;
     out->k_slices = dense_k_slices(lp.K / 8, (lp.N / lp.n_fwd) * ((net->max_batch + 127) / 128), &kc_split);
   }
@@ -727,7 +746,7 @@ static cudaError_t ensure_kernel_attrs() {
 // the accumulator width is a template parameter of the GEMM kernels (wgmma takes N as an immediate)
 template <int KIND>
 static cudaError_t launch_rows(bp::RowsArgs& a, cudaStream_t st) {
-  void (*kern)(bp::RowsArgs, int, int, int);
+  void (*kern)(bp::RowsArgs, int, int, int, int);
   switch (a.N) {
     case 16: kern = bp::bp_rows_kernel<KIND, 16>; break;
     case 32: kern = bp::bp_rows_kernel<KIND, 32>; break;
@@ -736,12 +755,14 @@ static cudaError_t launch_rows(bp::RowsArgs& a, cudaStream_t st) {
     default: return cudaErrorInvalidValue;
   }
   { cudaError_t e0 = ensure_kernel_attrs(); if (e0 != cudaSuccess) return e0; }
-  const RowsSmem m = rows_smem(a.w_res != 0, a.w_res_chunks, a.w_pitch, a.mode, (size_t)a.n_stage_ents, (size_t)a.n_units);
+  const int epi_planes = KIND == 2 ? bp::dgrad_epi_planes(a.src_act, a.accumulate) : 0;
+  const RowsSmem m = rows_smem(a.w_res != 0, a.w_res_chunks, a.w_pitch, a.mode, (size_t)a.n_stage_ents, (size_t)a.n_units, a.N,
+                               epi_planes);
   if (m.n_stages < 2) return cudaErrorInvalidConfiguration;
-  const int smem = 128 + m.wres_bytes + m.n_stages * m.stage_bytes + m.tab_bytes;
+  const int smem = 128 + m.wres_bytes + m.n_stages * m.stage_bytes + m.epi_banks * m.epi_bank_bytes + m.tab_bytes;
   const int total = a.n_units * a.n_btiles;
   const int grid = std::min(total, kSMs);
-  XLAUNCH(kern, grid, bp::RW_THREADS, smem, st, a, m.n_stages, m.stage_bytes, m.wres_bytes);
+  XLAUNCH(kern, grid, bp::RW_THREADS, smem, st, a, m.n_stages, m.stage_bytes, m.wres_bytes, m.epi_banks);
   return cudaPeekAtLastError();
 }
 
@@ -804,10 +825,6 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   *launches = 2;
   return cudaPeekAtLastError();
 }
-
-// the activation whose derivative a data-gradient epilogue applies: none for the activations past tanh, whose tensors
-// collect the gradient wrt their output until act_backward
-static inline int dgrad_act(const LayerPlan& lp) { return act_is_ext(lp.src_act) ? 0 : lp.src_act; }
 
 // data gradient of tensor-core layer i into the planes of its source tensor
 static cudaError_t tc_dgrad(xtb_net* net, int i, int B, int accumulate, float* db_part, cudaStream_t st) {
