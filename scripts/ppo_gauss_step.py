@@ -5,7 +5,7 @@ network, alternated in one process.
 Shapes:
   pendulum: PpoMlp [3] -> A = 1, tanh [64, 64], separate towers; E = 10 envs x T = 200 steps, BATCH_SIZE 200, 8 epochs
   pixel:    PpoCnn 84x84x4 uint8 -> A = 3, relu [256], shared tower; E = 32 x T = 128, BATCH_SIZE 320, 4 epochs
-Variants: gauss_fused (the fused Gaussian heads: heads_kernel<PpoGaussLoss> in training, gauss_infer_heads_kernel in
+Variants: gauss_fused (the fused Gaussian heads: heads_kernel<PpoGaussLoss> in training, infer_heads_kernel<DiagGaussian> in
 inference; the default), gauss_layers (xtb_set_fuse_heads(0)), and the same two for Categorical at the same A.  Per variant and round: warm-up
 replays, then CUDA events around `--replays` graph replays of the train call and of one T-step rollout inference; the
 rounds alternate the variants.  Launches per call come from xtb_launch_count around one eager (non-graph) call.  Prints

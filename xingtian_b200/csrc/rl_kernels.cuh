@@ -112,70 +112,63 @@ __device__ inline void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
   }
 }
 
-__global__ void sample_kernel(const float* __restrict__ logits, int B, int A,
-                              const float* __restrict__ uniforms, uint64_t seed, uint64_t offset,
-                              int32_t* __restrict__ action, float* __restrict__ logp) {
-  pdl_wait(); pdl_trigger();
-  int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  const float* l = logits + (long long)b * A;
+// Categorical draw of sample b (xt/model/tf_dist.py:89-130): Gumbel-max over its logits lg[0..A), A <= n (n: the
+// size of a register array, whose loops are unrolled, or A).  Uniform i is u[i] when u is set, else a word of
+// Philox4x32-10 on counter (b, i / 4, offset) mapped into (0, 1).  The first maximum wins, like np.argmax.  Returns the
+// action; logp = its log-probability.
+template <class LG>
+__device__ __forceinline__ int categorical_draw(const LG& lg, int n, int A, const float* u, int b, uint64_t seed,
+                                                uint64_t offset, float& logp) {
   float mx = -INFINITY;
-  for (int i = 0; i < A; i++) mx = fmaxf(mx, l[i]);
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i < A) mx = fmaxf(mx, lg[i]);
   float z = 0.f;
-  for (int i = 0; i < A; i++) z += expf(l[i] - mx);
-  float lz = logf(z);
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i < A) z += expf(lg[i] - mx);
+  const float lz = logf(z);
   float best = -INFINITY; int bi = 0;
   uint32_t c[4] = {0, 0, 0, 0};
-  for (int i = 0; i < A; i++) {
-    float u;
-    if (uniforms) {
-      u = uniforms[(long long)b * A + i];
-    } else {
-      if ((i & 3) == 0) {
-        c[0] = (uint32_t)b; c[1] = (uint32_t)(i >> 2);
-        c[2] = (uint32_t)(offset & 0xffffffffu); c[3] = (uint32_t)(offset >> 32);
-        philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
+#pragma unroll
+  for (int i = 0; i < n; i++) {
+    if (i < A) {
+      float ui;
+      if (u) {
+        ui = u[i];
+      } else {
+        if ((i & 3) == 0) {
+          c[0] = (uint32_t)b; c[1] = (uint32_t)(i >> 2);
+          c[2] = (uint32_t)(offset & 0xffffffffu); c[3] = (uint32_t)(offset >> 32);
+          philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
+        }
+        ui = (float)(c[i & 3] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
       }
-      u = (float)(c[i & 3] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
+      const float s = lg[i] - logf(-logf(ui));
+      if (s > best) { best = s; bi = i; }
     }
-    float g = -logf(-logf(u));
-    float s = l[i] + g;
-    if (s > best) { best = s; bi = i; }   // first maximum wins, like np.argmax
   }
-  action[b] = bi;
-  logp[b] = l[bi] - mx - lz;
+  float la = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i == bi) la = lg[i];
+  logp = la - mx - lz;
+  return bi;
 }
 
-// rollout variant: Philox offset = *offset_dev + t_add (device-resident counter so that CUDA-graph replays
-// draw fresh noise), and the value head output is copied out alongside.
-__global__ void sample_rollout_kernel(const float* __restrict__ logits, const float* __restrict__ v_in, int B, int A,
-                                      uint64_t seed, const unsigned long long* __restrict__ offset_dev, int t_add,
-                                      int32_t* __restrict__ action, float* __restrict__ logp, float* __restrict__ v_out) {
+// One thread per sample: the categorical draw from logits [B, A] with uniforms [B, A] if set, else Philox at `offset`,
+// or at *offset_dev + t_add when offset_dev is set (the device-resident counter of rollout inference, so that CUDA-graph
+// replays draw fresh noise).  v_out != NULL: the value head output is copied out alongside.
+__global__ void sample_kernel(const float* __restrict__ logits, int B, int A, const float* __restrict__ uniforms,
+                              uint64_t seed, uint64_t offset, const unsigned long long* __restrict__ offset_dev, int t_add,
+                              int32_t* __restrict__ action, float* __restrict__ logp, const float* __restrict__ v_in,
+                              float* __restrict__ v_out) {
   pdl_wait(); pdl_trigger();
-  int b = blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  uint64_t offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
-  const float* l = logits + (long long)b * A;
-  float mx = -INFINITY;
-  for (int i = 0; i < A; i++) mx = fmaxf(mx, l[i]);
-  float z = 0.f;
-  for (int i = 0; i < A; i++) z += expf(l[i] - mx);
-  float lz = logf(z);
-  float best = -INFINITY; int bi = 0;
-  uint32_t c[4] = {0, 0, 0, 0};
-  for (int i = 0; i < A; i++) {
-    if ((i & 3) == 0) {
-      c[0] = (uint32_t)b; c[1] = (uint32_t)(i >> 2);
-      c[2] = (uint32_t)(offset & 0xffffffffu); c[3] = (uint32_t)(offset >> 32);
-      philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
-    }
-    float u = (float)(c[i & 3] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
-    float s = l[i] - logf(-logf(u));
-    if (s > best) { best = s; bi = i; }
-  }
-  action[b] = bi;
-  logp[b] = l[bi] - mx - lz;
-  v_out[b] = v_in[b];
+  if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
+  float lp;
+  action[b] = categorical_draw(logits + (long long)b * A, A, A, uniforms ? uniforms + (long long)b * A : nullptr, b, seed,
+                               offset, lp);
+  logp[b] = lp;
+  if (v_out) v_out[b] = v_in[b];
 }
 __global__ void bump_counter_kernel(unsigned long long* ctr, int add) {
   pdl_wait(); pdl_trigger(); *ctr += (unsigned long long)add; }
@@ -194,6 +187,25 @@ __global__ void argmax_kernel(const float* __restrict__ q, int B, int A, int32_t
 // PPO loss + gradient wrt (logits, v).  One thread per sample.
 // ------------------------------------------------------------------------------------------
 struct PpoHyperDev { float clip_ratio, ent_coef, vf_clip, critic_coef; };
+
+// The clipped surrogate and the clipped value loss of one sample, whatever the action distribution: surr, dsurr =
+// d surr / d logp_a (through s1 when s1 <= s2, else through the clip: zero outside the range), critic = the critic
+// term of the loss, dv = d loss / d v.
+struct PpoClipTerms { float surr, dsurr, critic, dv; };
+__device__ __forceinline__ PpoClipTerms ppo_clip_terms(float logp_a, float old_logp, float ad, float vv, float ov, float R,
+                                                       const PpoHyperDev& hp, float inv_count) {
+  const float ratio = expf(logp_a - old_logp);
+  const float s1 = ratio * ad;
+  const float s2 = fminf(fmaxf(ratio, 1.f - hp.clip_ratio), 1.f + hp.clip_ratio) * ad;
+  const float surr = fminf(s1, s2);
+  const float dsurr = (s1 <= s2) ? ratio * ad
+                                 : ((ratio >= 1.f - hp.clip_ratio && ratio <= 1.f + hp.clip_ratio) ? ratio * ad : 0.f);
+  const float l1 = (vv - R) * (vv - R);
+  const float vc = ov + fminf(fmaxf(vv - ov, -hp.vf_clip), hp.vf_clip);
+  const float l2 = (vc - R) * (vc - R);
+  const float dvl = (l1 >= l2) ? 2.f * (vv - R) : ((vv - ov >= -hp.vf_clip && vv - ov <= hp.vf_clip) ? 2.f * (vc - R) : 0.f);
+  return {surr, dsurr, hp.critic_coef * 0.5f * fmaxf(l1, l2), hp.critic_coef * 0.5f * dvl * inv_count};
+}
 
 __global__ void ppo_loss_kernel(const float* __restrict__ logits, const float* __restrict__ v,
                                 const int32_t* __restrict__ idx, const int32_t* __restrict__ action,
@@ -217,34 +229,16 @@ __global__ void ppo_loss_kernel(const float* __restrict__ logits, const float* _
     float H = 0.f;
     for (int i = 0; i < A; i++) { float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
     int a = action[r];
-    float logp_a = lg[a] - mx - lz;
-    float ratio = expf(logp_a - old_logp[r]);
-    float ad = adv[r];
-    float s1 = ratio * ad;
-    float rc = fminf(fmaxf(ratio, 1.f - hp.clip_ratio), 1.f + hp.clip_ratio);
-    float s2 = rc * ad;
-    float surr = fminf(s1, s2);
-    // d surr / d logp_a : through s1 when s1<=s2, else through the clip (zero outside the range)
-    float dsurr;
-    if (s1 <= s2) dsurr = ratio * ad;
-    else dsurr = (ratio >= 1.f - hp.clip_ratio && ratio <= 1.f + hp.clip_ratio) ? ratio * ad : 0.f;
-    float vv = v[b], R = target_v[r], ov = old_v[r];
-    float l1 = (vv - R) * (vv - R);
-    float dcl = fminf(fmaxf(vv - ov, -hp.vf_clip), hp.vf_clip);
-    float vc = ov + dcl;
-    float l2 = (vc - R) * (vc - R);
-    float dvl;
-    if (l1 >= l2) dvl = 2.f * (vv - R);
-    else dvl = (vv - ov >= -hp.vf_clip && vv - ov <= hp.vf_clip) ? 2.f * (vc - R) : 0.f;
-    lsum = (-surr - hp.ent_coef * H + hp.critic_coef * 0.5f * fmaxf(l1, l2)) * inv_count;
-    dv[b] = hp.critic_coef * 0.5f * dvl * inv_count;
+    const PpoClipTerms c = ppo_clip_terms(lg[a] - mx - lz, old_logp[r], adv[r], v[b], old_v[r], target_v[r], hp, inv_count);
+    lsum = (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
+    dv[b] = c.dv;
     for (int i = 0; i < A; i++) {
       float rl = lg[i] - mx;
       float p = expf(rl) / z;
       float logp_i = rl - lz;
       float dlogp = ((i == a) ? 1.f : 0.f) - p;             // d logp_a / d l_i
       float dH = -p * (logp_i + H);                           // d H / d l_i
-      dlogits[(long long)b * A + i] = (-dsurr * dlogp - hp.ent_coef * dH) * inv_count;
+      dlogits[(long long)b * A + i] = (-c.dsurr * dlogp - hp.ent_coef * dH) * inv_count;
     }
   }
   block_atomic_add(lsum, loss_out);
@@ -491,30 +485,18 @@ struct PpoLoss {
     float logp_a = 0.f;
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) logp_a = lg[i] - mx - lz;
-    float ratio = expf(logp_a - a.old_logp[r]);
-    float ad = a.adv[r];
-    float s1 = ratio * ad;
-    float s2 = fminf(fmaxf(ratio, 1.f - a.hp.clip_ratio), 1.f + a.hp.clip_ratio) * ad;
-    float surr = fminf(s1, s2);
-    float dsurr = (s1 <= s2) ? ratio * ad
-                             : ((ratio >= 1.f - a.hp.clip_ratio && ratio <= 1.f + a.hp.clip_ratio) ? ratio * ad : 0.f);
-    float R = a.target_v[r], ov = a.old_v[r];
-    float l1 = (vv - R) * (vv - R);
-    float vc = ov + fminf(fmaxf(vv - ov, -a.hp.vf_clip), a.hp.vf_clip);
-    float l2 = (vc - R) * (vc - R);
-    float dvl = (l1 >= l2) ? 2.f * (vv - R)
-                           : ((vv - ov >= -a.hp.vf_clip && vv - ov <= a.hp.vf_clip) ? 2.f * (vc - R) : 0.f);
-    dv = a.hp.critic_coef * 0.5f * dvl * a.inv_count;
+    const PpoClipTerms c = ppo_clip_terms(logp_a, a.old_logp[r], a.adv[r], vv, a.old_v[r], a.target_v[r], a.hp, a.inv_count);
+    dv = c.dv;
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) {
       dl[i] = 0.f;
       if (i < A) {
         float rl = lg[i] - mx, p = expf(rl) / z;
-        dl[i] = (-dsurr * (((i == ac) ? 1.f : 0.f) - p) + a.hp.ent_coef * p * (rl - lz + H)) * a.inv_count;
+        dl[i] = (-c.dsurr * (((i == ac) ? 1.f : 0.f) - p) + a.hp.ent_coef * p * (rl - lz + H)) * a.inv_count;
       }
     }
     if (lane == 0) {
-      lsum += (-surr - a.hp.ent_coef * H + a.hp.critic_coef * 0.5f * fmaxf(l1, l2)) * a.inv_count;
+      lsum += (-c.surr - a.hp.ent_coef * H + c.critic) * a.inv_count;
       if (a.logits_out) for (int i = 0; i < A; i++) a.logits_out[(long long)b * A + i] = lg[i];
       if (a.v_out) a.v_out[b] = vv;
       dbv += dv;
@@ -730,68 +712,6 @@ __global__ void __launch_bounds__(256) dueling_dgrad_kernel(const float* __restr
   }
 }
 
-// Inference heads: logits / value of both dense heads + Gumbel-max sampling in one kernel (one warp per sample).
-// Philox offset = *offset_dev + t_add (device-resident counter, see sample_rollout_kernel).
-template <int HEAD_KPL, int HEAD_AMAX>
-__global__ void __launch_bounds__(256)
-ppo_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v, const float* __restrict__ w_pi,
-                       const float* __restrict__ b_pi, const float* __restrict__ w_v, const float* __restrict__ b_v,
-                       int B, int K, int A, uint64_t seed, const unsigned long long* __restrict__ offset_dev, int t_add,
-                       int32_t* __restrict__ action, float* __restrict__ logp, float* __restrict__ v_out,
-                       float* __restrict__ logits_out) {
-  pdl_wait(); pdl_trigger();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
-  const int kpl = K / 32;
-  const uint64_t offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
-  for (int b = blockIdx.x * nwarp + warp; b < B; b += gridDim.x * nwarp) {
-    float acc[HEAD_AMAX + 1];
-#pragma unroll
-    for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = 0.f;
-#pragma unroll
-    for (int j = 0; j < HEAD_KPL; j++) {
-      if (j < kpl) {
-        int k = lane + 32 * j;
-        float hp = h_pi[(long long)b * K + k], hv = h_v[(long long)b * K + k];
-#pragma unroll
-        for (int i = 0; i < HEAD_AMAX; i++) if (i < A) acc[i] = fmaf(hp, w_pi[k * A + i], acc[i]);
-        acc[HEAD_AMAX] = fmaf(hv, w_v[k], acc[HEAD_AMAX]);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
-    if (lane == 0) {
-      float lg[HEAD_AMAX]; float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) { lg[i] = (i < A) ? acc[i] + b_pi[i] : -INFINITY; mx = fmaxf(mx, lg[i]); }
-      float z = 0.f;
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) if (i < A) z += expf(lg[i] - mx);
-      float lz = logf(z), best = -INFINITY; int bi = 0;
-      uint32_t c[4] = {0, 0, 0, 0};
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) {
-        if (i < A) {
-          if ((i & 3) == 0) {
-            c[0] = (uint32_t)b; c[1] = (uint32_t)(i >> 2);
-            c[2] = (uint32_t)(offset & 0xffffffffu); c[3] = (uint32_t)(offset >> 32);
-            philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
-          }
-          float u = (float)(c[i & 3] >> 8) * 5.9604644775390625e-08f + 2.98023223876953125e-08f;
-          float sc = lg[i] - logf(-logf(u));
-          if (sc > best) { best = sc; bi = i; }
-          if (logits_out) logits_out[(long long)b * A + i] = lg[i];
-        }
-      }
-      float la = 0.f;
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) if (i == bi) la = lg[i];
-      action[b] = bi;
-      logp[b] = la - mx - lz;
-      v_out[b] = acc[HEAD_AMAX] + b_v[0];
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------
 // Diagonal Gaussian policy of PPO (xt/model/tf_dist.py:49-86, xt/model/ppo/ppo.py:75-83): mean = pi_latent [B, A],
 // log_std = the A floats of the pi_logstd variable, std = exp(log_std).
@@ -882,25 +802,14 @@ ppo_gauss_loss_kernel(const float* __restrict__ mean, const float* __restrict__ 
       if (i < A) { z[i] = (x[i] - m[i]) / sd[i]; q += z[i] * z[i]; }
     }
     const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
-    const float ratio = expf(logp_a - old_logp[r]);
-    const float ad = adv[r];
-    const float s1 = ratio * ad;
-    const float s2 = fminf(fmaxf(ratio, 1.f - hp.clip_ratio), 1.f + hp.clip_ratio) * ad;
-    const float surr = fminf(s1, s2);
-    const float dsurr = (s1 <= s2) ? ratio * ad
-                                   : ((ratio >= 1.f - hp.clip_ratio && ratio <= 1.f + hp.clip_ratio) ? ratio * ad : 0.f);
-    const float vv = v[b], R = target_v[r], ov = old_v[r];
-    const float l1 = (vv - R) * (vv - R);
-    const float vc = ov + fminf(fmaxf(vv - ov, -hp.vf_clip), hp.vf_clip);
-    const float l2 = (vc - R) * (vc - R);
-    const float dvl = (l1 >= l2) ? 2.f * (vv - R) : ((vv - ov >= -hp.vf_clip && vv - ov <= hp.vf_clip) ? 2.f * (vc - R) : 0.f);
-    lsum += (-surr - hp.ent_coef * H + hp.critic_coef * 0.5f * fmaxf(l1, l2)) * inv_count;
-    dv[b] = hp.critic_coef * 0.5f * dvl * inv_count;
+    const PpoClipTerms c = ppo_clip_terms(logp_a, old_logp[r], adv[r], v[b], old_v[r], target_v[r], hp, inv_count);
+    lsum += (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
+    dv[b] = c.dv;
 #pragma unroll
     for (int i = 0; i < AMAX; i++) {
       if (i < A) {
-        dmean[(long long)b * A + i] = -dsurr * (z[i] / sd[i]) * inv_count;
-        acc[i] += (-dsurr * (z[i] * z[i] - 1.f) - hp.ent_coef) * inv_count;
+        dmean[(long long)b * A + i] = -c.dsurr * (z[i] / sd[i]) * inv_count;
+        acc[i] += (-c.dsurr * (z[i] * z[i] - 1.f) - hp.ent_coef) * inv_count;
       }
     }
   }
@@ -946,45 +855,85 @@ struct PpoGaussLoss {
     }
     const float vv = acc[HEAD_AMAX] + a.b_v[0];
     const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
-    const float ratio = expf(logp_a - a.old_logp[r]);
-    const float ad = a.adv[r];
-    const float s1 = ratio * ad;
-    const float s2 = fminf(fmaxf(ratio, 1.f - a.hp.clip_ratio), 1.f + a.hp.clip_ratio) * ad;
-    const float surr = fminf(s1, s2);
-    const float dsurr = (s1 <= s2) ? ratio * ad
-                                   : ((ratio >= 1.f - a.hp.clip_ratio && ratio <= 1.f + a.hp.clip_ratio) ? ratio * ad : 0.f);
-    const float R = a.target_v[r], ov = a.old_v[r];
-    const float l1 = (vv - R) * (vv - R);
-    const float vc = ov + fminf(fmaxf(vv - ov, -a.hp.vf_clip), a.hp.vf_clip);
-    const float l2 = (vc - R) * (vc - R);
-    const float dvl = (l1 >= l2) ? 2.f * (vv - R)
-                                 : ((vv - ov >= -a.hp.vf_clip && vv - ov <= a.hp.vf_clip) ? 2.f * (vc - R) : 0.f);
-    dv = a.hp.critic_coef * 0.5f * dvl * a.inv_count;
+    const PpoClipTerms c = ppo_clip_terms(logp_a, a.old_logp[r], a.adv[r], vv, a.old_v[r], a.target_v[r], a.hp, a.inv_count);
+    dv = c.dv;
 #pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? -dsurr * (z[i] / sd[i]) * a.inv_count : 0.f;
+    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? -c.dsurr * (z[i] / sd[i]) * a.inv_count : 0.f;
     if (lane == 0) {
-      lsum += (-surr - a.hp.ent_coef * H + a.hp.critic_coef * 0.5f * fmaxf(l1, l2)) * a.inv_count;
+      lsum += (-c.surr - a.hp.ent_coef * H + c.critic) * a.inv_count;
       if (a.v_out) a.v_out[b] = vv;
       dbv += dv;
 #pragma unroll
       for (int i = 0; i < HEAD_AMAX; i++) {
         if (a.logits_out && i < A) a.logits_out[(long long)b * A + i] = mean[i];
         dbp[i] += dl[i];
-        if (i < A) dls[i] += (-dsurr * (z[i] * z[i] - 1.f) - a.hp.ent_coef) * a.inv_count;
+        if (i < A) dls[i] += (-c.dsurr * (z[i] * z[i] - 1.f) - a.hp.ent_coef) * a.inv_count;
       }
     }
   }
 };
 
-// Gaussian inference heads: mean / value of both dense heads and the sample of gauss_sample_kernel (Philox offset
-// *offset_dev + t_add) in one kernel, one warp per sample; the Gaussian counterpart of ppo_infer_heads_kernel.
-template <int HEAD_KPL, int HEAD_AMAX>
+// Action distributions of the PPO pipeline.  Action: the action element, one per sample (Categorical: int32 [B]) or A
+// per sample (DiagGaussian: float [B, A]); kLogStd: the policy owns the log_std parameters; Loss: its heads_kernel
+// policy.  infer(): lane 0 of infer_heads_kernel turns the head sums acc (as in heads_kernel) into the sample's draw,
+// writes action / logp and, when head_out is set, the pi head's output (logits / mean).
+struct Categorical {
+  using Action = int32_t;
+  using Loss = PpoLoss;
+  static constexpr bool kLogStd = false;
+  __host__ __device__ static constexpr int action_width(int) { return 1; }
+  template <int HEAD_AMAX>
+  static __device__ __forceinline__ void infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float*, int b, int A,
+                                               uint64_t seed, uint64_t offset, int32_t* action, float* logp, float* head_out) {
+    float lg[HEAD_AMAX];
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) lg[i] = (i < A) ? acc[i] + b_pi[i] : -INFINITY;
+    if (head_out) {
+#pragma unroll
+      for (int i = 0; i < HEAD_AMAX; i++) if (i < A) head_out[(long long)b * A + i] = lg[i];
+    }
+    float lp;
+    action[b] = categorical_draw(lg, HEAD_AMAX, A, nullptr, b, seed, offset, lp);
+    logp[b] = lp;
+  }
+};
+
+// the sample of gauss_sample_kernel
+struct DiagGaussian {
+  using Action = float;
+  using Loss = PpoGaussLoss;
+  static constexpr bool kLogStd = true;
+  __host__ __device__ static constexpr int action_width(int A) { return A; }
+  template <int HEAD_AMAX>
+  static __device__ __forceinline__ void infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float* log_std, int b,
+                                               int A, uint64_t seed, uint64_t offset, float* action, float* logp, float* head_out) {
+    float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) {
+      if (i < A) {
+        if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
+        const float m = acc[i] + b_pi[i], ls = log_std[i], sd = expf(ls);
+        const float x = m + sd * n4[i & 3];
+        const float z = (x - m) / sd;
+        q += z * z; sls += ls;
+        action[(long long)b * A + i] = x;
+        if (head_out) head_out[(long long)b * A + i] = m;
+      }
+    }
+    logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+  }
+};
+
+// Inference heads of PPO: the pi head (logits / mean) and the value head of one dense layer each, then the draw of
+// DIST at Philox offset *offset_dev + t_add (the device-resident counter of rollout inference), in one kernel, one warp
+// per sample.  log_std: DiagGaussian only.
+template <class DIST, int HEAD_KPL, int HEAD_AMAX>
 __global__ void __launch_bounds__(256)
-gauss_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v, const float* __restrict__ w_pi,
-                         const float* __restrict__ b_pi, const float* __restrict__ w_v, const float* __restrict__ b_v,
-                         const float* __restrict__ log_std, int B, int K, int A, uint64_t seed,
-                         const unsigned long long* __restrict__ offset_dev, int t_add, float* __restrict__ action,
-                         float* __restrict__ logp, float* __restrict__ v_out, float* __restrict__ mean_out) {
+infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v, const float* __restrict__ w_pi,
+                   const float* __restrict__ b_pi, const float* __restrict__ w_v, const float* __restrict__ b_v,
+                   const float* __restrict__ log_std, int B, int K, int A, uint64_t seed,
+                   const unsigned long long* __restrict__ offset_dev, int t_add, typename DIST::Action* __restrict__ action,
+                   float* __restrict__ logp, float* __restrict__ v_out, float* __restrict__ head_out) {
   pdl_wait(); pdl_trigger();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   const int kpl = K / 32;
@@ -1006,20 +955,7 @@ gauss_infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict
 #pragma unroll
     for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
     if (lane == 0) {
-      float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) {
-        if (i < A) {
-          if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
-          const float m = acc[i] + b_pi[i], ls = log_std[i], sd = expf(ls);
-          const float x = m + sd * n4[i & 3];
-          const float z = (x - m) / sd;
-          q += z * z; sls += ls;
-          action[(long long)b * A + i] = x;
-          if (mean_out) mean_out[(long long)b * A + i] = m;
-        }
-      }
-      logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+      DIST::template infer<HEAD_AMAX>(acc, b_pi, log_std, b, A, seed, offset, action, logp, head_out);
       v_out[b] = acc[HEAD_AMAX] + b_v[0];
     }
   }

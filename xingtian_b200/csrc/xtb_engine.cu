@@ -1471,7 +1471,8 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
 extern "C" int xtb_categorical_sample(const float* logits, int batch, int adim, const float* uniforms,
                                       uint64_t seed, uint64_t offset, int32_t* action, float* logp, void* stream) {
   if (!logits || !action || !logp || batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_categorical_sample: bad argument");
-  XLAUNCH(sample_kernel, (batch + 127) / 128, 128, 0, S(stream), logits, batch, adim, uniforms, seed, offset, action, logp);
+  XLAUNCH(sample_kernel, (batch + 127) / 128, 128, 0, S(stream), logits, batch, adim, uniforms, seed, offset,
+          (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
   LAUNCH_CHECK();
   return XTB_OK;
 }
@@ -1868,10 +1869,11 @@ static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
   return sc.end();
 }
 
-// heads_kernel instantiations: K hidden units (K % 32 == 0) and A actions, A <= 8 with K <= 256 or A <= 4 with K <= 512
-static bool heads_fit(int K, int A) {
+// Fused-heads instantiations for K hidden units (K % 32 == 0) and A actions: heads_kernel (training) covers A <= 8 with
+// K <= 256 or A <= 4 with K <= 512; infer_heads_kernel (infer) covers A <= 8 with K <= 512
+static bool heads_fit(int K, int A, bool infer = false) {
   const int kpl = K / 32;
-  return K % 32 == 0 && A <= 8 && (kpl <= 8 || (kpl <= 16 && A <= 4));
+  return K % 32 == 0 && A <= 8 && (kpl <= 8 || (kpl <= 16 && (infer || A <= 4)));
 }
 template <class LOSS>
 static void launch_heads(const PpoHeadsArgs& a, int blocks, size_t shb, cudaStream_t st) {
@@ -1880,6 +1882,14 @@ static void launch_heads(const PpoHeadsArgs& a, int blocks, size_t shb, cudaStre
   else if (kpl <= 8 && a.A <= 4) XLAUNCH((heads_kernel<LOSS, 8, 4>), blocks, 256, shb, st, a);
   else if (kpl <= 8) XLAUNCH((heads_kernel<LOSS, 8, 8>), blocks, 256, shb, st, a);
   else XLAUNCH((heads_kernel<LOSS, 16, 4>), blocks, 256, shb, st, a);
+}
+template <class DIST, class... Args>
+static void launch_infer_heads(int K, int A, int blocks, cudaStream_t st, Args... args) {
+  const int kpl = K / 32;
+  if (kpl <= 2) XLAUNCH((infer_heads_kernel<DIST, 2, 8>), blocks, 256, 0, st, args...);
+  else if (kpl <= 8 && A <= 4) XLAUNCH((infer_heads_kernel<DIST, 8, 4>), blocks, 256, 0, st, args...);
+  else if (kpl <= 8) XLAUNCH((infer_heads_kernel<DIST, 8, 8>), blocks, 256, 0, st, args...);
+  else XLAUNCH((infer_heads_kernel<DIST, 16, 8>), blocks, 256, 0, st, args...);
 }
 
 // The epoch x minibatch loop of PPO.train (xt/model/ppo/ppo.py:111-132): minibatch k of epoch e holds rows
@@ -1918,22 +1928,23 @@ static float ppo_inv_world() {
 }
 
 // Fused PPO heads of tensors pi_t / v_t: both heads are linear dense layers on hidden (non-observation) tensors of equal
-// width within the heads_kernel limits, and the fused-heads mode is on
-static bool ppo_heads_fusable(const xtb_net* net, int pi_t, int v_t) {
+// width within the heads_kernel limits (infer: the infer_heads_kernel limits), and the fused-heads mode is on
+static bool ppo_heads_fusable(const xtb_net* net, int pi_t, int v_t, bool infer) {
   const LayerPlan& lpi = net->L[pi_t - 1];
   const LayerPlan& lv = net->L[v_t - 1];
   return g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
-         lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && heads_fit(lpi.K, net->tsize[pi_t]);
+         lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && heads_fit(lpi.K, net->tsize[pi_t], infer);
 }
 
-// One fused PPO minibatch after the forward of the layers below the heads: heads_kernel<LOSS> evaluates both heads, the
-// loss and their backward, writes the gradient wrt the hidden tensors (straight into their planes when the hidden layer
-// runs on tensor cores), and its per-block slabs are queued for the ordered reduction at the end of the backward pass of
-// the layers below.  `a` carries the loss inputs (idx, rollout arrays, hyper-parameters); ls_off >= 0: the offset of
-// the log_std floats whose gradient the policy adds to the slab (LOSS::kLogStd).
+// One fused minibatch after the forward of the layers below the heads pi_t / v_t (the PPO heads, or the dueling value /
+// adv streams): heads_kernel<LOSS> evaluates both heads, the loss and their backward, writes the gradient wrt the
+// hidden tensors (straight into their planes when the hidden layer runs on tensor cores), and its per-block slabs are
+// queued for the ordered reduction at the end of the backward pass of the layers below, which follows.  `a` carries
+// the loss inputs (idx, rollout arrays, hyper-parameters); the slab's loss goes to *loss_dst; ls_off >= 0: the offset
+// of the log_std floats whose gradient the policy adds to the slab (LOSS::kLogStd).
 template <class LOSS>
-static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, int pi_t, int v_t, unsigned skip,
-                           long long ls_off, float* step_loss, void* stream) {
+static int heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, int pi_t, int v_t, unsigned skip,
+                       long long ls_off, float* loss_dst, void* stream) {
   const LayerPlan& lpi = net->L[pi_t - 1];
   const LayerPlan& lv = net->L[v_t - 1];
   const int adim = net->tsize[pi_t];
@@ -1956,7 +1967,6 @@ static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int m
   bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src) && !ext_pi;
   bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src) && !ext_v;
   unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
-  a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
   a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = dgrad_act(lpi); a.act_v = dgrad_act(lv); a.shared = lpi.d.src == lv.d.src ? 1 : 0;
   int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
   const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2 + (LOSS::kLogStd ? adim : 0);
@@ -1979,7 +1989,7 @@ static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int m
     if (!a.shared && bh_v_ok) seg(HK * adim + 2 * HK, HK, net->L[lv.d.src - 1].b_off, nullptr);
     seg(HK * adim + 3 * HK, adim, lpi.b_off, nullptr);
     seg(HK * adim + 3 * HK + adim, 1, lv.b_off, nullptr);
-    seg(HK * adim + 3 * HK + adim + 1, 1, 0, step_loss);
+    seg(HK * adim + 3 * HK + adim + 1, 1, 0, loss_dst);
     if (LOSS::kLogStd) seg(HK * adim + 3 * HK + adim + 2, adim, ls_off, nullptr);
   }
   int srcs[2] = {lpi.d.src, lv.d.src};
@@ -1988,120 +1998,111 @@ static int ppo_heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int m
   return net_backward_impl(net, obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm, hdy);
 }
 
-static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E,
-                            const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t,
-                            float* loss_per_step, float inv_world, void* stream) {
-  int heads[2] = {pi_t, v_t};
-  int adim = net->tsize[pi_t];
-  const LayerPlan& lpi = net->L[pi_t - 1];
-  const LayerPlan& lv = net->L[v_t - 1];
-  const bool fuse = ppo_heads_fusable(net, pi_t, v_t);
-  unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
-  return ppo_epoch_loop(net, opt, N, B, E, perm, loss_per_step, stream, [&](const int32_t* idx, int mb, float* step_loss) -> int {
-      // fp32 row-major copies: the hidden tensors the fused heads read, or the head outputs the loss kernel reads
-      unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
-      int rc = net_forward_impl(net, nullptr, ro->obs, idx, mb, stream, skip, want);
-      if (rc) return rc;
-      if (fuse) {
-        PpoHeadsArgs a;
-        memset(&a, 0, sizeof a);
-        a.idx = idx; a.action = ro->action; a.old_logp = ro->old_logp; a.adv = ro->adv; a.old_v = ro->old_v; a.target_v = ro->target_v;
-        a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
-        return ppo_heads_fused<PpoLoss>(net, ro->obs, a, mb, pi_t, v_t, skip, -1, step_loss, stream);
-      }
-      rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, ro->action, ro->old_logp,
-                             ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
-                             xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), step_loss, stream);
-      if (rc) return rc;
-      return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, true, 0u, 0u, g_comm);
-  });
-}
+// names and capture tags of the exported PPO calls of each action distribution
+template <class DIST> struct PpoCalls;
+template <> struct PpoCalls<Categorical> {
+  static constexpr const char *train = "xtb_ppo_train", *infer = "xtb_ppo_rollout_infer", *predict = "xtb_actor_predict_host";
+  static constexpr GraphTag train_tag = kPpoTrain, infer_tag = kRolloutInfer;
+};
+template <> struct PpoCalls<DiagGaussian> {
+  static constexpr const char *train = "xtb_ppo_gauss_train", *infer = "xtb_ppo_gauss_rollout_infer",
+                              *predict = "xtb_ppo_gauss_predict_host";
+  static constexpr GraphTag train_tag = kPpoGaussTrain, infer_tag = kGaussRolloutInfer;
+};
 
-// The Gaussian policy: under the fused-heads conditions of xtb_ppo_train one heads_kernel<PpoGaussLoss> launch per
-// minibatch (the log_std gradient is A more slab floats, reduced in block order into its slot); otherwise layer by
-// layer: forward, xtb_ppo_gauss_loss_grad (the log_std gradient straight into its slot of the zeroed gradient bucket),
-// then the backward pass of the network, which keeps that slot.
-static int ppo_gauss_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int N, int B, int E,
-                                  const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t,
-                                  float* loss_per_step, float inv_world, void* stream) {
+// The epoch x minibatch loop of PPO.train for the action distribution DIST.  Under the fused-heads conditions one
+// heads_kernel<DIST::Loss> launch per minibatch (a DiagGaussian's log_std gradient is A more slab floats, reduced in
+// block order into its slot); otherwise layer by layer: forward, the loss kernel (a DiagGaussian's log_std gradient
+// straight into its slot of the zeroed gradient bucket), then the backward pass of the network, which keeps that slot.
+template <class DIST, class RO>
+static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, int B, int E, const int32_t* perm,
+                            const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, float inv_world,
+                            void* stream) {
   int heads[2] = {pi_t, v_t};
   const int adim = net->tsize[pi_t];
-  const long long ls_off = net->L[ls_t - 1].w_off;
+  const long long ls_off = DIST::kLogStd ? net->L[ls_t - 1].w_off : -1;
   const LayerPlan& lpi = net->L[pi_t - 1];
   const LayerPlan& lv = net->L[v_t - 1];
-  const bool fuse = ppo_heads_fusable(net, pi_t, v_t);
+  const bool fuse = ppo_heads_fusable(net, pi_t, v_t, false);
   const unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
   return ppo_epoch_loop(net, opt, N, B, E, perm, loss_per_step, stream, [&](const int32_t* idx, int mb, float* step_loss) -> int {
+    // fp32 row-major copies: the hidden tensors the fused heads read, or the head outputs the loss kernel reads
     const unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
     int rc = net_forward_impl(net, nullptr, ro->obs, idx, mb, stream, skip, want);
     if (rc) return rc;
     if (fuse) {
       PpoHeadsArgs a;
       memset(&a, 0, sizeof a);
-      a.idx = idx; a.action_f = ro->action; a.log_std = net->params + ls_off; a.old_logp = ro->old_logp; a.adv = ro->adv;
-      a.old_v = ro->old_v; a.target_v = ro->target_v;
+      a.idx = idx; a.old_logp = ro->old_logp; a.adv = ro->adv; a.old_v = ro->old_v; a.target_v = ro->target_v;
+      if constexpr (DIST::kLogStd) { a.action_f = ro->action; a.log_std = net->params + ls_off; }
+      else a.action = ro->action;
+      a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
       a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
-      return ppo_heads_fused<PpoGaussLoss>(net, ro->obs, a, mb, pi_t, v_t, skip, ls_off, step_loss, stream);
+      return heads_fused<typename DIST::Loss>(net, ro->obs, a, mb, pi_t, v_t, skip, ls_off, step_loss, stream);
     }
-    CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
-    rc = xtb_ppo_gauss_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), net->params + ls_off, idx, ro->action,
-                                 ro->old_logp, ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
-                                 xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), net->grads + ls_off, step_loss,
-                                 stream);
+    if constexpr (DIST::kLogStd) {
+      CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
+      rc = xtb_ppo_gauss_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), net->params + ls_off, idx, ro->action,
+                                   ro->old_logp, ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
+                                   xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), net->grads + ls_off, step_loss,
+                                   stream);
+    } else {
+      rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, ro->action, ro->old_logp, ro->adv,
+                             ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb, xtb_net_tensor_grad(net, pi_t),
+                             xtb_net_tensor_grad(net, v_t), step_loss, stream);
+    }
     if (rc) return rc;
-    return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, false, 0u, 0u, g_comm);
+    return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, !DIST::kLogStd, 0u, 0u, g_comm);
   });
 }
 
-// head tensors of the Gaussian entry points: mean (pi_t), value (v_t, 1 wide) and the logstd layer's tensor (ls_t) of
-// the same width as the mean
-static int gauss_heads_check(const char* fn, const xtb_net* net, int pi_t, int v_t, int ls_t) {
+// head tensors of the PPO entry points: pi_t (logits / mean, at most MAX_ADIM wide), v_t (value, 1 wide) and, for a
+// distribution with log_std, the logstd layer's tensor ls_t of the mean's width
+template <class DIST>
+static int ppo_heads_check(const char* fn, const xtb_net* net, int pi_t, int v_t, int ls_t) {
   const int nl = (int)net->L.size();
-  if (pi_t < 1 || pi_t > nl || v_t < 1 || v_t > nl || ls_t < 1 || ls_t > nl || net->tsize[v_t] != 1)
+  if (pi_t < 1 || pi_t > nl || v_t < 1 || v_t > nl || net->tsize[v_t] != 1 || net->tsize[pi_t] > MAX_ADIM ||
+      (DIST::kLogStd && (ls_t < 1 || ls_t > nl)))
     return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
+  if (!DIST::kLogStd) return XTB_OK;
   const LayerPlan& ls = net->L[ls_t - 1];
   if (ls.d.kind != XTB_LOGSTD || ls.N != net->tsize[pi_t]) return fail(XTB_ERR_ARG, "%s: tensor %d is not a logstd layer of the mean's width", fn, ls_t);
   return XTB_OK;
 }
 
+template <class DIST, class RO>
+static int ppo_train(xtb_net* net, xtb_adam* opt, const RO* ro, int n_sample, int batch_size, int n_epoch, const int32_t* perm,
+                     const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, int use_graph, void* stream) {
+  const char* fn = PpoCalls<DIST>::train;
+  if (!net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v || !perm || !hp ||
+      !loss_per_step)
+    return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
+  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "%s: optimiser/net size mismatch", fn);
+  if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
+  if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
+  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
+  const float inv_world = ppo_inv_world();
+  return run_graph(capture_key(PpoCalls<DIST>::train_tag, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
+                               loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
+                               hp->critic_coef, pi_t, v_t, ls_t),
+                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
+    return ppo_train_launch<DIST>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_t, v_t, ls_t, loss_per_step, inv_world, st);
+  });
+}
+
 extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample,
                              int batch_size, int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp,
                              int pi_tensor, int v_tensor, float* loss_per_step, int use_graph, void* stream) {
-  if (!net || !opt || !ro || !perm || !hp || !loss_per_step) return fail(XTB_ERR_ARG, "xtb_ppo_train: null pointer");
-  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_ppo_train: net not bound");
-  if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_train: bad sizes");
-  if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
-  int nl = (int)net->L.size();
-  if (pi_tensor < 1 || pi_tensor > nl || v_tensor < 1 || v_tensor > nl || net->tsize[v_tensor] != 1)
-    return fail(XTB_ERR_ARG, "xtb_ppo_train: bad head tensors");
-  const float inv_world = ppo_inv_world();
-  return run_graph(capture_key(kPpoTrain, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v,
-                               perm, loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
-                               hp->critic_coef, pi_tensor, v_tensor),
-                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
-    return ppo_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, loss_per_step, inv_world, st);
-  });
+  return ppo_train<Categorical>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, 0, loss_per_step,
+                                use_graph, stream);
 }
 
 extern "C" int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int n_sample, int batch_size,
                                    int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor,
                                    int logstd_tensor, float* loss_per_step, int use_graph, void* stream) {
-  if (!net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v || !perm || !hp ||
-      !loss_per_step)
-    return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: null pointer");
-  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_ppo_gauss_train: net not bound");
-  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: optimiser/net size mismatch");
-  if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_train: bad sizes");
-  if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
-  if (int rc = gauss_heads_check("xtb_ppo_gauss_train", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
-  const float inv_world = ppo_inv_world();
-  return run_graph(capture_key(kPpoGaussTrain, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v,
-                               ro->target_v, perm, loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef,
-                               hp->vf_clip, hp->critic_coef, pi_tensor, v_tensor, logstd_tensor),
-                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
-    return ppo_gauss_train_launch(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, logstd_tensor,
-                                  loss_per_step, inv_world, st);
-  });
+  return ppo_train<DiagGaussian>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, logstd_tensor,
+                                 loss_per_step, use_graph, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2241,55 +2242,22 @@ static bool dueling_fusable(const xtb_net* net, int q_tensor) {
          lv.d.src == la.d.src && heads_fit(lv.K, lv.N) && !act_is_ext(lv.src_act);
 }
 
-// The online half of the dueling TD step in one heads_kernel launch: both streams' forward, the combine, TD target and
-// loss, the streams' backward and the gradient wrt the hidden tensor (straight into its planes when its layer runs on
-// the tensor cores); then the backward pass of the layers below, with the slab reductions queued like ppo_train_launch's.
+// The online half of the dueling TD step in one heads_kernel launch (heads_fused with the value stream as the pi head
+// and the adv stream as the value head): both streams' forward, the combine, TD target and loss, the streams' backward
+// and the gradient wrt the hidden tensor; then the backward pass of the layers below.
 static int dueling_td_fused(xtb_net* net, const void* obs, const int32_t* idx, const int32_t* action, const float* reward,
                             const uint8_t* done, const float* disc, int n, float gamma, float huber, int q_tensor,
                             const float* qn_t, const float* qn_o, float inv_count, float* loss_out, cudaStream_t st) {
   const LayerPlan& lq = net->L[q_tensor - 1];
-  const LayerPlan& lv = net->L[lq.d.src - 1];
-  const LayerPlan& la = net->L[lq.d.k - 1];
-  const int h = lv.d.src, K = lv.K, A = lv.N;
+  const int h = net->L[lq.d.src - 1].d.src;
   const unsigned skip = (1u << (q_tensor - 1)) | (1u << (lq.d.src - 1)) | (1u << (lq.d.k - 1));
   int rc = net_forward_impl(net, nullptr, obs, idx, n, st, skip, 1u << h);
   if (rc) return rc;
-  CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), st));
-  net->pending.clear();
   PpoHeadsArgs a;
   memset(&a, 0, sizeof a);
-  a.h_pi = a.h_v = (const float*)(net->ws + net->out_off[h]);
-  a.g_pi = a.g_v = (float*)(net->ws + net->gout_off[h]);
-  const bool bp = use_tc(net->L[h - 1]) && net->plane_elems[h] > 0;
-  a.gp_hi = a.gv_hi = bp ? gout_bp(net, h).hi : nullptr; a.gp_lo = a.gv_lo = net->plane_elems[h];
-  a.pitch = net->pitch;
-  a.w_pi = net->params + lv.w_off; a.b_pi = net->params + lv.b_off; a.w_v = net->params + la.w_off; a.b_v = net->params + la.b_off;
-  bool bh_ok = net->L[h - 1].d.kind == XTB_DENSE;   // the hidden layer's bias gradient, when h feeds nothing but the streams
-  for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], h) && !(skip & (1u << j))) bh_ok = false;
   a.idx = idx; a.action = action; a.reward = reward; a.done = done; a.disc = disc; a.qn_t = qn_t; a.qn_o = qn_o; a.loss_in = loss_out;
-  a.B = n; a.K = K; a.A = A; a.act_pi = a.act_v = lv.src_act; a.shared = 1;
   a.gamma = gamma; a.huber = huber; a.inv_count = inv_count;
-  const int blocks = std::max(1, std::min(kSMs, (n + 7) / 8));
-  const int nacc = K * A + 3 * K + A + 2;
-  a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
-  { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
-  launch_heads<DuelingTdLoss>(a, blocks, (size_t)8 * nacc * sizeof(float), st);
-  LAUNCH_CHECK();
-  auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
-    bp::RedSeg r;
-    memset(&r, 0, sizeof r);
-    r.part = a.part + off; r.n_slabs = blocks; r.slab = a.slab; r.count = count; r.kind = 1;
-    r.dst_off = dst_off; r.alpha = 1.f; r.dst_ptr = dst_ptr;
-    net->pending.push_back(r);
-  };
-  seg(0, K * A, lv.w_off, nullptr);
-  seg(K * A, K, la.w_off, nullptr);
-  if (bh_ok) seg(K * A + K, K, net->L[h - 1].b_off, nullptr);
-  seg(K * A + 3 * K, A, lv.b_off, nullptr);
-  seg(K * A + 3 * K + A, 1, la.b_off, nullptr);
-  seg(K * A + 3 * K + A + 1, 1, 0, loss_out);
-  int heads[1] = {h};
-  return net_backward_impl(net, obs, idx, n, heads, 1, st, skip, false, bh_ok ? (1u << h) : 0u, bp ? (1u << h) : 0u, g_comm);
+  return heads_fused<DuelingTdLoss>(net, obs, a, n, lq.d.src, lq.d.k, skip, -1, loss_out, st);
 }
 
 // DQN.train (xt/algorithm/dqn/dqn.py:61-103) on a device replay ring: rows idx[0..n) of (obs, next_obs, action, reward,
@@ -2343,33 +2311,40 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
 // ------------------------------------------------------------------------------------------
 // rollout inference: T batched policy evaluations over the E stacked observations
 // ------------------------------------------------------------------------------------------
-static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* step_idx, int E, int T, int pi_t, int v_t,
-                                uint64_t seed, unsigned long long* offset_dev, int32_t* action, float* logp, float* value,
-                                void* stream) {
-  int adim = net->tsize[pi_t];
+// T policy evaluations of the action distribution DIST: per step the forward of the layers below the heads and
+// infer_heads_kernel (both heads and the draw) within the fused-inference limits, otherwise every layer and then the
+// sampling kernel; the draws are the same either way.  step_idx NULL: step t reads observation rows t*E .. (t+1)*E - 1.
+template <class DIST>
+static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* step_idx, int E, int T, int pi_t, int v_t, int ls_t,
+                                uint64_t seed, unsigned long long* offset_dev, typename DIST::Action* action, float* logp,
+                                float* value, void* stream) {
+  const int adim = net->tsize[pi_t];
+  const float* log_std = DIST::kLogStd ? net->params + net->L[ls_t - 1].w_off : nullptr;
   const LayerPlan& lpi = net->L[pi_t - 1];
   const LayerPlan& lv = net->L[v_t - 1];
-  int kpl = lpi.K / 32;
-  bool fuse = g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
-              lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && lpi.K % 32 == 0 && adim <= 8 && kpl <= 16;
-  unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
+  const bool fuse = ppo_heads_fusable(net, pi_t, v_t, true);
+  const unsigned skip = fuse ? ((1u << (pi_t - 1)) | (1u << (v_t - 1))) : 0u;
+  const unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
+  const size_t row_bytes = (size_t)net->tsize[0] * (net->desc.input_u8 ? 1 : sizeof(float));
+  float* pi_out = xtb_net_tensor(net, pi_t);
+  const float* v_in = xtb_net_tensor(net, v_t);
   for (int t = 0; t < T; t++) {
-    unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_t) | (1u << v_t));
-    int rc = net_forward_impl(net, nullptr, obs, step_idx ? step_idx + (long long)t * E : nullptr, E, stream, skip, want);
+    const void* obs_t = step_idx ? obs : (const void*)((const char*)obs + (size_t)t * E * row_bytes);
+    int rc = net_forward_impl(net, nullptr, obs_t, step_idx ? step_idx + (long long)t * E : nullptr, E, stream, skip, want);
     if (rc) return rc;
-    int32_t* a_t = action + (long long)t * E; float* lp_t = logp + (long long)t * E; float* v_o = value + (long long)t * E;
+    typename DIST::Action* a_t = action + (long long)t * E * DIST::action_width(adim);
+    float* lp_t = logp + (long long)t * E; float* v_o = value + (long long)t * E;
     if (fuse) {
-      const float* hp = (const float*)(net->ws + net->out_off[lpi.d.src]);
-      const float* hv = (const float*)(net->ws + net->out_off[lv.d.src]);
-      const float *wp = net->params + lpi.w_off, *bp = net->params + lpi.b_off, *wv = net->params + lv.w_off, *bv = net->params + lv.b_off;
-      int blocks = std::max(1, std::min(kSMs, (E + 7) / 8));
-      if (kpl <= 2) XLAUNCH((ppo_infer_heads_kernel<2, 8>), blocks, 256, 0, S(stream), hp, hv, wp, bp, wv, bv, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, xtb_net_tensor(net, pi_t));
-      else if (kpl <= 8 && adim <= 4) XLAUNCH((ppo_infer_heads_kernel<8, 4>), blocks, 256, 0, S(stream), hp, hv, wp, bp, wv, bv, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, xtb_net_tensor(net, pi_t));
-      else if (kpl <= 8) XLAUNCH((ppo_infer_heads_kernel<8, 8>), blocks, 256, 0, S(stream), hp, hv, wp, bp, wv, bv, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, xtb_net_tensor(net, pi_t));
-      else XLAUNCH((ppo_infer_heads_kernel<16, 8>), blocks, 256, 0, S(stream), hp, hv, wp, bp, wv, bv, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, xtb_net_tensor(net, pi_t));
+      launch_infer_heads<DIST>(lpi.K, adim, std::max(1, std::min(kSMs, (E + 7) / 8)), S(stream),
+                               (const float*)(net->ws + net->out_off[lpi.d.src]), (const float*)(net->ws + net->out_off[lv.d.src]),
+                               net->params + lpi.w_off, net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off,
+                               log_std, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, pi_out);
+    } else if constexpr (DIST::kLogStd) {
+      XLAUNCH(gauss_sample_kernel, (E + 127) / 128, 128, 0, S(stream), pi_out, log_std, E, adim, (const float*)nullptr, seed,
+              (uint64_t)0, offset_dev, t, a_t, lp_t, v_in, v_o);
     } else {
-      XLAUNCH(sample_rollout_kernel, (E + 127) / 128, 128, 0, S(stream), xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), E, adim, seed,
-                                                                   offset_dev, t, a_t, lp_t, v_o);
+      XLAUNCH(sample_kernel, (E + 127) / 128, 128, 0, S(stream), pi_out, E, adim, (const float*)nullptr, seed, (uint64_t)0,
+              offset_dev, t, a_t, lp_t, v_in, v_o);
     }
     LAUNCH_CHECK();
   }
@@ -2378,72 +2353,34 @@ static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* st
   return XTB_OK;
 }
 
-extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
-                                     int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                                     int32_t* action, float* logp, float* value, int use_graph, void* stream) {
-  if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "xtb_ppo_rollout_infer: null pointer");
-  int nl = (int)net->L.size();
-  if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_rollout_infer: bad sizes");
-  if (pi_tensor < 1 || pi_tensor > nl || v_tensor < 1 || v_tensor > nl || net->tsize[v_tensor] != 1 || net->tsize[pi_tensor] > MAX_ADIM)
-    return fail(XTB_ERR_ARG, "xtb_ppo_rollout_infer: bad head tensors");
-  return run_graph(capture_key(kRolloutInfer, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value, n_env, n_step,
-                               pi_tensor, v_tensor, seed),
+template <class DIST>
+static int ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step, int pi_t, int v_t,
+                             int ls_t, uint64_t seed, unsigned long long* offset_dev, typename DIST::Action* action, float* logp,
+                             float* value, int use_graph, void* stream) {
+  const char* fn = PpoCalls<DIST>::infer;
+  if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
+  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
+  return run_graph(capture_key(PpoCalls<DIST>::infer_tag, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value,
+                               n_env, n_step, pi_t, v_t, ls_t, seed),
                    use_graph, stream, [&](void* st) {
-    return rollout_infer_launch(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, seed, offset_dev, action, logp, value, st);
+    return rollout_infer_launch<DIST>(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev, action, logp, value, st);
   });
 }
 
-// Gaussian actor: per step the forward of the layers below the heads and gauss_infer_heads_kernel (both heads and the
-// sample) within the fused-inference limits of xtb_ppo_rollout_infer; otherwise every layer, then gauss_sample_kernel
+extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
+                                     int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
+                                     int32_t* action, float* logp, float* value, int use_graph, void* stream) {
+  return ppo_rollout_infer<Categorical>(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, 0, seed, offset_dev, action, logp,
+                                        value, use_graph, stream);
+}
+
 extern "C" int xtb_ppo_gauss_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
                                            int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
                                            unsigned long long* offset_dev, float* action, float* logp, float* value, int use_graph,
                                            void* stream) {
-  if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_rollout_infer: null pointer");
-  if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_rollout_infer: bad sizes");
-  if (int rc = gauss_heads_check("xtb_ppo_gauss_rollout_infer", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
-  return run_graph(capture_key(kGaussRolloutInfer, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value, n_env, n_step,
-                               pi_tensor, v_tensor, logstd_tensor, seed),
-                   use_graph, stream, [&](void* st) -> int {
-    const int adim = net->tsize[pi_tensor];
-    const float* log_std = net->params + net->L[logstd_tensor - 1].w_off;
-    const LayerPlan& lpi = net->L[pi_tensor - 1];
-    const LayerPlan& lv = net->L[v_tensor - 1];
-    const int kpl = lpi.K / 32;
-    // the fused-inference limits of rollout_infer_launch: both heads in gauss_infer_heads_kernel
-    const bool fuse = g_fuse_heads && lpi.d.kind == XTB_DENSE && lv.d.kind == XTB_DENSE && lpi.d.act == 0 && lv.d.act == 0 &&
-                      lpi.d.src != 0 && lv.d.src != 0 && lpi.K == lv.K && lpi.K % 32 == 0 && adim <= 8 && kpl <= 16;
-    const unsigned skip = fuse ? ((1u << (pi_tensor - 1)) | (1u << (v_tensor - 1))) : 0u;
-    const unsigned want = fuse ? ((1u << lpi.d.src) | (1u << lv.d.src)) : ((1u << pi_tensor) | (1u << v_tensor));
-    // step_idx NULL: step t reads observation rows t*n_env .. (t+1)*n_env - 1
-    const size_t row_bytes = (size_t)net->tsize[0] * (net->desc.input_u8 ? 1 : sizeof(float));
-    for (int t = 0; t < n_step; t++) {
-      const void* obs_t = step_idx ? obs : (const void*)((const char*)obs + (size_t)t * n_env * row_bytes);
-      int rc = net_forward_impl(net, nullptr, obs_t, step_idx ? step_idx + (long long)t * n_env : nullptr, n_env, st, skip, want);
-      if (rc) return rc;
-      float* a_t = action + (long long)t * n_env * adim; float* lp_t = logp + (long long)t * n_env; float* v_o = value + (long long)t * n_env;
-      if (fuse) {
-        const float* hp = (const float*)(net->ws + net->out_off[lpi.d.src]);
-        const float* hv = (const float*)(net->ws + net->out_off[lv.d.src]);
-        const float *wp = net->params + lpi.w_off, *bp = net->params + lpi.b_off, *wv = net->params + lv.w_off, *bv = net->params + lv.b_off;
-        const int blocks = std::max(1, std::min(kSMs, (n_env + 7) / 8));
-        const unsigned long long* od = offset_dev;
-        float* mean_out = xtb_net_tensor(net, pi_tensor);
-        if (kpl <= 2) XLAUNCH((gauss_infer_heads_kernel<2, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
-        else if (kpl <= 8 && adim <= 4) XLAUNCH((gauss_infer_heads_kernel<8, 4>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
-        else if (kpl <= 8) XLAUNCH((gauss_infer_heads_kernel<8, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
-        else XLAUNCH((gauss_infer_heads_kernel<16, 8>), blocks, 256, 0, S(st), hp, hv, wp, bp, wv, bv, log_std, n_env, lpi.K, adim, seed, od, t, a_t, lp_t, v_o, mean_out);
-      } else {
-        XLAUNCH(gauss_sample_kernel, (n_env + 127) / 128, 128, 0, S(st), (const float*)xtb_net_tensor(net, pi_tensor), log_std, n_env,
-                adim, (const float*)nullptr, seed, (uint64_t)0, (const unsigned long long*)offset_dev, t, a_t, lp_t,
-                (const float*)xtb_net_tensor(net, v_tensor), v_o);
-      }
-      LAUNCH_CHECK();
-    }
-    XLAUNCH(bump_counter_kernel, 1, 1, 0, S(st), offset_dev, n_step);
-    LAUNCH_CHECK();
-    return XTB_OK;
-  });
+  return ppo_rollout_infer<DiagGaussian>(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, logstd_tensor, seed, offset_dev,
+                                         action, logp, value, use_graph, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2465,25 +2402,36 @@ extern "C" int xtb_copy_h2d_staged(void* dst, const void* src, size_t bytes, voi
   return XTB_OK;
 }
 // PPO.predict with host buffers in one call (xt/model/ppo/ppo.py:104-109): staged H2D of the observations, the
-// (graphed) forward + sampling, one packed D2H of [action | logp | value] and a stream synchronise.
-extern "C" int xtb_actor_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                                      int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                                      float* out_dev, float* out_host, float* logits_host, int use_graph, void* stream) {
-  if (!net || !obs_host || !obs_dev || !out_dev || !out_host) return fail(XTB_ERR_ARG, "xtb_actor_predict_host: null pointer");
+// (graphed) rollout inference of one step into the packed block out_dev = [action | logp | value], one D2H of it (and
+// of the pi head's output into head_host when set) and a stream synchronise.
+template <class DIST>
+static int ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env, int pi_t, int v_t,
+                            int ls_t, uint64_t seed, unsigned long long* offset_dev, float* out_dev, float* out_host,
+                            float* head_host, int use_graph, void* stream) {
+  const char* fn = PpoCalls<DIST>::predict;
+  if (!net || !obs_host || !obs_dev || !out_dev || !out_host) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
+  const size_t aw = DIST::action_width(net->tsize[pi_t]);
   StreamScope sc;
   int src = sc.begin(stream, use_graph != 0);
   if (src) return src;
-  void* st = (void*)sc.st;
   CUDA_TRY(xtb::Stager::instance().stage_h2d(obs_dev, obs_host, obs_bytes, sc.st));
-  int rc = xtb_ppo_rollout_infer(net, obs_dev, nullptr, n_env, 1, pi_tensor, v_tensor, seed, offset_dev,
-                                 reinterpret_cast<int32_t*>(out_dev), out_dev + n_env, out_dev + 2 * (size_t)n_env, use_graph, st);
+  int rc = ppo_rollout_infer<DIST>(net, obs_dev, nullptr, n_env, 1, pi_t, v_t, ls_t, seed, offset_dev,
+                                   reinterpret_cast<typename DIST::Action*>(out_dev), out_dev + aw * n_env,
+                                   out_dev + (aw + 1) * n_env, use_graph, (void*)sc.st);
   if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(out_host, out_dev, sizeof(float) * 3 * (size_t)n_env, cudaMemcpyDeviceToHost, sc.st));
-  if (logits_host)
-    CUDA_TRY(cudaMemcpyAsync(logits_host, xtb_net_tensor(net, pi_tensor), sizeof(float) * (size_t)n_env * net->tsize[pi_tensor],
+  CUDA_TRY(cudaMemcpyAsync(out_host, out_dev, sizeof(float) * (aw + 2) * (size_t)n_env, cudaMemcpyDeviceToHost, sc.st));
+  if (head_host)
+    CUDA_TRY(cudaMemcpyAsync(head_host, xtb_net_tensor(net, pi_t), sizeof(float) * (size_t)n_env * net->tsize[pi_t],
                              cudaMemcpyDeviceToHost, sc.st));
   CUDA_TRY(cudaStreamSynchronize(sc.st));
   return sc.end();
+}
+extern "C" int xtb_actor_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
+                                      int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
+                                      float* out_dev, float* out_host, float* logits_host, int use_graph, void* stream) {
+  return ppo_predict_host<Categorical>(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, 0, seed, offset_dev, out_dev,
+                                       out_host, logits_host, use_graph, stream);
 }
 extern "C" int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
                                     int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
@@ -2495,19 +2443,8 @@ extern "C" int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, si
                                           int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
                                           unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
                                           void* stream) {
-  if (!net || !obs_host || !obs_dev || !out_dev || !out_host) return fail(XTB_ERR_ARG, "xtb_ppo_gauss_predict_host: null pointer");
-  if (int rc = gauss_heads_check("xtb_ppo_gauss_predict_host", net, pi_tensor, v_tensor, logstd_tensor)) return rc;
-  const size_t adim = (size_t)net->tsize[pi_tensor];
-  StreamScope sc;
-  int src = sc.begin(stream, use_graph != 0);
-  if (src) return src;
-  CUDA_TRY(xtb::Stager::instance().stage_h2d(obs_dev, obs_host, obs_bytes, sc.st));
-  int rc = xtb_ppo_gauss_rollout_infer(net, obs_dev, nullptr, n_env, 1, pi_tensor, v_tensor, logstd_tensor, seed, offset_dev, out_dev,
-                                       out_dev + adim * n_env, out_dev + (adim + 1) * n_env, use_graph, (void*)sc.st);
-  if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(out_host, out_dev, sizeof(float) * (adim + 2) * (size_t)n_env, cudaMemcpyDeviceToHost, sc.st));
-  CUDA_TRY(cudaStreamSynchronize(sc.st));
-  return sc.end();
+  return ppo_predict_host<DiagGaussian>(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, logstd_tensor, seed,
+                                        offset_dev, out_dev, out_host, nullptr, use_graph, stream);
 }
 extern "C" int xtb_copy_d2h(void* dst, const void* src, size_t bytes, void* stream) {
   CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S(stream)));
