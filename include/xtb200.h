@@ -87,7 +87,9 @@ typedef struct xtb_layer_desc {
 } xtb_layer_desc;
 
 typedef struct xtb_net_desc {
-  int32_t input_u8;        /* 1: uint8 observation decoded as x*scale (model_utils.py:187-189) */
+  int32_t input_u8;        /* 1: uint8 observation decoded as x*scale (model_utils.py:187-189); 2: int8 observation (each
+                              byte b read as b < 128 ? b : b - 256, then times scale: uint8 frames fed to the int8
+                              placeholder of MuzeroCnn with obs_type int8); 0: float; other values XTB_ERR_ARG */
   float scale;             /* 1/255 for uint8 Atari frames, 1 for float observations */
   int32_t in_h, in_w, in_c; /* observation HWC; vectors use 1,1,dim */
   int32_t n_layers;
@@ -132,6 +134,7 @@ int xtb_net_layer_plan(const xtb_net* net, int layer, xtb_layer_plan* out);
 int xtb_net_tensor_size(const xtb_net* net, int t);
 size_t xtb_net_workspace_bytes(const xtb_net* net);
 /* params/grads: [param_count] floats; workspace: xtb_net_workspace_bytes() bytes */
+/* A net with tensor-core layers needs `params` 16-byte aligned (XTB_ERR_ARG otherwise). */
 int xtb_net_bind(xtb_net* net, float* params, float* grads, void* workspace, size_t workspace_bytes);
 /* same, with the initialisation work (workspace clear, weight blobs) ordered on `stream`; returns after it completed */
 int xtb_net_bind_stream(xtb_net* net, float* params, float* grads, void* workspace, size_t workspace_bytes, void* stream);
@@ -416,6 +419,68 @@ int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, size_t obs_by
                                int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
                                unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
                                void* stream);
+
+/* ---- MuZero: replaces MuzeroModel's train / inference graphs (xt/model/muzero/muzero_model.py:74-239) ----------------
+ * The model is three nets: representation (obs -> hidden h, H wide), dynamics (concat(h, one_hot(a)) -> next hidden and
+ * reward logits) and prediction (h -> policy logits, value logits).  Their softmax outputs are evaluated by the kernels,
+ * so the policy, value and reward heads are linear dense layers.  The three nets are bound to slices [rep | dyn | pred],
+ * in this order, of one parameter buffer (MuzeroBase's Keras weight-list order; gaps between the slices are allowed, e.g.
+ * to keep each slice 16-byte aligned as xtb_net_bind requires of a net with tensor-core layers), and to the slices at
+ * the same offsets of one gradient buffer; the optimiser spans the buffer from the first slice to the last.  The
+ * dynamics net is bound to its parameter slice and to a gradient buffer of its own OUTSIDE the shared one, which every
+ * application of it fills before it is added to its slice in a fixed order.  The dynamics and prediction nets read float
+ * observations (decode scale 1) with dense layers only.
+ *   h(x) = sign(x)(sqrt(|x| + 1) - 1) + 0.001 x   (value_compression, muzero_utils.py:38-40)
+ *   two-hot target of a scalar x (conver_value, muzero_model.py:200-216): v = h(clip(x, min, max) - min) in float64,
+ *     1 - frac(v) at floor(v), frac(v) at floor(v) + 1
+ *   scalar of a support (value_transform, :218-226): clip(h^-1(sum_j softmax_j j) + min, min, max), h^-1 in closed form
+ * Supports and the action count are at most 1024 wide. */
+typedef struct xtb_muzero xtb_muzero;
+typedef struct xtb_muzero_desc {
+  int32_t unroll;                 /* K (td_step) */
+  int32_t rep_h;                  /* representation net: hidden-state tensor (relu / tanh / linear), H wide */
+  int32_t dyn_h, dyn_r;           /* dynamics net: next hidden state (H wide, relu / tanh / linear) and reward logits */
+  int32_t pred_p, pred_v;         /* prediction net: policy logits (A wide) and value logits */
+  float value_min, value_max;     /* value support range */
+  float reward_min, reward_max;   /* reward support range */
+} xtb_muzero_desc;
+/* Checks the nets and their binding and allocates the step's device scratch for up to max_batch samples (the prediction
+ * net must hold (unroll + 1) * max_batch rows).  The nets must outlive the object and stay bound as they were. */
+int xtb_muzero_create(xtb_net* rep, xtb_net* dyn, xtb_net* pred, const xtb_muzero_desc* desc, int max_batch, xtb_muzero** out);
+void xtb_muzero_destroy(xtb_muzero* mz);
+/* One training batch of B samples (device arrays). */
+typedef struct xtb_muzero_batch {
+  const void* obs;              /* [B, ...] observations of the representation net */
+  const int32_t* action;        /* [B, unroll] */
+  const float* target_value;    /* [B, unroll + 1] scalars */
+  const float* target_reward;   /* [B, unroll + 1] scalars (column `unroll` is not used) */
+  const float* target_policy;   /* [B, unroll + 1, A] */
+  int32_t unroll;               /* must equal the model's */
+} xtb_muzero_batch;
+/* MuzeroModel.train (muzero_model.py:103-140, 154-169) as one step: h_0 = rep(obs); for k < K h_{k+1}, r_k =
+ * dyn(concat(h_k, one_hot(a_k))); policy/value of h_0..h_K as one prediction pass over (K+1) B rows;
+ *   loss = CE(p_0, pi_0) + CE(v_0, z_0) + sum_{k<K} [CE(r_k, u_k) + CE(p_{k+1}, pi_{k+1}) + CE(v_{k+1}, z_{k+1})]
+ *   CE(p, t) = mean_b mean_j -t_j log(p_j + 1e-10)   (p = softmax of the logits)
+ * the gradient of every term under the sum scaled by 1/K, the gradient reaching h_{k+1} (k+1 < K) from dynamics step k+1
+ * scaled by 0.5 (h_0 unscaled); backward (dynamics recomputed step by step); one Adam step of `opt` (created over the
+ * whole buffer, no clipping) and the weight refresh of the three nets.  *loss_out = loss_offset + loss, its terms summed
+ * in a fixed order.  value_out != NULL: [B] the value of every observation after the update (value_inference).
+ * XTB_ERR_STATE, launching nothing, while a gradient hook or communicator is installed. */
+int xtb_muzero_train(xtb_muzero* mz, xtb_adam* opt, const xtb_muzero_batch* batch_in, int batch, float loss_offset,
+                     float* loss_out, float* value_out, int use_graph, void* stream);
+/* initial_inference / value_inference (muzero_model.py:74-82, 228-239) over `batch` observations: hidden [B, H],
+ * value [B] scalars, policy [B, A] probabilities; any output may be NULL. */
+int xtb_muzero_initial_inference(xtb_muzero* mz, const void* obs, int batch, float* hidden_out, float* value_out,
+                                 float* policy_out, int use_graph, void* stream);
+/* recurrent_inference (muzero_model.py:84-96) over `batch` hidden states [B, H] and actions [B]: next hidden [B, H],
+ * reward [B] and value [B] scalars, policy [B, A] probabilities; any output may be NULL. */
+int xtb_muzero_recurrent_inference(xtb_muzero* mz, const float* hidden, const int32_t* action, int batch, float* hidden_out,
+                                   float* reward_out, float* value_out, float* policy_out, int use_graph, void* stream);
+/* xtb_net_backward that also writes d loss / d observation [batch, obs width] into dobs (overwritten): the data-gradient
+ * GEMM of every dense layer that reads the observation, summed in layer order.  Float observations with scale 1 read
+ * by dense layers only; otherwise XTB_ERR_ARG. */
+int xtb_net_backward_input(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
+                           const int32_t* head_tensors, int n_heads, float* dobs, void* stream);
 
 /* Data-parallel hook (SURVEY 8(e)): called between backward and the optimiser with the flat
  * gradient bucket; must SUM it over ranks on `stream` (e.g. ncclAllReduce).  Called once with

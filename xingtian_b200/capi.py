@@ -53,6 +53,17 @@ class ImpalaTraj(C.Structure):
                 ("done", C.c_void_p)]
 
 
+class MuzeroDesc(C.Structure):
+    _fields_ = [("unroll", C.c_int32), ("rep_h", C.c_int32), ("dyn_h", C.c_int32), ("dyn_r", C.c_int32), ("pred_p", C.c_int32),
+                ("pred_v", C.c_int32), ("value_min", C.c_float), ("value_max", C.c_float), ("reward_min", C.c_float),
+                ("reward_max", C.c_float)]
+
+
+class MuzeroBatch(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("target_value", C.c_void_p), ("target_reward", C.c_void_p),
+                ("target_policy", C.c_void_p), ("unroll", C.c_int32)]
+
+
 _P = C.c_void_p
 GRAD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
 _SIGS = {
@@ -121,6 +132,12 @@ _SIGS = {
                                               _P, C.c_int, _P]),
     "xtb_ppo_gauss_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P,
                                              _P, C.c_int, _P]),
+    "xtb_muzero_create": (C.c_int, [_P, _P, _P, C.POINTER(MuzeroDesc), C.c_int, C.POINTER(_P)]),
+    "xtb_muzero_destroy": (None, [_P]),
+    "xtb_muzero_train": (C.c_int, [_P, _P, C.POINTER(MuzeroBatch), C.c_int, C.c_float, _P, _P, C.c_int, _P]),
+    "xtb_muzero_initial_inference": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P]),
+    "xtb_muzero_recurrent_inference": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
     "xtb_set_grad_hook": (C.c_int, [GRAD_HOOK, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

@@ -1170,7 +1170,8 @@ __global__ void bp_wprep_kernel(const float* __restrict__ params, const BlobSeg*
   *reinterpret_cast<uint4*>(o + lo_off) = l;
 }
 
-// uint8 frames [n][H][W][4] (+ minibatch gather) -> batch-planar space-to-depth plane (exact in bf16, hi only):
+// uint8 frames [n][H][W][4] (+ minibatch gather) -> batch-planar space-to-depth plane (exact in bf16, hi only); with
+// is_signed every byte is read as int8 (two's complement, -128..127, also exact in bf16):
 // the image is embedded at (padT, padL) in a zero canvas of [4*H4][4*W4] pixels, pixel block (Y, X) = 64 features
 // (dy, dx, c); a 16-byte output piece = 8 source bytes (2 pixels x 4 channels).
 // One block = one image row of 32 samples.  Phase 1 reads that row of every sample with 16-byte loads (contiguous
@@ -1180,7 +1181,7 @@ constexpr int DEC_SAMPLES = 32;
 constexpr int DEC_THREADS = 256;
 __global__ void __launch_bounds__(DEC_THREADS)
 bp_decode_s2d_kernel(const uint8_t* __restrict__ obs, const int32_t* __restrict__ idx, int B, int H, int W, int H4, int W4,
-                     int padT, int padL, BpT dst) {
+                     int padT, int padL, int is_signed, BpT dst) {
   // One block = one image row (canvas row Y, sub-row dy) of DEC_SAMPLES samples: 4*H4 x ceil(B/32) blocks, so that the
   // inference batch (B = 32: one sample group) still spreads over 84 blocks.
   extern __shared__ __align__(16) uint8_t dec_sm[];
@@ -1212,10 +1213,14 @@ bp_decode_s2d_kernel(const uint8_t* __restrict__ obs, const int32_t* __restrict_
     uint4 o = make_uint4(0, 0, 0, 0);
     if (lane < ns && u8 >= 0 && u8 < half_units) {
       const uint2 v = *reinterpret_cast<const uint2*>(dec_sm + lane * sstride + u8 * 8);
-      o.x = pack_bf16((float)(v.x & 0xff), (float)((v.x >> 8) & 0xff));
-      o.y = pack_bf16((float)((v.x >> 16) & 0xff), (float)(v.x >> 24));
-      o.z = pack_bf16((float)(v.y & 0xff), (float)((v.y >> 8) & 0xff));
-      o.w = pack_bf16((float)((v.y >> 16) & 0xff), (float)(v.y >> 24));
+      auto byte = [is_signed](uint32_t w, int sh) {
+        const uint32_t u = (w >> sh) & 0xffu;
+        return is_signed ? (float)(int8_t)u : (float)u;
+      };
+      o.x = pack_bf16(byte(v.x, 0), byte(v.x, 8));
+      o.y = pack_bf16(byte(v.x, 16), byte(v.x, 24));
+      o.z = pack_bf16(byte(v.y, 0), byte(v.y, 8));
+      o.w = pack_bf16(byte(v.y, 16), byte(v.y, 24));
     }
     if (lane < ns)
       *reinterpret_cast<uint4*>(dst.hi + ((long long)((Y * W4 + X) * 8 + dy * 2 + dxh) * dst.pitch + b0 + lane) * 8) = o;

@@ -1100,4 +1100,148 @@ __global__ void mse_loss_kernel(const float* __restrict__ q, const float* __rest
   block_atomic_add(lsum, loss_out);
 }
 
+// ------------------------------------------------------------------------------------------
+// MuZero (xt/model/muzero/muzero_model.py, muzero_utils.py): categorical value / reward supports and the unrolled step
+// ------------------------------------------------------------------------------------------
+constexpr int MZ_MAX_SUPPORT = 1024;   // widest support (and action count) the warp-per-row kernels take
+constexpr int MZ_THREADS = 256;        // 8 rows per block
+// h(x) = sign(x) (sqrt(|x| + 1) - 1) + 0.001 x and its closed-form inverse (muzero_utils.py:38-47), in float64 as numpy
+__device__ inline double mz_h(double x) { return (x > 0 ? 1.0 : (x < 0 ? -1.0 : 0.0)) * (sqrt(fabs(x) + 1.0) - 1.0) + 0.001 * x; }
+__device__ inline double mz_h_inv(double x) {
+  const double s = x > 0 ? 1.0 : (x < 0 ? -1.0 : 0.0);
+  const double r = (sqrt(1.0 + 4.0 * 0.001 * (fabs(x) + 1.0 + 0.001)) - 1.0) / (2.0 * 0.001);
+  return s * (r * r - 1.0);
+}
+// warp-wide softmax statistics of one row: max and log of the sum of exp(l - max)
+__device__ inline void warp_softmax_stats(const float* l, int S, int lane, float& mx, float& lz) {
+  mx = -INFINITY;
+  for (int j = lane; j < S; j += 32) mx = fmaxf(mx, l[j]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  float z = 0.f;
+  for (int j = lane; j < S; j += 32) z += expf(l[j] - mx);
+  lz = logf(warp_sum(z));
+}
+
+// conver_value (muzero_model.py:200-216): out row r = i * B + b holds the two-hot projection of x[b * T + i]:
+// v = h(clip(x, min, max) - min), 1 - frac(v) at floor(v) and frac(v) at floor(v) + 1 (dropped past the support).
+__global__ void mz_support_project_kernel(const float* __restrict__ x, int rows, int B, int T, int S, float vmin, float vmax,
+                                          float* __restrict__ out) {
+  pdl_wait(); pdl_trigger();
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const int i = r / B, b = r - i * B;
+  const double v = mz_h(fmin(fmax((double)x[(long long)b * T + i], (double)vmin), (double)vmax) - (double)vmin);
+  const double fl = floor(v);
+  const int idx = (int)fl;
+  const float rest = (float)(v - fl);
+  float* o = out + (long long)r * S;
+  for (int j = lane; j < S; j += 32) o[j] = j == idx ? 1.f - rest : (j == idx + 1 ? rest : 0.f);
+}
+
+// value_transform (muzero_model.py:218-226) of softmax(logits[r]): clip(h_inv(sum_j p_j j) + min, min, max)
+__global__ void mz_support_value_kernel(const float* __restrict__ logits, int rows, int S, float vmin, float vmax,
+                                        float* __restrict__ out) {
+  pdl_wait(); pdl_trigger();
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const float* l = logits + (long long)r * S;
+  float mx, lz;
+  warp_softmax_stats(l, S, lane, mx, lz);
+  double e = 0.0;
+  for (int j = lane; j < S; j += 32) e += (double)expf(l[j] - mx - lz) * j;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+  if (lane == 0) out[r] = (float)fmin(fmax(mz_h_inv(e) + (double)vmin, (double)vmin), (double)vmax);
+}
+
+// cross_entropy (muzero_utils.py:31-34) of p = softmax(logits[r]) against target row t(r), t(r) = r when T == 0, else
+// (r % B) * T + r / B (targets stored sample-major [B, T, S], rows step-major):
+//   l_r = inv_bs * sum_j -t_j log(p_j + 1e-10),   inv_bs = 1 / (B S): the batch mean of the mean over the support
+// dlogits[r] = gradient of g_r l_r through log(p + 1e-10) and the softmax Jacobian, g_r = 1 for r < full_rows and
+// g_rest after (the 1/K gradient scale of the unrolled terms); the value is not scaled.  part[block] = the sum of its
+// rows' l_r, warp by warp in order: with mz_ordered_sum_kernel the loss has no atomics and a fixed summation order.
+__global__ void __launch_bounds__(MZ_THREADS)
+mz_support_ce_kernel(const float* __restrict__ logits, int rows, int S, const float* __restrict__ tgt, int B, int T, int full_rows,
+                     float g_rest, float inv_bs, float* __restrict__ dlogits, float* __restrict__ part) {
+  pdl_wait(); pdl_trigger();
+  __shared__ float red[MZ_THREADS / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.x * (MZ_THREADS / 32) + warp;
+  float lrow = 0.f;
+  if (r < rows) {
+    const float* l = logits + (long long)r * S;
+    const long long tr = T ? (long long)(r % B) * T + r / B : r;
+    const float* t = tgt + tr * S;
+    float mx, lz;
+    warp_softmax_stats(l, S, lane, mx, lz);
+    const float c = (r < full_rows ? 1.f : g_rest) * inv_bs;
+    float f = 0.f, pg = 0.f;
+    for (int j = lane; j < S; j += 32) {
+      const float p = expf(l[j] - mx - lz);
+      f += -t[j] * logf(p + 1e-10f);
+      pg += p * (-c * t[j] / (p + 1e-10f));
+    }
+    f = warp_sum(f); pg = warp_sum(pg);
+    for (int j = lane; j < S; j += 32) {
+      const float p = expf(l[j] - mx - lz);
+      dlogits[(long long)r * S + j] = p * (-c * t[j] / (p + 1e-10f) - pg);
+    }
+    lrow = f * inv_bs;
+  }
+  if (lane == 0) red[warp] = lrow;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < MZ_THREADS / 32; w++) s += red[w];
+    part[blockIdx.x] = s;
+  }
+}
+
+// *out = offset + sum of part[0..n) in a fixed order (one block)
+__global__ void mz_ordered_sum_kernel(const float* __restrict__ part, int n, float offset, float* __restrict__ out) {
+  pdl_wait(); pdl_trigger();
+  __shared__ float red[MZ_THREADS];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += MZ_THREADS) s += part[i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = offset;
+    for (int w = 0; w < MZ_THREADS; w++) t += red[w];
+    *out = t;
+  }
+}
+
+// the dynamics input concat(hidden, one_hot(action)) (muzero_model.py:120-123, 57-61): x[b] = [h[b, 0..H), e_a],
+// a = action[b * a_ld + a_col]
+__global__ void mz_concat_onehot_kernel(const float* __restrict__ h, int B, int H, const int32_t* __restrict__ action, int a_ld,
+                                        int a_col, int A, float* __restrict__ x) {
+  pdl_wait(); pdl_trigger();
+  const long long n = (long long)B * (H + A);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int b = (int)(i / (H + A)), j = (int)(i - (long long)b * (H + A));
+    x[i] = j < H ? h[(long long)b * H + j] : (j - H == action[(long long)b * a_ld + a_col] ? 1.f : 0.f);
+  }
+}
+
+// gradient wrt the pre-activation of a hidden state h [B, H] with activation `act`: the prediction network's input
+// gradient g plus c times the hidden part of the next dynamics step's input gradient dx [B, ld] (none: dx == NULL)
+__global__ void mz_hidden_grad_kernel(const float* __restrict__ g, const float* __restrict__ dx, int ld, float c,
+                                      const float* __restrict__ h, int act, int B, int H, float* __restrict__ out) {
+  pdl_wait(); pdl_trigger();
+  const long long n = (long long)B * H;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / H, j = i - b * H;
+    const float d = g[i] + (dx ? c * dx[b * ld + j] : 0.f);
+    out[i] = d * act_grad_from_out(act, h[i]);
+  }
+}
+
+// dst += src (the gradient of one dynamics application into the shared gradient buffer, step by step in order)
+__global__ void mz_accumulate_kernel(float* __restrict__ dst, const float* __restrict__ src, long long n) {
+  pdl_wait(); pdl_trigger();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] += src[i];
+}
+
 }  // namespace xtb

@@ -348,6 +348,7 @@ static bool conv_tables_fit(const LayerPlan& lp, uint32_t max_unit_stages) {
 extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net** out) {
   if (!desc || !out || max_batch <= 0) return fail(XTB_ERR_ARG, "xtb_net_create: null/invalid argument");
   if (desc->n_layers <= 0 || desc->n_layers > XTB_MAX_LAYERS) return fail(XTB_ERR_ARG, "n_layers out of range");
+  if (desc->input_u8 < 0 || desc->input_u8 > 2) return fail(XTB_ERR_ARG, "input_u8 %d not in 0..2", desc->input_u8);
   auto* net = new xtb_net();
   net->desc = *desc;
   net->max_batch = max_batch;
@@ -499,6 +500,8 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   // a tensor-core layer reads its source in batch-planar form: features must come in chunks of 8 (always true for
   // the shapes accepted above; a dense layer after an uncovered odd-width layer falls back)
   for (auto& lp : net->L) if (lp.tc && lp.d.src != 0 && net->tsize[lp.d.src] % 8) lp.tc = false;
+  // the weight-blob refresh (bp_wprep_kernel) reads a tensor-core layer's kernel with 16-byte loads
+  for (auto& lp : net->L) if (lp.tc && lp.w_off % 4) lp.tc = lp.s2d = false;
   // stage tables of the tensor-core conv layers; a layer whose tables do not fit in shared memory falls back
   for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_CONV) {
     if (conv_tables_fit(lp, build_conv_tables(lp))) continue;
@@ -638,6 +641,9 @@ extern "C" int xtb_net_sync_weights(xtb_net* net, void* stream);
 extern "C" int xtb_net_bind_stream(xtb_net* net, float* params, float* grads, void* workspace, size_t workspace_bytes, void* stream) {
   if (!net || !params || !workspace) return fail(XTB_ERR_ARG, "xtb_net_bind: null pointer");
   if (workspace_bytes < net->ws_bytes) return fail(XTB_ERR_ARG, "workspace too small: %zu < %zu", workspace_bytes, net->ws_bytes);
+  bool tc_layers = false;
+  for (const auto& lp : net->L) tc_layers |= lp.tc;
+  if (tc_layers && (uintptr_t)params % 16) return fail(XTB_ERR_ARG, "xtb_net_bind: parameters must be 16-byte aligned");
   drop_graphs_of(net);                     // captured graphs baked the old buffers in
   net->params = params; net->grads = grads; net->ws = (char*)workspace;
   cudaStream_t st = S(stream);
@@ -1115,7 +1121,7 @@ static int op_decode(xtb_net* net, const void* obs, const int32_t* idx, int B, c
   dim3 grid(4 * net->H4, (B + bp::DEC_SAMPLES - 1) / bp::DEC_SAMPLES);
   const int smem = bp::DEC_SAMPLES * (net->desc.in_w * 4 + 8);
   XLAUNCH(bp::bp_decode_s2d_kernel, grid, bp::DEC_THREADS, smem, st, (const uint8_t*)obs, idx, B, net->desc.in_h, net->desc.in_w, net->H4,
-          net->W4, first->g.padT, first->g.padL, obs_bp(net));
+          net->W4, first->g.padT, first->g.padL, net->desc.input_u8 == 2 ? 1 : 0, obs_bp(net));
   LAUNCH_CHECK();
   net->obs_bp_ok = true;
   return XTB_OK;
@@ -1155,7 +1161,10 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
   }
   if (lp.d.src == 0) {
     float alpha = net->desc.scale;
-    if (net->desc.input_u8) {
+    if (net->desc.input_u8 == 2) {
+      if (lp.d.kind == XTB_CONV) conv_fwd<int8_t>(lp, (const int8_t*)obs, idx, w, b, alpha, pre, B, st);
+      else dense_fwd<int8_t>(lp, (const int8_t*)obs, idx, w, b, alpha, pre, B, st);
+    } else if (net->desc.input_u8) {
       if (lp.d.kind == XTB_CONV) conv_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
       else dense_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
     } else {
@@ -1207,7 +1216,10 @@ static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, in
   bool need_colsum = false;
   if (lp.d.src == 0) {
     float alpha = net->desc.scale;
-    if (net->desc.input_u8) {
+    if (net->desc.input_u8 == 2) {
+      if (lp.d.kind == XTB_CONV) conv_wgrad<int8_t>(lp, (const int8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
+      else dense_wgrad<int8_t>(lp, (const int8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
+    } else if (net->desc.input_u8) {
       if (lp.d.kind == XTB_CONV) conv_wgrad<uint8_t>(lp, (const uint8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
       else dense_wgrad<uint8_t>(lp, (const uint8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
     } else {
@@ -1357,18 +1369,33 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
 static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                              const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
                              unsigned bias_done_tensors = 0u, unsigned heads_bp_mask = 0u, xtb_comm* comm = nullptr,
-                             unsigned heads_dy_mask = 0u);
+                             unsigned heads_dy_mask = 0u, float* dobs = nullptr);
 extern "C" int xtb_net_backward(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                                 const int32_t* head_tensors, int n_heads, void* stream) {
   return net_backward_impl(net, obs, gather_idx, batch, head_tensors, n_heads, stream, 0u, true);
+}
+// d loss / d observation is defined for float observations that only dense layers read (decode scale 1)
+static int input_grad_check(const xtb_net* net) {
+  if (net->desc.input_u8 || net->desc.scale != 1.f) return fail(XTB_ERR_ARG, "input gradient: the observation must be float with scale 1");
+  for (const auto& lp : net->L)
+    if (lp.d.src == 0 && lp.d.kind != XTB_DENSE && lp.d.kind != XTB_LOGSTD)
+      return fail(XTB_ERR_ARG, "input gradient: only dense layers may read the observation");
+  return XTB_OK;
+}
+extern "C" int xtb_net_backward_input(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
+                                      const int32_t* head_tensors, int n_heads, float* dobs, void* stream) {
+  if (!obs || !dobs || !head_tensors) return fail(XTB_ERR_ARG, "xtb_net_backward_input: null pointer");
+  return net_backward_impl(net, obs, gather_idx, batch, head_tensors, n_heads, stream, 0u, true, 0u, 0u, nullptr, 0u, dobs);
 }
 // head_tensors: tensors whose gradient was filled by the caller: fp32 row-major, or (bit set in heads_bp_mask) planes;
 // wrt the pre-activation, or (bit set in heads_dy_mask, a layer with an activation past tanh) wrt the output
 static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                              const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
-                             unsigned bias_done_tensors, unsigned heads_bp_mask, xtb_comm* comm, unsigned heads_dy_mask) {
+                             unsigned bias_done_tensors, unsigned heads_bp_mask, xtb_comm* comm, unsigned heads_dy_mask,
+                             float* dobs) {
   if (!net || !net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_net_backward: net not bound (grads required)");
   if (batch <= 0 || batch > net->max_batch) return fail(XTB_ERR_ARG, "batch out of range");
+  if (dobs) { int rc = input_grad_check(net); if (rc) return rc; }
   cudaStream_t st = S(stream);
   const int nl = (int)net->L.size();
   std::vector<char> has_grad(nl + 1, 0), written(nl + 1, 0);
@@ -1425,6 +1452,24 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
       if (rc) return rc;
       written[s] = 1; has_grad[s] = 1; dy[s] = 1;
     }
+  }
+  if (dobs) {   // d loss / d observation: the data-gradient GEMM of every dense layer reading it, summed in layer order
+    bool first = true;
+    for (int i = 0; i < nl; i++) {
+      const LayerPlan& lp = net->L[i];
+      if (lp.d.src != 0 || lp.d.kind != XTB_DENSE || (skip_mask & (1u << i))) continue;
+      if (!has_grad[i + 1]) continue;
+      int rc = ensure_f32(net, i + 1, batch, true, st);
+      if (rc) return rc;
+      ADense<float> al{(const float*)(net->ws + net->gout_off[i + 1]), nullptr, lp.N};
+      BTransposed bl{net->params + lp.w_off, lp.N};
+      // linear: the epilogue's activation source is never used (dobs stands in as a valid address)
+      EpiDgrad ep{dobs, dobs, 0, lp.K, first ? 0 : 1, nullptr, 0};
+      launch_gemm(al, bl, ep, batch, lp.K, lp.N, false, st);
+      LAUNCH_CHECK();
+      first = false;
+    }
+    if (first) CUDA_TRY(cudaMemsetAsync(dobs, 0, (size_t)batch * net->tsize[0] * sizeof(float), st));
   }
   int rc = flush_reductions(net, st);
   if (rc || !comm || comm->world == 1) return rc;
@@ -1794,10 +1839,10 @@ extern "C" int xtb_set_grad_hook(xtb_grad_hook hook, void* user) {
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kPpoGaussTrain,
-                kGaussRolloutInfer };
+                kGaussRolloutInfer, kMuzeroTrain, kMuzeroInitInfer, kMuzeroRecurInfer };
 struct CaptureKey {
   uint64_t tag;          // entry point
-  const void* own[4];    // net, target, opt, comm: destroying one, or rebinding a net, drops the graph
+  const void* own[6];    // net, target, opt, two more nets, comm: destroying one, or rebinding a net, drops the graph
   uint64_t mode[2];      // kernel-path and fused-heads modes
   uint64_t arg[21];      // every pointer and scalar argument; floats by bit pattern
   bool operator<(const CaptureKey& o) const { return memcmp(this, &o, sizeof(CaptureKey)) < 0; }
@@ -1837,7 +1882,7 @@ static void drop_graphs_of(const void* obj) {
 template <class F>
 static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
   if (!use_graph) return launch(stream);
-  key.own[3] = g_comm; key.mode[0] = g_tc_mode; key.mode[1] = g_fuse_heads;
+  key.own[5] = g_comm; key.mode[0] = g_tc_mode; key.mode[1] = g_fuse_heads;
   StreamScope sc;
   int src = sc.begin(stream, true);
   if (src) return src;
@@ -2229,6 +2274,252 @@ extern "C" int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_imp
     }
     return XTB_OK;
   });
+}
+
+// ---- MuZero (xt/model/muzero/muzero_model.py:103-140, 154-239) -------------------------------------------------------
+// The three networks (representation, dynamics, prediction) are separate xtb_nets bound to consecutive slices of one
+// parameter buffer and one gradient buffer (the Keras list order of MuzeroBase); the dynamics net's own gradient buffer
+// is scratch that each of its K applications fills before it is added to its slice.  The object owns the step's
+// device scratch, sized for max_batch samples.
+struct xtb_muzero {
+  xtb_net *rep = nullptr, *dyn = nullptr, *pred = nullptr;
+  xtb_muzero_desc d{};
+  int max_batch = 0, K = 0, H = 0, A = 0, Sv = 0, Sr = 0, n_part = 0;
+  int act_rep = 0, act_dyn = 0;
+  float* buf = nullptr;
+  float *hbuf = nullptr, *xbuf = nullptr, *rlog = nullptr, *dr = nullptr, *tv = nullptr, *tr = nullptr, *dh = nullptr,
+        *dx = nullptr, *part = nullptr;
+};
+static inline int mz_blocks(long long rows) { return (int)((rows + MZ_THREADS / 32 - 1) / (MZ_THREADS / 32)); }
+
+extern "C" int xtb_muzero_create(xtb_net* rep, xtb_net* dyn, xtb_net* pred, const xtb_muzero_desc* desc, int max_batch,
+                                 xtb_muzero** out) {
+  if (!rep || !dyn || !pred || !desc || !out) return fail(XTB_ERR_ARG, "xtb_muzero_create: null pointer");
+  for (xtb_net* n : {rep, dyn, pred})
+    if (!n->ws || !n->params || !n->grads) return fail(XTB_ERR_STATE, "xtb_muzero_create: every net must be bound");
+  const xtb_muzero_desc& d = *desc;
+  const int K = d.unroll;
+  if (K < 1 || max_batch < 1) return fail(XTB_ERR_ARG, "xtb_muzero_create: unroll %d / max_batch %d out of range", K, max_batch);
+  auto bad_t = [](const xtb_net* n, int t) { return t < 1 || t >= (int)n->tsize.size() || n->tsize[t] == 0; };
+  if (bad_t(rep, d.rep_h) || bad_t(dyn, d.dyn_h) || bad_t(dyn, d.dyn_r) || bad_t(pred, d.pred_p) || bad_t(pred, d.pred_v) ||
+      d.dyn_h == d.dyn_r || d.pred_p == d.pred_v)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: bad tensor ids");
+  const int H = rep->tsize[d.rep_h], A = pred->tsize[d.pred_p], Sv = pred->tsize[d.pred_v], Sr = dyn->tsize[d.dyn_r];
+  if (dyn->tsize[d.dyn_h] != H || dyn->tsize[0] != H + A || pred->tsize[0] != H)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: widths disagree (hidden %d, actions %d, dynamics input %d, prediction input %d)", H,
+                A, dyn->tsize[0], pred->tsize[0]);
+  if (A > MZ_MAX_SUPPORT || Sv > MZ_MAX_SUPPORT || Sr > MZ_MAX_SUPPORT)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: a support or the action count exceeds %d", MZ_MAX_SUPPORT);
+  if (!(d.value_max > d.value_min) || !(d.reward_max > d.reward_min)) return fail(XTB_ERR_ARG, "xtb_muzero_create: empty value range");
+  for (const xtb_net* n : {dyn, pred}) if (int rc = input_grad_check(n)) return rc;
+  const int act_rep = rep->L[d.rep_h - 1].d.act, act_dyn = dyn->L[d.dyn_h - 1].d.act;
+  if (act_is_ext(act_rep) || act_is_ext(act_dyn)) return fail(XTB_ERR_ARG, "xtb_muzero_create: hidden states must be relu / tanh / linear");
+  for (int t : {d.pred_p, d.pred_v}) if (pred->L[t - 1].d.act != XTB_ACT_NONE || pred->L[t - 1].d.kind != XTB_DENSE)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: policy and value heads must be linear dense layers");
+  if (dyn->L[d.dyn_r - 1].d.act != XTB_ACT_NONE || dyn->L[d.dyn_r - 1].d.kind != XTB_DENSE)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: the reward head must be a linear dense layer");
+  if (rep->max_batch < max_batch || dyn->max_batch < max_batch || (long long)pred->max_batch < (long long)(K + 1) * max_batch)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: nets hold fewer rows than max_batch (prediction: (unroll + 1) * max_batch)");
+  // one parameter buffer [rep | dyn | pred] and one gradient buffer with the same layout; dyn's bound gradients lie outside
+  float* g0 = rep->grads;
+  const long long o_dyn = dyn->params - rep->params, o_pred = pred->params - rep->params, total = o_pred + pred->n_params;
+  if (o_dyn < rep->n_params || o_pred < o_dyn + dyn->n_params || pred->grads != g0 + o_pred)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: nets must be bound to slices [rep | dyn | pred] of one buffer, in order");
+  if (dyn->grads + dyn->n_params > g0 && dyn->grads < g0 + total)
+    return fail(XTB_ERR_ARG, "xtb_muzero_create: the dynamics net's gradient scratch overlaps the shared gradient buffer");
+  auto* m = new xtb_muzero();
+  m->rep = rep; m->dyn = dyn; m->pred = pred; m->d = d; m->max_batch = max_batch;
+  m->K = K; m->H = H; m->A = A; m->Sv = Sv; m->Sr = Sr; m->act_rep = act_rep; m->act_dyn = act_dyn;
+  const long long Bm = max_batch, R1 = (long long)(K + 1) * Bm, RK = (long long)K * Bm;
+  m->n_part = 2 * mz_blocks(R1) + mz_blocks(RK);
+  const long long sizes[] = {R1 * H, RK * (H + A), RK * Sr, RK * Sr, R1 * Sv, RK * Sr, R1 * H, Bm * (H + A), m->n_part};
+  float** dst[] = {&m->hbuf, &m->xbuf, &m->rlog, &m->dr, &m->tv, &m->tr, &m->dh, &m->dx, &m->part};
+  long long tot = 0;
+  for (long long n : sizes) tot += (n + 63) / 64 * 64;
+  cudaError_t e = cudaMalloc(&m->buf, tot * sizeof(float));
+  if (e != cudaSuccess) { delete m; return fail(XTB_ERR_NOMEM, "xtb_muzero_create: %s", cudaGetErrorString(e)); }
+  e = cudaMemset(m->buf, 0, tot * sizeof(float));
+  if (e != cudaSuccess) { cudaFree(m->buf); delete m; return fail(XTB_ERR_CUDA, "xtb_muzero_create: %s", cudaGetErrorString(e)); }
+  float* p = m->buf;
+  for (int i = 0; i < 9; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
+  *out = m;
+  return XTB_OK;
+}
+
+extern "C" void xtb_muzero_destroy(xtb_muzero* m) {
+  if (!m) return;
+  drop_graphs_of(m);
+  cudaDeviceSynchronize();
+  cudaFree(m->buf);
+  delete m;
+}
+
+// shared argument checks of the MuZero entry points
+static int mz_check(const char* fn, const xtb_muzero* m, int batch) {
+  if (!m) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (g_comm || g_grad_hook) return fail(XTB_ERR_STATE, "%s: data-parallel training (gradient hook / communicator) is not supported", fn);
+  if (batch < 1 || batch > m->max_batch) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d]", fn, batch, m->max_batch);
+  return XTB_OK;
+}
+
+// prediction forward over `rows` hidden states (rows of m->hbuf), then softmax policy / value expectation if asked
+static int mz_predict(xtb_muzero* m, const float* hidden, int rows, float* value_out, float* policy_out, cudaStream_t st) {
+  const xtb_muzero_desc& d = m->d;
+  int rc = net_forward_impl(m->pred, nullptr, hidden, nullptr, rows, st, 0u, (1u << d.pred_p) | (1u << d.pred_v));
+  if (rc) return rc;
+  if (value_out) {
+    XLAUNCH(mz_support_value_kernel, mz_blocks(rows), MZ_THREADS, 0, st, (const float*)xtb_net_tensor(m->pred, d.pred_v), rows, m->Sv,
+            d.value_min, d.value_max, value_out);
+    LAUNCH_CHECK();
+  }
+  if (policy_out) {
+    XLAUNCH(softmax_rows_kernel, (rows + 127) / 128, 128, 0, st, (const float*)xtb_net_tensor(m->pred, d.pred_p), rows, m->A, policy_out);
+    LAUNCH_CHECK();
+  }
+  return XTB_OK;
+}
+
+// initial_inference / value_inference: representation then prediction
+static int mz_initial_launch(xtb_muzero* m, const void* obs, int B, float* hidden_out, float* value_out, float* policy_out,
+                             cudaStream_t st) {
+  int rc = net_forward_impl(m->rep, nullptr, obs, nullptr, B, st, 0u, 1u << m->d.rep_h);
+  if (rc) return rc;
+  const float* h = xtb_net_tensor(m->rep, m->d.rep_h);
+  if (hidden_out) CUDA_TRY(cudaMemcpyAsync(hidden_out, h, (size_t)B * m->H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return mz_predict(m, h, B, value_out, policy_out, st);
+}
+
+extern "C" int xtb_muzero_initial_inference(xtb_muzero* m, const void* obs, int batch, float* hidden_out, float* value_out,
+                                            float* policy_out, int use_graph, void* stream) {
+  if (int rc = mz_check("xtb_muzero_initial_inference", m, batch)) return rc;
+  if (!obs) return fail(XTB_ERR_ARG, "xtb_muzero_initial_inference: null observation");
+  CaptureKey key = capture_key(kMuzeroInitInfer, m->rep, m->dyn, nullptr, m, obs, batch, hidden_out, value_out, policy_out);
+  key.own[3] = m->pred; key.own[4] = m;
+  return run_graph(key, use_graph, stream, [&](void* st) { return mz_initial_launch(m, obs, batch, hidden_out, value_out, policy_out, S(st)); });
+}
+
+extern "C" int xtb_muzero_recurrent_inference(xtb_muzero* m, const float* hidden, const int32_t* action, int batch, float* hidden_out,
+                                              float* reward_out, float* value_out, float* policy_out, int use_graph, void* stream) {
+  if (int rc = mz_check("xtb_muzero_recurrent_inference", m, batch)) return rc;
+  if (!hidden || !action) return fail(XTB_ERR_ARG, "xtb_muzero_recurrent_inference: null pointer");
+  CaptureKey key = capture_key(kMuzeroRecurInfer, m->rep, m->dyn, nullptr, m, hidden, action, batch, hidden_out, reward_out, value_out,
+                               policy_out);
+  key.own[3] = m->pred; key.own[4] = m;
+  return run_graph(key, use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    const xtb_muzero_desc& d = m->d;
+    const int H = m->H, A = m->A;
+    XLAUNCH(mz_concat_onehot_kernel, std::min(4 * kSMs, (batch * (H + A) + 255) / 256), 256, 0, st, hidden, batch, H, action, 1, 0, A, m->xbuf);
+    LAUNCH_CHECK();
+    int rc = net_forward_impl(m->dyn, nullptr, m->xbuf, nullptr, batch, st, 0u, (1u << d.dyn_h) | (1u << d.dyn_r));
+    if (rc) return rc;
+    const float* h = xtb_net_tensor(m->dyn, d.dyn_h);
+    if (hidden_out) CUDA_TRY(cudaMemcpyAsync(hidden_out, h, (size_t)batch * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (reward_out) {
+      XLAUNCH(mz_support_value_kernel, mz_blocks(batch), MZ_THREADS, 0, st, (const float*)xtb_net_tensor(m->dyn, d.dyn_r), batch, m->Sr,
+              d.reward_min, d.reward_max, reward_out);
+      LAUNCH_CHECK();
+    }
+    return mz_predict(m, h, batch, value_out, policy_out, st);
+  });
+}
+
+// MuzeroModel.train (muzero_model.py:103-140, 154-169) over B samples
+static int mz_train_launch(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch& bt, int B, float loss_offset, float* loss_out,
+                           float* value_out, cudaStream_t st) {
+  const xtb_muzero_desc& d = m->d;
+  const int K = m->K, H = m->H, A = m->A, Sv = m->Sv, Sr = m->Sr, X = H + A;
+  const int R1 = (K + 1) * B, RK = K * B;
+  xtb_net *rep = m->rep, *dyn = m->dyn, *pred = m->pred;
+  const unsigned dyn_out = (1u << d.dyn_h) | (1u << d.dyn_r);
+  const int ew_blocks = std::min(4 * kSMs, (B * X + 255) / 256);
+  // two-hot targets: value rows step-major [K+1][B], reward rows [K][B] (the last reward target is not used)
+  XLAUNCH(mz_support_project_kernel, mz_blocks(R1), MZ_THREADS, 0, st, bt.target_value, R1, B, K + 1, Sv, d.value_min, d.value_max, m->tv);
+  LAUNCH_CHECK();
+  XLAUNCH(mz_support_project_kernel, mz_blocks(RK), MZ_THREADS, 0, st, bt.target_reward, RK, B, K + 1, Sr, d.reward_min, d.reward_max, m->tr);
+  LAUNCH_CHECK();
+  // h_0 = representation(obs); h_{k+1}, r_k = dynamics(concat(h_k, one_hot(a_k)))
+  int rc = net_forward_impl(rep, nullptr, bt.obs, nullptr, B, st, 0u, 1u << d.rep_h);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(m->hbuf, xtb_net_tensor(rep, d.rep_h), (size_t)B * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  for (int k = 0; k < K; k++) {
+    float* xk = m->xbuf + (size_t)k * B * X;
+    XLAUNCH(mz_concat_onehot_kernel, ew_blocks, 256, 0, st, (const float*)(m->hbuf + (size_t)k * B * H), B, H, bt.action, K, k, A, xk);
+    LAUNCH_CHECK();
+    rc = net_forward_impl(dyn, nullptr, xk, nullptr, B, st, 0u, dyn_out);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(m->hbuf + (size_t)(k + 1) * B * H, xtb_net_tensor(dyn, d.dyn_h), (size_t)B * H * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(m->rlog + (size_t)k * B * Sr, xtb_net_tensor(dyn, d.dyn_r), (size_t)B * Sr * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st));
+  }
+  // the K+1 prediction applications as one forward over (K+1) B rows
+  rc = net_forward_impl(pred, nullptr, m->hbuf, nullptr, R1, st, 0u, (1u << d.pred_p) | (1u << d.pred_v));
+  if (rc) return rc;
+  // losses: rows of h_0 at gradient scale 1, the unrolled terms at 1/K
+  const float gk = 1.f / K;
+  const int n1 = mz_blocks(R1);
+  XLAUNCH(mz_support_ce_kernel, n1, MZ_THREADS, 0, st, (const float*)xtb_net_tensor(pred, d.pred_p), R1, A, bt.target_policy, B, K + 1, B,
+          gk, 1.f / ((float)B * A), xtb_net_tensor_grad(pred, d.pred_p), m->part);
+  LAUNCH_CHECK();
+  XLAUNCH(mz_support_ce_kernel, n1, MZ_THREADS, 0, st, (const float*)xtb_net_tensor(pred, d.pred_v), R1, Sv, (const float*)m->tv, B, 0, B,
+          gk, 1.f / ((float)B * Sv), xtb_net_tensor_grad(pred, d.pred_v), m->part + n1);
+  LAUNCH_CHECK();
+  XLAUNCH(mz_support_ce_kernel, mz_blocks(RK), MZ_THREADS, 0, st, (const float*)m->rlog, RK, Sr, (const float*)m->tr, B, 0, 0, gk,
+          1.f / ((float)B * Sr), m->dr, m->part + 2 * n1);
+  LAUNCH_CHECK();
+  XLAUNCH(mz_ordered_sum_kernel, 1, MZ_THREADS, 0, st, (const float*)m->part, 2 * n1 + mz_blocks(RK), loss_offset, loss_out);
+  LAUNCH_CHECK();
+  // backward: prediction (with d loss / d h_i for every i), the dynamics steps newest first, the representation
+  const int32_t pheads[2] = {d.pred_p, d.pred_v}, dheads[2] = {d.dyn_h, d.dyn_r}, rheads[1] = {d.rep_h};
+  rc = net_backward_impl(pred, m->hbuf, nullptr, R1, pheads, 2, st, 0u, true, 0u, 0u, nullptr, 0u, m->dh);
+  if (rc) return rc;
+  float* gdyn = rep->grads + (dyn->params - rep->params);
+  CUDA_TRY(cudaMemsetAsync(gdyn, 0, dyn->n_params * sizeof(float), st));
+  for (int k = K - 1; k >= 0; k--) {
+    const float* xk = m->xbuf + (size_t)k * B * X;
+    if (k < K - 1) { rc = net_forward_impl(dyn, nullptr, xk, nullptr, B, st, 0u, dyn_out); if (rc) return rc; }   // recompute step k
+    // d h_{k+1}: prediction + 0.5 x the input gradient of step k+1 (scale_gradient(hidden, 0.5))
+    XLAUNCH(mz_hidden_grad_kernel, ew_blocks, 256, 0, st, (const float*)(m->dh + (size_t)(k + 1) * B * H),
+            (const float*)(k + 1 < K ? m->dx : nullptr), X, 0.5f, (const float*)xtb_net_tensor(dyn, d.dyn_h), m->act_dyn, B, H,
+            xtb_net_tensor_grad(dyn, d.dyn_h));
+    LAUNCH_CHECK();
+    CUDA_TRY(cudaMemcpyAsync(xtb_net_tensor_grad(dyn, d.dyn_r), m->dr + (size_t)k * B * Sr, (size_t)B * Sr * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st));
+    rc = net_backward_impl(dyn, xk, nullptr, B, dheads, 2, st, 0u, true, 0u, 0u, nullptr, 0u, m->dx);
+    if (rc) return rc;
+    XLAUNCH(mz_accumulate_kernel, std::min(4 * kSMs, (int)((dyn->n_params + 255) / 256)), 256, 0, st, gdyn, (const float*)dyn->grads,
+            dyn->n_params);
+    LAUNCH_CHECK();
+  }
+  // d h_0: prediction + the full input gradient of step 0 (h_0 is not scaled)
+  XLAUNCH(mz_hidden_grad_kernel, ew_blocks, 256, 0, st, (const float*)m->dh, (const float*)m->dx, X, 1.f,
+          (const float*)xtb_net_tensor(rep, d.rep_h), m->act_rep, B, H, xtb_net_tensor_grad(rep, d.rep_h));
+  LAUNCH_CHECK();
+  rc = net_backward_impl(rep, bt.obs, nullptr, B, rheads, 1, st, 0u, true);
+  if (rc) return rc;
+  // AdamOptimizer(LR).minimize over the whole buffer, then the weight blobs of the three nets
+  rc = adam_step_impl(opt, rep->params, rep->grads, 1.f, st, nullptr);
+  for (xtb_net* n : {rep, dyn, pred}) if (!rc) rc = xtb_net_sync_weights(n, st);
+  if (rc || !value_out) return rc;
+  // post-update value_inference of the batch (the learner's new priorities)
+  return mz_initial_launch(m, bt.obs, B, nullptr, value_out, nullptr, st);
+}
+
+extern "C" int xtb_muzero_train(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch* batch_in, int batch, float loss_offset,
+                                float* loss_out, float* value_out, int use_graph, void* stream) {
+  if (int rc = mz_check("xtb_muzero_train", m, batch)) return rc;
+  if (!opt || !batch_in || !loss_out) return fail(XTB_ERR_ARG, "xtb_muzero_train: null pointer");
+  const xtb_muzero_batch bt = *batch_in;
+  if (!bt.obs || !bt.action || !bt.target_value || !bt.target_reward || !bt.target_policy)
+    return fail(XTB_ERR_ARG, "xtb_muzero_train: null batch array");
+  if (bt.unroll != m->K) return fail(XTB_ERR_ARG, "xtb_muzero_train: batch unroll %d != model unroll %d", bt.unroll, m->K);
+  if (opt->count != (m->pred->params - m->rep->params) + m->pred->n_params)
+    return fail(XTB_ERR_ARG, "xtb_muzero_train: optimiser size %lld != parameter count", opt->count);
+  CaptureKey key = capture_key(kMuzeroTrain, m->rep, m->dyn, opt, m, bt.obs, bt.action, bt.target_value, bt.target_reward,
+                               bt.target_policy, batch, loss_offset, loss_out, value_out);
+  key.own[3] = m->pred; key.own[4] = m;
+  return run_graph(key, use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
 }
 
 // Dueling head that the fused TD step covers: q_tensor combines two linear dense layers that read the same hidden

@@ -51,7 +51,7 @@ class Net(object):
         self.names = ["obs"] + [l[0] for l in arch["layers"]]
         self.tid = {n: i for i, n in enumerate(self.names)}
         desc = capi.NetDesc()
-        desc.input_u8 = 1 if arch["input_dtype"] == "uint8" else 0
+        desc.input_u8 = {"uint8": 1, "int8": 2}.get(arch["input_dtype"], 0)
         desc.scale = float(arch["scale"])
         sd = tuple(arch["state_dim"])
         desc.in_h, desc.in_w, desc.in_c = (sd if len(sd) == 3 else (1, 1, int(np.prod(sd))))
@@ -116,6 +116,24 @@ class Net(object):
         with torch.cuda.device(self.device):
             check(self.lib.xtb_net_bind_stream(self.handle, _ptr(self.params), _ptr(self.grads),
                                                C.c_void_p(self._ws_base), ws_bytes, stream_ptr()))
+
+    def bind_to(self, params, grads):
+        """Rebind the network to `params` / `grads` (float32 device views of n_params floats, e.g. slices of a buffer shared
+        with other networks); the workspace is kept and its contents are reset."""
+        for t in (params, grads):
+            if t.numel() != self.n_params or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError("bind_to needs contiguous float32 views of %d floats" % self.n_params)
+        self.params, self.grads = params, grads
+        ws_bytes = int(self.lib.xtb_net_workspace_bytes(self.handle))
+        with torch.cuda.device(self.device):
+            check(self.lib.xtb_net_bind_stream(self.handle, _ptr(self.params), _ptr(self.grads),
+                                               C.c_void_p(self._ws_base), ws_bytes, stream_ptr()))
+
+    def backward_input(self, obs, batch, heads, dobs, idx=None):
+        """backward() that also writes d loss / d observation into `dobs` [batch, obs width] (xtb_net_backward_input)."""
+        arr = (C.c_int32 * len(heads))(*[self.tid[h] for h in heads])
+        check(self.lib.xtb_net_backward_input(self.handle, _ptr(obs), _ptr(idx), int(batch), arr, len(heads), _ptr(dobs),
+                                              stream_ptr()))
 
     def params_changed(self):
         """Must follow every host-side write into `self.params`: refreshes the bf16 hi/lo planes the

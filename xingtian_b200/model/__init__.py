@@ -5,3 +5,4 @@ from .impala import ImpalaCnnOpt  # noqa: F401
 from .dqn import DqnCnn, DqnMlp  # noqa: F401
 from .impala_mlp import ImpalaMlp  # noqa: F401
 from .impala_cnn import ImpalaCnn  # noqa: F401
+from .muzero import MuzeroCnn, MuzeroMlp, MuzeroModel  # noqa: F401

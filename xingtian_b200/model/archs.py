@@ -138,3 +138,51 @@ def impala_mlp(state_dim, action_dim, hidden_size, num_layers):
     _impala_heads(layers, action_dim)
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
                 outputs=["output_actions", "output_value"])
+
+
+def muzero_cnn(state_dim, action_dim, value_support, reward_support, hidden_out=256):
+    """MuzeroCnn (xt/model/muzero/muzero_cnn.py:42-67): representation, dynamics and prediction tables, in the order of
+    MuzeroBase's weight list.  The softmax heads are linear here; the engine's kernels evaluate the softmax.  Within the
+    prediction model Keras lists out_p before out_v: its layers are ordered by a depth-first walk from the outputs
+    [out_p, out_v], not by creation (out_v is created first)."""
+    if len(state_dim) != 3:
+        raise ValueError("MuzeroCnn needs an image observation, got {}".format(list(state_dim)))
+    a = action_dim
+    rep = dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0, layers=[
+        ("conv2d", "conv", "obs", _conv(32, 8, 4, "valid", "relu")),
+        ("conv2d_1", "conv", "conv2d", _conv(32, 4, 2, "valid", "relu")),
+        ("conv2d_2", "conv", "conv2d_1", _conv(64, 3, 1, "valid", "relu")),
+        ("dense", "dense", "conv2d_2", dict(n=hidden_out, act="relu")),
+    ], outputs=["dense"])
+    dyn = dict(input_dtype="float32", state_dim=(hidden_out + a,), scale=1.0, layers=[
+        ("dense", "dense", "obs", dict(n=256, act="relu")),
+        ("dense_1", "dense", "dense", dict(n=128, act="relu")),
+        ("out_h", "dense", "dense_1", dict(n=hidden_out, act="relu")),
+        ("out_r", "dense", "dense_1", dict(n=reward_support, act=None)),
+    ], outputs=["out_h", "out_r"])
+    pred = dict(input_dtype="float32", state_dim=(hidden_out,), scale=1.0, layers=[
+        ("dense", "dense", "obs", dict(n=128, act="relu")),
+        ("out_p", "dense", "dense", dict(n=a, act=None)),
+        ("out_v", "dense", "dense", dict(n=value_support, act=None)),
+    ], outputs=["out_p", "out_v"])
+    return rep, dyn, pred
+
+
+def muzero_mlp(state_dim, action_dim, value_support, reward_support, hidden1=64, hidden2=4):
+    """MuzeroMlp (xt/model/muzero/muzero_mlp.py:41-63): the same three models with HIDDEN1_UNITS / HIDDEN2_UNITS widths."""
+    a = action_dim
+    rep = dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=[
+        ("dense", "dense", "obs", dict(n=hidden1, act="relu")),
+        ("dense_1", "dense", "dense", dict(n=hidden2, act="relu")),
+    ], outputs=["dense_1"])
+    dyn = dict(input_dtype="float32", state_dim=(hidden2 + a,), scale=1.0, layers=[
+        ("dense", "dense", "obs", dict(n=hidden1, act="relu")),
+        ("out_h", "dense", "dense", dict(n=hidden2, act="relu")),
+        ("out_r", "dense", "dense", dict(n=reward_support, act=None)),
+    ], outputs=["out_h", "out_r"])
+    pred = dict(input_dtype="float32", state_dim=(hidden2,), scale=1.0, layers=[
+        ("dense", "dense", "obs", dict(n=hidden1, act="relu")),
+        ("out_p", "dense", "dense", dict(n=a, act=None)),
+        ("out_v", "dense", "dense", dict(n=value_support, act=None)),
+    ], outputs=["out_p", "out_v"])
+    return rep, dyn, pred
