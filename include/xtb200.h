@@ -316,7 +316,7 @@ int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs,
  * order[k*fit_batch ...] (device int32 [n], the host-drawn np.random.shuffle order) of obs / action_mat [n, A] (one-hot
  * y_true) / adv [n] / target_v [n]; per minibatch forward, the Keras loss (see xtb_impala_keras_loss_grad, value weight
  * 0.5), backward and the optimiser step.  *loss_out = the epoch loss: per-row loss summed over the n rows, over n.
- * Both calls return XTB_ERR_STATE, launching nothing, while a gradient hook or communicator is installed. */
+ * Both calls return XTB_ERR_STATE, launching nothing, while a communicator is installed. */
 int xtb_impala_keras_fit(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* order, const float* action_mat,
                          const float* adv, const float* target_v, int n, int fit_batch, int logit_tensor, int v_tensor,
                          float ent_coef, float* loss_out, int use_graph, void* stream);
@@ -465,7 +465,7 @@ typedef struct xtb_muzero_batch {
  * scaled by 0.5 (h_0 unscaled); backward (dynamics recomputed step by step); one Adam step of `opt` (created over the
  * whole buffer, no clipping) and the weight refresh of the three nets.  *loss_out = loss_offset + loss, its terms summed
  * in a fixed order.  value_out != NULL: [B] the value of every observation after the update (value_inference).
- * XTB_ERR_STATE, launching nothing, while a gradient hook or communicator is installed. */
+ * XTB_ERR_STATE, launching nothing, while a communicator is installed. */
 int xtb_muzero_train(xtb_muzero* mz, xtb_adam* opt, const xtb_muzero_batch* batch_in, int batch, float loss_offset,
                      float* loss_out, float* value_out, int use_graph, void* stream);
 /* initial_inference / value_inference (muzero_model.py:74-82, 228-239) over `batch` observations: hidden [B, H],
@@ -481,14 +481,6 @@ int xtb_muzero_recurrent_inference(xtb_muzero* mz, const float* hidden, const in
  * by dense layers only; otherwise XTB_ERR_ARG. */
 int xtb_net_backward_input(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                            const int32_t* head_tensors, int n_heads, float* dobs, void* stream);
-
-/* Data-parallel hook (SURVEY 8(e)): called between backward and the optimiser with the flat
- * gradient bucket; must SUM it over ranks on `stream` (e.g. ncclAllReduce).  Called once with
- * grads == NULL before the loop: must return the world size.  While a hook is installed the
- * loss/gradient scale becomes 1/(world*B_local) and CUDA-graph replay is disabled.
- * Reference precedent: xt/framework/trainer.py:82-92 (shared-memory gradient averaging). */
-typedef int (*xtb_grad_hook)(void* user, float* grads, long long count, void* stream);
-int xtb_set_grad_hook(xtb_grad_hook hook, void* user);
 
 /* Data-parallel communicator owned by the library (SURVEY 8(e); precedent zeus/trainer/trainer_tf.py:187-203): NCCL is
  * resolved with dlopen (`nccl_path` NULL = "libnccl.so.2").  Rank 0 calls xtb_comm_unique_id and ships the 128 bytes to

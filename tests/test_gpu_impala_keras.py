@@ -4,15 +4,13 @@ replay, argument validation and weight I/O.
 
 Bounds are those of test_gpu_dueling: loss within 5e-3 relative, the weight update within 5e-2 L2-relative of the float64
 oracle's (it absorbs a ReLU that flips between fp32 and float64 near zero)."""
-import ctypes as C
-
 import numpy as np
 import pytest
 import torch
 
 import impala_keras_oracle as iko
 from oracle import xt_oracle as orc
-from test_gpu_kernels import _keepalive, dev, l2_rel, rel_err, xb  # noqa: F401
+from test_gpu_kernels import _keepalive, dev, l2_rel, one_rank_comm, rel_err, xb  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -244,12 +242,8 @@ def test_invalid_arguments_launch_nothing(xb):
     assert lib.xtb_impala_keras_fit(big.net.handle, big.opt.handle, _ptr(obs), _ptr(order), _ptr(y), _ptr(adv), _ptr(tv), n, 8,
                                     big.net.tid[big.logit_name], big.net.tid[big.value_name], 0.01, _ptr(loss), 0,
                                     stream_ptr()) == -1
-    hook = capi.GRAD_HOOK(lambda *a: 0)
-    capi.check(lib.xtb_set_grad_hook(hook, None))
-    try:
+    with one_rank_comm():
         assert fit() == -3 and b"data-parallel" in lib.xtb_last_error()
-    finally:
-        capi.check(lib.xtb_set_grad_hook(C.cast(None, capi.GRAD_HOOK), None))
     assert lib.xtb_launch_count() == before
     assert fit() == 0
 

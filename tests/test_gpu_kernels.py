@@ -2,6 +2,7 @@
 
 Tolerances: bit-exact for action indices on shared noise; fp results within 1e-3 relative
 (BASELINE.json north_star), measured as max|gpu-ref| / max(max|ref|, floor)."""
+import contextlib
 import ctypes as C
 import os
 
@@ -47,6 +48,25 @@ def dev(a, dtype=None):
     t = t.cuda()
     _KEEP.append(t)
     return t
+
+
+@contextlib.contextmanager
+def one_rank_comm():
+    """A one-rank NCCL communicator installed for the duration: the library runs its data-parallel paths on one GPU"""
+    from xingtian_b200 import capi, engine
+    lib = capi.lib()
+    path = engine._nccl_path()
+    path = path.encode() if path else None
+    ident = (C.c_ubyte * 128)()
+    capi.check(lib.xtb_comm_unique_id(path, ident))
+    h = C.c_void_p()
+    capi.check(lib.xtb_comm_create(path, ident, 0, 1, C.byref(h)))
+    capi.check(lib.xtb_set_grad_comm(h))
+    try:
+        yield
+    finally:
+        capi.check(lib.xtb_set_grad_comm(None))
+        lib.xtb_comm_destroy(h)
 
 
 # ------------------------------------------------------------------------------------------- GAE

@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import muzero_oracle as mo
+from test_gpu_kernels import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -217,12 +218,8 @@ def test_invalid_arguments_launch_nothing():
     assert lib.xtb_muzero_initial_inference(m.handle, None, 4, None, None, None, 1, stream_ptr()) == -1
     assert lib.xtb_muzero_recurrent_inference(m.handle, _ptr(b["hid_in"]), _ptr(b["act1"]), 17, None, None, None, None, 1,
                                               stream_ptr()) == -1
-    hook = capi.GRAD_HOOK(lambda u, g, c, s: 1)
-    lib.xtb_set_grad_hook(hook, None)
-    try:
-        assert call(8) == -3
-    finally:
-        lib.xtb_set_grad_hook(C.cast(None, capi.GRAD_HOOK), None)
+    with one_rank_comm():
+        assert call(8) == -3 and b"data-parallel" in lib.xtb_last_error()
     # the create-time checks: a support wider than the kernels take, nets not bound to one buffer
     desc = capi.MuzeroDesc(m.td_step, 2, 2, 3, 2, 3, 0.0, 10.0, 0.0, 10.0)
     out = C.c_void_p()

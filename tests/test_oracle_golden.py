@@ -146,7 +146,7 @@ def test_vtrace_matches_naive_recursion():
 
 def test_data_parallel_gradient_identity():
     """SURVEY 8(e): sum over ranks of gradients computed with the 1/B_global scale == gradient of the global
-    minibatch (what xtb_ppo_train does when a gradient hook is installed)."""
+    minibatch (what xtb_ppo_train does with a communicator installed)."""
     import torch
     arch = orc.ppo_mlp_arch()
     w = orc.init_weights(arch, 3)

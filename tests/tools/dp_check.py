@@ -39,17 +39,14 @@ perms = [np.stack([np.random.default_rng(1000 * r + e).permutation(N) for e in r
 # ---- data-parallel run
 dp_first = None
 alg = make_alg(BL)
-dp = engine.GradAllReduce(alg.actor.net) if os.environ.get("XTB_DP") == "hook" else engine.GradComm()
+dp = engine.GradComm()
 fill(alg, [rank])
 loss_dp = alg.actor.train_device(N, perm=perms[rank])
 trace_dp = torch.tensor(alg.actor.last_losses, device="cuda")
 dist.all_reduce(trace_dp)                      # per-rank losses are partial sums of the global mean
 w_dp = np.concatenate([v.ravel() for v in alg.get_weights().values()])
 print('rank %d: dp run done' % rank, flush=True)
-if hasattr(dp, 'detach'):
-    dp.detach()
-else:
-    dp.close()
+dp.detach()
 # weights identical on every rank
 wt = torch.from_numpy(w_dp).cuda(); w0 = wt.clone(); dist.broadcast(w0, 0)
 assert torch.equal(wt, w0), "replicas diverged"

@@ -65,7 +65,6 @@ class MuzeroBatch(C.Structure):
 
 
 _P = C.c_void_p
-GRAD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p)
 _SIGS = {
     "xtb_version": (C.c_int, []),
     "xtb_last_error": (C.c_char_p, []),
@@ -138,7 +137,6 @@ _SIGS = {
     "xtb_muzero_initial_inference": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P]),
     "xtb_muzero_recurrent_inference": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
-    "xtb_set_grad_hook": (C.c_int, [GRAD_HOOK, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),
     "xtb_comm_destroy": (None, [_P]),

@@ -1827,12 +1827,6 @@ struct StreamScope {
 };
 static int g_fuse_heads = [] { const char* e = getenv("XTB_FUSE_HEADS"); return e ? atoi(e) : 1; }();
 extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
-static xtb_grad_hook g_grad_hook = nullptr;
-static void* g_grad_hook_user = nullptr;
-extern "C" int xtb_set_grad_hook(xtb_grad_hook hook, void* user) {
-  g_grad_hook = hook; g_grad_hook_user = user;
-  return XTB_OK;
-}
 
 // ---- CUDA-graph cache of the fused entry points ------------------------------------------------
 // A captured graph bakes in every kernel argument, so its key holds everything the capture reads.  capture_key()
@@ -1939,7 +1933,7 @@ static void launch_infer_heads(int K, int A, int blocks, cudaStream_t st, Args..
 
 // The epoch x minibatch loop of PPO.train (xt/model/ppo/ppo.py:111-132): minibatch k of epoch e holds rows
 // perm[e*N + k*B ...] (the last one ragged).  minibatch(idx, mb, loss) enqueues its forward, loss and backward; the
-// gradient hook and the optimiser step follow.
+// optimiser step follows.
 template <class STEP>
 static int ppo_epoch_loop(xtb_net* net, xtb_adam* opt, int N, int B, int E, const int32_t* perm, float* loss_per_step,
                           void* stream, STEP&& minibatch) {
@@ -1951,10 +1945,6 @@ static int ppo_epoch_loop(xtb_net* net, xtb_adam* opt, int N, int B, int E, cons
       int mb = std::min(B, N - s0);
       int rc = minibatch(perm + (long long)e * N + s0, mb, loss_per_step + step);
       if (rc) return rc;
-      if (g_grad_hook && !g_comm) {
-        rc = g_grad_hook(g_grad_hook_user, net->grads, net->n_params, stream);
-        if (rc) return fail(XTB_ERR_STATE, "gradient hook failed with %d", rc);
-      }
       rc = xtb_adam_step_net(opt, net, 1.f, stream);
       if (rc) return rc;
     }
@@ -1962,15 +1952,9 @@ static int ppo_epoch_loop(xtb_net* net, xtb_adam* opt, int N, int B, int E, cons
   return XTB_OK;
 }
 
-// loss / gradient scale of the PPO loops: 1 / world when data parallel (communicator or gradient hook), else 1
-static float ppo_inv_world() {
-  if (g_comm) return 1.f / g_comm->world;
-  if (g_grad_hook) {   // the hook sums gradients over ranks; every rank holds B/world samples
-    int rc = g_grad_hook(g_grad_hook_user, nullptr, 0, nullptr);   // query: returns world size when grads == NULL
-    return 1.f / (rc > 0 ? rc : 1);
-  }
-  return 1.f;
-}
+// loss / gradient scale of the training loops that average over the local batch: 1 / world while a communicator sums
+// the gradients over ranks, else 1
+static float dp_inv_world() { return g_comm ? 1.f / g_comm->world : 1.f; }
 
 // Fused PPO heads of tensors pi_t / v_t: both heads are linear dense layers on hidden (non-observation) tensors of equal
 // width within the heads_kernel limits (infer: the infer_heads_kernel limits), and the fused-heads mode is on
@@ -2127,11 +2111,11 @@ static int ppo_train(xtb_net* net, xtb_adam* opt, const RO* ro, int n_sample, in
   if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
   if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
   if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
-  const float inv_world = ppo_inv_world();
+  const float inv_world = dp_inv_world();
   return run_graph(capture_key(PpoCalls<DIST>::train_tag, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
                                loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
                                hp->critic_coef, pi_t, v_t, ls_t),
-                   use_graph && !(g_grad_hook && !g_comm), stream, [&](void* st) {
+                   use_graph, stream, [&](void* st) {
     return ppo_train_launch<DIST>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_t, v_t, ls_t, loss_per_step, inv_world, st);
   });
 }
@@ -2213,7 +2197,7 @@ static int keras_fit_launch(xtb_net* net, xtb_adam* opt, const void* obs, const 
 // arguments both IMPALA entry points share; data-parallel training is not supported by them
 static int keras_check(const char* fn, xtb_net* net, int lt, int vt) {
   if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
-  if (g_comm || g_grad_hook) return fail(XTB_ERR_STATE, "%s: data-parallel training (gradient hook / communicator) is not supported", fn);
+  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
   const int nl = (int)net->L.size();
   if (lt < 1 || lt > nl || vt < 1 || vt > nl || lt == vt || net->tsize[vt] != 1) return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
   if (net->tsize[lt] > MAX_ADIM) return fail(XTB_ERR_ARG, "%s: action dim %d > %d", fn, net->tsize[lt], MAX_ADIM);
@@ -2357,7 +2341,7 @@ extern "C" void xtb_muzero_destroy(xtb_muzero* m) {
 // shared argument checks of the MuZero entry points
 static int mz_check(const char* fn, const xtb_muzero* m, int batch) {
   if (!m) return fail(XTB_ERR_ARG, "%s: null object", fn);
-  if (g_comm || g_grad_hook) return fail(XTB_ERR_STATE, "%s: data-parallel training (gradient hook / communicator) is not supported", fn);
+  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
   if (batch < 1 || batch > m->max_batch) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d]", fn, batch, m->max_batch);
   return XTB_OK;
 }
@@ -2566,7 +2550,7 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
   if (q_tensor < 1 || q_tensor > nl || (int)target->L.size() != nl) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad head tensor");
   if (n_sample <= 0 || n_sample > net->max_batch || n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad batch");
   const int adim = net->tsize[q_tensor];
-  const float inv_world = g_comm ? 1.f / g_comm->world : 1.f;
+  const float inv_world = dp_inv_world();
   const bool fuse = dueling_fusable(net, q_tensor);
   return run_graph(capture_key(kDqnTrain, net, target, opt, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
                                n_sample, gamma, huber_delta, q_tensor),

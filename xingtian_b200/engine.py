@@ -353,35 +353,3 @@ class GradComm(object):
             check(self.lib.xtb_set_grad_comm(None))
             self.lib.xtb_comm_destroy(self.handle)
             self.handle = C.c_void_p()
-
-
-class GradAllReduce(object):
-    """Data-parallel learner (SURVEY 8(e)): one process per GPU, every rank holds the rollouts of its
-    own envs, gradients of the flat bucket are summed over ranks with NCCL between backward and the
-    optimiser (weights stay replicated because every rank applies the same clipped Adam update)."""
-
-    _active = None
-
-    def __init__(self, net, group=None):
-        import torch.distributed as dist
-        self.dist, self.group, self.net = dist, group, net
-        self.world = dist.get_world_size(group)
-
-        def hook(user, grads, count, stream):
-            try:
-                if not grads:
-                    return self.world
-                self.dist.all_reduce(self.net.grads, op=self.dist.ReduceOp.SUM, group=self.group)
-                return 0
-            except Exception:   # never unwind through C
-                import traceback
-                traceback.print_exc()
-                return -1
-
-        self._cb = capi.GRAD_HOOK(hook)
-        check(capi.lib().xtb_set_grad_hook(self._cb, None))
-        GradAllReduce._active = self
-
-    def close(self):
-        check(capi.lib().xtb_set_grad_hook(C.cast(None, capi.GRAD_HOOK), None))
-        GradAllReduce._active = None
