@@ -230,7 +230,10 @@ static uint32_t build_conv_tables(LayerPlan& lp) {
   return max_count;
 }
 
-struct PendingRed { bp::RedSeg s; };
+// Which forms of a tensor's value, and of its gradient, hold the current data: bits of the fp32 row-major buffer and
+// of the batch-planar planes.  Tensor 0 is the observation: its planes are the decoded-frame canvas.
+enum Form : uint8_t { kNone = 0, kF32 = 1, kPlanes = 2, kBoth = 3 };
+struct TensorForms { uint8_t val = kNone, grad = kNone; };
 
 struct xtb_net {
   xtb_net_desc desc;
@@ -250,9 +253,7 @@ struct xtb_net {
   std::vector<bp::BlobSeg> blob_segs;
   bool any_tc = false;
   float* params = nullptr; float* grads = nullptr; char* ws = nullptr;
-  // which representation of every tensor / tensor gradient is current
-  std::vector<char> f32_ok, bp_ok, gf32_ok, gbp_ok;
-  bool obs_bp_ok = false;
+  std::vector<TensorForms> cur;           // per tensor: changed only by wrote() / invalidate() / ensure_f32 / ensure_bp
   std::vector<bp::RedSeg> pending;        // ordered reductions queued by the running backward pass
 };
 
@@ -276,11 +277,23 @@ static inline bp::BpT out_bp(const xtb_net* n, int t) { return bp::BpT{(bp::bf16
 static inline bp::BpT gout_bp(const xtb_net* n, int t) { return bp::BpT{(bp::bf16*)(n->ws + n->gbp_off[t]), n->plane_elems[t], n->pitch}; }
 static inline bp::BpT obs_bp(const xtb_net* n) { return bp::BpT{(bp::bf16*)(n->ws + n->obs_bp_off), 0, n->pitch}; }
 static inline bp::BpT no_bp() { return bp::BpT{nullptr, 0, 0}; }
+// fp32 row-major value / gradient of tensor t, [max_batch][tsize]
+static inline float* out_f32(const xtb_net* n, int t) { return (float*)(n->ws + n->out_off[t]); }
+static inline float* gout_f32(const xtb_net* n, int t) { return (float*)(n->ws + n->gout_off[t]); }
 // retained pre-activation of tensor t, [max_batch][tsize] fp32; NULL unless its layer's activation keeps it (act_keeps_z)
 static inline float* z_buf(const xtb_net* n, int t) { return n->z_off[t] ? (float*)(n->ws + n->z_off[t]) : nullptr; }
 // where the GEMM of a layer with an activation past tanh (act_is_ext) writes its pre-activation: the retained buffer, or
 // the fp32 output that act_fwd_kernel then overwrites in place
-static inline float* pre_buf(const xtb_net* n, int t) { float* z = z_buf(n, t); return z ? z : (float*)(n->ws + n->out_off[t]); }
+static inline float* pre_buf(const xtb_net* n, int t) { float* z = z_buf(n, t); return z ? z : out_f32(n, t); }
+
+// the forms of tensor t's value (or gradient) that are current
+static inline uint8_t forms(const xtb_net* n, int t, bool grad) { return grad ? n->cur[t].grad : n->cur[t].val; }
+// the forms f of tensor t's value (or gradient) were just written: every other form is stale
+static inline void wrote(xtb_net* n, int t, bool grad, Form f) { (grad ? n->cur[t].grad : n->cur[t].val) = f; }
+// nothing of the values / of the gradients of any tensor is current
+static void invalidate(xtb_net* n, bool values, bool grads) {
+  for (TensorForms& c : n->cur) { if (values) c.val = kNone; if (grads) c.grad = kNone; }
+}
 static inline const bp::bf16* blob_hi(const xtb_net* n, const LayerPlan& lp) { return (const bp::bf16*)(n->ws + n->blob_off) + lp.blob_off; }
 static inline bool use_tc(const LayerPlan& lp) { return g_tc_mode && lp.tc; }
 
@@ -550,7 +563,6 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   for (auto& lp : net->L) if (lp.tc) {
     if (lp.d.kind == XTB_CONV) {
       lp.part_off = w; w += align_up((size_t)kSMs * lp.R * 128 * lp.N * sizeof(float), 256);
-    } else {
     }
     lp.dbpart_off = w; w += align_up((size_t)kSMs * 64 * sizeof(float), 256);
   }
@@ -579,12 +591,11 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   net->heads_part_off = w; w += align_up((size_t)kSMs * (512 * 8 + 3 * 512 + 16) * sizeof(float), 256);
   net->segs_off = w; w += align_up(sizeof(bp::BlobSeg) * XTB_MAX_LAYERS, 256);
   net->ws_bytes = w;
-  net->f32_ok.assign(nt, 0); net->bp_ok.assign(nt, 0); net->gf32_ok.assign(nt, 0); net->gbp_ok.assign(nt, 0);
+  net->cur.assign(nt, TensorForms{});
   *out = net;
   return XTB_OK;
 }
 
-static void drop_graphs_of(const void* obj);
 extern "C" void xtb_net_destroy(xtb_net* net) {
   if (!net) return;
   drop_graphs_of(net);
@@ -662,9 +673,7 @@ extern "C" int xtb_net_bind_stream(xtb_net* net, float* params, float* grads, vo
     CUDA_TRY(up(lp.dg_un_off, lp.dg_un.data(), lp.dg_un.size() * sizeof(bp::UnitEnt)));
     CUDA_TRY(up(lp.wg_off, lp.wg_tab.data(), lp.wg_tab.size() * sizeof(bp::WgEnt)));
   }
-  std::fill(net->f32_ok.begin(), net->f32_ok.end(), 0); std::fill(net->bp_ok.begin(), net->bp_ok.end(), 0);
-  std::fill(net->gf32_ok.begin(), net->gf32_ok.end(), 0); std::fill(net->gbp_ok.begin(), net->gbp_ok.end(), 0);
-  net->obs_bp_ok = false;
+  invalidate(net, true, true);
   int rc = xtb_net_sync_weights(net, stream);
   if (rc) return rc;
   // the segment table came from pageable host memory of this call: do not return before it is on the device
@@ -677,11 +686,11 @@ extern "C" int xtb_net_bind(xtb_net* net, float* params, float* grads, void* wor
 
 extern "C" float* xtb_net_tensor(xtb_net* net, int t) {
   if (!net || !net->ws || t < 1 || t >= (int)net->tsize.size()) return nullptr;
-  return (float*)(net->ws + net->out_off[t]);
+  return out_f32(net, t);
 }
 extern "C" float* xtb_net_tensor_grad(xtb_net* net, int t) {
   if (!net || !net->ws || t < 1 || t >= (int)net->tsize.size()) return nullptr;
-  return (float*)(net->ws + net->gout_off[t]);
+  return gout_f32(net, t);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -724,42 +733,61 @@ static void launch_gemm(const AL& al, const BL& bl, const EP& ep, int M, int N, 
 // ------------------------------------------------------------------------------------------
 // tensor-core launches
 // ------------------------------------------------------------------------------------------
+// Every instantiation of the kernel families that are chosen at run time, written once: the launches pick from these
+// tables and ensure_kernel_attrs opts all of them in to the large shared-memory carve-out.
+// The accumulator width is a template parameter of the GEMM kernels (wgmma takes N as an immediate): entry N / 16 - 1.
+template <int KIND>
+static void (*const kRowsKernels[])(bp::RowsArgs, int, int, int, int) = {
+    bp::bp_rows_kernel<KIND, 16>, bp::bp_rows_kernel<KIND, 32>, bp::bp_rows_kernel<KIND, 48>, bp::bp_rows_kernel<KIND, 64>};
+static void (*const kWgradKernels[])(bp::WgradArgs) = {bp::bp_wgrad_kernel<16>, bp::bp_wgrad_kernel<32>,
+                                                       bp::bp_wgrad_kernel<48>, bp::bp_wgrad_kernel<64>};
+template <class F, size_t C>
+static F by_width(F const (&tab)[C], int n) { return n > 0 && n % 16 == 0 && n / 16 <= (int)C ? tab[n / 16 - 1] : nullptr; }
+
+// Fused-heads instantiations, in the order they are tried: an entry covers K hidden units with K / 32 <= kpl per lane
+// and A <= amax actions
+template <class F> struct HeadsEnt { int kpl, amax; F kern; };
+template <class LOSS>
+static const HeadsEnt<void (*)(PpoHeadsArgs)> kHeadsKernels[] = {
+    {2, 8, heads_kernel<LOSS, 2, 8>}, {8, 4, heads_kernel<LOSS, 8, 4>}, {8, 8, heads_kernel<LOSS, 8, 8>},
+    {16, 4, heads_kernel<LOSS, 16, 4>}};
+template <class DIST>
+static const HeadsEnt<decltype(&infer_heads_kernel<DIST, 2, 8>)> kInferHeadsKernels[] = {
+    {2, 8, infer_heads_kernel<DIST, 2, 8>}, {8, 4, infer_heads_kernel<DIST, 8, 4>}, {8, 8, infer_heads_kernel<DIST, 8, 8>},
+    {16, 8, infer_heads_kernel<DIST, 16, 8>}};
+template <class E, size_t C>
+static const E* heads_pick(const E (&tab)[C], int K, int A) {
+  for (const E& e : tab)
+    if (K / 32 <= e.kpl && A <= e.amax) return &e;
+  return nullptr;
+}
+// an instantiation covers the heads (the same for every loss / distribution); infer: infer_heads_kernel
+static bool heads_fit(int K, int A, bool infer = false) {
+  return K % 32 == 0 && (infer ? heads_pick(kInferHeadsKernels<Categorical>, K, A) != nullptr
+                               : heads_pick(kHeadsKernels<PpoLoss>, K, A) != nullptr);
+}
+
 // opt-in to the large dynamic shared-memory carve-out, once per process and outside any stream capture
 static cudaError_t ensure_kernel_attrs() {
   static bool done = false;
   if (done) return cudaSuccess;
-  cudaError_t e;
-  const void* gemms[] = {
-      (const void*)bp::bp_rows_kernel<0, 16>, (const void*)bp::bp_rows_kernel<0, 32>, (const void*)bp::bp_rows_kernel<0, 48>,
-      (const void*)bp::bp_rows_kernel<0, 64>, (const void*)bp::bp_rows_kernel<1, 16>, (const void*)bp::bp_rows_kernel<1, 32>,
-      (const void*)bp::bp_rows_kernel<1, 48>, (const void*)bp::bp_rows_kernel<1, 64>, (const void*)bp::bp_rows_kernel<2, 16>,
-      (const void*)bp::bp_rows_kernel<2, 32>, (const void*)bp::bp_rows_kernel<2, 48>, (const void*)bp::bp_rows_kernel<2, 64>,
-      (const void*)bp::bp_wgrad_kernel<16>, (const void*)bp::bp_wgrad_kernel<32>, (const void*)bp::bp_wgrad_kernel<48>,
-      (const void*)bp::bp_wgrad_kernel<64>};
-  for (const void* k : gemms)
-    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  for (const void* k : {(const void*)heads_kernel<PpoLoss, 2, 8>, (const void*)heads_kernel<PpoLoss, 8, 4>,
-                        (const void*)heads_kernel<PpoLoss, 8, 8>, (const void*)heads_kernel<PpoLoss, 16, 4>,
-                        (const void*)heads_kernel<DuelingTdLoss, 2, 8>, (const void*)heads_kernel<DuelingTdLoss, 8, 4>,
-                        (const void*)heads_kernel<DuelingTdLoss, 8, 8>, (const void*)heads_kernel<DuelingTdLoss, 16, 4>,
-                        (const void*)heads_kernel<PpoGaussLoss, 2, 8>, (const void*)heads_kernel<PpoGaussLoss, 8, 4>,
-                        (const void*)heads_kernel<PpoGaussLoss, 8, 8>, (const void*)heads_kernel<PpoGaussLoss, 16, 4>})
-    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem)) != cudaSuccess) return e;
-  done = true;
-  return cudaSuccess;
+  cudaError_t e = cudaSuccess;
+  auto opt_in = [&](const void* k) { if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem); };
+  for (auto k : kRowsKernels<0>) opt_in((const void*)k);
+  for (auto k : kRowsKernels<1>) opt_in((const void*)k);
+  for (auto k : kRowsKernels<2>) opt_in((const void*)k);
+  for (auto k : kWgradKernels) opt_in((const void*)k);
+  for (const auto& h : kHeadsKernels<PpoLoss>) opt_in((const void*)h.kern);
+  for (const auto& h : kHeadsKernels<DuelingTdLoss>) opt_in((const void*)h.kern);
+  for (const auto& h : kHeadsKernels<PpoGaussLoss>) opt_in((const void*)h.kern);
+  done = e == cudaSuccess;
+  return e;
 }
 
-// the accumulator width is a template parameter of the GEMM kernels (wgmma takes N as an immediate)
 template <int KIND>
 static cudaError_t launch_rows(bp::RowsArgs& a, cudaStream_t st) {
-  void (*kern)(bp::RowsArgs, int, int, int, int);
-  switch (a.N) {
-    case 16: kern = bp::bp_rows_kernel<KIND, 16>; break;
-    case 32: kern = bp::bp_rows_kernel<KIND, 32>; break;
-    case 48: kern = bp::bp_rows_kernel<KIND, 48>; break;
-    case 64: kern = bp::bp_rows_kernel<KIND, 64>; break;
-    default: return cudaErrorInvalidValue;
-  }
+  const auto kern = by_width(kRowsKernels<KIND>, a.N);
+  if (!kern) return cudaErrorInvalidValue;
   { cudaError_t e0 = ensure_kernel_attrs(); if (e0 != cudaSuccess) return e0; }
   const int epi_planes = KIND == 2 ? bp::dgrad_epi_planes(a.src_act, a.accumulate) : 0;
   const RowsSmem m = rows_smem(a.w_res != 0, a.w_res_chunks, a.w_pitch, a.mode, (size_t)a.n_stage_ents, (size_t)a.n_units, a.N,
@@ -774,19 +802,29 @@ static cudaError_t launch_rows(bp::RowsArgs& a, cudaStream_t st) {
 
 // conv (mode 0): grid = R x slices, one accumulator per CTA
 static cudaError_t launch_wgrad(const bp::WgradArgs& a, int grid, cudaStream_t st) {
-  void (*kern)(bp::WgradArgs);
-  switch (a.N) {
-    case 16: kern = bp::bp_wgrad_kernel<16>; break;
-    case 32: kern = bp::bp_wgrad_kernel<32>; break;
-    case 48: kern = bp::bp_wgrad_kernel<48>; break;
-    case 64: kern = bp::bp_wgrad_kernel<64>; break;
-    default: return cudaErrorInvalidValue;
-  }
+  const auto kern = by_width(kWgradKernels, a.N);
+  if (!kern) return cudaErrorInvalidValue;
   { cudaError_t e0 = ensure_kernel_attrs(); if (e0 != cudaSuccess) return e0; }
   const size_t smem = wgrad_smem(a.mode, a.n_opix, a.R);
   if (smem > (size_t)kMaxDynSmem) return cudaErrorInvalidConfiguration;
   XLAUNCH(kern, grid, bp::WG_THREADS, (int)smem, st, a);
   return cudaPeekAtLastError();
+}
+
+// Queue the ordered reduction of n_slabs per-CTA slabs (stride `slab` floats, `count` of them each) into the gradient
+// bucket at dst_off, or at dst_ptr; flush_reductions runs the queue in one launch.  conv: the slabs are that conv
+// layer's weight-gradient accumulators [R][128][N], mapped back to its weight rows.
+static void queue_reduction(xtb_net* net, const float* part, int n_slabs, long long slab, int count, long long dst_off,
+                            float* dst_ptr = nullptr, const LayerPlan* conv = nullptr) {
+  bp::RedSeg r;
+  memset(&r, 0, sizeof r);
+  r.part = part; r.n_slabs = n_slabs; r.slab = slab; r.count = count; r.kind = conv ? 0 : 1;
+  r.dst_off = dst_off; r.dst_ptr = dst_ptr; r.alpha = 1.f;
+  if (conv) {
+    r.N = conv->N; r.C = conv->q.C; r.KW = conv->q.KW; r.mts = conv->mts; r.s2d_k4 = conv->s2d ? conv->k4 : 0;
+    r.alpha = conv->d.src == 0 ? net->desc.scale : 1.f;
+  }
+  net->pending.push_back(r);
 }
 
 // forward of a tensor-core layer.  want_f32: also store the fp32 row-major copy; want_bp: store the planes
@@ -801,7 +839,7 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   a.B = B; a.n_btiles = (B + 127) / 128; a.N = lp.n_fwd;
   const bool ext = act_is_ext(lp.d.act);      // linear into fp32; act_fwd_kernel follows (op_forward)
   a.out = want_bp && !ext ? out_bp(net, t) : no_bp();
-  a.out_f32 = ext ? pre_buf(net, t) : (want_f32 ? (float*)(net->ws + net->out_off[t]) : nullptr);
+  a.out_f32 = ext ? pre_buf(net, t) : (want_f32 ? out_f32(net, t) : nullptr);
   a.ld_f32 = net->tsize[t];
   a.bias = net->params + lp.b_off;
   a.alpha = lp.d.src == 0 ? net->desc.scale : 1.f;
@@ -875,14 +913,8 @@ static cudaError_t tc_wgrad(xtb_net* net, int i, int B, cudaStream_t st) {
     a.part = (float*)(net->ws + lp.part_off);
     // one wave: every accumulator gets the same number of CTAs, each adding a slice of the (pixel, sample chunk) list
     const int slices = std::max(1, std::min(kSMs / lp.R, a.n_opix * a.n_bsub));
-    const int grid = lp.R * slices;
-    bp::RedSeg r;
-    memset(&r, 0, sizeof r);
-    r.part = a.part; r.n_slabs = slices; r.slab = (long long)lp.R * 128 * lp.N; r.count = lp.R * 128 * lp.N; r.kind = 0;
-    r.N = lp.N; r.C = q.C; r.KW = q.KW; r.mts = lp.mts; r.s2d_k4 = lp.s2d ? lp.k4 : 0;
-    r.dst_off = lp.w_off; r.alpha = lp.d.src == 0 ? net->desc.scale : 1.f;
-    net->pending.push_back(r);
-    return launch_wgrad(a, grid, st);
+    queue_reduction(net, a.part, slices, (long long)lp.R * 128 * lp.N, lp.R * 128 * lp.N, lp.w_off, nullptr, &lp);
+    return launch_wgrad(a, lp.R * slices, st);
   }
   a.mode = 1;
   a.N = std::min(lp.n_fwd, 64);
@@ -907,29 +939,27 @@ extern "C" int xtb_net_sync_weights(xtb_net* net, void* stream) {
 
 // ---- representation changes ------------------------------------------------------------------
 static int ensure_bp(xtb_net* net, int t, int B, bool grad, cudaStream_t st) {
-  std::vector<char>& ok = grad ? net->gbp_ok : net->bp_ok;
-  if (ok[t]) return XTB_OK;
-  const std::vector<char>& f = grad ? net->gf32_ok : net->f32_ok;
-  if (!f[t]) return fail(XTB_ERR_STATE, "tensor %d has no current %s", t, grad ? "gradient" : "value");
-  const float* src = (const float*)(net->ws + (grad ? net->gout_off[t] : net->out_off[t]));
+  const uint8_t f = forms(net, t, grad);
+  if (f & kPlanes) return XTB_OK;
+  if (!(f & kF32)) return fail(XTB_ERR_STATE, "tensor %d has no current %s", t, grad ? "gradient" : "value");
+  const float* src = grad ? gout_f32(net, t) : out_f32(net, t);
   const int F = net->tsize[t], b_pad = (B + 15) & ~15;
   long long pieces = (long long)(F / 8) * b_pad;
   XLAUNCH(bp::bp_split_kernel, (unsigned)((pieces + 127) / 128), 128, 0, st, src, B, F, grad ? gout_bp(net, t) : out_bp(net, t));
   LAUNCH_CHECK();
-  ok[t] = 1;
+  wrote(net, t, grad, kBoth);
   return XTB_OK;
 }
 static int ensure_f32(xtb_net* net, int t, int B, bool grad, cudaStream_t st) {
-  std::vector<char>& ok = grad ? net->gf32_ok : net->f32_ok;
-  if (ok[t]) return XTB_OK;
-  const std::vector<char>& p = grad ? net->gbp_ok : net->bp_ok;
-  if (!p[t]) return fail(XTB_ERR_STATE, "tensor %d has no current %s", t, grad ? "gradient" : "value");
-  float* dst = (float*)(net->ws + (grad ? net->gout_off[t] : net->out_off[t]));
+  const uint8_t f = forms(net, t, grad);
+  if (f & kF32) return XTB_OK;
+  if (!(f & kPlanes)) return fail(XTB_ERR_STATE, "tensor %d has no current %s", t, grad ? "gradient" : "value");
+  float* dst = grad ? gout_f32(net, t) : out_f32(net, t);
   const int F = net->tsize[t];
   long long pieces = (long long)(F / 8) * B;
   XLAUNCH(bp::bp_merge_kernel, (unsigned)((pieces + 127) / 128), 128, 0, st, grad ? gout_bp(net, t) : out_bp(net, t), B, F, dst);
   LAUNCH_CHECK();
-  ok[t] = 1;
+  wrote(net, t, grad, kBoth);
   return XTB_OK;
 }
 
@@ -967,7 +997,6 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
     XLAUNCH(bp::bp_split_kernel, (unsigned)((pieces + 127) / 128), 128, 0, st, src, B_, F_, dst);
   };
   cudaError_t e = cudaSuccess;
-  int rc = XTB_OK;
   if (mode == 0 || mode == 1) {
     split(a, M, K, ta);
     // weight blob = batch-planar W^T with rows k: mode 0: b = W[K][N] -> rows K, features N.  mode 1: b = Bt[N][K]: the
@@ -1018,7 +1047,7 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
   cudaFree(pa); cudaFree(pw); cudaFree(pc); cudaFree(bias); cudaFree(part);
   if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "tc gemm launch: %s", cudaGetErrorString(e));
   if (e2 != cudaSuccess) return fail(XTB_ERR_CUDA, "tc gemm run: %s", cudaGetErrorString(e2));
-  return rc;
+  return XTB_OK;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1087,9 +1116,9 @@ __global__ void colsum_kernel(const float* __restrict__ dy, int M, int N, float*
 static int act_forward(xtb_net* net, int t, int B, cudaStream_t st) {
   const long long n = (long long)B * net->tsize[t];
   const unsigned blocks = (unsigned)std::min<long long>((n + 255) / 256, 8LL * kSMs);
-  XLAUNCH(act_fwd_kernel, blocks, 256, 0, st, (const float*)pre_buf(net, t), n, net->L[t - 1].d.act, (float*)(net->ws + net->out_off[t]));
+  XLAUNCH(act_fwd_kernel, blocks, 256, 0, st, (const float*)pre_buf(net, t), n, net->L[t - 1].d.act, out_f32(net, t));
   LAUNCH_CHECK();
-  net->f32_ok[t] = 1; net->bp_ok[t] = 0;
+  wrote(net, t, false, kF32);
   return XTB_OK;
 }
 // ... and in the backward pass: the gradient wrt its output, summed over its consumers, becomes the gradient wrt its
@@ -1099,22 +1128,19 @@ static int act_backward(xtb_net* net, int t, int B, cudaStream_t st) {
   int rc = ensure_f32(net, t, B, true, st);
   if (rc) return rc;
   const LayerPlan& lp = net->L[t - 1];
-  const float* u = z_buf(net, t) ? z_buf(net, t) : (const float*)(net->ws + net->out_off[t]);
+  const float* u = z_buf(net, t) ? z_buf(net, t) : out_f32(net, t);
   float* part = (float*)(net->ws + lp.act_part_off);
-  XLAUNCH(act_bwd_kernel, ACT_BWD_BLOCKS, ACT_BWD_THREADS, 0, st, (float*)(net->ws + net->gout_off[t]), u,
+  XLAUNCH(act_bwd_kernel, ACT_BWD_BLOCKS, ACT_BWD_THREADS, 0, st, gout_f32(net, t), u,
           (int)((long long)B * net->tsize[t] / lp.N), lp.N, lp.d.act, part);
   LAUNCH_CHECK();
-  bp::RedSeg r;
-  memset(&r, 0, sizeof r);
-  r.part = part; r.n_slabs = ACT_BWD_BLOCKS; r.slab = lp.N; r.count = lp.N; r.kind = 1; r.dst_off = lp.b_off; r.alpha = 1.f;
-  net->pending.push_back(r);
-  net->gf32_ok[t] = 1; net->gbp_ok[t] = 0;
+  queue_reduction(net, part, ACT_BWD_BLOCKS, lp.N, lp.N, lp.b_off);
+  wrote(net, t, true, kF32);
   return XTB_OK;
 }
 
 // uint8 frame decode (+ minibatch gather) into the space-to-depth observation canvas
 static int op_decode(xtb_net* net, const void* obs, const int32_t* idx, int B, cudaStream_t st) {
-  if (net->obs_bp_ok) return XTB_OK;
+  if (forms(net, 0, false) & kPlanes) return XTB_OK;
   const LayerPlan* first = nullptr;
   for (const auto& lp : net->L) if (lp.s2d && use_tc(lp)) { first = &lp; break; }
   if (!first) return XTB_OK;
@@ -1123,8 +1149,16 @@ static int op_decode(xtb_net* net, const void* obs, const int32_t* idx, int B, c
   XLAUNCH(bp::bp_decode_s2d_kernel, grid, bp::DEC_THREADS, smem, st, (const uint8_t*)obs, idx, B, net->desc.in_h, net->desc.in_w, net->H4,
           net->W4, first->g.padT, first->g.padL, net->desc.input_u8 == 2 ? 1 : 0, obs_bp(net));
   LAUNCH_CHECK();
-  net->obs_bp_ok = true;
+  wrote(net, 0, false, kPlanes);
   return XTB_OK;
+}
+
+// f(x) with the observation as the element type its loaders read: int8 (input_u8 == 2), uint8 (1) or float (0)
+template <class F>
+static void with_obs_type(const xtb_net* net, const void* obs, F&& f) {
+  if (net->desc.input_u8 == 2) f((const int8_t*)obs);
+  else if (net->desc.input_u8) f((const uint8_t*)obs);
+  else f((const float*)obs);
 }
 
 // forward of layer i; tc_allowed = parameters are the bound ones (their blobs are current)
@@ -1132,7 +1166,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
                       bool want_f32, cudaStream_t st) {
   const LayerPlan& lp = net->L[i];
   const int t = i + 1;
-  float* out = (float*)(net->ws + net->out_off[t]);
+  float* out = out_f32(net, t);
   const bool ext = act_is_ext(lp.d.act);
   float* pre = ext ? pre_buf(net, t) : out;      // the fp32 kernels write the activation, or the pre-activation (ext)
   const float* w = P + lp.w_off;
@@ -1142,10 +1176,10 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
     int rc = ensure_f32(net, lp.d.src, B, false, st);
     if (!rc) rc = ensure_f32(net, lp.d.k, B, false, st);
     if (rc) return rc;
-    XLAUNCH(dueling_fwd_kernel, (B + 7) / 8, 256, 0, st, (const float*)(net->ws + net->out_off[lp.d.src]),
-            (const float*)(net->ws + net->out_off[lp.d.k]), B, lp.out_size, out);
+    XLAUNCH(dueling_fwd_kernel, (B + 7) / 8, 256, 0, st, (const float*)out_f32(net, lp.d.src), (const float*)out_f32(net, lp.d.k), B,
+            lp.out_size, out);
     LAUNCH_CHECK();
-    net->f32_ok[t] = 1; net->bp_ok[t] = 0;
+    wrote(net, t, false, kF32);
     return XTB_OK;
   }
   if (tc_allowed && use_tc(lp)) {
@@ -1156,31 +1190,23 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
     if (te != cudaSuccess) return fail(XTB_ERR_CUDA, "tensor-core forward launch (layer %d): %s", i, cudaGetErrorString(te));
     g_launches.fetch_add(nl, std::memory_order_relaxed);
     if (ext) return act_forward(net, t, B, st);
-    net->bp_ok[t] = 1; net->f32_ok[t] = want_f32 ? 1 : 0;
+    wrote(net, t, false, want_f32 ? kBoth : kPlanes);
     return XTB_OK;
   }
+  auto gemm = [&](auto x, const int32_t* ix, float alpha) {
+    if (lp.d.kind == XTB_CONV) conv_fwd(lp, x, ix, w, b, alpha, pre, B, st);
+    else dense_fwd(lp, x, ix, w, b, alpha, pre, B, st);
+  };
   if (lp.d.src == 0) {
-    float alpha = net->desc.scale;
-    if (net->desc.input_u8 == 2) {
-      if (lp.d.kind == XTB_CONV) conv_fwd<int8_t>(lp, (const int8_t*)obs, idx, w, b, alpha, pre, B, st);
-      else dense_fwd<int8_t>(lp, (const int8_t*)obs, idx, w, b, alpha, pre, B, st);
-    } else if (net->desc.input_u8) {
-      if (lp.d.kind == XTB_CONV) conv_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
-      else dense_fwd<uint8_t>(lp, (const uint8_t*)obs, idx, w, b, alpha, pre, B, st);
-    } else {
-      if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, pre, B, st);
-      else dense_fwd<float>(lp, (const float*)obs, idx, w, b, alpha, pre, B, st);
-    }
+    with_obs_type(net, obs, [&](auto x) { gemm(x, idx, net->desc.scale); });
   } else {
     int rc = ensure_f32(net, lp.d.src, B, false, st);
     if (rc) return rc;
-    const float* x = (const float*)(net->ws + net->out_off[lp.d.src]);
-    if (lp.d.kind == XTB_CONV) conv_fwd<float>(lp, x, nullptr, w, b, 1.f, pre, B, st);
-    else dense_fwd<float>(lp, x, nullptr, w, b, 1.f, pre, B, st);
+    gemm((const float*)out_f32(net, lp.d.src), nullptr, 1.f);
   }
   LAUNCH_CHECK();
   if (ext) return act_forward(net, t, B, st);
-  net->f32_ok[t] = 1; net->bp_ok[t] = 0;
+  wrote(net, t, false, kF32);
   return XTB_OK;
 }
 
@@ -1190,57 +1216,42 @@ static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, in
   int t = i + 1;
   float* dw = net->grads + lp.w_off;
   float* db = net->grads + lp.b_off;
-  if (use_tc(lp)) {
+  const bool tc = use_tc(lp);
+  if (tc) {
     int rc = ensure_bp(net, t, B, true, st);
     if (rc) return rc;
     rc = lp.d.src == 0 ? op_decode(net, obs, idx, B, st) : ensure_bp(net, lp.d.src, B, false, st);
     if (rc) return rc;
     cudaError_t te = tc_wgrad(net, i, B, st);
     if (te != cudaSuccess) return fail(XTB_ERR_CUDA, "tensor-core wgrad launch (layer %d): %s", i, cudaGetErrorString(te));
-    LAUNCH_CHECK();
-    if (!bias_done) {   // bias gradient = column sums of dY over samples (and pixels); from the fp32 copy when it is current
-      if (net->gf32_ok[t]) {
-        int Mb = lp.d.kind == XTB_CONV ? B * lp.g.P : B;
-        dim3 gridb((lp.N + 31) / 32, (Mb + 1023) / 1024);
-        XLAUNCH(colsum_kernel, gridb, 256, 0, st, (const float*)(net->ws + net->gout_off[t]), Mb, lp.N, db);
-      } else {
-        XLAUNCH(bp::bp_colsum_kernel, (net->tsize[t] / 8 + 3) / 4, 128, 0, st, gout_bp(net, t), B, net->tsize[t], lp.N, db);
-      }
-      LAUNCH_CHECK();
-    }
-    return XTB_OK;
-  }
-  int rc = ensure_f32(net, t, B, true, st);
-  if (rc) return rc;
-  const float* dy = (const float*)(net->ws + net->gout_off[t]);
-  bool need_colsum = false;
-  if (lp.d.src == 0) {
-    float alpha = net->desc.scale;
-    if (net->desc.input_u8 == 2) {
-      if (lp.d.kind == XTB_CONV) conv_wgrad<int8_t>(lp, (const int8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-      else dense_wgrad<int8_t>(lp, (const int8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-    } else if (net->desc.input_u8) {
-      if (lp.d.kind == XTB_CONV) conv_wgrad<uint8_t>(lp, (const uint8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-      else dense_wgrad<uint8_t>(lp, (const uint8_t*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-    } else {
-      if (lp.d.kind == XTB_CONV) conv_wgrad<float>(lp, (const float*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-      else dense_wgrad<float>(lp, (const float*)obs, idx, dy, alpha, dw, B, st, !bias_done);
-    }
-    need_colsum = alpha != 1.f;
   } else {
-    rc = ensure_f32(net, lp.d.src, B, false, st);
+    int rc = ensure_f32(net, t, B, true, st);
     if (rc) return rc;
-    const float* x = (const float*)(net->ws + net->out_off[lp.d.src]);
-    if (lp.d.kind == XTB_CONV) conv_wgrad<float>(lp, x, nullptr, dy, 1.f, dw, B, st, !bias_done);
-    else dense_wgrad<float>(lp, x, nullptr, dy, 1.f, dw, B, st, !bias_done);
+    const float* dy = gout_f32(net, t);
+    auto gemm = [&](auto x, const int32_t* ix, float alpha) {
+      if (lp.d.kind == XTB_CONV) conv_wgrad(lp, x, ix, dy, alpha, dw, B, st, !bias_done);
+      else dense_wgrad(lp, x, ix, dy, alpha, dw, B, st, !bias_done);
+    };
+    if (lp.d.src == 0) {
+      with_obs_type(net, obs, [&](auto x) { gemm(x, idx, net->desc.scale); });
+    } else {
+      rc = ensure_f32(net, lp.d.src, B, false, st);
+      if (rc) return rc;
+      gemm((const float*)out_f32(net, lp.d.src), nullptr, 1.f);
+    }
   }
   LAUNCH_CHECK();
-  if (need_colsum && !bias_done) {   // bias gradient = column sums of dY
+  // bias gradient = column sums of dY over samples (and pixels), from the fp32 copy when it is current.  The fp32 GEMM
+  // adds it as one more row unless it scales its input (the observation's decode scale).
+  if (bias_done || (!tc && (lp.d.src != 0 || net->desc.scale == 1.f))) return XTB_OK;
+  if (forms(net, t, true) & kF32) {
     int Mb = lp.d.kind == XTB_CONV ? B * lp.g.P : B;
     dim3 gridb((lp.N + 31) / 32, (Mb + 1023) / 1024);
-    XLAUNCH(colsum_kernel, gridb, 256, 0, st, dy, Mb, lp.N, db);
-    LAUNCH_CHECK();
+    XLAUNCH(colsum_kernel, gridb, 256, 0, st, (const float*)gout_f32(net, t), Mb, lp.N, db);
+  } else {
+    XLAUNCH(bp::bp_colsum_kernel, (net->tsize[t] / 8 + 3) / 4, 128, 0, st, gout_bp(net, t), B, net->tsize[t], lp.N, db);
   }
+  LAUNCH_CHECK();
   return XTB_OK;
 }
 
@@ -1257,11 +1268,10 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
     if (!rc && acc) rc = ensure_f32(net, s, B, true, st);
     if (!rc && acc2) rc = ensure_f32(net, s2, B, true, st);
     if (rc) return rc;
-    XLAUNCH(dueling_dgrad_kernel, (B + 7) / 8, 256, 0, st, (const float*)(net->ws + net->gout_off[t]),
-            (const float*)(net->ws + net->out_off[s]), (const float*)(net->ws + net->out_off[s2]), B, lp.out_size, lp.src_act,
-            lp.adv_act, acc, acc2, (float*)(net->ws + net->gout_off[s]), (float*)(net->ws + net->gout_off[s2]));
+    XLAUNCH(dueling_dgrad_kernel, (B + 7) / 8, 256, 0, st, (const float*)gout_f32(net, t), (const float*)out_f32(net, s),
+            (const float*)out_f32(net, s2), B, lp.out_size, lp.src_act, lp.adv_act, acc, acc2, gout_f32(net, s), gout_f32(net, s2));
     LAUNCH_CHECK();
-    net->gf32_ok[s] = net->gf32_ok[s2] = 1; net->gbp_ok[s] = net->gbp_ok[s2] = 0;
+    wrote(net, s, true, kF32); wrote(net, s2, true, kF32);
     return XTB_OK;
   }
   if (use_tc(lp)) {
@@ -1275,13 +1285,9 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
     LAUNCH_CHECK();
     if (fuse_db) {
       const int units = lp.d.kind == XTB_CONV ? lp.q.H * lp.q.W : lp.K / lp.n_dg;
-      bp::RedSeg r;
-      memset(&r, 0, sizeof r);
-      r.part = dbp; r.n_slabs = std::min(kSMs, units * ((B + 127) / 128)); r.slab = lp.n_dg; r.count = lp.n_dg; r.kind = 1;
-      r.dst_off = net->L[s - 1].b_off; r.alpha = 1.f;
-      net->pending.push_back(r);
+      queue_reduction(net, dbp, std::min(kSMs, units * ((B + 127) / 128)), lp.n_dg, lp.n_dg, net->L[s - 1].b_off);
     }
-    net->gbp_ok[s] = 1; net->gf32_ok[s] = 0;
+    wrote(net, s, true, kPlanes);
     return XTB_OK;
   }
   int rc = ensure_f32(net, t, B, true, st);
@@ -1289,9 +1295,9 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
   rc = ensure_f32(net, s, B, false, st);
   if (rc) return rc;
   if (acc) { rc = ensure_f32(net, s, B, true, st); if (rc) return rc; }
-  const float* dy = (const float*)(net->ws + net->gout_off[t]);
-  const float* x = (const float*)(net->ws + net->out_off[s]);
-  float* gsrc = (float*)(net->ws + net->gout_off[s]);
+  const float* dy = gout_f32(net, t);
+  const float* x = out_f32(net, s);
+  float* gsrc = gout_f32(net, s);
   const float* w = net->params + lp.w_off;
   if (lp.d.kind == XTB_CONV) {
     ADgrad al{dy, lp.g, lp.dkyx, lp.dco, lp.sshift};
@@ -1305,7 +1311,7 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
     launch_gemm(al, bl, ep, B, lp.K, lp.N, false, st);
   }
   LAUNCH_CHECK();
-  net->gf32_ok[s] = 1; net->gbp_ok[s] = 0;
+  wrote(net, s, true, kF32);
   return XTB_OK;
 }
 
@@ -1343,8 +1349,7 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
   const bool tc_allowed = (P == net->params);   // foreign parameters have no weight blobs: fp32 kernels
   cudaStream_t st = S(stream);
   const int nl = (int)net->L.size();
-  net->obs_bp_ok = false;
-  for (int t = 1; t <= nl; t++) { net->f32_ok[t] = net->bp_ok[t] = 0; }
+  invalidate(net, true, false);
   for (int i = 0; i < nl; i++) {
     if (skip_mask & (1u << i)) continue;
     const LayerPlan& lp = net->L[i];
@@ -1366,13 +1371,24 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
   return XTB_OK;
 }
 
-static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
-                             const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
-                             unsigned bias_done_tensors = 0u, unsigned heads_bp_mask = 0u, xtb_comm* comm = nullptr,
-                             unsigned heads_dy_mask = 0u, float* dobs = nullptr);
+// What a backward pass starts from and does besides the layers' gradients.  Bit t of a mask stands for tensor t, bit i
+// of skip for layer i.
+struct BackwardOpts {
+  const int32_t* heads; int n_heads;   // tensors whose gradient the caller filled: fp32 row-major, wrt the pre-activation
+  unsigned heads_bp = 0u;              // ... of these, the ones filled in planes
+  unsigned heads_dy = 0u;              // ... the ones (layers with an activation past tanh) filled wrt the output
+  unsigned skip = 0u;                  // layers that are not run
+  bool zero_grads = true;              // zero the gradient bucket and drop queued reductions (else a fused loss kernel queued its own)
+  unsigned bias_done = 0u;             // tensors whose layer's bias gradient is already queued
+  float* dobs = nullptr;               // also d loss / d observation, into dobs
+  bool all_reduce = false;             // sum the gradient bucket over g_comm when one is installed
+  BackwardOpts(const int32_t* h, int n) : heads(h), n_heads(n) {}
+};
+static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch, void* stream,
+                             const BackwardOpts& o);
 extern "C" int xtb_net_backward(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                                 const int32_t* head_tensors, int n_heads, void* stream) {
-  return net_backward_impl(net, obs, gather_idx, batch, head_tensors, n_heads, stream, 0u, true);
+  return net_backward_impl(net, obs, gather_idx, batch, stream, BackwardOpts(head_tensors, n_heads));
 }
 // d loss / d observation is defined for float observations that only dense layers read (decode scale 1)
 static int input_grad_check(const xtb_net* net) {
@@ -1385,48 +1401,46 @@ static int input_grad_check(const xtb_net* net) {
 extern "C" int xtb_net_backward_input(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
                                       const int32_t* head_tensors, int n_heads, float* dobs, void* stream) {
   if (!obs || !dobs || !head_tensors) return fail(XTB_ERR_ARG, "xtb_net_backward_input: null pointer");
-  return net_backward_impl(net, obs, gather_idx, batch, head_tensors, n_heads, stream, 0u, true, 0u, 0u, nullptr, 0u, dobs);
+  BackwardOpts o(head_tensors, n_heads); o.dobs = dobs;
+  return net_backward_impl(net, obs, gather_idx, batch, stream, o);
 }
-// head_tensors: tensors whose gradient was filled by the caller: fp32 row-major, or (bit set in heads_bp_mask) planes;
-// wrt the pre-activation, or (bit set in heads_dy_mask, a layer with an activation past tanh) wrt the output
-static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch,
-                             const int32_t* head_tensors, int n_heads, void* stream, unsigned skip_mask, bool zero_grads,
-                             unsigned bias_done_tensors, unsigned heads_bp_mask, xtb_comm* comm, unsigned heads_dy_mask,
-                             float* dobs) {
+static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gather_idx, int batch, void* stream,
+                             const BackwardOpts& o) {
   if (!net || !net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_net_backward: net not bound (grads required)");
   if (batch <= 0 || batch > net->max_batch) return fail(XTB_ERR_ARG, "batch out of range");
-  if (dobs) { int rc = input_grad_check(net); if (rc) return rc; }
+  if (o.dobs) { int rc = input_grad_check(net); if (rc) return rc; }
   cudaStream_t st = S(stream);
+  xtb_comm* comm = o.all_reduce ? g_comm : nullptr;
   const int nl = (int)net->L.size();
   std::vector<char> has_grad(nl + 1, 0), written(nl + 1, 0);
   std::vector<char> dy(nl + 1, 0);          // the gradient is wrt the output of an act_is_ext layer: act_backward pending
   long long early_off = 0, early_cnt = 0;
-  for (int t = 1; t <= nl; t++) net->gf32_ok[t] = net->gbp_ok[t] = 0;
-  if (zero_grads) net->pending.clear();      // a fused loss kernel (zero_grads == false) has queued its own reductions
-  for (int h = 0; h < n_heads; h++) {
-    int t = head_tensors[h];
+  invalidate(net, false, true);
+  if (o.zero_grads) net->pending.clear();
+  for (int h = 0; h < o.n_heads; h++) {
+    int t = o.heads[h];
     if (t < 1 || t > nl || net->tsize[t] == 0) return fail(XTB_ERR_ARG, "bad head tensor %d", t);
-    has_grad[t] = 1; written[t] = 1; dy[t] = (heads_dy_mask >> t) & 1u;
-    if ((heads_bp_mask >> t) & 1u) net->gbp_ok[t] = 1; else net->gf32_ok[t] = 1;
+    has_grad[t] = 1; written[t] = 1; dy[t] = (o.heads_dy >> t) & 1u;
+    wrote(net, t, true, (o.heads_bp >> t) & 1u ? kPlanes : kF32);
   }
-  if (zero_grads) CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), st));
+  if (o.zero_grads) CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), st));
   // bias-gradient fusion: the bias gradient of the layer producing tensor s is the column sum of gout(s); when s has
   // exactly one consumer and that consumer's tensor-core data-gradient tile spans exactly the bias vector, its
   // epilogue accumulates the column sums (ordered partial sums, no atomics) and the separate pass is dropped
   std::vector<char> fuse_bias(nl + 1, 0);
   for (int s = 1; s <= nl; s++) {
-    if (bias_done_tensors & (1u << s)) { fuse_bias[s] = 2; continue; }
+    if (o.bias_done & (1u << s)) { fuse_bias[s] = 2; continue; }
     const LayerPlan& ps = net->L[s - 1];
     if (act_is_ext(ps.d.act)) continue;       // the column sums would be of the gradient wrt the output
     int consumers = 0, cj = -1;
-    for (int j = 0; j < nl; j++) if (reads(net->L[j], s) && !(skip_mask & (1u << j))) { consumers++; cj = j; }
+    for (int j = 0; j < nl; j++) if (reads(net->L[j], s) && !(o.skip & (1u << j))) { consumers++; cj = j; }
     if (consumers != 1) continue;
     const LayerPlan& c = net->L[cj];
     if (!use_tc(c)) continue;
     if (ps.d.kind == XTB_CONV ? c.n_dg == ps.N : (c.d.kind == XTB_DENSE && c.n_dg == ps.N && c.K == ps.N)) fuse_bias[s] = 1;
   }
   for (int i = nl - 1; i >= 0; i--) {
-    if (skip_mask & (1u << i)) continue;
+    if (o.skip & (1u << i)) continue;
     const LayerPlan& lp = net->L[i];
     int t = i + 1;
     if (!has_grad[t]) continue;   // tensor does not influence the loss
@@ -1453,23 +1467,23 @@ static int net_backward_impl(xtb_net* net, const void* obs, const int32_t* gathe
       written[s] = 1; has_grad[s] = 1; dy[s] = 1;
     }
   }
-  if (dobs) {   // d loss / d observation: the data-gradient GEMM of every dense layer reading it, summed in layer order
+  if (o.dobs) {   // d loss / d observation: the data-gradient GEMM of every dense layer reading it, summed in layer order
     bool first = true;
     for (int i = 0; i < nl; i++) {
       const LayerPlan& lp = net->L[i];
-      if (lp.d.src != 0 || lp.d.kind != XTB_DENSE || (skip_mask & (1u << i))) continue;
+      if (lp.d.src != 0 || lp.d.kind != XTB_DENSE || (o.skip & (1u << i))) continue;
       if (!has_grad[i + 1]) continue;
       int rc = ensure_f32(net, i + 1, batch, true, st);
       if (rc) return rc;
-      ADense<float> al{(const float*)(net->ws + net->gout_off[i + 1]), nullptr, lp.N};
+      ADense<float> al{(const float*)gout_f32(net, i + 1), nullptr, lp.N};
       BTransposed bl{net->params + lp.w_off, lp.N};
       // linear: the epilogue's activation source is never used (dobs stands in as a valid address)
-      EpiDgrad ep{dobs, dobs, 0, lp.K, first ? 0 : 1, nullptr, 0};
+      EpiDgrad ep{o.dobs, o.dobs, 0, lp.K, first ? 0 : 1, nullptr, 0};
       launch_gemm(al, bl, ep, batch, lp.K, lp.N, false, st);
       LAUNCH_CHECK();
       first = false;
     }
-    if (first) CUDA_TRY(cudaMemsetAsync(dobs, 0, (size_t)batch * net->tsize[0] * sizeof(float), st));
+    if (first) CUDA_TRY(cudaMemsetAsync(o.dobs, 0, (size_t)batch * net->tsize[0] * sizeof(float), st));
   }
   int rc = flush_reductions(net, st);
   if (rc || !comm || comm->world == 1) return rc;
@@ -1493,10 +1507,9 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
   if (layer < 0 || layer >= (int)net->L.size() || batch <= 0 || batch > net->max_batch) return fail(XTB_ERR_ARG, "bad layer/batch");
   cudaStream_t st = S(stream);
   // tensors the caller filled through xtb_net_tensor / xtb_net_tensor_grad are fp32 row-major
-  for (int t = 1; t <= (int)net->L.size(); t++) {
-    if (!net->f32_ok[t] && !net->bp_ok[t]) net->f32_ok[t] = 1;
-    if (!net->gf32_ok[t] && !net->gbp_ok[t]) net->gf32_ok[t] = 1;
-  }
+  for (int t = 1; t <= (int)net->L.size(); t++)
+    for (bool grad : {false, true})
+      if (forms(net, t, grad) == kNone) wrote(net, t, grad, kF32);
   if (which == 0) return op_forward(net, layer, net->params, true, obs, gather_idx, batch, false, st);
   if (which == 1) { int rc = op_wgrad(net, layer, obs, gather_idx, batch, st, true); net->pending.clear(); return rc; }
   if (which == 2) {
@@ -1505,7 +1518,7 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
     net->pending.clear();
     return rc;
   }
-  if (which == 3) { net->obs_bp_ok = false; return op_decode(net, obs, gather_idx, batch, st); }
+  if (which == 3) { wrote(net, 0, false, kNone); return op_decode(net, obs, gather_idx, batch, st); }   // decode again
   return fail(XTB_ERR_ARG, "xtb_net_bench_layer: which must be 0..3");
 }
 
@@ -1836,7 +1849,8 @@ enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKe
                 kGaussRolloutInfer, kMuzeroTrain, kMuzeroInitInfer, kMuzeroRecurInfer };
 struct CaptureKey {
   uint64_t tag;          // entry point
-  const void* own[6];    // net, target, opt, two more nets, comm: destroying one, or rebinding a net, drops the graph
+  const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
+                         // destroying one, or rebinding a net, drops the graph
   uint64_t mode[2];      // kernel-path and fused-heads modes
   uint64_t arg[21];      // every pointer and scalar argument; floats by bit pattern
   bool operator<(const CaptureKey& o) const { return memcmp(this, &o, sizeof(CaptureKey)) < 0; }
@@ -1846,12 +1860,14 @@ template <class T> static uint64_t key_word(T v) {
   else if constexpr (std::is_pointer_v<T>) return (uint64_t)(uintptr_t)v;
   else return (uint64_t)v;
 }
-template <class... A>
-static CaptureKey capture_key(GraphTag tag, const void* net, const void* target, const void* opt, A... args) {
+template <size_t N, class... A>
+static CaptureKey capture_key(GraphTag tag, const void* const (&owners)[N], A... args) {
+  static_assert(N < sizeof(CaptureKey::own) / sizeof(void*), "CaptureKey::own too small");
   static_assert(sizeof...(A) <= sizeof(CaptureKey::arg) / sizeof(uint64_t), "CaptureKey::arg too small");
   CaptureKey k;
   memset(&k, 0, sizeof k);
-  k.tag = tag; k.own[0] = net; k.own[1] = target; k.own[2] = opt;
+  k.tag = tag;
+  std::copy(owners, owners + N, k.own);
   const uint64_t w[] = {key_word(args)...};
   memcpy(k.arg, w, sizeof w);
   return k;
@@ -1908,29 +1924,6 @@ static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
   return sc.end();
 }
 
-// Fused-heads instantiations for K hidden units (K % 32 == 0) and A actions: heads_kernel (training) covers A <= 8 with
-// K <= 256 or A <= 4 with K <= 512; infer_heads_kernel (infer) covers A <= 8 with K <= 512
-static bool heads_fit(int K, int A, bool infer = false) {
-  const int kpl = K / 32;
-  return K % 32 == 0 && A <= 8 && (kpl <= 8 || (kpl <= 16 && (infer || A <= 4)));
-}
-template <class LOSS>
-static void launch_heads(const PpoHeadsArgs& a, int blocks, size_t shb, cudaStream_t st) {
-  const int kpl = a.K / 32;
-  if (kpl <= 2) XLAUNCH((heads_kernel<LOSS, 2, 8>), blocks, 256, shb, st, a);
-  else if (kpl <= 8 && a.A <= 4) XLAUNCH((heads_kernel<LOSS, 8, 4>), blocks, 256, shb, st, a);
-  else if (kpl <= 8) XLAUNCH((heads_kernel<LOSS, 8, 8>), blocks, 256, shb, st, a);
-  else XLAUNCH((heads_kernel<LOSS, 16, 4>), blocks, 256, shb, st, a);
-}
-template <class DIST, class... Args>
-static void launch_infer_heads(int K, int A, int blocks, cudaStream_t st, Args... args) {
-  const int kpl = K / 32;
-  if (kpl <= 2) XLAUNCH((infer_heads_kernel<DIST, 2, 8>), blocks, 256, 0, st, args...);
-  else if (kpl <= 8 && A <= 4) XLAUNCH((infer_heads_kernel<DIST, 8, 4>), blocks, 256, 0, st, args...);
-  else if (kpl <= 8) XLAUNCH((infer_heads_kernel<DIST, 8, 8>), blocks, 256, 0, st, args...);
-  else XLAUNCH((infer_heads_kernel<DIST, 16, 8>), blocks, 256, 0, st, args...);
-}
-
 // The epoch x minibatch loop of PPO.train (xt/model/ppo/ppo.py:111-132): minibatch k of epoch e holds rows
 // perm[e*N + k*B ...] (the last one ragged).  minibatch(idx, mb, loss) enqueues its forward, loss and backward; the
 // optimiser step follows.
@@ -1956,6 +1949,22 @@ static int ppo_epoch_loop(xtb_net* net, xtb_adam* opt, int N, int B, int E, cons
 // the gradients over ranks, else 1
 static float dp_inv_world() { return g_comm ? 1.f / g_comm->world : 1.f; }
 
+// What every learner entry point checks before it launches anything: none of the pointers it needs is NULL (`missing`:
+// each caller names its own), the net is bound with gradients, the optimiser spans the trained parameters (n_params,
+// 0: the net's; opt NULL: an inference call), the `rows` samples of one forward are in [1, max_rows] (0: the net's
+// max_batch) and, for a learner that cannot sum its gradients over ranks (dp_ok false), no communicator is installed.
+static int learner_check(const char* fn, bool missing, const xtb_net* net, const xtb_adam* opt, long long rows, bool dp_ok,
+                         long long max_rows = 0, long long n_params = 0) {
+  if (missing) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
+  if (!dp_ok && g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
+  if (opt && opt->count != (n_params ? n_params : net->n_params))
+    return fail(XTB_ERR_ARG, "%s: optimiser/net size mismatch (%lld != %lld)", fn, opt->count, n_params ? n_params : net->n_params);
+  if (!max_rows) max_rows = net->max_batch;
+  if (rows < 1 || rows > max_rows) return fail(XTB_ERR_ARG, "%s: batch %lld not in [1, %lld]", fn, rows, max_rows);
+  return XTB_OK;
+}
+
 // Fused PPO heads of tensors pi_t / v_t: both heads are linear dense layers on hidden (non-observation) tensors of equal
 // width within the heads_kernel limits (infer: the infer_heads_kernel limits), and the fused-heads mode is on
 static bool ppo_heads_fusable(const xtb_net* net, int pi_t, int v_t, bool infer) {
@@ -1980,8 +1989,8 @@ static int heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, i
   const int32_t* idx = a.idx;
   CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
   net->pending.clear();
-  a.h_pi = (const float*)(net->ws + net->out_off[lpi.d.src]); a.h_v = (const float*)(net->ws + net->out_off[lv.d.src]);
-  a.g_pi = (float*)(net->ws + net->gout_off[lpi.d.src]); a.g_v = (float*)(net->ws + net->gout_off[lv.d.src]);
+  a.h_pi = out_f32(net, lpi.d.src); a.h_v = out_f32(net, lv.d.src);
+  a.g_pi = gout_f32(net, lpi.d.src); a.g_v = gout_f32(net, lv.d.src);
   // hidden-layer gradients go straight into batch-planar planes when the hidden layer runs on tensor cores
   // (a hidden layer with an activation past tanh gets the gradient wrt its output, in fp32, and act_backward follows)
   const bool ext_pi = act_is_ext(lpi.src_act), ext_v = act_is_ext(lv.src_act);
@@ -1995,36 +2004,34 @@ static int heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, i
   auto only_feeds_heads = [&](int tsr) { for (int j = 0; j < (int)net->L.size(); j++) if (reads(net->L[j], tsr) && !(skip & (1u << j))) return false; return true; };
   bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src) && !ext_pi;
   bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src) && !ext_v;
-  unsigned bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
   a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = dgrad_act(lpi); a.act_v = dgrad_act(lv); a.shared = lpi.d.src == lv.d.src ? 1 : 0;
   int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
   const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2 + (LOSS::kLogStd ? adim : 0);
   a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
   size_t shb = (size_t)8 * nacc * sizeof(float);
   { cudaError_t ea = ensure_kernel_attrs(); if (ea != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel attributes: %s", cudaGetErrorString(ea)); }
-  launch_heads<LOSS>(a, blocks, shb, S(stream));
+  XLAUNCH(heads_pick(kHeadsKernels<LOSS>, a.K, a.A)->kern, blocks, 256, shb, S(stream), a);
   LAUNCH_CHECK();
   {   // ordered reduction of the per-block slabs (queued; runs with the other partial sums at the end of backward)
-    auto seg = [&](int off, int count, long long dst_off, float* dst_ptr) {
-      bp::RedSeg r;
-      memset(&r, 0, sizeof r);
-      r.part = a.part + off; r.n_slabs = blocks; r.slab = a.slab; r.count = count; r.kind = 1;
-      r.dst_off = dst_off; r.alpha = 1.f; r.dst_ptr = dst_ptr;
-      net->pending.push_back(r);
+    auto seg = [&](int off, int count, long long dst_off, float* dst_ptr = nullptr) {
+      queue_reduction(net, a.part + off, blocks, a.slab, count, dst_off, dst_ptr);
     };
-    seg(0, HK * adim, lpi.w_off, nullptr);
-    seg(HK * adim, HK, lv.w_off, nullptr);
-    if (bh_pi_ok) seg(HK * adim + HK, HK, net->L[lpi.d.src - 1].b_off, nullptr);
-    if (!a.shared && bh_v_ok) seg(HK * adim + 2 * HK, HK, net->L[lv.d.src - 1].b_off, nullptr);
-    seg(HK * adim + 3 * HK, adim, lpi.b_off, nullptr);
-    seg(HK * adim + 3 * HK + adim, 1, lv.b_off, nullptr);
+    seg(0, HK * adim, lpi.w_off);
+    seg(HK * adim, HK, lv.w_off);
+    if (bh_pi_ok) seg(HK * adim + HK, HK, net->L[lpi.d.src - 1].b_off);
+    if (!a.shared && bh_v_ok) seg(HK * adim + 2 * HK, HK, net->L[lv.d.src - 1].b_off);
+    seg(HK * adim + 3 * HK, adim, lpi.b_off);
+    seg(HK * adim + 3 * HK + adim, 1, lv.b_off);
     seg(HK * adim + 3 * HK + adim + 1, 1, 0, loss_dst);
-    if (LOSS::kLogStd) seg(HK * adim + 3 * HK + adim + 2, adim, ls_off, nullptr);
+    if (LOSS::kLogStd) seg(HK * adim + 3 * HK + adim + 2, adim, ls_off);
   }
-  int srcs[2] = {lpi.d.src, lv.d.src};
-  unsigned hbp = (bp_pi ? (1u << lpi.d.src) : 0u) | (bp_v ? (1u << lv.d.src) : 0u);   // the fused kernel wrote planes there
-  unsigned hdy = (ext_pi ? (1u << lpi.d.src) : 0u) | (ext_v ? (1u << lv.d.src) : 0u);
-  return net_backward_impl(net, obs, idx, mb, srcs, a.shared ? 1 : 2, stream, skip, false, bias_done, hbp, g_comm, hdy);
+  const int32_t srcs[2] = {lpi.d.src, lv.d.src};
+  BackwardOpts o(srcs, a.shared ? 1 : 2);
+  o.heads_bp = (bp_pi ? (1u << lpi.d.src) : 0u) | (bp_v ? (1u << lv.d.src) : 0u);   // the fused kernel wrote planes there
+  o.heads_dy = (ext_pi ? (1u << lpi.d.src) : 0u) | (ext_v ? (1u << lv.d.src) : 0u);
+  o.bias_done = (bh_pi_ok ? (1u << lpi.d.src) : 0u) | ((lpi.d.src != lv.d.src && bh_v_ok) ? (1u << lv.d.src) : 0u);
+  o.skip = skip; o.zero_grads = false; o.all_reduce = true;
+  return net_backward_impl(net, obs, idx, mb, stream, o);
 }
 
 // names and capture tags of the exported PPO calls of each action distribution
@@ -2047,7 +2054,7 @@ template <class DIST, class RO>
 static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, int B, int E, const int32_t* perm,
                             const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, float inv_world,
                             void* stream) {
-  int heads[2] = {pi_t, v_t};
+  const int32_t heads[2] = {pi_t, v_t};
   const int adim = net->tsize[pi_t];
   const long long ls_off = DIST::kLogStd ? net->L[ls_t - 1].w_off : -1;
   const LayerPlan& lpi = net->L[pi_t - 1];
@@ -2081,7 +2088,9 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, in
                              xtb_net_tensor_grad(net, v_t), step_loss, stream);
     }
     if (rc) return rc;
-    return net_backward_impl(net, ro->obs, idx, mb, heads, 2, stream, 0u, !DIST::kLogStd, 0u, 0u, g_comm);
+    BackwardOpts o(heads, 2);
+    o.zero_grads = !DIST::kLogStd; o.all_reduce = true;   // keep the log_std gradient the loss kernel stored
+    return net_backward_impl(net, ro->obs, idx, mb, stream, o);
   });
 }
 
@@ -2103,16 +2112,13 @@ template <class DIST, class RO>
 static int ppo_train(xtb_net* net, xtb_adam* opt, const RO* ro, int n_sample, int batch_size, int n_epoch, const int32_t* perm,
                      const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, int use_graph, void* stream) {
   const char* fn = PpoCalls<DIST>::train;
-  if (!net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v || !perm || !hp ||
-      !loss_per_step)
-    return fail(XTB_ERR_ARG, "%s: null pointer", fn);
-  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
-  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "%s: optimiser/net size mismatch", fn);
-  if (n_sample <= 0 || batch_size <= 0 || n_epoch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
-  if (std::min(batch_size, n_sample) > net->max_batch) return fail(XTB_ERR_ARG, "batch_size exceeds net max_batch");
+  const bool missing = !net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v ||
+                       !perm || !hp || !loss_per_step;
+  if (int rc = learner_check(fn, missing, net, opt, std::min(batch_size, n_sample), true)) return rc;
+  if (n_epoch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
   if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
   const float inv_world = dp_inv_world();
-  return run_graph(capture_key(PpoCalls<DIST>::train_tag, net, nullptr, opt, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
+  return run_graph(capture_key(PpoCalls<DIST>::train_tag, {net, opt}, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
                                loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
                                hp->critic_coef, pi_t, v_t, ls_t),
                    use_graph, stream, [&](void* st) {
@@ -2144,15 +2150,15 @@ extern "C" int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_ga
 extern "C" int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* gather_idx, const float* bp_logits,
                                 const int32_t* action, const uint8_t* done, const float* reward, int n_sample, int step_len,
                                 float gamma, int logit_tensor, int base_tensor, float* loss_out, int use_graph, void* stream) {
-  if (!net || !opt || !obs || !bp_logits || !action || !done || !reward || !loss_out) return fail(XTB_ERR_ARG, "xtb_impala_train: null pointer");
-  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "xtb_impala_train: net not bound");
+  const bool missing = !net || !opt || !obs || !bp_logits || !action || !done || !reward || !loss_out;
+  if (int rc = learner_check("xtb_impala_train", missing, net, opt, n_sample, true)) return rc;
   const int nl = (int)net->L.size();
   if (logit_tensor < 1 || logit_tensor > nl || base_tensor < 1 || base_tensor > nl || net->tsize[base_tensor] != 1)
     return fail(XTB_ERR_ARG, "xtb_impala_train: bad head tensors");
-  if (n_sample <= 0 || n_sample > net->max_batch || step_len < 2 || n_sample % step_len) return fail(XTB_ERR_ARG, "xtb_impala_train: bad sizes");
+  if (step_len < 2 || n_sample % step_len) return fail(XTB_ERR_ARG, "xtb_impala_train: bad sizes");
   const int adim = net->tsize[logit_tensor];
   if (adim > MAX_ADIM) return fail(XTB_ERR_ARG, "xtb_impala_train: action dim too large");
-  return run_graph(capture_key(kImpalaTrain, net, nullptr, opt, obs, gather_idx, bp_logits, action, done, reward, loss_out,
+  return run_graph(capture_key(kImpalaTrain, {net, opt}, obs, gather_idx, bp_logits, action, done, reward, loss_out,
                                n_sample, step_len, gamma, logit_tensor, base_tensor),
                    use_graph, stream, [&](void* st) -> int {
     int rc = net_forward_impl(net, nullptr, obs, gather_idx, n_sample, st, 0u, (1u << logit_tensor) | (1u << base_tensor));
@@ -2161,8 +2167,9 @@ extern "C" int xtb_impala_train(xtb_net* net, xtb_adam* opt, const void* obs, co
                               n_sample / step_len, step_len, adim, gamma, xtb_net_tensor_grad(net, logit_tensor),
                               xtb_net_tensor_grad(net, base_tensor), nullptr, nullptr, loss_out, st);
     if (rc) return rc;
-    int heads[2] = {logit_tensor, base_tensor};
-    rc = net_backward_impl(net, obs, gather_idx, n_sample, heads, 2, st, 0u, true, 0u, 0u, g_comm);
+    const int32_t heads[2] = {logit_tensor, base_tensor};
+    BackwardOpts o(heads, 2); o.all_reduce = true;
+    rc = net_backward_impl(net, obs, gather_idx, n_sample, st, o);
     if (rc) return rc;
     return xtb_adam_step_net(opt, net, 1.f, st);
   });
@@ -2178,7 +2185,7 @@ static int keras_fit_launch(xtb_net* net, xtb_adam* opt, const void* obs, const 
                             float* loss_out, void* stream) {
   CUDA_TRY(cudaMemsetAsync(loss_out, 0, sizeof(float), S(stream)));
   const int adim = net->tsize[lt];
-  int heads[2] = {lt, vt};
+  const int32_t heads[2] = {lt, vt};
   for (int s0 = 0; s0 < n; s0 += fit_batch) {
     const int mb = std::min(fit_batch, n - s0);
     int rc = net_forward_impl(net, nullptr, obs, obs_idx + s0, mb, stream, 0u, (1u << lt) | (1u << vt));
@@ -2186,7 +2193,7 @@ static int keras_fit_launch(xtb_net* net, xtb_adam* opt, const void* obs, const 
     rc = xtb_impala_keras_loss_grad(xtb_net_tensor(net, lt), xtb_net_tensor(net, vt), row_idx + s0, y, adv, tv, mb, adim, ent,
                                     0.5f, 1.f / n, xtb_net_tensor_grad(net, lt), xtb_net_tensor_grad(net, vt), loss_out, stream);
     if (rc) return rc;
-    rc = net_backward_impl(net, obs, obs_idx + s0, mb, heads, 2, stream, 0u, true);
+    rc = net_backward_impl(net, obs, obs_idx + s0, mb, stream, BackwardOpts(heads, 2));
     if (rc) return rc;
     rc = xtb_adam_step_net(opt, net, 1.f, stream);
     if (rc) return rc;
@@ -2194,10 +2201,8 @@ static int keras_fit_launch(xtb_net* net, xtb_adam* opt, const void* obs, const 
   return XTB_OK;
 }
 
-// arguments both IMPALA entry points share; data-parallel training is not supported by them
-static int keras_check(const char* fn, xtb_net* net, int lt, int vt) {
-  if (!net->ws || !net->grads) return fail(XTB_ERR_STATE, "%s: net not bound", fn);
-  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
+// head tensors of both IMPALA-Keras entry points: logits (at most MAX_ADIM wide) and value (1 wide)
+static int keras_heads_check(const char* fn, xtb_net* net, int lt, int vt) {
   const int nl = (int)net->L.size();
   if (lt < 1 || lt > nl || vt < 1 || vt > nl || lt == vt || net->tsize[vt] != 1) return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
   if (net->tsize[lt] > MAX_ADIM) return fail(XTB_ERR_ARG, "%s: action dim %d > %d", fn, net->tsize[lt], MAX_ADIM);
@@ -2207,13 +2212,11 @@ static int keras_check(const char* fn, xtb_net* net, int lt, int vt) {
 extern "C" int xtb_impala_keras_fit(xtb_net* net, xtb_adam* opt, const void* obs, const int32_t* order, const float* action_mat,
                                     const float* adv, const float* target_v, int n, int fit_batch, int logit_tensor, int v_tensor,
                                     float ent_coef, float* loss_out, int use_graph, void* stream) {
-  if (!net || !opt || !obs || !order || !action_mat || !adv || !target_v || !loss_out)
-    return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: null pointer");
-  if (int rc = keras_check("xtb_impala_keras_fit", net, logit_tensor, v_tensor)) return rc;
-  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: optimiser/net size mismatch");
-  if (n <= 0 || fit_batch <= 0) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: bad sizes");
-  if (std::min(n, fit_batch) > net->max_batch) return fail(XTB_ERR_ARG, "xtb_impala_keras_fit: batch exceeds net max_batch");
-  return run_graph(capture_key(kImpalaKerasFit, net, nullptr, opt, obs, order, action_mat, adv, target_v, n, fit_batch, logit_tensor,
+  const char* fn = "xtb_impala_keras_fit";
+  const bool missing = !net || !opt || !obs || !order || !action_mat || !adv || !target_v || !loss_out;
+  if (int rc = learner_check(fn, missing, net, opt, std::min(n, fit_batch), false)) return rc;
+  if (int rc = keras_heads_check(fn, net, logit_tensor, v_tensor)) return rc;
+  return run_graph(capture_key(kImpalaKerasFit, {net, opt}, obs, order, action_mat, adv, target_v, n, fit_batch, logit_tensor,
                                v_tensor, ent_coef, loss_out),
                    use_graph, stream, [&](void* st) {
     return keras_fit_launch(net, opt, obs, order, order, action_mat, adv, target_v, n, fit_batch, logit_tensor, v_tensor, ent_coef,
@@ -2225,16 +2228,15 @@ extern "C" int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_imp
                                       int fit_batch, const int32_t* order, int32_t* obs_idx, float gamma, float ent_coef,
                                       int logit_tensor, int v_tensor, float* pg_adv, float* target_v, float* loss_per_slice,
                                       int use_graph, void* stream) {
-  if (!net || !opt || !tr || !tr->obs || !tr->behav_prob || !tr->action_mat || !tr->reward || !tr->done || !order || !obs_idx ||
-      !pg_adv || !target_v || !loss_per_slice)
-    return fail(XTB_ERR_ARG, "xtb_impala_keras_train: null pointer");
-  if (int rc = keras_check("xtb_impala_keras_train", net, logit_tensor, v_tensor)) return rc;
-  if (opt->count != net->n_params) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: optimiser/net size mismatch");
-  if (n_traj <= 0 || ep_len <= 0 || slice <= 0 || fit_batch <= 0) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: bad sizes");
+  const char* fn = "xtb_impala_keras_train";
+  const bool missing = !net || !opt || !tr || !tr->obs || !tr->behav_prob || !tr->action_mat || !tr->reward || !tr->done || !order ||
+                       !obs_idx || !pg_adv || !target_v || !loss_per_slice;
   const long long n_state = (long long)n_traj * (ep_len + 1), n_train = (long long)n_traj * ep_len;
-  if (n_state > net->max_batch) return fail(XTB_ERR_ARG, "xtb_impala_keras_train: %lld states exceed net max_batch", n_state);
+  if (int rc = learner_check(fn, missing, net, opt, n_state, false)) return rc;
+  if (int rc = keras_heads_check(fn, net, logit_tensor, v_tensor)) return rc;
+  if (n_traj <= 0 || ep_len <= 0 || slice <= 0 || fit_batch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
   const xtb_impala_traj t = *tr;
-  return run_graph(capture_key(kImpalaKerasTrain, net, nullptr, opt, t.obs, t.behav_prob, t.action_mat, t.reward, t.done, n_traj,
+  return run_graph(capture_key(kImpalaKerasTrain, {net, opt}, t.obs, t.behav_prob, t.action_mat, t.reward, t.done, n_traj,
                                ep_len, slice, fit_batch, order, obs_idx, gamma, ent_coef, logit_tensor, v_tensor, pg_adv, target_v,
                                loss_per_slice),
                    use_graph, stream, [&](void* st) -> int {
@@ -2270,6 +2272,7 @@ struct xtb_muzero {
   xtb_muzero_desc d{};
   int max_batch = 0, K = 0, H = 0, A = 0, Sv = 0, Sr = 0, n_part = 0;
   int act_rep = 0, act_dyn = 0;
+  long long n_params = 0;      // floats of the shared parameter buffer
   float* buf = nullptr;
   float *hbuf = nullptr, *xbuf = nullptr, *rlog = nullptr, *dr = nullptr, *tv = nullptr, *tr = nullptr, *dh = nullptr,
         *dx = nullptr, *part = nullptr;
@@ -2313,7 +2316,7 @@ extern "C" int xtb_muzero_create(xtb_net* rep, xtb_net* dyn, xtb_net* pred, cons
     return fail(XTB_ERR_ARG, "xtb_muzero_create: the dynamics net's gradient scratch overlaps the shared gradient buffer");
   auto* m = new xtb_muzero();
   m->rep = rep; m->dyn = dyn; m->pred = pred; m->d = d; m->max_batch = max_batch;
-  m->K = K; m->H = H; m->A = A; m->Sv = Sv; m->Sr = Sr; m->act_rep = act_rep; m->act_dyn = act_dyn;
+  m->K = K; m->H = H; m->A = A; m->Sv = Sv; m->Sr = Sr; m->act_rep = act_rep; m->act_dyn = act_dyn; m->n_params = total;
   const long long Bm = max_batch, R1 = (long long)(K + 1) * Bm, RK = (long long)K * Bm;
   m->n_part = 2 * mz_blocks(R1) + mz_blocks(RK);
   const long long sizes[] = {R1 * H, RK * (H + A), RK * Sr, RK * Sr, R1 * Sv, RK * Sr, R1 * H, Bm * (H + A), m->n_part};
@@ -2338,12 +2341,10 @@ extern "C" void xtb_muzero_destroy(xtb_muzero* m) {
   delete m;
 }
 
-// shared argument checks of the MuZero entry points
-static int mz_check(const char* fn, const xtb_muzero* m, int batch) {
+// the learner checks of a MuZero entry point (opt NULL: an inference call) over its object's nets and batch limit
+static int mz_check(const char* fn, const xtb_muzero* m, bool missing, const xtb_adam* opt, int batch) {
   if (!m) return fail(XTB_ERR_ARG, "%s: null object", fn);
-  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
-  if (batch < 1 || batch > m->max_batch) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d]", fn, batch, m->max_batch);
-  return XTB_OK;
+  return learner_check(fn, missing, m->rep, opt, batch, false, m->max_batch, m->n_params);
 }
 
 // prediction forward over `rows` hidden states (rows of m->hbuf), then softmax policy / value expectation if asked
@@ -2375,21 +2376,17 @@ static int mz_initial_launch(xtb_muzero* m, const void* obs, int B, float* hidde
 
 extern "C" int xtb_muzero_initial_inference(xtb_muzero* m, const void* obs, int batch, float* hidden_out, float* value_out,
                                             float* policy_out, int use_graph, void* stream) {
-  if (int rc = mz_check("xtb_muzero_initial_inference", m, batch)) return rc;
-  if (!obs) return fail(XTB_ERR_ARG, "xtb_muzero_initial_inference: null observation");
-  CaptureKey key = capture_key(kMuzeroInitInfer, m->rep, m->dyn, nullptr, m, obs, batch, hidden_out, value_out, policy_out);
-  key.own[3] = m->pred; key.own[4] = m;
-  return run_graph(key, use_graph, stream, [&](void* st) { return mz_initial_launch(m, obs, batch, hidden_out, value_out, policy_out, S(st)); });
+  if (int rc = mz_check("xtb_muzero_initial_inference", m, !obs, nullptr, batch)) return rc;
+  return run_graph(capture_key(kMuzeroInitInfer, {m->rep, m->dyn, m->pred, m}, m, obs, batch, hidden_out, value_out, policy_out),
+                   use_graph, stream, [&](void* st) { return mz_initial_launch(m, obs, batch, hidden_out, value_out, policy_out, S(st)); });
 }
 
 extern "C" int xtb_muzero_recurrent_inference(xtb_muzero* m, const float* hidden, const int32_t* action, int batch, float* hidden_out,
                                               float* reward_out, float* value_out, float* policy_out, int use_graph, void* stream) {
-  if (int rc = mz_check("xtb_muzero_recurrent_inference", m, batch)) return rc;
-  if (!hidden || !action) return fail(XTB_ERR_ARG, "xtb_muzero_recurrent_inference: null pointer");
-  CaptureKey key = capture_key(kMuzeroRecurInfer, m->rep, m->dyn, nullptr, m, hidden, action, batch, hidden_out, reward_out, value_out,
-                               policy_out);
-  key.own[3] = m->pred; key.own[4] = m;
-  return run_graph(key, use_graph, stream, [&](void* sv) -> int {
+  if (int rc = mz_check("xtb_muzero_recurrent_inference", m, !hidden || !action, nullptr, batch)) return rc;
+  return run_graph(capture_key(kMuzeroRecurInfer, {m->rep, m->dyn, m->pred, m}, m, hidden, action, batch, hidden_out, reward_out,
+                               value_out, policy_out),
+                   use_graph, stream, [&](void* sv) -> int {
     cudaStream_t st = S(sv);
     const xtb_muzero_desc& d = m->d;
     const int H = m->H, A = m->A;
@@ -2456,7 +2453,9 @@ static int mz_train_launch(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch&
   LAUNCH_CHECK();
   // backward: prediction (with d loss / d h_i for every i), the dynamics steps newest first, the representation
   const int32_t pheads[2] = {d.pred_p, d.pred_v}, dheads[2] = {d.dyn_h, d.dyn_r}, rheads[1] = {d.rep_h};
-  rc = net_backward_impl(pred, m->hbuf, nullptr, R1, pheads, 2, st, 0u, true, 0u, 0u, nullptr, 0u, m->dh);
+  BackwardOpts po(pheads, 2), dopt(dheads, 2);
+  po.dobs = m->dh; dopt.dobs = m->dx;
+  rc = net_backward_impl(pred, m->hbuf, nullptr, R1, st, po);
   if (rc) return rc;
   float* gdyn = rep->grads + (dyn->params - rep->params);
   CUDA_TRY(cudaMemsetAsync(gdyn, 0, dyn->n_params * sizeof(float), st));
@@ -2470,7 +2469,7 @@ static int mz_train_launch(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch&
     LAUNCH_CHECK();
     CUDA_TRY(cudaMemcpyAsync(xtb_net_tensor_grad(dyn, d.dyn_r), m->dr + (size_t)k * B * Sr, (size_t)B * Sr * sizeof(float),
                              cudaMemcpyDeviceToDevice, st));
-    rc = net_backward_impl(dyn, xk, nullptr, B, dheads, 2, st, 0u, true, 0u, 0u, nullptr, 0u, m->dx);
+    rc = net_backward_impl(dyn, xk, nullptr, B, st, dopt);
     if (rc) return rc;
     XLAUNCH(mz_accumulate_kernel, std::min(4 * kSMs, (int)((dyn->n_params + 255) / 256)), 256, 0, st, gdyn, (const float*)dyn->grads,
             dyn->n_params);
@@ -2480,7 +2479,7 @@ static int mz_train_launch(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch&
   XLAUNCH(mz_hidden_grad_kernel, ew_blocks, 256, 0, st, (const float*)m->dh, (const float*)m->dx, X, 1.f,
           (const float*)xtb_net_tensor(rep, d.rep_h), m->act_rep, B, H, xtb_net_tensor_grad(rep, d.rep_h));
   LAUNCH_CHECK();
-  rc = net_backward_impl(rep, bt.obs, nullptr, B, rheads, 1, st, 0u, true);
+  rc = net_backward_impl(rep, bt.obs, nullptr, B, st, BackwardOpts(rheads, 1));
   if (rc) return rc;
   // AdamOptimizer(LR).minimize over the whole buffer, then the weight blobs of the three nets
   rc = adam_step_impl(opt, rep->params, rep->grads, 1.f, st, nullptr);
@@ -2492,18 +2491,14 @@ static int mz_train_launch(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch&
 
 extern "C" int xtb_muzero_train(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_batch* batch_in, int batch, float loss_offset,
                                 float* loss_out, float* value_out, int use_graph, void* stream) {
-  if (int rc = mz_check("xtb_muzero_train", m, batch)) return rc;
-  if (!opt || !batch_in || !loss_out) return fail(XTB_ERR_ARG, "xtb_muzero_train: null pointer");
+  const bool missing = !opt || !batch_in || !loss_out || !batch_in->obs || !batch_in->action || !batch_in->target_value ||
+                       !batch_in->target_reward || !batch_in->target_policy;
+  if (int rc = mz_check("xtb_muzero_train", m, missing, opt, batch)) return rc;
   const xtb_muzero_batch bt = *batch_in;
-  if (!bt.obs || !bt.action || !bt.target_value || !bt.target_reward || !bt.target_policy)
-    return fail(XTB_ERR_ARG, "xtb_muzero_train: null batch array");
   if (bt.unroll != m->K) return fail(XTB_ERR_ARG, "xtb_muzero_train: batch unroll %d != model unroll %d", bt.unroll, m->K);
-  if (opt->count != (m->pred->params - m->rep->params) + m->pred->n_params)
-    return fail(XTB_ERR_ARG, "xtb_muzero_train: optimiser size %lld != parameter count", opt->count);
-  CaptureKey key = capture_key(kMuzeroTrain, m->rep, m->dyn, opt, m, bt.obs, bt.action, bt.target_value, bt.target_reward,
-                               bt.target_policy, batch, loss_offset, loss_out, value_out);
-  key.own[3] = m->pred; key.own[4] = m;
-  return run_graph(key, use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
+  return run_graph(capture_key(kMuzeroTrain, {m->rep, m->dyn, m->pred, m, opt}, m, bt.obs, bt.action, bt.target_value,
+                               bt.target_reward, bt.target_policy, batch, loss_offset, loss_out, value_out),
+                   use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
 }
 
 // Dueling head that the fused TD step covers: q_tensor combines two linear dense layers that read the same hidden
@@ -2543,16 +2538,16 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
                              const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                              const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
                              float* qn_o, float* loss_out, int use_graph, void* stream) {
-  if (!net || !target || !opt || !obs || !next_obs || !action || !reward || !done || !qn_t || !loss_out)
-    return fail(XTB_ERR_ARG, "xtb_dqn_train: null pointer");
-  if (!net->ws || !net->grads || !target->ws) return fail(XTB_ERR_STATE, "xtb_dqn_train: nets not bound");
+  const bool missing = !net || !target || !opt || !obs || !next_obs || !action || !reward || !done || !qn_t || !loss_out;
+  if (int rc = learner_check("xtb_dqn_train", missing, net, opt, n_sample, true)) return rc;
+  if (!target->ws) return fail(XTB_ERR_STATE, "xtb_dqn_train: target net not bound");
   const int nl = (int)net->L.size();
   if (q_tensor < 1 || q_tensor > nl || (int)target->L.size() != nl) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad head tensor");
-  if (n_sample <= 0 || n_sample > net->max_batch || n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad batch");
+  if (n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: batch exceeds the target net's max_batch");
   const int adim = net->tsize[q_tensor];
   const float inv_world = dp_inv_world();
   const bool fuse = dueling_fusable(net, q_tensor);
-  return run_graph(capture_key(kDqnTrain, net, target, opt, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
+  return run_graph(capture_key(kDqnTrain, {net, target, opt}, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
                                n_sample, gamma, huber_delta, q_tensor),
                    use_graph, stream, [&](void* st) -> int {
     const size_t qbytes = (size_t)n_sample * adim * sizeof(float);
@@ -2575,8 +2570,9 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
       rc = xtb_dqn_td_loss_grad(xtb_net_tensor(net, q_tensor), qn_t, qn_o, idx, action, reward, done, disc, n_sample, adim, gamma,
                                 huber_delta, inv_count, xtb_net_tensor_grad(net, q_tensor), nullptr, loss_out, st);
       if (rc) return rc;
-      int heads[1] = {q_tensor};
-      rc = net_backward_impl(net, obs, idx, n_sample, heads, 1, st, 0u, true, 0u, 0u, g_comm);
+      const int32_t heads[1] = {q_tensor};
+      BackwardOpts o(heads, 1); o.all_reduce = true;
+      rc = net_backward_impl(net, obs, idx, n_sample, st, o);
       if (rc) return rc;
     }
     return xtb_adam_step_net(opt, net, 1.f, st);
@@ -2610,10 +2606,10 @@ static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* st
     typename DIST::Action* a_t = action + (long long)t * E * DIST::action_width(adim);
     float* lp_t = logp + (long long)t * E; float* v_o = value + (long long)t * E;
     if (fuse) {
-      launch_infer_heads<DIST>(lpi.K, adim, std::max(1, std::min(kSMs, (E + 7) / 8)), S(stream),
-                               (const float*)(net->ws + net->out_off[lpi.d.src]), (const float*)(net->ws + net->out_off[lv.d.src]),
-                               net->params + lpi.w_off, net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off,
-                               log_std, E, lpi.K, adim, seed, offset_dev, t, a_t, lp_t, v_o, pi_out);
+      XLAUNCH(heads_pick(kInferHeadsKernels<DIST>, lpi.K, adim)->kern, std::max(1, std::min(kSMs, (E + 7) / 8)), 256, 0, S(stream),
+              (const float*)out_f32(net, lpi.d.src), (const float*)out_f32(net, lv.d.src), net->params + lpi.w_off,
+              net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off, log_std, E, lpi.K, adim, seed, offset_dev, t,
+              a_t, lp_t, v_o, pi_out);
     } else if constexpr (DIST::kLogStd) {
       XLAUNCH(gauss_sample_kernel, (E + 127) / 128, 128, 0, S(stream), pi_out, log_std, E, adim, (const float*)nullptr, seed,
               (uint64_t)0, offset_dev, t, a_t, lp_t, v_in, v_o);
@@ -2636,7 +2632,7 @@ static int ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_
   if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
   if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
   if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
-  return run_graph(capture_key(PpoCalls<DIST>::infer_tag, net, nullptr, nullptr, obs, step_idx, offset_dev, action, logp, value,
+  return run_graph(capture_key(PpoCalls<DIST>::infer_tag, {net}, obs, step_idx, offset_dev, action, logp, value,
                                n_env, n_step, pi_t, v_t, ls_t, seed),
                    use_graph, stream, [&](void* st) {
     return rollout_infer_launch<DIST>(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev, action, logp, value, st);
