@@ -246,14 +246,17 @@ int xtb_impala_keras_loss_grad(const float* logits, const float* v, const int32_
  *      Adam(clipnorm) (xt/model/dqn/dqn_cnn.py:60) ----------------------------------- */
 typedef struct xtb_adam xtb_adam;
 enum xtb_clip_mode { XTB_CLIP_NONE = 0, XTB_CLIP_GLOBAL_NORM = 1, XTB_CLIP_PER_TENSOR = 2 };
-/* m, v: [count] floats (caller-owned, zero-initialised by this call); seg_offsets: n_seg+1
- * boundaries of the tensors inside the flat buffer (used by XTB_CLIP_PER_TENSOR). */
+/* m, v: [count] floats, 16-byte aligned (caller-owned, zero-initialised by this call); seg_offsets: n_seg+1
+ * non-decreasing boundaries of the tensors inside the flat buffer, from 0 to count (used by XTB_CLIP_PER_TENSOR; equal
+ * neighbours make an empty tensor).  clip_mode is one of xtb_clip_mode, and clip > 0 unless it is XTB_CLIP_NONE.
+ * Any other argument returns XTB_ERR_ARG before a CUDA call. */
 int xtb_adam_create(long long count, float lr, float beta1, float beta2, float eps, int clip_mode,
                     float clip, const long long* seg_offsets, int n_seg, float* m, float* v,
                     xtb_adam** out);
 void xtb_adam_destroy(xtb_adam* opt);
 /* grad_scale multiplies the gradient before clipping (1 normally). After the call
- * *xtb_adam_grad_norm() holds the pre-clip global norm (device float). */
+ * *xtb_adam_grad_norm() holds the pre-clip global norm of grad_scale * grads (device float).  params and grads must be
+ * 16-byte aligned (XTB_ERR_ARG, launching nothing, otherwise). */
 int xtb_adam_step(xtb_adam* opt, float* params, const float* grads, float grad_scale, void* stream);
 /* Same step on a bound network's parameters/gradients; the kernel also refreshes the weights' bf16 planes. */
 int xtb_adam_step_net(xtb_adam* opt, xtb_net* net, float grad_scale, void* stream);
@@ -265,8 +268,8 @@ int xtb_adam_set_lr(xtb_adam* opt, float lr);
 int xtb_adam_set_decay(xtb_adam* opt, float decay);
 /* Switch the optimiser handle to tf.train.RMSPropOptimizer(lr, decay, epsilon, centered=True) (momentum 0), the
  * `opt_type: rmsprop` branch of xt/model/impala/impala_cnn_opt.py:205-206: the `m` buffer of xtb_adam_create becomes the
- * mean-square slot and `mean_grad` (count floats) the mean-gradient slot; this call sets them to ones / zeros as TF
- * initialises them; `v` is unused.  Clipping, chunking and the weight-blob refresh are those of the Adam step. */
+ * mean-square slot and `mean_grad` (count floats, 16-byte aligned) the mean-gradient slot; this call sets them to
+ * ones / zeros as TF initialises them; `v` is unused.  Clipping, chunking and the weight-blob refresh are those of the Adam step. */
 int xtb_opt_use_rmsprop(xtb_adam* opt, float* mean_grad, float decay, float epsilon);
 
 /* ---- fused learner loops -------------------------------------------------------- */

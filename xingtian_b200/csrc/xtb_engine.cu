@@ -1684,15 +1684,27 @@ struct xtb_adam {
   double* norm_sq = nullptr; float* seg_scale = nullptr; AdamState* st = nullptr; AdamHyper* hyp = nullptr; unsigned int* ticket = nullptr;
 };
 
+// The optimiser kernels read and write every buffer as float4 wherever a chunk starts at a multiple of 4 elements.
+static inline bool misaligned16(const void* p) { return (uintptr_t)p % 16 != 0; }
+
 extern "C" int xtb_adam_create(long long count, float lr, float beta1, float beta2, float eps, int clip_mode,
                                float clip, const long long* seg_offsets, int n_seg, float* m, float* v,
                                xtb_adam** out) {
   if (count <= 0 || !m || !v || !out) return fail(XTB_ERR_ARG, "xtb_adam_create: bad argument");
+  if (clip_mode != XTB_CLIP_NONE && clip_mode != XTB_CLIP_GLOBAL_NORM && clip_mode != XTB_CLIP_PER_TENSOR)
+    return fail(XTB_ERR_ARG, "xtb_adam_create: unknown clip_mode %d", clip_mode);
+  // clip / max(norm, clip) climbs the gradient for clip < 0 and is 0/0 for clip = 0 and a zero gradient
+  if (clip_mode != XTB_CLIP_NONE && !(clip > 0.f))
+    return fail(XTB_ERR_ARG, "xtb_adam_create: clip must be > 0 with a clipping mode (got %g)", (double)clip);
+  if (misaligned16(m) || misaligned16(v)) return fail(XTB_ERR_ARG, "xtb_adam_create: m and v must be 16-byte aligned");
   std::vector<long long> seg;
   if (clip_mode == XTB_CLIP_PER_TENSOR) {
     if (!seg_offsets || n_seg <= 0) return fail(XTB_ERR_ARG, "per-tensor clip needs segment offsets");
     seg.assign(seg_offsets, seg_offsets + n_seg + 1);
     if (seg.front() != 0 || seg.back() != count) return fail(XTB_ERR_ARG, "segment offsets must span [0,count]");
+    for (int s = 0; s < n_seg; s++)        // a decreasing pair would hand the same parameters to two blocks
+      if (seg[s + 1] < seg[s])
+        return fail(XTB_ERR_ARG, "xtb_adam_create: segment offsets must not decrease (offset %d: %lld < %lld)", s + 1, seg[s + 1], seg[s]);
   } else {
     seg = {0, count};
   }
@@ -1753,6 +1765,8 @@ extern "C" int xtb_adam_step_net(xtb_adam* o, xtb_net* net, float grad_scale, vo
 }
 static int adam_step_impl(xtb_adam* o, float* params, const float* grads, float grad_scale, void* stream, xtb_net* net) {
   if (!o || !params || !grads) return fail(XTB_ERR_ARG, "xtb_adam_step: null pointer");
+  if (misaligned16(params) || misaligned16(grads) || misaligned16(o->m) || misaligned16(o->v) || misaligned16(o->mg))
+    return fail(XTB_ERR_ARG, "xtb_adam_step: params, grads and the optimiser slots must be 16-byte aligned");
   cudaStream_t st = S(stream);
   XLAUNCH(sqnorm_kernel, (o->n_blk + SQN_GROUP - 1) / SQN_GROUP, OPT_THREADS, 0, st, grads, o->blk_seg, o->blk_beg, o->blk_len, o->n_blk, o->norm_sq, o->ticket, o->st,
           (const AdamHyper*)o->hyp, o->seg_scale, o->n_seg, o->clip_mode, grad_scale);
@@ -1775,6 +1789,7 @@ static int adam_step_impl(xtb_adam* o, float* params, const float* grads, float 
 extern "C" const float* xtb_adam_grad_norm(const xtb_adam* o) { return o ? &o->st->grad_norm : nullptr; }
 extern "C" int xtb_opt_use_rmsprop(xtb_adam* o, float* mean_grad, float decay, float epsilon) {
   if (!o || !mean_grad) return fail(XTB_ERR_ARG, "xtb_opt_use_rmsprop: null pointer");
+  if (misaligned16(mean_grad)) return fail(XTB_ERR_ARG, "xtb_opt_use_rmsprop: mean_grad must be 16-byte aligned");
   if (!(decay > 0.f && decay < 1.f) || !(epsilon > 0.f)) return fail(XTB_ERR_ARG, "xtb_opt_use_rmsprop: decay in (0,1), epsilon > 0");
   drop_graphs_of(o);                       // captured steps baked the Adam kernel in
   {   // slot initial values of tf.train.RMSPropOptimizer: rms = ones, mg = zeros (one-time, synchronous)
