@@ -8,7 +8,13 @@ same forward with nothing but numpy indexing and a tensordot, in float64, so the
 Follows xt/model/model_utils.py:141-160 (Conv2D NHWC, HWIO kernels, 'valid' / 'same' padding as TensorFlow defines it:
 pad_total = max((ceil(in/s)-1)*s + k - in, 0), the smaller half first), :187-201 (uint8 -> /255), Keras Flatten
 (row-major over H, W, C) and Dense (x @ kernel + bias).
+
+It also holds the hidden activations of the reference's ACTIVATION_MAP (xt/model/model_utils.py:8-19) with TF 1.15's
+semantics, their constants and the derivative rules the kernels use (gemm_f32.cuh act_grad); xt_oracle takes the
+constants from here.
 """
+import math
+
 import numpy as np
 
 
@@ -35,16 +41,70 @@ def conv2d_nhwc(x, kernel, bias, stride, pad):
     return out + bias
 
 
-_ACT = {None: lambda v: v, "linear": lambda v: v, "relu": lambda v: np.maximum(v, 0.0), "tanh": np.tanh}
+LEAKY_ALPHA = 0.2                       # tf.nn.leaky_relu default
+SELU_SCALE = 1.0507009873554805         # tf.nn.selu
+SELU_ALPHA = 1.6732632423543772
+GELU_C = math.sqrt(2.0 / math.pi)       # xt/model/tf_utils.py:157-166
+GELU_A = 0.044715
+
+NEW = ("sigmoid", "softsign", "softplus", "leaky_relu", "elu", "selu", "swish", "gelu")   # past relu / tanh
+KEEPS_Z = ("softsign", "swish", "gelu")     # the backward takes their derivative from the pre-activation z
+
+
+def _sigmoid(x):
+    return 1.0 / (1.0 + np.exp(-x))
+
+
+_ACT = {
+    None: lambda v: v, "linear": lambda v: v, "relu": lambda v: np.maximum(v, 0.0), "tanh": np.tanh,
+    "sigmoid": _sigmoid,
+    "softsign": lambda x: x / (1 + np.abs(x)),
+    "softplus": lambda x: np.maximum(x, 0) + np.log1p(np.exp(-np.abs(x))),
+    "leaky_relu": lambda x: np.where(x > 0, x, LEAKY_ALPHA * x),
+    "elu": lambda x: np.where(x > 0, x, np.expm1(np.minimum(x, 0))),
+    "selu": lambda x: SELU_SCALE * np.where(x > 0, x, SELU_ALPHA * np.expm1(np.minimum(x, 0))),
+    "swish": lambda x: x * _sigmoid(x),
+    "gelu": lambda x: 0.5 * x * (1 + np.tanh(GELU_C * (x + GELU_A * x ** 3))),
+}
+
+
+def grad_rule(act, y, z):
+    """d act / d z as the kernels take it: from the output y, or from the pre-activation z for KEEPS_Z."""
+    if act == "sigmoid":
+        return y * (1 - y)
+    if act == "softsign":
+        return 1.0 / (1 + np.abs(z)) ** 2
+    if act == "softplus":
+        return -np.expm1(-y)
+    if act == "leaky_relu":
+        return np.where(y > 0, 1.0, LEAKY_ALPHA)
+    if act == "elu":
+        return np.where(y > 0, 1.0, y + 1)
+    if act == "selu":
+        return np.where(y > 0, SELU_SCALE, y + SELU_SCALE * SELU_ALPHA)
+    if act == "swish":
+        s = _sigmoid(z)
+        return s * (1 + z * (1 - s))
+    if act == "gelu":
+        t = np.tanh(GELU_C * (z + GELU_A * z ** 3))
+        return 0.5 * (1 + t) + 0.5 * z * (1 - t * t) * GELU_C * (1 + 3 * GELU_A * z * z)
+    raise KeyError(act)
 
 
 def forward(arch, weights, obs):
-    """dict name -> float64 activations of every layer (same arch dicts as xt_oracle)."""
+    """dict name -> float64 activations of every layer (same arch dicts as xt_oracle); a logstd layer holds a variable
+    and produces no tensor."""
     x = np.asarray(obs).astype(np.float64)
     if arch["input_dtype"] == "uint8":
         x = x / 255.0
     t = {"obs": x}
     for name, kind, src, sp in arch["layers"]:
+        if kind == "logstd":
+            continue
+        if kind == "dueling":
+            value, adv = t[src[0]], t[src[1]]
+            t[name] = adv + (value - value.mean(1, keepdims=True))
+            continue
         a = t[src]
         k = np.asarray(weights[name + "/kernel"], np.float64)
         b = np.asarray(weights[name + "/bias"], np.float64)

@@ -39,17 +39,30 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from oracle.np_f64 import GELU_A, GELU_C, LEAKY_ALPHA, SELU_ALPHA, SELU_SCALE
+
 # --------------------------------------------------------------------------- #
 # Architectures
 # --------------------------------------------------------------------------- #
-# layer tuple: (name, kind, src, spec) ; kind in {"conv","dense"}
-#   conv spec : dict(k=, s=, cout=, pad="valid"|"same", act=)
-#   dense spec: dict(n=, act=)
+# layer tuple: (name, kind, src, spec) ; kind in {"conv","dense","dueling","logstd"}
+#   conv spec   : dict(k=, s=, cout=, pad="valid"|"same", act=)
+#   dense spec  : dict(n=, act=)
+#   dueling     : src = (value, adv), spec {}; the parameter-free Q = adv + (value - mean(value))
+#   logstd spec : dict(n=A), src None; the (1, A) variable pi_logstd of the DiagGaussian head, no tensor
 # tensors are named after the layer that produces them; the input is "obs".
 
 
+def _ppo_heads(layers, tails, action_dim, diag_gaussian):
+    layers.append(("pi_latent", "dense", tails.get("shared", tails.get("pi")), dict(n=action_dim, act=None)))
+    layers.append(("output_value", "dense", tails.get("shared", tails.get("v")), dict(n=1, act=None)))
+    if diag_gaussian:
+        # tf.get_variable('pi_logstd', (1, A)) is created after the Keras model (xt/model/ppo/ppo.py:75-78), so it is
+        # the last variable TFVariables lists
+        layers.append(("pi_logstd", "logstd", None, dict(n=action_dim)))
+
+
 def ppo_cnn_arch(state_dim=(84, 84, 4), action_dim=4, hidden_sizes=(256,),
-                 activation="relu", vf_share_layers=True):
+                 activation="relu", vf_share_layers=True, diag_gaussian=False):
     """xt/model/model_utils.py:49-80 (get_cnn_backbone), :91-97, :120-162."""
     h, w, _ = state_dim
     if (h, w) == (84, 84):
@@ -74,16 +87,13 @@ def ppo_cnn_arch(state_dim=(84, 84, 4), action_dim=4, hidden_sizes=(256,),
             layers.append((name, "dense", src, dict(n=hs, act=activation)))
             src = name
         tails[p] = src
-    pi_src = tails["shared"] if vf_share_layers else tails["pi"]
-    v_src = tails["shared"] if vf_share_layers else tails["v"]
-    layers.append(("pi_latent", "dense", pi_src, dict(n=action_dim, act=None)))
-    layers.append(("output_value", "dense", v_src, dict(n=1, act=None)))
+    _ppo_heads(layers, tails, action_dim, diag_gaussian)
     return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0,
                 layers=layers, outputs=["pi_latent", "output_value"])
 
 
 def ppo_mlp_arch(state_dim=(4,), action_dim=2, hidden_sizes=(64, 64),
-                 activation="tanh", vf_share_layers=False):
+                 activation="tanh", vf_share_layers=False, diag_gaussian=False):
     """xt/model/model_utils.py:22-46 (get_mlp_backbone)."""
     layers = []
     prefixes = ["shared"] if vf_share_layers else ["pi", "v"]
@@ -95,10 +105,7 @@ def ppo_mlp_arch(state_dim=(4,), action_dim=2, hidden_sizes=(64, 64),
             layers.append((name, "dense", src, dict(n=hs, act=activation)))
             src = name
         tails[p] = src
-    pi_src = tails["shared"] if vf_share_layers else tails["pi"]
-    v_src = tails["shared"] if vf_share_layers else tails["v"]
-    layers.append(("pi_latent", "dense", pi_src, dict(n=action_dim, act=None)))
-    layers.append(("output_value", "dense", v_src, dict(n=1, act=None)))
+    _ppo_heads(layers, tails, action_dim, diag_gaussian)
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0,
                 layers=layers, outputs=["pi_latent", "output_value"])
 
@@ -121,8 +128,15 @@ def impala_cnn_arch(state_dim=(84, 84, 4), action_dim=4):
                 layers=layers, outputs=[sc + "conv2d_3", sc + "dense"])
 
 
-def dqn_cnn_arch(state_dim=(84, 84, 4), action_dim=4):
-    """xt/model/dqn/dqn_cnn.py:45-54 (dueling=False)."""
+def _dueling_head(layers, value, adv):
+    """xt/model/dqn/dqn_cnn.py:53-58, dqn_mlp.py:50-54: adv = Dense(1) on the value head's input, then the combine."""
+    layers.append((adv, "dense", layers[-1][2], dict(n=1, act=None)))
+    layers.append(("dueling", "dueling", (value, adv), {}))
+    return "dueling"
+
+
+def dqn_cnn_arch(state_dim=(84, 84, 4), action_dim=4, dueling=False):
+    """xt/model/dqn/dqn_cnn.py:45-58."""
     layers = [
         ("conv2d", "conv", "obs", dict(k=8, s=4, cout=32, pad="valid", act="relu")),
         ("conv2d_1", "conv", "conv2d", dict(k=4, s=2, cout=64, pad="valid", act="relu")),
@@ -130,21 +144,47 @@ def dqn_cnn_arch(state_dim=(84, 84, 4), action_dim=4):
         ("dense", "dense", "conv2d_2", dict(n=256, act="relu")),
         ("dense_1", "dense", "dense", dict(n=action_dim, act=None)),
     ]
+    out = _dueling_head(layers, "dense_1", "dense_2") if dueling else "dense_1"
     return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0,
-                layers=layers, outputs=["dense_1"])
+                layers=layers, outputs=[out])
 
 
-def dqn_mlp_arch(state_dim=(4,), action_dim=2, hidden_size=128, num_layers=1):
-    """xt/model/dqn/dqn_mlp.py:43-60 (dueling=False)."""
+def dqn_mlp_arch(state_dim=(4,), action_dim=2, hidden_size=128, num_layers=1, dueling=False):
+    """xt/model/dqn/dqn_mlp.py:43-60, :80-87."""
     layers = []
     src = "obs"
     for i in range(num_layers):
         name = "dense" if i == 0 else "dense_%d" % i
         layers.append((name, "dense", src, dict(n=hidden_size, act="relu")))
         src = name
-    layers.append(("dense_%d" % num_layers, "dense", src, dict(n=action_dim, act=None)))
+    out = "dense_%d" % num_layers
+    layers.append((out, "dense", src, dict(n=action_dim, act=None)))
+    if dueling:
+        out = _dueling_head(layers, out, "dense_%d" % (num_layers + 1))
     return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0,
-                layers=layers, outputs=["dense_%d" % num_layers])
+                layers=layers, outputs=[out])
+
+
+def _impala_keras_heads(trunk, action_dim):
+    """output_actions = Dense(A, softmax), output_value = Dense(1) on the last hidden tensor (impala_mlp.py:49-50,
+    impala_cnn.py:55-56); the softmax is applied by the loss and predict."""
+    src = trunk[-1][0]
+    return trunk + [("output_actions", "dense", src, dict(n=action_dim, act=None)),
+                    ("output_value", "dense", src, dict(n=1, act=None))]
+
+
+def impala_mlp_arch(state_dim=(4,), action_dim=2, hidden_size=128, num_layers=1):
+    """ImpalaMlp, xt/model/impala/impala_mlp.py:39-50: DqnMlp's trunk, then the two heads."""
+    trunk = dqn_mlp_arch(state_dim, action_dim, hidden_size, num_layers)["layers"][:num_layers]
+    return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0,
+                layers=_impala_keras_heads(trunk, action_dim), outputs=["output_actions", "output_value"])
+
+
+def impala_keras_cnn_arch(state_dim=(84, 84, 4), action_dim=4):
+    """ImpalaCnn (the Keras learner's model), xt/model/impala/impala_cnn.py:44-56: DqnCnn's trunk, then the two heads."""
+    trunk = dqn_cnn_arch(state_dim, action_dim)["layers"][:4]
+    return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0,
+                layers=_impala_keras_heads(trunk, action_dim), outputs=["output_actions", "output_value"])
 
 
 def _same_pad(size, k, s):
@@ -158,6 +198,11 @@ def tensor_shapes(arch):
     """Shape (per sample) of every named tensor."""
     shapes = {"obs": tuple(arch["state_dim"])}
     for name, kind, src, sp in arch["layers"]:
+        if kind == "logstd":
+            continue
+        if kind == "dueling":
+            shapes[name] = shapes[src[0]]
+            continue
         ish = shapes[src]
         if kind == "conv":
             h, w, _ = ish
@@ -176,10 +221,16 @@ def param_shapes(arch):
 
     Names follow xt/model/model_utils.py:87,96 (layer names) + Keras' '/kernel',
     '/bias' suffixes, the key set TFVariables.get_weights returns
-    (xt/model/tf_utils.py:99-102)."""
+    (xt/model/tf_utils.py:99-102).  A dueling layer owns no variable; a logstd layer owns the (1, A) variable named
+    after it."""
     shapes = tensor_shapes(arch)
     out = OrderedDict()
     for name, kind, src, sp in arch["layers"]:
+        if kind == "dueling":
+            continue
+        if kind == "logstd":
+            out[name] = (1, sp["n"])
+            continue
         ish = shapes[src]
         if kind == "conv":
             out[name + "/kernel"] = (sp["k"], sp["k"], ish[-1], sp["cout"])
@@ -191,14 +242,15 @@ def param_shapes(arch):
 
 
 def init_weights(arch, seed=0, baseline_norm_std=None):
-    """Keras default init: glorot_uniform kernels, zero biases.
+    """Keras default init: glorot_uniform kernels, zero biases; pi_logstd starts at zero (xt/model/ppo/ppo.py:75-78)
+    and draws nothing.
 
     ``baseline_norm_std`` restates custom_norm_initializer
     (xt/model/model_utils.py:204-211) for ImpalaCnnOpt's baseline dense."""
     rng = np.random.default_rng(seed)
     w = OrderedDict()
     for name, shp in param_shapes(arch).items():
-        if name.endswith("/bias"):
+        if not name.endswith("/kernel"):
             w[name] = np.zeros(shp, np.float32)
             continue
         if len(shp) == 4:
@@ -217,6 +269,15 @@ def init_weights(arch, seed=0, baseline_norm_std=None):
 
 _ACT = {
     None: lambda x: x, "linear": lambda x: x, "relu": torch.relu, "tanh": torch.tanh,
+    # the rest of the reference's ACTIVATION_MAP, as np_f64 states them (any float dtype)
+    "sigmoid": torch.sigmoid,
+    "softsign": lambda x: x / (1 + x.abs()),
+    "softplus": lambda x: torch.clamp(x, min=0) + torch.log1p(torch.exp(-x.abs())),
+    "leaky_relu": lambda x: torch.where(x > 0, x, LEAKY_ALPHA * x),
+    "elu": lambda x: torch.where(x > 0, x, torch.expm1(torch.clamp(x, max=0))),
+    "selu": lambda x: SELU_SCALE * torch.where(x > 0, x, SELU_ALPHA * torch.expm1(torch.clamp(x, max=0))),
+    "swish": lambda x: x * torch.sigmoid(x),
+    "gelu": lambda x: 0.5 * x * (1 + torch.tanh(GELU_C * (x + GELU_A * x ** 3))),
 }
 
 
@@ -243,12 +304,19 @@ class precision(object):
         return False
 
 
+def dueling_combine(value, adv):
+    """Q = adv + (value - mean over actions of value): the reference's arithmetic (xt/model/dqn/dqn_cnn.py:53-58,
+    dqn_mlp.py:80-87)."""
+    return adv + (value - value.mean(dim=1, keepdim=True))
+
+
 def forward(arch, weights, obs, keep=False):
     """Network forward in torch-CPU fp32.  obs: ndarray/tensor [B,*state_dim].
 
     uint8 inputs are cast and divided by 255 (model_utils.py:187-189,
     dqn_cnn.py:48, state_transform :192-201 with mean 0).  Conv = NHWC,
-    HWIO kernels (Keras Conv2D); flatten in HWC order (Keras Flatten on NHWC)."""
+    HWIO kernels (Keras Conv2D); flatten in HWC order (Keras Flatten on NHWC).
+    A logstd layer produces no tensor; its variable is read by the Gaussian head."""
     wt = {k: (v if torch.is_tensor(v) else torch.from_numpy(np.ascontiguousarray(v))).to(_PREC["t"]) for k, v in weights.items()}
     x = obs if torch.is_tensor(obs) else torch.from_numpy(np.ascontiguousarray(obs))
     if arch["input_dtype"] == "uint8":
@@ -257,6 +325,11 @@ def forward(arch, weights, obs, keep=False):
         x = x.to(_PREC["t"])
     t = {"obs": x}
     for name, kind, src, sp in arch["layers"]:
+        if kind == "logstd":
+            continue
+        if kind == "dueling":
+            t[name] = dueling_combine(t[src[0]], t[src[1]])
+            continue
         a = t[src]
         if kind == "conv":
             xin = a.permute(0, 3, 1, 2)  # NCHW
@@ -352,6 +425,55 @@ def ppo_predict(arch, weights, obs, uniforms):
 
 
 # --------------------------------------------------------------------------- #
+# DiagGaussian distribution (xt/model/tf_dist.py:49-86, xt/model/ppo/ppo.py:62-95)
+# --------------------------------------------------------------------------- #
+#   log_std    = tf.get_variable('pi_logstd', shape=(1, A), initializer=zeros)   (created after the Keras model)
+#   dist_param = concat([pi_latent, pi_latent * 0.0 + log_std]);  std = exp(log_std)
+#   sample     = mean + std * N(0, 1);   log_prob(x) = -neglog_prob(x)
+
+LOG_2PI = math.log(2.0 * math.pi)
+
+
+def _c(x, like):
+    return torch.as_tensor(x, dtype=like.dtype)
+
+
+def gauss_neglog_prob(x, mean, log_std):
+    """tf_dist.py:63-66, [B, 1]; log_std broadcasts over the batch"""
+    A = mean.shape[-1]
+    return (_c(0.5 * LOG_2PI, mean) * A + 0.5 * (((x - mean) / torch.exp(log_std)) ** 2).sum(-1, keepdim=True)) + \
+        log_std.expand_as(mean).sum(-1, keepdim=True)
+
+
+def gauss_log_prob(x, mean, log_std):
+    return -gauss_neglog_prob(x, mean, log_std)
+
+
+def gauss_entropy(log_std):
+    """tf_dist.py:71-72, [rows, 1]"""
+    return (log_std + _c(0.5 * (LOG_2PI + 1.0), log_std)).sum(-1, keepdim=True)
+
+
+def gauss_sample(mean, log_std, normals):
+    """tf_dist.py:85-86 with the standard normals supplied"""
+    return mean + torch.exp(log_std) * normals
+
+
+def dist_log_std(mean, log_std):
+    """the log_std half of dist_param: pi_latent * 0.0 + log_std (ppo.py:78) -- no gradient into pi_latent"""
+    return mean * 0.0 + log_std
+
+
+def ppo_gauss_predict(arch, weights, obs, normals):
+    """PPO.predict (ppo.py:104-109) with supplied normals: (action [B, A], logp [B, 1], v [B, 1])"""
+    with torch.no_grad():
+        mean, v = forward(arch, weights, obs)
+        ls = torch.from_numpy(np.asarray(weights["pi_logstd"])).to(mean.dtype)
+        x = gauss_sample(mean, ls, torch.from_numpy(np.asarray(normals)).to(mean.dtype))
+        return x.numpy(), gauss_log_prob(x, mean, ls).numpy(), v.numpy()
+
+
+# --------------------------------------------------------------------------- #
 # GAE  (agent side)
 # --------------------------------------------------------------------------- #
 
@@ -382,22 +504,37 @@ def gae(value, reward, done, gamma=GAMMA, lam=LAM):
 # PPO loss / optimiser / train loop
 # --------------------------------------------------------------------------- #
 
+def _surrogate(logp, old_logp, adv, clip_ratio):
+    """the clipped surrogate, xt/model/ppo/__init__.py:4-11"""
+    ratio = torch.exp(logp - old_logp)
+    s1 = ratio * adv
+    s2 = torch.clamp(ratio, 1.0 - clip_ratio, 1.0 + clip_ratio) * adv
+    return torch.minimum(s1, s2).mean()
+
+
+def _critic(v, old_v, target_v, vf_clip):
+    """the clipped value loss, xt/model/ppo/__init__.py:17-25"""
+    l1 = (v - target_v) ** 2
+    vclip = old_v + torch.clamp(v - old_v, -vf_clip, vf_clip)
+    l2 = (vclip - target_v) ** 2
+    return 0.5 * torch.maximum(l1, l2).mean()
+
+
 def ppo_loss(logits, v, action, old_logp, adv, old_v, target_v,
              clip_ratio, ent_coef, vf_clip, critic_coef):
     """xt/model/ppo/__init__.py:4-25 and xt/model/ppo/ppo.py:87-92.  All [B,1] but
     logits [B,A], action [B]."""
-    logp = categorical_logp(logits, action)
-    ratio = torch.exp(logp - old_logp)
-    s1 = ratio * adv
-    s2 = torch.clamp(ratio, 1.0 - clip_ratio, 1.0 + clip_ratio) * adv
-    surr = torch.minimum(s1, s2).mean()
+    surr = _surrogate(categorical_logp(logits, action), old_logp, adv, clip_ratio)
     ent = categorical_entropy(logits).mean()
     actor = -surr - ent_coef * ent
-    l1 = (v - target_v) ** 2
-    vclip = old_v + torch.clamp(v - old_v, -vf_clip, vf_clip)
-    l2 = (vclip - target_v) ** 2
-    critic = 0.5 * torch.maximum(l1, l2).mean()
-    return actor + critic_coef * critic
+    return actor + critic_coef * _critic(v, old_v, target_v, vf_clip)
+
+
+def ppo_gauss_loss(mean, log_std, v, action, old_logp, adv, old_v, target_v, clip_ratio, ent_coef, vf_clip, critic_coef):
+    """ppo_loss with the DiagGaussian head; mean and action [B, A], log_std [1, A], the rest [B, 1]"""
+    ls = dist_log_std(mean, log_std)
+    actor = -_surrogate(gauss_log_prob(action, mean, ls), old_logp, adv, clip_ratio) - ent_coef * gauss_entropy(ls).mean()
+    return actor + critic_coef * _critic(v, old_v, target_v, vf_clip)
 
 
 def clip_by_global_norm(grads, clip):
@@ -405,6 +542,15 @@ def clip_by_global_norm(grads, clip):
     gn = math.sqrt(sum(float((g.double() ** 2).sum()) for g in grads))
     scale = clip / max(gn, clip)
     return [g * scale for g in grads], gn
+
+
+def clip_per_tensor(grads, clipnorm):
+    """Keras `clipnorm`: each gradient tensor g scaled by clipnorm / ||g|| where its norm exceeds clipnorm."""
+    out = []
+    for g in grads:
+        n = float(g.double().pow(2).sum().sqrt())
+        out.append(g * (clipnorm / n) if n > clipnorm else g)
+    return out
 
 
 class TFAdam:
@@ -432,6 +578,23 @@ class TFAdam:
                 m.mul_(self.b1).add_(g, alpha=1 - self.b1)
                 v.mul_(self.b2).addcmul_(g, g, value=1 - self.b2)
                 p.sub_(float(lr_t) * m / (v.sqrt() + self.eps))
+
+
+class KerasAdam(TFAdam):
+    """Keras (OptimizerV2) Adam, as documented for TF-1.15: the tf.train.Adam update with eps 1e-7, optional
+    per-tensor clipnorm, and `decay`: lr / (1 + decay * iterations) with iterations counted before the step."""
+
+    def __init__(self, params, lr, clipnorm=None, decay=0.0, eps=1e-7):
+        super().__init__(params, lr, eps=eps)
+        self.base_lr, self.clipnorm, self.decay, self.iterations = lr, clipnorm, decay, 0
+
+    def step(self, grads):
+        if self.clipnorm:
+            grads = clip_per_tensor(grads, self.clipnorm)
+        f = self.f
+        self.lr = f(self.base_lr) / (f(1) + f(self.decay) * f(self.iterations)) if self.decay else self.base_lr
+        self.iterations += 1
+        super().step(grads)
 
 
 class TFRMSProp:
@@ -464,28 +627,47 @@ def _as_param_list(weights):
     return [torch.from_numpy(np.array(v, _PREC["np"], copy=True)).requires_grad_(True) for v in weights.values()]
 
 
-class PpoLearner:
-    """Restates xt/model/ppo/ppo.py:62-132 (graph + train loop) on torch-CPU."""
+class Learner:
+    """What the learner restatements share: the arch, and the weights as leaf tensors of the working precision, in the
+    order they were given."""
+
+    def __init__(self, arch, weights):
+        self.arch, self.names = arch, list(weights.keys())
+        self.params = _as_param_list(weights)
+
+    def named(self, params=None):
+        return dict(zip(self.names, self.params if params is None else params))
+
+    def weights(self):
+        return OrderedDict((n, p.detach().numpy().copy()) for n, p in zip(self.names, self.params))
+
+
+class PpoLearner(Learner):
+    """Restates xt/model/ppo/ppo.py:62-132 (graph + train loop) on torch-CPU.  The action distribution follows the arch,
+    as in the product: a logstd layer makes it DiagGaussian, its variable one more parameter (last, as TFVariables lists
+    it) that counts toward the global-norm clip and takes Adam steps like the others; actions are then float [N, A]."""
 
     def __init__(self, arch, weights, lr=3e-4, batch_size=200, critic_coef=1.0, ent_coef=1e-3,
                  clip_ratio=0.2, max_grad_norm=5.0, num_sgd_iter=4, vf_clip=5.0):
-        self.arch = arch
-        self.names = list(weights.keys())
-        self.params = _as_param_list(weights)
+        super().__init__(arch, weights)
+        self.logstd = next((name for name, kind, _, _ in arch["layers"] if kind == "logstd"), None)
         self.opt = TFAdam(self.params, lr)
         self.bs, self.cc, self.ec, self.cr = batch_size, critic_coef, ent_coef, clip_ratio
         self.mgn, self.iters, self.vfc = max_grad_norm, num_sgd_iter, vf_clip
         self.last_grad_norm = None
 
-    def weights(self):
-        return OrderedDict((n, p.detach().numpy().copy()) for n, p in zip(self.names, self.params))
-
     def loss_and_grads(self, obs, action, old_logp, adv, old_v, target_v):
-        w = dict(zip(self.names, self.params))
-        logits, v = forward(self.arch, w, obs)
-        tt = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=_PREC["np"])).view(-1, 1)
-        loss = ppo_loss(logits, v, torch.from_numpy(np.ascontiguousarray(action)), tt(old_logp), tt(adv),
-                        tt(old_v), tt(target_v), self.cr, self.ec, self.vfc, self.cc)
+        w = self.named()
+        head, v = forward(self.arch, w, obs)
+        f = _PREC["np"]
+        tt = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=f)).view(-1, 1)   # noqa: E731
+        hp = (self.cr, self.ec, self.vfc, self.cc)
+        if self.logstd is None:
+            loss = ppo_loss(head, v, torch.from_numpy(np.ascontiguousarray(action)), tt(old_logp), tt(adv),
+                            tt(old_v), tt(target_v), *hp)
+        else:
+            act = torch.from_numpy(np.ascontiguousarray(action, dtype=f)).view(head.shape)
+            loss = ppo_gauss_loss(head, w[self.logstd], v, act, tt(old_logp), tt(adv), tt(old_v), tt(target_v), *hp)
         grads = torch.autograd.grad(loss, self.params)
         return loss, grads
 
@@ -573,24 +755,19 @@ def impala_loss(tp_logits_flat, baseline_flat, bp_logits, actions, dones, reward
     return pi_loss + 0.5 * val_loss + 0.01 * ent_loss
 
 
-class ImpalaLearner:
+class ImpalaLearner(Learner):
     """Restates ImpalaCnnOpt's train graph (impala_cnn_opt.py:188-217, :251-265)."""
 
     def __init__(self, arch, weights, lr=0.0005, grad_norm_clip=40.0, sample_batch_step=128, gamma=0.99, opt_type="adam",
                  lr_schedule=None):
-        self.arch, self.names = arch, list(weights.keys())
-        self.params = _as_param_list(weights)
+        super().__init__(arch, weights)
         self.opt = TFAdam(self.params, lr) if opt_type == "adam" else TFRMSProp(self.params, lr)
         self.lr_schedule, self.global_step = (lr_schedule if opt_type == "adam" else None), 0
         self.clip, self.step_len, self.gamma = grad_norm_clip, sample_batch_step, gamma
         self.last_grad_norm = None
 
-    def weights(self):
-        return OrderedDict((n, p.detach().numpy().copy()) for n, p in zip(self.names, self.params))
-
     def loss_and_grads(self, state, bp_logits, actions, dones, rewards):
-        w = dict(zip(self.names, self.params))
-        logits, base = forward(self.arch, w, state)
+        logits, base = forward(self.arch, self.named(), state)
         loss = impala_loss(logits, base[:, 0], bp_logits, actions, dones, rewards, self.step_len, self.gamma)
         return loss, torch.autograd.grad(loss, self.params)
 
@@ -609,64 +786,55 @@ class ImpalaLearner:
 # DQN
 # --------------------------------------------------------------------------- #
 
-def dqn_targets(y_online, target_q, actions, rewards, dones, gamma=0.99, q_next_online=None):
-    """xt/algorithm/dqn/dqn.py:79-95: 1-step TD target written into y[k,a_k].
-    Double-DQN when q_next_online is given (:79-84)."""
-    y = np.array(y_online, np.float32, copy=True)
-    if q_next_online is not None:
-        best = np.argmax(q_next_online, 1)
-        maxq = target_q[np.arange(len(y)), best]
-    else:
-        maxq = np.max(target_q, 1)
+def dqn_targets(y_online, target_q, actions, rewards, dones, gamma=0.99, q_next_online=None, disc=None):
+    """xt/algorithm/dqn/dqn.py:79-95: 1-step TD target written into y[k,a_k], y in float32.
+    Double-DQN when q_next_online is given (:79-84).  `disc` holds a per-row discount (an n-step target, as
+    xtb_dqn_td_loss_grad takes it) that replaces gamma; y then keeps the working precision."""
+    y = np.array(y_online, np.float32 if disc is None else None, copy=True)
+    best = np.argmax(q_next_online if q_next_online is not None else target_q, 1)
+    maxq = target_q[np.arange(len(y)), best]
     for k in range(len(y)):
-        if dones[k]:
-            q = rewards[k]
-        else:
-            q = rewards[k] + gamma * maxq[k]
-        y[k][actions[k]] = q
+        y[k][actions[k]] = rewards[k] if dones[k] else rewards[k] + (gamma if disc is None else disc[k]) * maxq[k]
     return y
 
 
-class DqnLearner:
+class DqnLearner(Learner):
     """Restates DQN.train (xt/algorithm/dqn/dqn.py:61-103) + Keras compile(mse,
     Adam(clipnorm=10)) (xt/model/dqn/dqn_cnn.py:60-61): mse = mean over B*A;
-    clipnorm clips EACH gradient tensor to norm<=10; Adam eps=1e-7."""
+    clipnorm clips EACH gradient tensor to norm<=10; Adam eps=1e-7.  `disc` / `huber` extend the TD target and
+    loss the way xtb_dqn_td_loss_grad does: a per-row discount, and Huber with that delta."""
 
     def __init__(self, arch, weights, lr=0.00015, clipnorm=10.0, gamma=0.99, target_update_freq=1000,
                  double_dqn=False):
-        self.arch, self.names = arch, list(weights.keys())
-        self.params = _as_param_list(weights)
+        super().__init__(arch, weights)
         self.target = [p.detach().clone() for p in self.params]
         self.opt = TFAdam(self.params, lr, eps=1e-7)
         self.clipnorm, self.gamma, self.freq, self.double = clipnorm, gamma, target_update_freq, double_dqn
         self.train_count = 0
 
-    def weights(self):
-        return OrderedDict((n, p.detach().numpy().copy()) for n, p in zip(self.names, self.params))
-
     def predict(self, states, target=False):
-        w = dict(zip(self.names, self.target if target else self.params))
         with torch.no_grad():
-            return forward(self.arch, w, states)[0].numpy()
+            return forward(self.arch, self.named(self.target if target else None), states)[0].numpy()
 
-    def loss_and_grads(self, states, actions, rewards, new_states, dones):
+    def loss_and_grads(self, states, actions, rewards, new_states, dones, disc=None, huber=0.0):
         y_t = self.predict(states)
         tq = self.predict(new_states, target=True)
         qn = self.predict(new_states) if self.double else None
-        y = dqn_targets(y_t, tq, actions, rewards, dones, self.gamma, qn)
-        w = dict(zip(self.names, self.params))
-        q = forward(self.arch, w, states)[0]
-        loss = ((q - torch.from_numpy(y)) ** 2).mean()
+        y = dqn_targets(y_t, tq, actions, rewards, dones, self.gamma, qn, disc)
+        q = forward(self.arch, self.named(), states)[0]
+        diff = q - torch.from_numpy(y)
+        if huber > 0:
+            ad = diff.abs()
+            per = torch.where(ad <= huber, 0.5 * diff * diff, huber * (ad - 0.5 * huber))
+        else:
+            per = diff * diff
+        loss = per.mean()
         return loss, torch.autograd.grad(loss, self.params), y
 
-    def train(self, states, actions, rewards, new_states, dones):
-        loss, grads, _ = self.loss_and_grads(states, actions, rewards, new_states, dones)
+    def train(self, states, actions, rewards, new_states, dones, disc=None, huber=0.0):
+        loss, grads, _ = self.loss_and_grads(states, actions, rewards, new_states, dones, disc, huber)
         if self.clipnorm:
-            cg = []
-            for g in grads:
-                n = float(g.double().pow(2).sum().sqrt())
-                cg.append(g * (self.clipnorm / n) if n > self.clipnorm else g)
-            grads = cg
+            grads = clip_per_tensor(grads, self.clipnorm)
         self.opt.step(grads)
         self.train_count += 1
         if self.train_count % self.freq == 0:

@@ -3,46 +3,16 @@ impala_cnn.py), on top of oracle/xt_oracle.py.  TEST INFRASTRUCTURE ONLY.
 
 Pinned by tests/golden/impala_keras.npz (the reference's own _train_proc / train slicing and impala_loss closures,
 executed by tests/golden/make_golden_impala_keras.py): the V-trace variant, the slices, the loss value.  Restated from
-documented TF-1.15 behaviour and unpinned, like tf.train.AdamOptimizer in xt_oracle:
+documented TF-1.15 behaviour and unpinned, like tf.train.AdamOptimizer and KerasAdam in xt_oracle:
   * training_arrays.fit_loop: one np.random.shuffle(np.arange(n)) per fit call, consecutive batches of 128, the last
     one ragged;
-  * OptimizerV2 `decay`: lr / (1 + decay * iterations), iterations counted before the step; clipnorm per tensor;
   * the epoch loss fit reports: per-batch losses weighted by batch size, i.e. sum over rows of the row loss / n."""
-from collections import OrderedDict
-
 import numpy as np
 import torch
 
 from oracle import xt_oracle as orc
 
 FIT_BATCH = 128
-
-
-def _dense(name, src, n, act):
-    return (name, "dense", src, dict(n=n, act=act))
-
-
-def impala_mlp_arch(state_dim=(4,), action_dim=2, hidden_size=128, num_layers=1):
-    """impala_mlp.py:39-50 (the softmax of output_actions is applied by the loss / predict below)."""
-    layers, src = [], "obs"
-    for i in range(num_layers):
-        name = "dense" if i == 0 else "dense_%d" % i
-        layers.append(_dense(name, src, hidden_size, "relu"))
-        src = name
-    layers += [_dense("output_actions", src, action_dim, None), _dense("output_value", src, 1, None)]
-    return dict(input_dtype="float32", state_dim=tuple(state_dim), scale=1.0, layers=layers,
-                outputs=["output_actions", "output_value"])
-
-
-def impala_cnn_arch(state_dim=(84, 84, 4), action_dim=4):
-    """impala_cnn.py:44-56."""
-    layers = [("conv2d", "conv", "obs", dict(k=8, s=4, cout=32, pad="valid", act="relu")),
-              ("conv2d_1", "conv", "conv2d", dict(k=4, s=2, cout=64, pad="valid", act="relu")),
-              ("conv2d_2", "conv", "conv2d_1", dict(k=3, s=1, cout=64, pad="valid", act="relu")),
-              _dense("dense", "conv2d_2", 256, "relu"),
-              _dense("output_actions", "dense", action_dim, None), _dense("output_value", "dense", 1, None)]
-    return dict(input_dtype="uint8", state_dim=tuple(state_dim), scale=1.0 / 255.0, layers=layers,
-                outputs=["output_actions", "output_value"])
 
 
 # --------------------------------------------------------------------------------------------------------- V-trace
@@ -83,28 +53,6 @@ def impala_loss_value(probs, y, adv, ent=0.01):
     return float((adv.reshape(-1, 1) * (-y * lp) - ent * (-p * lp)).mean())
 
 
-# --------------------------------------------------------------------------------------------------------- optimiser
-class KerasAdam(orc.TFAdam):
-    """Keras (OptimizerV2) Adam: the tf.train.Adam update with eps 1e-7, optional per-tensor clipnorm, and `decay`:
-    lr / (1 + decay * iterations) with iterations counted before the step."""
-
-    def __init__(self, params, lr, clipnorm=None, decay=0.0, eps=1e-7):
-        super().__init__(params, lr, eps=eps)
-        self.base_lr, self.clipnorm, self.decay, self.iterations = lr, clipnorm, decay, 0
-
-    def step(self, grads):
-        if self.clipnorm:
-            out = []
-            for g in grads:
-                n = float(g.double().pow(2).sum().sqrt())
-                out.append(g * (self.clipnorm / n) if n > self.clipnorm else g)
-            grads = out
-        f = self.f
-        self.lr = f(self.base_lr) / (f(1) + f(self.decay) * f(self.iterations)) if self.decay else self.base_lr
-        self.iterations += 1
-        super().step(grads)
-
-
 def fit_batches(n, rng=np.random):
     """training_arrays.fit_loop(shuffle=True): the minibatches of one fit call."""
     order = np.arange(n)
@@ -112,22 +60,19 @@ def fit_batches(n, rng=np.random):
     return [order[s:s + FIT_BATCH] for s in range(0, n, FIT_BATCH)]
 
 
-class ImpalaKerasLearner:
-    """ImpalaMlp / ImpalaCnn (model.fit) and IMPALA.train on torch-CPU, in the precision of xt_oracle.precision."""
+class ImpalaKerasLearner(orc.Learner):
+    """ImpalaMlp / ImpalaCnn (model.fit) and IMPALA.train on torch-CPU, in the precision of xt_oracle.precision; the
+    archs are xt_oracle.impala_mlp_arch / impala_keras_cnn_arch."""
 
     def __init__(self, arch, weights, lr=3e-4, clipnorm=None, decay=0.0, ent=0.01, gamma=0.99, batch_size=512):
-        self.arch, self.names = arch, list(weights.keys())
-        self.params = orc._as_param_list(weights)
-        self.opt = KerasAdam(self.params, lr, clipnorm=clipnorm, decay=decay)
+        super().__init__(arch, weights)
+        self.opt = orc.KerasAdam(self.params, lr, clipnorm=clipnorm, decay=decay)
         self.ent, self.gamma, self.batch_size = ent, gamma, batch_size
         self.last = {}
 
-    def weights(self):
-        return OrderedDict((n, p.detach().numpy().copy()) for n, p in zip(self.names, self.params))
-
     def predict(self, obs):
         with torch.no_grad():
-            logits, v = orc.forward(self.arch, dict(zip(self.names, self.params)), obs)
+            logits, v = orc.forward(self.arch, self.named(), obs)
         return torch.softmax(logits, -1).numpy(), v.numpy()
 
     def fit(self, obs, adv, y, tv, rng=np.random):
@@ -135,7 +80,7 @@ class ImpalaKerasLearner:
         n, total = len(obs), 0.0
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a, orc._PREC["np"]))   # noqa: E731
         for mb in fit_batches(n, rng):
-            logits, v = orc.forward(self.arch, dict(zip(self.names, self.params)), obs[mb])
+            logits, v = orc.forward(self.arch, self.named(), obs[mb])
             rl = row_losses(logits, v, t(y[mb]), t(adv[mb]), t(tv[mb]), self.ent)
             grads = torch.autograd.grad(rl.mean(), self.params)
             self.opt.step(grads)

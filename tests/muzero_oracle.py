@@ -8,6 +8,8 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from oracle import xt_oracle as orc
+
 WEIGHT_DECAY = 1e-4
 
 
@@ -46,32 +48,13 @@ def support_value(probs, vmin, vmax):
     return np.clip(h_inv(e) + vmin, vmin, vmax)
 
 
-def param_count(arch):
-    shapes = {"obs": tuple(arch["state_dim"])}
-    n = 0
-    for name, kind, src, sp in arch["layers"]:
-        ish = shapes[src]
-        if kind == "conv":
-            oh, ow = (ish[0] - sp["k"]) // sp["s"] + 1, (ish[1] - sp["k"]) // sp["s"] + 1
-            n += sp["k"] * sp["k"] * ish[2] * sp["cout"] + sp["cout"]
-            shapes[name] = (oh, ow, sp["cout"])
-        else:
-            n += int(np.prod(ish)) * sp["n"] + sp["n"]
-            shapes[name] = (sp["n"],)
-    return n
-
-
 def weight_shapes(arch):
-    shapes, out = {"obs": tuple(arch["state_dim"])}, []
-    for name, kind, src, sp in arch["layers"]:
-        ish = shapes[src]
-        if kind == "conv":
-            out += [(sp["k"], sp["k"], ish[2], sp["cout"]), (sp["cout"],)]
-            shapes[name] = ((ish[0] - sp["k"]) // sp["s"] + 1, (ish[1] - sp["k"]) // sp["s"] + 1, sp["cout"])
-        else:
-            out += [(int(np.prod(ish)), sp["n"]), (sp["n"],)]
-            shapes[name] = (sp["n"],)
-    return out
+    """the Keras list's shapes of one network, kernel then bias per layer"""
+    return list(orc.param_shapes(arch).values())
+
+
+def param_count(arch):
+    return sum(int(np.prod(s)) for s in weight_shapes(arch))
 
 
 def split(archs, weights):

@@ -8,13 +8,10 @@ import numpy as np
 import pytest
 import torch
 
-import activations_oracle as ao
 from oracle import np_f64
 from oracle import xt_oracle as orc
 from xingtian_b200 import capi
 from xingtian_b200.model import archs
-
-ao.install()
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden", "activations.npz")
@@ -26,7 +23,7 @@ def _grid():
     return np.unique(x)
 
 
-@pytest.mark.parametrize("act", ao.NEW)
+@pytest.mark.parametrize("act", np_f64.NEW)
 def test_torch_and_numpy_f64_agree(act):
     x = _grid()
     t = orc._ACT[act](torch.from_numpy(x)).numpy()
@@ -39,15 +36,15 @@ def test_torch_and_numpy_f64_agree(act):
 
 def test_closed_forms_and_constants():
     x = _grid()
-    f = {k: np_f64._ACT[k](x) for k in ao.NEW}
+    f = {k: np_f64._ACT[k](x) for k in np_f64.NEW}
     with np.errstate(over="ignore"):
         np.testing.assert_allclose(f["sigmoid"], 1 / (1 + np.exp(-x)), rtol=1e-15)
     np.testing.assert_allclose(f["softplus"], np.logaddexp(0.0, x), rtol=1e-15)          # log(1 + e^x), accurately
     np.testing.assert_allclose(f["softsign"], x / (1 + np.abs(x)), rtol=1e-15)
     np.testing.assert_array_equal(f["leaky_relu"], np.maximum(x, 0.2 * x))
     np.testing.assert_allclose(f["elu"], np.where(x > 0, x, np.exp(np.minimum(x, 0)) - 1), rtol=1e-9, atol=1e-15)
-    assert ao.SELU_SCALE == 1.0507009873554805 and ao.SELU_ALPHA == 1.6732632423543772
-    np.testing.assert_allclose(f["selu"][x < 0] / ao.SELU_SCALE / ao.SELU_ALPHA, np.expm1(x[x < 0]), rtol=1e-15)
+    assert np_f64.SELU_SCALE == 1.0507009873554805 and np_f64.SELU_ALPHA == 1.6732632423543772
+    np.testing.assert_allclose(f["selu"][x < 0] / np_f64.SELU_SCALE / np_f64.SELU_ALPHA, np.expm1(x[x < 0]), rtol=1e-15)
     np.testing.assert_allclose(f["swish"], x / (1 + np.exp(-x)), rtol=1e-14)
     np.testing.assert_allclose(f["gelu"], 0.5 * x * (1 + np.tanh(np.sqrt(2 / np.pi) * (x + 0.044715 * x ** 3))), rtol=1e-15)
     assert abs(f["softplus"][np.searchsorted(x, 30.0)] - 30.0) < 1e-12          # stable at large x
@@ -68,7 +65,7 @@ def test_gelu_matches_reference_golden():
     assert np.all(np.abs(got32 - ref) <= tol)
 
 
-@pytest.mark.parametrize("act", ao.NEW)
+@pytest.mark.parametrize("act", np_f64.NEW)
 def test_kernel_derivative_rules_match_autograd(act):
     x = _grid()
     if act in ("leaky_relu", "selu", "elu", "softplus"):
@@ -77,7 +74,7 @@ def test_kernel_derivative_rules_match_autograd(act):
     z = torch.from_numpy(x).requires_grad_(True)
     y = orc._ACT[act](z)
     (g,) = torch.autograd.grad(y.sum(), z)
-    rule = ao.grad_rule(act, y.detach().numpy(), x)
+    rule = np_f64.grad_rule(act, y.detach().numpy(), x)
     g = g.numpy()
     err = np.abs(rule - g) / np.maximum(np.abs(g), 1.0)
     assert float(np.max(err)) <= 1e-10, (act, float(np.max(err)), x[np.argmax(err)])

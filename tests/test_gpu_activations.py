@@ -17,8 +17,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import activations_oracle as ao
-import gauss_oracle as gor
+from oracle import np_f64
 from oracle import xt_oracle as orc
 from test_gpu_kernels import (F32_FLOOR, REL, RELU_FLIP_F32, RELU_FLIP_TC, TC_FWD_BOUND, TC_GRAD_BOUND, _keepalive, dev,  # noqa: F401
                               l2_rel, rel_err, tc_mode, xb)
@@ -27,8 +26,6 @@ from test_gpu_plugins import alg_cfg
 from test_gpu_ppo_gauss import _desc
 
 pytestmark = pytest.mark.gpu
-
-ao.install()
 
 
 @pytest.fixture(autouse=True)
@@ -45,16 +42,16 @@ def _restore_module_config():
 
 
 SUBSET = ["s2d_84x84_k8_valid", "width_10x10_16to48_k3s1_same", "dag_two_tc_convs", "dense_80x48", "dense_4096x16", "fb_cin8"]
-KINKED = {"leaky_relu": lambda p: ao.LEAKY_ALPHA * p,
-          "selu": lambda p: ao.SELU_SCALE * ao.SELU_ALPHA * torch.expm1(torch.clamp(p, max=0))}
+KINKED = {"leaky_relu": lambda p: np_f64.LEAKY_ALPHA * p,
+          "selu": lambda p: np_f64.SELU_SCALE * np_f64.SELU_ALPHA * torch.expm1(torch.clamp(p, max=0))}
 
 
 def _act_t(act, p, mask):
     if act in KINKED and mask is not None:
         m = torch.from_numpy(mask).reshape(p.shape)
-        pos = p * (ao.SELU_SCALE if act == "selu" else 1.0)
+        pos = p * (np_f64.SELU_SCALE if act == "selu" else 1.0)
         return torch.where(m, pos, KINKED[act](p))
-    return ao.TORCH[act](p)
+    return orc._ACT[act](p)
 
 
 def _reference(arch, w, obs, dt, act, gh, masks=None):
@@ -84,7 +81,7 @@ def _reference(arch, w, obs, dt, act, gh, masks=None):
             {k: params[k].grad.numpy() for k in w})
 
 
-@pytest.mark.parametrize("act", ao.NEW)
+@pytest.mark.parametrize("act", np_f64.NEW)
 @pytest.mark.parametrize("case", SUBSET)
 def test_layer_engine(xb, tc_mode, case, act):
     from xingtian_b200.engine import Net
@@ -150,10 +147,9 @@ def _model(shape, act, B):
 def _arch(shape, act):
     s = SHAPES[shape]
     if s["model"] == "PpoCnn":
-        a = orc.ppo_cnn_arch(action_dim=s["A"], hidden_sizes=tuple(s["hidden"]), activation=act)
-    else:
-        a = orc.ppo_mlp_arch(state_dim=tuple(s["state_dim"]), action_dim=s["A"], hidden_sizes=tuple(s["hidden"]), activation=act)
-    return gor.with_logstd(a) if s["gauss"] else a
+        return orc.ppo_cnn_arch(action_dim=s["A"], hidden_sizes=tuple(s["hidden"]), activation=act, diag_gaussian=s["gauss"])
+    return orc.ppo_mlp_arch(state_dim=tuple(s["state_dim"]), action_dim=s["A"], hidden_sizes=tuple(s["hidden"]),
+                            activation=act, diag_gaussian=s["gauss"])
 
 
 def _step_data(shape, arch, w, B, seed):
@@ -164,9 +160,9 @@ def _step_data(shape, arch, w, B, seed):
     else:
         obs = rng.standard_normal((B,) + tuple(s["state_dim"])).astype(np.float32)
     if s["gauss"]:
-        mean, v = [t.detach().numpy() for t in gor.forward(arch, w, obs)]
+        mean, v = [t.detach().numpy() for t in orc.forward(arch, w, obs)]
         act = (mean + np.exp(w["pi_logstd"]) * 1.2 * rng.standard_normal((B, s["A"]))).astype(np.float32)
-        lp = gor.log_prob(torch.from_numpy(act), torch.from_numpy(mean), torch.from_numpy(w["pi_logstd"])).numpy()
+        lp = orc.gauss_log_prob(torch.from_numpy(act), torch.from_numpy(mean), torch.from_numpy(w["pi_logstd"])).numpy()
     else:
         logits, v = [t.detach().numpy() for t in orc.forward(arch, w, obs)]
         act = rng.integers(0, s["A"], B).astype(np.int32)
@@ -178,14 +174,13 @@ def _step_data(shape, arch, w, B, seed):
 
 
 def _oracle_step(shape, arch, w, obs, label, B, dt):
-    learner = gor.PpoLearner if SHAPES[shape]["gauss"] else orc.PpoLearner
     with orc.precision(dt):
-        ref = learner(arch, w, batch_size=B, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=1, vf_clip=0.5)
+        ref = orc.PpoLearner(arch, w,batch_size=B, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=1, vf_clip=0.5)
         loss, grads = ref.loss_and_grads(obs, *label)
         return float(loss.detach()), {k: g.detach().numpy() for k, g in zip(ref.names, grads)}
 
 
-@pytest.mark.parametrize("act", ao.NEW)
+@pytest.mark.parametrize("act", np_f64.NEW)
 @pytest.mark.parametrize("shape", list(SHAPES))
 def test_ppo_train_step_against_float64(xb, tc_mode, shape, act):
     """one SGD step with fused heads on and off: loss and every gradient at most 4x torch-CPU fp32's distance from
@@ -224,7 +219,7 @@ def test_ppo_train_step_against_float64(xb, tc_mode, shape, act):
         assert l2_rel(got[1][1][k], got[0][1][k]) < 1e-4, k
 
 
-@pytest.mark.parametrize("act", ao.NEW)
+@pytest.mark.parametrize("act", np_f64.NEW)
 @pytest.mark.parametrize("shape", list(SHAPES))
 def test_predict_against_oracle(xb, tc_mode, shape, act):
     """predict with supplied uniforms / normals: log-probs and values within 1e-3 of the float64 oracle, actions exact
@@ -241,7 +236,7 @@ def test_predict_against_oracle(xb, tc_mode, shape, act):
         n = rng.standard_normal((B, s["A"])).astype(np.float32)
         a, lp, v = m.predict(obs, normals=n)
         with orc.precision("f64"):
-            ra, rlp, rv = gor.predict(arch, w64, obs.astype(np.float64), n.astype(np.float64))
+            ra, rlp, rv = orc.ppo_gauss_predict(arch, w64, obs.astype(np.float64), n.astype(np.float64))
         assert rel_err(a, ra) < 1e-3
     else:
         u = (rng.random((B, s["A"])) * 0.99 + 0.005).astype(np.float32)

@@ -12,7 +12,6 @@ import numpy as np
 import pytest
 import torch
 
-import dueling_oracle as dor
 from oracle import xt_oracle as orc
 from parity_record import record as _record
 from test_gpu_kernels import (F32_FLOOR, REL, TC_FWD_BOUND, TC_GRAD_BOUND, _keepalive, dev, l2_rel, rel_err,  # noqa: F401
@@ -46,7 +45,7 @@ def _mlp(A, act):
 
 
 def _weights(arch, seed=11):
-    w = dor.init_weights(arch, seed=seed)
+    w = orc.init_weights(arch, seed=seed)
     rng = np.random.default_rng(seed + 1)
     for k in w:                                   # non-zero biases so the bias paths are exercised
         if k.endswith("/bias"):
@@ -62,7 +61,7 @@ def _reference(arch, w, x, dt, gh=None, masks=None):
     t, pre = {"obs": xt / 255.0 if arch["input_dtype"] == "uint8" else xt}, {}
     for name, kind, src, sp in arch["layers"]:
         if kind == "dueling":
-            p = dor.combine(t[src[0]], t[src[1]])
+            p = orc.dueling_combine(t[src[0]], t[src[1]])
         elif kind == "conv":
             a = t[src].permute(0, 3, 1, 2)
             p = torch.nn.functional.conv2d(a, params[name + "/kernel"].permute(3, 2, 0, 1), params[name + "/bias"],
@@ -92,7 +91,7 @@ def _engine_parity(arch, B, tc, tag):
     rng = np.random.default_rng(B + 7)
     shape = (B,) + tuple(arch["state_dim"])
     obs = rng.integers(0, 256, shape, dtype=np.uint8) if arch["input_dtype"] == "uint8" else rng.standard_normal(shape).astype(np.float32)
-    sizes = dor.tensor_shapes(arch)
+    sizes = orc.tensor_shapes(arch)
     gh = {h: rng.standard_normal((B, int(np.prod(sizes[h])))).astype(np.float32) for h in arch["outputs"]}
     obs_d = dev(obs)
     net.forward(obs_d, B)
@@ -230,9 +229,9 @@ def _fill(alg, s, a, r, s2, d):
 def _run_vs_oracle(alg, n, batch, steps, A, double=False, tol=5e-3, upd_tol=5e-2):
     s, a, r, s2, d = _transitions(n, A)
     w0 = alg.get_weights()
-    arch = dor.dqn_cnn_arch(action_dim=A, dueling=True)
-    assert list(w0) == list(dor.param_shapes(arch))
-    ref = dor.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=2, double_dqn=double)
+    arch = orc.dqn_cnn_arch(action_dim=A, dueling=True)
+    assert list(w0) == list(orc.param_shapes(arch))
+    ref = orc.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=2, double_dqn=double)
     _fill(alg, s, a, r, s2, d)
     for step in range(steps):
         random.seed(step)
@@ -279,8 +278,8 @@ def test_dueling_nstep_huber_step_matches_oracle(xb):
     disc = np.where(d, 0.0, 0.99 ** 3).astype(np.float32)
     r = (r + rng.standard_normal(n)).astype(np.float32)
     w0 = model.get_weights()
-    arch = dor.dqn_cnn_arch(action_dim=A, dueling=True)
-    ref = dor.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
+    arch = orc.dqn_cnn_arch(action_dim=A, dueling=True)
+    ref = orc.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
     loss = torch.zeros(1, dtype=torch.float32, device="cuda")
     model.train_td_device(alg.target_actor, dev(s), dev(a.astype(np.int32)), dev(r), dev(s2), dev(d.astype(np.uint8)), n, 0.99,
                           loss, disc=dev(disc), huber_delta=alg.huber_delta)
@@ -331,10 +330,10 @@ def test_fused_dueling_step_matches_layer_by_layer(xb, A):
     assert abs(lf - lu) < 1e-4 * max(1.0, abs(lu)), (lf, lu)
     upf = np.concatenate([(wf[k] - w0[k]).ravel() for k in w0]); upu = np.concatenate([(wu[k] - w0[k]).ravel() for k in w0])
     assert l2_rel(upf, upu) < 1e-2
-    arch = dor.dqn_cnn_arch(action_dim=A, dueling=True)
-    ref = dor.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
+    arch = orc.dqn_cnn_arch(action_dim=A, dueling=True)
+    ref = orc.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
     with orc.precision("f64"):
-        ref = dor.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
+        ref = orc.DqnLearner(arch, w0, lr=0.00015, clipnorm=10.0, target_update_freq=1000)
         rl = ref.train(*batch)
         rw = ref.weights()
     rup = np.concatenate([(rw[k] - w0[k]).ravel() for k in w0])
@@ -359,13 +358,13 @@ def test_dueling_weight_io(xb, tmp_path):
     assert not np.array_equal(fresh.predict(x), m.predict(x))
     fresh.load_model(path)
     np.testing.assert_array_equal(fresh.predict(x), m.predict(x))
-    q = dor.forward(dor.dqn_cnn_arch(action_dim=18, dueling=True), w, x)[0].numpy()
+    q = orc.forward(orc.dqn_cnn_arch(action_dim=18, dueling=True), w, x)[0].numpy()
     assert rel_err(m.predict(x), q) < 1e-3
     mlp = DqnMlp({"state_dim": [4], "action_dim": 2, "model_config": {"dueling": True, "init_seed": 1}})
-    ref = dor.init_weights(dor.dqn_mlp_arch(dueling=True), seed=4)
+    ref = orc.init_weights(orc.dqn_mlp_arch(dueling=True), seed=4)
     mlp.set_weights(dict(ref))
     got = mlp.get_weights()
     assert list(got) == ["dense/kernel", "dense/bias", "dense_1/kernel", "dense_1/bias", "dense_2/kernel", "dense_2/bias"]
     assert all(np.array_equal(got[k], ref[k]) for k in ref)
     xs = np.random.default_rng(1).standard_normal((7, 4)).astype(np.float32)
-    assert rel_err(mlp.predict(xs), dor.forward(dor.dqn_mlp_arch(dueling=True), ref, xs)[0].numpy()) < 1e-5
+    assert rel_err(mlp.predict(xs), orc.forward(orc.dqn_mlp_arch(dueling=True), ref, xs)[0].numpy()) < 1e-5

@@ -76,7 +76,7 @@ def test_vtrace_matches_float64(xb, n_traj, L, A):
     alg.train()
     pg, tv = alg.pg_adv.cpu().numpy(), alg.target_value.cpu().numpy()
     with orc.precision("f64"):
-        ref = iko.ImpalaKerasLearner(iko.impala_mlp_arch(action_dim=A), w0)
+        ref = iko.ImpalaKerasLearner(orc.impala_mlp_arch(action_dim=A), w0)
         probs, values = ref.predict(np.concatenate([t["cur_state"] for t in trajs]))
     st = lambda k: np.stack([np.asarray(t[k]) for t in trajs])   # noqa: E731
     rpg, rtv = iko.vtrace(probs.reshape(n_traj, L + 1, A), values.reshape(n_traj, L + 1), st("action"), st("real_action"),
@@ -112,7 +112,7 @@ def test_fit_matches_oracle(xb, tc, kind, A):
     lib.xtb_set_tc_mode(tc)
     try:
         model = _mlp(A) if kind == "mlp" else _cnn(A)
-        arch = iko.impala_mlp_arch(action_dim=A) if kind == "mlp" else iko.impala_cnn_arch(action_dim=A)
+        arch = orc.impala_mlp_arch(action_dim=A) if kind == "mlp" else orc.impala_keras_cnn_arch(action_dim=A)
         assert list(model.get_weights()) == list(orc.param_shapes(arch))
         torch.cuda.synchronize()
         n0 = lib.xtb_launch_count()
@@ -128,7 +128,7 @@ def test_adam_decay_matches_oracle(xb):
     """an exaggerated decay (0.1) over 5 Adam steps (640 rows), and not the undecayed result"""
     model = _mlp(4, LR=0.01)
     model.opt.set_decay(0.1)
-    arch = iko.impala_mlp_arch(action_dim=4)
+    arch = orc.impala_mlp_arch(action_dim=4)
     loss, rloss, w0, w1, rw = _fit_case(model, arch, 640, 9, None, decay=0.1, lr=0.01)
     assert abs(loss - rloss) < 5e-3 * max(1.0, abs(rloss)), (loss, rloss)
     err = l2_rel(_upd(w1, w0), _upd(rw, w0))
@@ -167,7 +167,7 @@ def _run_alg(alg, arch, trajs_per_call, L, A, state_dim, batch, calls=3, clipnor
 def test_impala_cartpole_config_matches_oracle(xb):
     """examples/cartpole_impala.yaml: ImpalaMlp [4] -> 2, episode_len 200, BATCH_SIZE 800, 2 trajectories per train"""
     alg = _alg("ImpalaMlp", 2, 200, 800, [4])
-    _run_alg(alg, iko.impala_mlp_arch(), 2, 200, 2, (4,), 800)
+    _run_alg(alg, orc.impala_mlp_arch(), 2, 200, 2, (4,), 800)
     s = np.random.default_rng(0).standard_normal(4).astype(np.float32)
     p, v = alg.predict(s)
     assert p.shape == (1, 2) and v.shape == (1, 1) and abs(float(p.sum()) - 1.0) < 1e-5
@@ -176,7 +176,7 @@ def test_impala_cartpole_config_matches_oracle(xb):
 def test_impala_cnn_two_slices_matches_oracle(xb):
     """uint8 ImpalaCnn, 4 x 50 steps, BATCH_SIZE 150: slices of 150 (128 + 22) and 50 rows"""
     alg = _alg("ImpalaCnn", 4, 50, 150, [84, 84, 4])
-    _run_alg(alg, iko.impala_cnn_arch(), 4, 50, 4, (84, 84, 4), 150, clipnorm=40.0, decay=5.12e-9)
+    _run_alg(alg, orc.impala_keras_cnn_arch(), 4, 50, 4, (84, 84, 4), 150, clipnorm=40.0, decay=5.12e-9)
 
 
 def test_graph_replay_equals_eager(xb):
@@ -264,6 +264,6 @@ def test_save_load_round_trip(xb, tmp_path):
     for a, b in zip(fresh.predict([x, None]), m.predict([x, None])):
         np.testing.assert_array_equal(a, b)
     with orc.precision("f64"):
-        p, v = iko.ImpalaKerasLearner(iko.impala_cnn_arch(action_dim=18), w).predict(x)
+        p, v = iko.ImpalaKerasLearner(orc.impala_keras_cnn_arch(action_dim=18), w).predict(x)
     got = m.predict([x, None])
     assert rel_err(got[0], p) < 1e-3 and rel_err(got[1], v) < 1e-3

@@ -1,7 +1,7 @@
 """The optimiser step that ends every training step (csrc/optim.cuh: sqnorm_kernel, then adam_kernel or rmsprop_kernel)
 against float64, and the weight-blob refresh those kernels perform, bit for bit against bp_wprep_kernel.
 
-Step: the oracle's tf.train.Adam (through the Keras restatement of tests/impala_keras_oracle.py for per-tensor clipnorm
+Step: the oracle's tf.train.Adam (through its Keras restatement, KerasAdam, for per-tensor clipnorm
 and `decay`) and centred RMSProp, with clip_by_global_norm, under precision("f64") as the yardstick and precision("f32")
 as the torch-CPU fp32 reference.  grad_scale multiplies the gradient before clipping (include/xtb200.h).  Segment layouts
 reach the optimiser's scalar paths: chunks that start off a multiple of 4 elements, 1..7-element tensors several to one
@@ -22,8 +22,6 @@ import numpy as np
 import pytest
 import torch
 
-import dueling_oracle as dor
-from impala_keras_oracle import KerasAdam
 from oracle import xt_oracle as orc
 from parity_record import record as _record
 from test_gpu_kernels import F32_FLOOR, REL, _keepalive, dev, l2_rel, rel_err, xb  # noqa: F401
@@ -66,7 +64,7 @@ REAL = {
     "ppo_mlp": lambda: _offsets(orc.param_shapes(orc.ppo_mlp_arch())),
     "ppo_cnn": lambda: _offsets(orc.param_shapes(orc.ppo_cnn_arch())),
     "impala_cnn": lambda: _offsets(orc.param_shapes(orc.impala_cnn_arch())),
-    "dqn_cnn_dueling": lambda: _offsets(dor.param_shapes(dor.dqn_cnn_arch(dueling=True))),
+    "dqn_cnn_dueling": lambda: _offsets(orc.param_shapes(orc.dqn_cnn_arch(dueling=True))),
 }
 BIG = {"ppo_cnn": 847493, "impala_cnn": 1005109, "dqn_cnn_dueling": 882341}
 BIG_ROWS = {("adam", "global"), ("adam", "per_tensor"), ("rmsprop", "global")}   # what the products run
@@ -124,14 +122,6 @@ def _gradients(offs, gs, eps, seed):
     return out, clip_global
 
 
-def _clip_per_tensor(gl, clip):
-    out = []
-    for g in gl:
-        n = float(g.double().pow(2).sum().sqrt())
-        out.append(g * (clip / n) if n > clip else g)
-    return out
-
-
 def _reference(offs, opt, mode, clip, gs, grads, lrs, decay, p0, prec):
     """parameters, optimiser state and pre-clip global norms of the oracle in `prec`"""
     dt = torch.float64 if prec == "f64" else torch.float32
@@ -139,7 +129,7 @@ def _reference(offs, opt, mode, clip, gs, grads, lrs, decay, p0, prec):
     with orc.precision(prec):
         ps = [torch.from_numpy(p0[a:b]).to(dt).clone() for a, b in segs]     # updated in place: never alias p0
         if opt == "adam":
-            o = KerasAdam(ps, LR, clipnorm=clip if mode == "per_tensor" else None, decay=decay, eps=ADAM_EPS)
+            o = orc.KerasAdam(ps, LR, clipnorm=clip if mode == "per_tensor" else None, decay=decay, eps=ADAM_EPS)
             o.b1, o.b2 = BETA1, BETA2
         else:
             o = orc.TFRMSProp(ps, LR, decay=RMS_RHO, eps=RMS_EPS)
@@ -150,7 +140,7 @@ def _reference(offs, opt, mode, clip, gs, grads, lrs, decay, p0, prec):
             if mode == "global":
                 gl, _ = orc.clip_by_global_norm(gl, clip)
             elif mode == "per_tensor" and opt == "rmsprop":
-                gl = _clip_per_tensor(gl, clip)                # (KerasAdam clips per tensor itself)
+                gl = orc.clip_per_tensor(gl, clip)            # (KerasAdam clips per tensor itself)
             if opt == "adam":
                 o.base_lr = lr
             else:
@@ -299,7 +289,7 @@ def _blob_nets():
             for case, (make, B, max_batch, gather, expect) in CASES.items()}
     nets["ppo_cnn"] = (orc.ppo_cnn_arch, 64)
     nets["impala_cnn"] = (orc.impala_cnn_arch, 64)
-    nets["dqn_cnn_dueling"] = (lambda: dor.dqn_cnn_arch(dueling=True), 64)
+    nets["dqn_cnn_dueling"] = (lambda: orc.dqn_cnn_arch(dueling=True), 64)
     return nets
 
 

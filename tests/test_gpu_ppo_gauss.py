@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 import torch
 
-import gauss_oracle as gor
 from oracle import xt_oracle as orc
 from test_gpu_kernels import RELU_FLIP_TC, _keepalive, dev, l2_rel, rel_err, tc_mode, xb  # noqa: F401
 from test_gpu_plugins import alg_cfg
@@ -48,8 +47,8 @@ def test_sample_with_supplied_normals(xb, A):
     n = rng.standard_normal((B, A)).astype(np.float32)
     act, logp = _sample(xb["lib"], mean, ls, n)
     with orc.precision("f64"):
-        x = gor.sample(torch.from_numpy(mean).double(), torch.from_numpy(ls).double(), torch.from_numpy(n).double())
-        lp = gor.log_prob(x, torch.from_numpy(mean).double(), torch.from_numpy(ls).double())
+        x = orc.gauss_sample(torch.from_numpy(mean).double(), torch.from_numpy(ls).double(), torch.from_numpy(n).double())
+        lp = orc.gauss_log_prob(x, torch.from_numpy(mean).double(), torch.from_numpy(ls).double())
     assert rel_err(act, x.numpy()) < 1e-6
     assert rel_err(logp, lp.numpy().ravel()) < 1e-5
     if A in (1, 3, 6):     # the reference's own DiagGaussianDist, executed over the TF shim
@@ -88,7 +87,7 @@ def _loss_inputs(B, A, seed):
     act = (rng.standard_normal((N, A)) * 1.3).astype(np.float32)
     act[idx] += mean
     with orc.precision("f64"):
-        lp = gor.log_prob(torch.from_numpy(act[idx]).double(), torch.from_numpy(mean).double(), torch.from_numpy(ls).double()).numpy()
+        lp = orc.gauss_log_prob(torch.from_numpy(act[idx]).double(), torch.from_numpy(mean).double(), torch.from_numpy(ls).double()).numpy()
     old_logp = np.zeros((N, 1), np.float32)
     old_logp[idx] = lp + 0.5 * rng.standard_normal((B, 1))      # ratio on both sides of the clip
     adv = rng.standard_normal((N, 1)).astype(np.float32)
@@ -101,7 +100,7 @@ def _oracle_loss(d, dt, hp):
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dt)   # noqa: E731
     mean, ls, v = t(d["mean"]).requires_grad_(True), t(d["ls"]).requires_grad_(True), t(d["v"]).requires_grad_(True)
     i = d["idx"]
-    loss = gor.ppo_gauss_loss(mean, ls, v, t(d["act"][i]), t(d["old_logp"][i]), t(d["adv"][i]), t(d["old_v"][i]), t(d["tv"][i]), *hp)
+    loss = orc.ppo_gauss_loss(mean, ls, v, t(d["act"][i]), t(d["old_logp"][i]), t(d["adv"][i]), t(d["old_v"][i]), t(d["tv"][i]), *hp)
     g = torch.autograd.grad(loss, (mean, ls, v))
     return float(loss), [x.numpy() for x in g]
 
@@ -115,7 +114,7 @@ def test_loss_grad_against_float64(xb, A, B):
     hp = (0.2, 0.01, 0.5, 1.0)     # clip, entropy, value clip, critic coefficient
     if B >= 37:
         i = d["idx"]
-        ratio = np.exp(-gor.neglog_prob(torch.from_numpy(d["act"][i]).double(), torch.from_numpy(d["mean"]).double(),
+        ratio = np.exp(-orc.gauss_neglog_prob(torch.from_numpy(d["act"][i]).double(), torch.from_numpy(d["mean"]).double(),
                                         torch.from_numpy(d["ls"]).double()).numpy() - d["old_logp"][i])
         assert (ratio < 0.8).any() and (ratio > 1.2).any() and (np.abs(d["v"] - d["old_v"][i]) > 0.5).any()
     g = {k: dev(v) for k, v in d.items()}
@@ -156,7 +155,7 @@ def _gauss_trajs(arch, w, lens, seed, state_dim, A, dtype):
     out = []
     for T in lens:
         obs = rng.integers(0, 256, (T,) + state_dim, dtype=np.uint8) if dtype == np.uint8 else rng.standard_normal((T,) + state_dim).astype(np.float32)
-        act, logp, _ = gor.predict(arch, w, obs, rng.standard_normal((T, A)).astype(np.float32))
+        act, logp, _ = orc.ppo_gauss_predict(arch, w, obs, rng.standard_normal((T, A)).astype(np.float32))
         done = np.zeros(T, bool); done[-1] = True
         out.append(dict(cur_state=obs, action=act.astype(np.float32), logp=(logp + 0.2 * rng.standard_normal((T, 1))).astype(np.float32),
                         value=rng.standard_normal((T + 1, 1)).astype(np.float32), reward=rng.standard_normal(T).astype(np.float32),
@@ -189,8 +188,8 @@ def test_pendulum_train_matches_oracle(xb, tc_mode):
     import xingtian_b200 as xtb
     alg = xtb.alg_builder("PPO", _pendulum_info(), alg_cfg(instance_num=10))
     w0 = alg.get_weights()
-    arch = gor.ppo_mlp_arch(state_dim=(3,), action_dim=1)
-    assert list(w0) == list(gor.param_shapes(arch)) and w0["pi_logstd"].shape == (1, 1) and not w0["pi_logstd"].any()
+    arch = orc.ppo_mlp_arch(state_dim=(3,), action_dim=1, diag_gaussian=True)
+    assert list(w0) == list(orc.param_shapes(arch)) and w0["pi_logstd"].shape == (1, 1) and not w0["pi_logstd"].any()
     assert sum(v.size for v in w0.values()) == 8963 == alg.actor.net.n_params
     lens = [int(x) for x in np.random.default_rng(4).integers(9, 200, 10)]
     trajs = _gauss_trajs(arch, w0, lens, 40, (3,), 1, np.float32)
@@ -198,7 +197,7 @@ def test_pendulum_train_matches_oracle(xb, tc_mode):
         alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "value", "reward", "done")})
     np.random.seed(9)
     loss = alg.train()
-    ref = gor.PpoLearner(arch, w0, lr=0.0003, batch_size=200, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=8)
+    ref = orc.PpoLearner(arch, w0, lr=0.0003, batch_size=200, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=8)
     np.random.seed(9)
     ref_loss, ref_trace = ref.train(*_reference_labels(trajs))
     assert len(ref_trace) == 8 * -(-sum(lens) // 200)
@@ -216,22 +215,22 @@ def test_ppo_cnn_gaussian_single_step(xb, tc_mode, act):
     tol = RELU_FLIP_TC if (act == "relu" and tc_mode == 1) else 1e-3
     alg = xtb.alg_builder("PPO", _cnn_info(batch=64, iters=1, act=act), alg_cfg())
     w0 = alg.get_weights()
-    arch = gor.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,), activation=act)
-    assert list(w0) == list(gor.param_shapes(arch))
+    arch = orc.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,), activation=act, diag_gaussian=True)
+    assert list(w0) == list(orc.param_shapes(arch))
     trajs = _gauss_trajs(arch, w0, [16, 16, 16, 16], 5, (84, 84, 4), 3, np.uint8)
     for tr in trajs:
         alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "value", "reward", "done")})
     np.random.seed(1)
     loss = alg.train()
     state, label = _reference_labels(trajs)
-    ref = gor.PpoLearner(arch, w0, lr=0.00025, batch_size=64, ent_coef=0.003, clip_ratio=0.1, num_sgd_iter=1)
+    ref = orc.PpoLearner(arch, w0, lr=0.00025, batch_size=64, ent_coef=0.003, clip_ratio=0.1, num_sgd_iter=1)
     np.random.seed(1)
     ref_loss, _ = ref.train(state, label)
     assert abs(loss - ref_loss) < 1e-3 * max(1.0, abs(ref_loss))
     assert abs(alg.actor.opt.grad_norm() - ref.last_grad_norm) < tol * ref.last_grad_norm
     g = alg.actor.net.get_weights(alg.actor.net.grads)
     np.random.seed(1); inds = np.arange(64); np.random.shuffle(inds)
-    _, grads = gor.PpoLearner(arch, w0, batch_size=64, ent_coef=0.003, clip_ratio=0.1).loss_and_grads(
+    _, grads = orc.PpoLearner(arch, w0, batch_size=64, ent_coef=0.003, clip_ratio=0.1).loss_and_grads(
         state[0][inds], *[x[inds] for x in label])
     errs = {k: (rel_err(g[k], gr.numpy()), l2_rel(g[k], gr.numpy())) for k, gr in zip(w0, grads)}
     print("single step (max-rel, l2-rel):", {k: ["%.1e" % a, "%.1e" % b] for k, (a, b) in errs.items()})
@@ -247,14 +246,14 @@ def test_ppo_cnn_gaussian_matches_oracle(xb, tc_mode):
     import xingtian_b200 as xtb
     alg = xtb.alg_builder("PPO", _cnn_info(act="tanh"), alg_cfg())
     w0 = alg.get_weights()
-    arch = gor.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,), activation="tanh")
-    assert list(w0) == list(gor.param_shapes(arch))
+    arch = orc.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,), activation="tanh", diag_gaussian=True)
+    assert list(w0) == list(orc.param_shapes(arch))
     trajs = _gauss_trajs(arch, w0, [16, 16, 16, 16], 5, (84, 84, 4), 3, np.uint8)
     for tr in trajs:
         alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "value", "reward", "done")})
     np.random.seed(3)
     loss = alg.train()
-    ref = gor.PpoLearner(arch, w0, lr=0.00025, batch_size=24, ent_coef=0.003, clip_ratio=0.1, num_sgd_iter=2)
+    ref = orc.PpoLearner(arch, w0, lr=0.00025, batch_size=24, ent_coef=0.003, clip_ratio=0.1, num_sgd_iter=2)
     np.random.seed(3)
     ref_loss, ref_trace = ref.train(*_reference_labels(trajs))
     _check_against_oracle(alg, ref, w0, loss, ref_loss, ref_trace, 5e-3)
@@ -277,10 +276,10 @@ def test_predict_contract_and_rollout(xb):
     assert act.shape == (1,) and agent.transition_data["logp"].shape == (1,)
     obs = rng.standard_normal((33, 3)).astype(np.float32)
     n = rng.standard_normal((33, 1)).astype(np.float32)
-    arch = gor.ppo_mlp_arch(state_dim=(3,), action_dim=1)
+    arch = orc.ppo_mlp_arch(state_dim=(3,), action_dim=1, diag_gaussian=True)
     ga, glp, gv = m.predict(obs, normals=n)
     with orc.precision("f64"):
-        ra, rlp, rv = gor.predict(arch, {k: v.astype(np.float64) for k, v in alg.get_weights().items()}, obs.astype(np.float64), n.astype(np.float64))
+        ra, rlp, rv = orc.ppo_gauss_predict(arch, {k: v.astype(np.float64) for k, v in alg.get_weights().items()}, obs.astype(np.float64), n.astype(np.float64))
     assert ga.shape == (33, 1) and rel_err(ga, ra) < 1e-4 and rel_err(glp, rlp) < 1e-4 and rel_err(gv, rv) < 1e-4
     pa, plp, pv = m.predict(obs)                         # host predict: Philox draws, one graph
     assert pa.shape == (33, 1) and plp.shape == (33, 1) and np.isfinite(pa).all()
@@ -329,7 +328,7 @@ def test_graph_replay_matches_eager(xb):
     outs = []
     for graph in (False, True):
         alg = xtb.alg_builder("PPO", _pendulum_info(graph=graph), alg_cfg(instance_num=10))
-        arch = gor.ppo_mlp_arch(state_dim=(3,), action_dim=1)
+        arch = orc.ppo_mlp_arch(state_dim=(3,), action_dim=1, diag_gaussian=True)
         r0 = alg.actor.net.lib.xtb_graph_replay_count()
         losses = []
         for it in range(2):
@@ -417,13 +416,13 @@ def _mlp_model(A, K, B, graph=False):
 def _mlp_step_data(m, A, K, B, seed):
     """a minibatch whose ratios reach both sides of the surrogate clip and whose values pass the value clip"""
     rng = np.random.default_rng(seed)
-    arch = gor.ppo_mlp_arch(state_dim=(3,), action_dim=A, hidden_sizes=(K, K))
+    arch = orc.ppo_mlp_arch(state_dim=(3,), action_dim=A, hidden_sizes=(K, K), diag_gaussian=True)
     w = m.get_weights()
     obs = rng.standard_normal((B, 3)).astype(np.float32)
-    mean, v = [t.detach().numpy() for t in gor.forward(arch, w, obs)]
+    mean, v = [t.detach().numpy() for t in orc.forward(arch, w, obs)]
     act = (mean + np.exp(w["pi_logstd"]) * 1.2 * rng.standard_normal((B, A))).astype(np.float32)
     with orc.precision("f64"):
-        lp = gor.log_prob(torch.from_numpy(act).double(), torch.from_numpy(mean).double(),
+        lp = orc.gauss_log_prob(torch.from_numpy(act).double(), torch.from_numpy(mean).double(),
                           torch.from_numpy(w["pi_logstd"]).double()).numpy()
     old_logp = (lp + 0.5 * rng.standard_normal((B, 1))).astype(np.float32)
     label = [act, old_logp, rng.standard_normal((B, 1)).astype(np.float32),
@@ -433,7 +432,7 @@ def _mlp_step_data(m, A, K, B, seed):
 
 def _oracle_step(arch, w, obs, label, B, dt):
     with orc.precision(dt):
-        ref = gor.PpoLearner(arch, w, batch_size=B, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=1, vf_clip=0.5)
+        ref = orc.PpoLearner(arch, w, batch_size=B, ent_coef=0.01, clip_ratio=0.2, num_sgd_iter=1, vf_clip=0.5)
         loss, grads = ref.loss_and_grads(obs, *label)
         return float(loss), {k: g.detach().numpy() for k, g in zip(ref.names, grads)}
 
@@ -512,7 +511,7 @@ def test_gauss_training_is_bitwise_reproducible(xb):
     order, the trunk runs on the tensor cores): two runs from the same weights and shuffle stream give identical loss
     traces and identical weights"""
     import xingtian_b200 as xtb
-    arch = gor.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,))
+    arch = orc.ppo_cnn_arch(action_dim=3, hidden_sizes=(256,), diag_gaussian=True)
     runs, w_init = [], None
     for _ in range(2):
         alg = xtb.alg_builder("PPO", _cnn_info(batch=320, iters=2), alg_cfg(instance_num=8))
@@ -555,12 +554,12 @@ def test_rollout_infer_against_float64(xb, tc_mode, A, K, fused):
     finally:
         lib.xtb_set_fuse_heads(1)
     assert (res[1][0] < res[0][0]) if fused else (res[1][0] == res[0][0]), (res[1][0], res[0][0])
-    arch = gor.ppo_mlp_arch(state_dim=(3,), action_dim=A, hidden_sizes=(K, K))
+    arch = orc.ppo_mlp_arch(state_dim=(3,), action_dim=A, hidden_sizes=(K, K), diag_gaussian=True)
     w = {k: v.astype(np.float64) for k, v in m.get_weights().items()}
     with orc.precision("f64"):
         for t in range(T):
             for fuse in (1, 0):
                 _, a_g, l_g, v_g, seed = res[fuse]
-                x, logp, v = gor.predict(arch, w, obs[t * E:(t + 1) * E].astype(np.float64), _box_muller(seed, t, E, A))
+                x, logp, v = orc.ppo_gauss_predict(arch, w, obs[t * E:(t + 1) * E].astype(np.float64), _box_muller(seed, t, E, A))
                 assert rel_err(a_g[t], x) < 1e-4 and rel_err(l_g[t], logp.ravel()) < 1e-4 and rel_err(v_g[t], v.ravel()) < 1e-4, \
                     (fuse, t, rel_err(a_g[t], x), rel_err(l_g[t], logp.ravel()), rel_err(v_g[t], v.ravel()))

@@ -79,7 +79,14 @@ def test_arch_tables_match_oracle():
              (archs.ppo_mlp((4,), 2, [64, 64], "tanh", False), orc.ppo_mlp_arch()),
              (archs.impala_cnn((84, 84, 4), 4), orc.impala_cnn_arch()),
              (archs.dqn_cnn((84, 84, 4), 4), orc.dqn_cnn_arch()),
-             (archs.dqn_mlp((4,), 2, 128, 1), orc.dqn_mlp_arch())]
+             (archs.dqn_mlp((4,), 2, 128, 1), orc.dqn_mlp_arch()),
+             (archs.ppo_cnn((84, 84, 4), 3, [512], "relu", True, diag_gaussian=True),
+              orc.ppo_cnn_arch(action_dim=3, hidden_sizes=(512,), diag_gaussian=True)),
+             (archs.ppo_mlp((3,), 1, [64, 64], "tanh", False, diag_gaussian=True), orc.ppo_mlp_arch((3,), 1, diag_gaussian=True)),
+             (archs.dqn_cnn((84, 84, 4), 18, dueling=True), orc.dqn_cnn_arch(action_dim=18, dueling=True)),
+             (archs.dqn_mlp((4,), 3, 64, 2, dueling=True), orc.dqn_mlp_arch((4,), 3, 64, 2, dueling=True)),
+             (archs.impala_mlp((4,), 2, 128, 1), orc.impala_mlp_arch()),
+             (archs.impala_keras_cnn((84, 84, 4), 4), orc.impala_keras_cnn_arch())]
     for a, b in pairs:
         assert [(l[0], l[1], l[2]) for l in a["layers"]] == [(l[0], l[1], l[2]) for l in b["layers"]]
         assert [l[3] for l in a["layers"]] == [l[3] for l in b["layers"]]

@@ -79,7 +79,7 @@ def test_loss_gradient_matches_finite_differences():
 def test_keras_adam_decay_closed_form():
     p = [torch.zeros(3, dtype=torch.float64)]
     with orc.precision("f64"):
-        opt = iko.KerasAdam(p, 0.01, decay=0.5)
+        opt = orc.KerasAdam(p, 0.01, decay=0.5)
         for it in range(3):
             opt.step([torch.ones(3, dtype=torch.float64)])
             assert opt.lr == pytest.approx(0.01 / (1 + 0.5 * it))
@@ -91,8 +91,8 @@ def test_registry_and_layer_tables():
     from xingtian_b200.registry import Registers
     from xingtian_b200.model import archs
     assert "IMPALA" in Registers.algorithm and "ImpalaMlp" in Registers.model and "ImpalaCnn" in Registers.model
-    for mine, ref, count in ((archs.impala_mlp((4,), 2, 128, 1), iko.impala_mlp_arch(), 1027),
-                             (archs.impala_keras_cnn((84, 84, 4), 4), iko.impala_cnn_arch(), 882341)):
+    for mine, ref, count in ((archs.impala_mlp((4,), 2, 128, 1), orc.impala_mlp_arch(), 1027),
+                             (archs.impala_keras_cnn((84, 84, 4), 4), orc.impala_keras_cnn_arch(), 882341)):
         assert mine == ref
         shapes = orc.param_shapes(mine)
         assert sum(int(np.prod(s)) for s in shapes.values()) == count

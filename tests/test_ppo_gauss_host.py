@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 import torch
 
-import gauss_oracle as gor
 from oracle import xt_oracle as orc
 from xingtian_b200.model import archs
 
@@ -28,13 +27,13 @@ def test_oracle_matches_reference_golden(A):
     clip, ent, vf_clip, cc = (float(x) for x in np.load(GOLDEN)["hyper"])
     t = lambda k: torch.from_numpy(g[k])   # noqa: E731
     mean, ls = t("mean"), t("log_std")
-    x = gor.sample(mean, ls, t("normals"))
+    x = orc.gauss_sample(mean, ls, t("normals"))
     _close(x, g["sample"])
-    dls = gor.dist_log_std(mean, ls)
-    _close(gor.log_prob(x, mean, dls), g["sample_logp"])
-    _close(gor.neglog_prob(t("behav"), mean, dls), g["behav_neglogp"])
-    _close(gor.entropy(dls), g["entropy"])
-    loss = gor.ppo_gauss_loss(mean, ls, t("out_v"), t("behav"), t("old_logp"), t("adv"), t("old_v"), t("target_v"),
+    dls = orc.dist_log_std(mean, ls)
+    _close(orc.gauss_log_prob(x, mean, dls), g["sample_logp"])
+    _close(orc.gauss_neglog_prob(t("behav"), mean, dls), g["behav_neglogp"])
+    _close(orc.gauss_entropy(dls), g["entropy"])
+    loss = orc.ppo_gauss_loss(mean, ls, t("out_v"), t("behav"), t("old_logp"), t("adv"), t("old_v"), t("target_v"),
                               clip, ent, vf_clip, cc)
     _close(loss, g["total_loss"])
     # the fixture's inputs reach both sides of the surrogate clip and the clipped value loss
@@ -53,13 +52,13 @@ def test_gradients_match_closed_form(A):
     mean = torch.from_numpy(rng.standard_normal((B, A))).requires_grad_(True)
     ls = torch.from_numpy(rng.standard_normal((1, A)) * 0.5).requires_grad_(True)
     x = torch.from_numpy(rng.standard_normal((B, A)))
-    dls = gor.dist_log_std(mean, ls)
-    gm, gl = torch.autograd.grad(gor.log_prob(x, mean, dls).sum(), (mean, ls))
+    dls = orc.dist_log_std(mean, ls)
+    gm, gl = torch.autograd.grad(orc.gauss_log_prob(x, mean, dls).sum(), (mean, ls))
     std = np.exp(ls.detach().numpy())
     z = (x.numpy() - mean.detach().numpy()) / std
     assert np.max(np.abs(gm.numpy() - z / std)) < 1e-12
     assert np.max(np.abs(gl.numpy() - (z * z - 1).sum(0, keepdims=True))) < 1e-12
-    gm, gl = torch.autograd.grad(gor.entropy(gor.dist_log_std(mean, ls)).mean(), (mean, ls))
+    gm, gl = torch.autograd.grad(orc.gauss_entropy(orc.dist_log_std(mean, ls)).mean(), (mean, ls))
     assert np.max(np.abs(gm.numpy())) == 0.0 and np.max(np.abs(gl.numpy() - 1.0)) < 1e-12
 
 
@@ -68,16 +67,16 @@ def test_gaussian_tables_and_names():
     gauss = archs.ppo_mlp(**PENDULUM, diag_gaussian=True)
     assert gauss["layers"][:-1] == cat["layers"] and gauss["outputs"] == cat["outputs"]
     assert gauss["layers"][-1] == ("pi_logstd", "logstd", None, dict(n=1))
-    shapes = gor.param_shapes(gauss)
+    shapes = orc.param_shapes(gauss)
     assert list(shapes)[-1] == "pi_logstd" and shapes["pi_logstd"] == (1, 1)
     assert list(shapes)[:-1] == list(orc.param_shapes(orc.ppo_mlp_arch((3,), 1))) == list(orc.param_shapes(cat))
     assert sum(int(np.prod(s)) for s in shapes.values()) == 2 * (3 * 64 + 64 + 64 * 64 + 64) + 65 + 65 + 1 == 8963
-    assert gauss["layers"] == gor.ppo_mlp_arch(state_dim=(3,), action_dim=1)["layers"]
+    assert gauss["layers"] == orc.ppo_mlp_arch(state_dim=(3,), action_dim=1, diag_gaussian=True)["layers"]
     cnn = archs.ppo_cnn((84, 84, 4), 3, [512], "relu", True, diag_gaussian=True)
     assert cnn["layers"][-1] == ("pi_logstd", "logstd", None, dict(n=3))
-    assert cnn["layers"] == gor.ppo_cnn_arch(action_dim=3, hidden_sizes=(512,))["layers"]
-    assert gor.param_shapes(cnn)["pi_logstd"] == (1, 3)
-    w = gor.init_weights(gauss, seed=0)
+    assert cnn["layers"] == orc.ppo_cnn_arch(action_dim=3, hidden_sizes=(512,), diag_gaussian=True)["layers"]
+    assert orc.param_shapes(cnn)["pi_logstd"] == (1, 3)
+    w = orc.init_weights(gauss, seed=0)
     assert list(w) == list(shapes) and not w["pi_logstd"].any()
 
 
