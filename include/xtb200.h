@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define XTB_VERSION 100
+#define XTB_VERSION 101
 
 enum xtb_status {
   XTB_OK = 0,
@@ -75,7 +75,8 @@ enum xtb_act {
  *        floats, reads no tensor (src must be 0) and produces none (its tensor is 0 wide, so no layer may read it and it
  *        cannot be a backward head); act must be XTB_ACT_NONE and 1 <= cout <= 32.  xtb_net_layer_params reports 1 row
  *        and A columns with bias_off = kernel_off + A (it has no bias).  It takes part in clipping, the optimiser and
- *        the gradient bucket like every other parameter; the PPO Gaussian entry points below read it by offset. */
+ *        the gradient bucket like every other parameter; the PPO calls below read it by offset when it is their
+ *        logstd_tensor. */
 typedef struct xtb_layer_desc {
   int32_t kind;      /* xtb_layer_kind */
   int32_t src;       /* tensor id of the input: 0 = observation, i+1 = output of layer i */
@@ -273,26 +274,41 @@ int xtb_adam_set_decay(xtb_adam* opt, float decay);
 int xtb_opt_use_rmsprop(xtb_adam* opt, float* mean_grad, float decay, float epsilon);
 
 /* ---- fused learner loops -------------------------------------------------------- */
-/* use_graph != 0 (xtb_ppo_train, xtb_ppo_gauss_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer,
- * xtb_ppo_gauss_rollout_infer and the predict calls built on them): the call's launches are captured once as a CUDA graph and replayed.  A graph is keyed on every
+/* use_graph != 0 (xtb_ppo_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer and xtb_ppo_predict_host built
+ * on it): the call's launches are captured once as a CUDA graph and replayed.  A graph is keyed on every
  * argument plus the kernel-path mode (xtb_set_tc_mode), the fused-heads mode (xtb_set_fuse_heads) and the installed
  * communicator (xtb_set_grad_comm), so a mode change takes effect at the next call.  It is dropped when its net,
  * target net, optimiser or communicator is destroyed, or when its net is rebound (xtb_net_bind). */
+/* The PPO calls (xtb_ppo_train, xtb_ppo_rollout_infer, xtb_ppo_predict_host) take the policy's heads as tensor ids:
+ * pi_tensor (the logits, or the DiagGaussian mean: at most 32 wide), v_tensor (the value, 1 wide) and logstd_tensor,
+ * which selects the action distribution, as PPO's action_type does (xt/model/ppo/ppo.py:62-95):
+ *   0        Categorical (see xtb_categorical_sample, xtb_ppo_loss_grad); actions are int32, one per sample;
+ *   > 0      DiagGaussian (see xtb_diag_gaussian_sample, xtb_ppo_gauss_loss_grad): the tensor id (layer index + 1) of an
+ *            XTB_LOGSTD layer as wide as pi_tensor; actions are A floats per sample.
+ * Any other value, or a logstd_tensor that is not such a layer, returns XTB_ERR_ARG before a launch.
+ * Fused heads: when both heads are linear dense layers on hidden (not observation) tensors of equal width K, K is a
+ * multiple of 32, and the fused-heads mode is on (xtb_set_fuse_heads), one kernel evaluates both heads --
+ *   training:  with the loss and their backward, for A <= 8 and K <= 256 or A <= 4 and K <= 512; its per-block partial
+ *              sums, a log_std gradient included, are reduced in block order, so with tensor-core trunk layers the
+ *              step is bitwise reproducible;
+ *   inference: with the draw, for A <= 8 and K <= 512.
+ * Every other shape runs layer by layer (forward, the loss or sampling kernel, backward); the draws are the same. */
 /* PPO.train (xt/model/ppo/ppo.py:111-132): for every minibatch slice of `perm`
  * (device int32 [n_epoch*n_sample], the host-generated np.random.shuffle order) run
- * forward, loss, backward, clip, Adam.  loss_per_step: device float [n_epoch*ceil(N/B)].
+ * forward, loss, backward, clip, Adam.  loss_per_step: device float [n_epoch*ceil(N/B)].  Without fused heads a
+ * DiagGaussian's log_std gradient goes straight into its slot of the bound gradient buffer.
  * All launches go to `stream`. */
 typedef struct xtb_ppo_rollout {
   const void* obs;            /* [N, H,W,C] uint8 / float */
-  const int32_t* action;      /* [N] */
+  const void* action;         /* behaviour actions: int32 [N] (Categorical) or float [N, A] (DiagGaussian) */
   const float* old_logp;      /* [N] */
   const float* adv;           /* [N] */
   const float* old_v;         /* [N] */
   const float* target_v;      /* [N] */
 } xtb_ppo_rollout;
-int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample,
-                  int batch_size, int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp,
-                  int pi_tensor, int v_tensor, float* loss_per_step, int use_graph, void* stream);
+int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample, int batch_size, int n_epoch,
+                  const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor, int logstd_tensor,
+                  float* loss_per_step, int use_graph, void* stream);
 
 /* ImpalaCnnOpt.train (xt/model/impala/impala_cnn_opt.py:251-265) as one captured step: forward over n_sample =
  * k*step_len env-major rows (rows gather_idx[b] of obs when non-NULL), in-graph V-trace + summed losses, backward,
@@ -342,28 +358,23 @@ int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_impala_traj* t
                            int use_graph, void* stream);
 
 /* Rollout inference: for t in [0,n_step): forward over n_env observations (row e of step t is
- * obs[step_idx[t*n_env+e]], NULL = rows t*n_env..), sample actions with Philox(seed, *offset_dev + t), and
- * write action/logp/value time-major [n_step, n_env]; finally *offset_dev += n_step.  This is the batched
- * replacement of the per-explorer batch-1 PPO.predict calls (xt/agent/ppo/ppo.py:35-45,
- * xt/algorithm/ppo/ppo.py:87-95). */
-int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
-                          int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                          int32_t* action, float* logp, float* value, int use_graph, void* stream);
+ * obs[step_idx[t*n_env+e]], NULL = rows t*n_env..), draw actions as xtb_categorical_sample / xtb_diag_gaussian_sample do
+ * with Philox4x32-10(seed, offset = *offset_dev + t), and write action [n_step, n_env] int32 or [n_step, n_env, A] float
+ * and logp / value [n_step, n_env] time-major; finally *offset_dev += n_step.  This is the batched replacement of the
+ * per-explorer batch-1 PPO.predict calls (xt/agent/ppo/ppo.py:35-45, xt/algorithm/ppo/ppo.py:87-95). */
+int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step, int pi_tensor,
+                          int v_tensor, int logstd_tensor, uint64_t seed, unsigned long long* offset_dev, void* action,
+                          float* logp, float* value, int use_graph, void* stream);
 
 /* PPO.predict (xt/model/ppo/ppo.py:104-109) on host buffers in one call: staged H2D of `obs_host` (pageable,
  * obs_bytes) into `obs_dev`, xtb_ppo_rollout_infer with n_step = 1 writing the packed block
- * out_dev = [action int32 | logp f32 | value f32] x n_env, one D2H into `out_host` (pinned) and a stream
- * synchronise: when it returns, out_host holds the step's results. */
-int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                         int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                         float* out_dev, float* out_host, int use_graph, void* stream);
-
-/* The same call for actors whose predict() also returns the logits (ImpalaCnnOpt.predict,
- * xt/model/impala/impala_cnn_opt.py:267-277: [logits, baseline, action]): additionally copies the [n_env, A] logits of
- * tensor `pi_tensor` into `logits_host` (pinned; NULL = skip) before the synchronise. */
-int xtb_actor_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                           int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                           float* out_dev, float* out_host, float* logits_host, int use_graph, void* stream);
+ *   out_dev = [action | logp f32 x n_env | value f32 x n_env], action int32 x n_env or (DiagGaussian) f32 x n_env*A,
+ * one D2H of it into `out_host` (pinned), one D2H of the [n_env, A] output of `pi_tensor` into `head_host` (pinned;
+ * NULL = skip: for actors whose predict() also returns the logits, ImpalaCnnOpt.predict,
+ * xt/model/impala/impala_cnn_opt.py:267-277) and a stream synchronise: when it returns, both hold the step's results. */
+int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env, int pi_tensor,
+                         int v_tensor, int logstd_tensor, uint64_t seed, unsigned long long* offset_dev, float* out_dev,
+                         float* out_host, float* head_host, int use_graph, void* stream);
 
 /* ---- PPO with a diagonal Gaussian policy (action_type DiagGaussian): replaces DiagGaussianDist
  *      (xt/model/tf_dist.py:49-86) as PPO.build_graph wires it (xt/model/ppo/ppo.py:62-95) --------------
@@ -388,40 +399,6 @@ int xtb_ppo_gauss_loss_grad(const float* mean, const float* v, const float* log_
                             const float* action, const float* old_logp, const float* adv, const float* old_v,
                             const float* target_v, int batch, int adim, const xtb_ppo_hyper* hp, float inv_count,
                             float* dmean, float* dv, float* dlog_std, float* loss_out, void* stream);
-/* PPO.train (ppo.py:111-132) with a Gaussian actor: the loop of xtb_ppo_train (same perm, minibatches, clip, Adam and
- * data-parallel handling) over the rollout below; logstd_tensor names the XTB_LOGSTD layer (its layer index + 1), whose
- * width must equal pi_tensor's.  Under the fused-heads conditions of xtb_ppo_train (both heads linear dense layers on
- * hidden tensors of equal width K, K a multiple of 32 with A <= 8 and K <= 256 or A <= 4 and K <= 512, fused-heads mode
- * on) both heads, the loss and their backward run in one kernel whose per-block partial sums, the log_std gradient's
- * included, are reduced in block order: with tensor-core trunk layers the step is bitwise reproducible.  Otherwise every
- * minibatch runs forward, xtb_ppo_gauss_loss_grad (log_std gradient straight into its slot of the bound gradient
- * buffer), backward and the optimiser step. */
-typedef struct xtb_ppo_gauss_rollout {
-  const void* obs;            /* [N, H,W,C] uint8 / float */
-  const float* action;        /* [N, A] behaviour actions */
-  const float* old_logp;      /* [N] */
-  const float* adv;           /* [N] */
-  const float* old_v;         /* [N] */
-  const float* target_v;      /* [N] */
-} xtb_ppo_gauss_rollout;
-int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int n_sample, int batch_size,
-                        int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor,
-                        int logstd_tensor, float* loss_per_step, int use_graph, void* stream);
-/* xtb_ppo_rollout_infer for a Gaussian actor: action [n_step, n_env, A] f32 drawn with Philox(seed, *offset_dev + t)
- * as xtb_diag_gaussian_sample; logp / value [n_step, n_env]; finally *offset_dev += n_step.  Within the fused-inference
- * limits of xtb_ppo_rollout_infer (linear dense heads on hidden tensors of equal width K, K a multiple of 32, K <= 512,
- * A <= 8, fused-heads mode on) one kernel evaluates both heads and the sample; otherwise the layer-by-layer forward is
- * followed by the sampling kernel.  The draws are the same either way. */
-int xtb_ppo_gauss_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
-                                int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
-                                unsigned long long* offset_dev, float* action, float* logp, float* value, int use_graph,
-                                void* stream);
-/* xtb_ppo_predict_host for a Gaussian actor (PPO.predict, ppo.py:104-109): the packed block is
- * out_dev = [action n_env*A | logp n_env | value n_env] floats, copied to out_host before the synchronise. */
-int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                               int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
-                               unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
-                               void* stream);
 
 /* ---- MuZero: replaces MuzeroModel's train / inference graphs (xt/model/muzero/muzero_model.py:74-239) ----------------
  * The model is three nets: representation (obs -> hidden h, H wide), dynamics (concat(h, one_hot(a)) -> next hidden and
@@ -509,7 +486,7 @@ int xtb_net_bench_layer(xtb_net* net, int layer, int which, const void* obs, con
 int xtb_set_tc_mode(int mode);
 /* 1 (default): xtb_ppo_train (and xtb_dqn_train on a dueling head) evaluates both heads, the loss and their backward
  * in one fused kernel; 0: layer-by-layer (also XTB_FUSE_HEADS=0).  Takes effect at the next call.  The same mode
- * selects the fused heads of xtb_ppo_gauss_train and of the rollout-inference calls. */
+ * selects the fused heads of the rollout-inference calls. */
 int xtb_set_fuse_heads(int on);
 int xtb_get_tc_mode(void);
 /* Self-test of the wgmma GEMM core on plain fp32 matrices (sizes multiples of 8):

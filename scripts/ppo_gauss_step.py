@@ -1,6 +1,5 @@
-"""Time the graph-replayed PPO train call (xtb_ppo_gauss_train / xtb_ppo_train) and rollout inference
-(xtb_ppo_gauss_rollout_infer / xtb_ppo_rollout_infer) of a DiagGaussian actor against a Categorical one with the same
-network, alternated in one process.
+"""Time the graph-replayed PPO train call (xtb_ppo_train) and rollout inference (xtb_ppo_rollout_infer) of a
+DiagGaussian actor against a Categorical one with the same network, alternated in one process.
 
 Shapes:
   pendulum: PpoMlp [3] -> A = 1, tanh [64, 64], separate towers; E = 10 envs x T = 200 steps, BATCH_SIZE 200, 8 epochs
@@ -62,10 +61,10 @@ def fill_rollout(m, sh, rng):
 def train_call(m, N):
     """the native train call train_device makes, without its loss read-back"""
     lib, ro = m.net.lib, m.rollout.as_struct()
-    args = (m.net.handle, m.opt.handle, C.byref(ro), N, int(m._batch_size), int(m.num_sgd_iter), C.c_void_p(m._perm_dev.data_ptr()),
-            C.byref(m.hyper), m.pi_t, m.v_t)
-    tail = (C.c_void_p(m._loss_dev.data_ptr()), 1 if m.use_graph else 0, C.c_void_p(torch.cuda.current_stream().cuda_stream))
-    rc = lib.xtb_ppo_gauss_train(*args, m.ls_t, *tail) if m.gaussian else lib.xtb_ppo_train(*args, *tail)
+    rc = lib.xtb_ppo_train(m.net.handle, m.opt.handle, C.byref(ro), N, int(m._batch_size), int(m.num_sgd_iter),
+                           C.c_void_p(m._perm_dev.data_ptr()), C.byref(m.hyper), m.pi_t, m.v_t, m.ls_t,
+                           C.c_void_p(m._loss_dev.data_ptr()), 1 if m.use_graph else 0,
+                           C.c_void_p(torch.cuda.current_stream().cuda_stream))
     assert rc == 0, lib.xtb_last_error()
 
 

@@ -39,8 +39,8 @@ rows.append(("  .. with the device observation ring", bench(lambda i: m.predict(
 m._obs_ring = None
 io = m._predict_io(E)
 off = m._offset_dev
-args = lambda st: (m.net.handle, st.ctypes.data, st.nbytes, io["obs_ptr"], E, m.pi_t, m.v_t, C.c_uint64(1), _ptr(off),
-                   io["out_dev_ptr"], io["pin_out_ptr"], 1, stream_ptr())
+args = lambda st: (m.net.handle, st.ctypes.data, st.nbytes, io["obs_ptr"], E, m.pi_t, m.v_t, m.ls_t, C.c_uint64(1), _ptr(off),
+                   io["out_dev_ptr"], io["pin_out_ptr"], None, 1, stream_ptr())
 rows.append(("xtb_ppo_predict_host alone (ctypes)", bench(lambda i: check(lib.xtb_ppo_predict_host(*args(frames[i & 7]))))))
 rows.append(("staged H2D of the frames + stream sync", bench(lambda i: (
     check(lib.xtb_copy_h2d_staged(io["obs_ptr"], frames[i & 7].ctypes.data, frames[i & 7].nbytes, stream_ptr())),

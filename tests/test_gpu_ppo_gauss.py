@@ -377,7 +377,7 @@ def test_malformed_descriptors_fail_without_launches(xb):
         assert lib.xtb_launch_count() == before
 
 
-def test_gaussian_entry_points_reject_wrong_tensors(xb):
+def test_rollout_infer_rejects_wrong_logstd_tensors(xb):
     import xingtian_b200 as xtb
     from xingtian_b200.engine import _ptr, stream_ptr
     alg = xtb.alg_builder("PPO", _pendulum_info(), alg_cfg())
@@ -387,12 +387,12 @@ def test_gaussian_entry_points_reject_wrong_tensors(xb):
     act, lp, val = torch.empty(4, 1, device="cuda"), torch.empty(4, device="cuda"), torch.empty(4, device="cuda")
     off = torch.zeros(1, dtype=torch.int64, device="cuda")
     before = lib.xtb_launch_count()
-    for ls_t in (m.pi_t, m.v_t, 0, len(m.net.names)):     # not the logstd layer / out of range
-        assert lib.xtb_ppo_gauss_rollout_infer(m.net.handle, _ptr(obs), None, 4, 1, m.pi_t, m.v_t, ls_t, C.c_uint64(1), _ptr(off),
-                                               _ptr(act), _ptr(lp), _ptr(val), 0, stream_ptr()) == -1
+    for ls_t in (m.pi_t, m.v_t, -1, len(m.net.names)):     # not the logstd layer / out of range
+        assert lib.xtb_ppo_rollout_infer(m.net.handle, _ptr(obs), None, 4, 1, m.pi_t, m.v_t, ls_t, C.c_uint64(1), _ptr(off),
+                                         _ptr(act), _ptr(lp), _ptr(val), 0, stream_ptr()) == -1
     assert lib.xtb_launch_count() == before
-    assert lib.xtb_ppo_gauss_rollout_infer(m.net.handle, _ptr(obs), None, 4, 1, m.pi_t, m.v_t, m.ls_t, C.c_uint64(1), _ptr(off),
-                                           _ptr(act), _ptr(lp), _ptr(val), 0, stream_ptr()) == 0
+    assert lib.xtb_ppo_rollout_infer(m.net.handle, _ptr(obs), None, 4, 1, m.pi_t, m.v_t, m.ls_t, C.c_uint64(1), _ptr(off),
+                                     _ptr(act), _ptr(lp), _ptr(val), 0, stream_ptr()) == 0
     # the logstd tensor is not a backward head
     with pytest.raises(RuntimeError):
         m.net.backward(obs, 4, ["pi_logstd"])

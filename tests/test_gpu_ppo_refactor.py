@@ -48,7 +48,7 @@ def test_rollout_infer_without_step_idx_reads_each_steps_rows(fuse_heads):
     np.testing.assert_array_equal(val_n, val_i)
 
 
-def test_ppo_train_rejects_optimiser_of_another_size():
+def test_categorical_ppo_train_rejects_optimiser_of_another_size():
     import xingtian_b200 as xb
     from xingtian_b200 import capi
     from xingtian_b200.engine import _ptr, stream_ptr
@@ -72,7 +72,7 @@ def test_ppo_train_rejects_optimiser_of_another_size():
         for use_graph in (0, 1):
             torch.cuda.synchronize()
             n0 = lib.xtb_launch_count()
-            rc = lib.xtb_ppo_train(m.net.handle, opt, C.byref(ro), N, N, 1, _ptr(perm), C.byref(m.hyper), m.pi_t, m.v_t,
+            rc = lib.xtb_ppo_train(m.net.handle, opt, C.byref(ro), N, N, 1, _ptr(perm), C.byref(m.hyper), m.pi_t, m.v_t, 0,
                                    _ptr(loss), use_graph, stream_ptr())
             assert rc == XTB_ERR_ARG
             assert b"size mismatch" in lib.xtb_last_error()

@@ -9,11 +9,11 @@ import pytest
 from oracle import xt_oracle as orc
 
 
-def test_library_builds_loads_and_exports_every_declared_symbol(repo_root):
+def test_library_builds_loads_and_exports_every_declared_symbol_of_abi_101(repo_root):
     from xingtian_b200 import build, capi
     build.build()
     lib = capi.lib()
-    assert lib.xtb_version() == 100
+    assert lib.xtb_version() == 101
     header = open(os.path.join(repo_root, "include", "xtb200.h")).read()
     declared = set(re.findall(r"\b(xtb_[a-z0-9_]+)\s*\(", header))
     assert declared, "no declarations parsed"
@@ -27,7 +27,7 @@ def test_library_builds_loads_and_exports_every_declared_symbol(repo_root):
     assert lib.xtb_gae(None, None, None, 1, 1, 0.99, 0.95, 0, None, None, None, None) == -1
     assert b"null" in lib.xtb_last_error()
     assert lib.xtb_copy_h2d_staged(None, None, 16, None) == -1      # argument check happens before any CUDA call
-    assert lib.xtb_ppo_predict_host(None, None, 0, None, 1, 1, 2, 0, None, None, None, 0, None) == -1
+    assert lib.xtb_ppo_predict_host(None, None, 0, None, 1, 1, 2, 0, 0, None, None, None, None, 0, None) == -1
     assert lib.xtb_launch_count() == launches
 
 

@@ -43,11 +43,6 @@ class PpoRollout(C.Structure):
                 ("old_v", C.c_void_p), ("target_v", C.c_void_p)]
 
 
-class PpoGaussRollout(C.Structure):
-    """xtb_ppo_gauss_rollout: as PpoRollout, with float behaviour actions [N, A]."""
-    _fields_ = PpoRollout._fields_
-
-
 class ImpalaTraj(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("behav_prob", C.c_void_p), ("action_mat", C.c_void_p), ("reward", C.c_void_p),
                 ("done", C.c_void_p)]
@@ -117,20 +112,15 @@ _SIGS = {
     "xtb_adam_set_lr": (C.c_int, [_P, C.c_float]),
     "xtb_adam_set_decay": (C.c_int, [_P, C.c_float]),
     "xtb_opt_use_rmsprop": (C.c_int, [_P, _P, C.c_float, C.c_float]),
-    "xtb_ppo_train": (C.c_int, [_P, _P, C.POINTER(PpoRollout), C.c_int, C.c_int, C.c_int, _P,
-                                C.POINTER(PpoHyper), C.c_int, C.c_int, _P, C.c_int, _P]),
-    "xtb_ppo_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
-    "xtb_ppo_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, C.c_int, _P]),
-    "xtb_actor_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_ppo_train": (C.c_int, [_P, _P, C.POINTER(PpoRollout), C.c_int, C.c_int, C.c_int, _P, C.POINTER(PpoHyper),
+                                C.c_int, C.c_int, C.c_int, _P, C.c_int, _P]),
+    "xtb_ppo_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P,
+                                        C.c_int, _P]),
+    "xtb_ppo_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P,
+                                       C.c_int, _P]),
     "xtb_diag_gaussian_sample": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "xtb_ppo_gauss_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(PpoHyper), C.c_float,
                                           _P, _P, _P, _P, _P]),
-    "xtb_ppo_gauss_train": (C.c_int, [_P, _P, C.POINTER(PpoGaussRollout), C.c_int, C.c_int, C.c_int, _P, C.POINTER(PpoHyper),
-                                      C.c_int, C.c_int, C.c_int, _P, C.c_int, _P]),
-    "xtb_ppo_gauss_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P,
-                                              _P, C.c_int, _P]),
-    "xtb_ppo_gauss_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P,
-                                             _P, C.c_int, _P]),
     "xtb_muzero_create": (C.c_int, [_P, _P, _P, C.POINTER(MuzeroDesc), C.c_int, C.POINTER(_P)]),
     "xtb_muzero_destroy": (None, [_P]),
     "xtb_muzero_train": (C.c_int, [_P, _P, C.POINTER(MuzeroBatch), C.c_int, C.c_float, _P, _P, C.c_int, _P]),

@@ -1860,8 +1860,8 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // A captured graph bakes in every kernel argument, so its key holds everything the capture reads.  capture_key()
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
-enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kPpoGaussTrain,
-                kGaussRolloutInfer, kMuzeroTrain, kMuzeroInitInfer, kMuzeroRecurInfer };
+enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
+                kMuzeroInitInfer, kMuzeroRecurInfer };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -2049,27 +2049,16 @@ static int heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, i
   return net_backward_impl(net, obs, idx, mb, stream, o);
 }
 
-// names and capture tags of the exported PPO calls of each action distribution
-template <class DIST> struct PpoCalls;
-template <> struct PpoCalls<Categorical> {
-  static constexpr const char *train = "xtb_ppo_train", *infer = "xtb_ppo_rollout_infer", *predict = "xtb_actor_predict_host";
-  static constexpr GraphTag train_tag = kPpoTrain, infer_tag = kRolloutInfer;
-};
-template <> struct PpoCalls<DiagGaussian> {
-  static constexpr const char *train = "xtb_ppo_gauss_train", *infer = "xtb_ppo_gauss_rollout_infer",
-                              *predict = "xtb_ppo_gauss_predict_host";
-  static constexpr GraphTag train_tag = kPpoGaussTrain, infer_tag = kGaussRolloutInfer;
-};
-
 // The epoch x minibatch loop of PPO.train for the action distribution DIST.  Under the fused-heads conditions one
 // heads_kernel<DIST::Loss> launch per minibatch (a DiagGaussian's log_std gradient is A more slab floats, reduced in
 // block order into its slot); otherwise layer by layer: forward, the loss kernel (a DiagGaussian's log_std gradient
 // straight into its slot of the zeroed gradient bucket), then the backward pass of the network, which keeps that slot.
-template <class DIST, class RO>
-static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, int B, int E, const int32_t* perm,
+template <class DIST>
+static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int N, int B, int E, const int32_t* perm,
                             const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, float inv_world,
                             void* stream) {
   const int32_t heads[2] = {pi_t, v_t};
+  const auto* action = static_cast<const typename DIST::Action*>(ro->action);
   const int adim = net->tsize[pi_t];
   const long long ls_off = DIST::kLogStd ? net->L[ls_t - 1].w_off : -1;
   const LayerPlan& lpi = net->L[pi_t - 1];
@@ -2085,20 +2074,20 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, in
       PpoHeadsArgs a;
       memset(&a, 0, sizeof a);
       a.idx = idx; a.old_logp = ro->old_logp; a.adv = ro->adv; a.old_v = ro->old_v; a.target_v = ro->target_v;
-      if constexpr (DIST::kLogStd) { a.action_f = ro->action; a.log_std = net->params + ls_off; }
-      else a.action = ro->action;
+      if constexpr (DIST::kLogStd) { a.action_f = action; a.log_std = net->params + ls_off; }
+      else a.action = action;
       a.logits_out = xtb_net_tensor(net, pi_t); a.v_out = xtb_net_tensor(net, v_t);
       a.hp = PpoHyperDev{hp->clip_ratio, hp->ent_coef, hp->vf_clip, hp->critic_coef}; a.inv_count = inv_world / mb;
       return heads_fused<typename DIST::Loss>(net, ro->obs, a, mb, pi_t, v_t, skip, ls_off, step_loss, stream);
     }
     if constexpr (DIST::kLogStd) {
       CUDA_TRY(cudaMemsetAsync(net->grads, 0, net->n_params * sizeof(float), S(stream)));
-      rc = xtb_ppo_gauss_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), net->params + ls_off, idx, ro->action,
+      rc = xtb_ppo_gauss_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), net->params + ls_off, idx, action,
                                    ro->old_logp, ro->adv, ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb,
                                    xtb_net_tensor_grad(net, pi_t), xtb_net_tensor_grad(net, v_t), net->grads + ls_off, step_loss,
                                    stream);
     } else {
-      rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, ro->action, ro->old_logp, ro->adv,
+      rc = xtb_ppo_loss_grad(xtb_net_tensor(net, pi_t), xtb_net_tensor(net, v_t), idx, action, ro->old_logp, ro->adv,
                              ro->old_v, ro->target_v, mb, adim, hp, inv_world / mb, xtb_net_tensor_grad(net, pi_t),
                              xtb_net_tensor_grad(net, v_t), step_loss, stream);
     }
@@ -2109,50 +2098,38 @@ static int ppo_train_launch(xtb_net* net, xtb_adam* opt, const RO* ro, int N, in
   });
 }
 
-// head tensors of the PPO entry points: pi_t (logits / mean, at most MAX_ADIM wide), v_t (value, 1 wide) and, for a
-// distribution with log_std, the logstd layer's tensor ls_t of the mean's width
-template <class DIST>
+// head tensors of the PPO entry points: pi_t (logits / mean, at most MAX_ADIM wide), v_t (value, 1 wide) and ls_t,
+// 0 for Categorical, else the DiagGaussian's logstd layer tensor of the mean's width
 static int ppo_heads_check(const char* fn, const xtb_net* net, int pi_t, int v_t, int ls_t) {
   const int nl = (int)net->L.size();
-  if (pi_t < 1 || pi_t > nl || v_t < 1 || v_t > nl || net->tsize[v_t] != 1 || net->tsize[pi_t] > MAX_ADIM ||
-      (DIST::kLogStd && (ls_t < 1 || ls_t > nl)))
+  if (pi_t < 1 || pi_t > nl || v_t < 1 || v_t > nl || net->tsize[v_t] != 1 || net->tsize[pi_t] > MAX_ADIM || ls_t < 0 ||
+      ls_t > nl)
     return fail(XTB_ERR_ARG, "%s: bad head tensors", fn);
-  if (!DIST::kLogStd) return XTB_OK;
+  if (!ls_t) return XTB_OK;
   const LayerPlan& ls = net->L[ls_t - 1];
   if (ls.d.kind != XTB_LOGSTD || ls.N != net->tsize[pi_t]) return fail(XTB_ERR_ARG, "%s: tensor %d is not a logstd layer of the mean's width", fn, ls_t);
   return XTB_OK;
 }
 
-template <class DIST, class RO>
-static int ppo_train(xtb_net* net, xtb_adam* opt, const RO* ro, int n_sample, int batch_size, int n_epoch, const int32_t* perm,
-                     const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step, int use_graph, void* stream) {
-  const char* fn = PpoCalls<DIST>::train;
+extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample, int batch_size, int n_epoch,
+                             const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step,
+                             int use_graph, void* stream) {
+  const char* fn = "xtb_ppo_train";
   const bool missing = !net || !opt || !ro || !ro->obs || !ro->action || !ro->old_logp || !ro->adv || !ro->old_v || !ro->target_v ||
                        !perm || !hp || !loss_per_step;
   if (int rc = learner_check(fn, missing, net, opt, std::min(batch_size, n_sample), true)) return rc;
   if (n_epoch <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
-  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
+  if (int rc = ppo_heads_check(fn, net, pi_t, v_t, ls_t)) return rc;
   const float inv_world = dp_inv_world();
-  return run_graph(capture_key(PpoCalls<DIST>::train_tag, {net, opt}, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
+  return run_graph(capture_key(kPpoTrain, {net, opt}, ro->obs, ro->action, ro->old_logp, ro->adv, ro->old_v, ro->target_v, perm,
                                loss_per_step, n_sample, batch_size, n_epoch, hp->clip_ratio, hp->ent_coef, hp->vf_clip,
                                hp->critic_coef, pi_t, v_t, ls_t),
                    use_graph, stream, [&](void* st) {
-    return ppo_train_launch<DIST>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_t, v_t, ls_t, loss_per_step, inv_world, st);
+    return ls_t ? ppo_train_launch<DiagGaussian>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_t, v_t, ls_t,
+                                                 loss_per_step, inv_world, st)
+                : ppo_train_launch<Categorical>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_t, v_t, ls_t,
+                                                loss_per_step, inv_world, st);
   });
-}
-
-extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample,
-                             int batch_size, int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp,
-                             int pi_tensor, int v_tensor, float* loss_per_step, int use_graph, void* stream) {
-  return ppo_train<Categorical>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, 0, loss_per_step,
-                                use_graph, stream);
-}
-
-extern "C" int xtb_ppo_gauss_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_gauss_rollout* ro, int n_sample, int batch_size,
-                                   int n_epoch, const int32_t* perm, const xtb_ppo_hyper* hp, int pi_tensor, int v_tensor,
-                                   int logstd_tensor, float* loss_per_step, int use_graph, void* stream) {
-  return ppo_train<DiagGaussian>(net, opt, ro, n_sample, batch_size, n_epoch, perm, hp, pi_tensor, v_tensor, logstd_tensor,
-                                 loss_per_step, use_graph, stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2639,34 +2616,36 @@ static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* st
   return XTB_OK;
 }
 
-template <class DIST>
-static int ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step, int pi_t, int v_t,
-                             int ls_t, uint64_t seed, unsigned long long* offset_dev, typename DIST::Action* action, float* logp,
-                             float* value, int use_graph, void* stream) {
-  const char* fn = PpoCalls<DIST>::infer;
-  if (!net || !net->ws || !obs || !offset_dev || !action || !logp || !value) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+// the checks of the rollout-inference calls past their own pointers: a bound net, the sizes and the head tensors
+static int ppo_infer_check(const char* fn, const xtb_net* net, const unsigned long long* offset_dev, int n_env, int n_step,
+                           int pi_t, int v_t, int ls_t) {
+  if (!net->ws || !offset_dev) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
   if (n_env <= 0 || n_env > net->max_batch || n_step <= 0) return fail(XTB_ERR_ARG, "%s: bad sizes", fn);
-  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
-  return run_graph(capture_key(PpoCalls<DIST>::infer_tag, {net}, obs, step_idx, offset_dev, action, logp, value,
-                               n_env, n_step, pi_t, v_t, ls_t, seed),
+  return ppo_heads_check(fn, net, pi_t, v_t, ls_t);
+}
+
+// rollout inference on checked arguments, graphed under one key per argument set
+static int ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step, int pi_t, int v_t,
+                             int ls_t, uint64_t seed, unsigned long long* offset_dev, void* action, float* logp, float* value,
+                             int use_graph, void* stream) {
+  return run_graph(capture_key(kRolloutInfer, {net}, obs, step_idx, offset_dev, action, logp, value, n_env, n_step, pi_t, v_t, ls_t,
+                               seed),
                    use_graph, stream, [&](void* st) {
-    return rollout_infer_launch<DIST>(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev, action, logp, value, st);
+    return ls_t ? rollout_infer_launch<DiagGaussian>(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev,
+                                                     static_cast<float*>(action), logp, value, st)
+                : rollout_infer_launch<Categorical>(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev,
+                                                    static_cast<int32_t*>(action), logp, value, st);
   });
 }
 
-extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
-                                     int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                                     int32_t* action, float* logp, float* value, int use_graph, void* stream) {
-  return ppo_rollout_infer<Categorical>(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, 0, seed, offset_dev, action, logp,
-                                        value, use_graph, stream);
-}
-
-extern "C" int xtb_ppo_gauss_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step,
-                                           int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
-                                           unsigned long long* offset_dev, float* action, float* logp, float* value, int use_graph,
-                                           void* stream) {
-  return ppo_rollout_infer<DiagGaussian>(net, obs, step_idx, n_env, n_step, pi_tensor, v_tensor, logstd_tensor, seed, offset_dev,
-                                         action, logp, value, use_graph, stream);
+extern "C" int xtb_ppo_rollout_infer(xtb_net* net, const void* obs, const int32_t* step_idx, int n_env, int n_step, int pi_t,
+                                     int v_t, int ls_t, uint64_t seed, unsigned long long* offset_dev, void* action, float* logp,
+                                     float* value, int use_graph, void* stream) {
+  const char* fn = "xtb_ppo_rollout_infer";
+  if (!net || !obs || !action || !logp || !value) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (int rc = ppo_infer_check(fn, net, offset_dev, n_env, n_step, pi_t, v_t, ls_t)) return rc;
+  return ppo_rollout_infer(net, obs, step_idx, n_env, n_step, pi_t, v_t, ls_t, seed, offset_dev, action, logp, value, use_graph,
+                           stream);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2690,21 +2669,19 @@ extern "C" int xtb_copy_h2d_staged(void* dst, const void* src, size_t bytes, voi
 // PPO.predict with host buffers in one call (xt/model/ppo/ppo.py:104-109): staged H2D of the observations, the
 // (graphed) rollout inference of one step into the packed block out_dev = [action | logp | value], one D2H of it (and
 // of the pi head's output into head_host when set) and a stream synchronise.
-template <class DIST>
-static int ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env, int pi_t, int v_t,
-                            int ls_t, uint64_t seed, unsigned long long* offset_dev, float* out_dev, float* out_host,
-                            float* head_host, int use_graph, void* stream) {
-  const char* fn = PpoCalls<DIST>::predict;
+extern "C" int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env, int pi_t,
+                                    int v_t, int ls_t, uint64_t seed, unsigned long long* offset_dev, float* out_dev,
+                                    float* out_host, float* head_host, int use_graph, void* stream) {
+  const char* fn = "xtb_ppo_predict_host";
   if (!net || !obs_host || !obs_dev || !out_dev || !out_host) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
-  if (int rc = ppo_heads_check<DIST>(fn, net, pi_t, v_t, ls_t)) return rc;
-  const size_t aw = DIST::action_width(net->tsize[pi_t]);
+  if (int rc = ppo_infer_check(fn, net, offset_dev, n_env, 1, pi_t, v_t, ls_t)) return rc;
+  const size_t aw = ls_t ? net->tsize[pi_t] : 1;   // action floats per env: the DiagGaussian's A, or one int32
   StreamScope sc;
   int src = sc.begin(stream, use_graph != 0);
   if (src) return src;
   CUDA_TRY(xtb::Stager::instance().stage_h2d(obs_dev, obs_host, obs_bytes, sc.st));
-  int rc = ppo_rollout_infer<DIST>(net, obs_dev, nullptr, n_env, 1, pi_t, v_t, ls_t, seed, offset_dev,
-                                   reinterpret_cast<typename DIST::Action*>(out_dev), out_dev + aw * n_env,
-                                   out_dev + (aw + 1) * n_env, use_graph, (void*)sc.st);
+  int rc = ppo_rollout_infer(net, obs_dev, nullptr, n_env, 1, pi_t, v_t, ls_t, seed, offset_dev, out_dev, out_dev + aw * n_env,
+                             out_dev + (aw + 1) * n_env, use_graph, (void*)sc.st);
   if (rc) return rc;
   CUDA_TRY(cudaMemcpyAsync(out_host, out_dev, sizeof(float) * (aw + 2) * (size_t)n_env, cudaMemcpyDeviceToHost, sc.st));
   if (head_host)
@@ -2712,25 +2689,6 @@ static int ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes
                              cudaMemcpyDeviceToHost, sc.st));
   CUDA_TRY(cudaStreamSynchronize(sc.st));
   return sc.end();
-}
-extern "C" int xtb_actor_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                                      int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                                      float* out_dev, float* out_host, float* logits_host, int use_graph, void* stream) {
-  return ppo_predict_host<Categorical>(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, 0, seed, offset_dev, out_dev,
-                                       out_host, logits_host, use_graph, stream);
-}
-extern "C" int xtb_ppo_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                                    int pi_tensor, int v_tensor, uint64_t seed, unsigned long long* offset_dev,
-                                    float* out_dev, float* out_host, int use_graph, void* stream) {
-  return xtb_actor_predict_host(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, seed, offset_dev, out_dev, out_host,
-                                nullptr, use_graph, stream);
-}
-extern "C" int xtb_ppo_gauss_predict_host(xtb_net* net, const void* obs_host, size_t obs_bytes, void* obs_dev, int n_env,
-                                          int pi_tensor, int v_tensor, int logstd_tensor, uint64_t seed,
-                                          unsigned long long* offset_dev, float* out_dev, float* out_host, int use_graph,
-                                          void* stream) {
-  return ppo_predict_host<DiagGaussian>(net, obs_host, obs_bytes, obs_dev, n_env, pi_tensor, v_tensor, logstd_tensor, seed,
-                                        offset_dev, out_dev, out_host, nullptr, use_graph, stream);
 }
 extern "C" int xtb_copy_d2h(void* dst, const void* src, size_t bytes, void* stream) {
   CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, S(stream)));

@@ -1,4 +1,5 @@
 """XTModel base: the reference's model surface (xt/model/model.py:30-136) over the CUDA engine."""
+import ctypes as C
 import glob
 import math
 import os
@@ -7,7 +8,8 @@ from collections import OrderedDict
 import numpy as np
 import torch
 
-from ..engine import Net, require_cuda
+from ..capi import check
+from ..engine import Net, _ptr, require_cuda, stream_ptr
 
 
 def glorot_uniform_(net, rng):
@@ -83,6 +85,65 @@ class XTModel(object):
         """xt/model/model.py:116-122 / tf_utils.py:135-144."""
         np_file = np.load(model_name)
         self.set_weights(OrderedDict(**np_file))
+
+
+class PolicyActor(object):
+    """The native sampling calls of an actor-critic policy (PPO, ImpalaCnnOpt).  The subclass sets `net`, `device`,
+    `use_graph`, `state_dim`, `action_dim`, `_obs_dt` (observation dtype) and the heads: `pi_t` (logits, or the
+    DiagGaussian mean), `v_t` (value) and `ls_t` (0 for Categorical, else the DiagGaussian's logstd tensor)."""
+
+    predict_head = False    # the host predict also copies the pi head's output (ImpalaCnnOpt.predict returns the logits)
+
+    def _init_sampling(self):
+        """Draw the Philox seed of every sampling call (one global np.random draw) and reset the counters."""
+        self._sample_seed = int(np.random.randint(0, 2 ** 31 - 1))
+        self._sample_offset = 0      # host counter of the calls that take their offset from the host
+        self._offset_dev = None      # device counter of rollout inference and host predict, created at first use
+        self._predict_ios = {}
+
+    def _offset(self):
+        if self._offset_dev is None:
+            self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
+        return self._offset_dev
+
+    def _predict_io(self, batch):
+        """Persistent staging of the host predict: device input, one packed device / pinned output block
+        [action | logp | value] (a DiagGaussian's action is A rows) and, with predict_head, a pinned [batch, A] block for
+        the pi head, so a call is 1 H2D + 1 graph launch + 1 D2H."""
+        io = self._predict_ios.get(batch)
+        if io is None:
+            rows = (self.action_dim if self.ls_t else 1) + 2
+            out_dev = torch.empty(rows, batch, dtype=torch.float32, device=self.device)
+            head = torch.empty(batch, self.action_dim, dtype=torch.float32).pin_memory() if self.predict_head else None
+            io = dict(obs=torch.empty((batch,) + tuple(self.state_dim), dtype=self._obs_dt, device=self.device),
+                      out_dev=out_dev, act=out_dev[0].view(torch.int32), logp=out_dev[rows - 2], val=out_dev[rows - 1],
+                      pin_out=torch.empty(rows, batch, dtype=torch.float32).pin_memory(), pin_head=head)
+            io["obs_ptr"], io["out_dev_ptr"], io["pin_out_ptr"] = _ptr(io["obs"]), _ptr(out_dev), _ptr(io["pin_out"])
+            io["pin_out_np"] = io["pin_out"].numpy()
+            self._predict_ios[batch] = io
+        return io
+
+    def _predict_host(self, state):
+        """Staged H2D of `state` -> graphed forward + sampling -> packed D2H (+ the pi head) -> stream sync, in one
+        native call; returns the IO block holding the results."""
+        batch = state.shape[0]
+        io = self._predict_io(batch)
+        self.net.ensure_batch(batch)
+        check(self.net.lib.xtb_ppo_predict_host(self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch,
+                                                self.pi_t, self.v_t, self.ls_t, C.c_uint64(self._sample_seed), _ptr(self._offset()),
+                                                io["out_dev_ptr"], io["pin_out_ptr"], _ptr(io["pin_head"]),
+                                                1 if self.use_graph else 0, stream_ptr()))
+        return io
+
+    def rollout_infer_device(self, obs_dev, step_idx, n_env, n_step, action, logp, value):
+        """n_step batched policy evaluations on device-resident observations as ONE CUDA graph (the learner-side
+        replacement of the explorers' per-step predict calls): time-major action / logp / value [n_step, n_env] (a
+        DiagGaussian's action f32 [n_step, n_env, A]); the pi head of the last step stays in net.tensor."""
+        self.net.ensure_batch(n_env)
+        check(self.net.lib.xtb_ppo_rollout_infer(self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step),
+                                                 self.pi_t, self.v_t, self.ls_t, C.c_uint64(self._sample_seed),
+                                                 _ptr(self._offset()), _ptr(action), _ptr(logp), _ptr(value),
+                                                 1 if self.use_graph else 0, stream_ptr()))
 
 
 def check_keep_model(model_path, keep_num):

@@ -1,4 +1,6 @@
 """ImpalaCnnOpt on the CUDA engine (xt/model/impala/impala_cnn_opt.py:64-297)."""
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -7,7 +9,7 @@ from ..capi import check
 from ..engine import Adam, Net, _ptr, stream_ptr
 from ..registry import Registers, import_config
 from . import archs
-from .base import XTModel, glorot_uniform_
+from .base import PolicyActor, XTModel, glorot_uniform_
 
 # xt/model/impala/default_config.py
 LR = 0.0003
@@ -16,8 +18,10 @@ GAMMA = 0.99
 
 
 @Registers.model
-class ImpalaCnnOpt(XTModel):
+class ImpalaCnnOpt(XTModel, PolicyActor):
     """IMPALA conv net with the V-trace loss evaluated inside the train step."""
+
+    predict_head = True
 
     def __init__(self, model_info):
         model_config = model_info.get("model_config", dict())
@@ -62,9 +66,10 @@ class ImpalaCnnOpt(XTModel):
             self.opt.use_rmsprop(decay=0.99, epsilon=0.1)          # impala_cnn_opt.py:205-206 (the schedule is Adam-only there)
         self._global_step = 0
         self._bufs = {}
-        self._sample_seed = int(np.random.randint(0, 2 ** 31 - 1))
-        self._sample_offset = 0
+        self._obs_dt = torch.uint8
+        self._init_sampling()
         self.logit_name, self.base_name = arch["outputs"]
+        self.pi_t, self.v_t, self.ls_t = self.net.tid[self.logit_name], self.net.tid[self.base_name], 0
         return self.net
 
     def _buffers(self, n):
@@ -122,50 +127,15 @@ class ImpalaCnnOpt(XTModel):
         loss = self.train_device(b["obs"], b["bp"], b["action"], b["done"], b["reward"], n, b["loss"])
         return float(loss.cpu()[0])
 
-    def _predict_io(self, n):
-        """Persistent staging of the host-facing predict(): device frames, packed device / pinned result blocks."""
-        io = self._bufs.get(("io", n))
-        if io is None:
-            dev = self.device
-            out_dev = torch.empty(3, n, dtype=torch.float32, device=dev)
-            io = dict(obs=torch.empty((n,) + tuple(self.state_dim), dtype=torch.uint8, device=dev), out_dev=out_dev,
-                      pin_out=torch.empty(3, n, dtype=torch.float32).pin_memory(),
-                      pin_logits=torch.empty(n, self.action_dim, dtype=torch.float32).pin_memory())
-            io["out_np"], io["logits_np"] = io["pin_out"].numpy(), io["pin_logits"].numpy()
-            self._bufs[("io", n)] = io
-        return io
-
-    def rollout_infer_device(self, obs_dev, step_idx, n_env, n_step, action, logp, value):
-        """n_step batched policy evaluations on device-resident frames as ONE CUDA graph (the learner-side replacement of
-        the explorers' per-step predict calls): time-major action / logp / baseline [n_step, n_env]; the logits of the last
-        step stay in net.tensor(logit_name)."""
-        import ctypes as C
-        if getattr(self, "_offset_dev", None) is None:
-            self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
-        self.net.ensure_batch(n_env)
-        check(self.net.lib.xtb_ppo_rollout_infer(self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step),
-                                                 self.net.tid[self.logit_name], self.net.tid[self.base_name],
-                                                 C.c_uint64(self._sample_seed), _ptr(self._offset_dev), _ptr(action), _ptr(logp),
-                                                 _ptr(value), 1 if self.use_graph else 0, stream_ptr()))
-
     def predict(self, state, uniforms=None):
         """impala_cnn_opt.py:267-277: [logits [B,A], baseline [B], action [B]]."""
         state = np.ascontiguousarray(state, np.uint8)
         n = state.shape[0]
         net = self.net
         if uniforms is None and n <= net.max_batch:
-            # staged H2D -> graphed forward + fused heads + Philox sampling -> packed D2H (+ logits) -> sync: one native call
-            import ctypes as C
-            io = self._predict_io(n)
-            if getattr(self, "_offset_dev", None) is None:
-                self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
-            net.ensure_batch(n)
-            check(net.lib.xtb_actor_predict_host(net.handle, state.ctypes.data, state.nbytes, _ptr(io["obs"]), n,
-                                                 net.tid[self.logit_name], net.tid[self.base_name], C.c_uint64(self._sample_seed),
-                                                 _ptr(self._offset_dev), _ptr(io["out_dev"]), _ptr(io["pin_out"]),
-                                                 _ptr(io["pin_logits"]), 1 if self.use_graph else 0, stream_ptr()))
-            out = io["out_np"]
-            return [io["logits_np"].copy(), out[2].copy(), out[0].view(np.int32).copy()]
+            io = self._predict_host(state)
+            out = io["pin_out_np"]
+            return [io["pin_head"].numpy().copy(), out[2].copy(), out[0].view(np.int32).copy()]
         b = self._buffers(n)
         net.ensure_batch(n)
         b["obs"].copy_(torch.from_numpy(state), non_blocking=True)
@@ -173,7 +143,6 @@ class ImpalaCnnOpt(XTModel):
         u = None
         if uniforms is not None:
             u = torch.from_numpy(np.ascontiguousarray(uniforms, np.float32)).to(self.device)
-        import ctypes as C
         check(net.lib.xtb_categorical_sample(_ptr(net.tensor(self.logit_name)), n, self.action_dim, _ptr(u),
                                              C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset),
                                              _ptr(b["action"]), _ptr(b["logp"]), stream_ptr()))

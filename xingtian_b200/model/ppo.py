@@ -9,7 +9,7 @@ from ..capi import check
 from ..engine import Adam, Net, _ptr, stream_ptr
 from ..registry import Registers, import_config
 from . import archs
-from .base import XTModel, glorot_uniform_
+from .base import PolicyActor, XTModel, glorot_uniform_
 
 # xt/model/ppo/default_config.py:1-12
 BATCH_SIZE = 200
@@ -74,13 +74,12 @@ class DeviceRollout(object):
         self.capacity = cap
 
     def as_struct(self):
-        cls = capi.PpoRollout if self.action_dim is None else capi.PpoGaussRollout
-        return cls(self.obs.data_ptr(), self.action.data_ptr(), self.old_logp.data_ptr(),
-                   self.adv.data_ptr(), self.old_v.data_ptr(), self.target_v.data_ptr())
+        return capi.PpoRollout(self.obs.data_ptr(), self.action.data_ptr(), self.old_logp.data_ptr(),
+                               self.adv.data_ptr(), self.old_v.data_ptr(), self.target_v.data_ptr())
 
 
 @Registers.model
-class PPO(XTModel):
+class PPO(XTModel, PolicyActor):
     """Build PPO network (xt/model/ppo/ppo.py:37-132)."""
 
     def __init__(self, model_info):
@@ -129,11 +128,10 @@ class PPO(XTModel):
         self._loss_dev = None
         self._pred_bufs = {}
         self._obs_ring = None
-        self._sample_seed = int(np.random.randint(0, 2 ** 31 - 1))
-        self._sample_offset = 0
+        self._init_sampling()
         self.pi_t = self.net.tid["pi_latent"]
         self.v_t = self.net.tid["output_value"]
-        self.ls_t = self.net.tid["pi_logstd"] if self.gaussian else None
+        self.ls_t = self.net.tid["pi_logstd"] if self.gaussian else 0
         return self.net
 
     # -- inference ---------------------------------------------------------------------------
@@ -182,40 +180,6 @@ class PPO(XTModel):
         v = vout if vout is not None else net.tensor("output_value")[:batch]
         return action[:batch], logp[:batch], v
 
-    def rollout_infer_device(self, obs_dev, step_idx, n_env, n_step, action, logp, value):
-        """T batched policy evaluations on device-resident observations (one CUDA graph): time-major
-        outputs action/logp/value [n_step, n_env] (a DiagGaussian actor: action f32 [n_step, n_env, A])."""
-        if getattr(self, "_offset_dev", None) is None:
-            self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
-        self.net.ensure_batch(n_env)
-        if self.gaussian:
-            check(self.net.lib.xtb_ppo_gauss_rollout_infer(
-                self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step), self.pi_t, self.v_t, self.ls_t,
-                C.c_uint64(self._sample_seed), _ptr(self._offset_dev), _ptr(action), _ptr(logp), _ptr(value),
-                1 if self.use_graph else 0, stream_ptr()))
-            return
-        check(self.net.lib.xtb_ppo_rollout_infer(self.net.handle, _ptr(obs_dev), _ptr(step_idx), int(n_env), int(n_step),
-                                                 self.pi_t, self.v_t, C.c_uint64(self._sample_seed), _ptr(self._offset_dev),
-                                                 _ptr(action), _ptr(logp), _ptr(value), 1 if self.use_graph else 0, stream_ptr()))
-
-    def _predict_io(self, batch):
-        """Persistent staging for the host-facing predict(): pinned input, device input, one packed
-        device/pinned output block [action | logp | value] so a call is 1 H2D + 1 graph launch + 1 D2H."""
-        io = self._pred_bufs.get(("io", batch))
-        if io is None:
-            dev = self.device
-            shape = (batch,) + tuple(self.state_dim)
-            # DiagGaussian: [action batch*A | logp batch | value batch] floats, as one [A + 2, batch] block
-            rows = self.action_dim + 2 if self.gaussian else 3
-            out_dev = torch.empty(rows, batch, dtype=torch.float32, device=dev)
-            io = dict(obs=torch.empty(shape, dtype=self._obs_dt, device=dev), out_dev=out_dev,
-                      act=out_dev[0].view(torch.int32), logp=out_dev[rows - 2], val=out_dev[rows - 1],
-                      pin_out=torch.empty(rows, batch, dtype=torch.float32).pin_memory())
-            io["obs_ptr"], io["out_dev_ptr"], io["pin_out_ptr"] = _ptr(io["obs"]), _ptr(out_dev), _ptr(io["pin_out"])
-            io["pin_out_np"] = io["pin_out"].numpy()
-            self._pred_bufs[("io", batch)] = io
-        return io
-
     def predict(self, state, uniforms=None, normals=None):
         """xt/model/ppo/ppo.py:104-109: (action [B] int32, logp [B,1], v [B,1]); a DiagGaussian actor returns action
         [B, A] float32 (`normals` [B, A] then replaces the Philox draws)."""
@@ -230,21 +194,8 @@ class PPO(XTModel):
             action, logp, v = self.predict_device(bufs["obs"], batch, None if self.gaussian else noise,
                                                   normals=noise if self.gaussian else None)
             return (action.cpu().numpy(), logp.cpu().numpy().reshape(batch, 1), v.cpu().numpy().reshape(batch, 1))
-        io = self._predict_io(batch)
-        if getattr(self, "_offset_dev", None) is None:
-            self._offset_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
-        self.net.ensure_batch(batch)
+        io = self._predict_host(state)
         ring = self._obs_ring
-        # staged H2D -> graphed forward + sampling -> packed D2H -> stream sync, in one native call
-        if self.gaussian:
-            check(self.net.lib.xtb_ppo_gauss_predict_host(
-                self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch, self.pi_t, self.v_t, self.ls_t,
-                C.c_uint64(self._sample_seed), _ptr(self._offset_dev), io["out_dev_ptr"], io["pin_out_ptr"],
-                1 if self.use_graph else 0, stream_ptr()))
-        else:
-            check(self.net.lib.xtb_ppo_predict_host(self.net.handle, state.ctypes.data, state.nbytes, io["obs_ptr"], batch,
-                                                    self.pi_t, self.v_t, C.c_uint64(self._sample_seed), _ptr(self._offset_dev),
-                                                    io["out_dev_ptr"], io["pin_out_ptr"], 1 if self.use_graph else 0, stream_ptr()))
         if ring is not None and batch == ring["E"]:
             # learner-side batched inference: the frames just uploaded ARE the rollout's cur_state -- keep them on the
             # device (time-major ring) so prepare_data can take them from here instead of a second H2D copy
@@ -282,16 +233,9 @@ class PPO(XTModel):
         self._perm_host[:perm.size].copy_(torch.from_numpy(perm))
         self._perm_dev[:perm.size].copy_(self._perm_host[:perm.size], non_blocking=True)
         ro = self.rollout.as_struct()
-        if self.gaussian:
-            check(self.net.lib.xtb_ppo_gauss_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs,
-                                                   int(self.num_sgd_iter), _ptr(self._perm_dev), C.byref(self.hyper),
-                                                   self.pi_t, self.v_t, self.ls_t, _ptr(self._loss_dev),
-                                                   1 if self.use_graph else 0, stream_ptr()))
-        else:
-            check(self.net.lib.xtb_ppo_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs,
-                                             int(self.num_sgd_iter), _ptr(self._perm_dev), C.byref(self.hyper),
-                                             self.pi_t, self.v_t, _ptr(self._loss_dev), 1 if self.use_graph else 0,
-                                             stream_ptr()))
+        check(self.net.lib.xtb_ppo_train(self.net.handle, self.opt.handle, C.byref(ro), int(nbatch), bs, int(self.num_sgd_iter),
+                                         _ptr(self._perm_dev), C.byref(self.hyper), self.pi_t, self.v_t, self.ls_t,
+                                         _ptr(self._loss_dev), 1 if self.use_graph else 0, stream_ptr()))
         losses = self._loss_dev[:steps].cpu().numpy()
         self.last_losses = losses
         return float(np.mean(losses))
