@@ -1,9 +1,17 @@
-// rl_kernels.cuh -- trajectory post-processing and loss kernels (HBM / latency bound).
-//   gae_kernel          : xt/agent/ppo/ppo.py:77-106      one warp per env, affine reverse scan
-//   sample_kernel       : xt/model/tf_dist.py:89-130      Gumbel-max + log-prob
-//   ppo_loss_kernel     : xt/model/ppo/__init__.py:4-25   loss + dlogits/dv, block-reduced loss
-//   vtrace_kernel       : xt/model/impala/vtrace.py:39-115 + impala_cnn_opt.py:299-351
-//   dqn_loss_kernel     : xt/algorithm/dqn/dqn.py:79-97 + Keras mse
+// rl_kernels.cuh -- trajectory post-processing, sampling and loss kernels (HBM / latency bound).
+//   gae_kernel                : xt/agent/ppo/ppo.py:77-106       one warp per env, affine reverse scan
+//   sample_kernel<DIST>       : xt/model/tf_dist.py:63-130       Categorical (Gumbel-max) / DiagGaussian draw + log-prob
+//   ppo_loss_kernel           : xt/model/ppo/__init__.py:4-25    Categorical loss + dlogits/dv, block-reduced loss
+//   ppo_gauss_loss_kernel     : xt/model/ppo/__init__.py:4-25    DiagGaussian loss + dmean/dv, ordered dlog_std and loss
+//   vtrace_kernel             : xt/model/impala/vtrace.py:39-115 + impala_cnn_opt.py:299-351
+//   dqn_loss_kernel           : xt/algorithm/dqn/dqn.py:79-97 + Keras mse (double DQN, n-step discount, Huber)
+//   nstep_kernel              : n-step returns of a device-resident rollout buffer
+//   heads_kernel<LOSS>        : both dense heads + the per-sample loss of LOSS + their backward, one warp per sample
+//   infer_heads_kernel<DIST>  : both dense heads + the draw of DIST (rollout inference), one warp per sample
+//   dueling_fwd / dgrad       : the dueling combine layer
+//   IMPALA Keras, MuZero      : softmax_rows, impala_keras_*, mse_loss; mz_*
+// The per-sample rules (categorical_draw / gaussian_draw, ppo_categorical_row, ppo_gauss_row, dqn_td_target / td_loss)
+// are written once: the standalone kernels of the layer-by-layer path and the fused heads kernels both call them.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -114,11 +122,15 @@ __device__ inline void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
 
 // Categorical draw of sample b (xt/model/tf_dist.py:89-130): Gumbel-max over its logits lg[0..A), A <= n (n: the
 // size of a register array, whose loops are unrolled, or A).  Uniform i is u[i] when u is set, else a word of
-// Philox4x32-10 on counter (b, i / 4, offset) mapped into (0, 1).  The first maximum wins, like np.argmax.  Returns the
-// action; logp = its log-probability.
+// Philox4x32-10 on counter (b, i / 4, offset) mapped into (0, 1).  The first maximum wins, like np.argmax.  Writes the
+// action to action[b] and, when head_out is set, the logits to its row b; returns the action's log-probability.
 template <class LG>
-__device__ __forceinline__ int categorical_draw(const LG& lg, int n, int A, const float* u, int b, uint64_t seed,
-                                                uint64_t offset, float& logp) {
+__device__ __forceinline__ float categorical_draw(const LG& lg, int n, int A, const float* u, int b, uint64_t seed,
+                                                  uint64_t offset, int32_t* action, float* head_out) {
+  if (head_out) {
+#pragma unroll
+    for (int i = 0; i < n; i++) if (i < A) head_out[(long long)b * A + i] = lg[i];
+  }
   float mx = -INFINITY;
 #pragma unroll
   for (int i = 0; i < n; i++) if (i < A) mx = fmaxf(mx, lg[i]);
@@ -149,27 +161,10 @@ __device__ __forceinline__ int categorical_draw(const LG& lg, int n, int A, cons
   float la = 0.f;
 #pragma unroll
   for (int i = 0; i < n; i++) if (i == bi) la = lg[i];
-  logp = la - mx - lz;
-  return bi;
+  action[b] = bi;
+  return la - mx - lz;
 }
 
-// One thread per sample: the categorical draw from logits [B, A] with uniforms [B, A] if set, else Philox at `offset`,
-// or at *offset_dev + t_add when offset_dev is set (the device-resident counter of rollout inference, so that CUDA-graph
-// replays draw fresh noise).  v_out != NULL: the value head output is copied out alongside.
-__global__ void sample_kernel(const float* __restrict__ logits, int B, int A, const float* __restrict__ uniforms,
-                              uint64_t seed, uint64_t offset, const unsigned long long* __restrict__ offset_dev, int t_add,
-                              int32_t* __restrict__ action, float* __restrict__ logp, const float* __restrict__ v_in,
-                              float* __restrict__ v_out) {
-  pdl_wait(); pdl_trigger();
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
-  float lp;
-  action[b] = categorical_draw(logits + (long long)b * A, A, A, uniforms ? uniforms + (long long)b * A : nullptr, b, seed,
-                               offset, lp);
-  logp[b] = lp;
-  if (v_out) v_out[b] = v_in[b];
-}
 __global__ void bump_counter_kernel(unsigned long long* ctr, int add) {
   pdl_wait(); pdl_trigger(); *ctr += (unsigned long long)add; }
 
@@ -207,6 +202,43 @@ __device__ __forceinline__ PpoClipTerms ppo_clip_terms(float logp_a, float old_l
   return {surr, dsurr, hp.critic_coef * 0.5f * fmaxf(l1, l2), hp.critic_coef * 0.5f * dvl * inv_count};
 }
 
+// Categorical PPO loss of sample b: actor loss with entropy + clipped critic loss (xt/model/ppo/__init__.py:4-25) on
+// its logits lg[0..A), A <= n (as in categorical_draw), and value vv; the rollout row is r = idx ? idx[b] : b.  Fills
+// dl[i] = d loss / d logit_i (0 for A <= i < n) and dv = d loss / d v; returns the sample's loss term.
+template <class LG, class DL>
+__device__ __forceinline__ float ppo_categorical_row(const LG& lg, int n, int A, float vv, const int32_t* idx, int b,
+                                                     const int32_t* action, const float* old_logp, const float* adv,
+                                                     const float* old_v, const float* target_v, const PpoHyperDev& hp,
+                                                     float inv_count, DL& dl, float& dv) {
+  float mx = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i < A) mx = fmaxf(mx, lg[i]);
+  float z = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i < A) z += expf(lg[i] - mx);
+  const float lz = logf(z);
+  float H = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i < A) { const float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
+  const int r = idx ? idx[b] : b;
+  const int ac = action[r];
+  float logp_a = 0.f;
+#pragma unroll
+  for (int i = 0; i < n; i++) if (i == ac) logp_a = lg[i] - mx - lz;
+  const PpoClipTerms c = ppo_clip_terms(logp_a, old_logp[r], adv[r], vv, old_v[r], target_v[r], hp, inv_count);
+  dv = c.dv;
+#pragma unroll
+  for (int i = 0; i < n; i++) {
+    float d = 0.f;
+    if (i < A) {   // d logp_a / d l_i = [i == a] - p_i,  d H / d l_i = -p_i (logp_i + H)
+      const float rl = lg[i] - mx, p = expf(rl) / z;
+      d = (-c.dsurr * (((i == ac) ? 1.f : 0.f) - p) + hp.ent_coef * p * (rl - lz + H)) * inv_count;
+    }
+    dl[i] = d;
+  }
+  return (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
+}
+
 __global__ void ppo_loss_kernel(const float* __restrict__ logits, const float* __restrict__ v,
                                 const int32_t* __restrict__ idx, const int32_t* __restrict__ action,
                                 const float* __restrict__ old_logp, const float* __restrict__ adv,
@@ -218,28 +250,9 @@ __global__ void ppo_loss_kernel(const float* __restrict__ logits, const float* _
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   float lsum = 0.f;
   if (b < B) {
-    int r = idx ? idx[b] : b;
-    const float* l = logits + (long long)b * A;
-    float lg[MAX_ADIM];
-    float mx = -INFINITY;
-    for (int i = 0; i < A; i++) { lg[i] = l[i]; mx = fmaxf(mx, lg[i]); }
-    float z = 0.f;
-    for (int i = 0; i < A; i++) z += expf(lg[i] - mx);
-    float lz = logf(z);
-    float H = 0.f;
-    for (int i = 0; i < A; i++) { float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
-    int a = action[r];
-    const PpoClipTerms c = ppo_clip_terms(lg[a] - mx - lz, old_logp[r], adv[r], v[b], old_v[r], target_v[r], hp, inv_count);
-    lsum = (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
-    dv[b] = c.dv;
-    for (int i = 0; i < A; i++) {
-      float rl = lg[i] - mx;
-      float p = expf(rl) / z;
-      float logp_i = rl - lz;
-      float dlogp = ((i == a) ? 1.f : 0.f) - p;             // d logp_a / d l_i
-      float dH = -p * (logp_i + H);                           // d H / d l_i
-      dlogits[(long long)b * A + i] = (-c.dsurr * dlogp - hp.ent_coef * dH) * inv_count;
-    }
+    float* dl = dlogits + (long long)b * A;
+    lsum = ppo_categorical_row(logits + (long long)b * A, A, A, v[b], idx, b, action, old_logp, adv, old_v, target_v, hp,
+                               inv_count, dl, dv[b]);
   }
   block_atomic_add(lsum, loss_out);
 }
@@ -359,6 +372,37 @@ __global__ void vtrace_kernel(const float* __restrict__ tp_logits, const float* 
 //   huber > 0    : Huber loss with that delta instead of the squared error (gradient clip(diff, -delta, delta))
 //   idx != NULL  : action / reward / done / disc are indexed through idx (minibatch rows of a replay ring)
 // ------------------------------------------------------------------------------------------
+// TD target of sample b, rollout row r: the max over the next-state Q row b of the target net (qn_o set: double DQN,
+// the target net's Q at the online net's argmax, the first maximum winning) bootstraps the reward unless done[r]
+__device__ __forceinline__ float dqn_td_target(const float* qn_t, const float* qn_o, const float* reward, const uint8_t* done,
+                                               const float* disc, float gamma, int b, int r, int A) {
+  const float* t = qn_t + (long long)b * A;
+  float mq;
+  if (qn_o) {
+    const float* o = qn_o + (long long)b * A;
+    float best = o[0]; int bi = 0;
+    for (int i = 1; i < A; i++) if (o[i] > best) { best = o[i]; bi = i; }
+    mq = t[bi];
+  } else {
+    mq = t[0];
+    for (int i = 1; i < A; i++) mq = fmaxf(mq, t[i]);
+  }
+  const float g = disc ? disc[r] : gamma;
+  return done[r] ? reward[r] : reward[r] + g * mq;
+}
+
+// loss of the TD error diff = Q(s, a) - y (the squared error, or with huber > 0 the Huber loss of that delta);
+// grad = d loss / d diff
+__device__ __forceinline__ float td_loss(float diff, float huber, float& grad) {
+  float l;
+  if (huber > 0.f) {
+    const float ad = fabsf(diff);
+    l = ad <= huber ? 0.5f * diff * diff : huber * (ad - 0.5f * huber);
+    grad = fminf(fmaxf(diff, -huber), huber);
+  } else { l = diff * diff; grad = 2.f * diff; }
+  return l;
+}
+
 __global__ void dqn_loss_kernel(const float* __restrict__ q, const float* __restrict__ qn_t,
                                 const float* __restrict__ qn_o, const int32_t* __restrict__ idx,
                                 const int32_t* __restrict__ action, const float* __restrict__ reward,
@@ -370,27 +414,10 @@ __global__ void dqn_loss_kernel(const float* __restrict__ q, const float* __rest
   float lsum = 0.f;
   if (b < B) {
     const int r = idx ? idx[b] : b;
-    const float* t = qn_t + (long long)b * A;
-    float mq;
-    if (qn_o) {
-      const float* o = qn_o + (long long)b * A;
-      float best = o[0]; int bi = 0;
-      for (int i = 1; i < A; i++) if (o[i] > best) { best = o[i]; bi = i; }
-      mq = t[bi];
-    } else {
-      mq = t[0];
-      for (int i = 1; i < A; i++) mq = fmaxf(mq, t[i]);
-    }
-    const float g = disc ? disc[r] : gamma;
-    float y = done[r] ? reward[r] : reward[r] + g * mq;
-    int a = action[r];
-    float diff = q[(long long)b * A + a] - y;
-    float grad, l;
-    if (huber > 0.f) {
-      const float ad = fabsf(diff);
-      l = ad <= huber ? 0.5f * diff * diff : huber * (ad - 0.5f * huber);
-      grad = fminf(fmaxf(diff, -huber), huber);
-    } else { l = diff * diff; grad = 2.f * diff; }
+    const float y = dqn_td_target(qn_t, qn_o, reward, done, disc, gamma, b, r, A);
+    const int a = action[r];
+    float grad;
+    const float l = td_loss(q[(long long)b * A + a] - y, huber, grad);
     for (int i = 0; i < A; i++) dq[(long long)b * A + i] = (i == a) ? grad * inv_count : 0.f;
     if (y_out) y_out[b] = y;
     lsum = l * inv_count;
@@ -462,7 +489,7 @@ struct PpoHeadsArgs {
 // the same values.  Fill dl[i] = dloss/d(pi head output i), dv = dloss/d(v head output) (0 for i >= A) and, on lane 0,
 // add the sample's loss to lsum and the bias gradients to dbp / dbv.  A policy with kLogStd also adds, on lane 0, the
 // gradient wrt the state-independent log_std to dls (an extra A slab floats); the others leave dls alone.
-// PPO: categorical actor loss with entropy + clipped critic loss (xt/model/ppo/__init__.py:4-25).
+// PPO: ppo_categorical_row on logits = acc[0..A) + b_pi, v = acc[HEAD_AMAX] + b_v.
 struct PpoLoss {
   static constexpr bool kLogStd = false;
   template <int HEAD_AMAX>
@@ -470,33 +497,14 @@ struct PpoLoss {
                                                 float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
                                                 float& dbv, float (&)[HEAD_AMAX]) {
     const int A = a.A;
-    float lg[HEAD_AMAX]; float mx = -INFINITY;
+    float lg[HEAD_AMAX];
 #pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) { lg[i] = (i < A) ? acc[i] + a.b_pi[i] : -INFINITY; mx = fmaxf(mx, lg[i]); }
-    float vv = acc[HEAD_AMAX] + a.b_v[0];
-    float z = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) z += expf(lg[i] - mx);
-    float lz = logf(z), H = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i < A) { float rl = lg[i] - mx; H += (expf(rl) / z) * (lz - rl); }
-    int r = a.idx ? a.idx[b] : b;
-    int ac = a.action[r];
-    float logp_a = 0.f;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) logp_a = lg[i] - mx - lz;
-    const PpoClipTerms c = ppo_clip_terms(logp_a, a.old_logp[r], a.adv[r], vv, a.old_v[r], a.target_v[r], a.hp, a.inv_count);
-    dv = c.dv;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) {
-      dl[i] = 0.f;
-      if (i < A) {
-        float rl = lg[i] - mx, p = expf(rl) / z;
-        dl[i] = (-c.dsurr * (((i == ac) ? 1.f : 0.f) - p) + a.hp.ent_coef * p * (rl - lz + H)) * a.inv_count;
-      }
-    }
+    for (int i = 0; i < HEAD_AMAX; i++) lg[i] = (i < A) ? acc[i] + a.b_pi[i] : -INFINITY;
+    const float vv = acc[HEAD_AMAX] + a.b_v[0];
+    const float l = ppo_categorical_row(lg, HEAD_AMAX, A, vv, a.idx, b, a.action, a.old_logp, a.adv, a.old_v, a.target_v, a.hp,
+                                        a.inv_count, dl, dv);
     if (lane == 0) {
-      lsum += (-c.surr - a.hp.ent_coef * H + c.critic) * a.inv_count;
+      lsum += l;
       if (a.logits_out) for (int i = 0; i < A; i++) a.logits_out[(long long)b * A + i] = lg[i];
       if (a.v_out) a.v_out[b] = vv;
       dbv += dv;
@@ -507,7 +515,7 @@ struct PpoLoss {
 };
 
 // Dueling DQN TD step: value = pi head [A], adv = v head [1], q = adv + (value - mean_a value) (xt/model/dqn/dqn_mlp.py:80-87),
-// then the TD target, loss and d(loss)/dq of dqn_loss_kernel.  Only the taken action carries gradient, g = c e_a, so
+// then dqn_td_target and td_loss, as in dqn_loss_kernel.  Only the taken action carries gradient, g = c e_a, so
 // dvalue = c (e_a - 1/A) and dadv = c.
 struct DuelingTdLoss {
   static constexpr bool kLogStd = false;
@@ -525,26 +533,9 @@ struct DuelingTdLoss {
     float q_a = 0.f;
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) q_a = adv + (val[i] - mean);
-    const float* t = a.qn_t + (long long)b * A;
-    float mq;
-    if (a.qn_o) {
-      const float* o = a.qn_o + (long long)b * A;
-      float best = o[0]; int bi = 0;
-      for (int i = 1; i < A; i++) if (o[i] > best) { best = o[i]; bi = i; }
-      mq = t[bi];
-    } else {
-      mq = t[0];
-      for (int i = 1; i < A; i++) mq = fmaxf(mq, t[i]);
-    }
-    const float g = a.disc ? a.disc[r] : a.gamma;
-    const float y = a.done[r] ? a.reward[r] : a.reward[r] + g * mq;
-    const float diff = q_a - y;
-    float grad, l;
-    if (a.huber > 0.f) {
-      const float ad = fabsf(diff);
-      l = ad <= a.huber ? 0.5f * diff * diff : a.huber * (ad - 0.5f * a.huber);
-      grad = fminf(fmaxf(diff, -a.huber), a.huber);
-    } else { l = diff * diff; grad = 2.f * diff; }
+    const float y = dqn_td_target(a.qn_t, a.qn_o, a.reward, a.done, a.disc, a.gamma, b, r, A);
+    float grad;
+    const float l = td_loss(q_a - y, a.huber, grad);
     const float c = grad * a.inv_count, cm = c / A;
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? ((i == ac) ? c : 0.f) - cm : 0.f;
@@ -720,7 +711,7 @@ constexpr float kHalfLog2Pi = 0.918938533204672742f;     // 0.5 log(2 pi)
 constexpr float kGaussEntConst = 1.418938533204672742f;  // 0.5 (log(2 pi) + 1)
 
 // standard normals n[0..4) of sample b, dimensions 4g..4g+3: one Philox call (counter (b, g, offset), the uniform
-// mapping of sample_kernel, never 0 or 1) and Box-Muller on the two pairs of its words
+// mapping of categorical_draw, never 0 or 1) and Box-Muller on the two pairs of its words
 __device__ inline void gauss_normals4(int b, int g, uint64_t seed, uint64_t offset, float (&n)[4]) {
   uint32_t c[4] = {(uint32_t)b, (uint32_t)g, (uint32_t)(offset & 0xffffffffu), (uint32_t)(offset >> 32)};
   philox4x32_10(c, (uint32_t)(seed & 0xffffffffu), (uint32_t)(seed >> 32));
@@ -735,42 +726,72 @@ __device__ inline void gauss_normals4(int b, int g, uint64_t seed, uint64_t offs
   }
 }
 
-// DiagGaussianDist.sample + log_prob, one thread per sample: x = mean + std n, logp = -neglog_prob(x) computed from x
-// (tf_dist.py:63-66, 85-86).  normals != NULL: n from it; else Philox with offset (or *offset_dev + t_add when
-// offset_dev is set: the device-resident counter of rollout inference).  v_out != NULL: the value head is copied out.
-__global__ void gauss_sample_kernel(const float* __restrict__ mean, const float* __restrict__ log_std, int B, int A,
-                                    const float* __restrict__ normals, uint64_t seed, uint64_t offset,
-                                    const unsigned long long* __restrict__ offset_dev, int t_add, float* __restrict__ action,
-                                    float* __restrict__ logp, const float* __restrict__ v_in, float* __restrict__ v_out) {
-  pdl_wait(); pdl_trigger();
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
-  const float* m = mean + (long long)b * A;
+// DiagGaussianDist.sample + log_prob of sample b (xt/model/tf_dist.py:63-66, 85-86) with mean m[0..A), A <= n (as in
+// categorical_draw): x_i = m_i + exp(log_std_i) n_i, n_i = nrm[i] when nrm is set, else normal i % 4 of gauss_normals4 at
+// counter (b, i / 4, offset).  Writes x to row b of action and, when head_out is set, the mean to its row b; returns
+// logp = -neglog_prob(x), computed from x.
+template <class M>
+__device__ __forceinline__ float gaussian_draw(const M& m, int n, int A, const float* log_std, const float* nrm, int b,
+                                               uint64_t seed, uint64_t offset, float* action, float* head_out) {
   float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int i = 0; i < A; i++) {
-    float n;
-    if (normals) {
-      n = normals[(long long)b * A + i];
-    } else {
-      if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
-      n = (i & 3) == 0 ? n4[0] : (i & 3) == 1 ? n4[1] : (i & 3) == 2 ? n4[2] : n4[3];
+#pragma unroll
+  for (int i = 0; i < n; i++) {
+    if (i < A) {
+      float nv;
+      if (nrm) {
+        nv = nrm[i];
+      } else {
+        if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
+        nv = (i & 3) == 0 ? n4[0] : (i & 3) == 1 ? n4[1] : (i & 3) == 2 ? n4[2] : n4[3];
+      }
+      const float ls = log_std[i], sd = expf(ls);
+      const float x = m[i] + sd * nv;
+      const float z = (x - m[i]) / sd;
+      q += z * z; sls += ls;
+      action[(long long)b * A + i] = x;
+      if (head_out) head_out[(long long)b * A + i] = m[i];
     }
-    const float ls = log_std[i], sd = expf(ls);
-    const float x = m[i] + sd * n;
-    const float z = (x - m[i]) / sd;
-    q += z * z; sls += ls;
-    action[(long long)b * A + i] = x;
   }
-  logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
-  if (v_out) v_out[b] = v_in[b];
+  return -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
 }
 
-// actor_loss_with_entropy + critic_loss (xt/model/ppo/__init__.py:4-25) on the Gaussian head, one block, a thread per
-// sample.  With z_i = (x_i - mean_i) / std_i (x = the behaviour action of row idx[b]):
+// Gaussian PPO loss of one sample: actor loss with entropy + clipped critic loss (xt/model/ppo/__init__.py:4-25) on its
+// mean m[0..A), A <= N, value vv and log_std[0..A).  x = the behaviour action of rollout row r; with std = exp(log_std)
+// and z_i = (x_i - m_i) / std_i:
 //   dlogp/dmean_i = z_i / std_i,  dlogp/dlog_std_i = z_i^2 - 1,  dH/dlog_std_i = 1
-// dmean / dv per sample; dlog_std and the loss are summed over the samples in a fixed order (warp butterflies, then the
-// warps in order), so the result is reproducible.  AMAX >= A.
+// Writes dm[i] = d loss / d mean_i for i < A, adds the sample's d loss / d log_std_i to dls[i] when add_ls is set, sets
+// dv = d loss / d v and returns the sample's loss term.
+template <int N, class M, class DM>
+__device__ __forceinline__ float ppo_gauss_row(const M& m, const float* log_std, int A, float vv, int r, const float* action,
+                                               const float* old_logp, const float* adv, const float* old_v, const float* target_v,
+                                               const PpoHyperDev& hp, float inv_count, DM& dm, float (&dls)[N], bool add_ls,
+                                               float& dv) {
+  const float* x = action + (long long)r * A;
+  float sd[N], z[N], q = 0.f, sls = 0.f, H = 0.f;
+#pragma unroll
+  for (int i = 0; i < N; i++) {
+    sd[i] = 1.f; z[i] = 0.f;
+    if (i < A) {
+      const float ls = log_std[i];
+      const float mi = m[i];
+      sd[i] = expf(ls);
+      z[i] = (x[i] - mi) / sd[i];
+      q += z[i] * z[i]; sls += ls; H += ls + kGaussEntConst;
+    }
+  }
+  const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+  const PpoClipTerms c = ppo_clip_terms(logp_a, old_logp[r], adv[r], vv, old_v[r], target_v[r], hp, inv_count);
+  dv = c.dv;
+#pragma unroll
+  for (int i = 0; i < N; i++) if (i < A) dm[i] = -c.dsurr * (z[i] / sd[i]) * inv_count;
+#pragma unroll
+  for (int i = 0; i < N; i++) if (i < A && add_ls) dls[i] += (-c.dsurr * (z[i] * z[i] - 1.f) - hp.ent_coef) * inv_count;
+  return (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
+}
+
+// ppo_gauss_row over a minibatch, one block, a thread per sample: dmean / dv per sample; dlog_std and the loss are
+// summed over the samples in a fixed order (warp butterflies, then the warps in order), so the result is reproducible.
+// AMAX >= A.
 constexpr int GAUSS_LOSS_THREADS = 256;
 template <int AMAX>
 __global__ void __launch_bounds__(GAUSS_LOSS_THREADS)
@@ -781,37 +802,14 @@ ppo_gauss_loss_kernel(const float* __restrict__ mean, const float* __restrict__ 
                       float* __restrict__ dlog_std, float* __restrict__ loss_out) {
   pdl_wait(); pdl_trigger();
   __shared__ float red[GAUSS_LOSS_THREADS / 32][AMAX + 1];
-  float ls[AMAX], sd[AMAX], acc[AMAX];
-  float H = 0.f, sls = 0.f;
+  float acc[AMAX];
 #pragma unroll
-  for (int i = 0; i < AMAX; i++) {
-    ls[i] = i < A ? log_std[i] : 0.f;
-    sd[i] = expf(ls[i]);
-    acc[i] = 0.f;
-    if (i < A) { H += ls[i] + kGaussEntConst; sls += ls[i]; }
-  }
+  for (int i = 0; i < AMAX; i++) acc[i] = 0.f;
   float lsum = 0.f;
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int r = idx ? idx[b] : b;
-    const float* m = mean + (long long)b * A;
-    const float* x = action + (long long)r * A;
-    float z[AMAX], q = 0.f;
-#pragma unroll
-    for (int i = 0; i < AMAX; i++) {
-      z[i] = 0.f;
-      if (i < A) { z[i] = (x[i] - m[i]) / sd[i]; q += z[i] * z[i]; }
-    }
-    const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
-    const PpoClipTerms c = ppo_clip_terms(logp_a, old_logp[r], adv[r], v[b], old_v[r], target_v[r], hp, inv_count);
-    lsum += (-c.surr - hp.ent_coef * H + c.critic) * inv_count;
-    dv[b] = c.dv;
-#pragma unroll
-    for (int i = 0; i < AMAX; i++) {
-      if (i < A) {
-        dmean[(long long)b * A + i] = -c.dsurr * (z[i] / sd[i]) * inv_count;
-        acc[i] += (-c.dsurr * (z[i] * z[i] - 1.f) - hp.ent_coef) * inv_count;
-      }
-    }
+    float* dm = dmean + (long long)b * A;
+    lsum += ppo_gauss_row(mean + (long long)b * A, log_std, A, v[b], idx ? idx[b] : b, action, old_logp, adv, old_v, target_v, hp,
+                          inv_count, dm, acc, true, dv[b]);
   }
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   lsum = warp_sum(lsum);
@@ -830,8 +828,8 @@ ppo_gauss_loss_kernel(const float* __restrict__ mean, const float* __restrict__ 
   }
 }
 
-// heads_kernel policy of the Gaussian PPO step: the loss of ppo_gauss_loss_kernel on mean = h . W_pi + b_pi and
-// v = h . W_v + b_v; the per-sample log_std gradient goes to dls (the extra A slab floats, reduced in block order).
+// heads_kernel policy of the Gaussian PPO step: ppo_gauss_row on mean = acc[0..A) + b_pi and v = acc[HEAD_AMAX] + b_v;
+// lane 0 adds the per-sample log_std gradient to dls (the extra A slab floats, reduced in block order).
 struct PpoGaussLoss {
   static constexpr bool kLogStd = true;
   template <int HEAD_AMAX>
@@ -839,35 +837,23 @@ struct PpoGaussLoss {
                                                 float (&dl)[HEAD_AMAX], float& dv, float& lsum, float (&dbp)[HEAD_AMAX],
                                                 float& dbv, float (&dls)[HEAD_AMAX]) {
     const int A = a.A;
+#pragma unroll
+    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = 0.f;
     const int r = a.idx ? a.idx[b] : b;
-    const float* x = a.action_f + (long long)r * A;
-    float mean[HEAD_AMAX], sd[HEAD_AMAX], z[HEAD_AMAX], q = 0.f, sls = 0.f, H = 0.f;
+    float mean[HEAD_AMAX];
 #pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) {
-      mean[i] = 0.f; sd[i] = 1.f; z[i] = 0.f;
-      if (i < A) {
-        const float ls = a.log_std[i];
-        mean[i] = acc[i] + a.b_pi[i];
-        sd[i] = expf(ls);
-        z[i] = (x[i] - mean[i]) / sd[i];
-        q += z[i] * z[i]; sls += ls; H += ls + kGaussEntConst;
-      }
-    }
+    for (int i = 0; i < HEAD_AMAX; i++) mean[i] = (i < A) ? acc[i] + a.b_pi[i] : 0.f;
     const float vv = acc[HEAD_AMAX] + a.b_v[0];
-    const float logp_a = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
-    const PpoClipTerms c = ppo_clip_terms(logp_a, a.old_logp[r], a.adv[r], vv, a.old_v[r], a.target_v[r], a.hp, a.inv_count);
-    dv = c.dv;
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? -c.dsurr * (z[i] / sd[i]) * a.inv_count : 0.f;
+    const float l = ppo_gauss_row(mean, a.log_std, A, vv, r, a.action_f, a.old_logp, a.adv, a.old_v, a.target_v, a.hp, a.inv_count,
+                                  dl, dls, lane == 0, dv);
     if (lane == 0) {
-      lsum += (-c.surr - a.hp.ent_coef * H + c.critic) * a.inv_count;
+      lsum += l;
       if (a.v_out) a.v_out[b] = vv;
       dbv += dv;
 #pragma unroll
       for (int i = 0; i < HEAD_AMAX; i++) {
         if (a.logits_out && i < A) a.logits_out[(long long)b * A + i] = mean[i];
         dbp[i] += dl[i];
-        if (i < A) dls[i] += (-c.dsurr * (z[i] * z[i] - 1.f) - a.hp.ent_coef) * a.inv_count;
       }
     }
   }
@@ -875,54 +861,68 @@ struct PpoGaussLoss {
 
 // Action distributions of the PPO pipeline.  Action: the action element, one per sample (Categorical: int32 [B]) or A
 // per sample (DiagGaussian: float [B, A]); kLogStd: the policy owns the log_std parameters; Loss: its heads_kernel
-// policy.  infer(): lane 0 of infer_heads_kernel turns the head sums acc (as in heads_kernel) into the sample's draw,
-// writes action / logp and, when head_out is set, the pi head's output (logits / mean).
+// policy; draw: its draw of sample b from the pi head's output (logits / mean) with noise row nz (uniforms / standard
+// normals) or, when nz is NULL, Philox at offset.  infer: the same draw in infer_heads_kernel, on the head sums acc (as
+// in heads_kernel) plus b_pi; returns logp.
 struct Categorical {
   using Action = int32_t;
   using Loss = PpoLoss;
   static constexpr bool kLogStd = false;
   __host__ __device__ static constexpr int action_width(int) { return 1; }
   template <int HEAD_AMAX>
-  static __device__ __forceinline__ void infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float*, int b, int A,
-                                               uint64_t seed, uint64_t offset, int32_t* action, float* logp, float* head_out) {
+  static __device__ __forceinline__ float infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float*, int b, int A,
+                                                uint64_t seed, uint64_t offset, int32_t* action, float* head_out) {
     float lg[HEAD_AMAX];
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) lg[i] = (i < A) ? acc[i] + b_pi[i] : -INFINITY;
-    if (head_out) {
-#pragma unroll
-      for (int i = 0; i < HEAD_AMAX; i++) if (i < A) head_out[(long long)b * A + i] = lg[i];
-    }
-    float lp;
-    action[b] = categorical_draw(lg, HEAD_AMAX, A, nullptr, b, seed, offset, lp);
-    logp[b] = lp;
+    return categorical_draw(lg, HEAD_AMAX, A, nullptr, b, seed, offset, action, head_out);
+  }
+  template <class H>
+  static __device__ __forceinline__ float draw(const H& head, int n, int A, const float*, const float* nz, int b, uint64_t seed,
+                                               uint64_t offset, int32_t* action, float* head_out) {
+    return categorical_draw(head, n, A, nz, b, seed, offset, action, head_out);
   }
 };
 
-// the sample of gauss_sample_kernel
 struct DiagGaussian {
   using Action = float;
   using Loss = PpoGaussLoss;
   static constexpr bool kLogStd = true;
   __host__ __device__ static constexpr int action_width(int A) { return A; }
   template <int HEAD_AMAX>
-  static __device__ __forceinline__ void infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float* log_std, int b,
-                                               int A, uint64_t seed, uint64_t offset, float* action, float* logp, float* head_out) {
-    float q = 0.f, sls = 0.f, n4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int i = 0; i < HEAD_AMAX; i++) {
-      if (i < A) {
-        if ((i & 3) == 0) gauss_normals4(b, i >> 2, seed, offset, n4);
-        const float m = acc[i] + b_pi[i], ls = log_std[i], sd = expf(ls);
-        const float x = m + sd * n4[i & 3];
-        const float z = (x - m) / sd;
-        q += z * z; sls += ls;
-        action[(long long)b * A + i] = x;
-        if (head_out) head_out[(long long)b * A + i] = m;
-      }
-    }
-    logp[b] = -((kHalfLog2Pi * (float)A + 0.5f * q) + sls);
+  static __device__ __forceinline__ float infer(const float (&acc)[HEAD_AMAX + 1], const float* b_pi, const float* log_std, int b,
+                                                int A, uint64_t seed, uint64_t offset, float* action, float* head_out) {
+    struct {   // mean i, formed where gaussian_draw reads it
+      const float (&acc)[HEAD_AMAX + 1]; const float* b_pi;
+      __device__ float operator[](int i) const { return acc[i] + b_pi[i]; }
+    } mean{acc, b_pi};
+    return gaussian_draw(mean, HEAD_AMAX, A, log_std, nullptr, b, seed, offset, action, head_out);
+  }
+  template <class H>
+  static __device__ __forceinline__ float draw(const H& head, int n, int A, const float* log_std, const float* nz, int b,
+                                               uint64_t seed, uint64_t offset, float* action, float* head_out) {
+    return gaussian_draw(head, n, A, log_std, nz, b, seed, offset, action, head_out);
   }
 };
+
+// One thread per sample: the draw of DIST from the pi head's output pi [B, A] with noise [B, A] if set, else Philox at
+// `offset`, or at *offset_dev + t_add when offset_dev is set (the device-resident counter of rollout inference, so that
+// CUDA-graph replays draw fresh noise).  log_std: DiagGaussian only.  v_out != NULL: the value head output is copied out
+// alongside.
+template <class DIST>
+__global__ void sample_kernel(const float* __restrict__ pi, const float* __restrict__ log_std, int B, int A,
+                              const float* __restrict__ noise, uint64_t seed, uint64_t offset,
+                              const unsigned long long* __restrict__ offset_dev, int t_add,
+                              typename DIST::Action* __restrict__ action, float* __restrict__ logp,
+                              const float* __restrict__ v_in, float* __restrict__ v_out) {
+  pdl_wait(); pdl_trigger();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
+  logp[b] = DIST::draw(pi + (long long)b * A, A, A, log_std, noise ? noise + (long long)b * A : nullptr, b, seed, offset, action,
+                       nullptr);
+  if (v_out) v_out[b] = v_in[b];
+}
 
 // Inference heads of PPO: the pi head (logits / mean) and the value head of one dense layer each, then the draw of
 // DIST at Philox offset *offset_dev + t_add (the device-resident counter of rollout inference), in one kernel, one warp
@@ -955,7 +955,7 @@ infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v
 #pragma unroll
     for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
     if (lane == 0) {
-      DIST::template infer<HEAD_AMAX>(acc, b_pi, log_std, b, A, seed, offset, action, logp, head_out);
+      logp[b] = DIST::template infer<HEAD_AMAX>(acc, b_pi, log_std, b, A, seed, offset, action, head_out);
       v_out[b] = acc[HEAD_AMAX] + b_v[0];
     }
   }

@@ -1529,8 +1529,8 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
 extern "C" int xtb_categorical_sample(const float* logits, int batch, int adim, const float* uniforms,
                                       uint64_t seed, uint64_t offset, int32_t* action, float* logp, void* stream) {
   if (!logits || !action || !logp || batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_categorical_sample: bad argument");
-  XLAUNCH(sample_kernel, (batch + 127) / 128, 128, 0, S(stream), logits, batch, adim, uniforms, seed, offset,
-          (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
+  XLAUNCH(sample_kernel<Categorical>, (batch + 127) / 128, 128, 0, S(stream), logits, (const float*)nullptr, batch, adim, uniforms,
+          seed, offset, (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
   LAUNCH_CHECK();
   return XTB_OK;
 }
@@ -1575,7 +1575,7 @@ extern "C" int xtb_diag_gaussian_sample(const float* mean, const float* log_std,
                                         uint64_t seed, uint64_t offset, float* action, float* logp, void* stream) {
   if (!mean || !log_std || !action || !logp || batch <= 0 || adim <= 0 || adim > MAX_ADIM)
     return fail(XTB_ERR_ARG, "xtb_diag_gaussian_sample: bad argument");
-  XLAUNCH(gauss_sample_kernel, (batch + 127) / 128, 128, 0, S(stream), mean, log_std, batch, adim, normals, seed, offset,
+  XLAUNCH(sample_kernel<DiagGaussian>, (batch + 127) / 128, 128, 0, S(stream), mean, log_std, batch, adim, normals, seed, offset,
           (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
   LAUNCH_CHECK();
   return XTB_OK;
@@ -2602,12 +2602,9 @@ static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* st
               (const float*)out_f32(net, lpi.d.src), (const float*)out_f32(net, lv.d.src), net->params + lpi.w_off,
               net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off, log_std, E, lpi.K, adim, seed, offset_dev, t,
               a_t, lp_t, v_o, pi_out);
-    } else if constexpr (DIST::kLogStd) {
-      XLAUNCH(gauss_sample_kernel, (E + 127) / 128, 128, 0, S(stream), pi_out, log_std, E, adim, (const float*)nullptr, seed,
-              (uint64_t)0, offset_dev, t, a_t, lp_t, v_in, v_o);
     } else {
-      XLAUNCH(sample_kernel, (E + 127) / 128, 128, 0, S(stream), pi_out, E, adim, (const float*)nullptr, seed, (uint64_t)0,
-              offset_dev, t, a_t, lp_t, v_in, v_o);
+      XLAUNCH(sample_kernel<DIST>, (E + 127) / 128, 128, 0, S(stream), pi_out, log_std, E, adim, (const float*)nullptr, seed,
+              (uint64_t)0, offset_dev, t, a_t, lp_t, v_in, v_o);
     }
     LAUNCH_CHECK();
   }
