@@ -40,10 +40,10 @@ def build(model_name, state_dim, A, L, batch, n_traj):
         from xingtian_b200.capi import ImpalaTraj, check
         from xingtian_b200.engine import _ptr, stream_ptr
         m, st, net = alg.actor, alg._store, alg.actor.net
-        tr = ImpalaTraj(_ptr(st["obs"]), _ptr(st["behav"]), _ptr(st["amat"]), _ptr(st["reward"]), _ptr(st["done"]))
-        check(net.lib.xtb_impala_keras_train(net.handle, m.opt.handle, tr, n_traj, L, batch, 128, _ptr(st["order"]),
-                                             _ptr(st["obs_idx"]), float(mod.GAMMA), float(m.ent_coef), net.tid[m.logit_name],
-                                             net.tid[m.value_name], _ptr(st["pg_adv"]), _ptr(st["tv"]), _ptr(st["loss"]),
+        tr = ImpalaTraj(_ptr(st.obs), _ptr(st.behav), _ptr(st.amat), _ptr(st.reward), _ptr(st.done))
+        check(net.lib.xtb_impala_keras_train(net.handle, m.opt.handle, tr, n_traj, L, batch, 128, _ptr(st.order),
+                                             _ptr(st.obs_idx), float(mod.GAMMA), float(m.ent_coef), net.tid[m.logit_name],
+                                             net.tid[m.value_name], _ptr(st.pg_adv), _ptr(st.tv), _ptr(st.loss),
                                              1 if graph else 0, stream_ptr()))
     return step
 

@@ -50,10 +50,11 @@ def make_trajs(E, T, seed, state_dim=(84, 84, 4), A=4, dtype=np.uint8):
     return trajs
 
 
-@pytest.mark.parametrize("raw", [False, True])
+@pytest.mark.parametrize("raw", [False, True, "mixed"])
 def test_ppo_cnn_train_matches_oracle(raw):
     """a8-a11 end to end: E trajectories -> prepare_data xE -> train(): per-step loss trace and final
-    weights vs the oracle PpoLearner under the same np.random shuffle stream (ragged last minibatch)."""
+    weights vs the oracle PpoLearner under the same np.random shuffle stream (ragged last minibatch).  "mixed" sends
+    every second trajectory raw, so device GAE runs per trajectory and its buffers grow past rows they never held."""
     import xingtian_b200 as xb
     E, T = 4, 16
     info = ppo_cnn_info(batch=24, iters=2)
@@ -66,8 +67,8 @@ def test_ppo_cnn_train_matches_oracle(raw):
     ref = orc.PpoLearner(arch, w0, lr=0.00025, batch_size=24, critic_coef=1.0, ent_coef=0.003, clip_ratio=0.1,
                          max_grad_norm=5.0, num_sgd_iter=2, vf_clip=5.0)
     trajs = make_trajs(E, T, seed=3)
-    for tr in trajs:
-        if raw:   # learner-side GAE on the device
+    for i, tr in enumerate(trajs):
+        if raw is True or (raw == "mixed" and i % 2):   # learner-side GAE on the device
             alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "value", "reward", "done")})
         else:     # reference message format (host GAE)
             alg.prepare_data({k: tr[k] for k in ("cur_state", "action", "logp", "adv", "old_value", "target_value")})
@@ -75,6 +76,9 @@ def test_ppo_cnn_train_matches_oracle(raw):
     loss = alg.train()
     np.random.seed(123)
     cat = lambda k: np.concatenate([t[k] for t in trajs])
+    ro = alg.actor.rollout
+    for key, ref_key in (("adv", "adv"), ("old_v", "old_value"), ("target_v", "target_value")):
+        assert rel_err(getattr(ro, key)[:E * T].cpu().numpy(), cat(ref_key).reshape(-1)) < 1e-4, key
     ref_loss, ref_trace = ref.train([cat("cur_state")], [cat("action"), cat("logp"), cat("adv").astype(np.float32),
                                                           cat("old_value"), cat("target_value").astype(np.float32)])
     trace = alg.actor.last_losses

@@ -225,3 +225,28 @@ def test_impala_lr_schedule_matches_linear_cosine_decay():
         want = orc.linear_cosine_decay(0.001, step, 20000.0, beta=0.000002 / 20000.0)
         assert abs(ImpalaCnnOpt.scheduled_lr(Stub(), step) - want) < 1e-15, step
     assert ImpalaCnnOpt.scheduled_lr(Stub(), 0) > ImpalaCnnOpt.scheduled_lr(Stub(), 10000) > ImpalaCnnOpt.scheduled_lr(Stub(), 20000)
+
+
+def test_device_store_grows_and_keeps_the_valid_rows():
+    """engine.DeviceStore on the CPU: a growth doubles the capacity (or takes the rows asked for), keeps the first n rows
+    of every field, and the arrays keep their addresses until the next growth; n past the capacity is an error."""
+    import torch
+    from xingtian_b200.engine import DeviceStore
+    st = DeviceStore(torch.device("cpu"), x=((3,), torch.float32), k=((), torch.int32))
+    st.reserve(5)
+    assert st.capacity == 5 and st.x.shape == (5, 3) and st.k.shape == (5,)
+    st.x[:4] = torch.arange(12, dtype=torch.float32).view(4, 3)
+    st.k[:4] = torch.arange(4, dtype=torch.int32)
+    st.n = 4
+    ptrs = (st.x.data_ptr(), st.k.data_ptr())
+    st.reserve(5)
+    assert (st.x.data_ptr(), st.k.data_ptr()) == ptrs
+    st.reserve(6)
+    assert st.capacity == 10
+    assert torch.equal(st.x[:4], torch.arange(12, dtype=torch.float32).view(4, 3))
+    assert torch.equal(st.k[:4], torch.arange(4, dtype=torch.int32))
+    st.reserve(25)
+    assert st.capacity == 25 and torch.equal(st.k[:4], torch.arange(4, dtype=torch.int32))
+    st.n = 26
+    with pytest.raises(ValueError, match="marked valid"):
+        st.reserve(30)

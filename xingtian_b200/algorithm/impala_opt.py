@@ -4,7 +4,7 @@ import os
 import numpy as np
 import torch
 
-from ..engine import stage_h2d
+from ..engine import DeviceStore, stage_h2d
 from ..registry import Registers, import_config
 from .base import Algorithm, FIFODistPolicy
 
@@ -19,7 +19,12 @@ class IMPALAOpt(Algorithm):
     def __init__(self, model_info, alg_config, **kwargs):
         import_config(globals(), alg_config)
         super().__init__(alg_name="impala", model_info=model_info["actor"], alg_config=alg_config)
-        self._store, self._count, self._losses, self._tmp = None, 0, None, None
+        m = self.actor
+        # grow-only device trajectory store: its addresses stay put between iterations, so the captured train-step graphs
+        # (keyed by their buffers) are replayed instead of re-captured
+        self._store = DeviceStore(m.device, obs=(tuple(m.state_dim), torch.uint8), bp=((m.action_dim,), torch.float32),
+                                  action=((), torch.int32), done=((), torch.uint8), reward=((), torch.float32))
+        self._losses, self._tmp = None, None
         self.async_flag = False
         self.dist_model_policy = FIFODistPolicy(alg_config["instance_num"], prepare_times=self._prepare_times_per_train)
 
@@ -33,42 +38,24 @@ class IMPALAOpt(Algorithm):
         rewards = np.asarray(episode_data["reward"])
         return states, behavior_logits, actions, dones, rewards
 
-    def _reserve(self, n):
-        """Grow-only device trajectory store (addresses stay put between iterations, so the captured train-step graphs --
-        keyed by their buffers -- are replayed instead of re-captured)."""
-        st = self._store
-        if st is not None and st["obs"].shape[0] >= n:
-            return st
-        cap = max(n, 2 * (st["obs"].shape[0] if st else 0))
-        dev = self.actor.device
-        new = dict(obs=torch.empty((cap,) + tuple(self.actor.state_dim), dtype=torch.uint8, device=dev),
-                   bp=torch.empty(cap, self.actor.action_dim, dtype=torch.float32, device=dev),
-                   action=torch.empty(cap, dtype=torch.int32, device=dev), done=torch.empty(cap, dtype=torch.uint8, device=dev),
-                   reward=torch.empty(cap, dtype=torch.float32, device=dev))
-        if st is not None and self._count:
-            for k in new:
-                new[k][:self._count].copy_(st[k][:self._count])
-        self._store = new
-        return new
-
     def prepare_data(self, train_data, **kwargs):
         """impala_opt.py:110-117 -- staged straight into the device store (pinned ring, asynchronous)."""
         state, logit, action, done, reward = self._data_proc(train_data)
-        n = len(state)
-        st = self._reserve(self._count + n)
-        sl = slice(self._count, self._count + n)
-        stage_h2d(st["obs"][sl], state, np.uint8)
-        stage_h2d(st["bp"][sl], logit, np.float32)
-        stage_h2d(st["action"][sl], np.asarray(action).reshape(-1), np.int32)
-        stage_h2d(st["done"][sl], np.ascontiguousarray(done, np.bool_).reshape(-1).view(np.uint8), np.uint8)
-        stage_h2d(st["reward"][sl], np.asarray(reward).reshape(-1), np.float32)
-        self._count += n
+        n, st = len(state), self._store
+        st.reserve(st.n + n)
+        sl = slice(st.n, st.n + n)
+        stage_h2d(st.obs[sl], state, np.uint8)
+        stage_h2d(st.bp[sl], logit, np.float32)
+        stage_h2d(st.action[sl], np.asarray(action).reshape(-1), np.int32)
+        stage_h2d(st.done[sl], np.ascontiguousarray(done, np.bool_).reshape(-1).view(np.uint8), np.uint8)
+        stage_h2d(st.reward[sl], np.asarray(reward).reshape(-1), np.float32)
+        st.n += n
 
     def train(self, **kwargs):
         """impala_opt.py:73-106: concatenate, slice by BATCH_SIZE, one SGD step per slice, mean loss."""
-        if self._count == 0:
+        cat, nbatch = self._store, self._store.n
+        if nbatch == 0:
             raise ValueError("need at least one array to concatenate")
-        cat, nbatch = self._store, self._count
         count = (nbatch + BATCH_SIZE - 1) // BATCH_SIZE
         if self._losses is None or self._losses.numel() < count:
             self._losses = torch.zeros(count, dtype=torch.float32, device=self.actor.device)
@@ -76,10 +63,9 @@ class IMPALAOpt(Algorithm):
         losses, tmp = self._losses[:count], self._tmp
         for i in range(count):
             s, e = i * BATCH_SIZE, min(nbatch, (i + 1) * BATCH_SIZE)
-            self.actor.train_device(cat["obs"][s:e], cat["bp"][s:e], cat["action"][s:e], cat["done"][s:e],
-                                    cat["reward"][s:e], e - s, tmp)
+            self.actor.train_device(cat.obs[s:e], cat.bp[s:e], cat.action[s:e], cat.done[s:e], cat.reward[s:e], e - s, tmp)
             losses[i:i + 1].copy_(tmp)
-        self._count = 0
+        cat.n = 0
         return float(losses.mean().cpu())
 
     def save(self, model_path, model_index):

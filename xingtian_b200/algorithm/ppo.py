@@ -1,12 +1,11 @@
 """PPO algorithm on the device rollout store (xt/algorithm/ppo/ppo.py:30-95)."""
-import ctypes as C
 import logging
 
 import numpy as np
 import torch
 
 from ..capi import check
-from ..engine import _ptr, stream_ptr
+from ..engine import DeviceStore, _ptr, stage_h2d, stream_ptr
 from ..registry import Registers, import_config
 from .base import Algorithm
 
@@ -25,6 +24,10 @@ class PPO(Algorithm):
     def __init__(self, model_info, alg_config, **kwargs):
         import_config(globals(), alg_config)
         super().__init__(alg_name=kwargs.get("name") or "ppo", model_info=model_info["actor"], alg_config=alg_config)
+        # raw trajectories: reward / done at their rollout rows, value[T+1] per trajectory back to back
+        dev = self.actor.device
+        self._raw_steps = DeviceStore(dev, rew=((), torch.float32), don=((), torch.uint8))
+        self._raw_values = DeviceStore(dev, val=((), torch.float32))
         self._init_train_list()
         self.async_flag = False
         self.sign_clip_reward = bool(alg_config.get("sign_clip_reward", False))
@@ -35,19 +38,11 @@ class PPO(Algorithm):
     def _init_train_list(self):
         self._count = 0           # samples staged so far
         self._raw_segments = []   # (offset, length, value offset) of trajectories that still need device GAE
-        if not hasattr(self, "_raw"):
-            self._raw = None      # device buffers of raw trajectories (kept across iterations)
+        # valid rows of the raw stores: up to the end of the last raw trajectory (rows of trajectories that came with their
+        # advantages are gaps, so the rollout's row count can be past the stores' capacity)
+        self._raw_steps.n = self._raw_values.n = 0
 
     # -- data path ---------------------------------------------------------------------------
-    def _stage(self, dst, arr, np_dtype):
-        """Copy one host (pageable) array into device tensor `dst` through the library's staged copy: worker
-        threads memcpy chunks into a pinned ring while the DMA of earlier chunks is in flight
-        (`xtb_copy_h2d_staged`); the source may be reused as soon as the call returns."""
-        a = np.ascontiguousarray(arr, dtype=np_dtype).reshape(dst.shape)
-        if not dst.is_contiguous():
-            raise ValueError("staging target must be contiguous")
-        check(self.actor.net.lib.xtb_copy_h2d_staged(_ptr(dst), a.ctypes.data, a.nbytes, stream_ptr()))
-
     def prepare_data(self, train_data, **kwargs):
         """`ring_rows` = (env_index, first_step, n_steps) instead of `cur_state`: the trajectory's frames are the ones the
         learner-side batched predict() already uploaded (model.keep_predict_obs); they are copied device to device."""
@@ -57,7 +52,6 @@ class PPO(Algorithm):
         ro.n = self._count
         ro.reserve(self._count + n)
         sl = slice(self._count, self._count + n)
-        obs_np = np.uint8 if self.actor.input_dtype == "uint8" else np.float32
         if ring_rows is not None:
             ring = self.actor._obs_ring
             e, t0 = int(ring_rows[0]), int(ring_rows[1]) % ring["T"]
@@ -65,42 +59,29 @@ class PPO(Algorithm):
                 raise ValueError("trajectory wraps around the observation ring")
             ro.obs[sl].copy_(ring["obs"][t0:t0 + n, e], non_blocking=True)
         else:
-            self._stage(ro.obs[sl], np.asarray(train_data["cur_state"]), obs_np)
+            stage_h2d(ro.obs[sl], np.asarray(train_data["cur_state"]), self.actor._np_dt)
         # int32 [n] actions, or float32 [n, A] for a DiagGaussian actor
-        self._stage(ro.action[sl], train_data["action"], np.float32 if ro.action.dim() == 2 else np.int32)
-        self._stage(ro.old_logp[sl], train_data["logp"], np.float32)
+        stage_h2d(ro.action[sl], train_data["action"], np.float32 if ro.action.dim() == 2 else np.int32)
+        stage_h2d(ro.old_logp[sl], train_data["logp"], np.float32)
         if "adv" in train_data:
-            self._stage(ro.adv[sl], train_data["adv"], np.float32)
-            self._stage(ro.old_v[sl], train_data["old_value"], np.float32)
-            self._stage(ro.target_v[sl], train_data["target_value"], np.float32)
+            stage_h2d(ro.adv[sl], train_data["adv"], np.float32)
+            stage_h2d(ro.old_v[sl], train_data["old_value"], np.float32)
+            stage_h2d(ro.target_v[sl], train_data["target_value"], np.float32)
         else:
             value = np.ascontiguousarray(train_data["value"], np.float32).reshape(-1)
             if value.size != n + 1:
                 raise ValueError("raw trajectory needs value[T+1] (bootstrap appended), got %d for T=%d" % (value.size, n))
-            raw = self._raw_store(self._count + n, len(self._raw_segments) + 1)
+            steps, values = self._raw_steps, self._raw_values
             voff = self._count + len(self._raw_segments)          # every earlier raw trajectory holds one bootstrap value more
-            self._stage(raw["val"][voff:voff + n + 1], value, np.float32)     # staged (asynchronous): no host sync per trajectory
-            self._stage(raw["rew"][sl], np.asarray(train_data["reward"]).reshape(-1), np.float32)
-            self._stage(raw["don"][sl], np.asarray(train_data["done"]).reshape(-1).astype(np.bool_, copy=False).view(np.uint8), np.uint8)
+            steps.reserve(self._count + n)
+            values.reserve(voff + n + 1)
+            stage_h2d(values.val[voff:voff + n + 1], value, np.float32)     # staged (asynchronous): no host sync per trajectory
+            stage_h2d(steps.rew[sl], np.asarray(train_data["reward"]).reshape(-1), np.float32)
+            stage_h2d(steps.don[sl], np.asarray(train_data["done"]).reshape(-1).astype(np.bool_, copy=False).view(np.uint8), np.uint8)
+            steps.n, values.n = self._count + n, voff + n + 1
             self._raw_segments.append((self._count, n, voff))
         self._count += n
         ro.n = self._count
-
-    def _raw_store(self, n, n_traj):
-        """Grow-only device buffers of the raw trajectories (value[T+1] per trajectory back to back, reward, done)."""
-        raw = self._raw
-        if raw is not None and raw["rew"].numel() >= n and raw["val"].numel() >= n + n_traj:
-            return raw
-        dev = self.actor.rollout.obs.device
-        cap = max(n, 2 * (raw["rew"].numel() if raw else 0))
-        cap_t = max(n_traj, 2 * ((raw["val"].numel() - raw["rew"].numel()) if raw else 0), 64)
-        new = dict(val=torch.empty(cap + cap_t, dtype=torch.float32, device=dev), rew=torch.empty(cap, dtype=torch.float32, device=dev),
-                   don=torch.empty(cap, dtype=torch.uint8, device=dev))
-        if raw is not None:
-            for k in new:
-                new[k][:raw[k].numel()].copy_(raw[k])
-        self._raw = new
-        return new
 
     def _device_gae(self):
         """GAE of the raw trajectories on the device: one launch over [E, T] when they are equally long and adjacent (the
@@ -110,12 +91,12 @@ class PPO(Algorithm):
         segs = self._raw_segments
         if not segs:
             return
-        raw = self._raw
+        steps, values = self._raw_steps, self._raw_values
         same = len({s[1] for s in segs}) == 1 and all(segs[i][0] + segs[i][1] == segs[i + 1][0] and segs[i][2] + segs[i][1] + 1 == segs[i + 1][2]
                                                       for i in range(len(segs) - 1))
         groups = [(segs[0][0], segs[0][1], segs[0][2], len(segs))] if same else [(o, t, v, 1) for o, t, v in segs]
         for off, t, voff, count in groups:
-            check(lib.xtb_gae(_ptr(raw["val"][voff:]), _ptr(raw["rew"][off:]), _ptr(raw["don"][off:]), count, t, GAMMA, LAM,
+            check(lib.xtb_gae(_ptr(values.val[voff:]), _ptr(steps.rew[off:]), _ptr(steps.don[off:]), count, t, GAMMA, LAM,
                               int(self.sign_clip_reward), _ptr(ro.adv[off:]), _ptr(ro.old_v[off:]), _ptr(ro.target_v[off:]), stream_ptr()))
         self._raw_segments = []
 

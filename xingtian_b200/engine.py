@@ -29,6 +29,33 @@ def stage_h2d(dst, arr, np_dtype):
     capi.check(capi.lib().xtb_copy_h2d_staged(_ptr(dst), a.ctypes.data, a.nbytes, stream_ptr()))
 
 
+class DeviceStore(object):
+    """Grow-only named device arrays: field `name` is [capacity, *row_shape] of its dtype, an attribute of the store.
+    The arrays keep their addresses until the next growth, so the CUDA graphs captured on them are replayed instead of
+    re-captured.  `n` is the number of valid rows, the ones a growth keeps."""
+
+    def __init__(self, device, **fields):
+        self.device, self.fields = device, fields    # name -> (row shape, torch dtype)
+        self.capacity = self.n = 0
+        for name in fields:
+            setattr(self, name, None)
+
+    def reserve(self, rows):
+        """Make room for `rows` rows: a growth reallocates every array to max(rows, 2 x capacity) rows and copies the
+        first `n` rows over."""
+        if self.n > self.capacity:
+            raise ValueError("store holds %d rows but %d are marked valid" % (self.capacity, self.n))
+        if rows <= self.capacity:
+            return
+        cap = max(int(rows), 2 * self.capacity)
+        for name, (shape, dtype) in self.fields.items():
+            new = torch.empty((cap,) + tuple(shape), dtype=dtype, device=self.device)
+            if self.n:
+                new[:self.n].copy_(getattr(self, name)[:self.n])
+            setattr(self, name, new)
+        self.capacity = cap
+
+
 def require_cuda():
     if not torch.cuda.is_available():
         raise RuntimeError("xingtian_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
@@ -264,6 +291,13 @@ class Adam(object):
         with torch.cuda.device(net.device):
             check(self.lib.xtb_adam_create(net.n_params, lr, beta1, beta2, eps, clip_mode, clip, seg,
                                            len(offs) - 1, _ptr(self.m), _ptr(self.v), C.byref(self.handle)))
+
+    @classmethod
+    def keras(cls, net, lr, clipnorm=None):
+        """keras.optimizers.Adam(lr, clipnorm): epsilon = K.epsilon() = 1e-7, each gradient tensor clipped to norm
+        `clipnorm` on its own (no clipping without one)."""
+        mode = capi.CLIP_PER_TENSOR if clipnorm else capi.CLIP_NONE
+        return cls(net, lr, eps=1e-7, clip_mode=mode, clip=float(clipnorm or 0.0))
 
     def __del__(self):
         try:

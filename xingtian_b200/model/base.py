@@ -38,6 +38,11 @@ class XTModel(object):
 
     def __init__(self, model_info):
         require_cuda()
+        model_config = model_info.get("model_config") or {}
+        seed = model_config.get("init_seed")
+        # the generator every initial weight is drawn from (not the global np.random stream)
+        self._init_rng = np.random.default_rng(seed) if seed is not None else np.random.default_rng()
+        self.use_graph = bool(model_config.get("use_cuda_graph", True))
         self.actor_var = None
         self._summary = model_info.get("summary", False)
         self.model_format = model_info.get("model_format")
@@ -59,6 +64,15 @@ class XTModel(object):
 
     def create_model(self, model_info):
         raise NotImplementedError
+
+    def seeded_net(self, arch, max_batch):
+        """A Net of `arch` with glorot_uniform_ weights from the model's init generator; the observations the model
+        takes (`_obs_dt` on the device, `_np_dt` on the host) are the arch's input dtype."""
+        net = Net(arch, max_batch=max_batch, device=self.device)
+        glorot_uniform_(net, self._init_rng)
+        u8 = arch["input_dtype"] == "uint8"
+        self._obs_dt, self._np_dt = (torch.uint8, np.uint8) if u8 else (torch.float32, np.float32)
+        return net
 
     def predict(self, state):
         raise NotImplementedError
@@ -134,6 +148,20 @@ class PolicyActor(object):
                                                 io["out_dev_ptr"], io["pin_out_ptr"], _ptr(io["pin_head"]),
                                                 1 if self.use_graph else 0, stream_ptr()))
         return io
+
+    def _draw(self, batch, action, logp, noise=None):
+        """Sample `batch` actions from the pi head of the last forward into the device tensors action / logp: Categorical
+        logits, or with ls_t the DiagGaussian mean and the pi_logstd weights.  `noise` (device [batch, A]: uniforms, or
+        normals for a DiagGaussian) replaces the Philox draws of (seed, `_sample_offset`); the host counter advances once."""
+        net = self.net
+        pi, seed, off = _ptr(net.tensor(net.names[self.pi_t])), C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset)
+        if self.ls_t:
+            check(net.lib.xtb_diag_gaussian_sample(pi, _ptr(net.view(net.names[self.ls_t])), batch, self.action_dim, _ptr(noise),
+                                                   seed, off, _ptr(action), _ptr(logp), stream_ptr()))
+        else:
+            check(net.lib.xtb_categorical_sample(pi, batch, self.action_dim, _ptr(noise), seed, off, _ptr(action), _ptr(logp),
+                                                 stream_ptr()))
+        self._sample_offset += 1
 
     def rollout_infer_device(self, obs_dev, step_idx, n_env, n_step, action, logp, value):
         """n_step batched policy evaluations on device-resident observations as ONE CUDA graph (the learner-side

@@ -2,12 +2,11 @@
 import numpy as np
 import torch
 
-from .. import capi
 from ..capi import check
-from ..engine import Adam, Net, _ptr, stream_ptr
+from ..engine import Adam, _ptr, stream_ptr
 from ..registry import Registers, import_config
 from . import archs
-from .base import XTModel, glorot_uniform_
+from .base import XTModel
 
 # xt/model/dqn/default_config.py
 HIDDEN_SIZE = 128
@@ -25,8 +24,6 @@ class _DqnBase(XTModel):
         self.action_dim = model_info["action_dim"]
         self.learning_rate = LR
         self.dueling = bool(model_config.get("dueling", False))
-        self._init_seed = model_config.get("init_seed")
-        self.use_graph = bool(model_config.get("use_cuda_graph", True))
         super().__init__(model_info)
 
     def build_arch(self):
@@ -35,15 +32,9 @@ class _DqnBase(XTModel):
     def create_model(self, model_info):
         arch = self.build_arch()
         self.arch = arch
-        self.net = Net(arch, max_batch=int(model_info.get("max_batch", 512)), device=self.device)
-        rng = np.random.default_rng(self._init_seed) if self._init_seed is not None else np.random.default_rng()
-        glorot_uniform_(self.net, rng)
-        mode = capi.CLIP_PER_TENSOR if self.clipnorm else capi.CLIP_NONE
-        # keras Adam: epsilon = K.epsilon() = 1e-7
-        self.opt = Adam(self.net, self.learning_rate, eps=1e-7, clip_mode=mode, clip=float(self.clipnorm or 0.0))
+        self.net = self.seeded_net(arch, int(model_info.get("max_batch", 512)))
+        self.opt = Adam.keras(self.net, self.learning_rate, self.clipnorm)
         self.q_name = arch["outputs"][0]   # the dueling combine layer when model_config has dueling: True
-        self._obs_dt = torch.uint8 if arch["input_dtype"] == "uint8" else torch.float32
-        self._np_dt = np.uint8 if arch["input_dtype"] == "uint8" else np.float32
         self._bufs = {}
         return self.net
 

@@ -1,15 +1,13 @@
 """ImpalaCnnOpt on the CUDA engine (xt/model/impala/impala_cnn_opt.py:64-297)."""
-import ctypes as C
-
 import numpy as np
 import torch
 
 from .. import capi
 from ..capi import check
-from ..engine import Adam, Net, _ptr, stream_ptr
+from ..engine import Adam, _ptr, stream_ptr
 from ..registry import Registers, import_config
 from . import archs
-from .base import PolicyActor, XTModel, glorot_uniform_
+from .base import PolicyActor, XTModel
 
 # xt/model/impala/default_config.py
 LR = 0.0003
@@ -36,8 +34,6 @@ class ImpalaCnnOpt(XTModel, PolicyActor):
         self.lr = LR
         self.grad_norm_clip = model_config.get("grad_norm_clip", 40.0)
         self.sample_batch_steps = model_config.get("sample_batch_step", 50)
-        self._init_seed = model_config.get("init_seed")
-        self.use_graph = bool(model_config.get("use_cuda_graph", True))
         if self.opt_type not in ("adam", "rmsprop"):
             raise KeyError("invalid opt_type: {}".format(self.opt_type))          # impala_cnn_opt.py:207-208
         if self.lr_schedule and len(self.lr_schedule) != 2:
@@ -51,13 +47,11 @@ class ImpalaCnnOpt(XTModel, PolicyActor):
         arch = archs.impala_cnn(self.state_dim, self.action_dim)
         arch["scale"] = 1.0 / float(self.sta_std)
         self.arch = arch
-        self.net = Net(arch, max_batch=int(model_info.get("max_batch", 512)), device=self.device)
-        rng = np.random.default_rng(self._init_seed) if self._init_seed is not None else np.random.default_rng()
-        glorot_uniform_(self.net, rng)
+        self.net = self.seeded_net(arch, int(model_info.get("max_batch", 512)))
         # baseline head: custom_norm_initializer(0.01) (model_utils.py:204-211, impala_cnn_opt.py:146)
         name = "explore_agent/dense/kernel"
         shape = self.net.ptable[name][1]
-        o = rng.standard_normal(shape).astype(np.float32)
+        o = self._init_rng.standard_normal(shape).astype(np.float32)
         o *= 0.01 / np.sqrt(np.square(o).sum(axis=0, keepdims=True))
         self.net.view(name).copy_(torch.from_numpy(o))
         self.net.params_changed()
@@ -66,7 +60,6 @@ class ImpalaCnnOpt(XTModel, PolicyActor):
             self.opt.use_rmsprop(decay=0.99, epsilon=0.1)          # impala_cnn_opt.py:205-206 (the schedule is Adam-only there)
         self._global_step = 0
         self._bufs = {}
-        self._obs_dt = torch.uint8
         self._init_sampling()
         self.logit_name, self.base_name = arch["outputs"]
         self.pi_t, self.v_t, self.ls_t = self.net.tid[self.logit_name], self.net.tid[self.base_name], 0
@@ -143,10 +136,7 @@ class ImpalaCnnOpt(XTModel, PolicyActor):
         u = None
         if uniforms is not None:
             u = torch.from_numpy(np.ascontiguousarray(uniforms, np.float32)).to(self.device)
-        check(net.lib.xtb_categorical_sample(_ptr(net.tensor(self.logit_name)), n, self.action_dim, _ptr(u),
-                                             C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset),
-                                             _ptr(b["action"]), _ptr(b["logp"]), stream_ptr()))
-        self._sample_offset += 1
+        self._draw(n, b["action"], b["logp"], u)
         logits = net.tensor(self.logit_name)[:n].cpu().numpy()
         base = net.tensor(self.base_name)[:n, 0].cpu().numpy()
         return [logits, base, b["action"].cpu().numpy()]

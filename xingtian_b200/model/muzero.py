@@ -74,8 +74,6 @@ class MuzeroModel(XTModel):
         self.td_step = int(td_step)
         self.learning_rate = LR
         self.max_batch = int(model_config.get("max_batch", 1024))
-        self._init_seed = model_config.get("init_seed")
-        self.use_graph = bool(model_config.get("use_cuda_graph", True))
         super().__init__(model_info)
 
     def build_archs(self):
@@ -105,9 +103,8 @@ class MuzeroModel(XTModel):
         for n, off in zip(nets, offs):
             g = self._dyn_grads if n is self.dyn else self.grads[off:off + n.n_params]
             n.bind_to(self.params[off:off + n.n_params], g)
-        rng = np.random.default_rng(self._init_seed) if self._init_seed is not None else np.random.default_rng()
         for n in nets:
-            glorot_uniform_(n, rng)
+            glorot_uniform_(n, self._init_rng)
         # the l2 term of build_train_graph is taken of get_weights() arrays: a constant of the initial weights, no gradient
         self.weight_decay_loss = float(WEIGHT_DECAY * sum(0.5 * np.sum(np.square(w, dtype=np.float64)) for w in self.get_weights()))
         flat = SimpleNamespace(params=self.params, n_params=self.n_params, device=self.device,

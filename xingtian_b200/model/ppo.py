@@ -6,10 +6,10 @@ import torch
 
 from .. import capi
 from ..capi import check
-from ..engine import Adam, Net, _ptr, stream_ptr
+from ..engine import Adam, DeviceStore, _ptr, stream_ptr
 from ..registry import Registers, import_config
 from . import archs
-from .base import PolicyActor, XTModel, glorot_uniform_
+from .base import PolicyActor, XTModel
 
 # xt/model/ppo/default_config.py:1-12
 BATCH_SIZE = 200
@@ -39,39 +39,15 @@ def minibatch_order(nbatch, num_sgd_iter):
     return out
 
 
-class DeviceRollout(object):
+class DeviceRollout(DeviceStore):
     """Device-resident PPO rollout (grow-only, so CUDA-graph pointers stay valid).  With `action_dim` (a DiagGaussian
     actor) the behaviour actions are float32 [N, action_dim], else int32 [N]."""
 
-    FIELDS = (("action", torch.int32), ("old_logp", torch.float32), ("adv", torch.float32),
-              ("old_v", torch.float32), ("target_v", torch.float32))
-
     def __init__(self, state_dim, obs_dtype, device, action_dim=None):
-        self.state_dim, self.obs_dtype, self.device = tuple(state_dim), obs_dtype, device
-        self.action_dim = action_dim
-        self.capacity = 0
-        self.obs = None
-        self.n = 0
-
-    def _field(self, key, dt, cap):
-        if key == "action" and self.action_dim is not None:
-            return torch.empty((cap, self.action_dim), dtype=torch.float32, device=self.device)
-        return torch.empty(cap, dtype=dt, device=self.device)
-
-    def reserve(self, n):
-        if n <= self.capacity:
-            return
-        cap = max(n, int(self.capacity * 1.5))
-        obs = torch.empty((cap,) + self.state_dim, dtype=self.obs_dtype, device=self.device)
-        new = {k: self._field(k, dt, cap) for k, dt in self.FIELDS}
-        if self.n:
-            obs[:self.n].copy_(self.obs[:self.n])
-            for k, _ in self.FIELDS:
-                new[k][:self.n].copy_(getattr(self, k)[:self.n])
-        self.obs = obs
-        for k, _ in self.FIELDS:
-            setattr(self, k, new[k])
-        self.capacity = cap
+        f32 = ((), torch.float32)
+        super().__init__(device, obs=(tuple(state_dim), obs_dtype),
+                         action=((), torch.int32) if action_dim is None else ((action_dim,), torch.float32),
+                         old_logp=f32, adv=f32, old_v=f32, target_v=f32)
 
     def as_struct(self):
         return capi.PpoRollout(self.obs.data_ptr(), self.action.data_ptr(), self.old_logp.data_ptr(),
@@ -98,8 +74,6 @@ class PPO(XTModel, PolicyActor):
         self.num_sgd_iter = model_config.get("NUM_SGD_ITER", NUM_SGD_ITER)
         self.verbose = model_config.get("SUMMARY", SUMMARY)
         self.vf_clip = model_config.get("VF_CLIP", VF_CLIP)
-        self.use_graph = bool(model_config.get("use_cuda_graph", True))
-        self._init_seed = model_config.get("init_seed")
         if self.action_type not in ("Categorical", "DiagGaussian"):
             raise NotImplementedError(
                 "action type: {} not match any implemented distributions.".format(self.action_type))
@@ -114,15 +88,10 @@ class PPO(XTModel, PolicyActor):
     def create_model(self, model_info):
         arch = self.build_arch()
         self.arch = arch
-        self.net = Net(arch, max_batch=max(int(self._batch_size), int(model_info.get("max_predict_batch", 1024))),
-                       device=self.device)
-        rng = np.random.default_rng(self._init_seed) if self._init_seed is not None else np.random.default_rng()
-        glorot_uniform_(self.net, rng)
+        self.net = self.seeded_net(arch, max(int(self._batch_size), int(model_info.get("max_predict_batch", 1024))))
         self.opt = Adam(self.net, self._lr, eps=1e-8, clip_mode=capi.CLIP_GLOBAL_NORM, clip=self._max_grad_norm)
         self.hyper = capi.PpoHyper(self.clip_ratio, self.ent_coef, self.vf_clip, self.critic_loss_coef)
-        obs_dt = torch.uint8 if self.input_dtype == "uint8" else torch.float32
-        self.rollout = DeviceRollout(self.state_dim, obs_dt, self.device, self.action_dim if self.gaussian else None)
-        self._obs_dt = obs_dt
+        self.rollout = DeviceRollout(self.state_dim, self._obs_dt, self.device, self.action_dim if self.gaussian else None)
         self._perm_dev = None
         self._perm_host = None
         self._loss_dev = None
@@ -155,6 +124,7 @@ class PPO(XTModel, PolicyActor):
         bufs = self._pred_buffers(batch) if out_action is None else None
         action = out_action if out_action is not None else bufs["action"]
         logp = out_logp if out_logp is not None else bufs["logp"]
+        noise = normals if self.gaussian else uniforms
         vout = torch.empty(batch, 1, dtype=torch.float32, device=self.device) if batch > net.max_batch else None
         while done < batch:
             mb = min(net.max_batch, batch - done)
@@ -162,18 +132,7 @@ class PPO(XTModel, PolicyActor):
                 net.forward(obs_dev[done:done + mb], mb)
             else:
                 net.forward(obs_dev, mb, idx=idx[done:done + mb])
-            if self.gaussian:
-                n = None if normals is None else normals[done:done + mb]
-                check(net.lib.xtb_diag_gaussian_sample(_ptr(net.tensor("pi_latent")), _ptr(net.view("pi_logstd")), mb,
-                                                       self.action_dim, _ptr(n), C.c_uint64(self._sample_seed),
-                                                       C.c_uint64(self._sample_offset), _ptr(action[done:done + mb]),
-                                                       _ptr(logp[done:done + mb]), stream_ptr()))
-            else:
-                u = None if uniforms is None else uniforms[done:done + mb]
-                check(net.lib.xtb_categorical_sample(_ptr(net.tensor("pi_latent")), mb, self.action_dim, _ptr(u),
-                                                     C.c_uint64(self._sample_seed), C.c_uint64(self._sample_offset),
-                                                     _ptr(action[done:done + mb]), _ptr(logp[done:done + mb]), stream_ptr()))
-            self._sample_offset += 1
+            self._draw(mb, action[done:done + mb], logp[done:done + mb], None if noise is None else noise[done:done + mb])
             if vout is not None:
                 vout[done:done + mb].copy_(net.tensor("output_value")[:mb])
             done += mb
@@ -183,7 +142,7 @@ class PPO(XTModel, PolicyActor):
     def predict(self, state, uniforms=None, normals=None):
         """xt/model/ppo/ppo.py:104-109: (action [B] int32, logp [B,1], v [B,1]); a DiagGaussian actor returns action
         [B, A] float32 (`normals` [B, A] then replaces the Philox draws)."""
-        state = np.ascontiguousarray(state, dtype=np.uint8 if self.input_dtype == "uint8" else np.float32)
+        state = np.ascontiguousarray(state, dtype=self._np_dt)
         batch = state.shape[0]
         noise = normals if self.gaussian else uniforms
         if noise is not None or batch > self.net.max_batch:
@@ -245,7 +204,7 @@ class PPO(XTModel, PolicyActor):
         ro = self.rollout
         ro.n = 0
         ro.reserve(nbatch)
-        np_obs = np.ascontiguousarray(state[0], dtype=np.uint8 if self.input_dtype == "uint8" else np.float32)
+        np_obs = np.ascontiguousarray(state[0], dtype=self._np_dt)
         ro.obs[:nbatch].copy_(torch.from_numpy(np_obs), non_blocking=True)
         if self.gaussian:
             act = np.ascontiguousarray(label[0], np.float32).reshape(nbatch, self.action_dim)
