@@ -456,6 +456,26 @@ int xtb_muzero_initial_inference(xtb_muzero* mz, const void* obs, int batch, flo
  * reward [B] and value [B] scalars, policy [B, A] probabilities; any output may be NULL. */
 int xtb_muzero_recurrent_inference(xtb_muzero* mz, const float* hidden, const int32_t* action, int batch, float* hidden_out,
                                    float* reward_out, float* value_out, float* policy_out, int use_graph, void* stream);
+/* Device scratch of the tree search for up to max_envs trees of up to max_simulations simulations each, for the action
+ * count and hidden width of `mz` (which it does not keep). */
+typedef struct xtb_muzero_tree xtb_muzero_tree;
+int xtb_muzero_tree_create(const xtb_muzero* mz, int max_envs, int max_simulations, xtb_muzero_tree** out);
+void xtb_muzero_tree_destroy(xtb_muzero_tree* tree);
+/* Mcts.run_mcts (xt/agent/muzero/mcts.py, util.py) over n_envs observations at once, one tree per observation, advanced
+ * in lock step: xtb_muzero_initial_inference of the observations gives the roots; the root priors become
+ * prior * (1 - exploration_frac) + noise * exploration_frac when noise [n_envs, A] (float64) is given; then each of
+ * num_simulations simulations descends every tree by
+ *   ucb = (log((N_p + pb_c_base + 1) / pb_c_base) + pb_c_init) * sqrt(N_p) / (N_c + 1) * prior
+ *         + (N_c > 0 ? normalize(value_sum / N_c) : 0)
+ * (ties to the higher action) to an unexpanded child, evaluates all leaves with one xtb_muzero_recurrent_inference
+ * launch sequence, expands them and backs the leaf value up the path (v = reward + discount * v), with one MinMaxStats
+ * per tree (normalize(x) = (x - min) / (max - min) once max > min, else x).  Tree statistics are float64, products
+ * rounded before they are added.  Writes the root child visit counts visit_counts_out [n_envs, A] and the root values
+ * root_value_out [n_envs] (float64).  n_envs in [1, min(tree max_envs, model max_batch)], num_simulations in
+ * [1, tree max_simulations], pb_c_base finite and positive; XTB_ERR_STATE while a communicator is installed. */
+int xtb_muzero_search(xtb_muzero* mz, xtb_muzero_tree* tree, const void* obs, int n_envs, int num_simulations,
+                      const double* noise, double pb_c_base, double pb_c_init, double discount, double exploration_frac,
+                      int32_t* visit_counts_out, double* root_value_out, int use_graph, void* stream);
 /* xtb_net_backward that also writes d loss / d observation [batch, obs width] into dobs (overwritten): the data-gradient
  * GEMM of every dense layer that reads the observation, summed in layer order.  Float observations with scale 1 read
  * by dense layers only; otherwise XTB_ERR_ARG. */

@@ -126,6 +126,10 @@ _SIGS = {
     "xtb_muzero_train": (C.c_int, [_P, _P, C.POINTER(MuzeroBatch), C.c_int, C.c_float, _P, _P, C.c_int, _P]),
     "xtb_muzero_initial_inference": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P]),
     "xtb_muzero_recurrent_inference": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_muzero_tree_create": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(_P)]),
+    "xtb_muzero_tree_destroy": (None, [_P]),
+    "xtb_muzero_search": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, _P,
+                                    C.c_int, _P]),
     "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

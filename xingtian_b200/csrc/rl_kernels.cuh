@@ -1244,4 +1244,163 @@ __global__ void mz_accumulate_kernel(float* __restrict__ dst, const float* __res
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] += src[i];
 }
 
+// ------------------------------------------------------------------------------------------
+// MuZero tree search (xt/agent/muzero/mcts.py, util.py): N trees advanced in lock step, one warp per tree
+// ------------------------------------------------------------------------------------------
+// Node 0 is the root; simulation s (1-based) expands node s.  Every expanded node has A child edges (prior, visit count,
+// value sum, expanded child node or -1); the root's own statistics live apart.  The statistics are float64, as NumPy 1.x
+// evaluated the reference's float32 priors times Python floats, and every product is rounded before it is added
+// (__dmul_rn / __dadd_rn: no contraction into fma, so the sums are the ones the reference's Python evaluates).
+struct MctsTrees {
+  int E, NN, A, H;         // trees allocated, nodes per tree (1 + max simulations), actions, hidden width
+  float* hid;              // [NN][E][H] hidden state of every expanded node (node-major: one simulation's rows are contiguous)
+  double* reward;          // [E][NN] node reward
+  double* prior;           // [E][NN][A] edge prior
+  double* vsum;            // [E][NN][A] edge value sum
+  int* visits;             // [E][NN][A] edge visit count
+  int* child;              // [E][NN][A] expanded child node, -1 while unexpanded
+  double* root_vsum;       // [E]
+  int* root_visits;        // [E]
+  double* minmax;          // [E][2] MinMaxStats(None): minimum, maximum
+  int* path_node;          // [E][NN] search path: parent node and action of every step
+  int* path_act;           // [E][NN]
+  int* depth;              // [E] steps on the current path
+};
+constexpr int MCTS_THREADS = 128;   // 4 trees per block
+
+__device__ inline void mcts_minmax_update(double* mm, double v) {   // Python's min / max keep the first of equals
+  if (v < mm[0]) mm[0] = v;
+  if (v > mm[1]) mm[1] = v;
+}
+
+// root of tree e from the initial inference's policy: priors prior * (1 - frac) + noise * frac when noise is given
+__global__ void __launch_bounds__(MCTS_THREADS)
+mcts_root_kernel(MctsTrees t, int N, const float* __restrict__ policy, const double* __restrict__ noise, double frac) {
+  pdl_wait(); pdl_trigger();
+  const int e = blockIdx.x * (MCTS_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (e >= N) return;
+  const int A = t.A;
+  const long long base = (long long)e * t.NN * A;
+  for (int a = lane; a < A; a += 32) {
+    double p = (double)policy[(long long)e * A + a];
+    if (noise) p = __dadd_rn(__dmul_rn(p, 1.0 - frac), __dmul_rn(noise[(long long)e * A + a], frac));
+    t.prior[base + a] = p;
+    t.vsum[base + a] = 0.0;
+    t.visits[base + a] = 0;
+    t.child[base + a] = -1;
+  }
+  if (lane == 0) {
+    t.reward[(long long)e * t.NN] = 0.0;
+    t.root_vsum[e] = 0.0;
+    t.root_visits[e] = 0;
+    t.minmax[2 * e] = INFINITY;
+    t.minmax[2 * e + 1] = -INFINITY;
+  }
+}
+
+// One descent per tree (Mcts.run_mcts / select_child / ucb_score): from the root, while the chosen child is expanded,
+// pick the child of the largest (ucb, action) -- ties go to the higher action, as max() over the reference's tuples --
+//   ucb = (log((N_p + pb_c_base + 1) / pb_c_base) + pb_c_init) * (sqrt(N_p) / (N_c + 1)) * prior
+//         + (N_c > 0 ? normalize(value_sum / N_c) : 0)
+// Records the path, and writes the dynamics input concat(hidden of the leaf's parent, one_hot(action)) as row e of x
+// [N, H + A] (the layout mz_concat_onehot_kernel writes).
+__global__ void __launch_bounds__(MCTS_THREADS)
+mcts_select_kernel(MctsTrees t, int N, double pb_c_base, double pb_c_init, float* __restrict__ x) {
+  pdl_wait(); pdl_trigger();
+  const int e = blockIdx.x * (MCTS_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (e >= N) return;
+  const int A = t.A, NN = t.NN;
+  const long long base = (long long)e * NN * A;
+  const double mn = t.minmax[2 * e], mx = t.minmax[2 * e + 1];
+  int node = 0, np = t.root_visits[e], d = 0, act;
+  while (true) {
+    const double pb = __dadd_rn(log(__dadd_rn(__dadd_rn((double)np, pb_c_base), 1.0) / pb_c_base), pb_c_init);
+    const double sq = sqrt((double)np);
+    double best = -INFINITY;
+    int besta = -1;
+    for (int a = lane; a < A; a += 32) {
+      const long long i = base + (long long)node * A + a;
+      const int nc = t.visits[i];
+      double s = __dmul_rn(__dmul_rn(pb, sq / (double)(nc + 1)), t.prior[i]);
+      if (nc > 0) {
+        const double v = t.vsum[i] / (double)nc;
+        s = __dadd_rn(s, mx > mn ? (v - mn) / (mx - mn) : v);
+      }
+      if (s > best || (s == best && a > besta)) { best = s; besta = a; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double s2 = __shfl_xor_sync(0xffffffffu, best, o);
+      const int a2 = __shfl_xor_sync(0xffffffffu, besta, o);
+      if (s2 > best || (s2 == best && a2 > besta)) { best = s2; besta = a2; }
+    }
+    act = besta < 0 ? 0 : besta;   // only when every score is NaN
+    if (lane == 0) { t.path_node[(long long)e * NN + d] = node; t.path_act[(long long)e * NN + d] = act; }
+    d++;
+    const long long i = base + (long long)node * A + act;
+    const int c = t.child[i];
+    if (c < 0) break;
+    np = t.visits[i];
+    node = c;
+  }
+  if (lane == 0) t.depth[e] = d;
+  const int H = t.H;
+  const float* h = t.hid + ((long long)node * t.E + e) * H;
+  float* xr = x + (long long)e * (H + A);
+  for (int j = lane; j < H; j += 32) xr[j] = h[j];
+  for (int j = lane; j < A; j += 32) xr[H + j] = j == act ? 1.f : 0.f;
+}
+
+// Expansion of node s (init_node) from the recurrent inference's reward and policy, then Mcts.backpropagate from the
+// leaf to the root: value_sum += v, visit_count += 1, minmax.update(value()), v = reward + discount * v.  The node's
+// hidden row was written into t.hid by the inference.
+__global__ void __launch_bounds__(MCTS_THREADS)
+mcts_expand_backup_kernel(MctsTrees t, int N, int s, const float* __restrict__ reward, const float* __restrict__ value,
+                          const float* __restrict__ policy, double discount) {
+  pdl_wait(); pdl_trigger();
+  const int e = blockIdx.x * (MCTS_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (e >= N) return;
+  const int A = t.A, NN = t.NN;
+  const long long base = (long long)e * NN * A, nb = base + (long long)s * A;
+  for (int a = lane; a < A; a += 32) {
+    t.prior[nb + a] = (double)policy[(long long)e * A + a];
+    t.vsum[nb + a] = 0.0;
+    t.visits[nb + a] = 0;
+    t.child[nb + a] = -1;
+  }
+  if (lane != 0) return;
+  const int d = t.depth[e];
+  const int* pn = t.path_node + (long long)e * NN;
+  const int* pa = t.path_act + (long long)e * NN;
+  t.child[base + (long long)pn[d - 1] * A + pa[d - 1]] = s;
+  t.reward[(long long)e * NN + s] = (double)reward[e];
+  double* mm = t.minmax + 2 * e;
+  double v = (double)value[e];
+  for (int k = d - 1; k >= 0; k--) {
+    const long long i = base + (long long)pn[k] * A + pa[k];
+    const double sum = __dadd_rn(t.vsum[i], v);
+    const int n = t.visits[i] + 1;
+    t.vsum[i] = sum;
+    t.visits[i] = n;
+    mcts_minmax_update(mm, sum / (double)n);
+    v = __dadd_rn(t.reward[(long long)e * NN + t.child[i]], __dmul_rn(discount, v));
+  }
+  const double sum = __dadd_rn(t.root_vsum[e], v);
+  const int n = t.root_visits[e] + 1;
+  t.root_vsum[e] = sum;
+  t.root_visits[e] = n;
+  mcts_minmax_update(mm, sum / (double)n);
+}
+
+// get_info: root child visit counts [N, A] and root value value_sum / visit_count [N]
+__global__ void __launch_bounds__(MCTS_THREADS)
+mcts_result_kernel(MctsTrees t, int N, int32_t* __restrict__ counts, double* __restrict__ root_value) {
+  pdl_wait(); pdl_trigger();
+  const int e = blockIdx.x * (MCTS_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (e >= N) return;
+  const int A = t.A;
+  for (int a = lane; a < A; a += 32) counts[(long long)e * A + a] = t.visits[(long long)e * t.NN * A + a];
+  if (lane == 0) root_value[e] = t.root_vsum[e] / (double)t.root_visits[e];
+}
+
 }  // namespace xtb

@@ -1861,7 +1861,7 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
-                kMuzeroInitInfer, kMuzeroRecurInfer };
+                kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -1872,6 +1872,7 @@ struct CaptureKey {
 };
 template <class T> static uint64_t key_word(T v) {
   if constexpr (std::is_same_v<T, float>) { uint32_t u; memcpy(&u, &v, sizeof u); return u; }
+  else if constexpr (std::is_same_v<T, double>) { uint64_t u; memcpy(&u, &v, sizeof u); return u; }
   else if constexpr (std::is_pointer_v<T>) return (uint64_t)(uintptr_t)v;
   else return (uint64_t)v;
 }
@@ -2373,6 +2374,22 @@ extern "C" int xtb_muzero_initial_inference(xtb_muzero* m, const void* obs, int 
                    use_graph, stream, [&](void* st) { return mz_initial_launch(m, obs, batch, hidden_out, value_out, policy_out, S(st)); });
 }
 
+// recurrent_inference after its input concat(hidden, one_hot(action)) is in m->xbuf: dynamics then prediction
+static int mz_dynamics_launch(xtb_muzero* m, int batch, float* hidden_out, float* reward_out, float* value_out, float* policy_out,
+                              cudaStream_t st) {
+  const xtb_muzero_desc& d = m->d;
+  int rc = net_forward_impl(m->dyn, nullptr, m->xbuf, nullptr, batch, st, 0u, (1u << d.dyn_h) | (1u << d.dyn_r));
+  if (rc) return rc;
+  const float* h = xtb_net_tensor(m->dyn, d.dyn_h);
+  if (hidden_out) CUDA_TRY(cudaMemcpyAsync(hidden_out, h, (size_t)batch * m->H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (reward_out) {
+    XLAUNCH(mz_support_value_kernel, mz_blocks(batch), MZ_THREADS, 0, st, (const float*)xtb_net_tensor(m->dyn, d.dyn_r), batch, m->Sr,
+            d.reward_min, d.reward_max, reward_out);
+    LAUNCH_CHECK();
+  }
+  return mz_predict(m, h, batch, value_out, policy_out, st);
+}
+
 extern "C" int xtb_muzero_recurrent_inference(xtb_muzero* m, const float* hidden, const int32_t* action, int batch, float* hidden_out,
                                               float* reward_out, float* value_out, float* policy_out, int use_graph, void* stream) {
   if (int rc = mz_check("xtb_muzero_recurrent_inference", m, !hidden || !action, nullptr, batch)) return rc;
@@ -2380,20 +2397,90 @@ extern "C" int xtb_muzero_recurrent_inference(xtb_muzero* m, const float* hidden
                                value_out, policy_out),
                    use_graph, stream, [&](void* sv) -> int {
     cudaStream_t st = S(sv);
-    const xtb_muzero_desc& d = m->d;
     const int H = m->H, A = m->A;
     XLAUNCH(mz_concat_onehot_kernel, std::min(4 * kSMs, (batch * (H + A) + 255) / 256), 256, 0, st, hidden, batch, H, action, 1, 0, A, m->xbuf);
     LAUNCH_CHECK();
-    int rc = net_forward_impl(m->dyn, nullptr, m->xbuf, nullptr, batch, st, 0u, (1u << d.dyn_h) | (1u << d.dyn_r));
+    return mz_dynamics_launch(m, batch, hidden_out, reward_out, value_out, policy_out, st);
+  });
+}
+
+// ---- MuZero tree search (xt/agent/muzero/mcts.py) ---------------------------------------------------------------------
+// The device state of up to max_envs trees of up to 1 + max_simulations expanded nodes (MctsTrees), plus the float
+// outputs of the inference calls the search makes.
+struct xtb_muzero_tree {
+  MctsTrees t{};
+  int max_sims = 0;
+  void* buf = nullptr;
+  float *reward = nullptr, *value = nullptr, *policy = nullptr;   // [E], [E], [E, A]
+};
+
+extern "C" int xtb_muzero_tree_create(const xtb_muzero* m, int max_envs, int max_simulations, xtb_muzero_tree** out) {
+  if (!m || !out) return fail(XTB_ERR_ARG, "xtb_muzero_tree_create: null pointer");
+  if (max_envs < 1 || max_simulations < 1 || max_simulations > (1 << 20))
+    return fail(XTB_ERR_ARG, "xtb_muzero_tree_create: max_envs %d / max_simulations %d out of range", max_envs, max_simulations);
+  const long long E = max_envs, NN = max_simulations + 1, A = m->A, H = m->H;
+  // byte sizes, in the order of `dst` below; each piece starts 256-byte aligned
+  const long long sizes[] = {NN * E * H * 4, E * NN * 8, E * NN * A * 8, E * NN * A * 8, E * NN * A * 4, E * NN * A * 4, E * 8, E * 4,
+                             E * 2 * 8, E * NN * 4, E * NN * 4, E * 4, E * 4, E * 4, E * A * 4};
+  auto* tr = new xtb_muzero_tree();
+  MctsTrees& t = tr->t;
+  void** dst[] = {(void**)&t.hid, (void**)&t.reward, (void**)&t.prior, (void**)&t.vsum, (void**)&t.visits, (void**)&t.child,
+                  (void**)&t.root_vsum, (void**)&t.root_visits, (void**)&t.minmax, (void**)&t.path_node, (void**)&t.path_act,
+                  (void**)&t.depth, (void**)&tr->reward, (void**)&tr->value, (void**)&tr->policy};
+  long long tot = 0;
+  for (long long n : sizes) tot += align_up(n, 256);
+  cudaError_t e = cudaMalloc(&tr->buf, tot);
+  if (e != cudaSuccess) { delete tr; return fail(XTB_ERR_NOMEM, "xtb_muzero_tree_create: %s", cudaGetErrorString(e)); }
+  char* p = (char*)tr->buf;
+  for (int i = 0; i < 15; i++) { *dst[i] = p; p += align_up(sizes[i], 256); }
+  t.E = max_envs; t.NN = (int)NN; t.A = (int)A; t.H = (int)H;
+  tr->max_sims = max_simulations;
+  *out = tr;
+  return XTB_OK;
+}
+
+extern "C" void xtb_muzero_tree_destroy(xtb_muzero_tree* tr) {
+  if (!tr) return;
+  drop_graphs_of(tr);
+  cudaDeviceSynchronize();
+  cudaFree(tr->buf);
+  delete tr;
+}
+
+extern "C" int xtb_muzero_search(xtb_muzero* m, xtb_muzero_tree* tr, const void* obs, int n_envs, int num_simulations,
+                                 const double* noise, double pb_c_base, double pb_c_init, double discount, double exploration_frac,
+                                 int32_t* visit_counts_out, double* root_value_out, int use_graph, void* stream) {
+  const char* fn = "xtb_muzero_search";
+  if (int rc = mz_check(fn, m, !tr || !obs || !visit_counts_out || !root_value_out, nullptr, n_envs)) return rc;
+  if (tr->t.A != m->A || tr->t.H != m->H)
+    return fail(XTB_ERR_ARG, "%s: tree made for %d actions / hidden width %d, model has %d / %d", fn, tr->t.A, tr->t.H, m->A, m->H);
+  if (n_envs > tr->t.E) return fail(XTB_ERR_ARG, "%s: %d environments, the tree holds %d", fn, n_envs, tr->t.E);
+  if (num_simulations < 1 || num_simulations > tr->max_sims)
+    return fail(XTB_ERR_ARG, "%s: num_simulations %d not in [1, %d]", fn, num_simulations, tr->max_sims);
+  if (!std::isfinite(pb_c_base) || !(pb_c_base > 0)) return fail(XTB_ERR_ARG, "%s: pb_c_base %g is not finite and positive", fn, pb_c_base);
+  return run_graph(capture_key(kMuzeroSearch, {m->rep, m->dyn, m->pred, m, tr}, m, tr, obs, n_envs, num_simulations, noise, pb_c_base,
+                               pb_c_init, discount, exploration_frac, visit_counts_out, root_value_out),
+                   use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    const MctsTrees& t = tr->t;
+    const int N = n_envs, blocks = (N + MCTS_THREADS / 32 - 1) / (MCTS_THREADS / 32);
+    const size_t rows = (size_t)t.E * t.H;   // floats of one node's block of hidden rows
+    int rc = mz_initial_launch(m, obs, N, t.hid, nullptr, tr->policy, st);
     if (rc) return rc;
-    const float* h = xtb_net_tensor(m->dyn, d.dyn_h);
-    if (hidden_out) CUDA_TRY(cudaMemcpyAsync(hidden_out, h, (size_t)batch * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (reward_out) {
-      XLAUNCH(mz_support_value_kernel, mz_blocks(batch), MZ_THREADS, 0, st, (const float*)xtb_net_tensor(m->dyn, d.dyn_r), batch, m->Sr,
-              d.reward_min, d.reward_max, reward_out);
+    XLAUNCH(mcts_root_kernel, blocks, MCTS_THREADS, 0, st, t, N, (const float*)tr->policy, noise, exploration_frac);
+    LAUNCH_CHECK();
+    for (int s = 1; s <= num_simulations; s++) {
+      XLAUNCH(mcts_select_kernel, blocks, MCTS_THREADS, 0, st, t, N, pb_c_base, pb_c_init, m->xbuf);
+      LAUNCH_CHECK();
+      rc = mz_dynamics_launch(m, N, t.hid + s * rows, tr->reward, tr->value, tr->policy, st);
+      if (rc) return rc;
+      XLAUNCH(mcts_expand_backup_kernel, blocks, MCTS_THREADS, 0, st, t, N, s, (const float*)tr->reward, (const float*)tr->value,
+              (const float*)tr->policy, discount);
       LAUNCH_CHECK();
     }
-    return mz_predict(m, h, batch, value_out, policy_out, st);
+    XLAUNCH(mcts_result_kernel, blocks, MCTS_THREADS, 0, st, t, N, visit_counts_out, root_value_out);
+    LAUNCH_CHECK();
+    return XTB_OK;
   });
 }
 

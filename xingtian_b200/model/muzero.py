@@ -2,7 +2,8 @@
 
 The representation, dynamics and prediction networks are three engine nets bound to consecutive slices of one flat
 parameter buffer (and one gradient buffer) in MuzeroBase's Keras weight-list order, trained by one Adam.  The unrolled
-training step, the support projections and the inference calls run in libxtb200 (xtb_muzero_*)."""
+training step, the support projections, the inference calls and the tree search over many observations at once
+(search / search_device) run in libxtb200 (xtb_muzero_*)."""
 import ctypes as C
 import math
 import os
@@ -131,6 +132,7 @@ class MuzeroModel(XTModel):
 
     def __del__(self):
         try:
+            self._drop_tree()
             if getattr(self, "handle", None) and self.handle.value:
                 capi.lib().xtb_muzero_destroy(self.handle)
                 self.handle = C.c_void_p()
@@ -280,6 +282,70 @@ class MuzeroModel(XTModel):
         stage_h2d(b["act1"], np.asarray([int(action)]), np.int32)
         value, reward, policy, hidden = self.recurrent_inference_batch(b["hid_in"], b["act1"], 1)
         return NetworkOutput(float(value[0].cpu()), float(reward[0].cpu()), policy[0].cpu().numpy(), hidden[0].cpu().numpy())
+
+    # ---- tree search ----------------------------------------------------------------------------------------------
+    def _search_tree(self, n, num_simulations):
+        """The tree scratch for n trees of num_simulations simulations: created on first use, grown (never shrunk) when
+        a call needs more trees or simulations than it holds."""
+        envs, sims = getattr(self, "_tree_size", (0, 0))
+        if n > envs or num_simulations > sims:
+            envs, sims = max(n, envs), max(num_simulations, sims)
+            self._drop_tree()
+            tree = C.c_void_p()
+            with torch.cuda.device(self.device):
+                check(capi.lib().xtb_muzero_tree_create(self.handle, envs, sims, C.byref(tree)))
+            self._tree, self._tree_size = tree, (envs, sims)
+        return self._tree
+
+    def _drop_tree(self):
+        tree = getattr(self, "_tree", None)
+        if tree is not None and tree.value:
+            capi.lib().xtb_muzero_tree_destroy(tree)
+        self._tree, self._tree_size = None, (0, 0)
+
+    def _search_buffers(self, n):
+        """[n] float64 root values followed by the [n, A] int32 visit counts in one device block (one download), and the
+        [n, A] float64 noise."""
+        key = ("search", n)
+        b = self._bufs.get(key)
+        if b is None:
+            A = self.action_dim
+            out = torch.empty(n + (n * A + 1) // 2, dtype=torch.float64, device=self.device)
+            b = dict(out=out, root_value=out[:n], counts=out[n:].view(torch.int32)[:n * A].view(n, A),
+                     noise=torch.empty(n, A, dtype=torch.float64, device=self.device))
+            self._bufs[key] = b
+        return b
+
+    def search_device(self, obs, n, num_simulations, noise=None, visit_counts=None, root_value=None, pb_c_base=19652,
+                      pb_c_init=1.25, discount=0.997, exploration_frac=0.25):
+        """Mcts.run_mcts (xt/agent/muzero/mcts.py) over n device observations at once, one tree each (xtb_muzero_search):
+        -> (visit_counts [n, A] int32, root_value [n] float64) device tensors.  noise [n, A] float64 (device) mixes
+        into the root priors as the reference's add_exploration_noise.  Without visit_counts / root_value the results go
+        to buffers of this model, per n, that the next search of the same size overwrites."""
+        self._check_batch(n)
+        b = self._search_buffers(n)
+        visit_counts = b["counts"] if visit_counts is None else visit_counts
+        root_value = b["root_value"] if root_value is None else root_value
+        tree = self._search_tree(n, int(num_simulations))
+        check(capi.lib().xtb_muzero_search(self.handle, tree, _ptr(obs), int(n), int(num_simulations), _ptr(noise),
+                                           float(pb_c_base), float(pb_c_init), float(discount), float(exploration_frac),
+                                           _ptr(visit_counts), _ptr(root_value), 1 if self.use_graph else 0, stream_ptr()))
+        return visit_counts, root_value
+
+    def search(self, obs, num_simulations, noise=None, **kw):
+        """search_device on host observations [n, ...] (and host noise [n, A]): staged uploads, one search, one download
+        -> (visit_counts [n, A] int32, root_value [n] float64) numpy arrays."""
+        obs = self._host_obs(obs)
+        n = obs.shape[0]
+        self._check_batch(n)
+        b, sb = self._buffers(n), self._search_buffers(n)
+        stage_h2d(b["obs"], obs, self._np_dt)
+        if noise is not None:
+            stage_h2d(sb["noise"], np.asarray(noise), np.float64)
+        self.search_device(b["obs"], n, num_simulations, sb["noise"] if noise is not None else None, **kw)
+        host = sb["out"].cpu().numpy()
+        A = self.action_dim
+        return host[n:].view(np.int32)[:n * A].reshape(n, A).copy(), host[:n].copy()
 
     def value_inference(self, input_data):
         """muzero_model.py:228-239: the scalar value of every observation (any count: max_batch rows per call)."""
