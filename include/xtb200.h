@@ -476,6 +476,57 @@ void xtb_muzero_tree_destroy(xtb_muzero_tree* tree);
 int xtb_muzero_search(xtb_muzero* mz, xtb_muzero_tree* tree, const void* obs, int n_envs, int num_simulations,
                       const double* noise, double pb_c_base, double pb_c_init, double discount, double exploration_frac,
                       int32_t* visit_counts_out, double* root_value_out, int use_graph, void* stream);
+/* ---- QMIX: replaces QMixModel's train and explore graphs (xt/model/qmix/qmix_tf.py:172-589) -------------------------
+ * One weight set is a flat float buffer [fc1 | GRU | fc2 | mixer]: fc1 = dense(H, relu) on the agent inputs (net `fc1`,
+ * obs_dim wide), the GRUCell's rnn/gru_cell/gates/kernel [2H, 2H], gates/bias [2H], candidate/kernel [2H, H] and
+ * candidate/bias [H] back to back at float offset gru_off (kernel rows: x first, then h), fc2 = dense(A) on the GRU
+ * outputs (net `fc2`, H wide, float input) and the mixer's hypernetworks, one net `hyper` on the state whose 7 dense layers
+ * are, in order, hyper_w1 (hypernet_embed relu, then E n_agents linear), hyper_b1 (E linear, on the state),
+ * hyper_w_final (hypernet_embed relu, then E linear) and val_for_bias (E relu, then 1 linear) -- the TF variable order
+ * of the eval_agent and eval_mixer scopes.  The three nets are bound to their slices of the eval set (gaps between the
+ * slices are allowed) and of a gradient buffer with the same layout; the optimiser spans the set (per-tensor clipping:
+ * one segment per variable).  Target and explore sets are caller buffers with the same layout (an explore set needs
+ * only the agent part).
+ * Limits (XTB_ERR_ARG otherwise, at create): 1 <= H with the GRU kernels' shared-memory plan fitting (H <= 128),
+ * n_agents <= 32, n_actions <= 255 (the reference casts actions to uint8), mixing embed E <= 128. */
+typedef struct xtb_qmix xtb_qmix;
+typedef struct xtb_qmix_desc {
+  int32_t batch;          /* B episodes per training batch */
+  int32_t episode_limit;  /* L: a batch holds L + 1 steps of agent inputs and L transitions */
+  int32_t n_agents;
+  int32_t use_double_q;
+  float gamma;
+  long long gru_off;      /* offset (floats) of gates/kernel in a weight set */
+} xtb_qmix_desc;
+int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyper, const xtb_qmix_desc* desc, xtb_qmix** out);
+void xtb_qmix_destroy(xtb_qmix* q);
+/* One training batch (device arrays). */
+typedef struct xtb_qmix_batch {
+  const float* obs;         /* [B, L+1, n_agents, obs_dim] agent inputs */
+  const int32_t* seq_len;   /* [B n_agents] GRU sequence lengths (train_obs_len, sequence b n_agents + a), read at run time,
+                               clamped to [0, L+1] */
+  const float* avail;       /* [B, L+1, n_agents, A] available actions (0 = unavailable) */
+  const int32_t* actions;   /* [B, L, n_agents] taken actions in [0, A) */
+  const float* state;       /* [B, L, state_dim] eval mixer input (batch["state"][:, :-1]) */
+  const float* next_state;  /* [B, L, state_dim] target mixer input (batch["state"][:, 1:]) */
+  const float* reward;      /* [B, L] */
+  const float* terminated;  /* [B, L] */
+  const float* mask;        /* [B, L] */
+} xtb_qmix_batch;
+/* QMixModel.train (qmix_tf.py:351-492, 546-589) as one step: the target and eval agents over all B (L+1) n_agents rows
+ * (fc1 and fc2 on the engine, the GRU recurrence of dynamic_rnn as one persistent kernel: outputs at t >= seq_len are
+ * zero), both hypernetworks over the B L state rows, the fused mixer / TD kernel (see qmix.cuh), the backward (the GRU's
+ * in reverse time, its weight gradients as GEMMs over all rows) and one step of `opt`, which must be set to centred
+ * RMSProp by the caller (xtb_opt_use_rmsprop, decay 0.95, epsilon 1.5e-7, per-tensor clip at grad_norm_clip), then the
+ * weight refresh of the three nets.  *loss_out = sum (mask td)^2 / sum mask, summed in a fixed order.  target: the
+ * target weight set.  XTB_ERR_STATE while a communicator is installed. */
+int xtb_qmix_train(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qmix_batch* batch, float* loss_out, int use_graph,
+                   void* stream);
+/* QMixModel.infer_actions (qmix_tf.py:242-251) for one environment: fc1 -> one GRU step -> fc2 with the weight set
+ * `explore` on obs [n_agents, obs_dim]; hidden [n_agents, H] is read as the state and overwritten with the new one;
+ * q_out [n_agents, A]. */
+int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream);
+
 /* xtb_net_backward that also writes d loss / d observation [batch, obs width] into dobs (overwritten): the data-gradient
  * GEMM of every dense layer that reads the observation, summed in layer order.  Float observations with scale 1 read
  * by dense layers only; otherwise XTB_ERR_ARG. */

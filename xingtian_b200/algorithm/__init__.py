@@ -6,3 +6,4 @@ from .impala import IMPALA  # noqa: F401
 from .dqn import DQN  # noqa: F401
 from .replay_buffer import ReplayBuffer, DeviceReplayBuffer  # noqa: F401
 from .muzero import Muzero  # noqa: F401
+from .qmix import QMixAlg  # noqa: F401

@@ -59,6 +59,16 @@ class MuzeroBatch(C.Structure):
                 ("target_policy", C.c_void_p), ("unroll", C.c_int32)]
 
 
+class QmixDesc(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("episode_limit", C.c_int32), ("n_agents", C.c_int32), ("use_double_q", C.c_int32),
+                ("gamma", C.c_float), ("gru_off", C.c_longlong)]
+
+
+class QmixBatch(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("seq_len", C.c_void_p), ("avail", C.c_void_p), ("actions", C.c_void_p), ("state", C.c_void_p),
+                ("next_state", C.c_void_p), ("reward", C.c_void_p), ("terminated", C.c_void_p), ("mask", C.c_void_p)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "xtb_version": (C.c_int, []),
@@ -130,6 +140,10 @@ _SIGS = {
     "xtb_muzero_tree_destroy": (None, [_P]),
     "xtb_muzero_search": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, _P,
                                     C.c_int, _P]),
+    "xtb_qmix_create": (C.c_int, [_P, _P, _P, C.POINTER(QmixDesc), C.POINTER(_P)]),
+    "xtb_qmix_destroy": (None, [_P]),
+    "xtb_qmix_train": (C.c_int, [_P, _P, _P, C.POINTER(QmixBatch), _P, C.c_int, _P]),
+    "xtb_qmix_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

@@ -16,6 +16,7 @@
 #include "gemm_f32.cuh"
 #include "optim.cuh"
 #include "rl_kernels.cuh"
+#include "qmix.cuh"
 #include "stager.cuh"
 #include "bp_gemm.cuh"
 #include "comm.cuh"
@@ -1861,7 +1862,7 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
-                kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch };
+                kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -2578,6 +2579,220 @@ extern "C" int xtb_muzero_train(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_b
   return run_graph(capture_key(kMuzeroTrain, {m->rep, m->dyn, m->pred, m, opt}, m, bt.obs, bt.action, bt.target_value,
                                bt.target_reward, bt.target_policy, batch, loss_offset, loss_out, value_out),
                    use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
+}
+
+// ---- QMIX (xt/model/qmix/qmix_tf.py) ----------------------------------------------------------------------------------
+// fc1, fc2 and the hypernetworks are engine nets bound to slices of the eval weight set; target and explore sets are
+// read through the nets' foreign-parameter forward.  The object owns the step's device scratch for the fixed batch.
+struct xtb_qmix {
+  xtb_net *fc1 = nullptr, *fc2 = nullptr, *hyp = nullptr;
+  xtb_qmix_desc d{};
+  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, E = 0, R = 0, BL = 0, S = 0, G = 0, n_part = 0;
+  size_t smem = 0;
+  long long o_gru = 0, o_fc2 = 0, o_hyp = 0, n_params = 0;
+  float* buf = nullptr;
+  float *qt = nullptr, *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr,
+        *w1t = nullptr, *b1t = nullptr, *wft = nullptr, *vt = nullptr, *part = nullptr;
+  int32_t* ones = nullptr;   // [n_agents] sequence lengths of the one-step inference
+};
+// hyper net: tensor ids of the w1, b1, w_final and v heads
+static const int kQw1 = 2, kQb1 = 3, kQwf = 5, kQv = 7;
+
+extern "C" int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyp, const xtb_qmix_desc* desc, xtb_qmix** out) {
+  const char* fn = "xtb_qmix_create";
+  if (!fc1 || !fc2 || !hyp || !desc || !out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  for (xtb_net* nt : {fc1, fc2, hyp})
+    if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  const xtb_qmix_desc& d = *desc;
+  auto dense = [](const xtb_net* nt, int i, int src, int act) {
+    const LayerPlan& lp = nt->L[i];
+    return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
+  };
+  if (fc1->L.size() != 1 || !dense(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
+    return fail(XTB_ERR_ARG, "%s: fc1 must be one relu dense layer on float agent inputs", fn);
+  const int H = fc1->tsize[1];
+  if (fc2->L.size() != 1 || !dense(fc2, 0, 0, XTB_ACT_NONE) || fc2->tsize[0] != H)
+    return fail(XTB_ERR_ARG, "%s: fc2 must be one linear dense layer on the %d-wide GRU output", fn, H);
+  if (int rc = input_grad_check(fc2)) return rc;
+  const int A = fc2->tsize[1], n = d.n_agents;
+  if (hyp->L.size() != 7 || !dense(hyp, 0, 0, XTB_ACT_RELU) || !dense(hyp, 1, 1, XTB_ACT_NONE) || !dense(hyp, 2, 0, XTB_ACT_NONE) ||
+      !dense(hyp, 3, 0, XTB_ACT_RELU) || !dense(hyp, 4, 4, XTB_ACT_NONE) || !dense(hyp, 5, 0, XTB_ACT_RELU) || !dense(hyp, 6, 6, XTB_ACT_NONE))
+    return fail(XTB_ERR_ARG, "%s: hyper must be hyper_w1 (2 layers), hyper_b1, hyper_w_final (2 layers), val_for_bias (2 layers)", fn);
+  const int E = hyp->tsize[kQb1];
+  if (n < 1 || n > QM_MAX_AGENTS) return fail(XTB_ERR_ARG, "%s: n_agents %d not in [1, %d]", fn, n, QM_MAX_AGENTS);
+  if (A < 1 || A > 255) return fail(XTB_ERR_ARG, "%s: n_actions %d not in [1, 255] (actions are uint8 in the reference)", fn, A);
+  if (E < 1 || E > QM_MAX_EMBED || hyp->tsize[kQw1] != E * n || hyp->tsize[kQwf] != E || hyp->tsize[6] != E || hyp->tsize[kQv] != 1)
+    return fail(XTB_ERR_ARG, "%s: mixer widths disagree (embed %d must be in [1, %d], w1 embed x n_agents, v 1)", fn, E, QM_MAX_EMBED);
+  if (d.batch < 1 || d.episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, d.batch, d.episode_limit);
+  const long long T = d.episode_limit + 1, R = (long long)d.batch * T * n, BL = (long long)d.batch * d.episode_limit;
+  if (R > (1LL << 30) / std::max(3 * H, 1)) return fail(XTB_ERR_ARG, "%s: batch too large", fn);
+  if (fc1->max_batch < R || fc2->max_batch < R || hyp->max_batch < BL)
+    return fail(XTB_ERR_ARG, "%s: nets hold fewer rows than a batch (fc1 / fc2: %lld, hyper: %lld)", fn, R, BL);
+  const int S = d.batch * n;
+  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
+  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
+  if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
+    return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
+  // [fc1 | gru | fc2 | hyper] in one buffer, the gradients at the same offsets
+  const long long o_gru = d.gru_off, o_fc2 = fc2->params - fc1->params, o_hyp = hyp->params - fc1->params;
+  const long long gru_n = 2LL * H * 2 * H + 2 * H + 2LL * H * H + H;
+  if (o_gru < fc1->n_params || o_fc2 < o_gru + gru_n || o_hyp < o_fc2 + fc2->n_params || fc2->grads != fc1->grads + o_fc2 ||
+      hyp->grads != fc1->grads + o_hyp)
+    return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2 | hyper] of one buffer, in order", fn);
+  auto* q = new xtb_qmix();
+  q->fc1 = fc1; q->fc2 = fc2; q->hyp = hyp; q->d = d;
+  q->B = d.batch; q->L = d.episode_limit; q->T = (int)T; q->n = n; q->A = A; q->H = H; q->E = E; q->R = (int)R; q->BL = (int)BL;
+  q->S = S; q->G = G; q->smem = qgru_smem_floats(H, G) * 4;
+  q->o_gru = o_gru; q->o_fc2 = o_fc2; q->o_hyp = o_hyp; q->n_params = o_hyp + hyp->n_params;
+  q->n_part = (int)((BL + QM_THREADS / 32 - 1) / (QM_THREADS / 32));
+  const long long sizes[] = {R * A, R * 2 * H, R * H, R * H, R * H, R * H, R * 2 * H, R * H, BL * n * E, BL * E, BL * E, BL, q->n_part + 2, n};
+  float** dst[] = {&q->qt, &q->xg, &q->xc, &q->hout, &q->rh, &q->dy, &q->dag, &q->dac, &q->w1t, &q->b1t, &q->wft, &q->vt, &q->part,
+                   (float**)&q->ones};
+  long long tot = 0;
+  for (long long s : sizes) tot += (s + 63) / 64 * 64;
+  cudaError_t e = cudaMalloc(&q->buf, tot * sizeof(float));
+  if (e != cudaSuccess) { delete q; return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e)); }
+  float* p = q->buf;
+  for (int i = 0; i < 14; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
+  std::vector<int32_t> ones(n, 1);
+  e = cudaMemset(q->buf, 0, tot * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemcpy(q->ones, ones.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q->smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q->smem);
+  if (e != cudaSuccess) { cudaFree(q->buf); delete q; return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  *out = q;
+  return XTB_OK;
+}
+
+extern "C" void xtb_qmix_destroy(xtb_qmix* q) {
+  if (!q) return;
+  drop_graphs_of(q);
+  cudaDeviceSynchronize();
+  cudaFree(q->buf);
+  delete q;
+}
+
+// fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding
+// S = rows / T sequences of T steps; the Q values stay in fc2's output tensor.  h0 / hT: see qmix_gru_fwd_kernel.
+static int qmix_agent_forward(xtb_qmix* q, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
+                              float* hT, int store, cudaStream_t st) {
+  const int H = q->H;
+  const float* W = P ? P : q->fc1->params;
+  const float *wg = W + q->o_gru, *bg = wg + 2 * H * 2 * H, *wc = bg + 2 * H, *bc = wc + 2 * H * H;
+  int rc = net_forward_impl(q->fc1, P, obs, nullptr, rows, st, 0u, 1u << 1);
+  if (rc) return rc;
+  const float* x = xtb_net_tensor(q->fc1, 1);
+  // the input projections of every step: x W[:H] + b for the gates and the candidate
+  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wg, 2 * H}, EpiBiasAct{q->xg, bg, 1.f, XTB_ACT_NONE, 2 * H, nullptr, 0}, rows,
+              2 * H, H, false, st);
+  LAUNCH_CHECK();
+  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wc, H}, EpiBiasAct{q->xc, bc, 1.f, XTB_ACT_NONE, H, nullptr, 0}, rows, H, H,
+              false, st);
+  LAUNCH_CHECK();
+  const int S = rows / T, G = q->G;
+  XLAUNCH(qmix_gru_fwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, q->xg, q->xc, h0, hT, q->hout, q->rh, seq_len, S, T,
+          q->n, H, G, store);
+  LAUNCH_CHECK();
+  return net_forward_impl(q->fc2, P ? P + q->o_fc2 : nullptr, q->hout, nullptr, rows, st, 0u, 1u << 1);
+}
+
+static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qmix_batch& b, float* loss_out, cudaStream_t st) {
+  const int H = q->H, A = q->A, E = q->E, n = q->n, R = q->R, BL = q->BL;
+  xtb_net *fc1 = q->fc1, *fc2 = q->fc2, *hyp = q->hyp;
+  const unsigned heads = (1u << kQw1) | (1u << kQb1) | (1u << kQwf) | (1u << kQv);
+  // target mixer's hypernetworks on the next states (kept), then the eval ones on the states
+  int rc = net_forward_impl(hyp, target + q->o_hyp, b.next_state, nullptr, BL, st, 0u, heads);
+  if (rc) return rc;
+  const std::pair<int, float*> tcopy[] = {{kQw1, q->w1t}, {kQb1, q->b1t}, {kQwf, q->wft}, {kQv, q->vt}};
+  for (const auto& c : tcopy)
+    CUDA_TRY(cudaMemcpyAsync(c.second, xtb_net_tensor(hyp, c.first), (size_t)BL * hyp->tsize[c.first] * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st));
+  rc = net_forward_impl(hyp, nullptr, b.state, nullptr, BL, st, 0u, heads);
+  if (rc) return rc;
+  // target agent (Q kept), then the eval agent with the activations of its backward
+  rc = qmix_agent_forward(q, target, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 0, st);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(q->qt, xtb_net_tensor(fc2, 1), (size_t)R * A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  rc = qmix_agent_forward(q, nullptr, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 1, st);
+  if (rc) return rc;
+  // mixers, TD loss and the gradients wrt the chosen Q and the hypernet outputs
+  float* dq = xtb_net_tensor_grad(fc2, 1);
+  float* msum = q->part + q->n_part;
+  CUDA_TRY(cudaMemsetAsync(dq, 0, (size_t)R * A * sizeof(float), st));
+  XLAUNCH(qmix_mask_sum_kernel, 1, QM_THREADS, 0, st, b.mask, BL, msum);
+  LAUNCH_CHECK();
+  XLAUNCH(qmix_mix_td_kernel, q->n_part, QM_THREADS, 0, st, (const float*)xtb_net_tensor(fc2, 1), (const float*)q->qt, b.avail, b.actions,
+          (const float*)xtb_net_tensor(hyp, kQw1), (const float*)xtb_net_tensor(hyp, kQb1), (const float*)xtb_net_tensor(hyp, kQwf),
+          (const float*)xtb_net_tensor(hyp, kQv), (const float*)q->w1t, (const float*)q->b1t, (const float*)q->wft, (const float*)q->vt,
+          b.reward, b.terminated, b.mask, (const float*)msum, q->B, q->L, n, A, E, q->d.gamma, q->d.use_double_q, dq, xtb_net_tensor_grad(hyp, kQw1),
+          xtb_net_tensor_grad(hyp, kQb1), xtb_net_tensor_grad(hyp, kQwf), xtb_net_tensor_grad(hyp, kQv), q->part);
+  LAUNCH_CHECK();
+  XLAUNCH(qmix_loss_kernel, 1, 32, 0, st, (const float*)q->part, q->n_part, (const float*)msum, loss_out);
+  LAUNCH_CHECK();
+  // backward: the hypernetworks, fc2 (with d loss / d GRU output), the GRU in reverse time, its weight gradients, fc1
+  const int32_t hheads[4] = {kQw1, kQb1, kQwf, kQv}, one[1] = {1};
+  rc = net_backward_impl(hyp, b.state, nullptr, BL, st, BackwardOpts(hheads, 4));
+  if (rc) return rc;
+  BackwardOpts o2(one, 1);
+  o2.dobs = q->dy;
+  rc = net_backward_impl(fc2, q->hout, nullptr, R, st, o2);
+  if (rc) return rc;
+  const float* W = fc1->params;
+  const float *wg = W + q->o_gru, *wc = wg + 2 * H * 2 * H + 2 * H;
+  float* gg = fc1->grads + q->o_gru;
+  float* gc = gg + 2 * H * 2 * H + 2 * H;
+  const int S = q->S, G = q->G;
+  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, (const float*)q->xg, (const float*)q->xc,
+          (const float*)q->hout, (const float*)q->dy, q->dag, q->dac, b.seq_len, S, q->T, n, H, G);
+  LAUNCH_CHECK();
+  const float* x = xtb_net_tensor(fc1, 1);
+  // [kernel; bias] gradients: [x | h_prev | 1]^T da_gates and [x | r h_prev | 1]^T da_candidate over all rows
+  launch_gemm(AGruFeat{x, q->hout, H, n, q->T, 1}, BRowMajor{q->dag, 2 * H}, EpiDgrad{gg, gg, 0, 2 * H, 0, nullptr, 0}, 2 * H + 1, 2 * H,
+              R, false, st);
+  LAUNCH_CHECK();
+  launch_gemm(AGruFeat{x, q->rh, H, n, q->T, 0}, BRowMajor{q->dac, H}, EpiDgrad{gc, gc, 0, H, 0, nullptr, 0}, 2 * H + 1, H, R, false, st);
+  LAUNCH_CHECK();
+  // d loss / d fc1 pre-activation = relu'(x) (da_gates W_g[:H]^T + da_candidate W_c[:H]^T)
+  float* dx = xtb_net_tensor_grad(fc1, 1);
+  launch_gemm(ADense<float>{q->dag, nullptr, 2 * H}, BTransposed{wg, 2 * H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 0, nullptr, 0}, R, H, 2 * H,
+              false, st);
+  LAUNCH_CHECK();
+  launch_gemm(ADense<float>{q->dac, nullptr, H}, BTransposed{wc, H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 1, nullptr, 0}, R, H, H, false, st);
+  LAUNCH_CHECK();
+  rc = net_backward_impl(fc1, b.obs, nullptr, R, st, BackwardOpts(one, 1));
+  if (rc) return rc;
+  // clip_by_norm per variable + centred RMSProp over the eval set, then the nets' weight blobs
+  rc = adam_step_impl(opt, fc1->params, fc1->grads, 1.f, st, nullptr);
+  for (xtb_net* nt : {fc1, fc2, hyp}) if (!rc) rc = xtb_net_sync_weights(nt, st);
+  return rc;
+}
+
+extern "C" int xtb_qmix_train(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qmix_batch* batch, float* loss_out, int use_graph,
+                              void* stream) {
+  const char* fn = "xtb_qmix_train";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  const bool missing = !opt || !target || !batch || !loss_out || !batch->obs || !batch->seq_len || !batch->avail || !batch->actions ||
+                       !batch->state || !batch->next_state || !batch->reward || !batch->terminated || !batch->mask;
+  if (int rc = learner_check(fn, missing, q->fc1, opt, q->R, false, q->R, q->n_params)) return rc;
+  if (!opt->mg) return fail(XTB_ERR_ARG, "%s: the optimiser must be centred RMSProp (xtb_opt_use_rmsprop)", fn);
+  const xtb_qmix_batch b = *batch;
+  return run_graph(capture_key(kQmixTrain, {q->fc1, q->fc2, q->hyp, q, opt}, q, target, b.obs, b.seq_len, b.avail, b.actions, b.state,
+                               b.next_state, b.reward, b.terminated, b.mask, loss_out),
+                   use_graph, stream, [&](void* st) { return qmix_train_launch(q, opt, target, b, loss_out, S(st)); });
+}
+
+extern "C" int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
+  const char* fn = "xtb_qmix_infer";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, q->fc1, nullptr, q->n, true)) return rc;
+  return run_graph(capture_key(kQmixInfer, {q->fc1, q->fc2, q->hyp, q}, q, explore, obs, hidden, q_out), use_graph, stream,
+                   [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    int rc = qmix_agent_forward(q, explore, obs, q->n, 1, q->ones, hidden, hidden, 0, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(q->fc2, 1), (size_t)q->n * q->A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return XTB_OK;
+  });
 }
 
 // Dueling head that the fused TD step covers: q_tensor combines two linear dense layers that read the same hidden

@@ -6,3 +6,4 @@ from .dqn import DqnCnn, DqnMlp  # noqa: F401
 from .impala_mlp import ImpalaMlp  # noqa: F401
 from .impala_cnn import ImpalaCnn  # noqa: F401
 from .muzero import MuzeroCnn, MuzeroMlp, MuzeroModel  # noqa: F401
+from .qmix import QMixModel  # noqa: F401
