@@ -487,7 +487,7 @@ int xtb_muzero_search(xtb_muzero* mz, xtb_muzero_tree* tree, const void* obs, in
  * slices are allowed) and of a gradient buffer with the same layout; the optimiser spans the set (per-tensor clipping:
  * one segment per variable).  Target and explore sets are caller buffers with the same layout (an explore set needs
  * only the agent part).
- * Limits (XTB_ERR_ARG otherwise, at create): 1 <= H with the GRU kernels' shared-memory plan fitting (H <= 128),
+ * Limits (XTB_ERR_ARG otherwise, at create): 1 <= H with the GRU kernels' shared-memory plan fitting (H <= 137),
  * n_agents <= 32, n_actions <= 255 (the reference casts actions to uint8), mixing embed E <= 128. */
 typedef struct xtb_qmix xtb_qmix;
 typedef struct xtb_qmix_desc {

@@ -76,6 +76,16 @@ def first_argmax(x):
     return torch.where(x == mx, idx, x.shape[-1]).min(-1).values
 
 
+def count_ties(q, avail, mask):
+    """Masked-in (episode, step t, agent) rows whose step t + 1 Q values (q [B, T, n, A], avail [B, T, n, A], mask
+    [B, T - 1]) have two or more available actions at the maximum over the available ones: the rows where the TD
+    target's argmax (double Q) or max has a tie to break."""
+    q, av = np.asarray(q)[:, 1:], np.asarray(avail)[:, 1:] > 0
+    q = np.where(av, q, -np.inf)
+    at_max = av & (q == q.max(-1, keepdims=True))
+    return int(((at_max.sum(-1) >= 2) & (np.asarray(mask)[..., None] > 0)).sum())
+
+
 def td_loss(w, wt, batch, gamma, double_q):
     """The loss of build_train_graph on a host batch (dict of arrays, the QMixModel.train arguments)."""
     obs, avail = _t(batch["obs"]), _t(batch["avail"])

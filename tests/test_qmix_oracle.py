@@ -45,17 +45,36 @@ def test_outputs_past_the_sequence_length_are_zero():
     with orc.precision("f64"):
         wt = {k: qo._t(v) for k, v in w.items()}
         obs = qo._t(rng.normal(size=(2, 6, 2, 5)))
-        q, _ = qo.agent_forward(wt, obs, [4, 4, 2, 2])
-        q = q.numpy()
+        h0 = qo._t(rng.normal(size=(4, 4)))
+        q, hT = qo.agent_forward(wt, obs, [4, 4, 2, 0], h0)     # sequence b n + a: episode 1's agent 1 has length 0
+        q, hT, h0 = q.numpy(), hT.numpy(), h0.numpy()
     bias = w["dense_1/bias"]
     np.testing.assert_allclose(q[0, 4:], np.broadcast_to(bias, q[0, 4:].shape), rtol=0, atol=0)
     np.testing.assert_allclose(q[1, 2:], np.broadcast_to(bias, q[1, 2:].shape), rtol=0, atol=0)
-    assert np.abs(q[0, :4] - bias).max() > 1e-3
+    np.testing.assert_allclose(q[1, :, 1], np.broadcast_to(bias, q[1, :, 1].shape), rtol=0, atol=0)
+    assert np.abs(q[0, :4] - bias).max() > 1e-3 and np.abs(q[1, :2, 0] - bias).max() > 1e-3
+    np.testing.assert_array_equal(hT[3], h0[3])
+    assert np.abs(hT[:3] - h0[:3]).max() > 1e-3
 
 
 def test_double_q_argmax_ties_go_to_the_lowest_index():
     x = torch.tensor([[1.0, 3.0, 3.0, -999999.0], [-999999.0, -999999.0, -999999.0, -999999.0], [2.0, 0.0, 2.0, 5.0]])
     assert qo.first_argmax(x).tolist() == [1, 0, 3]
+
+
+def test_count_ties_counts_available_maxima_of_the_next_step_on_masked_in_rows():
+    q = np.zeros((1, 3, 2, 4))
+    avail = np.ones((1, 3, 2, 4))
+    q[0, 1, 0] = [5, 5, 1, 0]                          # step 0, agent 0: tie
+    q[0, 1, 1] = [5, 5, 9, 0]
+    avail[0, 1, 1, 2] = 0                              # agent 1: the 9 is unavailable, so 5 and 5 tie
+    q[0, 2, 0] = [1, 7, 7, 7]
+    avail[0, 2, 0, 1:3] = 0                            # step 1, agent 0: one 7 left available, no tie
+    q[0, 2, 1] = [2, 2, 0, 0]                          # step 1, agent 1: tie, but the row is masked out below
+    assert qo.count_ties(q, avail, np.array([[1.0, 1.0]])) == 3
+    assert qo.count_ties(q, avail, np.array([[1.0, 0.0]])) == 2
+    avail[0, 1] = 0                                    # all unavailable (padding): nothing to break
+    assert qo.count_ties(q, avail, np.array([[1.0, 0.0]])) == 0
 
 
 def test_loss_gradient_matches_finite_differences():

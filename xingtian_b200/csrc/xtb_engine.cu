@@ -2657,8 +2657,10 @@ extern "C" int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyp, const x
   std::vector<int32_t> ones(n, 1);
   e = cudaMemset(q->buf, 0, tot * sizeof(float));
   if (e == cudaSuccess) e = cudaMemcpy(q->ones, ones.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q->smem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q->smem);
+  // The opt-in is a property of the kernel, shared by every live object: it is set to the most any object may use
+  // (this object's smem would shrink it under an earlier object with a wider GRU or more sequences per CTA).
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
   if (e != cudaSuccess) { cudaFree(q->buf); delete q; return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
   *out = q;
   return XTB_OK;
