@@ -272,6 +272,11 @@ int xtb_adam_set_decay(xtb_adam* opt, float decay);
  * mean-square slot and `mean_grad` (count floats, 16-byte aligned) the mean-gradient slot; this call sets them to
  * ones / zeros as TF initialises them; `v` is unused.  Clipping, chunking and the weight-blob refresh are those of the Adam step. */
 int xtb_opt_use_rmsprop(xtb_adam* opt, float* mean_grad, float decay, float epsilon);
+/* Switch the optimiser handle to tf.train.RMSPropOptimizer(lr, decay, epsilon) with its defaults centered=False and
+ * momentum 0: ms = decay ms + (1 - decay) g^2, theta -= lr g / sqrt(ms + epsilon).  The `m` buffer of xtb_adam_create
+ * becomes the `rms` slot, set to ones here as TF initialises it; `v` is unused.  Clipping, chunking and the weight-blob
+ * refresh are those of the Adam step. */
+int xtb_opt_use_rmsprop_plain(xtb_adam* opt, float decay, float epsilon);
 
 /* ---- fused learner loops -------------------------------------------------------- */
 /* use_graph != 0 (xtb_ppo_train, xtb_impala_train, xtb_dqn_train, xtb_ppo_rollout_infer and xtb_ppo_predict_host built
@@ -526,6 +531,71 @@ int xtb_qmix_train(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qm
  * `explore` on obs [n_agents, obs_dim]; hidden [n_agents, H] is read as the state and overwritten with the new one;
  * q_out [n_agents, A]. */
 int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream);
+
+/* ---- SCC: replaces SCCModel's train and explore graphs (xt/model/scc/scc_tf.py:195-707) -----------------------------
+ * The agent network and its explore step are QMIX's (above): fc1 / GRU / fc2 in the same layout, with the same limits
+ * on H, n_agents and n_actions.  A weight set is one flat float buffer [fc1 | GRU | fc2 | critic nets | head]:
+ *   - multi-channel critic (enable_critic_multi_channel, scc_tf.py:290-313): one net per agent group, in group order,
+ *     each dense(U, relu) -> dense(U, relu) on one agent's (obs, one-hot action) slice of D = o + A floats (o = obs_shape
+ *     - n_actions - n_agents, the raw observation width); the head kernel is [n_agents U, 1] (concat) or [U, 1] (add);
+ *   - single-channel critic (scc_tf.py:283-289): one net dense(U, relu) -> dense(U, relu) on the n_agents D row and a
+ *     [U, 1] head kernel;
+ *   then the head bias [1], at float offset head_off (a multiple of 4).  The nets are bound to their slices (in this order,
+ *   each starting at a multiple of 4 floats) of the eval set and of a gradient buffer with the same layout.  The target
+ *   set has the same layout (only its critic part is read: the reference has no target agent); an explore set needs only
+ *   the agent part.
+ * Limits (XTB_ERR_ARG at create, before any launch): those of QMIX's agent (H <= 137, n_agents <= 32, n_actions <= 255);
+ * 1 <= U <= 512 (dense_unit_number); 0 <= n_groups <= 8 with every group non-empty and the groups summing to n_agents
+ * (the reference's reshape would not fit otherwise); channel_merge 0 (concat) or 1 (add); mc_sample_times >= 1 when
+ * n_agents > 2; critic nets holding B L group-size rows (multi-channel) or B L V rows (single-channel, V below). */
+typedef struct xtb_scc xtb_scc;
+#define XTB_SCC_MAX_GROUPS 8
+typedef struct xtb_scc_desc {
+  int32_t batch;            /* B episodes per training batch */
+  int32_t episode_limit;    /* L */
+  int32_t n_agents;
+  int32_t n_groups;         /* 0: single-channel critic; else the multi-channel critic's group count */
+  int32_t group[XTB_SCC_MAX_GROUPS];   /* agents per group (agent_group_dict, scc_tf.py:56-60) */
+  int32_t channel_merge;    /* 0 concat, 1 add */
+  int32_t mc_sample_times;
+  float gamma;
+  long long gru_off;        /* offset (floats) of gates/kernel in a weight set */
+  long long head_off;       /* offset (floats) of the critic head's kernel */
+} xtb_scc_desc;
+/* critic: n_groups nets (1 when n_groups = 0) */
+int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic, const xtb_scc_desc* desc, xtb_scc** out);
+void xtb_scc_destroy(xtb_scc* q);
+typedef struct xtb_scc_batch {
+  const float* obs;         /* [B, L+1, n_agents, obs_dim] agent inputs */
+  const float* raw_obs;     /* [B, L+1, n_agents, o] batch["obs"]; steps t < L build the critic states */
+  const int32_t* seq_len;   /* [B n_agents] GRU sequence lengths, read at run time, clamped to [0, L+1] */
+  const int32_t* actions;   /* [B, L, n_agents] taken actions in [0, A) */
+  const float* reward;      /* [B, L] */
+  const float* terminated;  /* [B, L] */
+  const float* mask;        /* [B, L] */
+  const uint32_t* subsets;  /* [n_agents, mc_sample_times] agent bitmasks of the Monte-Carlo subsets (scc_tf.py:665-668);
+                               read by the single-channel critic with n_agents > 2 only (else may be NULL) */
+} xtb_scc_batch;
+/* SCCModel.train (scc_tf.py:535-564 with the graph of 321-448) as one step:
+ *   - critic states s[b, t] = concat_a [raw_obs[b, t, a], one_hot(actions[b, t, a])], t < L, read shifted as the
+ *     reference's alias leaves them: s'[b, t] = s[b, min(t + 1, L - 1)] for every critic evaluation;
+ *   - the eval agent over all B (L+1) n_agents rows; the eval and target critics on s';
+ *   - credits from the eval critic before the update: n_agents <= 2, V(s') - V(s' with agent i's slice zeroed);
+ *     n_agents > 2, the mean over the subsets S of V(s' with the actions of S zeroed) - V(... of S and i zeroed).  In
+ *     multi-channel mode only agent i's channel differs, so this is u_i(s') - u_i(masked), independent of S;
+ *   - mixer loss sum (mask (V - (r + gamma (1 - term) V_target)))^2 / sum mask; actor loss
+ *     sum (mask Q_chosen - mask credit)^2 / (n_agents sum mask);
+ *   - one step of critic_opt (Adam, over [critic nets | head]) and of actor_opt (xtb_opt_use_rmsprop_plain, over
+ *     [fc1 | GRU | fc2]), each clipping every variable by norm or neither (the reference clips both only when
+ *     actor_grad_norm_clip > 0), then the nets' weight refresh.
+ * loss_out[0] = mixer loss, loss_out[1] = actor loss, summed in a fixed order.  XTB_ERR_STATE while a communicator is
+ * installed.  Single-channel critics with n_agents > 2 evaluate 2 n_agents mc_sample_times credit variants per row. */
+int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const float* target, const xtb_scc_batch* batch,
+                  float* loss_out, int use_graph, void* stream);
+/* SCCModel.infer_actions: as xtb_qmix_infer. */
+int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream);
+/* SCCModel.get_mixer_output (scc_tf.py:500-503): v_out[r] = V_eval(states[r]) for states [rows, n_agents D], rows <= B L. */
+int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream);
 
 /* xtb_net_backward that also writes d loss / d observation [batch, obs width] into dobs (overwritten): the data-gradient
  * GEMM of every dense layer that reads the observation, summed in layer order.  Float observations with scale 1 read

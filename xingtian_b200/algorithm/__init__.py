@@ -7,3 +7,4 @@ from .dqn import DQN  # noqa: F401
 from .replay_buffer import ReplayBuffer, DeviceReplayBuffer  # noqa: F401
 from .muzero import Muzero  # noqa: F401
 from .qmix import QMixAlg  # noqa: F401
+from .scc import SCCAlg  # noqa: F401

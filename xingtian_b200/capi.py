@@ -69,6 +69,17 @@ class QmixBatch(C.Structure):
                 ("next_state", C.c_void_p), ("reward", C.c_void_p), ("terminated", C.c_void_p), ("mask", C.c_void_p)]
 
 
+class SccDesc(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("episode_limit", C.c_int32), ("n_agents", C.c_int32), ("n_groups", C.c_int32),
+                ("group", C.c_int32 * 8), ("channel_merge", C.c_int32), ("mc_sample_times", C.c_int32), ("gamma", C.c_float),
+                ("gru_off", C.c_longlong), ("head_off", C.c_longlong)]
+
+
+class SccBatch(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("raw_obs", C.c_void_p), ("seq_len", C.c_void_p), ("actions", C.c_void_p), ("reward", C.c_void_p),
+                ("terminated", C.c_void_p), ("mask", C.c_void_p), ("subsets", C.c_void_p)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "xtb_version": (C.c_int, []),
@@ -122,6 +133,7 @@ _SIGS = {
     "xtb_adam_set_lr": (C.c_int, [_P, C.c_float]),
     "xtb_adam_set_decay": (C.c_int, [_P, C.c_float]),
     "xtb_opt_use_rmsprop": (C.c_int, [_P, _P, C.c_float, C.c_float]),
+    "xtb_opt_use_rmsprop_plain": (C.c_int, [_P, C.c_float, C.c_float]),
     "xtb_ppo_train": (C.c_int, [_P, _P, C.POINTER(PpoRollout), C.c_int, C.c_int, C.c_int, _P, C.POINTER(PpoHyper),
                                 C.c_int, C.c_int, C.c_int, _P, C.c_int, _P]),
     "xtb_ppo_rollout_infer": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P,
@@ -144,6 +156,11 @@ _SIGS = {
     "xtb_qmix_destroy": (None, [_P]),
     "xtb_qmix_train": (C.c_int, [_P, _P, _P, C.POINTER(QmixBatch), _P, C.c_int, _P]),
     "xtb_qmix_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_scc_create": (C.c_int, [_P, _P, C.POINTER(_P), C.POINTER(SccDesc), C.POINTER(_P)]),
+    "xtb_scc_destroy": (None, [_P]),
+    "xtb_scc_train": (C.c_int, [_P, _P, _P, _P, C.POINTER(SccBatch), _P, C.c_int, _P]),
+    "xtb_scc_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_scc_critic": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, _P]),
     "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

@@ -157,6 +157,9 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
 // tf.train.RMSPropOptimizer(lr, decay, epsilon, centered=True), momentum 0 (xt/model/impala/impala_cnn_opt.py:205-206):
 //   mg = rho mg + (1 - rho) g;  ms = rho ms + (1 - rho) g^2;  theta -= lr g / sqrt(ms - mg^2 + eps)
 // (TF initialises ms to ONES, mg to zeros).  Same chunking, clip scales and weight-blob refresh as adam_kernel.
+// CENTRED = false is tf.train.RMSPropOptimizer's default (centered=False, momentum 0): ms as above and
+// theta -= lr g / sqrt(ms + eps); mg is not read.
+template <bool CENTRED>
 __global__ void __launch_bounds__(OPT_THREADS)
 rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ ms, float* __restrict__ mg,
                const int* __restrict__ blk_seg, const long long* __restrict__ blk_beg, const int* __restrict__ blk_len,
@@ -172,28 +175,38 @@ rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __rest
     const long long j = beg + i;
     const float4 g4 = *reinterpret_cast<const float4*>(g + j);
     const float4 s4 = *reinterpret_cast<const float4*>(ms + j);
-    const float4 a4 = *reinterpret_cast<const float4*>(mg + j);
+    const float4 a4 = CENTRED ? *reinterpret_cast<const float4*>(mg + j) : make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 p4 = *reinterpret_cast<const float4*>(p + j);
     float gg[4] = {g4.x * sc, g4.y * sc, g4.z * sc, g4.w * sc};
     float ss[4] = {s4.x, s4.y, s4.z, s4.w}, aa[4] = {a4.x, a4.y, a4.z, a4.w}, pp[4] = {p4.x, p4.y, p4.z, p4.w};
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      aa[q] = rho * aa[q] + (1.f - rho) * gg[q];
       ss[q] = rho * ss[q] + (1.f - rho) * gg[q] * gg[q];
-      pp[q] -= lr * gg[q] / sqrtf(ss[q] - aa[q] * aa[q] + rms_eps);
+      if (CENTRED) {
+        aa[q] = rho * aa[q] + (1.f - rho) * gg[q];
+        pp[q] -= lr * gg[q] / sqrtf(ss[q] - aa[q] * aa[q] + rms_eps);
+      } else {
+        pp[q] -= lr * gg[q] / sqrtf(ss[q] + rms_eps);
+      }
     }
     *reinterpret_cast<float4*>(ms + j) = make_float4(ss[0], ss[1], ss[2], ss[3]);
-    *reinterpret_cast<float4*>(mg + j) = make_float4(aa[0], aa[1], aa[2], aa[3]);
+    if (CENTRED) *reinterpret_cast<float4*>(mg + j) = make_float4(aa[0], aa[1], aa[2], aa[3]);
     *reinterpret_cast<float4*>(p + j) = make_float4(pp[0], pp[1], pp[2], pp[3]);
     if (w_hi) bp::blob_store4(bsegs, n_bsegs, w_hi, w_lo_off, j, pp);
   }
   for (int i = nv + threadIdx.x; i < n; i += OPT_THREADS) {
     const long long j = beg + i;
     const float gg = g[j] * sc;
-    const float aa = rho * mg[j] + (1.f - rho) * gg;
     const float ss = rho * ms[j] + (1.f - rho) * gg * gg;
-    mg[j] = aa; ms[j] = ss;
-    const float pn = p[j] - lr * gg / sqrtf(ss - aa * aa + rms_eps);
+    ms[j] = ss;
+    float pn;
+    if (CENTRED) {
+      const float aa = rho * mg[j] + (1.f - rho) * gg;
+      mg[j] = aa;
+      pn = p[j] - lr * gg / sqrtf(ss - aa * aa + rms_eps);
+    } else {
+      pn = p[j] - lr * gg / sqrtf(ss + rms_eps);
+    }
     p[j] = pn;
     if (w_hi) bp::blob_store1(bsegs, n_bsegs, w_hi, w_lo_off, j, pn);
   }

@@ -17,6 +17,7 @@
 #include "optim.cuh"
 #include "rl_kernels.cuh"
 #include "qmix.cuh"
+#include "scc.cuh"
 #include "stager.cuh"
 #include "bp_gemm.cuh"
 #include "comm.cuh"
@@ -1681,6 +1682,7 @@ struct xtb_adam {
   int clip_mode = 0, n_seg = 0, n_blk = 0;
   float *m = nullptr, *v = nullptr;
   float* mg = nullptr; float rms_rho = 0.f, rms_eps = 0.f;   // centred RMSProp instead of Adam when mg != NULL (m = ms)
+  bool rms_plain = false;                                    // uncentred RMSProp instead of Adam (m = ms, mg unused)
   int* blk_seg = nullptr; long long* blk_beg = nullptr; int* blk_len = nullptr;
   double* norm_sq = nullptr; float* seg_scale = nullptr; AdamState* st = nullptr; AdamHyper* hyp = nullptr; unsigned int* ticket = nullptr;
 };
@@ -1773,8 +1775,8 @@ static int adam_step_impl(xtb_adam* o, float* params, const float* grads, float 
           (const AdamHyper*)o->hyp, o->seg_scale, o->n_seg, o->clip_mode, grad_scale);
   LAUNCH_CHECK();
   const bool blobs = net && !net->blob_segs.empty();
-  if (o->mg) {
-    XLAUNCH(rmsprop_kernel, o->n_blk, OPT_THREADS, 0, st, params, grads, o->m, o->mg, o->blk_seg, o->blk_beg, o->blk_len,
+  if (o->mg || o->rms_plain) {
+    XLAUNCH(o->mg ? rmsprop_kernel<true> : rmsprop_kernel<false>, o->n_blk, OPT_THREADS, 0, st, params, grads, o->m, o->mg, o->blk_seg, o->blk_beg, o->blk_len,
             o->seg_scale, (const AdamHyper*)o->hyp, o->rms_rho, o->rms_eps, blobs ? (const bp::BlobSeg*)(net->ws + net->segs_off) : nullptr,
             blobs ? (int)net->blob_segs.size() : 0, blobs ? (__nv_bfloat16*)(net->ws + net->blob_off) : nullptr, blobs ? net->blob_elems : 0LL);
     LAUNCH_CHECK();
@@ -1799,7 +1801,19 @@ extern "C" int xtb_opt_use_rmsprop(xtb_adam* o, float* mean_grad, float decay, f
     CUDA_TRY(cudaMemcpy(o->m, ones.data(), ones.size() * sizeof(float), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemset(mean_grad, 0, ones.size() * sizeof(float)));
   }
-  o->mg = mean_grad; o->rms_rho = decay; o->rms_eps = epsilon;
+  o->mg = mean_grad; o->rms_rho = decay; o->rms_eps = epsilon; o->rms_plain = false;
+  return XTB_OK;
+}
+extern "C" int xtb_opt_use_rmsprop_plain(xtb_adam* o, float decay, float epsilon) {
+  if (!o) return fail(XTB_ERR_ARG, "xtb_opt_use_rmsprop_plain: null pointer");
+  if (!(decay > 0.f && decay < 1.f) || !(epsilon > 0.f)) return fail(XTB_ERR_ARG, "xtb_opt_use_rmsprop_plain: decay in (0,1), epsilon > 0");
+  drop_graphs_of(o);
+  {   // the `rms` slot of tf.train.RMSPropOptimizer starts at ones (one-time, synchronous)
+    std::vector<float> ones((size_t)o->count, 1.f);
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(o->m, ones.data(), ones.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  o->mg = nullptr; o->rms_rho = decay; o->rms_eps = epsilon; o->rms_plain = true;
   return XTB_OK;
 }
 extern "C" int xtb_adam_set_lr(xtb_adam* o, float lr) {
@@ -1862,7 +1876,8 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // zeroes it and fills the entry point, the owners and the arguments; run_graph() adds the communicator and the
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
-                kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer };
+                kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
+                kSccTrain, kSccInfer, kSccCritic };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -2674,9 +2689,12 @@ extern "C" void xtb_qmix_destroy(xtb_qmix* q) {
   delete q;
 }
 
+// The agent network (fc1 -> GRU -> fc2) is shared by QMIX and SCC: Q is xtb_qmix or xtb_scc, which both carry the nets,
+// the agent widths and the agent scratch under the same names.
 // fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding
 // S = rows / T sequences of T steps; the Q values stay in fc2's output tensor.  h0 / hT: see qmix_gru_fwd_kernel.
-static int qmix_agent_forward(xtb_qmix* q, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
+template <class Q>
+static int qmix_agent_forward(Q* q, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
                               float* hT, int store, cudaStream_t st) {
   const int H = q->H;
   const float* W = P ? P : q->fc1->params;
@@ -2696,6 +2714,51 @@ static int qmix_agent_forward(xtb_qmix* q, const float* P, const float* obs, int
           q->n, H, G, store);
   LAUNCH_CHECK();
   return net_forward_impl(q->fc2, P ? P + q->o_fc2 : nullptr, q->hout, nullptr, rows, st, 0u, 1u << 1);
+}
+
+// Backward of qmix_agent_forward (store = 1, the eval set, all R rows) from d loss / d Q in fc2's output gradient: fc2
+// (with d loss / d GRU output), the GRU in reverse time, its weight gradients as GEMMs over all rows, fc1.
+template <class Q>
+static int qmix_agent_backward(Q* q, const float* obs, const int32_t* seq_len, cudaStream_t st) {
+  const int H = q->H, R = q->R, n = q->n;
+  const int32_t one[1] = {1};
+  BackwardOpts o2(one, 1);
+  o2.dobs = q->dy;
+  int rc = net_backward_impl(q->fc2, q->hout, nullptr, R, st, o2);
+  if (rc) return rc;
+  const float* W = q->fc1->params;
+  const float *wg = W + q->o_gru, *wc = wg + 2 * H * 2 * H + 2 * H;
+  float* gg = q->fc1->grads + q->o_gru;
+  float* gc = gg + 2 * H * 2 * H + 2 * H;
+  const int S = q->S, G = q->G;
+  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, (const float*)q->xg, (const float*)q->xc,
+          (const float*)q->hout, (const float*)q->dy, q->dag, q->dac, seq_len, S, q->T, q->n, H, G);
+  LAUNCH_CHECK();
+  const float* x = xtb_net_tensor(q->fc1, 1);
+  // [kernel; bias] gradients: [x | h_prev | 1]^T da_gates and [x | r h_prev | 1]^T da_candidate over all rows
+  launch_gemm(AGruFeat{x, q->hout, H, n, q->T, 1}, BRowMajor{q->dag, 2 * H}, EpiDgrad{gg, gg, 0, 2 * H, 0, nullptr, 0}, 2 * H + 1, 2 * H,
+              R, false, st);
+  LAUNCH_CHECK();
+  launch_gemm(AGruFeat{x, q->rh, H, n, q->T, 0}, BRowMajor{q->dac, H}, EpiDgrad{gc, gc, 0, H, 0, nullptr, 0}, 2 * H + 1, H, R, false, st);
+  LAUNCH_CHECK();
+  // d loss / d fc1 pre-activation = relu'(x) (da_gates W_g[:H]^T + da_candidate W_c[:H]^T)
+  float* dx = xtb_net_tensor_grad(q->fc1, 1);
+  launch_gemm(ADense<float>{q->dag, nullptr, 2 * H}, BTransposed{wg, 2 * H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 0, nullptr, 0}, R, H, 2 * H,
+              false, st);
+  LAUNCH_CHECK();
+  launch_gemm(ADense<float>{q->dac, nullptr, H}, BTransposed{wc, H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 1, nullptr, 0}, R, H, H, false, st);
+  LAUNCH_CHECK();
+  return net_backward_impl(q->fc1, obs, nullptr, R, st, BackwardOpts(one, 1));
+}
+
+// One step of the agent for one environment: fc1 -> GRU -> fc2 of the weight set `explore` on obs [n, obs_dim], hidden
+// [n, H] read and overwritten, q_out [n, A]
+template <class Q>
+static int qmix_agent_step(Q* q, const float* explore, const float* obs, float* hidden, float* q_out, cudaStream_t st) {
+  int rc = qmix_agent_forward(q, explore, obs, q->n, 1, q->ones, hidden, hidden, 0, st);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(q->fc2, 1), (size_t)q->n * q->A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return XTB_OK;
 }
 
 static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qmix_batch& b, float* loss_out, cudaStream_t st) {
@@ -2731,37 +2794,11 @@ static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, co
   LAUNCH_CHECK();
   XLAUNCH(qmix_loss_kernel, 1, 32, 0, st, (const float*)q->part, q->n_part, (const float*)msum, loss_out);
   LAUNCH_CHECK();
-  // backward: the hypernetworks, fc2 (with d loss / d GRU output), the GRU in reverse time, its weight gradients, fc1
-  const int32_t hheads[4] = {kQw1, kQb1, kQwf, kQv}, one[1] = {1};
+  // backward: the hypernetworks, then the agent
+  const int32_t hheads[4] = {kQw1, kQb1, kQwf, kQv};
   rc = net_backward_impl(hyp, b.state, nullptr, BL, st, BackwardOpts(hheads, 4));
   if (rc) return rc;
-  BackwardOpts o2(one, 1);
-  o2.dobs = q->dy;
-  rc = net_backward_impl(fc2, q->hout, nullptr, R, st, o2);
-  if (rc) return rc;
-  const float* W = fc1->params;
-  const float *wg = W + q->o_gru, *wc = wg + 2 * H * 2 * H + 2 * H;
-  float* gg = fc1->grads + q->o_gru;
-  float* gc = gg + 2 * H * 2 * H + 2 * H;
-  const int S = q->S, G = q->G;
-  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, (const float*)q->xg, (const float*)q->xc,
-          (const float*)q->hout, (const float*)q->dy, q->dag, q->dac, b.seq_len, S, q->T, n, H, G);
-  LAUNCH_CHECK();
-  const float* x = xtb_net_tensor(fc1, 1);
-  // [kernel; bias] gradients: [x | h_prev | 1]^T da_gates and [x | r h_prev | 1]^T da_candidate over all rows
-  launch_gemm(AGruFeat{x, q->hout, H, n, q->T, 1}, BRowMajor{q->dag, 2 * H}, EpiDgrad{gg, gg, 0, 2 * H, 0, nullptr, 0}, 2 * H + 1, 2 * H,
-              R, false, st);
-  LAUNCH_CHECK();
-  launch_gemm(AGruFeat{x, q->rh, H, n, q->T, 0}, BRowMajor{q->dac, H}, EpiDgrad{gc, gc, 0, H, 0, nullptr, 0}, 2 * H + 1, H, R, false, st);
-  LAUNCH_CHECK();
-  // d loss / d fc1 pre-activation = relu'(x) (da_gates W_g[:H]^T + da_candidate W_c[:H]^T)
-  float* dx = xtb_net_tensor_grad(fc1, 1);
-  launch_gemm(ADense<float>{q->dag, nullptr, 2 * H}, BTransposed{wg, 2 * H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 0, nullptr, 0}, R, H, 2 * H,
-              false, st);
-  LAUNCH_CHECK();
-  launch_gemm(ADense<float>{q->dac, nullptr, H}, BTransposed{wc, H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 1, nullptr, 0}, R, H, H, false, st);
-  LAUNCH_CHECK();
-  rc = net_backward_impl(fc1, b.obs, nullptr, R, st, BackwardOpts(one, 1));
+  rc = qmix_agent_backward(q, b.obs, b.seq_len, st);
   if (rc) return rc;
   // clip_by_norm per variable + centred RMSProp over the eval set, then the nets' weight blobs
   rc = adam_step_impl(opt, fc1->params, fc1->grads, 1.f, st, nullptr);
@@ -2788,11 +2825,272 @@ extern "C" int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* ob
   if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
   if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, q->fc1, nullptr, q->n, true)) return rc;
   return run_graph(capture_key(kQmixInfer, {q->fc1, q->fc2, q->hyp, q}, q, explore, obs, hidden, q_out), use_graph, stream,
-                   [&](void* sv) -> int {
-    cudaStream_t st = S(sv);
-    int rc = qmix_agent_forward(q, explore, obs, q->n, 1, q->ones, hidden, hidden, 0, st);
+                   [&](void* st) { return qmix_agent_step(q, explore, obs, hidden, q_out, S(st)); });
+}
+
+// ---- SCC (xt/model/scc/scc_tf.py) ------------------------------------------------------------------------------------
+// The agent is QMIX's (qmix_agent_forward / _backward / _step); the critic's hidden layers are engine nets, one per agent
+// group (multi-channel) or one over the whole row, bound to slices of the eval set; the target critic is read through
+// their foreign-parameter forward.  See scc.cuh for the critic layout.
+struct xtb_scc {
+  xtb_net *fc1 = nullptr, *fc2 = nullptr;
+  xtb_net* cn[SCC_MAX_GROUPS] = {};
+  xtb_scc_desc d{};
+  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, R = 0, BL = 0, S = 0, G = 0;
+  int ncn = 0, multi = 0, concat = 0, U = 0, D = 0, o = 0, mc = 1, V = 0, C = 0, K = 0, n_part = 0, n_chunk = 0;
+  int a0[SCC_MAX_GROUPS + 1] = {};
+  size_t smem = 0;
+  long long o_gru = 0, o_fc2 = 0, o_mix = 0, o_head = 0, o_cn[SCC_MAX_GROUPS] = {}, agent_size = 0, n_params = 0;
+  float* buf = nullptr;
+  float *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr;
+  float *xs = nullptr, *xm = nullptr, *ht = nullptr, *hm = nullptr, *dv = nullptr, *part = nullptr, *hpart = nullptr;
+  int32_t* ones = nullptr;
+};
+
+// critic rows of group j (channel rows of the multi-channel critic, whole rows of the single-channel one) for `rows` states
+static inline long long scc_rows(const xtb_scc* q, int j, long long rows) { return q->multi ? rows * (q->a0[j + 1] - q->a0[j]) : rows; }
+// SccH over a group-major buffer of `rows` states, U floats per channel row
+static SccH scc_groups(const xtb_scc* q, const float* base, long long rows, int width) {
+  SccH h{};
+  h.ng = q->ncn;
+  for (int j = 0; j <= q->ncn; j++) h.a0[j] = q->a0[j];
+  for (int j = 0; j < q->ncn; j++) h.h[j] = base + (q->multi ? rows * q->a0[j] : 0) * width;
+  return h;
+}
+// SccH over the nets' own second-layer outputs (or their gradients)
+static SccH scc_nets(const xtb_scc* q, bool grad) {
+  SccH h{};
+  h.ng = q->ncn;
+  for (int j = 0; j <= q->ncn; j++) h.a0[j] = q->a0[j];
+  for (int j = 0; j < q->ncn; j++) h.h[j] = grad ? xtb_net_tensor_grad(q->cn[j], 2) : xtb_net_tensor(q->cn[j], 2);
+  return h;
+}
+
+extern "C" int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic, const xtb_scc_desc* desc, xtb_scc** out) {
+  const char* fn = "xtb_scc_create";
+  if (!fc1 || !fc2 || !critic || !desc || !out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  const xtb_scc_desc& d = *desc;
+  const int n = d.n_agents;
+  if (n < 1 || n > QM_MAX_AGENTS) return fail(XTB_ERR_ARG, "%s: n_agents %d not in [1, %d]", fn, n, QM_MAX_AGENTS);
+  if (d.n_groups < 0 || d.n_groups > SCC_MAX_GROUPS) return fail(XTB_ERR_ARG, "%s: n_groups %d not in [0, %d]", fn, d.n_groups, SCC_MAX_GROUPS);
+  const int ncn = d.n_groups ? d.n_groups : 1;
+  int a0[SCC_MAX_GROUPS + 1] = {0};
+  if (d.n_groups) {
+    for (int j = 0; j < d.n_groups; j++) {
+      if (d.group[j] < 1) return fail(XTB_ERR_ARG, "%s: group %d has %d agents", fn, j, d.group[j]);
+      a0[j + 1] = a0[j] + d.group[j];
+    }
+    if (a0[d.n_groups] != n) return fail(XTB_ERR_ARG, "%s: the groups hold %d agents, not n_agents %d", fn, a0[d.n_groups], n);
+  } else {
+    a0[1] = 1;
+  }
+  if (d.n_groups && d.channel_merge != 0 && d.channel_merge != 1)
+    return fail(XTB_ERR_ARG, "%s: channel_merge %d is neither concat (0) nor add (1)", fn, d.channel_merge);
+  if (n > 2 && d.mc_sample_times < 1) return fail(XTB_ERR_ARG, "%s: mc_sample_times %d < 1", fn, d.mc_sample_times);
+  if (d.batch < 1 || d.episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, d.batch, d.episode_limit);
+  for (xtb_net* nt : {fc1, fc2})
+    if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  for (int j = 0; j < ncn; j++)
+    if (!critic[j] || !critic[j]->ws || !critic[j]->params || !critic[j]->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  auto dense = [](const xtb_net* nt, int i, int src, int act) {
+    const LayerPlan& lp = nt->L[i];
+    return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
+  };
+  if (fc1->L.size() != 1 || !dense(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
+    return fail(XTB_ERR_ARG, "%s: fc1 must be one relu dense layer on float agent inputs", fn);
+  const int H = fc1->tsize[1];
+  if (fc2->L.size() != 1 || !dense(fc2, 0, 0, XTB_ACT_NONE) || fc2->tsize[0] != H)
+    return fail(XTB_ERR_ARG, "%s: fc2 must be one linear dense layer on the %d-wide GRU output", fn, H);
+  if (int rc = input_grad_check(fc2)) return rc;
+  const int A = fc2->tsize[1];
+  if (A < 1 || A > 255) return fail(XTB_ERR_ARG, "%s: n_actions %d not in [1, 255] (actions are uint8 in the reference)", fn, A);
+  const int U = critic[0]->L.empty() ? 0 : critic[0]->tsize[1];
+  const int in_w = critic[0]->tsize[0];
+  const int D = d.n_groups ? in_w : in_w / n, o = D - A;
+  for (int j = 0; j < ncn; j++) {
+    const xtb_net* c = critic[j];
+    if (c->L.size() != 2 || !dense(c, 0, 0, XTB_ACT_RELU) || !dense(c, 1, 1, XTB_ACT_RELU) || c->desc.input_u8 || c->desc.scale != 1.f ||
+        c->tsize[1] != U || c->tsize[2] != U || c->tsize[0] != in_w)
+      return fail(XTB_ERR_ARG, "%s: every critic net must be dense(U, relu) -> dense(U, relu) on the same float input", fn);
+  }
+  if (U < 1 || U > SCC_MAX_UNITS) return fail(XTB_ERR_ARG, "%s: dense_unit_number %d not in [1, %d]", fn, U, SCC_MAX_UNITS);
+  if (o < 0 || (!d.n_groups && in_w != n * D))
+    return fail(XTB_ERR_ARG, "%s: critic input %d is not n_agents x (obs + n_actions %d)", fn, in_w, A);
+  const long long T = d.episode_limit + 1, R = (long long)d.batch * T * n, BL = (long long)d.batch * d.episode_limit;
+  const int V = d.n_groups ? 0 : (n <= 2 ? n : 2 * n * d.mc_sample_times);
+  if (R > (1LL << 30) / std::max(3 * H, 1) || BL * n * std::max(D, U) * std::max(V, 1) > (1LL << 30))
+    return fail(XTB_ERR_ARG, "%s: batch too large", fn);
+  if (fc1->max_batch < R || fc2->max_batch < R) return fail(XTB_ERR_ARG, "%s: fc1 / fc2 hold fewer rows than a batch (%lld)", fn, R);
+  for (int j = 0; j < ncn; j++) {
+    const long long need = d.n_groups ? BL * (a0[j + 1] - a0[j]) : BL * std::max(V, 1);
+    if (critic[j]->max_batch < need) return fail(XTB_ERR_ARG, "%s: critic net %d holds fewer than %lld rows", fn, j, need);
+  }
+  const int S = d.batch * n;
+  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
+  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
+  if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
+    return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
+  // [fc1 | gru | fc2 | critic nets | head kernel, head bias] in one buffer, the gradients at the same offsets
+  const int C = d.n_groups ? n : 1, concat = d.n_groups ? d.channel_merge == 0 : 1, K = concat ? C * U : U;
+  const long long o_gru = d.gru_off, o_fc2 = fc2->params - fc1->params, gru_n = 2LL * H * 2 * H + 2 * H + 2LL * H * H + H;
+  bool ok = o_gru >= fc1->n_params && o_fc2 >= o_gru + gru_n && fc2->grads == fc1->grads + o_fc2;
+  long long prev = o_fc2 + fc2->n_params, o_cn[SCC_MAX_GROUPS] = {};
+  for (int j = 0; j < ncn && ok; j++) {
+    o_cn[j] = critic[j]->params - fc1->params;
+    ok = o_cn[j] >= prev && critic[j]->grads == fc1->grads + o_cn[j] && o_cn[j] % 4 == 0;
+    prev = o_cn[j] + critic[j]->n_params;
+  }
+  if (!ok || d.head_off < prev || d.head_off % 4 != 0)
+    return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2 | critic nets | head] of one buffer, in order", fn);
+  auto* q = new xtb_scc();
+  q->fc1 = fc1; q->fc2 = fc2; q->d = d;
+  for (int j = 0; j < ncn; j++) { q->cn[j] = critic[j]; q->o_cn[j] = o_cn[j]; }
+  for (int j = 0; j <= ncn; j++) q->a0[j] = a0[j];
+  q->B = d.batch; q->L = d.episode_limit; q->T = (int)T; q->n = n; q->A = A; q->H = H; q->R = (int)R; q->BL = (int)BL;
+  q->S = S; q->G = G; q->smem = qgru_smem_floats(H, G) * 4;
+  q->ncn = ncn; q->multi = d.n_groups > 0; q->concat = concat; q->U = U; q->D = D; q->o = o; q->mc = std::max(1, d.mc_sample_times);
+  q->V = V; q->C = C; q->K = K;
+  q->o_gru = o_gru; q->o_fc2 = o_fc2; q->o_mix = o_cn[0]; q->o_head = d.head_off; q->agent_size = o_fc2 + fc2->n_params;
+  q->n_params = d.head_off + K + 1;
+  q->n_part = (int)((BL + SCC_THREADS / 32 - 1) / (SCC_THREADS / 32));
+  q->n_chunk = (int)((BL + SCC_HG_ROWS - 1) / SCC_HG_ROWS);
+  const long long xm_n = q->multi ? BL * n * D : BL * n * D * V, hm_n = q->multi ? BL * n * U : BL * U * V;
+  const long long sizes[] = {R * 2 * H, R * H, R * H, R * H, R * H, R * 2 * H, R * H, BL * n * D, std::max(xm_n, 1LL), BL * C * U,
+                             std::max(hm_n, 1LL), BL, 2LL * q->n_part + 2, (long long)q->n_chunk * (K + 1), n};
+  float** dst[] = {&q->xg, &q->xc, &q->hout, &q->rh, &q->dy, &q->dag, &q->dac, &q->xs, &q->xm, &q->ht, &q->hm, &q->dv, &q->part,
+                   &q->hpart, (float**)&q->ones};
+  const int n_bufs = (int)(sizeof(sizes) / sizeof(sizes[0]));
+  long long tot = 0;
+  for (long long sz : sizes) tot += (sz + 63) / 64 * 64;
+  cudaError_t e = cudaMalloc(&q->buf, tot * sizeof(float));
+  if (e != cudaSuccess) { delete q; return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e)); }
+  float* p = q->buf;
+  for (int i = 0; i < n_bufs; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
+  std::vector<int32_t> ones(n, 1);
+  e = cudaMemset(q->buf, 0, tot * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemcpy(q->ones, ones.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e != cudaSuccess) { cudaFree(q->buf); delete q; return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  *out = q;
+  return XTB_OK;
+}
+
+extern "C" void xtb_scc_destroy(xtb_scc* q) {
+  if (!q) return;
+  drop_graphs_of(q);
+  cudaDeviceSynchronize();
+  cudaFree(q->buf);
+  delete q;
+}
+
+static unsigned scc_grid(long long total) { return (unsigned)std::min<long long>((total + 255) / 256, 8LL * kSMs); }
+
+static int scc_train_launch(xtb_scc* q, xtb_adam* copt, xtb_adam* aopt, const float* target, const xtb_scc_batch& b, float* loss_out,
+                            cudaStream_t st) {
+  const int n = q->n, A = q->A, U = q->U, BL = q->BL, R = q->R;
+  // critic inputs (shifted), sum of the mask
+  XLAUNCH(scc_inputs_kernel, scc_grid((long long)BL * n * q->D), 256, 0, st, b.raw_obs, b.actions, b.subsets, q->xs, q->xm, q->B, q->L, n,
+          q->o, A, q->multi, q->mc, scc_groups(q, nullptr, BL, q->D));
+  LAUNCH_CHECK();
+  float* msum = q->part + 2 * q->n_part;
+  XLAUNCH(qmix_mask_sum_kernel, 1, QM_THREADS, 0, st, b.mask, BL, msum);
+  LAUNCH_CHECK();
+  // per critic net: the target on the full rows, the eval on the credit rows (both kept), the eval on the full rows
+  const SccH xs = scc_groups(q, q->xs, BL, q->D), xm = scc_groups(q, q->xm, BL, q->D);
+  const SccH ht = scc_groups(q, q->ht, BL, U), hm = scc_groups(q, q->hm, BL, U);
+  for (int j = 0; j < q->ncn; j++) {
+    xtb_net* c = q->cn[j];
+    const long long rows = scc_rows(q, j, BL), mrows = q->multi ? rows : (long long)BL * q->V;
+    int rc = net_forward_impl(c, target + q->o_cn[j], xs.h[j], nullptr, (int)rows, st, 0u, 1u << 2);
     if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(q->fc2, 1), (size_t)q->n * q->A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync((float*)ht.h[j], xtb_net_tensor(c, 2), (size_t)rows * U * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    rc = net_forward_impl(c, nullptr, xm.h[j], nullptr, (int)mrows, st, 0u, 1u << 2);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync((float*)hm.h[j], xtb_net_tensor(c, 2), (size_t)mrows * U * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    rc = net_forward_impl(c, nullptr, xs.h[j], nullptr, (int)rows, st, 0u, 1u << 2);
+    if (rc) return rc;
+  }
+  // the eval agent with the activations of its backward
+  int rc = qmix_agent_forward(q, nullptr, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 1, st);
+  if (rc) return rc;
+  // critic head, TD loss, credits, actor loss and their gradients
+  float* dq = xtb_net_tensor_grad(q->fc2, 1);
+  CUDA_TRY(cudaMemsetAsync(dq, 0, (size_t)R * A * sizeof(float), st));
+  const float* P = q->fc1->params;
+  SccStep sp{scc_nets(q, false), ht, hm, (long long)BL * U, scc_nets(q, true)};
+  XLAUNCH(scc_step_kernel, q->n_part, SCC_THREADS, 0, st, sp, P + q->o_head, target + q->o_head, (const float*)xtb_net_tensor(q->fc2, 1),
+          b.actions, b.reward, b.terminated, b.mask, (const float*)msum, q->B, q->L, n, A, U, q->concat, q->multi, q->mc, q->d.gamma,
+          q->dv, dq, q->part);
+  LAUNCH_CHECK();
+  XLAUNCH(scc_head_grad_kernel, dim3(q->n_chunk, (q->K + 1 + 127) / 128), 128, 0, st, sp.eh, (const float*)q->dv, BL, U, q->concat,
+          q->hpart);
+  LAUNCH_CHECK();
+  XLAUNCH(scc_reduce_kernel, (q->K + 2 + 127) / 128, 128, 0, st, (const float*)q->hpart, q->n_chunk, q->K, q->fc1->grads + q->o_head,
+          (const float*)q->part, q->n_part, (const float*)msum, n, loss_out);
+  LAUNCH_CHECK();
+  // backward: the critic nets, then the agent
+  const int32_t two[1] = {2};
+  for (int j = 0; j < q->ncn; j++) {
+    rc = net_backward_impl(q->cn[j], xs.h[j], nullptr, (int)scc_rows(q, j, BL), st, BackwardOpts(two, 1));
+    if (rc) return rc;
+  }
+  rc = qmix_agent_backward(q, b.obs, b.seq_len, st);
+  if (rc) return rc;
+  // Adam over the critic slice, RMSProp over the agent slice (each with its clip_by_norm), then the nets' weight blobs
+  rc = adam_step_impl(copt, q->fc1->params + q->o_mix, q->fc1->grads + q->o_mix, 1.f, st, nullptr);
+  if (!rc) rc = adam_step_impl(aopt, q->fc1->params, q->fc1->grads, 1.f, st, nullptr);
+  for (int j = 0; j < q->ncn && !rc; j++) rc = xtb_net_sync_weights(q->cn[j], st);
+  for (xtb_net* nt : {q->fc1, q->fc2}) if (!rc) rc = xtb_net_sync_weights(nt, st);
+  return rc;
+}
+
+extern "C" int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const float* target, const xtb_scc_batch* batch,
+                             float* loss_out, int use_graph, void* stream) {
+  const char* fn = "xtb_scc_train";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  const bool missing = !critic_opt || !actor_opt || !target || !batch || !loss_out || !batch->obs || !batch->raw_obs || !batch->seq_len ||
+                       !batch->actions || !batch->reward || !batch->terminated || !batch->mask || (!q->multi && q->n > 2 && !batch->subsets);
+  if (int rc = learner_check(fn, missing, q->fc1, actor_opt, q->R, false, q->R, q->agent_size)) return rc;
+  if (critic_opt->count != q->n_params - q->o_mix)
+    return fail(XTB_ERR_ARG, "%s: critic optimiser size %lld != %lld", fn, critic_opt->count, q->n_params - q->o_mix);
+  if (critic_opt->mg || critic_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the critic optimiser must be Adam", fn);
+  if (!actor_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the actor optimiser must be uncentred RMSProp (xtb_opt_use_rmsprop_plain)", fn);
+  const xtb_scc_batch b = *batch;
+  return run_graph(capture_key(kSccTrain, {q->fc1, q->cn[0], q, critic_opt, actor_opt}, q, target, b.obs, b.raw_obs, b.seq_len,
+                               b.actions, b.reward, b.terminated, b.mask, b.subsets, loss_out),
+                   use_graph, stream, [&](void* st) { return scc_train_launch(q, critic_opt, actor_opt, target, b, loss_out, S(st)); });
+}
+
+extern "C" int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
+  const char* fn = "xtb_scc_infer";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, q->fc1, nullptr, q->n, true)) return rc;
+  return run_graph(capture_key(kSccInfer, {q->fc1, q->fc2, q}, q, explore, obs, hidden, q_out), use_graph, stream,
+                   [&](void* st) { return qmix_agent_step(q, explore, obs, hidden, q_out, S(st)); });
+}
+
+extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream) {
+  const char* fn = "xtb_scc_critic";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (int rc = learner_check(fn, !states || !v_out, q->fc1, nullptr, rows, true, q->BL)) return rc;
+  return run_graph(capture_key(kSccCritic, {q->fc1, q->cn[0], q}, q, states, rows, v_out), use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    const float* in = states;
+    if (q->multi) {
+      XLAUNCH(scc_split_kernel, scc_grid((long long)rows * q->n * q->D), 256, 0, st, states, q->xs, rows, q->n, q->D,
+              scc_groups(q, nullptr, rows, q->D));
+      LAUNCH_CHECK();
+      in = q->xs;
+    }
+    const SccH xs = scc_groups(q, in, rows, q->D);
+    for (int j = 0; j < q->ncn; j++) {
+      int rc = net_forward_impl(q->cn[j], nullptr, xs.h[j], nullptr, (int)scc_rows(q, j, rows), st, 0u, 1u << 2);
+      if (rc) return rc;
+    }
+    XLAUNCH(scc_value_kernel, (rows + SCC_THREADS / 32 - 1) / (SCC_THREADS / 32), SCC_THREADS, 0, st, scc_nets(q, false),
+            (const float*)(q->fc1->params + q->o_head), rows, q->U, q->concat, v_out);
+    LAUNCH_CHECK();
     return XTB_OK;
   });
 }

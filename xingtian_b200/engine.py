@@ -307,8 +307,13 @@ class Adam(object):
         except Exception:
             pass
 
-    def use_rmsprop(self, decay=0.99, epsilon=0.1):
-        """tf.train.RMSPropOptimizer(lr, decay, epsilon, centered=True): mean-square slot starts at ones, mean-gradient at zeros."""
+    def use_rmsprop(self, decay=0.99, epsilon=0.1, centered=True):
+        """tf.train.RMSPropOptimizer(lr, decay, epsilon, centered): mean-square slot starts at ones, mean-gradient (centred
+        only; else None) at zeros."""
+        if not centered:
+            self.mean_grad = None
+            check(self.lib.xtb_opt_use_rmsprop_plain(self.handle, float(decay), float(epsilon)))
+            return
         self.mean_grad = torch.zeros_like(self.net.params)
         check(self.lib.xtb_opt_use_rmsprop(self.handle, _ptr(self.mean_grad), float(decay), float(epsilon)))
 
