@@ -332,7 +332,9 @@ class SCCModel(QMixModel):
         subsets = self.draw_subsets() if n > 2 else None
         b = self._train_buffers()
         stage_h2d(b["obs"], batch_trajectories, np.float32)
-        stage_h2d(b["raw_obs"], raw.reshape(B, L + 1, n, self.o_shape), np.float32)
+        if self.o_shape:
+            # with no raw observation columns the critic states are the one-hot actions alone: nothing reads raw_obs
+            stage_h2d(b["raw_obs"], raw.reshape(B, L + 1, n, self.o_shape), np.float32)
         stage_h2d(b["seq_len"], seq_len, np.int32)
         stage_h2d(b["actions"], act, np.int32)
         stage_h2d(b["reward"], rewards, np.float32)
