@@ -907,10 +907,12 @@ struct DiagGaussian {
 
 // One thread per sample: the draw of DIST from the pi head's output pi [B, A] with noise [B, A] if set, else Philox at
 // `offset`, or at *offset_dev + t_add when offset_dev is set (the device-resident counter of rollout inference, so that
-// CUDA-graph replays draw fresh noise).  log_std: DiagGaussian only.  v_out != NULL: the value head output is copied out
-// alongside.
+// CUDA-graph replays draw fresh noise).  The B rows are consecutive steps of `period` samples (period = B: one step):
+// row b is sample b % period of step b / period and draws at Philox index b % period and offset + b / period, so a
+// row's draw does not depend on how many steps one launch covers.  log_std: DiagGaussian only.  v_out != NULL: the
+// value head output is copied out alongside.
 template <class DIST>
-__global__ void sample_kernel(const float* __restrict__ pi, const float* __restrict__ log_std, int B, int A,
+__global__ void sample_kernel(const float* __restrict__ pi, const float* __restrict__ log_std, int B, int period, int A,
                               const float* __restrict__ noise, uint64_t seed, uint64_t offset,
                               const unsigned long long* __restrict__ offset_dev, int t_add,
                               typename DIST::Action* __restrict__ action, float* __restrict__ logp,
@@ -919,19 +921,23 @@ __global__ void sample_kernel(const float* __restrict__ pi, const float* __restr
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   if (offset_dev) offset = (uint64_t)(*offset_dev) + (uint64_t)t_add;
-  logp[b] = DIST::draw(pi + (long long)b * A, A, A, log_std, noise ? noise + (long long)b * A : nullptr, b, seed, offset, action,
-                       nullptr);
+  const int s = b / period, e = b - s * period;
+  const long long r0 = (long long)s * period;   // the step's first row: the draw writes row e of the step's slice
+  logp[b] = DIST::draw(pi + (long long)b * A, A, A, log_std, noise ? noise + (long long)b * A : nullptr, e, seed,
+                       offset + (uint64_t)s, action + r0 * DIST::action_width(A), nullptr);
   if (v_out) v_out[b] = v_in[b];
 }
 
 // Inference heads of PPO: the pi head (logits / mean) and the value head of one dense layer each, then the draw of
 // DIST at Philox offset *offset_dev + t_add (the device-resident counter of rollout inference), in one kernel, one warp
-// per sample.  log_std: DiagGaussian only.
+// per sample.  Rows are consecutive steps of `period` samples as in sample_kernel: row b draws at Philox index
+// b % period and offset *offset_dev + t_add + b / period.  head_out (the pi head's rows): required.  log_std:
+// DiagGaussian only.
 template <class DIST, int HEAD_KPL, int HEAD_AMAX>
 __global__ void __launch_bounds__(256)
 infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v, const float* __restrict__ w_pi,
                    const float* __restrict__ b_pi, const float* __restrict__ w_v, const float* __restrict__ b_v,
-                   const float* __restrict__ log_std, int B, int K, int A, uint64_t seed,
+                   const float* __restrict__ log_std, int B, int period, int K, int A, uint64_t seed,
                    const unsigned long long* __restrict__ offset_dev, int t_add, typename DIST::Action* __restrict__ action,
                    float* __restrict__ logp, float* __restrict__ v_out, float* __restrict__ head_out) {
   pdl_wait(); pdl_trigger();
@@ -955,7 +961,10 @@ infer_heads_kernel(const float* __restrict__ h_pi, const float* __restrict__ h_v
 #pragma unroll
     for (int i = 0; i <= HEAD_AMAX; i++) acc[i] = warp_sum(acc[i]);
     if (lane == 0) {
-      logp[b] = DIST::template infer<HEAD_AMAX>(acc, b_pi, log_std, b, A, seed, offset, action, head_out);
+      const int s = b / period, e = b - s * period;
+      const long long r0 = (long long)s * period;
+      logp[b] = DIST::template infer<HEAD_AMAX>(acc, b_pi, log_std, e, A, seed, offset + (uint64_t)s,
+                                                action + r0 * DIST::action_width(A), head_out + r0 * A);
       v_out[b] = acc[HEAD_AMAX] + b_v[0];
     }
   }

@@ -348,6 +348,19 @@ static int dense_k_slices(int kchunks, int tiles, int* kc_split) {
   }
   return 1;
 }
+// Split-K plan of a dense tensor-core forward over B rows whose slice count is chosen for split_rows rows (rollout
+// inference evaluates several steps per forward and chooses for one step's rows, so that a row's sums do not depend
+// on how many steps share the launch): nz slices of kc_split chunks, partial sums in nz slabs of [round16(B)][N] floats.
+// The workspace planner sizes the split-K region with it, as the launch uses it.
+struct DenseSplit { int nz, kc_split; size_t part_bytes; };
+static DenseSplit dense_split(const LayerPlan& lp, int B, int split_rows) {
+  DenseSplit d;
+  d.nz = dense_k_slices(lp.K / 8, (lp.N / lp.n_fwd) * ((split_rows + 127) / 128), &d.kc_split);
+  d.part_bytes = d.nz > 1 ? (size_t)d.nz * ((B + 15) & ~15) * lp.N * sizeof(float) : 0;
+  return d;
+}
+// Steps per forward of rollout inference over E environments: as many as fit max_batch rows, at least one
+static int infer_chunk_steps(int max_batch, int E) { return std::max(1, max_batch / E); }
 // A conv layer stays on the tensor cores only if its stage tables fit: the forward and data-gradient launches get at
 // least two ring stages beside their table (the data gradient with the epilogue buffers of an accumulating launch, the
 // largest it can need), the weight-gradient table fits beside the WG_STAGES stages, and no unit needs more stages than
@@ -574,14 +587,14 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     lp.dg_st_off = place(lp.dg_st.size() * sizeof(bp::StageEnt)); lp.dg_un_off = place(lp.dg_un.size() * sizeof(bp::UnitEnt));
     lp.wg_off = place(lp.wg_tab.size() * sizeof(bp::WgEnt));
   }
-  // split-K partial sums of a dense forward: n_z slabs of [round16(B)][N] with n_z <= kSMs / (N tiles * batch tiles) + 1
+  // split-K partial sums of a dense forward: the largest over the forwards the net runs, B rows split for E rows with
+  // E <= B <= max_batch; a rollout-inference chunk of E environments (the most rows at a given E) covers every B = E
   net->splitk_off = w;
   {
     size_t need = 0;
-    for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_DENSE) {
-      size_t rows = (size_t)(kSMs / (lp.N / lp.n_fwd) + 1) * 128 + net->pitch;
-      need = std::max(need, rows * lp.N * sizeof(float));
-    }
+    for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_DENSE)
+      for (int E = 1; E <= max_batch; E++)
+        need = std::max(need, dense_split(lp, infer_chunk_steps(max_batch, E) * E, E).part_bytes);
     w += align_up(need + 256, 256);
   }
   for (auto& lp : net->L)
@@ -829,8 +842,10 @@ static void queue_reduction(xtb_net* net, const float* part, int n_slabs, long l
   net->pending.push_back(r);
 }
 
-// forward of a tensor-core layer.  want_f32: also store the fp32 row-major copy; want_bp: store the planes
-static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool want_bp, cudaStream_t st, long long* launches) {
+// forward of a tensor-core layer over B rows, a dense layer split over K as for split_rows rows (dense_split).
+// want_f32: also store the fp32 row-major copy; want_bp: store the planes
+static cudaError_t tc_forward(xtb_net* net, int i, int B, int split_rows, bool want_f32, bool want_bp, cudaStream_t st,
+                              long long* launches) {
   const LayerPlan& lp = net->L[i];
   const int t = i + 1;
   bp::RowsArgs a;
@@ -857,7 +872,9 @@ static cudaError_t tc_forward(xtb_net* net, int i, int B, bool want_f32, bool wa
   }
   a.mode = 2;
   a.kchunks = lp.K / 8; a.n_ntiles = lp.N / lp.n_fwd;
-  const int nz = dense_k_slices(a.kchunks, a.n_ntiles * a.n_btiles, &a.kc_split);
+  const DenseSplit sp = dense_split(lp, B, split_rows);
+  const int nz = sp.nz;
+  a.kc_split = sp.kc_split;
   a.n_units = a.n_ntiles * nz;
   if (nz == 1) return launch_rows<0>(a, st);
   a.part = (float*)(net->ws + net->splitk_off);
@@ -1163,9 +1180,9 @@ static void with_obs_type(const xtb_net* net, const void* obs, F&& f) {
   else f((const float*)obs);
 }
 
-// forward of layer i; tc_allowed = parameters are the bound ones (their blobs are current)
+// forward of layer i; tc_allowed = parameters are the bound ones (their blobs are current); split_rows: see tc_forward
 static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, const void* obs, const int32_t* idx, int B,
-                      bool want_f32, cudaStream_t st) {
+                      int split_rows, bool want_f32, cudaStream_t st) {
   const LayerPlan& lp = net->L[i];
   const int t = i + 1;
   float* out = out_f32(net, t);
@@ -1188,7 +1205,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
     int rc = lp.d.src == 0 ? op_decode(net, obs, idx, B, st) : ensure_bp(net, lp.d.src, B, false, st);
     if (rc) return rc;
     long long nl = 0;
-    cudaError_t te = tc_forward(net, i, B, want_f32, true, st, &nl);
+    cudaError_t te = tc_forward(net, i, B, split_rows, want_f32, true, st, &nl);
     if (te != cudaSuccess) return fail(XTB_ERR_CUDA, "tensor-core forward launch (layer %d): %s", i, cudaGetErrorString(te));
     g_launches.fetch_add(nl, std::memory_order_relaxed);
     if (ext) return act_forward(net, t, B, st);
@@ -1335,15 +1352,16 @@ static int flush_reductions(xtb_net* net, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------
 // forward / backward
 // ------------------------------------------------------------------------------------------
-// want_f32_mask: bit t set = tensor t is needed in fp32 row-major form (all tensors for the public entry point)
+// want_f32_mask: bit t set = tensor t is needed in fp32 row-major form (all tensors for the public entry point).
+// split_rows: the rows the dense split-K forwards are planned for (tc_forward); 0 = batch
 static int net_forward_impl(xtb_net* net, const float* params, const void* obs, const int32_t* gather_idx,
-                            int batch, void* stream, unsigned skip_mask, unsigned want_f32_mask);
+                            int batch, void* stream, unsigned skip_mask, unsigned want_f32_mask, int split_rows = 0);
 extern "C" int xtb_net_forward(xtb_net* net, const float* params, const void* obs, const int32_t* gather_idx,
                                int batch, void* stream) {
   return net_forward_impl(net, params, obs, gather_idx, batch, stream, 0u, ~0u);
 }
 static int net_forward_impl(xtb_net* net, const float* params, const void* obs, const int32_t* gather_idx,
-                            int batch, void* stream, unsigned skip_mask, unsigned want_f32_mask) {
+                            int batch, void* stream, unsigned skip_mask, unsigned want_f32_mask, int split_rows) {
   if (!net || !net->ws) return fail(XTB_ERR_STATE, "xtb_net_forward: net not bound");
   if (batch <= 0 || batch > net->max_batch) return fail(XTB_ERR_ARG, "batch %d out of range (max %d)", batch, net->max_batch);
   if (!obs) return fail(XTB_ERR_ARG, "obs is null");
@@ -1362,7 +1380,7 @@ static int net_forward_impl(xtb_net* net, const float* params, const void* obs, 
     if (lp.d.kind == XTB_DENSE)
       for (int j = i + 1; j < nl; j++)
         if (reads(net->L[j], i + 1) && !(skip_mask & (1u << j)) && !(tc_allowed && use_tc(net->L[j]))) direct = true;
-    int rc = op_forward(net, i, P, tc_allowed, obs, gather_idx, batch, direct, st);
+    int rc = op_forward(net, i, P, tc_allowed, obs, gather_idx, batch, split_rows ? split_rows : batch, direct, st);
     if (rc) return rc;
   }
   for (int t = 1; t <= nl; t++) {
@@ -1512,7 +1530,7 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
   for (int t = 1; t <= (int)net->L.size(); t++)
     for (bool grad : {false, true})
       if (forms(net, t, grad) == kNone) wrote(net, t, grad, kF32);
-  if (which == 0) return op_forward(net, layer, net->params, true, obs, gather_idx, batch, false, st);
+  if (which == 0) return op_forward(net, layer, net->params, true, obs, gather_idx, batch, batch, false, st);
   if (which == 1) { int rc = op_wgrad(net, layer, obs, gather_idx, batch, st, true); net->pending.clear(); return rc; }
   if (which == 2) {
     if (net->L[layer].d.src == 0) return fail(XTB_ERR_ARG, "layer reads the observation: no data gradient");
@@ -1531,8 +1549,8 @@ extern "C" int xtb_net_bench_layer(xtb_net* net, int layer, int which, const voi
 extern "C" int xtb_categorical_sample(const float* logits, int batch, int adim, const float* uniforms,
                                       uint64_t seed, uint64_t offset, int32_t* action, float* logp, void* stream) {
   if (!logits || !action || !logp || batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_categorical_sample: bad argument");
-  XLAUNCH(sample_kernel<Categorical>, (batch + 127) / 128, 128, 0, S(stream), logits, (const float*)nullptr, batch, adim, uniforms,
-          seed, offset, (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
+  XLAUNCH(sample_kernel<Categorical>, (batch + 127) / 128, 128, 0, S(stream), logits, (const float*)nullptr, batch, batch, adim,
+          uniforms, seed, offset, (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
   LAUNCH_CHECK();
   return XTB_OK;
 }
@@ -1577,8 +1595,8 @@ extern "C" int xtb_diag_gaussian_sample(const float* mean, const float* log_std,
                                         uint64_t seed, uint64_t offset, float* action, float* logp, void* stream) {
   if (!mean || !log_std || !action || !logp || batch <= 0 || adim <= 0 || adim > MAX_ADIM)
     return fail(XTB_ERR_ARG, "xtb_diag_gaussian_sample: bad argument");
-  XLAUNCH(sample_kernel<DiagGaussian>, (batch + 127) / 128, 128, 0, S(stream), mean, log_std, batch, adim, normals, seed, offset,
-          (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
+  XLAUNCH(sample_kernel<DiagGaussian>, (batch + 127) / 128, 128, 0, S(stream), mean, log_std, batch, batch, adim, normals, seed,
+          offset, (const unsigned long long*)nullptr, 0, action, logp, (const float*)nullptr, (float*)nullptr);
   LAUNCH_CHECK();
   return XTB_OK;
 }
@@ -3176,9 +3194,12 @@ extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const
 // ------------------------------------------------------------------------------------------
 // rollout inference: T batched policy evaluations over the E stacked observations
 // ------------------------------------------------------------------------------------------
-// T policy evaluations of the action distribution DIST: per step the forward of the layers below the heads and
-// infer_heads_kernel (both heads and the draw) within the fused-inference limits, otherwise every layer and then the
-// sampling kernel; the draws are the same either way.  step_idx NULL: step t reads observation rows t*E .. (t+1)*E - 1.
+// T policy evaluations of the action distribution DIST, infer_chunk_steps(max_batch, E) steps per forward (the last
+// chunk ragged): per chunk the forward of the layers below the heads and infer_heads_kernel (both heads and the draw)
+// within the fused-inference limits, otherwise every layer and then the sampling kernel; the draws are the same either
+// way.  The steps are independent (fixed weights, draws keyed on (env, step)), and every kernel of a chunk computes a
+// row as it would in a one-step forward: the dense split-K is chosen for E rows, whatever the chunk holds.  So the
+// results do not depend on the chunking.  step_idx NULL: step t reads observation rows t*E .. (t+1)*E - 1.
 template <class DIST>
 static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* step_idx, int E, int T, int pi_t, int v_t, int ls_t,
                                 uint64_t seed, unsigned long long* offset_dev, typename DIST::Action* action, float* logp,
@@ -3193,23 +3214,32 @@ static int rollout_infer_launch(xtb_net* net, const void* obs, const int32_t* st
   const size_t row_bytes = (size_t)net->tsize[0] * (net->desc.input_u8 ? 1 : sizeof(float));
   float* pi_out = xtb_net_tensor(net, pi_t);
   const float* v_in = xtb_net_tensor(net, v_t);
-  for (int t = 0; t < T; t++) {
-    const void* obs_t = step_idx ? obs : (const void*)((const char*)obs + (size_t)t * E * row_bytes);
-    int rc = net_forward_impl(net, nullptr, obs_t, step_idx ? step_idx + (long long)t * E : nullptr, E, stream, skip, want);
+  const int c = infer_chunk_steps(net->max_batch, E);
+  int n = 0;   // steps in the chunk
+  for (int t0 = 0; t0 < T; t0 += c) {
+    n = std::min(c, T - t0);
+    const int rows = n * E;
+    const long long r0 = (long long)t0 * E;
+    const void* obs_t = step_idx ? obs : (const void*)((const char*)obs + (size_t)r0 * row_bytes);
+    int rc = net_forward_impl(net, nullptr, obs_t, step_idx ? step_idx + r0 : nullptr, rows, stream, skip, want, E);
     if (rc) return rc;
-    typename DIST::Action* a_t = action + (long long)t * E * DIST::action_width(adim);
-    float* lp_t = logp + (long long)t * E; float* v_o = value + (long long)t * E;
+    typename DIST::Action* a_t = action + r0 * DIST::action_width(adim);
+    float* lp_t = logp + r0; float* v_o = value + r0;
     if (fuse) {
-      XLAUNCH(heads_pick(kInferHeadsKernels<DIST>, lpi.K, adim)->kern, std::max(1, std::min(kSMs, (E + 7) / 8)), 256, 0, S(stream),
-              (const float*)out_f32(net, lpi.d.src), (const float*)out_f32(net, lv.d.src), net->params + lpi.w_off,
-              net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off, log_std, E, lpi.K, adim, seed, offset_dev, t,
-              a_t, lp_t, v_o, pi_out);
+      XLAUNCH(heads_pick(kInferHeadsKernels<DIST>, lpi.K, adim)->kern, std::max(1, std::min(kSMs, (rows + 7) / 8)), 256, 0,
+              S(stream), (const float*)out_f32(net, lpi.d.src), (const float*)out_f32(net, lv.d.src), net->params + lpi.w_off,
+              net->params + lpi.b_off, net->params + lv.w_off, net->params + lv.b_off, log_std, rows, E, lpi.K, adim, seed,
+              offset_dev, t0, a_t, lp_t, v_o, pi_out);
     } else {
-      XLAUNCH(sample_kernel<DIST>, (E + 127) / 128, 128, 0, S(stream), pi_out, log_std, E, adim, (const float*)nullptr, seed,
-              (uint64_t)0, offset_dev, t, a_t, lp_t, v_in, v_o);
+      XLAUNCH(sample_kernel<DIST>, (rows + 127) / 128, 128, 0, S(stream), pi_out, log_std, rows, E, adim, (const float*)nullptr,
+              seed, (uint64_t)0, offset_dev, t0, a_t, lp_t, v_in, v_o);
     }
     LAUNCH_CHECK();
   }
+  // the pi head of the last step goes to rows [0, E) of its tensor, where a one-step call leaves it
+  if (n > 1)
+    CUDA_TRY(cudaMemcpyAsync(pi_out, pi_out + (size_t)(n - 1) * E * adim, sizeof(float) * (size_t)E * adim,
+                             cudaMemcpyDeviceToDevice, S(stream)));
   XLAUNCH(bump_counter_kernel, 1, 1, 0, S(stream), offset_dev, T);
   LAUNCH_CHECK();
   return XTB_OK;
