@@ -298,6 +298,11 @@ int xtb_opt_use_rmsprop_plain(xtb_adam* opt, float decay, float epsilon);
  *              step is bitwise reproducible;
  *   inference: with the draw, for A <= 8 and K <= 512.
  * Every other shape runs layer by layer (forward, the loss or sampling kernel, backward); the draws are the same. */
+/* The fused-heads instantiation the PPO calls would launch for these heads under the current fused-heads mode: the
+ * training kernel (infer == 0) or the rollout-inference kernel (infer != 0), as (*kpl, *amax): it covers K <= 32 * kpl
+ * hidden units and A <= amax actions; (0, 0) when the heads run layer by layer.  Head tensors the PPO calls reject
+ * return XTB_ERR_ARG, as there.  Launches nothing. */
+int xtb_ppo_heads_plan(const xtb_net* net, int pi_tensor, int v_tensor, int infer, int* kpl, int* amax);
 /* PPO.train (xt/model/ppo/ppo.py:111-132): for every minibatch slice of `perm`
  * (device int32 [n_epoch*n_sample], the host-generated np.random.shuffle order) run
  * forward, loss, backward, clip, Adam.  loss_per_step: device float [n_epoch*ceil(N/B)].  Without fused heads a

@@ -399,11 +399,11 @@ def test_rollout_infer_rejects_wrong_logstd_tensors(xb):
 
 
 # ---- the fused Gaussian heads: train step (heads_kernel<PpoGaussLoss>) and rollout inference (gauss_infer_heads_kernel)
-def _mlp_model(A, K, B, graph=False):
+def _mlp_model(A, K, B, graph=False, max_predict=1024):
     """PpoMlp [3] -> A with tanh [K, K] separate towers and a non-zero pi_logstd; one epoch of one minibatch of B"""
     import xingtian_b200  # noqa: F401
     from xingtian_b200.registry import Registers
-    m = Registers.model["PpoMlp"]({"state_dim": [3], "action_dim": A, "model_config": {
+    m = Registers.model["PpoMlp"]({"state_dim": [3], "action_dim": A, "max_predict_batch": max_predict, "model_config": {
         "BATCH_SIZE": B, "NUM_SGD_ITER": 1, "hidden_sizes": [K, K], "activation": "tanh", "VF_SHARE_LAYERS": False,
         "action_type": "DiagGaussian", "init_seed": 3, "VF_CLIP": 0.5, "ENTROPY_LOSS": 0.01, "LOSS_CLIPPING": 0.2,
         "use_cuda_graph": graph}})
@@ -437,10 +437,14 @@ def _oracle_step(arch, w, obs, label, B, dt):
         return float(loss), {k: g.detach().numpy() for k, g in zip(ref.names, grads)}
 
 
+# K = 512 reaches the heads_kernel entry for up to 512 hidden units and 4 actions (A = 8 then trains layer by layer), and
+# B = 1057 the grid-stride loop: 132 blocks x 8 warps, so a warp's lane 0 sums the log_std gradient of two samples
+TRAIN_STEP_CASES = [(A, K, B) for A in (1, 3, 8) for K in (64, 256) for B in (1, 37, 200, 512)] + \
+    [(3, 512, 37), (3, 512, 1057), (8, 512, 37)]
+
+
 @pytest.mark.parametrize("fuse", [1, 0], ids=["fused", "layers"])
-@pytest.mark.parametrize("B", [1, 37, 200, 512])
-@pytest.mark.parametrize("K", [64, 256])
-@pytest.mark.parametrize("A", [1, 3, 8])
+@pytest.mark.parametrize("A,K,B", TRAIN_STEP_CASES)
 def test_train_step_against_float64(xb, tc_mode, A, K, B, fuse):
     """one Gaussian SGD step, fused heads and layer by layer, on both kernel paths: loss and every gradient, pi_logstd's
     included, at most 4x torch-CPU fp32's distance from float64 (+ the bf16x3 bound on the tensor-core path)"""
@@ -532,18 +536,22 @@ def test_gauss_training_is_bitwise_reproducible(xb):
     assert not np.array_equal(runs[0][1]["pi_logstd"], w_init["pi_logstd"])
 
 
-@pytest.mark.parametrize("A,K,fused", [(1, 64, True), (3, 64, True), (8, 256, True), (3, 512, True), (9, 64, False),
-                                       (3, 48, False)])
-def test_rollout_infer_against_float64(xb, tc_mode, A, K, fused):
+ROLLOUT_CASES = [pytest.param(A, K, fused, 37, 3, 1024, id="%d-%d-%s" % (A, K, fused))
+                 for A, K, fused in [(1, 64, True), (3, 64, True), (8, 256, True), (3, 512, True), (9, 64, False), (3, 48, False)]]
+# the chunk of C5's inference: 8 steps x 512 envs = 4096 rows, grid-stride over 132 blocks x 8 warps
+ROLLOUT_CASES.append(pytest.param(3, 256, True, 512, 8, 4096, id="3-256-True-E512-T8-M4096"))
+
+
+@pytest.mark.parametrize("A,K,fused,E,T,M", ROLLOUT_CASES)
+def test_rollout_infer_against_float64(xb, tc_mode, A, K, fused, E, T, M):
     """rollout inference, fused heads within the limits (K % 32 == 0, A <= 8, K <= 512) and layer by layer outside:
     actions, log-probs and values against float64 with the same Philox normals; fewer launches when fused"""
     lib = xb["lib"]
-    E, T = 37, 3
     res = {}
     try:
         for fuse in (1, 0):
             lib.xtb_set_fuse_heads(fuse)
-            m = _mlp_model(A, K, 64)
+            m = _mlp_model(A, K, 64, max_predict=M)
             rng = np.random.default_rng(5)
             obs = rng.standard_normal((E * T, 3)).astype(np.float32)
             obs_d = torch.from_numpy(obs).cuda()

@@ -2146,6 +2146,24 @@ static int ppo_heads_check(const char* fn, const xtb_net* net, int pi_t, int v_t
   return XTB_OK;
 }
 
+// the heads_kernel (infer: infer_heads_kernel) entry the PPO calls launch for these heads, (0, 0) when layer by layer
+extern "C" int xtb_ppo_heads_plan(const xtb_net* net, int pi_t, int v_t, int infer, int* kpl, int* amax) {
+  const char* fn = "xtb_ppo_heads_plan";
+  if (!net || !kpl || !amax) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (int rc = ppo_heads_check(fn, net, pi_t, v_t, 0)) return rc;
+  *kpl = *amax = 0;
+  if (!ppo_heads_fusable(net, pi_t, v_t, infer != 0)) return XTB_OK;
+  const int K = net->L[pi_t - 1].K, A = net->tsize[pi_t];
+  if (infer) {
+    const auto* e = heads_pick(kInferHeadsKernels<Categorical>, K, A);
+    *kpl = e->kpl; *amax = e->amax;
+  } else {
+    const auto* e = heads_pick(kHeadsKernels<PpoLoss>, K, A);
+    *kpl = e->kpl; *amax = e->amax;
+  }
+  return XTB_OK;
+}
+
 extern "C" int xtb_ppo_train(xtb_net* net, xtb_adam* opt, const xtb_ppo_rollout* ro, int n_sample, int batch_size, int n_epoch,
                              const int32_t* perm, const xtb_ppo_hyper* hp, int pi_t, int v_t, int ls_t, float* loss_per_step,
                              int use_graph, void* stream) {

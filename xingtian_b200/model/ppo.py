@@ -172,6 +172,13 @@ class PPO(XTModel, PolicyActor):
         self._obs_ring = dict(E=int(env_num), T=int(steps), t=0,
                               obs=torch.empty((int(steps), int(env_num)) + tuple(self.state_dim), dtype=self._obs_dt, device=self.device))
 
+    def heads_plan(self, infer):
+        """(kpl, amax) of the fused-heads kernel that training (infer False) or rollout inference (infer True) launches
+        for this policy's heads under the current fused-heads mode; (0, 0) when they run layer by layer."""
+        kpl, amax = C.c_int(), C.c_int()
+        check(self.net.lib.xtb_ppo_heads_plan(self.net.handle, self.pi_t, self.v_t, 1 if infer else 0, C.byref(kpl), C.byref(amax)))
+        return kpl.value, amax.value
+
     # -- training ----------------------------------------------------------------------------
     def make_perm(self, nbatch):
         """Index order of xt/model/ppo/ppo.py:114-121: `inds` shuffled in place every epoch."""
