@@ -2307,6 +2307,27 @@ extern "C" int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_imp
   });
 }
 
+// ---- Scratch of the native objects ------------------------------------------------------------------------------------
+// One piece of an object's device scratch: the pointer it is carved into and its length in elements of that pointer's type
+struct Piece {
+  void** slot;
+  size_t bytes;
+  template <class T> Piece(T** p, long long count) : slot(reinterpret_cast<void**>(p)), bytes((size_t)count * sizeof(T)) {}
+};
+// An object's scratch as one zero-filled cudaMalloc into *buf, every piece 256-byte aligned; on failure nothing is left
+// allocated
+static int carve_scratch(const char* fn, void** buf, const std::vector<Piece>& pieces) {
+  size_t tot = 0;
+  for (const Piece& pc : pieces) tot += align_up(pc.bytes, 256);
+  cudaError_t e = cudaMalloc(buf, tot);
+  if (e != cudaSuccess) return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e));
+  e = cudaMemset(*buf, 0, tot);
+  if (e != cudaSuccess) { cudaFree(*buf); return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  char* p = (char*)*buf;
+  for (const Piece& pc : pieces) { *pc.slot = p; p += align_up(pc.bytes, 256); }
+  return XTB_OK;
+}
+
 // ---- MuZero (xt/model/muzero/muzero_model.py:103-140, 154-239) -------------------------------------------------------
 // The three networks (representation, dynamics, prediction) are separate xtb_nets bound to consecutive slices of one
 // parameter buffer and one gradient buffer (the Keras list order of MuzeroBase); the dynamics net's own gradient buffer
@@ -2318,7 +2339,7 @@ struct xtb_muzero {
   int max_batch = 0, K = 0, H = 0, A = 0, Sv = 0, Sr = 0, n_part = 0;
   int act_rep = 0, act_dyn = 0;
   long long n_params = 0;      // floats of the shared parameter buffer
-  float* buf = nullptr;
+  void* buf = nullptr;
   float *hbuf = nullptr, *xbuf = nullptr, *rlog = nullptr, *dr = nullptr, *tv = nullptr, *tr = nullptr, *dh = nullptr,
         *dx = nullptr, *part = nullptr;
 };
@@ -2364,16 +2385,12 @@ extern "C" int xtb_muzero_create(xtb_net* rep, xtb_net* dyn, xtb_net* pred, cons
   m->K = K; m->H = H; m->A = A; m->Sv = Sv; m->Sr = Sr; m->act_rep = act_rep; m->act_dyn = act_dyn; m->n_params = total;
   const long long Bm = max_batch, R1 = (long long)(K + 1) * Bm, RK = (long long)K * Bm;
   m->n_part = 2 * mz_blocks(R1) + mz_blocks(RK);
-  const long long sizes[] = {R1 * H, RK * (H + A), RK * Sr, RK * Sr, R1 * Sv, RK * Sr, R1 * H, Bm * (H + A), m->n_part};
-  float** dst[] = {&m->hbuf, &m->xbuf, &m->rlog, &m->dr, &m->tv, &m->tr, &m->dh, &m->dx, &m->part};
-  long long tot = 0;
-  for (long long n : sizes) tot += (n + 63) / 64 * 64;
-  cudaError_t e = cudaMalloc(&m->buf, tot * sizeof(float));
-  if (e != cudaSuccess) { delete m; return fail(XTB_ERR_NOMEM, "xtb_muzero_create: %s", cudaGetErrorString(e)); }
-  e = cudaMemset(m->buf, 0, tot * sizeof(float));
-  if (e != cudaSuccess) { cudaFree(m->buf); delete m; return fail(XTB_ERR_CUDA, "xtb_muzero_create: %s", cudaGetErrorString(e)); }
-  float* p = m->buf;
-  for (int i = 0; i < 9; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
+  if (int rc = carve_scratch("xtb_muzero_create", &m->buf, {{&m->hbuf, R1 * H}, {&m->xbuf, RK * (H + A)}, {&m->rlog, RK * Sr},
+                                                            {&m->dr, RK * Sr}, {&m->tv, R1 * Sv}, {&m->tr, RK * Sr}, {&m->dh, R1 * H},
+                                                            {&m->dx, Bm * (H + A)}, {&m->part, m->n_part}})) {
+    delete m;
+    return rc;
+  }
   *out = m;
   return XTB_OK;
 }
@@ -2471,20 +2488,16 @@ extern "C" int xtb_muzero_tree_create(const xtb_muzero* m, int max_envs, int max
   if (max_envs < 1 || max_simulations < 1 || max_simulations > (1 << 20))
     return fail(XTB_ERR_ARG, "xtb_muzero_tree_create: max_envs %d / max_simulations %d out of range", max_envs, max_simulations);
   const long long E = max_envs, NN = max_simulations + 1, A = m->A, H = m->H;
-  // byte sizes, in the order of `dst` below; each piece starts 256-byte aligned
-  const long long sizes[] = {NN * E * H * 4, E * NN * 8, E * NN * A * 8, E * NN * A * 8, E * NN * A * 4, E * NN * A * 4, E * 8, E * 4,
-                             E * 2 * 8, E * NN * 4, E * NN * 4, E * 4, E * 4, E * 4, E * A * 4};
   auto* tr = new xtb_muzero_tree();
   MctsTrees& t = tr->t;
-  void** dst[] = {(void**)&t.hid, (void**)&t.reward, (void**)&t.prior, (void**)&t.vsum, (void**)&t.visits, (void**)&t.child,
-                  (void**)&t.root_vsum, (void**)&t.root_visits, (void**)&t.minmax, (void**)&t.path_node, (void**)&t.path_act,
-                  (void**)&t.depth, (void**)&tr->reward, (void**)&tr->value, (void**)&tr->policy};
-  long long tot = 0;
-  for (long long n : sizes) tot += align_up(n, 256);
-  cudaError_t e = cudaMalloc(&tr->buf, tot);
-  if (e != cudaSuccess) { delete tr; return fail(XTB_ERR_NOMEM, "xtb_muzero_tree_create: %s", cudaGetErrorString(e)); }
-  char* p = (char*)tr->buf;
-  for (int i = 0; i < 15; i++) { *dst[i] = p; p += align_up(sizes[i], 256); }
+  if (int rc = carve_scratch("xtb_muzero_tree_create", &tr->buf,
+                             {{&t.hid, NN * E * H}, {&t.reward, E * NN}, {&t.prior, E * NN * A}, {&t.vsum, E * NN * A},
+                              {&t.visits, E * NN * A}, {&t.child, E * NN * A}, {&t.root_vsum, E}, {&t.root_visits, E},
+                              {&t.minmax, E * 2}, {&t.path_node, E * NN}, {&t.path_act, E * NN}, {&t.depth, E},
+                              {&tr->reward, E}, {&tr->value, E}, {&tr->policy, E * A}})) {
+    delete tr;
+    return rc;
+  }
   t.E = max_envs; t.NN = (int)NN; t.A = (int)A; t.H = (int)H;
   tr->max_sims = max_simulations;
   *out = tr;
@@ -2632,19 +2645,172 @@ extern "C" int xtb_muzero_train(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_b
                    use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
 }
 
-// ---- QMIX (xt/model/qmix/qmix_tf.py) ----------------------------------------------------------------------------------
-// fc1, fc2 and the hypernetworks are engine nets bound to slices of the eval weight set; target and explore sets are
-// read through the nets' foreign-parameter forward.  The object owns the step's device scratch for the fixed batch.
-struct xtb_qmix {
-  xtb_net *fc1 = nullptr, *fc2 = nullptr, *hyp = nullptr;
-  xtb_qmix_desc d{};
-  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, E = 0, R = 0, BL = 0, S = 0, G = 0, n_part = 0;
+// ---- The recurrent agent of QMIX and SCC (xt/model/qmix/qmix_tf.py: fc1 -> GRU -> fc2) --------------------------------
+// fc1 and fc2 are engine nets bound to the slices [fc1 | gru | fc2] at the front of their object's eval weight set, the
+// GRU's kernels and biases at o_gru; other weight sets are read through the nets' foreign-parameter forward.  A training
+// batch is B episodes of T = L + 1 steps of n agents: R = B T n agent rows, BL = B L steps and S = B n GRU sequences, G
+// of them per CTA of the GRU kernels with smem bytes of shared memory.
+struct QmixAgent {
+  xtb_net *fc1 = nullptr, *fc2 = nullptr;
+  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, R = 0, BL = 0, S = 0, G = 0;
   size_t smem = 0;
-  long long o_gru = 0, o_fc2 = 0, o_hyp = 0, n_params = 0;
-  float* buf = nullptr;
-  float *qt = nullptr, *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr,
-        *w1t = nullptr, *b1t = nullptr, *wft = nullptr, *vt = nullptr, *part = nullptr;
-  int32_t* ones = nullptr;   // [n_agents] sequence lengths of the one-step inference
+  long long o_gru = 0, o_fc2 = 0;
+  float *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr;
+  int32_t* ones = nullptr;   // [n] sequence lengths of the one-step inference
+};
+
+// layer i of nt is a dense layer on tensor src with activation act
+static bool dense_layer(const xtb_net* nt, int i, int src, int act) {
+  const LayerPlan& lp = nt->L[i];
+  return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
+}
+
+// The agent's checks and sizes for `batch` episodes of `episode_limit` steps of `n_agents` agents with the GRU at gru_off,
+// into *a: all of them but the nets' row capacity (agent_capacity), which the caller checks after its own size bounds.
+static int agent_plan(const char* fn, xtb_net* fc1, xtb_net* fc2, int batch, int episode_limit, int n_agents, long long gru_off,
+                      QmixAgent* a) {
+  for (xtb_net* nt : {fc1, fc2})
+    if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  if (fc1->L.size() != 1 || !dense_layer(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
+    return fail(XTB_ERR_ARG, "%s: fc1 must be one relu dense layer on float agent inputs", fn);
+  const int H = fc1->tsize[1];
+  if (fc2->L.size() != 1 || !dense_layer(fc2, 0, 0, XTB_ACT_NONE) || fc2->tsize[0] != H)
+    return fail(XTB_ERR_ARG, "%s: fc2 must be one linear dense layer on the %d-wide GRU output", fn, H);
+  if (int rc = input_grad_check(fc2)) return rc;
+  const int A = fc2->tsize[1], n = n_agents;
+  if (n < 1 || n > QM_MAX_AGENTS) return fail(XTB_ERR_ARG, "%s: n_agents %d not in [1, %d]", fn, n, QM_MAX_AGENTS);
+  if (A < 1 || A > 255) return fail(XTB_ERR_ARG, "%s: n_actions %d not in [1, 255] (actions are uint8 in the reference)", fn, A);
+  if (batch < 1 || episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, batch, episode_limit);
+  const long long T = episode_limit + 1LL, R = batch * T * n;
+  if (R > (1LL << 30) / std::max(3 * H, 1)) return fail(XTB_ERR_ARG, "%s: batch too large", fn);
+  const int S = batch * n;
+  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
+  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
+  if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
+    return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
+  // the gradients at the same offsets as the weights
+  const long long o_fc2 = fc2->params - fc1->params, gru_n = 2LL * H * 2 * H + 2 * H + 2LL * H * H + H;
+  if (gru_off < fc1->n_params || o_fc2 < gru_off + gru_n || fc2->grads != fc1->grads + o_fc2)
+    return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2] at the front of one buffer, in order", fn);
+  a->fc1 = fc1; a->fc2 = fc2;
+  a->B = batch; a->L = episode_limit; a->T = (int)T; a->n = n; a->A = A; a->H = H; a->R = (int)R; a->BL = batch * episode_limit;
+  a->S = S; a->G = G; a->smem = qgru_smem_floats(H, G) * 4;
+  a->o_gru = gru_off; a->o_fc2 = o_fc2;
+  return XTB_OK;
+}
+
+// fc1 and fc2 hold the R rows of a training batch
+static int agent_capacity(const char* fn, const QmixAgent& a) {
+  if (a.fc1->max_batch < a.R || a.fc2->max_batch < a.R) return fail(XTB_ERR_ARG, "%s: fc1 / fc2 hold fewer rows than a batch (%d)", fn, a.R);
+  return XTB_OK;
+}
+
+// The object's scratch in one carve_scratch into *buf, the agent's pieces before the object's own `pieces`; then the
+// one-step inference's sequence lengths and the GRU kernels' shared-memory opt-in.  On failure nothing stays allocated.
+static int agent_alloc(const char* fn, QmixAgent& a, void** buf, std::vector<Piece> pieces) {
+  const long long R = a.R, H = a.H;
+  pieces.insert(pieces.begin(), {{&a.xg, R * 2 * H}, {&a.xc, R * H}, {&a.hout, R * H}, {&a.rh, R * H}, {&a.dy, R * H},
+                                 {&a.dag, R * 2 * H}, {&a.dac, R * H}, {&a.ones, a.n}});
+  if (int rc = carve_scratch(fn, buf, pieces)) return rc;
+  std::vector<int32_t> ones(a.n, 1);
+  cudaError_t e = cudaMemcpy(a.ones, ones.data(), a.n * sizeof(int32_t), cudaMemcpyHostToDevice);
+  // The opt-in is a property of the kernel, shared by every live object: it is set to the most any object may use
+  // (this object's smem would shrink it under an earlier object with a wider GRU or more sequences per CTA).
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e == cudaSuccess) return XTB_OK;
+  cudaFree(*buf);
+  return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+}
+
+// fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding
+// S = rows / T sequences of T steps; the Q values stay in fc2's output tensor.  h0 / hT: see qmix_gru_fwd_kernel.
+static int qmix_agent_forward(QmixAgent& a, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
+                              float* hT, int store, cudaStream_t st) {
+  const int H = a.H;
+  const float* W = P ? P : a.fc1->params;
+  const float *wg = W + a.o_gru, *bg = wg + 2 * H * 2 * H, *wc = bg + 2 * H, *bc = wc + 2 * H * H;
+  int rc = net_forward_impl(a.fc1, P, obs, nullptr, rows, st, 0u, 1u << 1);
+  if (rc) return rc;
+  const float* x = xtb_net_tensor(a.fc1, 1);
+  // the input projections of every step: x W[:H] + b for the gates and the candidate
+  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wg, 2 * H}, EpiBiasAct{a.xg, bg, 1.f, XTB_ACT_NONE, 2 * H, nullptr, 0}, rows,
+              2 * H, H, false, st);
+  LAUNCH_CHECK();
+  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wc, H}, EpiBiasAct{a.xc, bc, 1.f, XTB_ACT_NONE, H, nullptr, 0}, rows, H, H,
+              false, st);
+  LAUNCH_CHECK();
+  const int S = rows / T, G = a.G;
+  XLAUNCH(qmix_gru_fwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, wg, wc, a.xg, a.xc, h0, hT, a.hout, a.rh, seq_len, S, T,
+          a.n, H, G, store);
+  LAUNCH_CHECK();
+  return net_forward_impl(a.fc2, P ? P + a.o_fc2 : nullptr, a.hout, nullptr, rows, st, 0u, 1u << 1);
+}
+
+// Backward of qmix_agent_forward (store = 1, the eval set, all R rows) from d loss / d Q in fc2's output gradient: fc2
+// (with d loss / d GRU output), the GRU in reverse time, its weight gradients as GEMMs over all rows, fc1.
+static int qmix_agent_backward(QmixAgent& a, const float* obs, const int32_t* seq_len, cudaStream_t st) {
+  const int H = a.H, R = a.R, n = a.n;
+  const int32_t one[1] = {1};
+  BackwardOpts o2(one, 1);
+  o2.dobs = a.dy;
+  int rc = net_backward_impl(a.fc2, a.hout, nullptr, R, st, o2);
+  if (rc) return rc;
+  const float* W = a.fc1->params;
+  const float *wg = W + a.o_gru, *wc = wg + 2 * H * 2 * H + 2 * H;
+  float* gg = a.fc1->grads + a.o_gru;
+  float* gc = gg + 2 * H * 2 * H + 2 * H;
+  const int S = a.S, G = a.G;
+  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, wg, wc, (const float*)a.xg, (const float*)a.xc,
+          (const float*)a.hout, (const float*)a.dy, a.dag, a.dac, seq_len, S, a.T, a.n, H, G);
+  LAUNCH_CHECK();
+  const float* x = xtb_net_tensor(a.fc1, 1);
+  // [kernel; bias] gradients: [x | h_prev | 1]^T da_gates and [x | r h_prev | 1]^T da_candidate over all rows
+  launch_gemm(AGruFeat{x, a.hout, H, n, a.T, 1}, BRowMajor{a.dag, 2 * H}, EpiDgrad{gg, gg, 0, 2 * H, 0, nullptr, 0}, 2 * H + 1, 2 * H,
+              R, false, st);
+  LAUNCH_CHECK();
+  launch_gemm(AGruFeat{x, a.rh, H, n, a.T, 0}, BRowMajor{a.dac, H}, EpiDgrad{gc, gc, 0, H, 0, nullptr, 0}, 2 * H + 1, H, R, false, st);
+  LAUNCH_CHECK();
+  // d loss / d fc1 pre-activation = relu'(x) (da_gates W_g[:H]^T + da_candidate W_c[:H]^T)
+  float* dx = xtb_net_tensor_grad(a.fc1, 1);
+  launch_gemm(ADense<float>{a.dag, nullptr, 2 * H}, BTransposed{wg, 2 * H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 0, nullptr, 0}, R, H, 2 * H,
+              false, st);
+  LAUNCH_CHECK();
+  launch_gemm(ADense<float>{a.dac, nullptr, H}, BTransposed{wc, H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 1, nullptr, 0}, R, H, H, false, st);
+  LAUNCH_CHECK();
+  return net_backward_impl(a.fc1, obs, nullptr, R, st, BackwardOpts(one, 1));
+}
+
+// One step of the agent for one environment: fc1 -> GRU -> fc2 of the weight set `explore` on obs [n, obs_dim], hidden
+// [n, H] read and overwritten, q_out [n, A]
+static int qmix_agent_step(QmixAgent& a, const float* explore, const float* obs, float* hidden, float* q_out, cudaStream_t st) {
+  int rc = qmix_agent_forward(a, explore, obs, a.n, 1, a.ones, hidden, hidden, 0, st);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(a.fc2, 1), (size_t)a.n * a.A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return XTB_OK;
+}
+
+// xtb_qmix_infer and xtb_scc_infer: the agent step of object obj, graph-replayed under the object's tag and owners
+template <size_t N>
+static int agent_infer(const char* fn, GraphTag tag, const void* const (&owners)[N], const void* obj, QmixAgent& a, const float* explore,
+                       const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
+  if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, a.fc1, nullptr, a.n, true)) return rc;
+  return run_graph(capture_key(tag, owners, obj, explore, obs, hidden, q_out), use_graph, stream,
+                   [&](void* st) { return qmix_agent_step(a, explore, obs, hidden, q_out, S(st)); });
+}
+
+// ---- QMIX (xt/model/qmix/qmix_tf.py) ----------------------------------------------------------------------------------
+// The agent and the hypernetworks, an engine net bound to the slice after fc2 of the eval weight set; target and explore
+// sets are read through the nets' foreign-parameter forward.  The object owns the step's device scratch for the fixed
+// batch.
+struct xtb_qmix {
+  QmixAgent ag;
+  xtb_net* hyp = nullptr;
+  xtb_qmix_desc d{};
+  int E = 0, n_part = 0;
+  long long o_hyp = 0, n_params = 0;
+  void* buf = nullptr;
+  float *qt = nullptr, *w1t = nullptr, *b1t = nullptr, *wft = nullptr, *vt = nullptr, *part = nullptr;
 };
 // hyper net: tensor ids of the w1, b1, w_final and v heads
 static const int kQw1 = 2, kQb1 = 3, kQwf = 5, kQv = 7;
@@ -2652,67 +2818,32 @@ static const int kQw1 = 2, kQb1 = 3, kQwf = 5, kQv = 7;
 extern "C" int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyp, const xtb_qmix_desc* desc, xtb_qmix** out) {
   const char* fn = "xtb_qmix_create";
   if (!fc1 || !fc2 || !hyp || !desc || !out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
-  for (xtb_net* nt : {fc1, fc2, hyp})
-    if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
   const xtb_qmix_desc& d = *desc;
-  auto dense = [](const xtb_net* nt, int i, int src, int act) {
-    const LayerPlan& lp = nt->L[i];
-    return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
-  };
-  if (fc1->L.size() != 1 || !dense(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
-    return fail(XTB_ERR_ARG, "%s: fc1 must be one relu dense layer on float agent inputs", fn);
-  const int H = fc1->tsize[1];
-  if (fc2->L.size() != 1 || !dense(fc2, 0, 0, XTB_ACT_NONE) || fc2->tsize[0] != H)
-    return fail(XTB_ERR_ARG, "%s: fc2 must be one linear dense layer on the %d-wide GRU output", fn, H);
-  if (int rc = input_grad_check(fc2)) return rc;
-  const int A = fc2->tsize[1], n = d.n_agents;
-  if (hyp->L.size() != 7 || !dense(hyp, 0, 0, XTB_ACT_RELU) || !dense(hyp, 1, 1, XTB_ACT_NONE) || !dense(hyp, 2, 0, XTB_ACT_NONE) ||
-      !dense(hyp, 3, 0, XTB_ACT_RELU) || !dense(hyp, 4, 4, XTB_ACT_NONE) || !dense(hyp, 5, 0, XTB_ACT_RELU) || !dense(hyp, 6, 6, XTB_ACT_NONE))
+  QmixAgent ag;
+  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, d.n_agents, d.gru_off, &ag)) return rc;
+  if (!hyp->ws || !hyp->params || !hyp->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  if (hyp->L.size() != 7 || !dense_layer(hyp, 0, 0, XTB_ACT_RELU) || !dense_layer(hyp, 1, 1, XTB_ACT_NONE) ||
+      !dense_layer(hyp, 2, 0, XTB_ACT_NONE) || !dense_layer(hyp, 3, 0, XTB_ACT_RELU) || !dense_layer(hyp, 4, 4, XTB_ACT_NONE) ||
+      !dense_layer(hyp, 5, 0, XTB_ACT_RELU) || !dense_layer(hyp, 6, 6, XTB_ACT_NONE))
     return fail(XTB_ERR_ARG, "%s: hyper must be hyper_w1 (2 layers), hyper_b1, hyper_w_final (2 layers), val_for_bias (2 layers)", fn);
-  const int E = hyp->tsize[kQb1];
-  if (n < 1 || n > QM_MAX_AGENTS) return fail(XTB_ERR_ARG, "%s: n_agents %d not in [1, %d]", fn, n, QM_MAX_AGENTS);
-  if (A < 1 || A > 255) return fail(XTB_ERR_ARG, "%s: n_actions %d not in [1, 255] (actions are uint8 in the reference)", fn, A);
+  const int E = hyp->tsize[kQb1], n = ag.n;
   if (E < 1 || E > QM_MAX_EMBED || hyp->tsize[kQw1] != E * n || hyp->tsize[kQwf] != E || hyp->tsize[6] != E || hyp->tsize[kQv] != 1)
     return fail(XTB_ERR_ARG, "%s: mixer widths disagree (embed %d must be in [1, %d], w1 embed x n_agents, v 1)", fn, E, QM_MAX_EMBED);
-  if (d.batch < 1 || d.episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, d.batch, d.episode_limit);
-  const long long T = d.episode_limit + 1, R = (long long)d.batch * T * n, BL = (long long)d.batch * d.episode_limit;
-  if (R > (1LL << 30) / std::max(3 * H, 1)) return fail(XTB_ERR_ARG, "%s: batch too large", fn);
-  if (fc1->max_batch < R || fc2->max_batch < R || hyp->max_batch < BL)
-    return fail(XTB_ERR_ARG, "%s: nets hold fewer rows than a batch (fc1 / fc2: %lld, hyper: %lld)", fn, R, BL);
-  const int S = d.batch * n;
-  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
-  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
-  if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
-    return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
+  const long long R = ag.R, BL = ag.BL;
+  if (int rc = agent_capacity(fn, ag)) return rc;
+  if (hyp->max_batch < BL) return fail(XTB_ERR_ARG, "%s: hyper holds fewer rows than a batch (%lld)", fn, BL);
   // [fc1 | gru | fc2 | hyper] in one buffer, the gradients at the same offsets
-  const long long o_gru = d.gru_off, o_fc2 = fc2->params - fc1->params, o_hyp = hyp->params - fc1->params;
-  const long long gru_n = 2LL * H * 2 * H + 2 * H + 2LL * H * H + H;
-  if (o_gru < fc1->n_params || o_fc2 < o_gru + gru_n || o_hyp < o_fc2 + fc2->n_params || fc2->grads != fc1->grads + o_fc2 ||
-      hyp->grads != fc1->grads + o_hyp)
+  const long long o_hyp = hyp->params - fc1->params;
+  if (o_hyp < ag.o_fc2 + fc2->n_params || hyp->grads != fc1->grads + o_hyp)
     return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2 | hyper] of one buffer, in order", fn);
   auto* q = new xtb_qmix();
-  q->fc1 = fc1; q->fc2 = fc2; q->hyp = hyp; q->d = d;
-  q->B = d.batch; q->L = d.episode_limit; q->T = (int)T; q->n = n; q->A = A; q->H = H; q->E = E; q->R = (int)R; q->BL = (int)BL;
-  q->S = S; q->G = G; q->smem = qgru_smem_floats(H, G) * 4;
-  q->o_gru = o_gru; q->o_fc2 = o_fc2; q->o_hyp = o_hyp; q->n_params = o_hyp + hyp->n_params;
+  q->ag = ag; q->hyp = hyp; q->d = d; q->E = E; q->o_hyp = o_hyp; q->n_params = o_hyp + hyp->n_params;
   q->n_part = (int)((BL + QM_THREADS / 32 - 1) / (QM_THREADS / 32));
-  const long long sizes[] = {R * A, R * 2 * H, R * H, R * H, R * H, R * H, R * 2 * H, R * H, BL * n * E, BL * E, BL * E, BL, q->n_part + 2, n};
-  float** dst[] = {&q->qt, &q->xg, &q->xc, &q->hout, &q->rh, &q->dy, &q->dag, &q->dac, &q->w1t, &q->b1t, &q->wft, &q->vt, &q->part,
-                   (float**)&q->ones};
-  long long tot = 0;
-  for (long long s : sizes) tot += (s + 63) / 64 * 64;
-  cudaError_t e = cudaMalloc(&q->buf, tot * sizeof(float));
-  if (e != cudaSuccess) { delete q; return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e)); }
-  float* p = q->buf;
-  for (int i = 0; i < 14; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
-  std::vector<int32_t> ones(n, 1);
-  e = cudaMemset(q->buf, 0, tot * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemcpy(q->ones, ones.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice);
-  // The opt-in is a property of the kernel, shared by every live object: it is set to the most any object may use
-  // (this object's smem would shrink it under an earlier object with a wider GRU or more sequences per CTA).
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-  if (e != cudaSuccess) { cudaFree(q->buf); delete q; return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  if (int rc = agent_alloc(fn, q->ag, &q->buf, {{&q->qt, R * ag.A}, {&q->w1t, BL * n * E}, {&q->b1t, BL * E}, {&q->wft, BL * E},
+                                                 {&q->vt, BL}, {&q->part, q->n_part + 2}})) {
+    delete q;
+    return rc;
+  }
   *out = q;
   return XTB_OK;
 }
@@ -2725,81 +2856,10 @@ extern "C" void xtb_qmix_destroy(xtb_qmix* q) {
   delete q;
 }
 
-// The agent network (fc1 -> GRU -> fc2) is shared by QMIX and SCC: Q is xtb_qmix or xtb_scc, which both carry the nets,
-// the agent widths and the agent scratch under the same names.
-// fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding
-// S = rows / T sequences of T steps; the Q values stay in fc2's output tensor.  h0 / hT: see qmix_gru_fwd_kernel.
-template <class Q>
-static int qmix_agent_forward(Q* q, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
-                              float* hT, int store, cudaStream_t st) {
-  const int H = q->H;
-  const float* W = P ? P : q->fc1->params;
-  const float *wg = W + q->o_gru, *bg = wg + 2 * H * 2 * H, *wc = bg + 2 * H, *bc = wc + 2 * H * H;
-  int rc = net_forward_impl(q->fc1, P, obs, nullptr, rows, st, 0u, 1u << 1);
-  if (rc) return rc;
-  const float* x = xtb_net_tensor(q->fc1, 1);
-  // the input projections of every step: x W[:H] + b for the gates and the candidate
-  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wg, 2 * H}, EpiBiasAct{q->xg, bg, 1.f, XTB_ACT_NONE, 2 * H, nullptr, 0}, rows,
-              2 * H, H, false, st);
-  LAUNCH_CHECK();
-  launch_gemm(ADense<float>{x, nullptr, H}, BRowMajor{wc, H}, EpiBiasAct{q->xc, bc, 1.f, XTB_ACT_NONE, H, nullptr, 0}, rows, H, H,
-              false, st);
-  LAUNCH_CHECK();
-  const int S = rows / T, G = q->G;
-  XLAUNCH(qmix_gru_fwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, q->xg, q->xc, h0, hT, q->hout, q->rh, seq_len, S, T,
-          q->n, H, G, store);
-  LAUNCH_CHECK();
-  return net_forward_impl(q->fc2, P ? P + q->o_fc2 : nullptr, q->hout, nullptr, rows, st, 0u, 1u << 1);
-}
-
-// Backward of qmix_agent_forward (store = 1, the eval set, all R rows) from d loss / d Q in fc2's output gradient: fc2
-// (with d loss / d GRU output), the GRU in reverse time, its weight gradients as GEMMs over all rows, fc1.
-template <class Q>
-static int qmix_agent_backward(Q* q, const float* obs, const int32_t* seq_len, cudaStream_t st) {
-  const int H = q->H, R = q->R, n = q->n;
-  const int32_t one[1] = {1};
-  BackwardOpts o2(one, 1);
-  o2.dobs = q->dy;
-  int rc = net_backward_impl(q->fc2, q->hout, nullptr, R, st, o2);
-  if (rc) return rc;
-  const float* W = q->fc1->params;
-  const float *wg = W + q->o_gru, *wc = wg + 2 * H * 2 * H + 2 * H;
-  float* gg = q->fc1->grads + q->o_gru;
-  float* gc = gg + 2 * H * 2 * H + 2 * H;
-  const int S = q->S, G = q->G;
-  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, q->smem, st, wg, wc, (const float*)q->xg, (const float*)q->xc,
-          (const float*)q->hout, (const float*)q->dy, q->dag, q->dac, seq_len, S, q->T, q->n, H, G);
-  LAUNCH_CHECK();
-  const float* x = xtb_net_tensor(q->fc1, 1);
-  // [kernel; bias] gradients: [x | h_prev | 1]^T da_gates and [x | r h_prev | 1]^T da_candidate over all rows
-  launch_gemm(AGruFeat{x, q->hout, H, n, q->T, 1}, BRowMajor{q->dag, 2 * H}, EpiDgrad{gg, gg, 0, 2 * H, 0, nullptr, 0}, 2 * H + 1, 2 * H,
-              R, false, st);
-  LAUNCH_CHECK();
-  launch_gemm(AGruFeat{x, q->rh, H, n, q->T, 0}, BRowMajor{q->dac, H}, EpiDgrad{gc, gc, 0, H, 0, nullptr, 0}, 2 * H + 1, H, R, false, st);
-  LAUNCH_CHECK();
-  // d loss / d fc1 pre-activation = relu'(x) (da_gates W_g[:H]^T + da_candidate W_c[:H]^T)
-  float* dx = xtb_net_tensor_grad(q->fc1, 1);
-  launch_gemm(ADense<float>{q->dag, nullptr, 2 * H}, BTransposed{wg, 2 * H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 0, nullptr, 0}, R, H, 2 * H,
-              false, st);
-  LAUNCH_CHECK();
-  launch_gemm(ADense<float>{q->dac, nullptr, H}, BTransposed{wc, H}, EpiDgrad{dx, x, XTB_ACT_RELU, H, 1, nullptr, 0}, R, H, H, false, st);
-  LAUNCH_CHECK();
-  return net_backward_impl(q->fc1, obs, nullptr, R, st, BackwardOpts(one, 1));
-}
-
-// One step of the agent for one environment: fc1 -> GRU -> fc2 of the weight set `explore` on obs [n, obs_dim], hidden
-// [n, H] read and overwritten, q_out [n, A]
-template <class Q>
-static int qmix_agent_step(Q* q, const float* explore, const float* obs, float* hidden, float* q_out, cudaStream_t st) {
-  int rc = qmix_agent_forward(q, explore, obs, q->n, 1, q->ones, hidden, hidden, 0, st);
-  if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(q->fc2, 1), (size_t)q->n * q->A * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return XTB_OK;
-}
-
 static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qmix_batch& b, float* loss_out, cudaStream_t st) {
-  const int H = q->H, A = q->A, E = q->E, n = q->n, R = q->R, BL = q->BL;
-  xtb_net *fc1 = q->fc1, *fc2 = q->fc2, *hyp = q->hyp;
+  QmixAgent& a = q->ag;
+  const int A = a.A, E = q->E, n = a.n, R = a.R, BL = a.BL;
+  xtb_net *fc1 = a.fc1, *fc2 = a.fc2, *hyp = q->hyp;
   const unsigned heads = (1u << kQw1) | (1u << kQb1) | (1u << kQwf) | (1u << kQv);
   // target mixer's hypernetworks on the next states (kept), then the eval ones on the states
   int rc = net_forward_impl(hyp, target + q->o_hyp, b.next_state, nullptr, BL, st, 0u, heads);
@@ -2811,10 +2871,10 @@ static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, co
   rc = net_forward_impl(hyp, nullptr, b.state, nullptr, BL, st, 0u, heads);
   if (rc) return rc;
   // target agent (Q kept), then the eval agent with the activations of its backward
-  rc = qmix_agent_forward(q, target, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 0, st);
+  rc = qmix_agent_forward(a, target, b.obs, R, a.T, b.seq_len, nullptr, nullptr, 0, st);
   if (rc) return rc;
   CUDA_TRY(cudaMemcpyAsync(q->qt, xtb_net_tensor(fc2, 1), (size_t)R * A * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  rc = qmix_agent_forward(q, nullptr, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 1, st);
+  rc = qmix_agent_forward(a, nullptr, b.obs, R, a.T, b.seq_len, nullptr, nullptr, 1, st);
   if (rc) return rc;
   // mixers, TD loss and the gradients wrt the chosen Q and the hypernet outputs
   float* dq = xtb_net_tensor_grad(fc2, 1);
@@ -2825,7 +2885,7 @@ static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, co
   XLAUNCH(qmix_mix_td_kernel, q->n_part, QM_THREADS, 0, st, (const float*)xtb_net_tensor(fc2, 1), (const float*)q->qt, b.avail, b.actions,
           (const float*)xtb_net_tensor(hyp, kQw1), (const float*)xtb_net_tensor(hyp, kQb1), (const float*)xtb_net_tensor(hyp, kQwf),
           (const float*)xtb_net_tensor(hyp, kQv), (const float*)q->w1t, (const float*)q->b1t, (const float*)q->wft, (const float*)q->vt,
-          b.reward, b.terminated, b.mask, (const float*)msum, q->B, q->L, n, A, E, q->d.gamma, q->d.use_double_q, dq, xtb_net_tensor_grad(hyp, kQw1),
+          b.reward, b.terminated, b.mask, (const float*)msum, a.B, a.L, n, A, E, q->d.gamma, q->d.use_double_q, dq, xtb_net_tensor_grad(hyp, kQw1),
           xtb_net_tensor_grad(hyp, kQb1), xtb_net_tensor_grad(hyp, kQwf), xtb_net_tensor_grad(hyp, kQv), q->part);
   LAUNCH_CHECK();
   XLAUNCH(qmix_loss_kernel, 1, 32, 0, st, (const float*)q->part, q->n_part, (const float*)msum, loss_out);
@@ -2834,7 +2894,7 @@ static int qmix_train_launch(xtb_qmix* q, xtb_adam* opt, const float* target, co
   const int32_t hheads[4] = {kQw1, kQb1, kQwf, kQv};
   rc = net_backward_impl(hyp, b.state, nullptr, BL, st, BackwardOpts(hheads, 4));
   if (rc) return rc;
-  rc = qmix_agent_backward(q, b.obs, b.seq_len, st);
+  rc = qmix_agent_backward(a, b.obs, b.seq_len, st);
   if (rc) return rc;
   // clip_by_norm per variable + centred RMSProp over the eval set, then the nets' weight blobs
   rc = adam_step_impl(opt, fc1->params, fc1->grads, 1.f, st, nullptr);
@@ -2848,39 +2908,33 @@ extern "C" int xtb_qmix_train(xtb_qmix* q, xtb_adam* opt, const float* target, c
   if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
   const bool missing = !opt || !target || !batch || !loss_out || !batch->obs || !batch->seq_len || !batch->avail || !batch->actions ||
                        !batch->state || !batch->next_state || !batch->reward || !batch->terminated || !batch->mask;
-  if (int rc = learner_check(fn, missing, q->fc1, opt, q->R, false, q->R, q->n_params)) return rc;
+  if (int rc = learner_check(fn, missing, q->ag.fc1, opt, q->ag.R, false, q->ag.R, q->n_params)) return rc;
   if (!opt->mg) return fail(XTB_ERR_ARG, "%s: the optimiser must be centred RMSProp (xtb_opt_use_rmsprop)", fn);
   const xtb_qmix_batch b = *batch;
-  return run_graph(capture_key(kQmixTrain, {q->fc1, q->fc2, q->hyp, q, opt}, q, target, b.obs, b.seq_len, b.avail, b.actions, b.state,
-                               b.next_state, b.reward, b.terminated, b.mask, loss_out),
+  return run_graph(capture_key(kQmixTrain, {q->ag.fc1, q->ag.fc2, q->hyp, q, opt}, q, target, b.obs, b.seq_len, b.avail, b.actions,
+                               b.state, b.next_state, b.reward, b.terminated, b.mask, loss_out),
                    use_graph, stream, [&](void* st) { return qmix_train_launch(q, opt, target, b, loss_out, S(st)); });
 }
 
 extern "C" int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
-  const char* fn = "xtb_qmix_infer";
-  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
-  if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, q->fc1, nullptr, q->n, true)) return rc;
-  return run_graph(capture_key(kQmixInfer, {q->fc1, q->fc2, q->hyp, q}, q, explore, obs, hidden, q_out), use_graph, stream,
-                   [&](void* st) { return qmix_agent_step(q, explore, obs, hidden, q_out, S(st)); });
+  if (!q) return fail(XTB_ERR_ARG, "xtb_qmix_infer: null object");
+  return agent_infer("xtb_qmix_infer", kQmixInfer, {q->ag.fc1, q->ag.fc2, q->hyp, q}, q, q->ag, explore, obs, hidden, q_out, use_graph,
+                     stream);
 }
 
 // ---- SCC (xt/model/scc/scc_tf.py) ------------------------------------------------------------------------------------
-// The agent is QMIX's (qmix_agent_forward / _backward / _step); the critic's hidden layers are engine nets, one per agent
-// group (multi-channel) or one over the whole row, bound to slices of the eval set; the target critic is read through
-// their foreign-parameter forward.  See scc.cuh for the critic layout.
+// The agent is QMIX's; the critic's hidden layers are engine nets, one per agent group (multi-channel) or one over the
+// whole row, bound to slices of the eval set after fc2; the target critic is read through their foreign-parameter
+// forward.  See scc.cuh for the critic layout.
 struct xtb_scc {
-  xtb_net *fc1 = nullptr, *fc2 = nullptr;
+  QmixAgent ag;
   xtb_net* cn[SCC_MAX_GROUPS] = {};
   xtb_scc_desc d{};
-  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, R = 0, BL = 0, S = 0, G = 0;
   int ncn = 0, multi = 0, concat = 0, U = 0, D = 0, o = 0, mc = 1, V = 0, C = 0, K = 0, n_part = 0, n_chunk = 0;
   int a0[SCC_MAX_GROUPS + 1] = {};
-  size_t smem = 0;
-  long long o_gru = 0, o_fc2 = 0, o_mix = 0, o_head = 0, o_cn[SCC_MAX_GROUPS] = {}, agent_size = 0, n_params = 0;
-  float* buf = nullptr;
-  float *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr;
+  long long o_mix = 0, o_head = 0, o_cn[SCC_MAX_GROUPS] = {}, agent_size = 0, n_params = 0;
+  void* buf = nullptr;
   float *xs = nullptr, *xm = nullptr, *ht = nullptr, *hm = nullptr, *dv = nullptr, *part = nullptr, *hpart = nullptr;
-  int32_t* ones = nullptr;
 };
 
 // critic rows of group j (channel rows of the multi-channel critic, whole rows of the single-channel one) for `rows` states
@@ -2907,7 +2961,6 @@ extern "C" int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic
   if (!fc1 || !fc2 || !critic || !desc || !out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
   const xtb_scc_desc& d = *desc;
   const int n = d.n_agents;
-  if (n < 1 || n > QM_MAX_AGENTS) return fail(XTB_ERR_ARG, "%s: n_agents %d not in [1, %d]", fn, n, QM_MAX_AGENTS);
   if (d.n_groups < 0 || d.n_groups > SCC_MAX_GROUPS) return fail(XTB_ERR_ARG, "%s: n_groups %d not in [0, %d]", fn, d.n_groups, SCC_MAX_GROUPS);
   const int ncn = d.n_groups ? d.n_groups : 1;
   int a0[SCC_MAX_GROUPS + 1] = {0};
@@ -2923,54 +2976,35 @@ extern "C" int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic
   if (d.n_groups && d.channel_merge != 0 && d.channel_merge != 1)
     return fail(XTB_ERR_ARG, "%s: channel_merge %d is neither concat (0) nor add (1)", fn, d.channel_merge);
   if (n > 2 && d.mc_sample_times < 1) return fail(XTB_ERR_ARG, "%s: mc_sample_times %d < 1", fn, d.mc_sample_times);
-  if (d.batch < 1 || d.episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, d.batch, d.episode_limit);
-  for (xtb_net* nt : {fc1, fc2})
-    if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
+  QmixAgent ag;
+  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, n, d.gru_off, &ag)) return rc;
   for (int j = 0; j < ncn; j++)
     if (!critic[j] || !critic[j]->ws || !critic[j]->params || !critic[j]->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
-  auto dense = [](const xtb_net* nt, int i, int src, int act) {
-    const LayerPlan& lp = nt->L[i];
-    return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
-  };
-  if (fc1->L.size() != 1 || !dense(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
-    return fail(XTB_ERR_ARG, "%s: fc1 must be one relu dense layer on float agent inputs", fn);
-  const int H = fc1->tsize[1];
-  if (fc2->L.size() != 1 || !dense(fc2, 0, 0, XTB_ACT_NONE) || fc2->tsize[0] != H)
-    return fail(XTB_ERR_ARG, "%s: fc2 must be one linear dense layer on the %d-wide GRU output", fn, H);
-  if (int rc = input_grad_check(fc2)) return rc;
-  const int A = fc2->tsize[1];
-  if (A < 1 || A > 255) return fail(XTB_ERR_ARG, "%s: n_actions %d not in [1, 255] (actions are uint8 in the reference)", fn, A);
+  const int A = ag.A;
   const int U = critic[0]->L.empty() ? 0 : critic[0]->tsize[1];
   const int in_w = critic[0]->tsize[0];
   const int D = d.n_groups ? in_w : in_w / n, o = D - A;
   for (int j = 0; j < ncn; j++) {
     const xtb_net* c = critic[j];
-    if (c->L.size() != 2 || !dense(c, 0, 0, XTB_ACT_RELU) || !dense(c, 1, 1, XTB_ACT_RELU) || c->desc.input_u8 || c->desc.scale != 1.f ||
-        c->tsize[1] != U || c->tsize[2] != U || c->tsize[0] != in_w)
+    if (c->L.size() != 2 || !dense_layer(c, 0, 0, XTB_ACT_RELU) || !dense_layer(c, 1, 1, XTB_ACT_RELU) || c->desc.input_u8 ||
+        c->desc.scale != 1.f || c->tsize[1] != U || c->tsize[2] != U || c->tsize[0] != in_w)
       return fail(XTB_ERR_ARG, "%s: every critic net must be dense(U, relu) -> dense(U, relu) on the same float input", fn);
   }
   if (U < 1 || U > SCC_MAX_UNITS) return fail(XTB_ERR_ARG, "%s: dense_unit_number %d not in [1, %d]", fn, U, SCC_MAX_UNITS);
   if (o < 0 || (!d.n_groups && in_w != n * D))
     return fail(XTB_ERR_ARG, "%s: critic input %d is not n_agents x (obs + n_actions %d)", fn, in_w, A);
-  const long long T = d.episode_limit + 1, R = (long long)d.batch * T * n, BL = (long long)d.batch * d.episode_limit;
+  const long long BL = ag.BL;
   const int V = d.n_groups ? 0 : (n <= 2 ? n : 2 * n * d.mc_sample_times);
-  if (R > (1LL << 30) / std::max(3 * H, 1) || BL * n * std::max(D, U) * std::max(V, 1) > (1LL << 30))
-    return fail(XTB_ERR_ARG, "%s: batch too large", fn);
-  if (fc1->max_batch < R || fc2->max_batch < R) return fail(XTB_ERR_ARG, "%s: fc1 / fc2 hold fewer rows than a batch (%lld)", fn, R);
+  if (BL * n * std::max(D, U) * std::max(V, 1) > (1LL << 30)) return fail(XTB_ERR_ARG, "%s: batch too large", fn);
+  if (int rc = agent_capacity(fn, ag)) return rc;
   for (int j = 0; j < ncn; j++) {
     const long long need = d.n_groups ? BL * (a0[j + 1] - a0[j]) : BL * std::max(V, 1);
     if (critic[j]->max_batch < need) return fail(XTB_ERR_ARG, "%s: critic net %d holds fewer than %lld rows", fn, j, need);
   }
-  const int S = d.batch * n;
-  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
-  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
-  if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
-    return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
   // [fc1 | gru | fc2 | critic nets | head kernel, head bias] in one buffer, the gradients at the same offsets
   const int C = d.n_groups ? n : 1, concat = d.n_groups ? d.channel_merge == 0 : 1, K = concat ? C * U : U;
-  const long long o_gru = d.gru_off, o_fc2 = fc2->params - fc1->params, gru_n = 2LL * H * 2 * H + 2 * H + 2LL * H * H + H;
-  bool ok = o_gru >= fc1->n_params && o_fc2 >= o_gru + gru_n && fc2->grads == fc1->grads + o_fc2;
-  long long prev = o_fc2 + fc2->n_params, o_cn[SCC_MAX_GROUPS] = {};
+  bool ok = true;
+  long long prev = ag.o_fc2 + fc2->n_params, o_cn[SCC_MAX_GROUPS] = {};
   for (int j = 0; j < ncn && ok; j++) {
     o_cn[j] = critic[j]->params - fc1->params;
     ok = o_cn[j] >= prev && critic[j]->grads == fc1->grads + o_cn[j] && o_cn[j] % 4 == 0;
@@ -2979,35 +3013,22 @@ extern "C" int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic
   if (!ok || d.head_off < prev || d.head_off % 4 != 0)
     return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2 | critic nets | head] of one buffer, in order", fn);
   auto* q = new xtb_scc();
-  q->fc1 = fc1; q->fc2 = fc2; q->d = d;
+  q->ag = ag; q->d = d;
   for (int j = 0; j < ncn; j++) { q->cn[j] = critic[j]; q->o_cn[j] = o_cn[j]; }
   for (int j = 0; j <= ncn; j++) q->a0[j] = a0[j];
-  q->B = d.batch; q->L = d.episode_limit; q->T = (int)T; q->n = n; q->A = A; q->H = H; q->R = (int)R; q->BL = (int)BL;
-  q->S = S; q->G = G; q->smem = qgru_smem_floats(H, G) * 4;
   q->ncn = ncn; q->multi = d.n_groups > 0; q->concat = concat; q->U = U; q->D = D; q->o = o; q->mc = std::max(1, d.mc_sample_times);
   q->V = V; q->C = C; q->K = K;
-  q->o_gru = o_gru; q->o_fc2 = o_fc2; q->o_mix = o_cn[0]; q->o_head = d.head_off; q->agent_size = o_fc2 + fc2->n_params;
+  q->o_mix = o_cn[0]; q->o_head = d.head_off; q->agent_size = ag.o_fc2 + fc2->n_params;
   q->n_params = d.head_off + K + 1;
   q->n_part = (int)((BL + SCC_THREADS / 32 - 1) / (SCC_THREADS / 32));
   q->n_chunk = (int)((BL + SCC_HG_ROWS - 1) / SCC_HG_ROWS);
   const long long xm_n = q->multi ? BL * n * D : BL * n * D * V, hm_n = q->multi ? BL * n * U : BL * U * V;
-  const long long sizes[] = {R * 2 * H, R * H, R * H, R * H, R * H, R * 2 * H, R * H, BL * n * D, std::max(xm_n, 1LL), BL * C * U,
-                             std::max(hm_n, 1LL), BL, 2LL * q->n_part + 2, (long long)q->n_chunk * (K + 1), n};
-  float** dst[] = {&q->xg, &q->xc, &q->hout, &q->rh, &q->dy, &q->dag, &q->dac, &q->xs, &q->xm, &q->ht, &q->hm, &q->dv, &q->part,
-                   &q->hpart, (float**)&q->ones};
-  const int n_bufs = (int)(sizeof(sizes) / sizeof(sizes[0]));
-  long long tot = 0;
-  for (long long sz : sizes) tot += (sz + 63) / 64 * 64;
-  cudaError_t e = cudaMalloc(&q->buf, tot * sizeof(float));
-  if (e != cudaSuccess) { delete q; return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e)); }
-  float* p = q->buf;
-  for (int i = 0; i < n_bufs; i++) { *dst[i] = p; p += (sizes[i] + 63) / 64 * 64; }
-  std::vector<int32_t> ones(n, 1);
-  e = cudaMemset(q->buf, 0, tot * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemcpy(q->ones, ones.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-  if (e != cudaSuccess) { cudaFree(q->buf); delete q; return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  if (int rc = agent_alloc(fn, q->ag, &q->buf, {{&q->xs, BL * n * D}, {&q->xm, std::max(xm_n, 1LL)}, {&q->ht, BL * C * U},
+                                                 {&q->hm, std::max(hm_n, 1LL)}, {&q->dv, BL}, {&q->part, 2LL * q->n_part + 2},
+                                                 {&q->hpart, (long long)q->n_chunk * (K + 1)}})) {
+    delete q;
+    return rc;
+  }
   *out = q;
   return XTB_OK;
 }
@@ -3024,9 +3045,10 @@ static unsigned scc_grid(long long total) { return (unsigned)std::min<long long>
 
 static int scc_train_launch(xtb_scc* q, xtb_adam* copt, xtb_adam* aopt, const float* target, const xtb_scc_batch& b, float* loss_out,
                             cudaStream_t st) {
-  const int n = q->n, A = q->A, U = q->U, BL = q->BL, R = q->R;
+  QmixAgent& a = q->ag;
+  const int n = a.n, A = a.A, U = q->U, BL = a.BL, R = a.R;
   // critic inputs (shifted), sum of the mask
-  XLAUNCH(scc_inputs_kernel, scc_grid((long long)BL * n * q->D), 256, 0, st, b.raw_obs, b.actions, b.subsets, q->xs, q->xm, q->B, q->L, n,
+  XLAUNCH(scc_inputs_kernel, scc_grid((long long)BL * n * q->D), 256, 0, st, b.raw_obs, b.actions, b.subsets, q->xs, q->xm, a.B, a.L, n,
           q->o, A, q->multi, q->mc, scc_groups(q, nullptr, BL, q->D));
   LAUNCH_CHECK();
   float* msum = q->part + 2 * q->n_part;
@@ -3048,21 +3070,21 @@ static int scc_train_launch(xtb_scc* q, xtb_adam* copt, xtb_adam* aopt, const fl
     if (rc) return rc;
   }
   // the eval agent with the activations of its backward
-  int rc = qmix_agent_forward(q, nullptr, b.obs, R, q->T, b.seq_len, nullptr, nullptr, 1, st);
+  int rc = qmix_agent_forward(a, nullptr, b.obs, R, a.T, b.seq_len, nullptr, nullptr, 1, st);
   if (rc) return rc;
   // critic head, TD loss, credits, actor loss and their gradients
-  float* dq = xtb_net_tensor_grad(q->fc2, 1);
+  float* dq = xtb_net_tensor_grad(a.fc2, 1);
   CUDA_TRY(cudaMemsetAsync(dq, 0, (size_t)R * A * sizeof(float), st));
-  const float* P = q->fc1->params;
+  const float* P = a.fc1->params;
   SccStep sp{scc_nets(q, false), ht, hm, (long long)BL * U, scc_nets(q, true)};
-  XLAUNCH(scc_step_kernel, q->n_part, SCC_THREADS, 0, st, sp, P + q->o_head, target + q->o_head, (const float*)xtb_net_tensor(q->fc2, 1),
-          b.actions, b.reward, b.terminated, b.mask, (const float*)msum, q->B, q->L, n, A, U, q->concat, q->multi, q->mc, q->d.gamma,
+  XLAUNCH(scc_step_kernel, q->n_part, SCC_THREADS, 0, st, sp, P + q->o_head, target + q->o_head, (const float*)xtb_net_tensor(a.fc2, 1),
+          b.actions, b.reward, b.terminated, b.mask, (const float*)msum, a.B, a.L, n, A, U, q->concat, q->multi, q->mc, q->d.gamma,
           q->dv, dq, q->part);
   LAUNCH_CHECK();
   XLAUNCH(scc_head_grad_kernel, dim3(q->n_chunk, (q->K + 1 + 127) / 128), 128, 0, st, sp.eh, (const float*)q->dv, BL, U, q->concat,
           q->hpart);
   LAUNCH_CHECK();
-  XLAUNCH(scc_reduce_kernel, (q->K + 2 + 127) / 128, 128, 0, st, (const float*)q->hpart, q->n_chunk, q->K, q->fc1->grads + q->o_head,
+  XLAUNCH(scc_reduce_kernel, (q->K + 2 + 127) / 128, 128, 0, st, (const float*)q->hpart, q->n_chunk, q->K, a.fc1->grads + q->o_head,
           (const float*)q->part, q->n_part, (const float*)msum, n, loss_out);
   LAUNCH_CHECK();
   // backward: the critic nets, then the agent
@@ -3071,13 +3093,13 @@ static int scc_train_launch(xtb_scc* q, xtb_adam* copt, xtb_adam* aopt, const fl
     rc = net_backward_impl(q->cn[j], xs.h[j], nullptr, (int)scc_rows(q, j, BL), st, BackwardOpts(two, 1));
     if (rc) return rc;
   }
-  rc = qmix_agent_backward(q, b.obs, b.seq_len, st);
+  rc = qmix_agent_backward(a, b.obs, b.seq_len, st);
   if (rc) return rc;
   // Adam over the critic slice, RMSProp over the agent slice (each with its clip_by_norm), then the nets' weight blobs
-  rc = adam_step_impl(copt, q->fc1->params + q->o_mix, q->fc1->grads + q->o_mix, 1.f, st, nullptr);
-  if (!rc) rc = adam_step_impl(aopt, q->fc1->params, q->fc1->grads, 1.f, st, nullptr);
+  rc = adam_step_impl(copt, a.fc1->params + q->o_mix, a.fc1->grads + q->o_mix, 1.f, st, nullptr);
+  if (!rc) rc = adam_step_impl(aopt, a.fc1->params, a.fc1->grads, 1.f, st, nullptr);
   for (int j = 0; j < q->ncn && !rc; j++) rc = xtb_net_sync_weights(q->cn[j], st);
-  for (xtb_net* nt : {q->fc1, q->fc2}) if (!rc) rc = xtb_net_sync_weights(nt, st);
+  for (xtb_net* nt : {a.fc1, a.fc2}) if (!rc) rc = xtb_net_sync_weights(nt, st);
   return rc;
 }
 
@@ -3086,35 +3108,33 @@ extern "C" int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_o
   const char* fn = "xtb_scc_train";
   if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
   const bool missing = !critic_opt || !actor_opt || !target || !batch || !loss_out || !batch->obs || !batch->raw_obs || !batch->seq_len ||
-                       !batch->actions || !batch->reward || !batch->terminated || !batch->mask || (!q->multi && q->n > 2 && !batch->subsets);
-  if (int rc = learner_check(fn, missing, q->fc1, actor_opt, q->R, false, q->R, q->agent_size)) return rc;
+                       !batch->actions || !batch->reward || !batch->terminated || !batch->mask || (!q->multi && q->ag.n > 2 && !batch->subsets);
+  if (int rc = learner_check(fn, missing, q->ag.fc1, actor_opt, q->ag.R, false, q->ag.R, q->agent_size)) return rc;
   if (critic_opt->count != q->n_params - q->o_mix)
     return fail(XTB_ERR_ARG, "%s: critic optimiser size %lld != %lld", fn, critic_opt->count, q->n_params - q->o_mix);
   if (critic_opt->mg || critic_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the critic optimiser must be Adam", fn);
   if (!actor_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the actor optimiser must be uncentred RMSProp (xtb_opt_use_rmsprop_plain)", fn);
   const xtb_scc_batch b = *batch;
-  return run_graph(capture_key(kSccTrain, {q->fc1, q->cn[0], q, critic_opt, actor_opt}, q, target, b.obs, b.raw_obs, b.seq_len,
+  return run_graph(capture_key(kSccTrain, {q->ag.fc1, q->cn[0], q, critic_opt, actor_opt}, q, target, b.obs, b.raw_obs, b.seq_len,
                                b.actions, b.reward, b.terminated, b.mask, b.subsets, loss_out),
                    use_graph, stream, [&](void* st) { return scc_train_launch(q, critic_opt, actor_opt, target, b, loss_out, S(st)); });
 }
 
 extern "C" int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
-  const char* fn = "xtb_scc_infer";
-  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
-  if (int rc = learner_check(fn, !explore || !obs || !hidden || !q_out, q->fc1, nullptr, q->n, true)) return rc;
-  return run_graph(capture_key(kSccInfer, {q->fc1, q->fc2, q}, q, explore, obs, hidden, q_out), use_graph, stream,
-                   [&](void* st) { return qmix_agent_step(q, explore, obs, hidden, q_out, S(st)); });
+  if (!q) return fail(XTB_ERR_ARG, "xtb_scc_infer: null object");
+  return agent_infer("xtb_scc_infer", kSccInfer, {q->ag.fc1, q->ag.fc2, q}, q, q->ag, explore, obs, hidden, q_out, use_graph, stream);
 }
 
 extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream) {
   const char* fn = "xtb_scc_critic";
   if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
-  if (int rc = learner_check(fn, !states || !v_out, q->fc1, nullptr, rows, true, q->BL)) return rc;
-  return run_graph(capture_key(kSccCritic, {q->fc1, q->cn[0], q}, q, states, rows, v_out), use_graph, stream, [&](void* sv) -> int {
+  if (int rc = learner_check(fn, !states || !v_out, q->ag.fc1, nullptr, rows, true, q->ag.BL)) return rc;
+  return run_graph(capture_key(kSccCritic, {q->ag.fc1, q->cn[0], q}, q, states, rows, v_out), use_graph, stream, [&](void* sv) -> int {
     cudaStream_t st = S(sv);
     const float* in = states;
+    const int n = q->ag.n;
     if (q->multi) {
-      XLAUNCH(scc_split_kernel, scc_grid((long long)rows * q->n * q->D), 256, 0, st, states, q->xs, rows, q->n, q->D,
+      XLAUNCH(scc_split_kernel, scc_grid((long long)rows * n * q->D), 256, 0, st, states, q->xs, rows, n, q->D,
               scc_groups(q, nullptr, rows, q->D));
       LAUNCH_CHECK();
       in = q->xs;
@@ -3125,7 +3145,7 @@ extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* 
       if (rc) return rc;
     }
     XLAUNCH(scc_value_kernel, (rows + SCC_THREADS / 32 - 1) / (SCC_THREADS / 32), SCC_THREADS, 0, st, scc_nets(q, false),
-            (const float*)(q->fc1->params + q->o_head), rows, q->U, q->concat, v_out);
+            (const float*)(q->ag.fc1->params + q->o_head), rows, q->U, q->concat, v_out);
     LAUNCH_CHECK();
     return XTB_OK;
   });

@@ -31,14 +31,28 @@ def _align(x):
 
 @Registers.model
 class QMixModel(XTModel):
-    """QMixModel (qmix_tf.py:23-589).  model_info["scene"] = "explore" builds the acting network only, "train" all five."""
+    """QMixModel (qmix_tf.py:23-589).  model_info["scene"] = "explore" builds the acting network only, "train" all five.
+
+    SCCModel shares the agent: its config fields, nets and variable table, its weight sets, the explore step and the
+    native object's lifetime (the entry points named by _native)."""
+
+    _native = "xtb_qmix"   # the native object's entry points: <_native>_infer and <_native>_destroy
 
     def __init__(self, model_info):
+        model_config = self._agent_config(model_info)
+        self.lr = model_config.get("lr", 0.0005)
+        self.grad_norm_clip = model_config.get("grad_norm_clip", 10)
+        self.embed_dim = int(model_config["mixing_embed_dim"])
+        self.use_double_q = bool(model_config.get("use_double_q", True))
+        # read by the train graph only (_build_mix_net2), as in the reference
+        self.hypernet_embed = int(model_config["hypernet_embed"]) if self.g_type == "train" else int(model_config.get("hypernet_embed", 1))
+        super().__init__(model_info)
+
+    def _agent_config(self, model_info):
+        """The model_config fields of the agent and its training batch -> model_config."""
         model_config = model_info.get("model_config", None) or {}
         self.model_config = model_config
         self.gamma = model_config.get("gamma", 0.99)
-        self.lr = model_config.get("lr", 0.0005)
-        self.grad_norm_clip = model_config.get("grad_norm_clip", 10)
         self.n_agents = int(model_config["n_agents"])
         self.obs_shape = int(model_config["obs_shape"])
         self.rnn_hidden_dim = int(model_config["rnn_hidden_dim"])
@@ -47,23 +61,14 @@ class QMixModel(XTModel):
         self.batch_size = int(model_config["batch_size"])
         self.avail_action_num = self.n_actions
         self.state_dim = int(np.prod(model_config["state_shape"]))
-        self.embed_dim = int(model_config["mixing_embed_dim"])
-        self.use_double_q = bool(model_config.get("use_double_q", True))
         self.g_type = model_info.get("scene", "explore")
-        # read by the train graph only (_build_mix_net2), as in the reference
-        self.hypernet_embed = int(model_config["hypernet_embed"]) if self.g_type == "train" else int(model_config.get("hypernet_embed", 1))
-        super().__init__(model_info)
+        return model_config
 
     # ---- construction ---------------------------------------------------------------------------------------------
     def create_model(self, model_info):
-        H, A, n, E, he = self.rnn_hidden_dim, self.n_actions, self.n_agents, self.embed_dim, self.hypernet_embed
+        n, E, he = self.n_agents, self.embed_dim, self.hypernet_embed
         train = self.g_type == "train"
-        # the explore scene keeps a minimal training shape: only the one-step inference runs
-        B, L = (self.batch_size, self.fix_seq_length) if train else (1, 1)
-        rows, state_rows = B * (L + 1) * n, B * L
-        fc1_a = dict(input_dtype="float32", state_dim=(self.obs_shape,), scale=1.0,
-                     layers=[("dense", "dense", "obs", dict(n=H, act="relu"))])
-        fc2_a = dict(input_dtype="float32", state_dim=(H,), scale=1.0, layers=[("dense_1", "dense", "obs", dict(n=A, act=None))])
+        B, L = self._agent_nets(train)
         hyp_a = dict(input_dtype="float32", state_dim=(self.state_dim,), scale=1.0, layers=[
             ("hyper_w1/dense", "dense", "obs", dict(n=he, act="relu")),
             ("hyper_w1/dense_1", "dense", "hyper_w1/dense", dict(n=E * n, act=None)),
@@ -73,44 +78,13 @@ class QMixModel(XTModel):
             ("val_for_bias/dense", "dense", "obs", dict(n=E, act="relu")),
             ("val_for_bias/dense_1", "dense", "val_for_bias/dense", dict(n=1, act=None)),
         ])
-        self.fc1 = Net(fc1_a, max_batch=rows, device=self.device)
-        self.fc2 = Net(fc2_a, max_batch=rows, device=self.device)
-        self.hyper = Net(hyp_a, max_batch=state_rows, device=self.device)
-        gru = OrderedDict([("rnn/gru_cell/gates/kernel", (2 * H, 2 * H)), ("rnn/gru_cell/gates/bias", (2 * H,)),
-                           ("rnn/gru_cell/candidate/kernel", (2 * H, H)), ("rnn/gru_cell/candidate/bias", (H,))])
-        self.gru_off = _align(self.fc1.n_params)
-        o_fc2 = _align(self.gru_off + sum(int(np.prod(s)) for s in gru.values()))
-        o_hyp = _align(o_fc2 + self.fc2.n_params)
-        self.agent_size = o_fc2 + self.fc2.n_params
+        self.hyper = Net(hyp_a, max_batch=B * L, device=self.device)
+        o_hyp = _align(self.agent_size)
         self.n_params = o_hyp + self.hyper.n_params
-        # variable tables: name -> (offset in a weight set, shape), in TF variable order
-        self.agent_vars, self.mixer_vars = OrderedDict(), OrderedDict()
-        for name, (off, shape) in self.fc1.ptable.items():
-            self.agent_vars[name] = (off, shape)
-        off = self.gru_off
-        for name, shape in gru.items():
-            self.agent_vars[name] = (off, shape)
-            off += int(np.prod(shape))
-        for name, (o, shape) in self.fc2.ptable.items():
-            self.agent_vars[name] = (o_fc2 + o, shape)
         for name, (o, shape) in self.hyper.ptable.items():
             self.mixer_vars[name] = (o_hyp + o, shape)
+        self._weight_sets([(self.hyper, o_hyp)], target_agent=True)
         dev = self.device
-        self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.grads = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.target = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.explore = torch.zeros(self.agent_size, dtype=torch.float32, device=dev)
-        for net, o in ((self.fc1, 0), (self.fc2, o_fc2), (self.hyper, o_hyp)):
-            net.bind_to(self.params[o:o + net.n_params], self.grads[o:o + net.n_params])
-        # each sub-graph initialised on its own, in the order the reference builds them
-        self._init_set(self.explore, self.agent_vars)
-        if train:
-            self._init_set(self.params, self.agent_vars)
-            self._init_set(self.target, self.agent_vars)
-            self._init_set(self.params, self.mixer_vars)
-            self._init_set(self.target, self.mixer_vars)
-        for net in (self.fc1, self.fc2, self.hyper):
-            net.params_changed()
         self.opt = None
         if train:
             starts = [o for o, _ in list(self.agent_vars.values()) + list(self.mixer_vars.values())] + [self.n_params]
@@ -124,13 +98,67 @@ class QMixModel(XTModel):
         self.handle = C.c_void_p()
         with torch.cuda.device(dev):
             check(capi.lib().xtb_qmix_create(self.fc1.handle, self.fc2.handle, self.hyper.handle, C.byref(desc), C.byref(self.handle)))
+        self._acting_state()
+        return self.fc1
+
+    def _agent_nets(self, train):
+        """fc1 and fc2 for the scene's training batch and the agent's variable table -> (batch, episode limit).  The
+        explore scene keeps a minimal training shape: only the one-step inference runs."""
+        H, A, n = self.rnn_hidden_dim, self.n_actions, self.n_agents
+        B, L = (self.batch_size, self.fix_seq_length) if train else (1, 1)
+        fc1_a = dict(input_dtype="float32", state_dim=(self.obs_shape,), scale=1.0,
+                     layers=[("dense", "dense", "obs", dict(n=H, act="relu"))])
+        fc2_a = dict(input_dtype="float32", state_dim=(H,), scale=1.0, layers=[("dense_1", "dense", "obs", dict(n=A, act=None))])
+        self.fc1 = Net(fc1_a, max_batch=B * (L + 1) * n, device=self.device)
+        self.fc2 = Net(fc2_a, max_batch=B * (L + 1) * n, device=self.device)
+        gru = OrderedDict([("rnn/gru_cell/gates/kernel", (2 * H, 2 * H)), ("rnn/gru_cell/gates/bias", (2 * H,)),
+                           ("rnn/gru_cell/candidate/kernel", (2 * H, H)), ("rnn/gru_cell/candidate/bias", (H,))])
+        self.gru_off = _align(self.fc1.n_params)
+        self.o_fc2 = _align(self.gru_off + sum(int(np.prod(s)) for s in gru.values()))
+        self.agent_size = self.o_fc2 + self.fc2.n_params
+        # variable tables: name -> (offset in a weight set, shape), in TF variable order
+        self.agent_vars, self.mixer_vars = OrderedDict(), OrderedDict()
+        for name, (off, shape) in self.fc1.ptable.items():
+            self.agent_vars[name] = (off, shape)
+        off = self.gru_off
+        for name, shape in gru.items():
+            self.agent_vars[name] = (off, shape)
+            off += int(np.prod(shape))
+        for name, (o, shape) in self.fc2.ptable.items():
+            self.agent_vars[name] = (self.o_fc2 + o, shape)
         self._B, self._L = B, L
-        self.hidden = torch.zeros(n, H, dtype=torch.float32, device=dev)
+        return B, L
+
+    def _weight_sets(self, mixer_nets, target_agent):
+        """The eval set (with its gradients), the target set and the explore agent, with fc1, fc2 and mixer_nets
+        [(net, offset)] bound to the eval set.  Each sub-graph is initialised on its own, in the order the reference
+        builds them; target_agent: the train graph has a target agent."""
+        dev = self.device
+        self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
+        self.grads = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
+        self.target = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
+        self.explore = torch.zeros(self.agent_size, dtype=torch.float32, device=dev)
+        nets = [(self.fc1, 0), (self.fc2, self.o_fc2)] + mixer_nets
+        for net, o in nets:
+            net.bind_to(self.params[o:o + net.n_params], self.grads[o:o + net.n_params])
+        self._init_set(self.explore, self.agent_vars)
+        if self.g_type == "train":
+            self._init_set(self.params, self.agent_vars)
+            if target_agent:
+                self._init_set(self.target, self.agent_vars)
+            self._init_set(self.params, self.mixer_vars)
+            self._init_set(self.target, self.mixer_vars)
+        for net, _ in nets:
+            net.params_changed()
+
+    def _acting_state(self):
+        """The hidden state and the one-step inference's staging; the training buffers are made at first use."""
+        n, dev = self.n_agents, self.device
+        self.hidden = torch.zeros(n, self.rnn_hidden_dim, dtype=torch.float32, device=dev)
         self._io = dict(obs1=torch.empty(n, self.obs_shape, dtype=torch.float32, device=dev),
-                        q1=torch.empty(n, A, dtype=torch.float32, device=dev))
+                        q1=torch.empty(n, self.n_actions, dtype=torch.float32, device=dev))
         self._bufs = None
         self.net = self.fc1
-        return self.fc1
 
     def _init_set(self, flat, table):
         """TF 1.15 initialisers: glorot_uniform kernels (dense and GRUCell alike), zero biases except the GRU gates bias,
@@ -148,7 +176,7 @@ class QMixModel(XTModel):
     def __del__(self):
         try:
             if getattr(self, "handle", None) and self.handle.value:
-                capi.lib().xtb_qmix_destroy(self.handle)
+                getattr(capi.lib(), self._native + "_destroy")(self.handle)
                 self.handle = C.c_void_p()
         except Exception:
             pass
@@ -216,8 +244,8 @@ class QMixModel(XTModel):
         x = np.asarray(agent_inputs, dtype=np.float32).reshape(self.n_agents, self.obs_shape)
         io = self._io
         stage_h2d(io["obs1"], x, np.float32)
-        check(capi.lib().xtb_qmix_infer(self.handle, _ptr(self.explore), _ptr(io["obs1"]), _ptr(self.hidden), _ptr(io["q1"]),
-                                        1 if self.use_graph else 0, stream_ptr()))
+        check(getattr(capi.lib(), self._native + "_infer")(self.handle, _ptr(self.explore), _ptr(io["obs1"]), _ptr(self.hidden),
+                                                           _ptr(io["q1"]), 1 if self.use_graph else 0, stream_ptr()))
         return io["q1"].cpu().numpy().reshape(1, self.n_agents, self.n_actions)
 
     # ---- training ---------------------------------------------------------------------------------------------------
@@ -234,10 +262,9 @@ class QMixModel(XTModel):
                               loss=torch.zeros(1, **f32))
         return self._bufs
 
-    def train(self, batch_trajectories, train_obs_len, avail_actions, actions, cur_stats, target_stats, rewards, terminated, mask):
-        """qmix_tf.py:546-589: one RMSProp step on a [batch_size, episode_limit (+1), ...] batch -> loss."""
-        if self.opt is None:
-            raise RuntimeError("QMixModel.train needs the train scene")
+    def _agent_batch(self, train_obs_len, actions):
+        """A train call's sequence lengths [batch_size * n_agents] and actions [batch_size, episode_limit, n_agents],
+        checked -> (seq_len, actions)."""
         B, L, n, A = self._B, self._L, self.n_agents, self.n_actions
         seq_len = np.asarray(train_obs_len).reshape(-1)
         if seq_len.size != B * n or np.any(seq_len < 0) or np.any(seq_len > L + 1):
@@ -245,6 +272,13 @@ class QMixModel(XTModel):
         act = np.asarray(actions).reshape(B, L, n)
         if np.any(act < 0) or np.any(act >= A):
             raise ValueError("actions must be in [0, {})".format(A))
+        return seq_len, act
+
+    def train(self, batch_trajectories, train_obs_len, avail_actions, actions, cur_stats, target_stats, rewards, terminated, mask):
+        """qmix_tf.py:546-589: one RMSProp step on a [batch_size, episode_limit (+1), ...] batch -> loss."""
+        if self.opt is None:
+            raise RuntimeError("QMixModel.train needs the train scene")
+        seq_len, act = self._agent_batch(train_obs_len, actions)
         b = self._train_buffers()
         stage_h2d(b["obs"], batch_trajectories, np.float32)
         stage_h2d(b["seq_len"], seq_len, np.int32)

@@ -8,7 +8,6 @@ agent, so only the critic part of the target set is used.  The training step (xt
 (xtb_scc_infer) and the critic (xtb_scc_critic) run in libxtb200."""
 import ctypes as C
 import random
-from collections import OrderedDict
 from types import SimpleNamespace
 
 import numpy as np
@@ -28,29 +27,20 @@ AGENT_GROUPS = {"2s3z": [2, 3], "3s5z": [3, 5], "3s5z_vs_3s6z": [3, 5], "1c3s5z"
 @Registers.model
 class SCCModel(QMixModel):
     """SCCModel (scc_tf.py:39-707).  model_info["scene"] = "explore" builds the acting network only, "train" also the
-    eval agent and both critics.  Weights, saving and the explore step are QMixModel's."""
+    eval agent and both critics.  The agent, weights, saving and the explore step are QMixModel's."""
+
+    _native = "xtb_scc"
 
     def __init__(self, model_info):
-        model_config = model_info.get("model_config", None) or {}
-        self.model_config = model_config
+        model_config = self._agent_config(model_info)
         map_name = model_config["map_name"]
         self.agent_group = list(AGENT_GROUPS[map_name]) if map_name in AGENT_GROUPS else [model_config["n_agents"]]
-        self.gamma = model_config.get("gamma", 0.99)
         self.c_lr = model_config.get("c_lr", 0.0005)
         self.a_lr = model_config.get("a_lr", 0.0005)
         self.mixer_grad_norm_clip = model_config.get("mixer_grad_norm_clip", 10)
         self.actor_grad_norm_clip = model_config.get("actor_grad_norm_clip", 10)
-        self.n_agents = int(model_config["n_agents"])
-        self.rnn_hidden_dim = int(model_config["rnn_hidden_dim"])
-        self.fix_seq_length = int(model_config["episode_limit"])
-        self.n_actions = int(model_config["n_actions"])
-        self.obs_shape = int(model_config["obs_shape"])
-        self.batch_size = int(model_config["batch_size"])
-        self.avail_action_num = self.n_actions
-        self.state_dim = int(np.prod(model_config["state_shape"]))
         self.use_double_q = model_config.get("use_double_q", True)
         self.o_shape = self.obs_shape - self.n_actions - self.n_agents
-        self.g_type = model_info.get("scene", "explore")
         if self.g_type == "train":
             # read when the train graph is built (scc_tf.py:280-313, 379-380)
             if not self.use_double_q:
@@ -65,29 +55,9 @@ class SCCModel(QMixModel):
 
     # ---- construction ---------------------------------------------------------------------------------------------
     def create_model(self, model_info):
-        H, A, n = self.rnn_hidden_dim, self.n_actions, self.n_agents
+        A, n = self.n_actions, self.n_agents
         train = self.g_type == "train"
-        B, L = (self.batch_size, self.fix_seq_length) if train else (1, 1)
-        rows = B * (L + 1) * n
-        fc1_a = dict(input_dtype="float32", state_dim=(self.obs_shape,), scale=1.0,
-                     layers=[("dense", "dense", "obs", dict(n=H, act="relu"))])
-        fc2_a = dict(input_dtype="float32", state_dim=(H,), scale=1.0, layers=[("dense_1", "dense", "obs", dict(n=A, act=None))])
-        self.fc1 = Net(fc1_a, max_batch=rows, device=self.device)
-        self.fc2 = Net(fc2_a, max_batch=rows, device=self.device)
-        gru = OrderedDict([("rnn/gru_cell/gates/kernel", (2 * H, 2 * H)), ("rnn/gru_cell/gates/bias", (2 * H,)),
-                           ("rnn/gru_cell/candidate/kernel", (2 * H, H)), ("rnn/gru_cell/candidate/bias", (H,))])
-        self.gru_off = _align(self.fc1.n_params)
-        o_fc2 = _align(self.gru_off + sum(int(np.prod(s)) for s in gru.values()))
-        self.agent_size = o_fc2 + self.fc2.n_params
-        self.agent_vars, self.mixer_vars = OrderedDict(), OrderedDict()
-        for name, (off, shape) in self.fc1.ptable.items():
-            self.agent_vars[name] = (off, shape)
-        off = self.gru_off
-        for name, shape in gru.items():
-            self.agent_vars[name] = (off, shape)
-            off += int(np.prod(shape))
-        for name, (o, shape) in self.fc2.ptable.items():
-            self.agent_vars[name] = (o_fc2 + o, shape)
+        B, L = self._agent_nets(train)
         self.critics = []
         end = self.agent_size
         if train:
@@ -116,21 +86,9 @@ class SCCModel(QMixModel):
             self.mixer_vars["v/bias"] = (o + K, (1,))
             end = o + K + 1
         self.n_params = end
+        # the sub-graphs initialised as scc_tf.py:180-182, 321-391 builds them: the train graph has no target agent
+        self._weight_sets([(c, c.o) for c in self.critics], target_agent=False)
         dev = self.device
-        self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.grads = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.target = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.explore = torch.zeros(self.agent_size, dtype=torch.float32, device=dev)
-        for net, o in [(self.fc1, 0), (self.fc2, o_fc2)] + [(c, c.o) for c in self.critics]:
-            net.bind_to(self.params[o:o + net.n_params], self.grads[o:o + net.n_params])
-        # each sub-graph initialised on its own, in the order the reference builds them (scc_tf.py:180-182, 321-391)
-        self._init_set(self.explore, self.agent_vars)
-        if train:
-            self._init_set(self.params, self.agent_vars)
-            self._init_set(self.params, self.mixer_vars)
-            self._init_set(self.target, self.mixer_vars)
-        for net in [self.fc1, self.fc2] + self.critics:
-            net.params_changed()
         self.opt = self.critic_opt = None
         desc = capi.SccDesc()
         desc.batch, desc.episode_limit, desc.n_agents, desc.gamma, desc.gru_off = B, L, n, float(self.gamma), self.gru_off
@@ -165,13 +123,8 @@ class SCCModel(QMixModel):
                 check(capi.lib().xtb_scc_create(self.fc1.handle, self.fc2.handle, nets, C.byref(desc), C.byref(self.handle)))
         else:
             self._explore_handle()
-        self._B, self._L = B, L
-        self.hidden = torch.zeros(n, H, dtype=torch.float32, device=dev)
-        self._io = dict(obs1=torch.empty(n, self.obs_shape, dtype=torch.float32, device=dev),
-                        q1=torch.empty(n, A, dtype=torch.float32, device=dev))
-        self._bufs = None
+        self._acting_state()
         self.mixer_loss = self.actor_loss = None
-        self.net = self.fc1
         return self.fc1
 
     def _explore_handle(self):
@@ -199,30 +152,11 @@ class SCCModel(QMixModel):
         with torch.cuda.device(self.device):
             check(capi.lib().xtb_scc_create(self.fc1.handle, self.fc2.handle, nets, C.byref(desc), C.byref(self.handle)))
 
-    def __del__(self):
-        try:
-            if getattr(self, "handle", None) and self.handle.value:
-                capi.lib().xtb_scc_destroy(self.handle)
-                self.handle = C.c_void_p()
-        except Exception:
-            pass
-
     # ---- weights ----------------------------------------------------------------------------------------------------
     def assign_targets(self):
         """eval mixer -> target mixer (scc_tf.py:450-457); the agent has no target."""
         if self.mixer_vars:
             self.target[self.o_mix:].copy_(self.params[self.o_mix:])
-
-    # ---- acting -----------------------------------------------------------------------------------------------------
-    def infer_actions(self, agent_inputs):
-        """Q values [1, n_agents, n_actions] of agent_inputs [1, 1, n_agents, obs_shape]; the hidden state stays on the
-        device between calls."""
-        x = np.asarray(agent_inputs, dtype=np.float32).reshape(self.n_agents, self.obs_shape)
-        io = self._io
-        stage_h2d(io["obs1"], x, np.float32)
-        check(capi.lib().xtb_scc_infer(self.handle, _ptr(self.explore), _ptr(io["obs1"]), _ptr(self.hidden), _ptr(io["q1"]),
-                                       1 if self.use_graph else 0, stream_ptr()))
-        return io["q1"].cpu().numpy().reshape(1, self.n_agents, self.n_actions)
 
     # ---- critic -----------------------------------------------------------------------------------------------------
     def _require_train(self, what):
@@ -319,16 +253,11 @@ class SCCModel(QMixModel):
         """scc_tf.py:505-564: the critic's Adam step and the agents' RMSProp step on one batch -> actor loss + mixer loss
         (both kept: self.mixer_loss, self.actor_loss).  avail_actions and the states are not read by the train graph."""
         self._require_train("train")
-        B, L, n, A = self._B, self._L, self.n_agents, self.n_actions
+        B, L, n = self._B, self._L, self.n_agents
         raw = np.asarray(obs)
         if raw.shape[-1] != self.o_shape:
             raise ValueError("obs is {} wide, not obs_shape - n_actions - n_agents = {}".format(raw.shape[-1], self.o_shape))
-        seq_len = np.asarray(train_obs_len).reshape(-1)
-        if seq_len.size != B * n or np.any(seq_len < 0) or np.any(seq_len > L + 1):
-            raise ValueError("train_obs_len: {} lengths in [0, {}] expected".format(B * n, L + 1))
-        act = np.asarray(actions).reshape(B, L, n)
-        if np.any(act < 0) or np.any(act >= A):
-            raise ValueError("actions must be in [0, {})".format(A))
+        seq_len, act = self._agent_batch(train_obs_len, actions)
         subsets = self.draw_subsets() if n > 2 else None
         b = self._train_buffers()
         stage_h2d(b["obs"], batch_trajectories, np.float32)
