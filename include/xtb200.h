@@ -110,6 +110,7 @@ long long xtb_graph_replay_count(void);
 /* ---- network: replaces XTModel's TF graph (xt/model/model.py:30-127) ---------- */
 /* Flat fp32 parameter layout: per layer, kernel [K,N] (HWIO flattened) then bias [N];
  * identical to iterating TFVariables' ordered dict (xt/model/tf_utils.py:84-102). */
+/* xtb_net_create plans on the host and makes no CUDA call: it needs no device. */
 int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net** out);
 void xtb_net_destroy(xtb_net* net);
 long long xtb_net_param_count(const xtb_net* net);

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -61,6 +62,36 @@ extern "C" long long xtb_launch_count(void) { return g_launches.load(); }
 
 static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// ---- Scratch of the native objects ------------------------------------------------------------------------------------
+// One piece of an object's device scratch: the pointer it is carved into, its length in elements of that pointer's type
+// and, optionally, the host contents it starts with (otherwise zeros)
+struct Piece {
+  void** slot;
+  size_t bytes;
+  const void* init;
+  template <class T> Piece(T** p, long long count, const T* init = nullptr)
+      : slot(reinterpret_cast<void**>(p)), bytes((size_t)count * sizeof(T)), init(init) {}
+};
+// An object's scratch as one cudaMalloc into *buf, every piece 256-byte aligned and filled.  The fill runs on the legacy
+// stream, which a non-blocking stream is not ordered after, so the call returns only once it is complete.  On failure
+// nothing is left allocated.
+static int carve_scratch(const char* fn, void** buf, const std::vector<Piece>& pieces) {
+  size_t tot = 0;
+  for (const Piece& pc : pieces) tot += align_up(pc.bytes, 256);
+  cudaError_t e = cudaMalloc(buf, tot);
+  if (e != cudaSuccess) return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e));
+  e = cudaMemset(*buf, 0, tot);
+  char* p = (char*)*buf;
+  for (const Piece& pc : pieces) {
+    *pc.slot = p;
+    if (pc.init && e == cudaSuccess) e = cudaMemcpy(p, pc.init, pc.bytes, cudaMemcpyHostToDevice);
+    p += align_up(pc.bytes, 256);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
+  if (e != cudaSuccess) { cudaFree(*buf); return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
+  return XTB_OK;
+}
 
 // ---- data-parallel communicator ---------------------------------------------------------------
 static NcclApi g_nccl;
@@ -145,9 +176,8 @@ struct LayerPlan {
   long long w_off = 0, b_off = 0;
   int src_act = 0;       // activation of the producing layer of the source tensor
   int adv_act = 0;       // dueling: activation of the producing layer of the 1-wide stream (tensor d.k)
-  // device tables (conv, fp32 path)
-  int* koff = nullptr; int* kyx = nullptr;            // forward / wgrad, indexed by k=(ky,kx,ci)
-  int* dkyx = nullptr; int* dco = nullptr; int* wk = nullptr;  // dgrad, indexed by k=(ky,kx,co)
+  // conv: index tables of the fp32 kernels (see ConvTabs) and their workspace offset
+  std::vector<int> im2col; size_t im2col_off = 0;
   int Kd = 0;            // KH*KW*Cout
   int sshift = 0;
   bool pad = false;
@@ -237,6 +267,9 @@ static uint32_t build_conv_tables(LayerPlan& lp) {
 enum Form : uint8_t { kNone = 0, kF32 = 1, kPlanes = 2, kBoth = 3 };
 struct TensorForms { uint8_t val = kNone, grad = kNone; };
 
+// A table built on the host by xtb_net_create and the workspace byte offset it is uploaded to by every bind
+struct HostTable { size_t off; const void* data; size_t bytes; };
+
 struct xtb_net {
   xtb_net_desc desc;
   int max_batch = 0, pitch = 0;
@@ -253,6 +286,7 @@ struct xtb_net {
   size_t blob_off = 0; long long blob_elems = 0;       // weight blobs: hi plane, lo plane follows
   size_t splitk_off = 0, zeros_off = 0, segs_off = 0, heads_part_off = 0;
   std::vector<bp::BlobSeg> blob_segs;
+  std::vector<HostTable> tables;          // the segment table, the stage walks and the im2col tables, in the workspace
   bool any_tc = false;
   float* params = nullptr; float* grads = nullptr; char* ws = nullptr;
   std::vector<TensorForms> cur;           // per tensor: changed only by wrote() / invalidate() / ensure_f32 / ensure_bp
@@ -298,6 +332,13 @@ static void invalidate(xtb_net* n, bool values, bool grads) {
 }
 static inline const bp::bf16* blob_hi(const xtb_net* n, const LayerPlan& lp) { return (const bp::bf16*)(n->ws + n->blob_off) + lp.blob_off; }
 static inline bool use_tc(const LayerPlan& lp) { return g_tc_mode && lp.tc; }
+// The fp32 kernels' index tables of a conv layer, one workspace region [koff K][kyx K][dkyx Kd][dco Kd][wk Kd]: forward
+// and weight gradient indexed by k = (ky, kx, ci), data gradient by k = (ky, kx, co)
+struct ConvTabs { const int *koff, *kyx, *dkyx, *dco, *wk; };
+static inline ConvTabs conv_tabs(const xtb_net* n, const LayerPlan& lp) {
+  const int* t = (const int*)(n->ws + lp.im2col_off);
+  return ConvTabs{t, t + lp.K, t + 2 * lp.K, t + 2 * lp.K + lp.Kd, t + 2 * lp.K + 2 * lp.Kd};
+}
 
 static int pick_tile(int n) { return n % 64 == 0 ? 64 : (n % 32 == 0 ? 32 : (n % 16 == 0 ? 16 : 0)); }
 
@@ -377,7 +418,7 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   if (!desc || !out || max_batch <= 0) return fail(XTB_ERR_ARG, "xtb_net_create: null/invalid argument");
   if (desc->n_layers <= 0 || desc->n_layers > XTB_MAX_LAYERS) return fail(XTB_ERR_ARG, "n_layers out of range");
   if (desc->input_u8 < 0 || desc->input_u8 > 2) return fail(XTB_ERR_ARG, "input_u8 %d not in 0..2", desc->input_u8);
-  auto* net = new xtb_net();
+  std::unique_ptr<xtb_net> net(new xtb_net());
   net->desc = *desc;
   net->max_batch = max_batch;
   net->pitch = (max_batch + 15) / 16 * 16;
@@ -392,13 +433,13 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     LayerPlan lp;
     lp.d = desc->layers[i];
     const auto& d = lp.d;
-    if (d.src < 0 || d.src > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: bad src %d", i, d.src); }
-    if (d.act < XTB_ACT_NONE || d.act > XTB_ACT_GELU) { delete net; return fail(XTB_ERR_ARG, "layer %d: unknown activation %d", i, d.act); }
+    if (d.src < 0 || d.src > i) return fail(XTB_ERR_ARG, "layer %d: bad src %d", i, d.src);
+    if (d.act < XTB_ACT_NONE || d.act > XTB_ACT_GELU) return fail(XTB_ERR_ARG, "layer %d: unknown activation %d", i, d.act);
     if (d.kind == XTB_LOGSTD) {
       // parameter-only: A floats (pi_logstd), no input, no output tensor
-      if (d.src != 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a logstd layer reads no tensor (src must be 0)", i); }
-      if (d.cout < 1 || d.cout > MAX_ADIM) { delete net; return fail(XTB_ERR_ARG, "layer %d: logstd width %d not in [1, %d]", i, d.cout, MAX_ADIM); }
-      if (d.act != XTB_ACT_NONE) { delete net; return fail(XTB_ERR_ARG, "layer %d: a logstd layer has no activation", i); }
+      if (d.src != 0) return fail(XTB_ERR_ARG, "layer %d: a logstd layer reads no tensor (src must be 0)", i);
+      if (d.cout < 1 || d.cout > MAX_ADIM) return fail(XTB_ERR_ARG, "layer %d: logstd width %d not in [1, %d]", i, d.cout, MAX_ADIM);
+      if (d.act != XTB_ACT_NONE) return fail(XTB_ERR_ARG, "layer %d: a logstd layer has no activation", i);
       lp.K = 1; lp.N = d.cout;
       shp[i + 1] = {1, 1, 0};
       net->tsize[i + 1] = 0;
@@ -410,17 +451,17 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     {   // no layer reads the (0-wide) tensor of a logstd layer
       const bool bad_src = d.src > 0 && desc->layers[d.src - 1].kind == XTB_LOGSTD;
       const bool bad_k = d.kind == XTB_DUELING && d.k > 0 && d.k <= i && desc->layers[d.k - 1].kind == XTB_LOGSTD;
-      if (bad_src || bad_k) { delete net; return fail(XTB_ERR_ARG, "layer %d: reads the tensor of a logstd layer", i); }
+      if (bad_src || bad_k) return fail(XTB_ERR_ARG, "layer %d: reads the tensor of a logstd layer", i);
     }
     if (d.kind == XTB_DUELING) {
       // combine of two earlier layers: src = the A-wide stream, k = the 1-wide stream; no parameters
-      if (d.src == 0 || d.k == 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer cannot read the observation", i); }
-      if (d.k < 0 || d.k > i) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling 1-wide input %d is not an earlier layer", i, d.k); }
-      if (d.k == d.src) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling inputs must be two different tensors", i); }
-      if (net->tsize[d.k] != 1) { delete net; return fail(XTB_ERR_ARG, "layer %d: dueling input %d is %d wide, not 1", i, d.k, net->tsize[d.k]); }
-      if (d.act != XTB_ACT_NONE) { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer has no activation", i); }
+      if (d.src == 0 || d.k == 0) return fail(XTB_ERR_ARG, "layer %d: a dueling layer cannot read the observation", i);
+      if (d.k < 0 || d.k > i) return fail(XTB_ERR_ARG, "layer %d: dueling 1-wide input %d is not an earlier layer", i, d.k);
+      if (d.k == d.src) return fail(XTB_ERR_ARG, "layer %d: dueling inputs must be two different tensors", i);
+      if (net->tsize[d.k] != 1) return fail(XTB_ERR_ARG, "layer %d: dueling input %d is %d wide, not 1", i, d.k, net->tsize[d.k]);
+      if (d.act != XTB_ACT_NONE) return fail(XTB_ERR_ARG, "layer %d: a dueling layer has no activation", i);
       if (act_is_ext(tact[d.src]) || act_is_ext(tact[d.k]))
-        { delete net; return fail(XTB_ERR_ARG, "layer %d: a dueling layer reads relu / tanh / linear tensors only", i); }
+        return fail(XTB_ERR_ARG, "layer %d: a dueling layer reads relu / tanh / linear tensors only", i);
       lp.in_size = lp.out_size = net->tsize[d.src];
       lp.src_act = tact[d.src]; lp.adv_act = tact[d.k];
       shp[i + 1] = {1, 1, lp.out_size};
@@ -438,7 +479,7 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
       lp.d.kind = XTB_DENSE;
     }
     if (lp.d.kind == XTB_CONV) {
-      if (d.stride != 1 && d.stride != 2 && d.stride != 4) { delete net; return fail(XTB_ERR_ARG, "layer %d: stride must be 1,2,4", i); }
+      if (d.stride != 1 && d.stride != 2 && d.stride != 4) return fail(XTB_ERR_ARG, "layer %d: stride must be 1,2,4", i);
       ConvGeom& g = lp.g;
       g.H = is.h; g.W = is.w; g.C = is.c; g.KH = g.KW = d.k; g.S = d.stride; g.Cout = d.cout;
       if (d.pad_same) {
@@ -448,14 +489,15 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
       } else {
         g.OH = (g.H - d.k) / d.stride + 1; g.OW = (g.W - d.k) / d.stride + 1; g.padT = g.padL = 0;
       }
-      if (g.OH <= 0 || g.OW <= 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: empty conv output", i); }
+      if (g.OH <= 0 || g.OW <= 0) return fail(XTB_ERR_ARG, "layer %d: empty conv output", i);
       g.K = d.k * d.k * g.C; g.P = g.OH * g.OW;
       g.mP = fastdiv_magic(g.P); g.mOW = fastdiv_magic(g.OW); g.mHW = fastdiv_magic(g.H * g.W); g.mW = fastdiv_magic(g.W);
       lp.K = g.K; lp.N = d.cout; lp.Kd = d.k * d.k * d.cout;
       lp.sshift = d.stride == 1 ? 0 : (d.stride == 2 ? 1 : 2);
       shp[i + 1] = {g.OH, g.OW, d.cout};
-      // tables (fp32 path)
-      std::vector<int> koff(g.K), kyx(g.K), dkyx(lp.Kd), dco(lp.Kd), wk(lp.Kd);
+      // index tables of the fp32 kernels, in the order of ConvTabs
+      lp.im2col.resize(2 * g.K + 3 * lp.Kd);
+      int *koff = lp.im2col.data(), *kyx = koff + g.K, *dkyx = kyx + g.K, *dco = dkyx + lp.Kd, *wk = dco + lp.Kd;
       for (int ky = 0; ky < d.k; ky++)
         for (int kx = 0; kx < d.k; kx++) {
           for (int ci = 0; ci < g.C; ci++) {
@@ -470,18 +512,6 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
             wk[k] = (ky * d.k + kx) * g.C * d.cout + co;
           }
         }
-      auto up = [&](int** dst, const std::vector<int>& v) -> cudaError_t {
-        cudaError_t e = cudaMalloc(dst, v.size() * sizeof(int));
-        if (e != cudaSuccess) return e;
-        return cudaMemcpy(*dst, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice);
-      };
-      cudaError_t e;
-      if ((e = up(&lp.koff, koff)) != cudaSuccess || (e = up(&lp.kyx, kyx)) != cudaSuccess ||
-          (e = up(&lp.dkyx, dkyx)) != cudaSuccess || (e = up(&lp.dco, dco)) != cudaSuccess ||
-          (e = up(&lp.wk, wk)) != cudaSuccess) {
-        delete net;
-        return fail(XTB_ERR_CUDA, "table upload failed: %s", cudaGetErrorString(e));
-      }
       // ---- tensor-core plan
       lp.q = g;
       const bool cout_ok = d.cout % 16 == 0 && d.cout <= 64;
@@ -513,10 +543,9 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
         lp.n_fwd = pick_tile(lp.N); lp.n_dg = pick_tile(lp.K);
       }
     } else {
-      delete net;
       return fail(XTB_ERR_ARG, "layer %d: unknown kind %d", i, d.kind);
     }
-    if (lp.N <= 0) { delete net; return fail(XTB_ERR_ARG, "layer %d: zero outputs", i); }
+    if (lp.N <= 0) return fail(XTB_ERR_ARG, "layer %d: zero outputs", i);
     tact[i + 1] = d.act;
     lp.out_size = shp[i + 1].h * shp[i + 1].w * shp[i + 1].c;
     net->tsize[i + 1] = lp.out_size;
@@ -581,11 +610,17 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
     }
     lp.dbpart_off = w; w += align_up((size_t)kSMs * 64 * sizeof(float), 256);
   }
+  // a host-built table: its region, and its entry in the list every bind uploads
+  auto table = [&](const auto& v) {
+    const size_t o = w, bytes = v.size() * sizeof(v[0]);
+    w += align_up(bytes, 256);
+    if (bytes) net->tables.push_back(HostTable{o, v.data(), bytes});
+    return o;
+  };
   for (auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_CONV) {
-    auto place = [&](size_t bytes) { size_t o = w; w += align_up(bytes, 256); return o; };
-    lp.fwd_st_off = place(lp.fwd_st.size() * sizeof(bp::StageEnt)); lp.fwd_un_off = place(lp.fwd_un.size() * sizeof(bp::UnitEnt));
-    lp.dg_st_off = place(lp.dg_st.size() * sizeof(bp::StageEnt)); lp.dg_un_off = place(lp.dg_un.size() * sizeof(bp::UnitEnt));
-    lp.wg_off = place(lp.wg_tab.size() * sizeof(bp::WgEnt));
+    lp.fwd_st_off = table(lp.fwd_st); lp.fwd_un_off = table(lp.fwd_un);
+    lp.dg_st_off = table(lp.dg_st); lp.dg_un_off = table(lp.dg_un);
+    lp.wg_off = table(lp.wg_tab);
   }
   // split-K partial sums of a dense forward: the largest over the forwards the net runs, B rows split for E rows with
   // E <= B <= max_batch; a rollout-inference chunk of E environments (the most rows at a given E) covers every B = E
@@ -605,18 +640,19 @@ extern "C" int xtb_net_create(const xtb_net_desc* desc, int max_batch, xtb_net**
   // per-block parameter-gradient slabs of the fused PPO heads kernel (K <= 512 hidden units, A <= 8 actions)
   net->heads_part_off = w; w += align_up((size_t)kSMs * (512 * 8 + 3 * 512 + 16) * sizeof(float), 256);
   net->segs_off = w; w += align_up(sizeof(bp::BlobSeg) * XTB_MAX_LAYERS, 256);
+  if (!net->blob_segs.empty())
+    net->tables.push_back(HostTable{net->segs_off, net->blob_segs.data(), net->blob_segs.size() * sizeof(bp::BlobSeg)});
+  // every conv layer: the fp32 kernels also run tensor-core layers (xtb_set_tc_mode(0), forwards with other parameters)
+  for (auto& lp : net->L) if (lp.d.kind == XTB_CONV) lp.im2col_off = table(lp.im2col);
   net->ws_bytes = w;
   net->cur.assign(nt, TensorForms{});
-  *out = net;
+  *out = net.release();
   return XTB_OK;
 }
 
 extern "C" void xtb_net_destroy(xtb_net* net) {
   if (!net) return;
   drop_graphs_of(net);
-  for (auto& lp : net->L) {
-    cudaFree(lp.koff); cudaFree(lp.kyx); cudaFree(lp.dkyx); cudaFree(lp.dco); cudaFree(lp.wk);
-  }
   delete net;
 }
 
@@ -677,21 +713,12 @@ extern "C" int xtb_net_bind_stream(xtb_net* net, float* params, float* grads, vo
   // Planes start as zeros: rows beyond the current batch are read (never used) by full-tile operand copies and
   // must be finite; the zero buffer feeds out-of-image chunks of padded weight-gradient operands.
   CUDA_TRY(cudaMemsetAsync(net->ws, 0, net->ws_bytes, st));
-  if (!net->blob_segs.empty())
-    CUDA_TRY(cudaMemcpyAsync(net->ws + net->segs_off, net->blob_segs.data(), net->blob_segs.size() * sizeof(bp::BlobSeg),
-                             cudaMemcpyHostToDevice, st));
-  for (const auto& lp : net->L) if (lp.tc && lp.d.kind == XTB_CONV) {
-    auto up = [&](size_t off, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(net->ws + off, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess; };
-    CUDA_TRY(up(lp.fwd_st_off, lp.fwd_st.data(), lp.fwd_st.size() * sizeof(bp::StageEnt)));
-    CUDA_TRY(up(lp.fwd_un_off, lp.fwd_un.data(), lp.fwd_un.size() * sizeof(bp::UnitEnt)));
-    CUDA_TRY(up(lp.dg_st_off, lp.dg_st.data(), lp.dg_st.size() * sizeof(bp::StageEnt)));
-    CUDA_TRY(up(lp.dg_un_off, lp.dg_un.data(), lp.dg_un.size() * sizeof(bp::UnitEnt)));
-    CUDA_TRY(up(lp.wg_off, lp.wg_tab.data(), lp.wg_tab.size() * sizeof(bp::WgEnt)));
-  }
+  for (const HostTable& t : net->tables)
+    CUDA_TRY(cudaMemcpyAsync(net->ws + t.off, t.data, t.bytes, cudaMemcpyHostToDevice, st));
   invalidate(net, true, true);
   int rc = xtb_net_sync_weights(net, stream);
   if (rc) return rc;
-  // the segment table came from pageable host memory of this call: do not return before it is on the device
+  // the tables are copied from pageable host memory: do not return before they are on the device
   CUDA_TRY(cudaStreamSynchronize(st));
   return XTB_OK;
 }
@@ -998,18 +1025,17 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
   const int fb = N;                                  // mode 2: features of B
   const int nt = pick_tile(N);
   if (!nt) return fail(XTB_ERR_ARG, "N must be a multiple of 16");
-  bp::bf16 *pa = nullptr, *pw = nullptr, *pc = nullptr; float* part = nullptr; float* bias = nullptr;
   const long long ea = (long long)fa * pitch;
   const long long ew = mode == 2 ? (long long)fb * pitch : (mode == 1 ? (long long)K * ((N + 15) / 16 * 16) : (long long)N * K);   // weight blob / second activation
   const long long ec = (long long)N * pitch;
-  CUDA_TRY(cudaMalloc(&pa, 2 * ea * sizeof(bp::bf16)));
-  CUDA_TRY(cudaMalloc(&pw, 2 * ew * sizeof(bp::bf16) + 256));
-  CUDA_TRY(cudaMalloc(&pc, 2 * ec * sizeof(bp::bf16) + 4096));
-  CUDA_TRY(cudaMalloc(&bias, (size_t)std::max(N, 64) * sizeof(float)));
-  CUDA_TRY(cudaMemsetAsync(pa, 0, 2 * ea * sizeof(bp::bf16), st));
-  CUDA_TRY(cudaMemsetAsync(pw, 0, 2 * ew * sizeof(bp::bf16) + 256, st));
-  CUDA_TRY(cudaMemsetAsync(pc, 0, 2 * ec * sizeof(bp::bf16) + 4096, st));
-  CUDA_TRY(cudaMemsetAsync(bias, 0, (size_t)std::max(N, 64) * sizeof(float), st));
+  // mode 0 split-K: nz slices of kc_split K chunks
+  const int kchunks = K / 8, kc_split = mode == 0 && ksplit > 1 ? ((kchunks + ksplit - 1) / ksplit + 7) / 8 * 8 : kchunks;
+  const int nz = (kchunks + kc_split - 1) / kc_split;
+  bp::bf16 *pa, *pw, *pc; float *bias, *part;
+  void* buf;
+  if (int rc = carve_scratch("xtb_tc_gemm_test", &buf, {{&pa, 2 * ea}, {&pw, 2 * ew + 128}, {&pc, 2 * ec + 2048},
+                                                        {&bias, std::max(N, 64)}, {&part, nz > 1 ? (long long)nz * M * N : 0}}))
+    return rc;
   bp::BpT ta{pa, ea, pitch}, tw{pw, ew, mode == 2 ? pitch : K}, tcp{pc, ec, pitch};
   auto split = [&](const float* src, int B_, int F_, bp::BpT dst) {
     long long pieces = (long long)(F_ / 8) * ((B_ + 15) & ~15);
@@ -1026,14 +1052,11 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
     memset(&r, 0, sizeof r);
     r.a = ta; r.a_split = 1; r.w_hi = pw; r.w_lo = pw + ew; r.w_pitch = tw.pitch;
     r.mode = 2; r.B = M; r.n_btiles = (M + 127) / 128; r.N = nt; r.n_ntiles = N / nt;
-    r.kchunks = K / 8; r.kc_split = r.kchunks;
+    r.kchunks = kchunks; r.kc_split = kc_split;
     r.bias = bias; r.alpha = 1.f; r.act = 0;
     if (mode == 0) {
-      int nz = 1;
-      if (ksplit > 1) { r.kc_split = ((r.kchunks + ksplit - 1) / ksplit + 7) / 8 * 8; nz = (r.kchunks + r.kc_split - 1) / r.kc_split; }
       r.n_units = r.n_ntiles * nz;
       if (nz > 1) {
-        CUDA_TRY(cudaMalloc(&part, (size_t)nz * M * N * sizeof(float)));
         r.part = part; r.part_z = (long long)M * N; r.ld_part = N;
         e = launch_rows<1>(r, st);
         long long pieces = (long long)(N / 8) * ((M + 15) & ~15) * bp::FIN_ZL;
@@ -1063,7 +1086,7 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
   }
   g_launches.fetch_add(4, std::memory_order_relaxed);
   cudaError_t e2 = cudaStreamSynchronize(st);
-  cudaFree(pa); cudaFree(pw); cudaFree(pc); cudaFree(bias); cudaFree(part);
+  cudaFree(buf);
   if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "tc gemm launch: %s", cudaGetErrorString(e));
   if (e2 != cudaSuccess) return fail(XTB_ERR_CUDA, "tc gemm run: %s", cudaGetErrorString(e2));
   return XTB_OK;
@@ -1073,13 +1096,14 @@ extern "C" int xtb_tc_gemm_test(int mode, const float* a, const float* b, float*
 // fp32 CUDA-core layer ops
 // ------------------------------------------------------------------------------------------
 template <typename T>
-static void conv_fwd(const LayerPlan& lp, const T* x, const int32_t* idx, const float* w, const float* b,
+static void conv_fwd(const xtb_net* net, const LayerPlan& lp, const T* x, const int32_t* idx, const float* w, const float* b,
                      float alpha, float* out, int B, cudaStream_t st) {
   int M = B * lp.g.P;
   BRowMajor bl{w, lp.N};
   EpiBiasAct ep{out, b, alpha, act_is_ext(lp.d.act) ? 0 : lp.d.act, lp.N, nullptr, 0};
-  if (lp.pad) { AIm2col<T, true> al{x, idx, lp.g, lp.koff, lp.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
-  else { AIm2col<T, false> al{x, idx, lp.g, lp.koff, lp.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
+  const ConvTabs tab = conv_tabs(net, lp);
+  if (lp.pad) { AIm2col<T, true> al{x, idx, lp.g, tab.koff, tab.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
+  else { AIm2col<T, false> al{x, idx, lp.g, tab.koff, tab.kyx}; launch_gemm(al, bl, ep, M, lp.N, lp.K, false, st); }
 }
 template <typename T>
 static void dense_fwd(const LayerPlan& lp, const T* x, const int32_t* idx, const float* w, const float* b,
@@ -1090,7 +1114,7 @@ static void dense_fwd(const LayerPlan& lp, const T* x, const int32_t* idx, const
   launch_gemm(al, bl, ep, B, lp.N, lp.K, false, st);
 }
 template <typename T>
-static void conv_wgrad(const LayerPlan& lp, const T* x, const int32_t* idx, const float* dy, float alpha,
+static void conv_wgrad(const xtb_net* net, const LayerPlan& lp, const T* x, const int32_t* idx, const float* dy, float alpha,
                        float* dw, int B, cudaStream_t st, bool bias_row = true) {
   int Mr = B * lp.g.P;
   BRowMajor bl{dy, lp.N};
@@ -1098,8 +1122,9 @@ static void conv_wgrad(const LayerPlan& lp, const T* x, const int32_t* idx, cons
   // rows 0..K-1 scaled by alpha (input decode scale); the bias row (K) must not be scaled:
   // it rides in the same GEMM only when alpha == 1, else colsum_kernel computes it.
   int rows = lp.K + ((alpha == 1.f && bias_row) ? 1 : 0);
-  if (lp.pad) { AIm2colT<T, true> al{x, idx, lp.g, lp.koff, lp.kyx, Mr}; launch_gemm(al, bl, ep, rows, lp.N, Mr, true, st); }
-  else { AIm2colT<T, false> al{x, idx, lp.g, lp.koff, lp.kyx, Mr}; launch_gemm(al, bl, ep, rows, lp.N, Mr, true, st); }
+  const ConvTabs tab = conv_tabs(net, lp);
+  if (lp.pad) { AIm2colT<T, true> al{x, idx, lp.g, tab.koff, tab.kyx, Mr}; launch_gemm(al, bl, ep, rows, lp.N, Mr, true, st); }
+  else { AIm2colT<T, false> al{x, idx, lp.g, tab.koff, tab.kyx, Mr}; launch_gemm(al, bl, ep, rows, lp.N, Mr, true, st); }
 }
 template <typename T>
 static void dense_wgrad(const LayerPlan& lp, const T* x, const int32_t* idx, const float* dy, float alpha,
@@ -1213,7 +1238,7 @@ static int op_forward(xtb_net* net, int i, const float* P, bool tc_allowed, cons
     return XTB_OK;
   }
   auto gemm = [&](auto x, const int32_t* ix, float alpha) {
-    if (lp.d.kind == XTB_CONV) conv_fwd(lp, x, ix, w, b, alpha, pre, B, st);
+    if (lp.d.kind == XTB_CONV) conv_fwd(net, lp, x, ix, w, b, alpha, pre, B, st);
     else dense_fwd(lp, x, ix, w, b, alpha, pre, B, st);
   };
   if (lp.d.src == 0) {
@@ -1248,7 +1273,7 @@ static int op_wgrad(xtb_net* net, int i, const void* obs, const int32_t* idx, in
     if (rc) return rc;
     const float* dy = gout_f32(net, t);
     auto gemm = [&](auto x, const int32_t* ix, float alpha) {
-      if (lp.d.kind == XTB_CONV) conv_wgrad(lp, x, ix, dy, alpha, dw, B, st, !bias_done);
+      if (lp.d.kind == XTB_CONV) conv_wgrad(net, lp, x, ix, dy, alpha, dw, B, st, !bias_done);
       else dense_wgrad(lp, x, ix, dy, alpha, dw, B, st, !bias_done);
     };
     if (lp.d.src == 0) {
@@ -1319,8 +1344,9 @@ static int op_dgrad(xtb_net* net, int i, int acc, int B, cudaStream_t st, bool f
   float* gsrc = gout_f32(net, s);
   const float* w = net->params + lp.w_off;
   if (lp.d.kind == XTB_CONV) {
-    ADgrad al{dy, lp.g, lp.dkyx, lp.dco, lp.sshift};
-    BConvDgrad bl{w, lp.wk, lp.N};
+    const ConvTabs tab = conv_tabs(net, lp);
+    ADgrad al{dy, lp.g, tab.dkyx, tab.dco, lp.sshift};
+    BConvDgrad bl{w, tab.wk, lp.N};
     EpiDgrad ep{gsrc, x, dgrad_act(lp), lp.g.C, acc, nullptr, 0};
     launch_gemm(al, bl, ep, B * lp.g.H * lp.g.W, lp.g.C, lp.Kd, false, st);
   } else {
@@ -1703,6 +1729,7 @@ struct xtb_adam {
   bool rms_plain = false;                                    // uncentred RMSProp instead of Adam (m = ms, mg unused)
   int* blk_seg = nullptr; long long* blk_beg = nullptr; int* blk_len = nullptr;
   double* norm_sq = nullptr; float* seg_scale = nullptr; AdamState* st = nullptr; AdamHyper* hyp = nullptr; unsigned int* ticket = nullptr;
+  void* buf = nullptr;                                       // the one allocation the pointers above are carved from
 };
 
 // The optimiser kernels read and write every buffer as float4 wherever a chunk starts at a multiple of 4 elements.
@@ -1739,29 +1766,18 @@ extern "C" int xtb_adam_create(long long count, float lr, float beta1, float bet
     }
   o->n_blk = (int)bseg.size();
   AdamState init{1.f, 1.f, 0.f, 0.f, 0u};
-  cudaError_t e = cudaSuccess;
-  auto chk = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
-  chk(cudaMalloc(&o->blk_seg, o->n_blk * sizeof(int)));
-  chk(cudaMalloc(&o->blk_beg, o->n_blk * sizeof(long long)));
-  chk(cudaMalloc(&o->blk_len, o->n_blk * sizeof(int)));
-  chk(cudaMalloc(&o->norm_sq, o->n_seg * sizeof(double)));
-  chk(cudaMalloc(&o->seg_scale, o->n_seg * sizeof(float)));
-  chk(cudaMalloc(&o->st, sizeof(AdamState)));
-  chk(cudaMalloc(&o->hyp, sizeof(AdamHyper)));
-  chk(cudaMalloc(&o->ticket, sizeof(unsigned int)));
-  if (e == cudaSuccess) {
-    chk(cudaMemcpy(o->blk_seg, bseg.data(), o->n_blk * sizeof(int), cudaMemcpyHostToDevice));
-    chk(cudaMemcpy(o->blk_beg, bbeg.data(), o->n_blk * sizeof(long long), cudaMemcpyHostToDevice));
-    chk(cudaMemcpy(o->blk_len, blen.data(), o->n_blk * sizeof(int), cudaMemcpyHostToDevice));
-    chk(cudaMemset(o->norm_sq, 0, o->n_seg * sizeof(double)));
-    chk(cudaMemcpy(o->st, &init, sizeof init, cudaMemcpyHostToDevice));
-    chk(cudaMemset(o->ticket, 0, sizeof(unsigned int)));
-    AdamHyper hy{lr, beta1, beta2, eps, clip, 0.f};
-    chk(cudaMemcpy(o->hyp, &hy, sizeof hy, cudaMemcpyHostToDevice));
-    chk(cudaMemset(m, 0, count * sizeof(float)));
-    chk(cudaMemset(v, 0, count * sizeof(float)));
+  AdamHyper hy{lr, beta1, beta2, eps, clip, 0.f};
+  // carve_scratch's synchronize also completes these fills before the call returns
+  cudaError_t e = cudaMemset(m, 0, count * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(v, 0, count * sizeof(float));
+  if (e != cudaSuccess) { delete o; return fail(XTB_ERR_CUDA, "xtb_adam_create: %s", cudaGetErrorString(e)); }
+  if (int rc = carve_scratch("xtb_adam_create", &o->buf, {{&o->blk_seg, o->n_blk, bseg.data()}, {&o->blk_beg, o->n_blk, bbeg.data()},
+                                                          {&o->blk_len, o->n_blk, blen.data()}, {&o->norm_sq, o->n_seg},
+                                                          {&o->seg_scale, o->n_seg}, {&o->st, 1, &init}, {&o->hyp, 1, &hy},
+                                                          {&o->ticket, 1}})) {
+    delete o;
+    return rc;
   }
-  if (e != cudaSuccess) { xtb_adam_destroy(o); return fail(XTB_ERR_CUDA, "xtb_adam_create: %s", cudaGetErrorString(e)); }
   *out = o;
   return XTB_OK;
 }
@@ -1769,8 +1785,8 @@ extern "C" int xtb_adam_create(long long count, float lr, float beta1, float bet
 extern "C" void xtb_adam_destroy(xtb_adam* o) {
   if (!o) return;
   drop_graphs_of(o);
-  cudaFree(o->blk_seg); cudaFree(o->blk_beg); cudaFree(o->blk_len);
-  cudaFree(o->norm_sq); cudaFree(o->seg_scale); cudaFree(o->st); cudaFree(o->hyp); cudaFree(o->ticket);
+  cudaDeviceSynchronize();
+  cudaFree(o->buf);
   delete o;
 }
 
@@ -2307,27 +2323,6 @@ extern "C" int xtb_impala_keras_train(xtb_net* net, xtb_adam* opt, const xtb_imp
   });
 }
 
-// ---- Scratch of the native objects ------------------------------------------------------------------------------------
-// One piece of an object's device scratch: the pointer it is carved into and its length in elements of that pointer's type
-struct Piece {
-  void** slot;
-  size_t bytes;
-  template <class T> Piece(T** p, long long count) : slot(reinterpret_cast<void**>(p)), bytes((size_t)count * sizeof(T)) {}
-};
-// An object's scratch as one zero-filled cudaMalloc into *buf, every piece 256-byte aligned; on failure nothing is left
-// allocated
-static int carve_scratch(const char* fn, void** buf, const std::vector<Piece>& pieces) {
-  size_t tot = 0;
-  for (const Piece& pc : pieces) tot += align_up(pc.bytes, 256);
-  cudaError_t e = cudaMalloc(buf, tot);
-  if (e != cudaSuccess) return fail(XTB_ERR_NOMEM, "%s: %s", fn, cudaGetErrorString(e));
-  e = cudaMemset(*buf, 0, tot);
-  if (e != cudaSuccess) { cudaFree(*buf); return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e)); }
-  char* p = (char*)*buf;
-  for (const Piece& pc : pieces) { *pc.slot = p; p += align_up(pc.bytes, 256); }
-  return XTB_OK;
-}
-
 // ---- MuZero (xt/model/muzero/muzero_model.py:103-140, 154-239) -------------------------------------------------------
 // The three networks (representation, dynamics, prediction) are separate xtb_nets bound to consecutive slices of one
 // parameter buffer and one gradient buffer (the Keras list order of MuzeroBase); the dynamics net's own gradient buffer
@@ -2705,22 +2700,19 @@ static int agent_capacity(const char* fn, const QmixAgent& a) {
   return XTB_OK;
 }
 
-// The object's scratch in one carve_scratch into *buf, the agent's pieces before the object's own `pieces`; then the
-// one-step inference's sequence lengths and the GRU kernels' shared-memory opt-in.  On failure nothing stays allocated.
+// The GRU kernels' shared-memory opt-in, then the object's scratch in one carve_scratch into *buf: the agent's pieces,
+// with the one-step inference's sequence lengths, before the object's own `pieces`.  On failure nothing stays allocated.
 static int agent_alloc(const char* fn, QmixAgent& a, void** buf, std::vector<Piece> pieces) {
-  const long long R = a.R, H = a.H;
-  pieces.insert(pieces.begin(), {{&a.xg, R * 2 * H}, {&a.xc, R * H}, {&a.hout, R * H}, {&a.rh, R * H}, {&a.dy, R * H},
-                                 {&a.dag, R * 2 * H}, {&a.dac, R * H}, {&a.ones, a.n}});
-  if (int rc = carve_scratch(fn, buf, pieces)) return rc;
-  std::vector<int32_t> ones(a.n, 1);
-  cudaError_t e = cudaMemcpy(a.ones, ones.data(), a.n * sizeof(int32_t), cudaMemcpyHostToDevice);
   // The opt-in is a property of the kernel, shared by every live object: it is set to the most any object may use
   // (this object's smem would shrink it under an earlier object with a wider GRU or more sequences per CTA).
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  cudaError_t e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
-  if (e == cudaSuccess) return XTB_OK;
-  cudaFree(*buf);
-  return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  const long long R = a.R, H = a.H;
+  const std::vector<int32_t> ones(a.n, 1);
+  pieces.insert(pieces.begin(), {{&a.xg, R * 2 * H}, {&a.xc, R * H}, {&a.hout, R * H}, {&a.rh, R * H}, {&a.dy, R * H},
+                                 {&a.dag, R * 2 * H}, {&a.dac, R * H}, {&a.ones, a.n, ones.data()}});
+  return carve_scratch(fn, buf, pieces);
 }
 
 // fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding

@@ -61,6 +61,37 @@ def require_cuda():
         raise RuntimeError("xingtian_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
 
 
+def net_desc(arch):
+    """The xtb_net_desc of `arch` (layers = list of (name, kind, src_name, spec), see Net); xtb_net_create plans it on
+    the host."""
+    tid = {n: i for i, n in enumerate(["obs"] + [l[0] for l in arch["layers"]])}
+    desc = capi.NetDesc()
+    desc.input_u8 = {"uint8": 1, "int8": 2}.get(arch["input_dtype"], 0)
+    desc.scale = float(arch["scale"])
+    sd = tuple(arch["state_dim"])
+    desc.in_h, desc.in_w, desc.in_c = (sd if len(sd) == 3 else (1, 1, int(np.prod(sd))))
+    desc.n_layers = len(arch["layers"])
+    if desc.n_layers > capi.XTB_MAX_LAYERS:
+        raise ValueError("too many layers")
+    for i, (name, kind, src, sp) in enumerate(arch["layers"]):
+        ld = desc.layers[i]
+        if kind == "dueling":
+            ld.kind, ld.src, ld.k, ld.act = capi.DUELING, tid[src[0]], tid[src[1]], capi.ACT[None]
+            continue
+        if kind == "logstd":
+            ld.kind, ld.src, ld.cout, ld.act = capi.LOGSTD, 0, sp["n"], capi.ACT[None]
+            continue
+        ld.kind = capi.CONV if kind == "conv" else capi.DENSE
+        ld.src = tid[src]
+        ld.act = capi.ACT[sp.get("act")]
+        if kind == "conv":
+            ld.k, ld.stride, ld.cout = sp["k"], sp["s"], sp["cout"]
+            ld.pad_same = 1 if sp["pad"] == "same" else 0
+        else:
+            ld.cout = sp["n"]
+    return desc
+
+
 class Net(object):
     """One network (layers = list of (name, kind, src_name, spec)) living in device memory.
 
@@ -77,31 +108,7 @@ class Net(object):
         self.max_batch = int(max_batch)
         self.names = ["obs"] + [l[0] for l in arch["layers"]]
         self.tid = {n: i for i, n in enumerate(self.names)}
-        desc = capi.NetDesc()
-        desc.input_u8 = {"uint8": 1, "int8": 2}.get(arch["input_dtype"], 0)
-        desc.scale = float(arch["scale"])
-        sd = tuple(arch["state_dim"])
-        desc.in_h, desc.in_w, desc.in_c = (sd if len(sd) == 3 else (1, 1, int(np.prod(sd))))
-        desc.n_layers = len(arch["layers"])
-        if desc.n_layers > capi.XTB_MAX_LAYERS:
-            raise ValueError("too many layers")
-        for i, (name, kind, src, sp) in enumerate(arch["layers"]):
-            ld = desc.layers[i]
-            if kind == "dueling":
-                ld.kind, ld.src, ld.k, ld.act = capi.DUELING, self.tid[src[0]], self.tid[src[1]], capi.ACT[None]
-                continue
-            if kind == "logstd":
-                ld.kind, ld.src, ld.cout, ld.act = capi.LOGSTD, 0, sp["n"], capi.ACT[None]
-                continue
-            ld.kind = capi.CONV if kind == "conv" else capi.DENSE
-            ld.src = self.tid[src]
-            ld.act = capi.ACT[sp.get("act")]
-            if kind == "conv":
-                ld.k, ld.stride, ld.cout = sp["k"], sp["s"], sp["cout"]
-                ld.pad_same = 1 if sp["pad"] == "same" else 0
-            else:
-                ld.cout = sp["n"]
-        self._desc = desc
+        self._desc = net_desc(arch)
         self.handle = C.c_void_p()
         self.params = self.grads = None
         self._create(self.max_batch)
