@@ -106,6 +106,8 @@ const char* xtb_last_error(void);
 long long xtb_launch_count(void);
 /* Number of CUDA-graph replays (fused training loop / rollout inference) the library has issued. */
 long long xtb_graph_replay_count(void);
+/* Number of CUDA graphs the library has captured (a replay of a cached graph does not count). */
+long long xtb_graph_capture_count(void);
 
 /* ---- network: replaces XTModel's TF graph (xt/model/model.py:30-127) ---------- */
 /* Flat fp32 parameter layout: per layer, kernel [K,N] (HWIO flattened) then bias [N];
@@ -339,6 +341,58 @@ int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs,
                   const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                   const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
                   float* qn_o, float* loss_out, int use_graph, void* stream);
+/* xtb_dqn_train with importance weights: sample b's loss and gradient are scaled by weights[b] (Keras train_on_batch with
+ * sample_weight: loss = 1/(B A) sum_b weights[b] sum_a e_ba), and td_abs[b] = |y_b - Q(s_b, a_b)| from the online forward
+ * before the update.  Either may be NULL; with both NULL the step is xtb_dqn_train's. */
+int xtb_dqn_train_weighted(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
+                           const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
+                           const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
+                           float* qn_o, const float* weights, float* td_abs, float* loss_out, int use_graph, void* stream);
+
+/* ---- prioritized experience replay (Schaul et al., proportional variant) over the slots of a device replay ring: the
+ *      rules of PrioritizedReplayBuffer (xt/algorithm/prioritized_replay_buffer_muzero.py:77-200), leaf i = ring slot i ----
+ * Insert: every slot written (wrapped slots included) gets max_priority ** alpha; max_priority starts at 1, is the
+ *   largest raw priority an update wrote and is never lowered.
+ * Sample B indices with replacement, stratified: mass_k = (u_k + k) total / B, u_k uniform in [0, 1); the draw descends
+ *   to the first leaf whose running sum exceeds mass_k, and one past the stored slots is clamped to count - 1.  total
+ *   is the sum over ALL stored leaves (the reference's sum(0, len - 1) has an exclusive end and never draws slot len - 1;
+ *   the reference DQN has no prioritized replay, so nothing binds to that).
+ * Importance weights, in float64, stored as float32: p_min = max(min_leaf / total, 1e-5),
+ *   w_k = ((leaf[idx_k] / total) count) ** -beta / (p_min count) ** -beta.
+ * Update: the reference's sequential loop over k: leaf[idx_k] = (|delta_k| + eps) ** alpha (an index named twice takes
+ *   the later k) and max_priority = max(max_priority, |delta_k| + eps).  An entry whose priority is not finite is skipped
+ *   and sets XTB_PER_NONFINITE.
+ * The sum and min trees are float64 over capacity rounded up to a power of two (empty leaves: 0 and +inf); every
+ * internal node is op(left, right) of its final children, so the trees are bitwise a function of their leaves.  The
+ * trees, count, max_priority, the status bits and the Philox offset live in one device allocation of the object and
+ * are read by the kernels, so one captured xtb_dqn_per_train graph serves every step while the ring fills.
+ * xtb_per_add / _sample / _update / xtb_dqn_per_train return XTB_ERR_STATE while a communicator is installed. */
+typedef struct xtb_per xtb_per;
+#define XTB_PER_NONFINITE 1   /* status: an update met a priority that is not finite (and did not write it) */
+#define XTB_PER_BAD_INDEX 2   /* status: an update named a slot outside [0, count) */
+#define XTB_PER_EMPTY 4       /* status: a draw from a tree with no stored slot (it wrote idx 0, w 0) */
+/* capacity >= 1 (the ring's), alpha >= 0, eps > 0 (finite), seed: the Philox key of the device draws. */
+int xtb_per_create(int capacity, double alpha, double eps, uint64_t seed, xtb_per** out);
+void xtb_per_destroy(xtb_per* per);
+/* Insert: ring slots [first_slot, first_slot + n) were written (a wrapped write is two calls); count covers them. */
+int xtb_per_add(xtb_per* per, int first_slot, int n, void* stream);
+/* B = batch draws into idx [B] int32 and w [B] float32, beta > 0.  uniforms [B] float64 in [0, 1) when non-NULL;
+ * otherwise u_k = 53 bits of Philox4x32-10 on counter (k, 0, offset) and the object's seed, ((x0 >> 5) 2^26 + (x1 >> 6))
+ * 2^-53, and the device offset advances by one. */
+int xtb_per_sample(xtb_per* per, int batch, double beta, const double* uniforms, int32_t* idx, float* w, void* stream);
+/* Update leaves idx[0..n) from td_abs[0..n) (|TD error|, float32). */
+int xtb_per_update(xtb_per* per, const int32_t* idx, const float* td_abs, int n, void* stream);
+/* Read-only snapshot after a device synchronise; any output may be NULL.  sum_host / min_host: [2 leaves] float64 in
+ * heap order (node 1 the root, node i's children 2i and 2i + 1, leaf j at node leaves + j). */
+int xtb_per_state(const xtb_per* per, int* leaves, int* count, double* max_priority, int* status, unsigned long long* offset,
+                  double* sum_host, double* min_host);
+/* One prioritized DQN step as one captured graph: xtb_per_sample of n_sample rows (Philox) into idx / w,
+ * xtb_dqn_train_weighted on them (weights w, |TD error| into td_abs), xtb_per_update(idx, td_abs), and a copy of the
+ * status bits into *status_out (device int32).  beta > 0. */
+int xtb_dqn_per_train(xtb_per* per, xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
+                      const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int n_sample,
+                      float gamma, float huber_delta, double beta, int q_tensor, float* qn_t, float* qn_o, int32_t* idx,
+                      float* w, float* td_abs, float* loss_out, int32_t* status_out, int use_graph, void* stream);
 
 /* IMPALA with the Keras learner (xt/algorithm/impala/impala.py, xt/model/impala/impala_mlp.py, impala_cnn.py).  The
  * policy head `logit_tensor` is the linear `output_actions` layer; its softmax is evaluated in the kernels.

@@ -1,10 +1,14 @@
 """Replay buffers: the reference's host deque (xt/algorithm/replay_buffer.py:24-42) and a
 device-resident ring used by the fused DQN step."""
+import ctypes as C
 import random
 from collections import deque
 
 import numpy as np
 import torch
+
+from ..capi import check, lib
+from ..engine import stream_ptr
 
 
 class ReplayBuffer(object):
@@ -27,10 +31,20 @@ class ReplayBuffer(object):
 class DeviceReplayBuffer(object):
     """Ring of transitions in HBM: frames are stored once per transition slot as (s, s') uint8
     pairs like the reference deque (56 KB / transition at 84x84x4); sampling draws the same
-    `random.sample(range(size), k)` indices on the host and gathers on the device."""
+    `random.sample(range(size), k)` indices on the host and gathers on the device.
 
-    def __init__(self, buffer_size, state_dim, obs_dtype, device):
+    `prioritized` = (alpha, eps, seed): the ring also owns a native sum / min tree over its slots (xtb_per, leaf i = slot
+    i) that every written slot enters at the largest priority so far; the prioritized DQN step samples and updates it
+    on the device."""
+
+    def __init__(self, buffer_size, state_dim, obs_dtype, device, prioritized=None):
         self.capacity = int(buffer_size)
+        self.per = None
+        if prioritized is not None:
+            alpha, eps, seed = prioritized
+            h = C.c_void_p()
+            check(lib().xtb_per_create(self.capacity, float(alpha), float(eps), int(seed), C.byref(h)))
+            self.per = h
         self.device = device
         self.state_dim = tuple(state_dim)
         self.obs_dtype = obs_dtype
@@ -57,6 +71,14 @@ class DeviceReplayBuffer(object):
         if self.keep_disc:
             self.disc = mk((new,), torch.float32, self.disc)
         self._alloc = new
+
+    def __del__(self):
+        try:
+            if getattr(self, "per", None) is not None:
+                lib().xtb_per_destroy(self.per)
+                self.per = None
+        except Exception:  # interpreter shutdown
+            pass
 
     def size(self):
         return self.count
@@ -86,6 +108,8 @@ class DeviceReplayBuffer(object):
             self.action[sl].copy_(act[src]); self.reward[sl].copy_(rew[src]); self.done[sl].copy_(don[src])
             if self.keep_disc and dsc is not None:
                 self.disc[sl].copy_(dsc[src])
+            if self.per is not None:
+                check(lib().xtb_per_add(self.per, self.head, k, stream_ptr()))
             self.head = (self.head + k) % self.capacity
             self.count = min(self.capacity, self.count + k)
             done_n += k

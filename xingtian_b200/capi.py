@@ -15,6 +15,7 @@ CONV, DENSE, DUELING, LOGSTD = 0, 1, 2, 3
 ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "sigmoid": 3, "softsign": 4, "softplus": 5, "leaky_relu": 6, "elu": 7,
        "selu": 8, "swish": 9, "gelu": 10}
 CLIP_NONE, CLIP_GLOBAL_NORM, CLIP_PER_TENSOR = 0, 1, 2
+PER_NONFINITE, PER_BAD_INDEX, PER_EMPTY = 1, 2, 4     # xtb_per status bits
 
 
 class LayerDesc(C.Structure):
@@ -86,6 +87,7 @@ _SIGS = {
     "xtb_last_error": (C.c_char_p, []),
     "xtb_launch_count": (C.c_longlong, []),
     "xtb_graph_replay_count": (C.c_longlong, []),
+    "xtb_graph_capture_count": (C.c_longlong, []),
     "xtb_net_create": (C.c_int, [C.POINTER(NetDesc), C.c_int, C.POINTER(_P)]),
     "xtb_net_destroy": (None, [_P]),
     "xtb_net_param_count": (C.c_longlong, [_P]),
@@ -116,6 +118,17 @@ _SIGS = {
     "xtb_impala_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _P, C.c_int, _P]),
     "xtb_dqn_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_int, _P, _P, _P,
                                C.c_int, _P]),
+    "xtb_dqn_train_weighted": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_int, _P, _P,
+                                        _P, _P, _P, C.c_int, _P]),
+    "xtb_per_create": (C.c_int, [C.c_int, C.c_double, C.c_double, C.c_uint64, C.POINTER(_P)]),
+    "xtb_per_destroy": (None, [_P]),
+    "xtb_per_add": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "xtb_per_sample": (C.c_int, [_P, C.c_int, C.c_double, _P, _P, _P, _P]),
+    "xtb_per_update": (C.c_int, [_P, _P, _P, C.c_int, _P]),
+    "xtb_per_state": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                C.POINTER(C.c_ulonglong), _P, _P]),
+    "xtb_dqn_per_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_double, C.c_int,
+                                   _P, _P, _P, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_mse_loss_grad": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
     "xtb_softmax": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
     "xtb_impala_keras_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,

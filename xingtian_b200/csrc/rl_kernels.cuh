@@ -371,6 +371,9 @@ __global__ void vtrace_kernel(const float* __restrict__ tp_logits, const float* 
 //   disc != NULL : per-sample bootstrap discount (gamma^n of an n-step return built by nstep_kernel; 0 = terminated)
 //   huber > 0    : Huber loss with that delta instead of the squared error (gradient clip(diff, -delta, delta))
 //   idx != NULL  : action / reward / done / disc are indexed through idx (minibatch rows of a replay ring)
+//   wt != NULL   : sample b's loss and gradient are scaled by wt[b] (prioritized replay's importance weights; Keras
+//                  train_on_batch with sample_weight: loss = 1/(B A) sum_b wt[b] sum_a e_ba)
+//   td_abs != NULL : td_abs[b] = |y - Q(s, a)| of the forward before the update (the new priorities)
 // ------------------------------------------------------------------------------------------
 // TD target of sample b, rollout row r: the max over the next-state Q row b of the target net (qn_o set: double DQN,
 // the target net's Q at the online net's argmax, the first maximum winning) bootstraps the reward unless done[r]
@@ -407,8 +410,9 @@ __global__ void dqn_loss_kernel(const float* __restrict__ q, const float* __rest
                                 const float* __restrict__ qn_o, const int32_t* __restrict__ idx,
                                 const int32_t* __restrict__ action, const float* __restrict__ reward,
                                 const uint8_t* __restrict__ done, const float* __restrict__ disc,
-                                int B, int A, float gamma, float huber, float inv_count, float* __restrict__ dq,
-                                float* __restrict__ y_out, float* __restrict__ loss_out) {
+                                int B, int A, float gamma, float huber, float inv_count, const float* __restrict__ wt,
+                                float* __restrict__ dq, float* __restrict__ y_out, float* __restrict__ td_abs,
+                                float* __restrict__ loss_out) {
   pdl_wait(); pdl_trigger();
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   float lsum = 0.f;
@@ -417,7 +421,10 @@ __global__ void dqn_loss_kernel(const float* __restrict__ q, const float* __rest
     const float y = dqn_td_target(qn_t, qn_o, reward, done, disc, gamma, b, r, A);
     const int a = action[r];
     float grad;
-    const float l = td_loss(q[(long long)b * A + a] - y, huber, grad);
+    const float diff = q[(long long)b * A + a] - y;
+    float l = td_loss(diff, huber, grad);
+    if (wt) { l *= wt[b]; grad *= wt[b]; }
+    if (td_abs) td_abs[b] = fabsf(diff);
     for (int i = 0; i < A; i++) dq[(long long)b * A + i] = (i == a) ? grad * inv_count : 0.f;
     if (y_out) y_out[b] = y;
     lsum = l * inv_count;
@@ -481,6 +488,7 @@ struct PpoHeadsArgs {
   // reduction of the loss slot writes loss_in + this step's loss).
   const float* qn_t; const float* qn_o; const float* reward; const uint8_t* done; const float* disc; const float* loss_in;
   float gamma, huber;
+  const float* wt; float* td_abs;          // optional per-sample loss weights and |TD error| output, as dqn_loss_kernel
   // Gaussian PPO (PpoGaussLoss): float behaviour actions [N, A] indexed through idx, and the A floats of pi_logstd
   const float* action_f; const float* log_std;
 };
@@ -535,12 +543,14 @@ struct DuelingTdLoss {
     for (int i = 0; i < HEAD_AMAX; i++) if (i == ac) q_a = adv + (val[i] - mean);
     const float y = dqn_td_target(a.qn_t, a.qn_o, a.reward, a.done, a.disc, a.gamma, b, r, A);
     float grad;
-    const float l = td_loss(q_a - y, a.huber, grad);
+    float l = td_loss(q_a - y, a.huber, grad);
+    if (a.wt) { l *= a.wt[b]; grad *= a.wt[b]; }
     const float c = grad * a.inv_count, cm = c / A;
 #pragma unroll
     for (int i = 0; i < HEAD_AMAX; i++) dl[i] = (i < A) ? ((i == ac) ? c : 0.f) - cm : 0.f;
     dv = c;
     if (lane == 0) {
+      if (a.td_abs) a.td_abs[b] = fabsf(q_a - y);
       lsum += l * a.inv_count;
       if (b == 0) lsum += *a.loss_in;
       dbv += dv;

@@ -17,6 +17,7 @@
 #include "gemm_f32.cuh"
 #include "optim.cuh"
 #include "rl_kernels.cuh"
+#include "per.cuh"
 #include "qmix.cuh"
 #include "scc.cuh"
 #include "stager.cuh"
@@ -1661,16 +1662,24 @@ extern "C" int xtb_vtrace_loss_grad(const float* tp_logits, const float* baselin
   return XTB_OK;
 }
 
+// dqn_loss_kernel with its optional per-sample weights `wt` and |TD error| output `td_abs` (NULL: the plain step)
+static int dqn_td_loss(const float* q, const float* q_next_target, const float* q_next_online, const int32_t* idx,
+                       const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int batch, int adim,
+                       float gamma, float huber_delta, float inv_count, const float* wt, float* dq, float* y_out, float* td_abs,
+                       float* loss_out, void* stream) {
+  XLAUNCH(dqn_loss_kernel, (batch + 127) / 128, 128, 0, S(stream), q, q_next_target, q_next_online, idx, action, reward, done, disc,
+          batch, adim, gamma, huber_delta, inv_count, wt, dq, y_out, td_abs, loss_out);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
 extern "C" int xtb_dqn_td_loss_grad(const float* q, const float* q_next_target, const float* q_next_online, const int32_t* idx,
                                     const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int batch,
                                     int adim, float gamma, float huber_delta, float inv_count, float* dq, float* y_out,
                                     float* loss_out, void* stream) {
   if (!q || !q_next_target || !action || !reward || !done || !dq || !loss_out) return fail(XTB_ERR_ARG, "xtb_dqn_td_loss_grad: null pointer");
   if (batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_dqn_td_loss_grad: bad sizes");
-  XLAUNCH(dqn_loss_kernel, (batch + 127) / 128, 128, 0, S(stream), q, q_next_target, q_next_online, idx, action, reward, done, disc,
-          batch, adim, gamma, huber_delta, inv_count, dq, y_out, loss_out);
-  LAUNCH_CHECK();
-  return XTB_OK;
+  return dqn_td_loss(q, q_next_target, q_next_online, idx, action, reward, done, disc, batch, adim, gamma, huber_delta, inv_count,
+                     nullptr, dq, y_out, nullptr, loss_out, stream);
 }
 extern "C" int xtb_dqn_loss_grad(const float* q, const float* q_next_target, const float* q_next_online,
                                  const int32_t* action, const float* reward, const uint8_t* done, int batch,
@@ -1911,7 +1920,7 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
                 kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
-                kSccTrain, kSccInfer, kSccCritic };
+                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -1942,7 +1951,9 @@ struct GraphVal { cudaGraphExec_t exec; long long kernels; };
 static constexpr size_t kMaxCachedGraphs = 256;   // beyond it the cache is emptied (keys are buffer addresses)
 static std::map<CaptureKey, GraphVal> g_graphs;
 static std::atomic<long long> g_graph_replays{0};
+static std::atomic<long long> g_graph_captures{0};
 extern "C" long long xtb_graph_replay_count(void) { return g_graph_replays.load(); }
+extern "C" long long xtb_graph_capture_count(void) { return g_graph_captures.load(); }
 
 // cached graphs hold raw pointers into their owners: they die with the object (a later object may be allocated at
 // the same address) and with a net's binding
@@ -1983,6 +1994,7 @@ static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
       g_graphs.clear();
     }
     it = g_graphs.emplace(key, GraphVal{exec, captured}).first;
+    g_graph_captures.fetch_add(1, std::memory_order_relaxed);
   }
   CUDA_TRY(cudaGraphLaunch(it->second.exec, sc.st));
   g_launches.fetch_add(it->second.kernels, std::memory_order_relaxed);
@@ -3159,7 +3171,8 @@ static bool dueling_fusable(const xtb_net* net, int q_tensor) {
 // and the gradient wrt the hidden tensor; then the backward pass of the layers below.
 static int dueling_td_fused(xtb_net* net, const void* obs, const int32_t* idx, const int32_t* action, const float* reward,
                             const uint8_t* done, const float* disc, int n, float gamma, float huber, int q_tensor,
-                            const float* qn_t, const float* qn_o, float inv_count, float* loss_out, cudaStream_t st) {
+                            const float* qn_t, const float* qn_o, float inv_count, const float* wt, float* td_abs, float* loss_out,
+                            cudaStream_t st) {
   const LayerPlan& lq = net->L[q_tensor - 1];
   const int h = net->L[lq.d.src - 1].d.src;
   const unsigned skip = (1u << (q_tensor - 1)) | (1u << (lq.d.src - 1)) | (1u << (lq.d.k - 1));
@@ -3168,7 +3181,7 @@ static int dueling_td_fused(xtb_net* net, const void* obs, const int32_t* idx, c
   PpoHeadsArgs a;
   memset(&a, 0, sizeof a);
   a.idx = idx; a.action = action; a.reward = reward; a.done = done; a.disc = disc; a.qn_t = qn_t; a.qn_o = qn_o; a.loss_in = loss_out;
-  a.gamma = gamma; a.huber = huber; a.inv_count = inv_count;
+  a.gamma = gamma; a.huber = huber; a.inv_count = inv_count; a.wt = wt; a.td_abs = td_abs;
   return heads_fused<DuelingTdLoss>(net, obs, a, n, lq.d.src, lq.d.k, skip, -1, loss_out, st);
 }
 
@@ -3176,48 +3189,191 @@ static int dueling_td_fused(xtb_net* net, const void* obs, const int32_t* idx, c
 // done[, disc]); target-network forward on s', optional double-DQN online forward on s', online forward on s, TD target +
 // loss gradient, backward, clip + Adam.  qn_t / qn_o: scratch [n, adim] (qn_o NULL = plain DQN).  Reference mode:
 // disc = NULL, huber_delta = 0.  With a communicator every rank holds n of world*n samples: inv_count = 1/(world*n*adim).
+// wt / td_abs (both may be NULL): per-sample loss weights and the |TD error| output of the loss kernels.
+static int dqn_check(const char* fn, bool missing, xtb_net* net, xtb_net* target, xtb_adam* opt, int n_sample, int q_tensor) {
+  if (int rc = learner_check(fn, missing, net, opt, n_sample, true)) return rc;
+  if (!target->ws) return fail(XTB_ERR_STATE, "%s: target net not bound", fn);
+  const int nl = (int)net->L.size();
+  if (q_tensor < 1 || q_tensor > nl || (int)target->L.size() != nl) return fail(XTB_ERR_ARG, "%s: bad head tensor", fn);
+  if (n_sample > target->max_batch) return fail(XTB_ERR_ARG, "%s: batch exceeds the target net's max_batch", fn);
+  return XTB_OK;
+}
+static int dqn_train_launch(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
+                            const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
+                            const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
+                            float* qn_o, const float* wt, float* td_abs, float* loss_out, void* st) {
+  const int adim = net->tsize[q_tensor];
+  const size_t qbytes = (size_t)n_sample * adim * sizeof(float);
+  int rc = net_forward_impl(target, nullptr, next_obs, idx, n_sample, st, 0u, 1u << q_tensor);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(qn_t, xtb_net_tensor(target, q_tensor), qbytes, cudaMemcpyDeviceToDevice, S(st)));
+  if (qn_o) {
+    rc = net_forward_impl(net, nullptr, next_obs, idx, n_sample, st, 0u, 1u << q_tensor);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(qn_o, xtb_net_tensor(net, q_tensor), qbytes, cudaMemcpyDeviceToDevice, S(st)));
+  }
+  const float inv_count = dp_inv_world() / ((float)n_sample * adim);
+  if (dueling_fusable(net, q_tensor)) {
+    rc = dueling_td_fused(net, obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor, qn_t, qn_o,
+                          inv_count, wt, td_abs, loss_out, S(st));
+    if (rc) return rc;
+  } else {
+    rc = net_forward_impl(net, nullptr, obs, idx, n_sample, st, 0u, 1u << q_tensor);
+    if (rc) return rc;
+    rc = dqn_td_loss(xtb_net_tensor(net, q_tensor), qn_t, qn_o, idx, action, reward, done, disc, n_sample, adim, gamma,
+                     huber_delta, inv_count, wt, xtb_net_tensor_grad(net, q_tensor), nullptr, td_abs, loss_out, st);
+    if (rc) return rc;
+    const int32_t heads[1] = {q_tensor};
+    BackwardOpts o(heads, 1); o.all_reduce = true;
+    rc = net_backward_impl(net, obs, idx, n_sample, st, o);
+    if (rc) return rc;
+  }
+  return xtb_adam_step_net(opt, net, 1.f, st);
+}
 extern "C" int xtb_dqn_train(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
                              const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                              const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
                              float* qn_o, float* loss_out, int use_graph, void* stream) {
   const bool missing = !net || !target || !opt || !obs || !next_obs || !action || !reward || !done || !qn_t || !loss_out;
-  if (int rc = learner_check("xtb_dqn_train", missing, net, opt, n_sample, true)) return rc;
-  if (!target->ws) return fail(XTB_ERR_STATE, "xtb_dqn_train: target net not bound");
-  const int nl = (int)net->L.size();
-  if (q_tensor < 1 || q_tensor > nl || (int)target->L.size() != nl) return fail(XTB_ERR_ARG, "xtb_dqn_train: bad head tensor");
-  if (n_sample > target->max_batch) return fail(XTB_ERR_ARG, "xtb_dqn_train: batch exceeds the target net's max_batch");
-  const int adim = net->tsize[q_tensor];
-  const float inv_world = dp_inv_world();
-  const bool fuse = dueling_fusable(net, q_tensor);
+  if (int rc = dqn_check("xtb_dqn_train", missing, net, target, opt, n_sample, q_tensor)) return rc;
   return run_graph(capture_key(kDqnTrain, {net, target, opt}, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o, loss_out,
                                n_sample, gamma, huber_delta, q_tensor),
                    use_graph, stream, [&](void* st) -> int {
-    const size_t qbytes = (size_t)n_sample * adim * sizeof(float);
-    int rc = net_forward_impl(target, nullptr, next_obs, idx, n_sample, st, 0u, 1u << q_tensor);
+    return dqn_train_launch(net, target, opt, obs, next_obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor,
+                            qn_t, qn_o, nullptr, nullptr, loss_out, st);
+  });
+}
+extern "C" int xtb_dqn_train_weighted(xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
+                                      const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
+                                      const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
+                                      float* qn_o, const float* weights, float* td_abs, float* loss_out, int use_graph, void* stream) {
+  const bool missing = !net || !target || !opt || !obs || !next_obs || !action || !reward || !done || !qn_t || !loss_out;
+  if (int rc = dqn_check("xtb_dqn_train_weighted", missing, net, target, opt, n_sample, q_tensor)) return rc;
+  return run_graph(capture_key(kDqnTrainWeighted, {net, target, opt}, obs, next_obs, idx, action, reward, done, disc, qn_t, qn_o,
+                               weights, td_abs, loss_out, n_sample, gamma, huber_delta, q_tensor),
+                   use_graph, stream, [&](void* st) -> int {
+    return dqn_train_launch(net, target, opt, obs, next_obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor,
+                            qn_t, qn_o, weights, td_abs, loss_out, st);
+  });
+}
+
+// ---- prioritized replay (per.cuh) -------------------------------------------------------------------------------------
+struct xtb_per {
+  PerTree t{};
+  int capacity = 0;
+  double alpha = 0, eps = 0;
+  uint64_t seed = 0;
+  void* buf = nullptr;         // the one device allocation: both trees, the update scratch and the PerState
+};
+
+extern "C" int xtb_per_create(int capacity, double alpha, double eps, uint64_t seed, xtb_per** out) {
+  if (!out) return fail(XTB_ERR_ARG, "xtb_per_create: null pointer");
+  if (capacity < 1 || capacity > (1 << 30)) return fail(XTB_ERR_ARG, "xtb_per_create: capacity %d not in [1, 2^30]", capacity);
+  if (!std::isfinite(alpha) || alpha < 0) return fail(XTB_ERR_ARG, "xtb_per_create: alpha %g is not finite and >= 0", alpha);
+  if (!std::isfinite(eps) || !(eps > 0)) return fail(XTB_ERR_ARG, "xtb_per_create: eps %g is not finite and > 0", eps);
+  auto* p = new xtb_per();
+  PerTree& t = p->t;
+  t.leaves = 1; t.depth = 0;
+  while (t.leaves < capacity) { t.leaves *= 2; t.depth++; }
+  const std::vector<double> inf((size_t)2 * t.leaves, INFINITY);
+  const std::vector<int32_t> none((size_t)t.leaves, -1);
+  PerState st0{};
+  st0.max_priority = 1.0;
+  if (int rc = carve_scratch("xtb_per_create", &p->buf, {{&t.sum, 2LL * t.leaves}, {&t.mn, 2LL * t.leaves, inf.data()},
+                                                        {&t.last, (long long)t.leaves, none.data()}, {&t.st, 1, &st0}})) {
+    delete p;
+    return rc;
+  }
+  p->capacity = capacity; p->alpha = alpha; p->eps = eps; p->seed = seed;
+  *out = p;
+  return XTB_OK;
+}
+
+extern "C" void xtb_per_destroy(xtb_per* p) {
+  if (!p) return;
+  drop_graphs_of(p);
+  cudaDeviceSynchronize();
+  cudaFree(p->buf);
+  delete p;
+}
+
+static int per_check(const char* fn, const xtb_per* p, bool missing) {
+  if (!p || missing) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
+  return XTB_OK;
+}
+static int per_sample_launch(xtb_per* p, int batch, double beta, const double* uniforms, int32_t* idx, float* w, void* stream) {
+  XLAUNCH(per_sample_kernel, 1, std::min(kPerThreads, (batch + 31) / 32 * 32), 0, S(stream), p->t, batch, beta, uniforms, p->seed,
+          idx, w);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+static int per_update_launch(xtb_per* p, const int32_t* idx, const float* td_abs, int n, void* stream) {
+  XLAUNCH(per_update_kernel, 1, std::min(kPerThreads, (n + 31) / 32 * 32), 0, S(stream), p->t, idx, td_abs, n, p->alpha, p->eps);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_per_add(xtb_per* p, int first_slot, int n, void* stream) {
+  if (int rc = per_check("xtb_per_add", p, false)) return rc;
+  if (first_slot < 0 || n < 1 || (long long)first_slot + n > p->capacity)
+    return fail(XTB_ERR_ARG, "xtb_per_add: slots [%d, %d + %d) not inside [0, %d)", first_slot, first_slot, n, p->capacity);
+  XLAUNCH(per_insert_kernel, 1, kPerThreads, 0, S(stream), p->t, first_slot, n, p->alpha);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_per_sample(xtb_per* p, int batch, double beta, const double* uniforms, int32_t* idx, float* w, void* stream) {
+  if (int rc = per_check("xtb_per_sample", p, !idx || !w)) return rc;
+  if (batch < 1) return fail(XTB_ERR_ARG, "xtb_per_sample: batch %d is not positive", batch);
+  if (!std::isfinite(beta) || !(beta > 0)) return fail(XTB_ERR_ARG, "xtb_per_sample: beta %g is not finite and > 0", beta);
+  return per_sample_launch(p, batch, beta, uniforms, idx, w, stream);
+}
+
+extern "C" int xtb_per_update(xtb_per* p, const int32_t* idx, const float* td_abs, int n, void* stream) {
+  if (int rc = per_check("xtb_per_update", p, !idx || !td_abs)) return rc;
+  if (n < 1) return fail(XTB_ERR_ARG, "xtb_per_update: batch %d is not positive", n);
+  return per_update_launch(p, idx, td_abs, n, stream);
+}
+
+extern "C" int xtb_per_state(const xtb_per* p, int* leaves, int* count, double* max_priority, int* status,
+                             unsigned long long* offset, double* sum_host, double* min_host) {
+  if (!p) return fail(XTB_ERR_ARG, "xtb_per_state: null pointer");
+  CUDA_TRY(cudaDeviceSynchronize());
+  PerState st;
+  CUDA_TRY(cudaMemcpy(&st, p->t.st, sizeof st, cudaMemcpyDeviceToHost));
+  if (sum_host) CUDA_TRY(cudaMemcpy(sum_host, p->t.sum, sizeof(double) * 2 * p->t.leaves, cudaMemcpyDeviceToHost));
+  if (min_host) CUDA_TRY(cudaMemcpy(min_host, p->t.mn, sizeof(double) * 2 * p->t.leaves, cudaMemcpyDeviceToHost));
+  if (leaves) *leaves = p->t.leaves;
+  if (count) *count = st.count;
+  if (max_priority) *max_priority = st.max_priority;
+  if (status) *status = st.status;
+  if (offset) *offset = st.offset;
+  return XTB_OK;
+}
+
+extern "C" int xtb_dqn_per_train(xtb_per* p, xtb_net* net, xtb_net* target, xtb_adam* opt, const void* obs, const void* next_obs,
+                                 const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int n_sample,
+                                 float gamma, float huber_delta, double beta, int q_tensor, float* qn_t, float* qn_o, int32_t* idx,
+                                 float* w, float* td_abs, float* loss_out, int32_t* status_out, int use_graph, void* stream) {
+  const char* fn = "xtb_dqn_per_train";
+  const bool missing = !net || !target || !opt || !obs || !next_obs || !action || !reward || !done || !qn_t || !loss_out || !idx ||
+                       !w || !td_abs || !status_out;
+  if (int rc = per_check(fn, p, missing)) return rc;
+  if (int rc = dqn_check(fn, missing, net, target, opt, n_sample, q_tensor)) return rc;
+  if (!std::isfinite(beta) || !(beta > 0)) return fail(XTB_ERR_ARG, "%s: beta %g is not finite and > 0", fn, beta);
+  return run_graph(capture_key(kDqnPerTrain, {net, target, opt, p}, obs, next_obs, action, reward, done, disc, n_sample, gamma,
+                               huber_delta, beta, q_tensor, qn_t, qn_o, idx, w, td_abs, loss_out, status_out),
+                   use_graph, stream, [&](void* st) -> int {
+    int rc = per_sample_launch(p, n_sample, beta, nullptr, idx, w, st);
     if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(qn_t, xtb_net_tensor(target, q_tensor), qbytes, cudaMemcpyDeviceToDevice, S(st)));
-    if (qn_o) {
-      rc = net_forward_impl(net, nullptr, next_obs, idx, n_sample, st, 0u, 1u << q_tensor);
-      if (rc) return rc;
-      CUDA_TRY(cudaMemcpyAsync(qn_o, xtb_net_tensor(net, q_tensor), qbytes, cudaMemcpyDeviceToDevice, S(st)));
-    }
-    const float inv_count = inv_world / ((float)n_sample * adim);
-    if (fuse) {
-      rc = dueling_td_fused(net, obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor, qn_t, qn_o,
-                            inv_count, loss_out, S(st));
-      if (rc) return rc;
-    } else {
-      rc = net_forward_impl(net, nullptr, obs, idx, n_sample, st, 0u, 1u << q_tensor);
-      if (rc) return rc;
-      rc = xtb_dqn_td_loss_grad(xtb_net_tensor(net, q_tensor), qn_t, qn_o, idx, action, reward, done, disc, n_sample, adim, gamma,
-                                huber_delta, inv_count, xtb_net_tensor_grad(net, q_tensor), nullptr, loss_out, st);
-      if (rc) return rc;
-      const int32_t heads[1] = {q_tensor};
-      BackwardOpts o(heads, 1); o.all_reduce = true;
-      rc = net_backward_impl(net, obs, idx, n_sample, st, o);
-      if (rc) return rc;
-    }
-    return xtb_adam_step_net(opt, net, 1.f, st);
+    rc = dqn_train_launch(net, target, opt, obs, next_obs, idx, action, reward, done, disc, n_sample, gamma, huber_delta, q_tensor,
+                          qn_t, qn_o, w, td_abs, loss_out, st);
+    if (rc) return rc;
+    rc = per_update_launch(p, idx, td_abs, n_sample, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(status_out, &p->t.st->status, sizeof(int32_t), cudaMemcpyDeviceToDevice, S(st)));
+    return XTB_OK;
   });
 }
 

@@ -77,14 +77,8 @@ class _DqnBase(XTModel):
         self.opt.step()
         return float(b["loss"].cpu()[0])
 
-    def train_td_device(self, target_model, obs, action, reward, next_obs, done, n, gamma, loss_buf, double_dqn=False,
-                        idx=None, disc=None, huber_delta=0.0):
-        """Fused DQN.train (xt/algorithm/dqn/dqn.py:61-97) on device-resident transitions: target forward,
-        (double-DQN online forward on s'), online forward on s, TD target + loss gradient, backward, Adam -- one native
-        call replayed as a CUDA graph.  `idx` (int32 device tensor): the step uses rows idx[0..n) of the given buffers
-        (a replay ring) without copying them; `disc`: per-row n-step bootstrap discount; huber_delta > 0: Huber loss."""
-        net = self.net
-        net.ensure_batch(n)
+    def _td_scratch(self, target_model, n):
+        self.net.ensure_batch(n)
         target_model.net.ensure_batch(n)
         key = ("td", n)
         sc = self._bufs.get(key)
@@ -92,11 +86,42 @@ class _DqnBase(XTModel):
             sc = dict(qn_t=torch.empty(n, self.action_dim, dtype=torch.float32, device=self.device),
                       qn_o=torch.empty(n, self.action_dim, dtype=torch.float32, device=self.device))
             self._bufs[key] = sc
+        return sc
+
+    def train_td_device(self, target_model, obs, action, reward, next_obs, done, n, gamma, loss_buf, double_dqn=False,
+                        idx=None, disc=None, huber_delta=0.0, *, weights=None, td_abs=None):
+        """Fused DQN.train (xt/algorithm/dqn/dqn.py:61-97) on device-resident transitions: target forward,
+        (double-DQN online forward on s'), online forward on s, TD target + loss gradient, backward, Adam -- one native
+        call replayed as a CUDA graph.  `idx` (int32 device tensor): the step uses rows idx[0..n) of the given buffers
+        (a replay ring) without copying them; `disc`: per-row n-step bootstrap discount; huber_delta > 0: Huber loss.
+        `weights` (float32 device [n]): importance weights scaling each sample's loss and gradient; `td_abs` (float32
+        device [n]): receives |TD error| of each sample from the forward before the update."""
+        net = self.net
+        sc = self._td_scratch(target_model, n)
         loss_buf.zero_()
-        check(net.lib.xtb_dqn_train(net.handle, target_model.net.handle, self.opt.handle, _ptr(obs), _ptr(next_obs), _ptr(idx),
-                                    _ptr(action), _ptr(reward), _ptr(done), _ptr(disc), int(n), float(gamma), float(huber_delta),
-                                    net.tid[self.q_name], _ptr(sc["qn_t"]), _ptr(sc["qn_o"]) if double_dqn else None,
-                                    _ptr(loss_buf), 1 if self.use_graph else 0, stream_ptr()))
+        common = (net.handle, target_model.net.handle, self.opt.handle, _ptr(obs), _ptr(next_obs), _ptr(idx), _ptr(action),
+                  _ptr(reward), _ptr(done), _ptr(disc), int(n), float(gamma), float(huber_delta), net.tid[self.q_name],
+                  _ptr(sc["qn_t"]), _ptr(sc["qn_o"]) if double_dqn else None)
+        if weights is None and td_abs is None:
+            check(net.lib.xtb_dqn_train(*common, _ptr(loss_buf), 1 if self.use_graph else 0, stream_ptr()))
+        else:
+            check(net.lib.xtb_dqn_train_weighted(*common, _ptr(weights), _ptr(td_abs), _ptr(loss_buf), 1 if self.use_graph else 0,
+                                                 stream_ptr()))
+        return loss_buf
+
+    def train_per_device(self, target_model, per, beta, obs, action, reward, next_obs, done, n, gamma, loss_buf, idx, weights,
+                         td_abs, status, double_dqn=False, disc=None, huber_delta=0.0):
+        """One prioritized-replay step as one CUDA graph (xtb_dqn_per_train): draw n ring rows from the sum tree `per`
+        into idx with importance weights (exponent beta) into weights, train_td_device on them with those weights and
+        td_abs, write the new priorities back and copy the tree's status bits into `status` (int32 device [1])."""
+        net = self.net
+        sc = self._td_scratch(target_model, n)
+        loss_buf.zero_()
+        check(net.lib.xtb_dqn_per_train(per, net.handle, target_model.net.handle, self.opt.handle, _ptr(obs), _ptr(next_obs),
+                                        _ptr(action), _ptr(reward), _ptr(done), _ptr(disc), int(n), float(gamma),
+                                        float(huber_delta), float(beta), net.tid[self.q_name], _ptr(sc["qn_t"]),
+                                        _ptr(sc["qn_o"]) if double_dqn else None, _ptr(idx), _ptr(weights), _ptr(td_abs),
+                                        _ptr(loss_buf), _ptr(status), 1 if self.use_graph else 0, stream_ptr()))
         return loss_buf
 
 
