@@ -699,32 +699,37 @@ class PpoLearner(Learner):
 
 def vtrace_from_logits(bp_logits, tp_logits, actions, discounts, rewards, values, bootstrap,
                        clip_rho=1.0, clip_pg_rho=1.0):
-    """xt/model/impala/vtrace.py:39-115.  Inputs time-major [T,B,(A)], fp32 numpy.
-    Returns vs[T,B], pg_adv[T,B]."""
-    f32 = np.float32
+    """xt/model/impala/vtrace.py:39-115.  Inputs time-major [T,B,(A)] numpy, computed in the working precision:
+    logits are cast to it, the other inputs widened to at least it.  Returns vs[T,B], pg_adv[T,B]."""
+    f = _PREC["np"]
 
     def logp(lg, a):
         m = lg.max(-1, keepdims=True)
         lse = m + np.log(np.exp(lg - m).sum(-1, keepdims=True))
         return np.take_along_axis(lg - lse, a[..., None].astype(np.int64), -1)[..., 0]
 
-    tlp = logp(tp_logits.astype(f32), actions)
-    blp = logp(bp_logits.astype(f32), actions)
-    rho = np.exp(tlp - blp).astype(f32)
-    crho = np.minimum(f32(clip_rho), rho)
-    cpg = np.minimum(f32(clip_pg_rho), rho)
-    cs = np.minimum(f32(1.0), rho)
+    def widen(x):
+        x = np.asarray(x)
+        return x.astype(np.promote_types(x.dtype, f), copy=False)
+
+    discounts, rewards, values, bootstrap = widen(discounts), widen(rewards), widen(values), widen(bootstrap)
+    tlp = logp(tp_logits.astype(f), actions)
+    blp = logp(bp_logits.astype(f), actions)
+    rho = np.exp(tlp - blp).astype(f)
+    crho = np.minimum(f(clip_rho), rho)
+    cpg = np.minimum(f(clip_pg_rho), rho)
+    cs = np.minimum(f(1.0), rho)
     nv = np.concatenate([values[1:], bootstrap[None]], 0)
     deltas = crho * (rewards + discounts * nv - values)
-    acc = np.zeros_like(bootstrap, dtype=f32)
-    out = np.zeros_like(values, dtype=f32)
+    acc = np.zeros_like(bootstrap, dtype=f)
+    out = np.zeros_like(values, dtype=f)
     for t in range(values.shape[0] - 1, -1, -1):
-        acc = (deltas[t] + discounts[t] * cs[t] * acc).astype(f32)
+        acc = (deltas[t] + discounts[t] * cs[t] * acc).astype(f)
         out[t] = acc
     vs = out + values
     vs_next = np.concatenate([vs[1:], bootstrap[None]], 0)
     pg = cpg * (rewards + discounts * vs_next - values)
-    return vs.astype(f32), pg.astype(f32)
+    return vs.astype(f), pg.astype(f)
 
 
 def split_batches(x, batch_step, drop_last=False):
@@ -737,16 +742,18 @@ def split_batches(x, batch_step, drop_last=False):
 
 def impala_loss(tp_logits_flat, baseline_flat, bp_logits, actions, dones, rewards, batch_step, gamma=0.99):
     """impala_cnn_opt.py:188-196 + :299-351.  tp_logits_flat [N,A] / baseline_flat [N]
-    torch tensors (grad flows); the rest numpy, env-major flat [N]."""
+    torch tensors (grad flows); the rest numpy, env-major flat [N].  The V-trace targets are computed in the working
+    precision."""
+    f = _PREC["np"]
     tp = split_batches(tp_logits_flat, batch_step, True)
     val = split_batches(baseline_flat, batch_step, True)
     boot = split_batches(baseline_flat, batch_step)[-1]
-    bp = split_batches(np.asarray(bp_logits, np.float32), batch_step, True)
+    bp = split_batches(np.asarray(bp_logits, f), batch_step, True)
     act = split_batches(np.asarray(actions, np.int32), batch_step, True)
-    disc = split_batches((~np.asarray(dones, bool)).astype(np.float32) * np.float32(gamma), batch_step, True)
-    rew = split_batches(np.clip(np.asarray(rewards, np.float32), -1, 1), batch_step, True)
+    disc = split_batches((~np.asarray(dones, bool)).astype(f) * f(gamma), batch_step, True)
+    rew = split_batches(np.clip(np.asarray(rewards, f), -1, 1), batch_step, True)
     vs, pg = vtrace_from_logits(bp, tp.detach().numpy(), act, disc, rew, val.detach().numpy(), boot.detach().numpy())
-    vs_t, pg_t = torch.from_numpy(vs), torch.from_numpy(pg)
+    vs_t, pg_t = torch.from_numpy(vs).to(_PREC["t"]), torch.from_numpy(pg).to(_PREC["t"])
     lsm = torch.log_softmax(tp, -1)
     xent = -lsm.gather(-1, torch.from_numpy(act.astype(np.int64))[..., None])[..., 0]
     pi_loss = (xent * pg_t).sum()

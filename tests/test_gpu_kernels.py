@@ -172,37 +172,6 @@ def test_ppo_loss_grad_matches_autograd(xb, B, A):
     assert rel_err(dv.cpu().numpy(), vt.grad.numpy()[:, 0]) < REL
 
 
-# ------------------------------------------------------------------------------------------- V-trace
-@pytest.mark.parametrize("k,S,A", [(4, 128, 4), (64, 128, 4), (1, 2, 4), (3, 50, 6)])
-def test_vtrace_loss_grad(xb, k, S, A):
-    from xingtian_b200.engine import _ptr, stream_ptr
-    rng = np.random.default_rng(k * 7 + S)
-    N = k * S
-    tp = rng.standard_normal((N, A)).astype(np.float32)
-    bp = (tp + 0.5 * rng.standard_normal((N, A))).astype(np.float32)
-    base = rng.standard_normal(N).astype(np.float32)
-    act = rng.integers(0, A, N).astype(np.int32)
-    done = rng.random(N) < 0.02
-    rew = rng.normal(0, 2, N).astype(np.float32)
-    tpt = torch.from_numpy(tp).requires_grad_(True); bt = torch.from_numpy(base).requires_grad_(True)
-    loss = orc.impala_loss(tpt, bt, bp, act, done, rew, S)
-    loss.backward()
-    dl = torch.empty(N, A, device="cuda"); db = torch.empty(N, device="cuda"); lo = torch.zeros(1, device="cuda")
-    vs = torch.empty(N, device="cuda"); pg = torch.empty(N, device="cuda")
-    xb["capi"].check(xb["lib"].xtb_vtrace_loss_grad(_ptr(dev(tp)), _ptr(dev(base)), _ptr(dev(bp)), _ptr(dev(act)), _ptr(dev(done.view(np.uint8))),
-                                                   _ptr(dev(rew)), k, S, A, 0.99, _ptr(dl), _ptr(db), _ptr(vs), _ptr(pg), _ptr(lo), stream_ptr()))
-    assert abs(float(lo.cpu()[0]) - float(loss)) < REL * max(1.0, abs(float(loss)))
-    assert rel_err(dl.cpu().numpy(), tpt.grad.numpy()) < REL
-    assert rel_err(db.cpu().numpy(), bt.grad.numpy()) < REL
-    # vs / pg_adv against the numpy restatement of vtrace.py
-    sb = lambda x, dl_=True: orc.split_batches(x, S, dl_)
-    vs_ref, pg_ref = orc.vtrace_from_logits(sb(bp), sb(tp), sb(act), sb((~done).astype(np.float32) * np.float32(0.99)),
-                                            sb(np.clip(rew, -1, 1)), sb(base), orc.split_batches(base, S)[-1])
-    got_vs = vs.cpu().numpy().reshape(k, S)[:, :S - 1].T
-    got_pg = pg.cpu().numpy().reshape(k, S)[:, :S - 1].T
-    assert rel_err(got_vs, vs_ref) < REL and rel_err(got_pg, pg_ref) < REL
-
-
 # ------------------------------------------------------------------------------------------- DQN
 @pytest.mark.parametrize("B,A,double", [(32, 4, False), (512, 4, False), (32, 6, True)])
 def test_dqn_target_and_mse(xb, B, A, double):
