@@ -657,6 +657,69 @@ int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hid
 /* SCCModel.get_mixer_output (scc_tf.py:500-503): v_out[r] = V_eval(states[r]) for states [rows, n_agents D], rows <= B L. */
 int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream);
 
+/* ---- InfoFlow recommender DQN: replaces DqnInfoFlowModel's Keras graph (xt/model/dqn/dqn_rec_model.py:63-169) and the
+ * target computation of DQNInfoFlowAlg.train (xt/algorithm/dqn/dqn_infoflw_alg.py:76-174) --------------------------------
+ * Inputs are int32 ids in [0, vocab) (Keras Embedding's cast; not checked on the device): user [user_dim], history_click
+ * and history_no_click [5 item_dim], item [item_dim].  With E = emb_dim and U = item_dim E, a weight set is one flat
+ * float buffer [gru | gru_1 | head]: each GRU is Keras GRU v1 (hard_sigmoid gates, reset_after=False, last output only)
+ * with kernel [U, 3U], recurrent_kernel [U, 3U] and bias [3U] back to back (gate columns [z | r | h]), gru at offset 0
+ * on the clicked history and gru_1 at gru1_off on the viewed one; the head is one net of three dense layers, dense
+ * (relu) on rows of D = user_dim E + 3U floats [Flatten(emb(user)) | h_click | h_noclick | Flatten(emb(item))], dense_1
+ * (relu) and q_value (1 wide, activation last_act), bound at head_off of the set and of a gradient buffer with the same
+ * layout.  The embedding table [vocab, E] is frozen and lives outside the set.
+ * Limits (XTB_ERR_ARG at create): every size positive, U <= 137 (the GRU kernels' shared-memory plan), gru1_off and
+ * head_off multiples of 64 with the slices in order and not overlapping. */
+typedef struct xtb_infoflow xtb_infoflow;
+typedef struct xtb_infoflow_desc {
+  int32_t user_dim, item_dim, emb_dim, vocab;
+  int32_t batch;            /* B transitions per training step */
+  int32_t last_act;         /* xtb_act of q_value */
+  double gamma;
+  long long gru_off;        /* 0 */
+  long long gru1_off;       /* offset (floats) of gru_1/kernel */
+  long long head_off;       /* offset (floats) of dense/kernel */
+  const float* table;       /* [vocab, emb_dim] Emb/embeddings (device) */
+} xtb_infoflow_desc;
+int xtb_infoflow_create(const xtb_infoflow_desc* desc, xtb_infoflow** out);
+void xtb_infoflow_destroy(xtb_infoflow* f);
+/* One minibatch of B transitions (device arrays).  The candidates of the next states are ragged: transition b's are
+ * rows cand_off[b] .. cand_off[b+1] of cand_item, and cand_off[B] must equal n_cand. */
+typedef struct xtb_infoflow_batch {
+  const int32_t* user;          /* [B, user_dim] */
+  const int32_t* click;         /* [B, 5 item_dim] */
+  const int32_t* noclick;       /* [B, 5 item_dim] */
+  const int32_t* item;          /* [B, item_dim] the action taken */
+  const int32_t* next_user;     /* [B, user_dim] */
+  const int32_t* next_click;    /* [B, 5 item_dim] */
+  const int32_t* next_noclick;  /* [B, 5 item_dim] */
+  const int32_t* cand_off;      /* [B + 1], read on the device */
+  const int32_t* cand_item;     /* [cand_cap, item_dim], rows past n_cand unread */
+  const double* reward;         /* [B] */
+  const int32_t* done;          /* [B] nonzero: done */
+  const float* label;           /* NULL: the target pass computes the targets; else the targets [B] of a plain fit step
+                                   (DqnInfoFlowModel.train), and the next_* / cand_* / reward / done fields may be NULL */
+  int32_t n_cand;               /* candidate rows of the batch */
+  int32_t cand_cap;             /* rows the target pass runs: >= max(n_cand, B), <= the head's max batch; callers keep it
+                                   to a few values (a power of two that only grows) so that few graphs are captured */
+} xtb_infoflow_batch;
+/* DQNInfoFlowAlg.train's target and DqnInfoFlowModel.train (one Keras fit step) as one graph:
+ *   1. target pass with the online weights: both GRUs once per transition on the next histories, the head on cand_cap
+ *      rows [next user | h_click | h_noclick | candidate item] (rows past n_cand zeroed), then
+ *      target[b] = reward[b] if done[b] else (float)(max_c q_c * gamma + reward[b]) in float64 (NaN propagates);
+ *   2. the training forward on the B transitions, the mse loss (*loss_out, before the update, summed in a fixed order),
+ *      the head's backward with d loss / d input, the GRUs' backward from the h_click / h_noclick slices (no gradient
+ *      into the frozen table) and their weight gradients as GEMMs over all step rows;
+ *   3. one step of `opt` (Keras Adam, epsilon 1e-7, no clipping) over [gru | gru_1 | head], then the head's weight refresh.
+ * With batch->label the target pass is skipped and the labels are the targets.  target_out [B] (may be NULL) receives
+ * the targets.  XTB_ERR_STATE while a communicator is installed: the GRUs'
+ * gradients are not summed over ranks. */
+int xtb_infoflow_train(xtb_infoflow* f, xtb_net* head, xtb_adam* opt, const xtb_infoflow_batch* batch, float* loss_out,
+                       float* target_out, int use_graph, void* stream);
+/* DqnInfoFlowModel.predict (dqn_rec_model.py:156-169): q_out[r] for n rows in the tiled dict form (user [n, user_dim],
+ * click / noclick [n, 5 item_dim], item [n, item_dim]), each row its own GRU sequences; n <= the head's max batch. */
+int xtb_infoflow_predict(xtb_infoflow* f, xtb_net* head, const int32_t* user, const int32_t* click, const int32_t* noclick,
+                         const int32_t* item, int n, float* q_out, int use_graph, void* stream);
+
 /* xtb_net_backward that also writes d loss / d observation [batch, obs width] into dobs (overwritten): the data-gradient
  * GEMM of every dense layer that reads the observation, summed in layer order.  Float observations with scale 1 read
  * by dense layers only; otherwise XTB_ERR_ARG. */

@@ -8,3 +8,4 @@ from .replay_buffer import ReplayBuffer, DeviceReplayBuffer  # noqa: F401
 from .muzero import Muzero  # noqa: F401
 from .qmix import QMixAlg  # noqa: F401
 from .scc import SCCAlg  # noqa: F401
+from .dqn_infoflow import DQNInfoFlowAlg  # noqa: F401

@@ -81,6 +81,18 @@ class SccBatch(C.Structure):
                 ("terminated", C.c_void_p), ("mask", C.c_void_p), ("subsets", C.c_void_p)]
 
 
+class InfoflowDesc(C.Structure):
+    _fields_ = [("user_dim", C.c_int32), ("item_dim", C.c_int32), ("emb_dim", C.c_int32), ("vocab", C.c_int32), ("batch", C.c_int32),
+                ("last_act", C.c_int32), ("gamma", C.c_double), ("gru_off", C.c_longlong), ("gru1_off", C.c_longlong),
+                ("head_off", C.c_longlong), ("table", C.c_void_p)]
+
+
+class InfoflowBatch(C.Structure):
+    _fields_ = [("user", C.c_void_p), ("click", C.c_void_p), ("noclick", C.c_void_p), ("item", C.c_void_p), ("next_user", C.c_void_p),
+                ("next_click", C.c_void_p), ("next_noclick", C.c_void_p), ("cand_off", C.c_void_p), ("cand_item", C.c_void_p),
+                ("reward", C.c_void_p), ("done", C.c_void_p), ("label", C.c_void_p), ("n_cand", C.c_int32), ("cand_cap", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "xtb_version": (C.c_int, []),
@@ -175,6 +187,10 @@ _SIGS = {
     "xtb_scc_train": (C.c_int, [_P, _P, _P, _P, C.POINTER(SccBatch), _P, C.c_int, _P]),
     "xtb_scc_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_scc_critic": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, _P]),
+    "xtb_infoflow_create": (C.c_int, [C.POINTER(InfoflowDesc), C.POINTER(_P)]),
+    "xtb_infoflow_destroy": (None, [_P]),
+    "xtb_infoflow_train": (C.c_int, [_P, _P, _P, C.POINTER(InfoflowBatch), _P, _P, C.c_int, _P]),
+    "xtb_infoflow_predict": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, _P, C.c_int, _P]),
     "xtb_net_backward_input": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int32), C.c_int, _P, _P]),
     "xtb_comm_unique_id": (C.c_int, [C.c_char_p, _P]),
     "xtb_comm_create": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.POINTER(_P)]),

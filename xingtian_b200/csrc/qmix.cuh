@@ -26,21 +26,37 @@ __host__ __device__ inline long long qgru_smem_floats(int H, int G) {
 }
 
 __device__ inline float qsigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+// Keras hard_sigmoid (TF 1.15 backend): clip(0.2 x + 0.5, 0, 1), each operation rounded as TF rounds it
+__device__ inline float qhard_sigmoid(float x) { return fminf(fmaxf(__fadd_rn(__fmul_rn(0.2f, x), 0.5f), 0.f), 1.f); }
+__device__ inline float qhard_sigmoid_grad(float v) { return v > 0.f && v < 1.f ? 0.2f : 0.f; }
 
-__device__ inline void qgru_load_weights(const float* __restrict__ Wg, const float* __restrict__ Wc, int H, float* wg, float* wc) {
+// Where a GRU's recurrent weights sit and which gate activation it uses.  The gate block is [H][2H] at wg (row stride
+// ldg), the reset gate in columns [r_col, r_col + H) and the update gate in the other H; the candidate block is
+// [H][H] at wc (row stride ldc).  The gate pre-activations xg / dag and the [r|u] activations share the gate block's
+// column order.
+//   TF GRUCell (QMIX, SCC): gates [r|u] (r_col 0) in rows H.. of gates/kernel [2H, 2H], candidate rows H.. of
+//   candidate/kernel [2H, H], sigmoid.
+//   Keras GRU v1: recurrent_kernel [H, 3H] = [z | r | h] read in place (ldg = ldc = 3H, r_col H), hard_sigmoid.
+struct GruRec {
+  const float* wg; const float* wc; int ldg, ldc, r_col, hard;
+};
+
+__device__ inline void qgru_load_weights(const GruRec& w, int H, float* wg, float* wc) {
   const int P2 = 2 * H + 1, P1 = H + 1;
-  for (int e = threadIdx.x; e < H * 2 * H; e += blockDim.x) { int k = e / (2 * H), j = e % (2 * H); wg[k * P2 + j] = Wg[(long long)(H + k) * 2 * H + j]; }
-  for (int e = threadIdx.x; e < H * H; e += blockDim.x) { int k = e / H, j = e % H; wc[k * P1 + j] = Wc[(long long)(H + k) * H + j]; }
+  for (int e = threadIdx.x; e < H * 2 * H; e += blockDim.x) { int k = e / (2 * H), j = e % (2 * H); wg[k * P2 + j] = w.wg[(long long)k * w.ldg + j]; }
+  for (int e = threadIdx.x; e < H * H; e += blockDim.x) { int k = e / H, j = e % H; wc[k * P1 + j] = w.wc[(long long)k * w.ldc + j]; }
 }
 
-// GRUCell (TF 1.15) over whole sequences inside tf.nn.dynamic_rnn.  xg [rows, 2H] holds x W_g[:H] + b_g, xc [rows, H]
-// holds x W_c[:H] + b_c (the input projections of every step, one GEMM each).  Per step t < len(s):
-//   [r|u] = sigmoid(xg + h W_g[H:]),  c = tanh(xc + (r * h) W_c[H:]),  h' = u h + (1 - u) c
+// A GRU over whole sequences: TF 1.15's GRUCell inside tf.nn.dynamic_rnn, or Keras's GRU v1 (reset_after=False),
+// whose recurrence is the same with another gate activation and weight layout (GruRec).  xg [rows, 2H] holds the input
+// projections x W_g + b_g of every step in the gate block's column order, xc [rows, H] holds x W_c + b_c (one GEMM
+// each).  Per step t < len(s):
+//   [r|u] = act(xg + h W_g),  c = tanh(xc + (r * h) W_c),  h' = u h + (1 - u) c
 // hout [rows, H] gets h' (zero for t >= len(s): dynamic_rnn's outputs past the sequence length); with `store`, xg is
 // overwritten by [r|u], xc by c and rh [rows, H] gets r * h (the backward pass's activations).  h0 [S, H] is the
 // initial state (NULL: zeros) and hT [S, H] (may alias h0, or NULL) the state after len(s) steps.
 __global__ void __launch_bounds__(QG_THREADS)
-qmix_gru_fwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, float* xg, float* xc, const float* h0, float* hT,
+qmix_gru_fwd_kernel(GruRec W, float* xg, float* xc, const float* h0, float* hT,
                     float* __restrict__ hout, float* __restrict__ rh, const int32_t* __restrict__ seq_len, int S, int T, int n, int H,
                     int G, int store) {
   extern __shared__ float sm[];
@@ -52,7 +68,8 @@ qmix_gru_fwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
   __shared__ int lens[64];
   pdl_wait(); pdl_trigger();
   const int s0 = blockIdx.x * G, ng = min(G, S - s0);
-  qgru_load_weights(Wg, Wc, H, wg, wc);
+  qgru_load_weights(W, H, wg, wc);
+  const int r_col = W.r_col;
   int tmax = 0;
   for (int g = 0; g < ng; g++) tmax = max(tmax, min(max(seq_len[s0 + g], 0), T));
   if (threadIdx.x < ng) lens[threadIdx.x] = min(max(seq_len[s0 + threadIdx.x], 0), T);
@@ -68,9 +85,10 @@ qmix_gru_fwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
       const float* h = hs + g * H;
       float acc = xg[row * 2 * H + j];
       for (int k = 0; k < H; k++) acc = fmaf(h[k], wg[k * P2 + j], acc);
-      const float v = qsigmoid(acc);
+      const float v = W.hard ? qhard_sigmoid(acc) : qsigmoid(acc);
       if (store) xg[row * 2 * H + j] = v;
-      if (j < H) rs[g * H + j] = v * h[j]; else us[g * H + j - H] = v;
+      const int jr = j - r_col;
+      if (jr >= 0 && jr < H) rs[g * H + jr] = v * h[jr]; else us[g * H + j - (H - r_col)] = v;
     }
     __syncthreads();
     for (int o = threadIdx.x; o < ng * H; o += blockDim.x) {
@@ -95,10 +113,12 @@ qmix_gru_fwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
 }
 
 // Backward of qmix_gru_fwd_kernel (store = 1, h0 = zeros) in reverse time, carrying dh.  dy [rows, H] is d loss / d hout.
-// Writes the gradients wrt the pre-activations of the gates, dag [rows, 2H] ([r|u]), and of the candidate, dac [rows, H]
-// (zero rows for t >= len(s)); the weight gradients and d loss / d x follow as GEMMs over all rows.
+// Writes the gradients wrt the pre-activations of the gates, dag [rows, 2H] (the gate block's column order), and of the
+// candidate, dac [rows, H] (zero rows for t >= len(s)); the weight gradients and d loss / d x follow as GEMMs over all
+// rows.  The gate derivative is taken from the activation: v (1 - v) for sigmoid; 0.2 inside hard_sigmoid's clip and 0
+// where it saturated (TF's clip_by_value gradient, except at a pre-activation within an fp32 rounding of +-2.5).
 __global__ void __launch_bounds__(QG_THREADS)
-qmix_gru_bwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, const float* __restrict__ ru, const float* __restrict__ cc,
+qmix_gru_bwd_kernel(GruRec W, const float* __restrict__ ru, const float* __restrict__ cc,
                     const float* __restrict__ hout, const float* __restrict__ dy, float* __restrict__ dag, float* __restrict__ dac,
                     const int32_t* __restrict__ seq_len, int S, int T, int n, int H, int G) {
   extern __shared__ float sm[];
@@ -106,11 +126,12 @@ qmix_gru_bwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
   float* wc = wg + H * (2 * H + 1);
   float* dh = wc + H * (H + 1);     // [G][H]  carried d loss / d h
   float* dn = dh + G * H;           // [G][H]  d loss / d h_prev, being summed
-  float* ds = dn + G * H;           // [G][3H] [da_r | da_u | da_c] of the current step
+  float* ds = dn + G * H;           // [G][3H] [gate block (da_r, da_u) | da_c] of the current step
   __shared__ int lens[64];
   pdl_wait(); pdl_trigger();
   const int s0 = blockIdx.x * G, ng = min(G, S - s0);
-  qgru_load_weights(Wg, Wc, H, wg, wc);
+  qgru_load_weights(W, H, wg, wc);
+  const int r_col = W.r_col, u_col = H - r_col, hard = W.hard;
   int tmax = 0;
   for (int g = 0; g < ng; g++) tmax = max(tmax, min(max(seq_len[s0 + g], 0), T));
   if (threadIdx.x < ng) lens[threadIdx.x] = min(max(seq_len[s0 + threadIdx.x], 0), T);
@@ -131,12 +152,12 @@ qmix_gru_bwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
       const long long row = row_of(g, t);
       const float hp = t > 0 ? hout[(row - n) * H + j] : 0.f;
       const float d = dy[row * H + j] + dh[o];
-      const float u = ru[row * 2 * H + H + j], c = cc[row * H + j];
-      const float da_u = d * (hp - c) * u * (1.f - u);
+      const float u = ru[row * 2 * H + u_col + j], c = cc[row * H + j];
+      const float da_u = hard ? d * (hp - c) * qhard_sigmoid_grad(u) : d * (hp - c) * u * (1.f - u);
       const float da_c = d * (1.f - u) * (1.f - c * c);
-      ds[g * 3 * H + H + j] = da_u;
+      ds[g * 3 * H + u_col + j] = da_u;
       ds[g * 3 * H + 2 * H + j] = da_c;
-      dag[row * 2 * H + H + j] = da_u;
+      dag[row * 2 * H + u_col + j] = da_u;
       dac[row * H + j] = da_c;
       dn[o] = d * u;
     }
@@ -149,10 +170,10 @@ qmix_gru_bwd_kernel(const float* __restrict__ Wg, const float* __restrict__ Wc, 
       float drh = 0.f;
       for (int j = 0; j < H; j++) drh = fmaf(dc[j], wc[k * P1 + j], drh);
       const float hp = t > 0 ? hout[(row - n) * H + k] : 0.f;
-      const float r = ru[row * 2 * H + k];
-      const float da_r = drh * hp * r * (1.f - r);
-      ds[g * 3 * H + k] = da_r;
-      dag[row * 2 * H + k] = da_r;
+      const float r = ru[row * 2 * H + r_col + k];
+      const float da_r = hard ? drh * hp * qhard_sigmoid_grad(r) : drh * hp * r * (1.f - r);
+      ds[g * 3 * H + r_col + k] = da_r;
+      dag[row * 2 * H + r_col + k] = da_r;
       dn[o] += drh * r;
     }
     __syncthreads();

@@ -20,6 +20,7 @@
 #include "per.cuh"
 #include "qmix.cuh"
 #include "scc.cuh"
+#include "infoflow.cuh"
 #include "stager.cuh"
 #include "bp_gemm.cuh"
 #include "comm.cuh"
@@ -1920,7 +1921,7 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
                 kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
-                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain };
+                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
@@ -2727,6 +2728,9 @@ static int agent_alloc(const char* fn, QmixAgent& a, void** buf, std::vector<Pie
   return carve_scratch(fn, buf, pieces);
 }
 
+// The recurrent halves of GRUCell's gates/kernel wg [2H, 2H] and candidate/kernel wc [2H, H] (see GruRec)
+static GruRec cell_rec(const float* wg, const float* wc, int H) { return GruRec{wg + 2LL * H * H, wc + (long long)H * H, 2 * H, H, 0, 0}; }
+
 // fc1 -> GRU -> fc2 of the weight set P (NULL: the eval set the nets are bound to) over `rows` agent rows holding
 // S = rows / T sequences of T steps; the Q values stay in fc2's output tensor.  h0 / hT: see qmix_gru_fwd_kernel.
 static int qmix_agent_forward(QmixAgent& a, const float* P, const float* obs, int rows, int T, const int32_t* seq_len, const float* h0,
@@ -2745,7 +2749,7 @@ static int qmix_agent_forward(QmixAgent& a, const float* P, const float* obs, in
               false, st);
   LAUNCH_CHECK();
   const int S = rows / T, G = a.G;
-  XLAUNCH(qmix_gru_fwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, wg, wc, a.xg, a.xc, h0, hT, a.hout, a.rh, seq_len, S, T,
+  XLAUNCH(qmix_gru_fwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, cell_rec(wg, wc, H), a.xg, a.xc, h0, hT, a.hout, a.rh, seq_len, S, T,
           a.n, H, G, store);
   LAUNCH_CHECK();
   return net_forward_impl(a.fc2, P ? P + a.o_fc2 : nullptr, a.hout, nullptr, rows, st, 0u, 1u << 1);
@@ -2765,7 +2769,7 @@ static int qmix_agent_backward(QmixAgent& a, const float* obs, const int32_t* se
   float* gg = a.fc1->grads + a.o_gru;
   float* gc = gg + 2 * H * 2 * H + 2 * H;
   const int S = a.S, G = a.G;
-  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, wg, wc, (const float*)a.xg, (const float*)a.xc,
+  XLAUNCH(qmix_gru_bwd_kernel, (S + G - 1) / G, QG_THREADS, a.smem, st, cell_rec(wg, wc, H), (const float*)a.xg, (const float*)a.xc,
           (const float*)a.hout, (const float*)a.dy, a.dag, a.dac, seq_len, S, a.T, a.n, H, G);
   LAUNCH_CHECK();
   const float* x = xtb_net_tensor(a.fc1, 1);
@@ -3151,6 +3155,239 @@ extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* 
     XLAUNCH(scc_value_kernel, (rows + SCC_THREADS / 32 - 1) / (SCC_THREADS / 32), SCC_THREADS, 0, st, scc_nets(q, false),
             (const float*)(q->ag.fc1->params + q->o_head), rows, q->U, q->concat, v_out);
     LAUNCH_CHECK();
+    return XTB_OK;
+  });
+}
+
+// ---- InfoFlow recommender DQN (xt/model/dqn/dqn_rec_model.py, xt/algorithm/dqn/dqn_infoflw_alg.py) -------------------
+// One flat weight buffer [gru | gru_1 | dense | dense_1 | q_value] (TF variable order, every slice 256-byte aligned):
+// each GRU is Keras's kernel [U, 3U], recurrent_kernel [U, 3U] and bias [3U] (gates [z | r | h]), the head (dense,
+// dense_1, q_value) an engine net bound to the slice at head_off, the gradients at the same offsets.  The frozen
+// embedding table lives outside it.  GRU i of S sequences runs on 5 S step rows (row s * 5 + t).  The object's scratch
+// grows with the sequences (transitions, or rows of a predict) and head input rows a call needs; a growth drops the
+// object's graphs.
+struct xtb_infoflow {
+  xtb_infoflow_desc d{};
+  int U = 0, D = 0, Du = 0;
+  int s_cap = 0, r_cap = 0;      // scratch capacity: GRU sequences, head input rows
+  void* buf = nullptr;
+  float *xs[2] = {}, *xg[2] = {}, *xc[2] = {}, *hout[2] = {}, *rh[2] = {}, *hT[2] = {}, *dy[2] = {};
+  float *dag = nullptr, *dac = nullptr, *x = nullptr, *dx = nullptr, *target = nullptr;
+  int32_t *len5 = nullptr, *iota = nullptr;
+};
+
+static long long if_gru_floats(long long U) { return 6 * U * U + 3 * U; }
+
+extern "C" int xtb_infoflow_create(const xtb_infoflow_desc* desc, xtb_infoflow** out) {
+  const char* fn = "xtb_infoflow_create";
+  if (!desc || !out || !desc->table) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  const xtb_infoflow_desc& d = *desc;
+  if (d.user_dim < 1 || d.item_dim < 1 || d.emb_dim < 1 || d.vocab < 1 || d.batch < 1)
+    return fail(XTB_ERR_ARG, "%s: user_dim %d, item_dim %d, emb_dim %d, vocab %d and batch %d must be positive", fn, d.user_dim,
+                d.item_dim, d.emb_dim, d.vocab, d.batch);
+  if (d.last_act < XTB_ACT_NONE || d.last_act > XTB_ACT_GELU) return fail(XTB_ERR_ARG, "%s: last_act %d is not an xtb_act", fn, d.last_act);
+  const long long U = (long long)d.item_dim * d.emb_dim;
+  if (U > 4096 || qgru_smem_floats((int)U, 1) * 4 > kMaxDynSmem)
+    return fail(XTB_ERR_ARG, "%s: item_dim x emb_dim = %lld GRU units: the GRU weights do not fit in shared memory (at most 137)", fn, U);
+  const long long gn = if_gru_floats(U);
+  if (d.gru_off != 0 || d.gru1_off < gn || d.head_off < d.gru1_off + gn || d.gru1_off % 64 || d.head_off % 64)
+    return fail(XTB_ERR_ARG, "%s: the weights must be slices [gru | gru_1 | head] from offset 0, each 64-float aligned", fn);
+  auto* f = new xtb_infoflow();
+  f->d = d; f->U = (int)U; f->Du = d.user_dim * d.emb_dim; f->D = f->Du + 3 * f->U;
+  *out = f;
+  return XTB_OK;
+}
+
+extern "C" void xtb_infoflow_destroy(xtb_infoflow* f) {
+  if (!f) return;
+  drop_graphs_of(f);
+  cudaDeviceSynchronize();
+  cudaFree(f->buf);
+  delete f;
+}
+
+// Scratch for S sequences and `rows` head input rows (grow-only; a growth drops the object's graphs)
+static int if_reserve(const char* fn, xtb_infoflow* f, int S, int rows) {
+  if (S <= f->s_cap && rows <= f->r_cap) return XTB_OK;
+  const int sc = std::max(S, f->s_cap), rc = std::max(rows, f->r_cap);
+  drop_graphs_of(f);
+  CUDA_TRY(cudaDeviceSynchronize());
+  cudaFree(f->buf);
+  f->buf = nullptr; f->s_cap = f->r_cap = 0;
+  // the opt-in is the kernels' and shared with QMIX / SCC: the most any object may use
+  cudaError_t e = cudaFuncSetAttribute(qmix_gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(qmix_gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+  if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  const long long R = 5LL * sc, U = f->U, D = f->D;
+  std::vector<int32_t> len5(sc, IF_HIST), iota(sc + 1LL);
+  for (int i = 0; i <= sc; i++) iota[i] = i;
+  std::vector<Piece> pieces;
+  for (int i = 0; i < 2; i++)
+    pieces.insert(pieces.end(), {{&f->xs[i], R * U}, {&f->xg[i], R * 2 * U}, {&f->xc[i], R * U}, {&f->hout[i], R * U},
+                                 {&f->rh[i], R * U}, {&f->hT[i], sc * U}, {&f->dy[i], R * U}});
+  pieces.insert(pieces.end(), {{&f->dag, R * 2 * U}, {&f->dac, R * U}, {&f->x, (long long)rc * D}, {&f->dx, (long long)sc * D},
+                               {&f->target, (long long)sc}, {&f->len5, (long long)sc, len5.data()},
+                               {&f->iota, sc + 1LL, iota.data()}});
+  if (int r = carve_scratch(fn, &f->buf, pieces)) return r;
+  f->s_cap = sc; f->r_cap = rc;
+  return XTB_OK;
+}
+
+// The head: dense (relu) on the D-wide rows, dense_1 (relu), q_value (1 wide, last_act)
+static int if_head_check(const char* fn, const xtb_infoflow* f, const xtb_net* head) {
+  if (!head) return fail(XTB_ERR_ARG, "%s: null head", fn);
+  if (!head->ws || !head->params || !head->grads) return fail(XTB_ERR_STATE, "%s: head not bound", fn);
+  if (head->L.size() != 3 || !dense_layer(head, 0, 0, XTB_ACT_RELU) || !dense_layer(head, 1, 1, XTB_ACT_RELU) ||
+      !dense_layer(head, 2, 2, f->d.last_act) || head->tsize[0] != f->D || head->tsize[3] != 1 || head->desc.input_u8 ||
+      head->desc.scale != 1.f)
+    return fail(XTB_ERR_ARG, "%s: head must be dense (relu), dense_1 (relu), q_value (1 wide, last_act) on %d-wide float rows", fn, f->D);
+  return XTB_OK;
+}
+
+// GRU i's recurrent weights in place (Keras GRU v1: recurrent_kernel [U, 3U] = [z | r | h], hard_sigmoid gates)
+static GruRec if_rec(const xtb_infoflow* f, const float* W) {
+  const float* rec = W + 3LL * f->U * f->U;
+  return GruRec{rec, rec + 2 * f->U, 3 * f->U, 3 * f->U, f->U, 1};
+}
+
+// GRU kernels' sequences per CTA for S sequences and their shared memory
+static int if_group(int U, int S, size_t* smem) {
+  int g = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
+  while (g > 1 && qgru_smem_floats(U, g) * 4 > kMaxDynSmem) g--;
+  *smem = qgru_smem_floats(U, g) * 4;
+  return g;
+}
+
+// Both GRUs of the weights P over S sequences from the ids click / noclick [S, 5 item_dim]: hT[i] = the last outputs
+// (return_sequences=False); with `store`, the activations of the backward pass
+static int if_grus(xtb_infoflow* f, const float* P, const int32_t* click, const int32_t* noclick, int S, int store, cudaStream_t st) {
+  const int U = f->U, R = 5 * S;
+  const long long n = (long long)R * U;
+  XLAUNCH(infoflow_gather_kernel, (int)std::min<long long>(4 * kSMs, (2 * n + IF_THREADS - 1) / IF_THREADS), IF_THREADS, 0, st, click,
+          noclick, f->d.table, n, f->d.emb_dim, f->xs[0], f->xs[1]);
+  LAUNCH_CHECK();
+  size_t smem = 0;
+  const int g = if_group(U, S, &smem);
+  for (int i = 0; i < 2; i++) {
+    const float* W = P + (i ? f->d.gru1_off : f->d.gru_off);
+    const float* bias = W + 6LL * U * U;
+    // the input projections: x kernel[:, :2U] + bias[:2U] ([z | r]) and x kernel[:, 2U:] + bias[2U:]
+    launch_gemm(ADense<float>{f->xs[i], nullptr, U}, BRowMajor{W, 3 * U}, EpiBiasAct{f->xg[i], bias, 1.f, XTB_ACT_NONE, 2 * U, nullptr, 0},
+                R, 2 * U, U, false, st);
+    LAUNCH_CHECK();
+    launch_gemm(ADense<float>{f->xs[i], nullptr, U}, BRowMajor{W + 2 * U, 3 * U},
+                EpiBiasAct{f->xc[i], bias + 2 * U, 1.f, XTB_ACT_NONE, U, nullptr, 0}, R, U, U, false, st);
+    LAUNCH_CHECK();
+    XLAUNCH(qmix_gru_fwd_kernel, (S + g - 1) / g, QG_THREADS, smem, st, if_rec(f, W), f->xg[i], f->xc[i], (const float*)nullptr, f->hT[i],
+            f->hout[i], f->rh[i], (const int32_t*)f->len5, S, IF_HIST, 1, U, g, store);
+    LAUNCH_CHECK();
+  }
+  return XTB_OK;
+}
+
+// Head input rows into f->x (see infoflow_rows_kernel) and the head's forward over `rows` of them
+static int if_rows_forward(xtb_infoflow* f, xtb_net* head, const int32_t* user, const int32_t* item, const int32_t* off, int B, int rows,
+                           cudaStream_t st) {
+  XLAUNCH(infoflow_rows_kernel, std::min(4 * kSMs, (rows + IF_THREADS / 32 - 1) / (IF_THREADS / 32)), IF_THREADS, 0, st, user, item, off,
+          (const float*)f->hT[0], (const float*)f->hT[1], f->d.table, B, rows, f->d.user_dim, f->d.item_dim, f->d.emb_dim, f->x);
+  LAUNCH_CHECK();
+  return net_forward_impl(head, nullptr, f->x, nullptr, rows, st, 0u, 1u << 3);
+}
+
+static int if_train_launch(xtb_infoflow* f, xtb_net* head, xtb_adam* opt, const xtb_infoflow_batch& b, int cap, float* loss_out,
+                           float* target_out, cudaStream_t st) {
+  const int B = f->d.batch, U = f->U, R = 5 * B;
+  float* P = head->params - f->d.head_off;
+  float* Gr = head->grads - f->d.head_off;
+  // target pass (dqn_infoflw_alg.py:94-153): the online net's Q of every candidate row of the next states, the
+  // next-state GRUs once per transition, then the segmented max and the TD target
+  float* target = target_out ? target_out : f->target;
+  int rc = XTB_OK;
+  if (b.label) {
+    if (target_out) CUDA_TRY(cudaMemcpyAsync(target_out, b.label, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    target = const_cast<float*>(b.label);
+  } else {
+    rc = if_grus(f, P, b.next_click, b.next_noclick, B, 0, st);
+    if (!rc) rc = if_rows_forward(f, head, b.next_user, b.cand_item, b.cand_off, B, cap, st);
+    if (rc) return rc;
+    XLAUNCH(infoflow_td_kernel, (B + IF_THREADS / 32 - 1) / (IF_THREADS / 32), IF_THREADS, 0, st, (const float*)xtb_net_tensor(head, 3),
+            b.cand_off, b.reward, b.done, B, f->d.gamma, target);
+    LAUNCH_CHECK();
+  }
+  // model.fit of the one minibatch: forward, mse (the pre-update loss) and backward
+  rc = if_grus(f, P, b.click, b.noclick, B, 1, st);
+  if (!rc) rc = if_rows_forward(f, head, b.user, b.item, f->iota, B, B, st);
+  if (rc) return rc;
+  const int act = f->d.last_act;
+  XLAUNCH(infoflow_mse_kernel, 1, IF_THREADS, 0, st, (const float*)xtb_net_tensor(head, 3), (const float*)target, B, act,
+          act_is_ext(act) ? 0 : 1, xtb_net_tensor_grad(head, 3), loss_out);
+  LAUNCH_CHECK();
+  const int32_t qh[1] = {3};
+  BackwardOpts o(qh, 1);
+  o.heads_dy = 1u << 3;
+  o.dobs = f->dx;
+  rc = net_backward_impl(head, f->x, nullptr, B, st, o);
+  if (rc) return rc;
+  // the GRUs from the h_click / h_noclick slices of d loss / d input (the embedding is frozen: nothing flows further)
+  size_t smem = 0;
+  const int g = if_group(U, B, &smem);
+  for (int i = 0; i < 2; i++) {
+    CUDA_TRY(cudaMemcpy2DAsync(f->dy[i] + (IF_HIST - 1) * U, (size_t)IF_HIST * U * sizeof(float), f->dx + f->Du + i * U,
+                               (size_t)f->D * sizeof(float), (size_t)U * sizeof(float), B, cudaMemcpyDeviceToDevice, st));
+    const long long o_w = i ? f->d.gru1_off : f->d.gru_off;
+    XLAUNCH(qmix_gru_bwd_kernel, (B + g - 1) / g, QG_THREADS, smem, st, if_rec(f, P + o_w), (const float*)f->xg[i], (const float*)f->xc[i],
+            (const float*)f->hout[i], (const float*)f->dy[i], f->dag, f->dac, (const int32_t*)f->len5, B, IF_HIST, 1, U, g);
+    LAUNCH_CHECK();
+    // [kernel; recurrent_kernel; bias] gradients, [3U] columns apart: [x | h_prev | 1]^T d[z|r] into columns [0, 2U) and
+    // [x | r h_prev | 1]^T d h^ into columns [2U, 3U)
+    float* gw = Gr + o_w;
+    launch_gemm(AGruFeat{f->xs[i], f->hout[i], U, 1, IF_HIST, 1}, BRowMajor{f->dag, 2 * U}, EpiDgrad{gw, gw, 0, 3 * U, 0, nullptr, 0},
+                2 * U + 1, 2 * U, R, false, st);
+    LAUNCH_CHECK();
+    launch_gemm(AGruFeat{f->xs[i], f->rh[i], U, 1, IF_HIST, 0}, BRowMajor{f->dac, U}, EpiDgrad{gw + 2 * U, gw + 2 * U, 0, 3 * U, 0, nullptr, 0},
+                2 * U + 1, U, R, false, st);
+    LAUNCH_CHECK();
+  }
+  // Keras Adam over [gru | gru_1 | head], then the head's weight blobs
+  rc = adam_step_impl(opt, P, Gr, 1.f, st, nullptr);
+  if (!rc) rc = xtb_net_sync_weights(head, st);
+  return rc;
+}
+
+extern "C" int xtb_infoflow_train(xtb_infoflow* f, xtb_net* head, xtb_adam* opt, const xtb_infoflow_batch* batch, float* loss_out,
+                                  float* target_out, int use_graph, void* stream) {
+  const char* fn = "xtb_infoflow_train";
+  if (!f) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (int rc = if_head_check(fn, f, head)) return rc;
+  const bool missing = !opt || !batch || !loss_out || !batch->user || !batch->click || !batch->noclick || !batch->item ||
+                       (!batch->label && (!batch->next_user || !batch->next_click || !batch->next_noclick || !batch->cand_off ||
+                                          !batch->cand_item || !batch->reward || !batch->done));
+  const int B = f->d.batch;
+  if (int rc = learner_check(fn, missing, head, opt, B, false, 0, f->d.head_off + head->n_params)) return rc;
+  const xtb_infoflow_batch b = *batch;
+  if (b.n_cand < 0 || b.cand_cap < std::max(b.n_cand, B) || b.cand_cap > head->max_batch)
+    return fail(XTB_ERR_ARG, "%s: cand_cap %d must hold n_cand %d and the batch %d, and the head %d rows", fn, b.cand_cap, b.n_cand, B,
+                head->max_batch);
+  if (int rc = if_reserve(fn, f, B, b.cand_cap)) return rc;
+  return run_graph(capture_key(kInfoflowTrain, {head, f, opt}, f, b.user, b.click, b.noclick, b.item, b.next_user, b.next_click,
+                               b.next_noclick, b.cand_off, b.cand_item, b.reward, b.done, b.label, b.cand_cap, loss_out, target_out),
+                   use_graph, stream, [&](void* st) { return if_train_launch(f, head, opt, b, b.cand_cap, loss_out, target_out, S(st)); });
+}
+
+extern "C" int xtb_infoflow_predict(xtb_infoflow* f, xtb_net* head, const int32_t* user, const int32_t* click, const int32_t* noclick,
+                                    const int32_t* item, int n, float* q_out, int use_graph, void* stream) {
+  const char* fn = "xtb_infoflow_predict";
+  if (!f) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  if (int rc = if_head_check(fn, f, head)) return rc;
+  if (int rc = learner_check(fn, !user || !click || !noclick || !item || !q_out, head, nullptr, n, true)) return rc;
+  if (int rc = if_reserve(fn, f, n, n)) return rc;
+  return run_graph(capture_key(kInfoflowPredict, {head, f}, f, user, click, noclick, item, n, q_out), use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    const float* P = head->params - f->d.head_off;
+    int rc = if_grus(f, P, click, noclick, n, 0, st);
+    if (!rc) rc = if_rows_forward(f, head, user, item, f->iota, n, n, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(q_out, xtb_net_tensor(head, 3), (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
     return XTB_OK;
   });
 }

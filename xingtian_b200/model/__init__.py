@@ -8,3 +8,4 @@ from .impala_cnn import ImpalaCnn  # noqa: F401
 from .muzero import MuzeroCnn, MuzeroMlp, MuzeroModel  # noqa: F401
 from .qmix import QMixModel  # noqa: F401
 from .scc import SCCModel  # noqa: F401
+from .dqn_infoflow import DqnInfoFlowModel  # noqa: F401
