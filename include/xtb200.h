@@ -541,6 +541,84 @@ void xtb_muzero_tree_destroy(xtb_muzero_tree* tree);
 int xtb_muzero_search(xtb_muzero* mz, xtb_muzero_tree* tree, const void* obs, int n_envs, int num_simulations,
                       const double* noise, double pb_c_base, double pb_c_init, double discount, double exploration_frac,
                       int32_t* visit_counts_out, double* root_value_out, int use_graph, void* stream);
+
+/* ---- MuZero trajectory replay on the device: the Muzero learner's buffer (xt/algorithm/muzero/muzero.py over
+ *      prioritized_replay_buffer_muzero.py) with its rules and float64 arithmetic, kept in HBM ----------------------------
+ * Storage: a pool of pool_steps steps (observation rows of obs_bytes as the representation net reads them, actions
+ *   int32, target values float64, rewards float32, child visits [A] float32) and `capacity` trajectory slots.  Slot s
+ *   holds the trajectory at pool [off, off + len); the caller places trajectories (xtb_muzero_replay_add), evicting the
+ *   oldest when a new one does not fit.  An evicted slot keeps its place in count, its leaf is 0 and stays 0.
+ * Trees, float64, every internal node left + right of its final children:
+ *   trajectory tree: leaf s = the weight of slot s's position tree (its root / (len - K)), capacity rounded up to a
+ *     power of two; position tree of a slot: leaf i < len - K = |value_i - target_value_i|, capacity = len rounded up.
+ * Draw of B samples from uniforms u [2B] (float64, the host's random.random() calls in its order):
+ *   trajectory k: mass = u[k] step + k step, step = reduce(0, count - 1) / B, where reduce(0, n - 1) sums leaves
+ *     0 .. n - 2 in the order of the host segment tree's midpoint recursion (its exclusive end); the descent takes the
+ *     first leaf whose running sum exceeds the mass, with the host's subtractions.  A descent that ends on a slot
+ *     without a live trajectory (evicted, or past count through rounding) takes the nearest live slot below it,
+ *     wrapping from slot 0 to count - 1, and sets XTB_MZR_REMAPPED;
+ *   its position: mass = u[B + k] total + 0 total in that slot's tree, total = reduce(0, len - K - 1), clamped to
+ *     len - K - 1.
+ * Update from post-step values v [B]: new_pri_k = max(|v_k - target_value[pos_k]|, 1e-5) (NaN stays NaN); in batch
+ *   order k, position leaf pos_k of slot_k takes new_pri_k, then trajectory leaf k (the batch position, the reference's
+ *   rule) takes slot_k's weight at that moment unless slot k holds no live trajectory.  The sequence stops before the
+ *   first entry whose priority is not > 0 (XTB_MZR_BAD_PRIORITY) or that names no live slot, a position outside it or
+ *   a batch position k >= count (XTB_MZR_BAD_INDEX).
+ * The masses are formed as the host forms them: both products rounded, then the sum (no fused multiply-add).
+ * Every value that changes from call to call (count, the slot table, both tree levels, the status) is on the device,
+ * so one captured xtb_muzero_replay_train graph serves the run while the ring fills and wraps.
+ * xtb_muzero_replay_add / _sample / _update / _train return XTB_ERR_STATE, launching nothing, while a communicator is
+ * installed (create and the read-only state snapshot do not train and are allowed). */
+typedef struct xtb_muzero_replay xtb_muzero_replay;
+typedef struct xtb_muzero_replay_slot {
+  int64_t off;      /* first pool step */
+  int32_t len;      /* steps */
+  int32_t live;     /* 1: holds its trajectory; 0: empty or evicted */
+} xtb_muzero_replay_slot;
+/* The minibatch a draw gathers (device arrays of B rows), laid out as xtb_muzero_batch reads it. */
+typedef struct xtb_muzero_replay_batch {
+  void* obs;                /* [B, obs_bytes] */
+  int32_t* action;          /* [B, unroll] */
+  float* target_value;      /* [B, unroll + 1] */
+  float* target_reward;     /* [B, unroll + 1] */
+  float* target_policy;     /* [B, unroll + 1, A] */
+} xtb_muzero_replay_batch;
+#define XTB_MZR_BAD_PRIORITY 1   /* status: an update met a priority that is not > 0; it and the entries after it were not applied */
+#define XTB_MZR_REMAPPED 2       /* status: a draw's descent ended on a slot without a live trajectory */
+#define XTB_MZR_BAD_INDEX 4      /* status: an update named no live slot, a position outside it or a batch position past
+                                    count; not applied from there */
+/* capacity (BUFFER_SIZE) >= 1, pool_steps >= 1, unroll K >= 1, obs_bytes >= 1, n_actions A in [1, 1024], max_batch >= 1:
+ * the largest B of a draw. */
+int xtb_muzero_replay_create(int capacity, long long pool_steps, int unroll, long long obs_bytes, int n_actions, int max_batch,
+                             xtb_muzero_replay** out);
+void xtb_muzero_replay_destroy(xtb_muzero_replay* r);
+/* Store one trajectory of len steps (K + 1 < len <= pool_steps) from device arrays obs [len, obs_bytes], action [len],
+ * target_value [len] (float64), reward [len], child_visits [len, A] at slot `slot` and pool [off, off + len), after
+ * evicting slots [evict_first, evict_first + n_evict) mod capacity (which must not include `slot`).  values [len]
+ * (float64) gives the values of the position priorities; NULL: xtb_muzero_initial_inference of mz on the stored pool
+ * rows, max_batch rows per forward as the host's value_inference. */
+int xtb_muzero_replay_add(xtb_muzero_replay* r, xtb_muzero* mz, int slot, long long off, int evict_first, int n_evict,
+                          const void* obs, const int32_t* action, const double* target_value, const float* reward,
+                          const float* child_visits, int len, const double* values, void* stream);
+/* The draw of B in [1, max_batch] samples from uniforms [2B] into slot_out [B] / pos_out [B] (int32) and the gathered
+ * batch.  Resets the status to this draw's bits.  XTB_ERR_STATE when nothing is stored. */
+int xtb_muzero_replay_sample(xtb_muzero_replay* r, int batch, const double* uniforms, int32_t* slot_out, int32_t* pos_out,
+                             const xtb_muzero_replay_batch* out, void* stream);
+/* The update of B entries (slot [B], pos [B] from a draw) from values [B] float64.  B in [1, min(max_batch, count)]:
+ * batch position B - 1 must be a stored slot, as the host's update requires (XTB_ERR_ARG otherwise). */
+int xtb_muzero_replay_update(xtb_muzero_replay* r, int batch, const int32_t* slot, const int32_t* pos, const double* values,
+                             void* stream);
+/* One learner step: xtb_muzero_replay_sample, xtb_muzero_train of mz / opt on the gathered batch (loss_offset,
+ * *loss_out) with the post-update values, xtb_muzero_replay_update from them, and a copy of the status into
+ * *status_out (device int32).  B in [1, min(max_batch, count)], as for the update. */
+int xtb_muzero_replay_train(xtb_muzero_replay* r, xtb_muzero* mz, xtb_adam* opt, int batch, const double* uniforms,
+                            int32_t* slot_out, int32_t* pos_out, const xtb_muzero_replay_batch* out, float loss_offset,
+                            float* loss_out, int32_t* status_out, int use_graph, void* stream);
+/* Read-only snapshot after a device synchronise; any output may be NULL.  slots [capacity]; traj_tree [2 tree_leaves]
+ * heap order; forest [4 pool_steps]: slot s's position tree is the 2 cap doubles at forest + 4 off. */
+int xtb_muzero_replay_state(const xtb_muzero_replay* r, int* count, int* status, int* tree_leaves,
+                            xtb_muzero_replay_slot* slots, double* traj_tree, double* forest);
+
 /* ---- QMIX: replaces QMixModel's train and explore graphs (xt/model/qmix/qmix_tf.py:172-589) -------------------------
  * One weight set is a flat float buffer [fc1 | GRU | fc2 | mixer]: fc1 = dense(H, relu) on the agent inputs (net `fc1`,
  * obs_dim wide), the GRUCell's rnn/gru_cell/gates/kernel [2H, 2H], gates/bias [2H], candidate/kernel [2H, H] and

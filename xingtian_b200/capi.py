@@ -16,6 +16,7 @@ ACT = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "sigmoid": 3, "softsign": 4, 
        "selu": 8, "swish": 9, "gelu": 10}
 CLIP_NONE, CLIP_GLOBAL_NORM, CLIP_PER_TENSOR = 0, 1, 2
 PER_NONFINITE, PER_BAD_INDEX, PER_EMPTY = 1, 2, 4     # xtb_per status bits
+MZR_BAD_PRIORITY, MZR_REMAPPED, MZR_BAD_INDEX = 1, 2, 4   # xtb_muzero_replay status bits
 
 
 class LayerDesc(C.Structure):
@@ -58,6 +59,15 @@ class MuzeroDesc(C.Structure):
 class MuzeroBatch(C.Structure):
     _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("target_value", C.c_void_p), ("target_reward", C.c_void_p),
                 ("target_policy", C.c_void_p), ("unroll", C.c_int32)]
+
+
+class MuzeroReplaySlot(C.Structure):
+    _fields_ = [("off", C.c_int64), ("len", C.c_int32), ("live", C.c_int32)]
+
+
+class MuzeroReplayBatch(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("target_value", C.c_void_p), ("target_reward", C.c_void_p),
+                ("target_policy", C.c_void_p)]
 
 
 class QmixDesc(C.Structure):
@@ -178,6 +188,14 @@ _SIGS = {
     "xtb_muzero_tree_destroy": (None, [_P]),
     "xtb_muzero_search": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, _P, _P,
                                     C.c_int, _P]),
+    "xtb_muzero_replay_create": (C.c_int, [C.c_int, C.c_longlong, C.c_int, C.c_longlong, C.c_int, C.c_int, C.POINTER(_P)]),
+    "xtb_muzero_replay_destroy": (None, [_P]),
+    "xtb_muzero_replay_add": (C.c_int, [_P, _P, C.c_int, C.c_longlong, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P, _P]),
+    "xtb_muzero_replay_sample": (C.c_int, [_P, C.c_int, _P, _P, _P, C.POINTER(MuzeroReplayBatch), _P]),
+    "xtb_muzero_replay_update": (C.c_int, [_P, C.c_int, _P, _P, _P, _P]),
+    "xtb_muzero_replay_train": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.POINTER(MuzeroReplayBatch), C.c_float, _P, _P,
+                                          C.c_int, _P]),
+    "xtb_muzero_replay_state": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P]),
     "xtb_qmix_create": (C.c_int, [_P, _P, _P, C.POINTER(QmixDesc), C.POINTER(_P)]),
     "xtb_qmix_destroy": (None, [_P]),
     "xtb_qmix_train": (C.c_int, [_P, _P, _P, C.POINTER(QmixBatch), _P, C.c_int, _P]),

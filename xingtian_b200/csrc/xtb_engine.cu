@@ -18,6 +18,7 @@
 #include "optim.cuh"
 #include "rl_kernels.cuh"
 #include "per.cuh"
+#include "muzero_replay.cuh"
 #include "qmix.cuh"
 #include "scc.cuh"
 #include "infoflow.cuh"
@@ -1921,10 +1922,10 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
                 kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
-                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict };
+                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict, kMuzeroReplayTrain };
 struct CaptureKey {
   uint64_t tag;          // entry point
-  const void* own[6];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[5]):
+  const void* own[7];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[6]):
                          // destroying one, or rebinding a net, drops the graph
   uint64_t mode[2];      // kernel-path and fused-heads modes
   uint64_t arg[21];      // every pointer and scalar argument; floats by bit pattern
@@ -1970,7 +1971,7 @@ static void drop_graphs_of(const void* obj) {
 template <class F>
 static int run_graph(CaptureKey key, int use_graph, void* stream, F&& launch) {
   if (!use_graph) return launch(stream);
-  key.own[5] = g_comm; key.mode[0] = g_tc_mode; key.mode[1] = g_fuse_heads;
+  key.own[6] = g_comm; key.mode[0] = g_tc_mode; key.mode[1] = g_fuse_heads;
   StreamScope sc;
   int src = sc.begin(stream, true);
   if (src) return src;
@@ -2651,6 +2652,188 @@ extern "C" int xtb_muzero_train(xtb_muzero* m, xtb_adam* opt, const xtb_muzero_b
   return run_graph(capture_key(kMuzeroTrain, {m->rep, m->dyn, m->pred, m, opt}, m, bt.obs, bt.action, bt.target_value,
                                bt.target_reward, bt.target_policy, batch, loss_offset, loss_out, value_out),
                    use_graph, stream, [&](void* st) { return mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, value_out, S(st)); });
+}
+
+// ---- MuZero trajectory replay (muzero_replay.cuh) ---------------------------------------------------------------------
+// The pool, the slot table, both tree levels and the state are one device allocation; `count` mirrors the device's so
+// that a draw from an empty buffer is refused before a launch.
+struct xtb_muzero_replay {
+  MzrDev d{};
+  int capacity = 0, max_batch = 0, count = 0;
+  long long pool = 0;
+  void* buf = nullptr;
+  float* vbuf = nullptr;       // [max(pool, max_batch)] float values: value inference of an add, post-step values of a train
+};
+
+extern "C" int xtb_muzero_replay_create(int capacity, long long pool_steps, int unroll, long long obs_bytes, int n_actions,
+                                        int max_batch, xtb_muzero_replay** out) {
+  const char* fn = "xtb_muzero_replay_create";
+  if (!out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (capacity < 1 || capacity > (1 << 30) || pool_steps < 1 || pool_steps > (1LL << 36) || unroll < 1 || obs_bytes < 1 ||
+      n_actions < 1 || n_actions > MZ_MAX_SUPPORT || max_batch < 1)
+    return fail(XTB_ERR_ARG, "%s: capacity %d / pool_steps %lld / unroll %d / obs_bytes %lld / actions %d / max_batch %d out of range",
+                fn, capacity, pool_steps, unroll, obs_bytes, n_actions, max_batch);
+  auto* r = new xtb_muzero_replay();
+  MzrDev& d = r->d;
+  d.tleaves = 1;
+  while (d.tleaves < capacity) d.tleaves *= 2;
+  d.row_bytes = obs_bytes; d.K = unroll; d.A = n_actions;
+  const long long P = pool_steps;
+  if (int rc = carve_scratch(fn, &r->buf, {{&d.obs, P * obs_bytes}, {&d.action, P}, {&d.tv, P}, {&d.reward, P},
+                                           {&d.child, P * n_actions}, {&d.traj, 2LL * d.tleaves}, {&d.forest, 4 * P},
+                                           {&d.slot, (long long)capacity}, {&d.st, 1}, {&d.wt, (long long)max_batch},
+                                           {&r->vbuf, std::max<long long>(P, max_batch)}})) {
+    delete r;
+    return rc;
+  }
+  r->capacity = capacity; r->pool = P; r->max_batch = max_batch;
+  *out = r;
+  return XTB_OK;
+}
+
+extern "C" void xtb_muzero_replay_destroy(xtb_muzero_replay* r) {
+  if (!r) return;
+  drop_graphs_of(r);
+  cudaDeviceSynchronize();
+  cudaFree(r->buf);
+  delete r;
+}
+
+static int mzr_check(const char* fn, const xtb_muzero_replay* r, bool missing) {
+  if (!r || missing) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
+  return XTB_OK;
+}
+// the model reads the replay's observation rows, actions and unroll
+static int mzr_model_check(const char* fn, const xtb_muzero_replay* r, const xtb_muzero* m) {
+  const long long row = (long long)m->rep->tsize[0] * (m->rep->desc.input_u8 ? 1 : (long long)sizeof(float));
+  if (m->K != r->d.K || m->A != r->d.A || row != r->d.row_bytes)
+    return fail(XTB_ERR_ARG, "%s: model (unroll %d, %d actions, %lld-byte observations) does not match the replay (%d, %d, %lld)", fn,
+                m->K, m->A, row, r->d.K, r->d.A, r->d.row_bytes);
+  return XTB_OK;
+}
+static int mzr_batch_check(const char* fn, const xtb_muzero_replay* r, int batch, const xtb_muzero_replay_batch* out) {
+  if (!out || !out->obs || !out->action || !out->target_value || !out->target_reward || !out->target_policy)
+    return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (batch < 1 || batch > r->max_batch) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d]", fn, batch, r->max_batch);
+  if (r->count < 1) return fail(XTB_ERR_STATE, "%s: no trajectory stored", fn);
+  return XTB_OK;
+}
+// an update writes trajectory leaf k for every batch position k: each must be a stored slot, as the host's
+// update_priorities requires
+static int mzr_update_batch_check(const char* fn, const xtb_muzero_replay* r, int batch) {
+  if (batch < 1 || batch > r->max_batch) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d]", fn, batch, r->max_batch);
+  if (batch > r->count) return fail(XTB_ERR_ARG, "%s: batch %d exceeds the %d stored slots", fn, batch, r->count);
+  return XTB_OK;
+}
+
+static int mzr_sample_launch(xtb_muzero_replay* r, int B, const double* u, int32_t* slot, int32_t* pos, const xtb_muzero_replay_batch& o,
+                             cudaStream_t st) {
+  XLAUNCH(mzr_draw_kernel, 1, std::min(kMzrThreads, (B + 31) / 32 * 32), 0, st, r->d, B, u, slot, pos);
+  LAUNCH_CHECK();
+  XLAUNCH(mzr_gather_kernel, B, 256, 0, st, r->d, (const int32_t*)slot, (const int32_t*)pos, (uint8_t*)o.obs, o.action, o.target_value,
+          o.target_reward, o.target_policy);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+static int mzr_update_launch(xtb_muzero_replay* r, int B, const int32_t* slot, const int32_t* pos, const float* vf, const double* vd,
+                             cudaStream_t st) {
+  XLAUNCH(mzr_update_kernel, 1, kMzrThreads, 0, st, r->d, B, slot, pos, vf, vd);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+extern "C" int xtb_muzero_replay_add(xtb_muzero_replay* r, xtb_muzero* m, int slot, long long off, int evict_first, int n_evict,
+                                     const void* obs, const int32_t* action, const double* target_value, const float* reward,
+                                     const float* child_visits, int len, const double* values, void* stream) {
+  const char* fn = "xtb_muzero_replay_add";
+  if (int rc = mzr_check(fn, r, !obs || !action || !target_value || !reward || !child_visits || (!values && !m))) return rc;
+  const MzrDev& d = r->d;
+  if (len <= d.K + 1 || len > r->pool) return fail(XTB_ERR_ARG, "%s: length %d not in [%d, %lld]", fn, len, d.K + 2, r->pool);
+  if (slot < 0 || slot >= r->capacity || off < 0 || off + len > r->pool)
+    return fail(XTB_ERR_ARG, "%s: slot %d / pool range [%lld, %lld) outside the replay", fn, slot, off, off + len);
+  if (evict_first < 0 || evict_first >= r->capacity || n_evict < 0 || n_evict >= r->capacity ||
+      (slot - evict_first + r->capacity) % r->capacity < n_evict)
+    return fail(XTB_ERR_ARG, "%s: eviction range %d + %d is not a set of other slots", fn, evict_first, n_evict);
+  if (!values) {
+    if (int rc = mz_check(fn, m, false, nullptr, 1)) return rc;
+    if (int rc = mzr_model_check(fn, r, m)) return rc;
+  }
+  cudaStream_t st = S(stream);
+  CUDA_TRY(cudaMemcpyAsync(d.obs + off * d.row_bytes, obs, (size_t)len * d.row_bytes, cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d.action + off, action, (size_t)len * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d.tv + off, target_value, (size_t)len * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d.reward + off, reward, (size_t)len * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d.child + off * d.A, child_visits, (size_t)len * d.A * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (!values) {
+    for (int s0 = 0; s0 < len; s0 += m->max_batch) {
+      const int n = std::min(m->max_batch, len - s0);
+      int rc = mz_initial_launch(m, d.obs + (off + s0) * d.row_bytes, n, nullptr, r->vbuf + s0, nullptr, st);
+      if (rc) return rc;
+    }
+  }
+  XLAUNCH(mzr_add_kernel, 1, kMzrThreads, 0, st, r->d, slot, off, len, evict_first, n_evict, r->capacity,
+          values ? (const float*)nullptr : (const float*)r->vbuf, values);
+  LAUNCH_CHECK();
+  r->count = std::max(r->count, slot + 1);
+  return XTB_OK;
+}
+
+extern "C" int xtb_muzero_replay_sample(xtb_muzero_replay* r, int batch, const double* uniforms, int32_t* slot_out, int32_t* pos_out,
+                                        const xtb_muzero_replay_batch* out, void* stream) {
+  const char* fn = "xtb_muzero_replay_sample";
+  if (int rc = mzr_check(fn, r, !uniforms || !slot_out || !pos_out)) return rc;
+  if (int rc = mzr_batch_check(fn, r, batch, out)) return rc;
+  return mzr_sample_launch(r, batch, uniforms, slot_out, pos_out, *out, S(stream));
+}
+
+extern "C" int xtb_muzero_replay_update(xtb_muzero_replay* r, int batch, const int32_t* slot, const int32_t* pos, const double* values,
+                                        void* stream) {
+  const char* fn = "xtb_muzero_replay_update";
+  if (int rc = mzr_check(fn, r, !slot || !pos || !values)) return rc;
+  if (int rc = mzr_update_batch_check(fn, r, batch)) return rc;
+  return mzr_update_launch(r, batch, slot, pos, nullptr, values, S(stream));
+}
+
+extern "C" int xtb_muzero_replay_train(xtb_muzero_replay* r, xtb_muzero* m, xtb_adam* opt, int batch, const double* uniforms,
+                                       int32_t* slot_out, int32_t* pos_out, const xtb_muzero_replay_batch* out, float loss_offset,
+                                       float* loss_out, int32_t* status_out, int use_graph, void* stream) {
+  const char* fn = "xtb_muzero_replay_train";
+  if (int rc = mzr_check(fn, r, !uniforms || !slot_out || !pos_out || !loss_out || !status_out)) return rc;
+  if (int rc = mz_check(fn, m, !opt, opt, batch)) return rc;
+  if (int rc = mzr_batch_check(fn, r, batch, out)) return rc;
+  if (int rc = mzr_update_batch_check(fn, r, batch)) return rc;
+  if (int rc = mzr_model_check(fn, r, m)) return rc;
+  const xtb_muzero_replay_batch o = *out;
+  return run_graph(capture_key(kMuzeroReplayTrain, {m->rep, m->dyn, m->pred, m, opt, r}, r, m, batch, uniforms, slot_out, pos_out,
+                               o.obs, o.action, o.target_value, o.target_reward, o.target_policy, loss_offset, loss_out, status_out),
+                   use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    int rc = mzr_sample_launch(r, batch, uniforms, slot_out, pos_out, o, st);
+    if (rc) return rc;
+    xtb_muzero_batch bt{o.obs, o.action, o.target_value, o.target_reward, o.target_policy, m->K};
+    rc = mz_train_launch(m, opt, bt, batch, loss_offset, loss_out, r->vbuf, st);
+    if (rc) return rc;
+    rc = mzr_update_launch(r, batch, slot_out, pos_out, r->vbuf, nullptr, st);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(status_out, &r->d.st->status, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    return XTB_OK;
+  });
+}
+
+extern "C" int xtb_muzero_replay_state(const xtb_muzero_replay* r, int* count, int* status, int* tree_leaves,
+                                       xtb_muzero_replay_slot* slots, double* traj_tree, double* forest) {
+  if (!r) return fail(XTB_ERR_ARG, "xtb_muzero_replay_state: null pointer");
+  CUDA_TRY(cudaDeviceSynchronize());
+  MzrState s;
+  CUDA_TRY(cudaMemcpy(&s, r->d.st, sizeof s, cudaMemcpyDeviceToHost));
+  if (slots) CUDA_TRY(cudaMemcpy(slots, r->d.slot, sizeof(xtb_muzero_replay_slot) * r->capacity, cudaMemcpyDeviceToHost));
+  if (traj_tree) CUDA_TRY(cudaMemcpy(traj_tree, r->d.traj, sizeof(double) * 2 * r->d.tleaves, cudaMemcpyDeviceToHost));
+  if (forest) CUDA_TRY(cudaMemcpy(forest, r->d.forest, sizeof(double) * 4 * r->pool, cudaMemcpyDeviceToHost));
+  if (count) *count = s.count;
+  if (status) *status = s.status;
+  if (tree_leaves) *tree_leaves = r->d.tleaves;
+  return XTB_OK;
 }
 
 // ---- The recurrent agent of QMIX and SCC (xt/model/qmix/qmix_tf.py: fc1 -> GRU -> fc2) --------------------------------
