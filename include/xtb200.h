@@ -735,6 +735,61 @@ int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hid
 /* SCCModel.get_mixer_output (scc_tf.py:500-503): v_out[r] = V_eval(states[r]) for states [rows, n_agents D], rows <= B L. */
 int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream);
 
+/* ---- QMIX / SCC episode replay in HBM: QMixAlg's ReplayBuffer (xt/algorithm/qmix/episode_buffer_np.py) and the batch
+ * assembly of QMixAlg.train (qmix_alg.py: build_inputs, the mask, max_t_filled) ------------------------------------------
+ * One device allocation holds `capacity` episode rows of T = episode_limit + 1 steps.  A row is, in this order, each field
+ * starting at a multiple of 16 bytes:
+ *   state f32 [T, state_dim] | obs f32 [T, n_agents, obs_dim] | actions i32 [T, n_agents] |
+ *   actions_onehot f32 [T, n_agents, A] | avail_actions i32 [T, n_agents, A] | reward f32 [T] | terminated u8 [T] |
+ *   filled i64 [T]
+ * The caller packs a row on the host and stores it with xtb_episode_replay_add; the ring bookkeeping (which slot,
+ * how many are stored) is the caller's, as in ReplayBuffer.insert_episode_batch, and the library mirrors the stored count
+ * (the highest slot written + 1).  The draws are the caller's too: each call below takes B host episode ids, each in
+ * [0, stored count), with 1 <= B <= stored count.  It copies them into the replay's id buffer with one staged upload and
+ * then reads them on the device, so one captured graph serves every draw, every episode length and the whole fill and
+ * wrap of the ring.
+ * Limits (XTB_ERR_ARG at create): capacity >= 1, episode_limit >= 1, 1 <= n_agents <= 32, 1 <= n_actions <= 255,
+ * obs_dim >= 0, state_dim >= 1.  Add, gather and the train calls return XTB_ERR_STATE, launching nothing, while a
+ * communicator is installed, and XTB_ERR_ARG, launching nothing, for a bad slot, row size, batch or id. */
+typedef struct xtb_episode_replay xtb_episode_replay;
+/* A drawn batch (device arrays; any may be NULL, and is then not written). */
+typedef struct xtb_episode_batch {
+  float* obs;           /* [B, L+1, n_agents, obs_dim (+ A) (+ n_agents)] agent inputs: obs | one-hot of the previous step's
+                           action (zeros at t = 0), with obs_last_action | one-hot of the agent id, with obs_agent_id */
+  float* raw_obs;       /* [B, L+1, n_agents, obs_dim] the stored observations */
+  int32_t* seq_len;     /* [B n_agents] max_t_filled(): the largest per-episode sum of filled, for every sequence */
+  float* avail;         /* [B, L+1, n_agents, A] */
+  int32_t* actions;     /* [B, L, n_agents] */
+  float* state;         /* [B, L, state_dim] state[:, :-1] */
+  float* next_state;    /* [B, L, state_dim] state[:, 1:] */
+  float* reward;        /* [B, L] */
+  float* terminated;    /* [B, L] */
+  float* mask;          /* [B, L] filled[:, :-1] with mask[:, 1:] *= 1 - terminated[:, :-1], in float32 */
+} xtb_episode_batch;
+/* obs_last_action / obs_agent_id: build_inputs' switches (0 or 1). */
+int xtb_episode_replay_create(int capacity, int episode_limit, int n_agents, int n_actions, int obs_dim, int state_dim,
+                              int obs_last_action, int obs_agent_id, xtb_episode_replay** out);
+void xtb_episode_replay_destroy(xtb_episode_replay* r);
+/* Bytes of one packed episode row. */
+long long xtb_episode_replay_row_bytes(const xtb_episode_replay* r);
+/* Store the packed row at host `row` (`bytes` must be the row size) in slot `slot` with one staged upload.  Every action
+ * of the first episode_limit steps must be in [0, A) and the sum of filled in [0, L+1] (XTB_ERR_ARG otherwise): the
+ * batch reads them as indices and sequence lengths. */
+int xtb_episode_replay_add(xtb_episode_replay* r, int slot, const void* row, long long bytes, void* stream);
+/* The batch of the B episodes `ids` (host) into *out; *max_t_out (device, may be NULL) = max_t_filled(). */
+int xtb_episode_replay_gather(xtb_episode_replay* r, int batch, const int32_t* ids, const xtb_episode_batch* out, int32_t* max_t_out,
+                              void* stream);
+/* QMixAlg.train on the device: the gather into *batch, then xtb_qmix_train of q / opt / target on it, as one call (one
+ * graph when use_graph).  B must be q's batch and the replay's shapes q's (agent input width, n_agents, A, L, state_dim).
+ * *loss_out as xtb_qmix_train; *max_t_out (device) = max_t_filled(). */
+int xtb_qmix_replay_train(xtb_episode_replay* r, xtb_qmix* q, xtb_adam* opt, const float* target, int batch, const int32_t* ids,
+                          const xtb_qmix_batch* bufs, float* loss_out, int32_t* max_t_out, int use_graph, void* stream);
+/* SCCAlg.train on the device: as xtb_qmix_replay_train with xtb_scc_train; the raw obs comes from the ring (obs_dim must
+ * be q's o).  bufs->subsets is the caller's, as for xtb_scc_train. */
+int xtb_scc_replay_train(xtb_episode_replay* r, xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const float* target, int batch,
+                         const int32_t* ids, const xtb_scc_batch* bufs, float* loss_out, int32_t* max_t_out, int use_graph,
+                         void* stream);
+
 /* ---- InfoFlow recommender DQN: replaces DqnInfoFlowModel's Keras graph (xt/model/dqn/dqn_rec_model.py:63-169) and the
  * target computation of DQNInfoFlowAlg.train (xt/algorithm/dqn/dqn_infoflw_alg.py:76-174) --------------------------------
  * Inputs are int32 ids in [0, vocab) (Keras Embedding's cast; not checked on the device): user [user_dim], history_click

@@ -1,12 +1,17 @@
 """QMixAlg (xt/algorithm/qmix/qmix_alg.py) over QMixModel: the host episode buffer, the agents' input assembly, the
 epsilon-greedy selector and the training batch preparation.  The network work is QMixModel's (xtb_qmix_train /
 xtb_qmix_infer); everything here is NumPy on the host and draws from the global np.random stream in the reference's
-order, so a seeded run samples the same episodes and picks the same actions."""
+order, so a seeded run samples the same episodes and picks the same actions.  With alg_config DEVICE_REPLAY the episode
+ring lives in HBM instead (DeviceEpisodeReplay) and the batch is assembled there, inside the model's training graph."""
+import ctypes as C
 import logging
 import os
 
 import numpy as np
+import torch
 
+from .. import capi
+from ..engine import _ptr, stream_ptr
 from ..registry import Registers
 from .base import Algorithm, ZFILL_LENGTH
 
@@ -110,6 +115,166 @@ class ReplayBuffer(EpisodeBatch):
         return self[np.random.choice(self.episodes_in_buffer, batch_size, replace=False)]
 
 
+class EpisodeRing(object):
+    """ReplayBuffer's bookkeeping without its arrays: the ring position, the stored count and the draw of the episode ids,
+    with the same rules and the same np.random calls."""
+
+    def __init__(self, buffer_size):
+        self.buffer_size = buffer_size
+        self.buffer_index = self.episodes_in_buffer = 0
+
+    def insert(self, k):
+        """Advance over k new episodes as insert_episode_batch does (a batch running past the end is split there) -> the
+        slot of each, in order."""
+        if self.buffer_index + k <= self.buffer_size:
+            slots = list(range(self.buffer_index, self.buffer_index + k))
+            self.buffer_index += k
+            self.episodes_in_buffer = max(self.episodes_in_buffer, self.buffer_index)
+            self.buffer_index %= self.buffer_size
+            return slots
+        left = self.buffer_size - self.buffer_index
+        return self.insert(left) + self.insert(k - left)
+
+    def can_sample(self, batch_size):
+        return self.episodes_in_buffer >= batch_size
+
+    def sample(self, batch_size):
+        """The ids ReplayBuffer.sample would gather: all of them, undrawn, when exactly batch_size are stored."""
+        if not self.can_sample(batch_size):
+            raise ValueError("{} episodes stored, {} requested".format(self.episodes_in_buffer, batch_size))
+        if self.episodes_in_buffer == batch_size:
+            return np.arange(batch_size)
+        return np.random.choice(self.episodes_in_buffer, batch_size, replace=False)
+
+
+# The fields of a packed episode row (xtb200.h, xtb_episode_replay): scheme key and stored dtype, in row order
+ROW_FIELDS = (("state", np.float32), ("obs", np.float32), ("actions", np.int32), ("actions_onehot", np.float32),
+              ("avail_actions", np.int32), ("reward", np.float32), ("terminated", np.uint8), ("filled", np.int64))
+
+
+class EpisodeRowPacker(object):
+    """One episode as DeviceEpisodeReplay stores it: the values ReplayBuffer's row would hold after insert_episode_batch
+    (EpisodeBatch.update on a one-episode scratch batch: the scheme dtypes, the actions one-hot, a caller's
+    actions_onehot written after actions winning), packed into one byte row of the device layout.  The one-hot is kept
+    as float32: the host path rounds its float64 to float32 once when it stages the batch, as this does."""
+
+    def __init__(self, scheme, groups, max_seq_length, preprocess):
+        self.scratch = EpisodeBatch(scheme, groups, 1, max_seq_length, preprocess=preprocess)
+        self.T, self.n, self.A = max_seq_length, groups["agents"], self.scratch.scheme["avail_actions"]["vshape"][0]
+        derived = {new_key for new_key, _ in self.scratch.preprocess.values()}
+        self.required = [k for k in self.scratch.data if k not in derived]
+        self.shapes = [(key, self.scratch.data[key].shape[1:], dt) for key, dt in ROW_FIELDS]
+        sizes = [int(np.prod(s)) * np.dtype(dt).itemsize for _, s, dt in self.shapes]
+        self.offsets = [int(o) for o in np.cumsum([0] + [(s + 15) // 16 * 16 for s in sizes])]
+        self.row_bytes = self.offsets[-1]
+
+    def pack(self, data):
+        """data {key: [T, ...]} -> the uint8 row.  ValueError for a missing field (the device ring keeps no earlier
+        episode's values to fall back on), an action of the first T - 1 steps outside [0, n_actions) or a filled sum
+        outside [0, T]: the training batch reads them as indices and lengths."""
+        missing = [k for k in self.required if k not in data]
+        if missing:
+            raise ValueError("the device replay stores whole episodes: {} missing".format(missing))
+        sb = self.scratch
+        act = np.array(data["actions"], dtype=sb.scheme["actions"]["dtype"]).reshape(sb.data["actions"].shape)
+        bad = (act[:, :-1] < 0) | (act[:, :-1] >= self.A)
+        if np.any(bad):
+            raise ValueError("actions must be in [0, {}), got {}".format(self.A, act[:, :-1][bad][0]))
+        sb.update(data, mark_filled=False)
+        filled = int(np.sum(sb.data["filled"]))
+        if not 0 <= filled <= self.T:
+            raise ValueError("filled sums to {}, not in [0, {}]".format(filled, self.T))
+        row = np.zeros(self.row_bytes, np.uint8)
+        for (key, shape, dt), o in zip(self.shapes, self.offsets):
+            v = np.ascontiguousarray(sb.data[key][0], dtype=dt).reshape(-1).view(np.uint8)
+            row[o:o + v.size] = v
+        return row
+
+    def fields(self, row):
+        """{key: array} views of a packed row, in their stored dtypes and [T, ...] shapes."""
+        return {key: row[o:o + int(np.prod(shape)) * np.dtype(dt).itemsize].view(dt).reshape(shape)
+                for (key, shape, dt), o in zip(self.shapes, self.offsets)}
+
+
+class DeviceEpisodeReplay(EpisodeRing):
+    """ReplayBuffer in HBM (xtb_episode_replay): episodes are packed on the host (EpisodeRowPacker) and stored with one
+    staged upload each; the ring bookkeeping and the draws stay on the host (EpisodeRing).  The training batch is
+    gathered on the device from the drawn ids, by gather() or inside the models' train_replay."""
+
+    def __init__(self, scheme, groups, buffer_size, max_seq_length, preprocess, obs_last_action, obs_agent_id, device=None):
+        super().__init__(buffer_size)
+        self.packer = EpisodeRowPacker(scheme, groups, max_seq_length, preprocess)
+        sh = self.packer.scratch.scheme
+        self.T, self.n, self.A = max_seq_length, groups["agents"], self.packer.A
+        self.obs_dim, self.state_dim = int(np.prod(sh["obs"]["vshape"])), int(np.prod(sh["state"]["vshape"]))
+        self.width = self.obs_dim + (self.A if obs_last_action else 0) + (self.n if obs_agent_id else 0)
+        self.switches = (int(bool(obs_last_action)), int(bool(obs_agent_id)))
+        self.device = device
+        self._bufs = {}
+        self._create()
+
+    def _create(self):
+        """The native ring (one device allocation)."""
+        self.device = torch.device("cuda", torch.cuda.current_device()) if self.device is None else torch.device(self.device)
+        self.handle = C.c_void_p()
+        with torch.cuda.device(self.device):
+            capi.check(capi.lib().xtb_episode_replay_create(self.buffer_size, self.T - 1, self.n, self.A, self.obs_dim, self.state_dim,
+                                                            *self.switches, C.byref(self.handle)))
+        if capi.lib().xtb_episode_replay_row_bytes(self.handle) != self.packer.row_bytes:
+            raise RuntimeError("episode row layout disagrees with the library's")
+
+    def _store(self, slot, row):
+        """One packed row into ring slot `slot` (one staged upload)."""
+        capi.check(capi.lib().xtb_episode_replay_add(self.handle, slot, row.ctypes.data, row.nbytes, stream_ptr()))
+
+    def __del__(self):
+        try:
+            if getattr(self, "handle", None) and self.handle.value:
+                capi.lib().xtb_episode_replay_destroy(self.handle)
+                self.handle = C.c_void_p()
+        except Exception:   # interpreter shutdown
+            pass
+
+    def insert_episode_batch(self, ep):
+        """Store ep's episodes at the ring position, as ReplayBuffer.insert_episode_batch; every episode is checked and
+        packed (ValueError) before anything is stored."""
+        rows = [ep.data] if ep.batch_size == 1 else [ep[i:i + 1].data for i in range(ep.batch_size)]
+        packed = [self.packer.pack(r) for r in rows]
+        before = self.buffer_index, self.episodes_in_buffer
+        try:
+            for row, slot in zip(packed, self.insert(len(packed))):
+                self._store(slot, row)
+        except Exception:    # a refused store (a communicator installed, say) leaves the ring where it was
+            self.buffer_index, self.episodes_in_buffer = before
+            raise
+
+    def buffers(self, B):
+        """Device buffers of a gathered B-episode batch (xtb_episode_batch), overwritten by the next gather of that size."""
+        b = self._bufs.get(B)
+        if b is None:
+            T, L, n, A, dev = self.T, self.T - 1, self.n, self.A, self.device
+            f32, i32 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int32, device=dev)
+            b = dict(obs=torch.empty(B, T, n, self.width, **f32), raw_obs=torch.empty(B, T, n, self.obs_dim, **f32),
+                     seq_len=torch.empty(B * n, **i32), avail=torch.empty(B, T, n, A, **f32), actions=torch.empty(B, L, n, **i32),
+                     state=torch.empty(B, L, self.state_dim, **f32), next_state=torch.empty(B, L, self.state_dim, **f32),
+                     reward=torch.empty(B, L, **f32), terminated=torch.empty(B, L, **f32), mask=torch.empty(B, L, **f32),
+                     max_t=torch.zeros(1, **i32))
+            bt = capi.EpisodeBatch()
+            for k in ("obs", "raw_obs", "seq_len", "avail", "actions", "state", "next_state", "reward", "terminated", "mask"):
+                setattr(bt, k, b[k].data_ptr())
+            b["batch"] = bt
+            self._bufs[B] = b
+        return b
+
+    def gather(self, ids):
+        """The training batch of episodes `ids` (xtb_episode_replay_gather) -> {name: device tensor} of buffers()."""
+        ids = np.ascontiguousarray(ids, np.int32)
+        b = self.buffers(len(ids))
+        capi.check(capi.lib().xtb_episode_replay_gather(self.handle, len(ids), ids.ctypes.data, C.byref(b["batch"]), _ptr(b["max_t"]),
+                                                        stream_ptr()))
+        return b
+
+
 class OneHot(object):
     """OneHotNp: integer [..., 1] -> float64 one-hot [..., out_dim]."""
 
@@ -161,11 +326,29 @@ class EpsilonGreedyActionSelector(object):
         return pick_random * random_actions + (1 - pick_random) * masked.argmax(axis=2)
 
 
+def _device_replay_flag(alg_config):
+    """alg_config DEVICE_REPLAY (or device_replay), a bool, default False; checked before anything touches CUDA."""
+    given = [(k, alg_config[k]) for k in ("DEVICE_REPLAY", "device_replay") if k in alg_config]
+    for k, v in given:
+        if not isinstance(v, (bool, np.bool_)):
+            raise ValueError("{} must be a bool, got {!r}".format(k, v))
+    if len(given) == 2 and bool(given[0][1]) != bool(given[1][1]):
+        raise ValueError("DEVICE_REPLAY and device_replay disagree")
+    return bool(given[0][1]) if given else False
+
+
 @Registers.algorithm
 class QMixAlg(Algorithm):
-    """QMixAlg (qmix_alg.py:102-410)."""
+    """QMixAlg (qmix_alg.py:102-410).
+
+    alg_config DEVICE_REPLAY True (or device_replay) keeps the episode ring in HBM (DeviceEpisodeReplay) in the train
+    scene: prepare_data packs and uploads each episode once and draws the ids with the host's np.random calls, and
+    train() gathers the batch and steps the model in one graph (the model's train_replay)."""
+
+    device_replay = False
 
     def __init__(self, model_info, alg_config, **kwargs):
+        device_replay = _device_replay_flag(alg_config)
         env_info = alg_config["env_attr"]
         alg_config.update({"n_agents": env_info["n_agents"], "n_actions": env_info["n_actions"],
                            "state_shape": env_info["state_shape"]})
@@ -193,8 +376,15 @@ class QMixAlg(Algorithm):
         self.last_target_update_episode = -9999.0
         self.groups = {"agents": env_info["n_agents"]}
         self.preprocess = {"actions": ("actions_onehot", [OneHot(out_dim=alg_config["n_actions"])])}
-        self.buffer = ReplayBuffer(self.scheme, self.groups, alg_config["buffer_size"], env_info["episode_limit"] + 1,
-                                   preprocess=self.preprocess)
+        # the device ring serves the learner only: the explore scene allocates nothing on the device
+        self.device_replay = device_replay and model_info["actor"]["scene"] == "train"
+        if self.device_replay:
+            self.buffer = DeviceEpisodeReplay(self.scheme, self.groups, alg_config["buffer_size"], env_info["episode_limit"] + 1,
+                                              self.preprocess, alg_config["obs_last_action"], alg_config["obs_agent_id"],
+                                              device=getattr(self.actor, "device", None))
+        else:
+            self.buffer = ReplayBuffer(self.scheme, self.groups, alg_config["buffer_size"], env_info["episode_limit"] + 1,
+                                       preprocess=self.preprocess)
         self.train_batch = None
         self.train_times = 0
 
@@ -246,12 +436,18 @@ class QMixAlg(Algorithm):
 
     def train(self, **kwargs):
         """One QMixModel.train on the drawn batch (nan without one), the explore-agent sync, and the target sync once
-        (episode_num - last sync) / target_update_interval >= 1."""
-        if not self.train_batch:
+        (episode_num - last sync) / target_update_interval >= 1.  With the device replay the batch is the drawn ids and
+        the step is the model's train_replay: one upload of the ids, one graph, one download of the loss and max_t."""
+        if self.train_batch is None:
             return np.nan
         episode_num = kwargs.get("episode_num")
         if not episode_num:
             raise KeyError("need episode num to update target network")
+        if self.device_replay:
+            self.train_times += 1
+            loss, max_ep_t = self.actor.train_replay(self.buffer, self.train_batch)
+            self._after_train(episode_num, max_ep_t)
+            return loss
         batch = self.train_batch
         max_ep_t = batch.max_t_filled()
         rewards = batch["reward"][:, :-1]
@@ -263,13 +459,17 @@ class QMixAlg(Algorithm):
         self.train_times += 1
         loss = self.actor.train(trajectories, [max_ep_t for _ in range(batch.batch_size * self.n_agents)], batch["avail_actions"],
                                 actions, batch["state"][:, :-1], batch["state"][:, 1:], rewards, terminated, mask)
+        self._after_train(episode_num, max_ep_t)
+        return loss
+
+    def _after_train(self, episode_num, max_ep_t):
+        """The explore-agent sync after every step, the target sync once per target_update_interval episodes."""
         self.actor.assign_explore_agent()
         if (episode_num - self.last_target_update_episode) / self.alg_config["target_update_interval"] >= 1.0:
             self.actor.assign_targets()
             logging.info("episode-%s, target Q network params replaced (train %d, seq-len %d)", episode_num, self.train_times,
                          max_ep_t)
             self.last_target_update_episode = episode_num
-        return loss
 
     def train_ready(self, elapsed_episode, **kwargs):
         """Ready once a batch can be sampled; before that the caller's dist_dummy_model is called (KeyError without one)."""

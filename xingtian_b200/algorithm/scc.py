@@ -29,6 +29,8 @@ class SCCAlg(QMixAlg):
         self.alg_name = "SCCAlg"
 
     def train(self, **kwargs):
+        if self.device_replay:
+            return super().train(**kwargs)     # SCCModel.train_replay reads the raw obs from the ring
         if not self.train_batch:
             return np.nan
         actor = self.actor

@@ -91,6 +91,12 @@ class SccBatch(C.Structure):
                 ("terminated", C.c_void_p), ("mask", C.c_void_p), ("subsets", C.c_void_p)]
 
 
+class EpisodeBatch(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("raw_obs", C.c_void_p), ("seq_len", C.c_void_p), ("avail", C.c_void_p), ("actions", C.c_void_p),
+                ("state", C.c_void_p), ("next_state", C.c_void_p), ("reward", C.c_void_p), ("terminated", C.c_void_p),
+                ("mask", C.c_void_p)]
+
+
 class InfoflowDesc(C.Structure):
     _fields_ = [("user_dim", C.c_int32), ("item_dim", C.c_int32), ("emb_dim", C.c_int32), ("vocab", C.c_int32), ("batch", C.c_int32),
                 ("last_act", C.c_int32), ("gamma", C.c_double), ("gru_off", C.c_longlong), ("gru1_off", C.c_longlong),
@@ -205,6 +211,13 @@ _SIGS = {
     "xtb_scc_train": (C.c_int, [_P, _P, _P, _P, C.POINTER(SccBatch), _P, C.c_int, _P]),
     "xtb_scc_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_scc_critic": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, _P]),
+    "xtb_episode_replay_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "xtb_episode_replay_destroy": (None, [_P]),
+    "xtb_episode_replay_row_bytes": (C.c_longlong, [_P]),
+    "xtb_episode_replay_add": (C.c_int, [_P, C.c_int, _P, C.c_longlong, _P]),
+    "xtb_episode_replay_gather": (C.c_int, [_P, C.c_int, _P, C.POINTER(EpisodeBatch), _P, _P]),
+    "xtb_qmix_replay_train": (C.c_int, [_P, _P, _P, _P, C.c_int, _P, C.POINTER(QmixBatch), _P, _P, C.c_int, _P]),
+    "xtb_scc_replay_train": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P, C.POINTER(SccBatch), _P, _P, C.c_int, _P]),
     "xtb_infoflow_create": (C.c_int, [C.POINTER(InfoflowDesc), C.POINTER(_P)]),
     "xtb_infoflow_destroy": (None, [_P]),
     "xtb_infoflow_train": (C.c_int, [_P, _P, _P, C.POINTER(InfoflowBatch), _P, _P, C.c_int, _P]),

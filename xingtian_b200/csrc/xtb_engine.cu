@@ -21,6 +21,7 @@
 #include "muzero_replay.cuh"
 #include "qmix.cuh"
 #include "scc.cuh"
+#include "episode_replay.cuh"
 #include "infoflow.cuh"
 #include "stager.cuh"
 #include "bp_gemm.cuh"
@@ -1922,7 +1923,8 @@ extern "C" int xtb_set_fuse_heads(int on) { g_fuse_heads = on; return XTB_OK; }
 // modes, which every capture reads.  Keys are compared bytewise.
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
                 kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
-                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict, kMuzeroReplayTrain };
+                kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict, kMuzeroReplayTrain,
+                kQmixReplayTrain, kSccReplayTrain };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[7];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[6]):
@@ -3294,17 +3296,23 @@ static int scc_train_launch(xtb_scc* q, xtb_adam* copt, xtb_adam* aopt, const fl
   return rc;
 }
 
+// xtb_scc_train's and xtb_scc_replay_train's checks of the object and both optimisers
+static int scc_learner_check(const char* fn, const xtb_scc* q, bool missing, const xtb_adam* critic_opt, const xtb_adam* actor_opt) {
+  if (int rc = learner_check(fn, missing, q->ag.fc1, actor_opt, q->ag.R, false, q->ag.R, q->agent_size)) return rc;
+  if (critic_opt->count != q->n_params - q->o_mix)
+    return fail(XTB_ERR_ARG, "%s: critic optimiser size %lld != %lld", fn, critic_opt->count, q->n_params - q->o_mix);
+  if (critic_opt->mg || critic_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the critic optimiser must be Adam", fn);
+  if (!actor_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the actor optimiser must be uncentred RMSProp (xtb_opt_use_rmsprop_plain)", fn);
+  return XTB_OK;
+}
+
 extern "C" int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const float* target, const xtb_scc_batch* batch,
                              float* loss_out, int use_graph, void* stream) {
   const char* fn = "xtb_scc_train";
   if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
   const bool missing = !critic_opt || !actor_opt || !target || !batch || !loss_out || !batch->obs || !batch->raw_obs || !batch->seq_len ||
                        !batch->actions || !batch->reward || !batch->terminated || !batch->mask || (!q->multi && q->ag.n > 2 && !batch->subsets);
-  if (int rc = learner_check(fn, missing, q->ag.fc1, actor_opt, q->ag.R, false, q->ag.R, q->agent_size)) return rc;
-  if (critic_opt->count != q->n_params - q->o_mix)
-    return fail(XTB_ERR_ARG, "%s: critic optimiser size %lld != %lld", fn, critic_opt->count, q->n_params - q->o_mix);
-  if (critic_opt->mg || critic_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the critic optimiser must be Adam", fn);
-  if (!actor_opt->rms_plain) return fail(XTB_ERR_ARG, "%s: the actor optimiser must be uncentred RMSProp (xtb_opt_use_rmsprop_plain)", fn);
+  if (int rc = scc_learner_check(fn, q, missing, critic_opt, actor_opt)) return rc;
   const xtb_scc_batch b = *batch;
   return run_graph(capture_key(kSccTrain, {q->ag.fc1, q->cn[0], q, critic_opt, actor_opt}, q, target, b.obs, b.raw_obs, b.seq_len,
                                b.actions, b.reward, b.terminated, b.mask, b.subsets, loss_out),
@@ -3339,6 +3347,168 @@ extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* 
             (const float*)(q->ag.fc1->params + q->o_head), rows, q->U, q->concat, v_out);
     LAUNCH_CHECK();
     return XTB_OK;
+  });
+}
+
+// ---- QMIX / SCC episode replay (episode_replay.cuh) -------------------------------------------------------------------
+// The ring and the drawn ids are one device allocation; `count` mirrors the stored slots so that a draw past them is
+// refused before a launch.
+struct xtb_episode_replay {
+  EprDev d{};
+  int capacity = 0, count = 0;
+  void* buf = nullptr;
+  int32_t* ids = nullptr;   // [capacity] the episode ids of the current call
+};
+
+extern "C" int xtb_episode_replay_create(int capacity, int episode_limit, int n_agents, int n_actions, int obs_dim, int state_dim,
+                                         int obs_last_action, int obs_agent_id, xtb_episode_replay** out) {
+  const char* fn = "xtb_episode_replay_create";
+  if (!out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (capacity < 1 || episode_limit < 1 || n_agents < 1 || n_agents > QM_MAX_AGENTS || n_actions < 1 || n_actions > 255 ||
+      obs_dim < 0 || state_dim < 1 || (obs_last_action != 0 && obs_last_action != 1) || (obs_agent_id != 0 && obs_agent_id != 1))
+    return fail(XTB_ERR_ARG, "%s: capacity %d / episode_limit %d / n_agents %d / n_actions %d / obs_dim %d / state_dim %d / switches %d %d "
+                "out of range", fn, capacity, episode_limit, n_agents, n_actions, obs_dim, state_dim, obs_last_action, obs_agent_id);
+  EprDev d{};
+  d.T = episode_limit + 1; d.n = n_agents; d.o = obs_dim; d.S = state_dim; d.A = n_actions;
+  d.last_action = obs_last_action; d.agent_id = obs_agent_id;
+  d.width = obs_dim + (obs_last_action ? n_actions : 0) + (obs_agent_id ? n_agents : 0);
+  const long long row = epr_layout(d);
+  if (row > (1LL << 40) / capacity) return fail(XTB_ERR_ARG, "%s: %d episodes of %lld bytes are too large", fn, capacity, row);
+  auto* r = new xtb_episode_replay();
+  r->d = d;
+  if (int rc = carve_scratch(fn, &r->buf, {{&r->d.ring, capacity * row}, {&r->ids, (long long)capacity}})) {
+    delete r;
+    return rc;
+  }
+  r->capacity = capacity;
+  *out = r;
+  return XTB_OK;
+}
+
+extern "C" void xtb_episode_replay_destroy(xtb_episode_replay* r) {
+  if (!r) return;
+  drop_graphs_of(r);
+  cudaDeviceSynchronize();
+  cudaFree(r->buf);
+  delete r;
+}
+
+extern "C" long long xtb_episode_replay_row_bytes(const xtb_episode_replay* r) { return r ? r->d.row_bytes : 0; }
+
+static int epr_check(const char* fn, const xtb_episode_replay* r, bool missing) {
+  if (!r || missing) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (g_comm) return fail(XTB_ERR_STATE, "%s: data-parallel training (communicator) is not supported", fn);
+  return XTB_OK;
+}
+
+extern "C" int xtb_episode_replay_add(xtb_episode_replay* r, int slot, const void* row, long long bytes, void* stream) {
+  const char* fn = "xtb_episode_replay_add";
+  if (int rc = epr_check(fn, r, !row)) return rc;
+  const EprDev& d = r->d;
+  if (slot < 0 || slot >= r->capacity) return fail(XTB_ERR_ARG, "%s: slot %d not in [0, %d)", fn, slot, r->capacity);
+  if (bytes != d.row_bytes) return fail(XTB_ERR_ARG, "%s: a row is %lld bytes, not %lld", fn, d.row_bytes, bytes);
+  // the batch reads the actions as indices and the filled sum as a sequence length: both are checked here
+  const uint8_t* h = static_cast<const uint8_t*>(row);
+  for (long long i = 0; i < (long long)(d.T - 1) * d.n; i++) {
+    int32_t a;
+    memcpy(&a, h + d.o_act + 4 * i, 4);
+    if (a < 0 || a >= d.A) return fail(XTB_ERR_ARG, "%s: action %d not in [0, %d)", fn, a, d.A);
+  }
+  uint64_t sum = 0;   // int64 addition wraps as NumPy's does
+  for (int t = 0; t < d.T; t++) {
+    int64_t f;
+    memcpy(&f, h + d.o_filled + 8 * t, 8);
+    sum += (uint64_t)f;
+  }
+  if ((int64_t)sum < 0 || (int64_t)sum > d.T) return fail(XTB_ERR_ARG, "%s: filled sums to %lld, not in [0, %d]", fn, (long long)(int64_t)sum, d.T);
+  CUDA_TRY(xtb::Stager::instance().stage_h2d(d.ring + (long long)slot * d.row_bytes, row, (size_t)bytes, S(stream)));
+  r->count = std::max(r->count, slot + 1);
+  return XTB_OK;
+}
+
+// B ids, each a stored slot, into the replay's id buffer (one staged upload on `stream`)
+static int epr_ids(const char* fn, xtb_episode_replay* r, int B, const int32_t* ids, void* stream) {
+  if (B < 1 || B > r->count) return fail(XTB_ERR_ARG, "%s: batch %d not in [1, %d stored episodes]", fn, B, r->count);
+  for (int b = 0; b < B; b++)
+    if (ids[b] < 0 || ids[b] >= r->count) return fail(XTB_ERR_ARG, "%s: id %d not in [0, %d)", fn, ids[b], r->count);
+  CUDA_TRY(xtb::Stager::instance().stage_h2d(r->ids, ids, sizeof(int32_t) * B, S(stream)));
+  return XTB_OK;
+}
+
+static int epr_gather_launch(xtb_episode_replay* r, int B, const xtb_episode_batch& o, int32_t* max_t, cudaStream_t st) {
+  if (o.seq_len || max_t) {
+    XLAUNCH(epr_seq_len_kernel, 1, 256, 0, st, r->d, (const int32_t*)r->ids, B, o.seq_len, max_t);
+    LAUNCH_CHECK();
+  }
+  XLAUNCH(epr_gather_kernel, dim3(r->d.T, B), kEprThreads, 0, st, r->d, (const int32_t*)r->ids, o);
+  LAUNCH_CHECK();
+  return XTB_OK;
+}
+
+// the replay's episodes are the agent's training batch
+static int epr_agent_check(const char* fn, const xtb_episode_replay* r, const QmixAgent& a, int B) {
+  if (B != a.B) return fail(XTB_ERR_ARG, "%s: batch %d is not the model's %d", fn, B, a.B);
+  const EprDev& d = r->d;
+  if (d.n != a.n || d.A != a.A || d.T != a.T || d.width != a.fc1->tsize[0])
+    return fail(XTB_ERR_ARG, "%s: replay (%d agents, %d actions, %d steps, inputs %d wide) does not match the model (%d, %d, %d, %d)", fn,
+                d.n, d.A, d.T, d.width, a.n, a.A, a.T, a.fc1->tsize[0]);
+  return XTB_OK;
+}
+
+extern "C" int xtb_episode_replay_gather(xtb_episode_replay* r, int batch, const int32_t* ids, const xtb_episode_batch* out, int32_t* max_t_out,
+                                         void* stream) {
+  const char* fn = "xtb_episode_replay_gather";
+  if (int rc = epr_check(fn, r, !ids || !out)) return rc;
+  if (int rc = epr_ids(fn, r, batch, ids, stream)) return rc;
+  return epr_gather_launch(r, batch, *out, max_t_out, S(stream));
+}
+
+extern "C" int xtb_qmix_replay_train(xtb_episode_replay* r, xtb_qmix* q, xtb_adam* opt, const float* target, int batch, const int32_t* ids,
+                                     const xtb_qmix_batch* bufs, float* loss_out, int32_t* max_t_out, int use_graph, void* stream) {
+  const char* fn = "xtb_qmix_replay_train";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  const bool missing = !ids || !opt || !target || !bufs || !loss_out || !max_t_out || !bufs->obs || !bufs->seq_len || !bufs->avail ||
+                       !bufs->actions || !bufs->state || !bufs->next_state || !bufs->reward || !bufs->terminated || !bufs->mask;
+  if (int rc = epr_check(fn, r, missing)) return rc;
+  if (int rc = learner_check(fn, false, q->ag.fc1, opt, q->ag.R, false, q->ag.R, q->n_params)) return rc;
+  if (!opt->mg) return fail(XTB_ERR_ARG, "%s: the optimiser must be centred RMSProp (xtb_opt_use_rmsprop)", fn);
+  if (int rc = epr_agent_check(fn, r, q->ag, batch)) return rc;
+  if (r->d.S != q->hyp->tsize[0]) return fail(XTB_ERR_ARG, "%s: replay states are %d wide, the mixer's %d", fn, r->d.S, q->hyp->tsize[0]);
+  if (int rc = epr_ids(fn, r, batch, ids, stream)) return rc;
+  const xtb_qmix_batch b = *bufs;
+  const xtb_episode_batch o{const_cast<float*>(b.obs), nullptr, const_cast<int32_t*>(b.seq_len), const_cast<float*>(b.avail),
+                            const_cast<int32_t*>(b.actions), const_cast<float*>(b.state), const_cast<float*>(b.next_state),
+                            const_cast<float*>(b.reward), const_cast<float*>(b.terminated), const_cast<float*>(b.mask)};
+  return run_graph(capture_key(kQmixReplayTrain, {q->ag.fc1, q->ag.fc2, q->hyp, q, opt, r}, r, q, target, batch, b.obs, b.seq_len, b.avail,
+                               b.actions, b.state, b.next_state, b.reward, b.terminated, b.mask, loss_out, max_t_out),
+                   use_graph, stream, [&](void* sv) -> int {
+    int rc = epr_gather_launch(r, batch, o, max_t_out, S(sv));
+    return rc ? rc : qmix_train_launch(q, opt, target, b, loss_out, S(sv));
+  });
+}
+
+extern "C" int xtb_scc_replay_train(xtb_episode_replay* r, xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const float* target, int batch,
+                                    const int32_t* ids, const xtb_scc_batch* bufs, float* loss_out, int32_t* max_t_out, int use_graph,
+                                    void* stream) {
+  const char* fn = "xtb_scc_replay_train";
+  if (!q) return fail(XTB_ERR_ARG, "%s: null object", fn);
+  const bool missing = !ids || !critic_opt || !actor_opt || !target || !bufs || !loss_out || !max_t_out || !bufs->obs || !bufs->raw_obs ||
+                       !bufs->seq_len || !bufs->actions || !bufs->reward || !bufs->terminated || !bufs->mask ||
+                       (!q->multi && q->ag.n > 2 && !bufs->subsets);
+  if (int rc = epr_check(fn, r, missing)) return rc;
+  if (int rc = scc_learner_check(fn, q, false, critic_opt, actor_opt)) return rc;
+  if (int rc = epr_agent_check(fn, r, q->ag, batch)) return rc;
+  if (r->d.o != q->o) return fail(XTB_ERR_ARG, "%s: replay observations are %d wide, the critic's %d", fn, r->d.o, q->o);
+  if (int rc = epr_ids(fn, r, batch, ids, stream)) return rc;
+  const xtb_scc_batch b = *bufs;
+  const xtb_episode_batch o{const_cast<float*>(b.obs), const_cast<float*>(b.raw_obs), const_cast<int32_t*>(b.seq_len), nullptr,
+                            const_cast<int32_t*>(b.actions), nullptr, nullptr, const_cast<float*>(b.reward), const_cast<float*>(b.terminated),
+                            const_cast<float*>(b.mask)};
+  return run_graph(capture_key(kSccReplayTrain, {q->ag.fc1, q->cn[0], q, critic_opt, actor_opt, r}, r, q, target, batch, b.obs, b.raw_obs,
+                               b.seq_len, b.actions, b.reward, b.terminated, b.mask, b.subsets, loss_out, max_t_out),
+                   use_graph, stream, [&](void* sv) -> int {
+    int rc = epr_gather_launch(r, batch, o, max_t_out, S(sv));
+    return rc ? rc : scc_train_launch(q, critic_opt, actor_opt, target, b, loss_out, S(sv));
   });
 }
 

@@ -292,6 +292,29 @@ class QMixModel(XTModel):
         self.train_device(b)
         return float(b["loss"].cpu()[0])
 
+    def _replay_out(self, n_loss):
+        """[n_loss losses | max_t_filled as int32] side by side, for one download per train_replay."""
+        if getattr(self, "_rout", None) is None:
+            self._rout = torch.zeros(n_loss + 1, dtype=torch.float32, device=self.device)
+        return self._rout
+
+    def train_replay(self, replay, ids):
+        """QMixAlg.train's step on the episodes `ids` of a DeviceEpisodeReplay (xtb_qmix_replay_train, graph-replayed
+        when the model uses graphs): one staged upload of the ids, the batch gathered into _train_buffers() and the
+        step of train(), one download -> (loss, max_t_filled)."""
+        if self.opt is None:
+            raise RuntimeError("QMixModel.train_replay needs the train scene")
+        b = self._train_buffers()
+        out = self._replay_out(1)
+        bt = capi.QmixBatch()
+        for k in ("obs", "seq_len", "avail", "actions", "state", "next_state", "reward", "terminated", "mask"):
+            setattr(bt, k, b[k].data_ptr())
+        ids = np.ascontiguousarray(ids, np.int32)
+        check(capi.lib().xtb_qmix_replay_train(replay.handle, self.handle, self.opt.handle, _ptr(self.target), len(ids), ids.ctypes.data,
+                                               C.byref(bt), _ptr(out[:1]), _ptr(out[1:]), 1 if self.use_graph else 0, stream_ptr()))
+        host = out.cpu().numpy()
+        return float(host[0]), int(host[1:].view(np.int32)[0])
+
     def train_device(self, b):
         """xtb_qmix_train on the device tensors of _train_buffers(); the loss lands in b["loss"]."""
         bt = capi.QmixBatch()

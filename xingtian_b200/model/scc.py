@@ -276,6 +276,28 @@ class SCCModel(QMixModel):
         self.mixer_loss, self.actor_loss = float(mixer), float(actor)
         return float(actor + mixer)
 
+    def train_replay(self, replay, ids):
+        """SCCAlg.train's step on the episodes `ids` of a DeviceEpisodeReplay (xtb_scc_replay_train): as
+        QMixModel.train_replay, with the raw obs gathered from the ring and the Monte-Carlo subsets drawn and uploaded
+        as train() does -> (actor + mixer loss, max_t_filled)."""
+        self._require_train("train_replay")
+        subsets = self.draw_subsets() if self.n_agents > 2 else None
+        b = self._train_buffers()
+        if subsets is not None:
+            stage_h2d(b["subsets"], subsets.view(np.int32)[:, :b["subsets"].shape[1]], np.int32)
+        out = self._replay_out(2)
+        bt = capi.SccBatch()
+        for k in ("obs", "raw_obs", "seq_len", "actions", "reward", "terminated", "mask", "subsets"):
+            setattr(bt, k, b[k].data_ptr())
+        ids = np.ascontiguousarray(ids, np.int32)
+        check(capi.lib().xtb_scc_replay_train(replay.handle, self.handle, self.critic_opt.handle, self.opt.handle, _ptr(self.target),
+                                              len(ids), ids.ctypes.data, C.byref(bt), _ptr(out[:2]), _ptr(out[2:]),
+                                              1 if self.use_graph else 0, stream_ptr()))
+        host = out.cpu().numpy()
+        mixer, actor = host[:2]
+        self.mixer_loss, self.actor_loss = float(mixer), float(actor)
+        return float(actor + mixer), int(host[2:].view(np.int32)[0])
+
     def train_device(self, b):
         """xtb_scc_train on the device tensors of _train_buffers(); [mixer loss, actor loss] land in b["loss"]."""
         bt = capi.SccBatch()
