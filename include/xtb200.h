@@ -217,11 +217,13 @@ int xtb_dqn_loss_grad(const float* q, const float* q_next_target, const float* q
 
 /* Same target/loss with the options BASELINE.json's north_star names (defaults = the reference): rows may be indexed
  * through idx (minibatch rows of a replay ring); disc != NULL is a per-row bootstrap discount (gamma^n of an n-step
- * return, 0 = the window hit a terminal step); huber_delta > 0 selects the Huber loss instead of the squared error. */
+ * return, 0 = the window hit a terminal step); huber_delta > 0 selects the Huber loss instead of the squared error.
+ * wt != NULL scales sample b's loss and gradient by wt[b] (Keras sample_weight); td_abs != NULL receives |y_b - q[b, a_b]|.
+ * dq is written in full: zero on every action not taken. */
 int xtb_dqn_td_loss_grad(const float* q, const float* q_next_target, const float* q_next_online, const int32_t* idx,
                          const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int batch,
-                         int adim, float gamma, float huber_delta, float inv_count, float* dq, float* y_out,
-                         float* loss_out, void* stream);
+                         int adim, float gamma, float huber_delta, float inv_count, const float* wt, float* dq,
+                         float* y_out, float* td_abs, float* loss_out, void* stream);
 /* n-step returns over env-major trajectories [n_env][n_step] (north_star "n-step TD-target kernel"; the reference's
  * DQN is 1-step, xt/algorithm/dqn/dqn.py:86-97): ret = sum_{k<m} gamma^k r_{t+k}, m = steps to the first terminal
  * (inclusive), n, or the end of the segment; disc = gamma^m or 0 after a terminal; last = row whose next-state
@@ -348,6 +350,10 @@ int xtb_dqn_train_weighted(xtb_net* net, xtb_net* target, xtb_adam* opt, const v
                            const int32_t* idx, const int32_t* action, const float* reward, const uint8_t* done,
                            const float* disc, int n_sample, float gamma, float huber_delta, int q_tensor, float* qn_t,
                            float* qn_o, const float* weights, float* td_abs, float* loss_out, int use_graph, void* stream);
+/* The heads_kernel entry the DQN steps launch for q_tensor under the current fused-heads mode: (kpl, amax) covering K <=
+ * 32 kpl hidden units and A <= amax actions; (0, 0) when the step runs layer by layer (q_tensor is not a fusable dueling
+ * layer).  A q_tensor out of range returns XTB_ERR_ARG.  Launches nothing. */
+int xtb_dqn_heads_plan(const xtb_net* net, int q_tensor, int* kpl, int* amax);
 
 /* ---- prioritized experience replay (Schaul et al., proportional variant) over the slots of a device replay ring: the
  *      rules of PrioritizedReplayBuffer (xt/algorithm/prioritized_replay_buffer_muzero.py:77-200), leaf i = ring slot i ----

@@ -795,9 +795,15 @@ class ImpalaLearner(Learner):
 
 def dqn_targets(y_online, target_q, actions, rewards, dones, gamma=0.99, q_next_online=None, disc=None):
     """xt/algorithm/dqn/dqn.py:79-95: 1-step TD target written into y[k,a_k], y in float32.
-    Double-DQN when q_next_online is given (:79-84).  `disc` holds a per-row discount (an n-step target, as
-    xtb_dqn_td_loss_grad takes it) that replaces gamma; y then keeps the working precision."""
-    y = np.array(y_online, np.float32 if disc is None else None, copy=True)
+    Double-DQN when q_next_online is given (:79-84), the first maximum of its row winning.  `disc` holds a per-row
+    discount (an n-step target, as xtb_dqn_td_loss_grad takes it) that replaces gamma; y then keeps the precision of
+    y_online.  Under precision("f64") y and every input it is built from are float64."""
+    if _PREC["np"] is np.float64:
+        y_online, target_q, rewards = (np.asarray(x, np.float64) for x in (y_online, target_q, rewards))
+        disc = None if disc is None else np.asarray(disc, np.float64)
+        y = np.array(y_online, copy=True)
+    else:
+        y = np.array(y_online, np.float32 if disc is None else None, copy=True)
     best = np.argmax(q_next_online if q_next_online is not None else target_q, 1)
     maxq = target_q[np.arange(len(y)), best]
     for k in range(len(y)):
@@ -809,12 +815,14 @@ class DqnLearner(Learner):
     """Restates DQN.train (xt/algorithm/dqn/dqn.py:61-103) + Keras compile(mse,
     Adam(clipnorm=10)) (xt/model/dqn/dqn_cnn.py:60-61): mse = mean over B*A;
     clipnorm clips EACH gradient tensor to norm<=10; Adam eps=1e-7.  `disc` / `huber` extend the TD target and
-    loss the way xtb_dqn_td_loss_grad does: a per-row discount, and Huber with that delta."""
+    loss the way xtb_dqn_td_loss_grad does: a per-row discount, and Huber with that delta; `weights` scale each row's
+    loss (Keras sample_weight).  The target net starts as a copy of the online weights, or from `target_weights`."""
 
     def __init__(self, arch, weights, lr=0.00015, clipnorm=10.0, gamma=0.99, target_update_freq=1000,
-                 double_dqn=False):
+                 double_dqn=False, target_weights=None):
         super().__init__(arch, weights)
-        self.target = [p.detach().clone() for p in self.params]
+        self.target = [p.detach().clone() for p in self.params] if target_weights is None else \
+            [p.detach() for p in _as_param_list(OrderedDict((n, target_weights[n]) for n in self.names))]
         self.opt = TFAdam(self.params, lr, eps=1e-7)
         self.clipnorm, self.gamma, self.freq, self.double = clipnorm, gamma, target_update_freq, double_dqn
         self.train_count = 0
@@ -823,7 +831,8 @@ class DqnLearner(Learner):
         with torch.no_grad():
             return forward(self.arch, self.named(self.target if target else None), states)[0].numpy()
 
-    def loss_and_grads(self, states, actions, rewards, new_states, dones, disc=None, huber=0.0):
+    def loss_and_grads(self, states, actions, rewards, new_states, dones, disc=None, huber=0.0, weights=None):
+        """the loss 1/(B A) sum_b w_b sum_a e_ba, its gradients, the targets y [B, A] and |y - Q(s, a)| [B]"""
         y_t = self.predict(states)
         tq = self.predict(new_states, target=True)
         qn = self.predict(new_states) if self.double else None
@@ -835,11 +844,14 @@ class DqnLearner(Learner):
             per = torch.where(ad <= huber, 0.5 * diff * diff, huber * (ad - 0.5 * huber))
         else:
             per = diff * diff
+        if weights is not None:
+            per = per * torch.from_numpy(np.asarray(weights)).to(per.dtype)[:, None]
         loss = per.mean()
-        return loss, torch.autograd.grad(loss, self.params), y
+        td_abs = diff.detach().abs().numpy()[np.arange(len(y)), np.asarray(actions, np.int64)]
+        return loss, torch.autograd.grad(loss, self.params), y, td_abs
 
     def train(self, states, actions, rewards, new_states, dones, disc=None, huber=0.0):
-        loss, grads, _ = self.loss_and_grads(states, actions, rewards, new_states, dones, disc, huber)
+        loss, grads, _, _ = self.loss_and_grads(states, actions, rewards, new_states, dones, disc, huber)
         if self.clipnorm:
             grads = clip_per_tensor(grads, self.clipnorm)
         self.opt.step(grads)

@@ -172,28 +172,6 @@ def test_ppo_loss_grad_matches_autograd(xb, B, A):
     assert rel_err(dv.cpu().numpy(), vt.grad.numpy()[:, 0]) < REL
 
 
-# ------------------------------------------------------------------------------------------- DQN
-@pytest.mark.parametrize("B,A,double", [(32, 4, False), (512, 4, False), (32, 6, True)])
-def test_dqn_target_and_mse(xb, B, A, double):
-    from xingtian_b200.engine import _ptr, stream_ptr
-    rng = np.random.default_rng(B + A)
-    q = rng.standard_normal((B, A)).astype(np.float32)
-    qt = rng.standard_normal((B, A)).astype(np.float32)
-    qo = rng.standard_normal((B, A)).astype(np.float32)
-    act = rng.integers(0, A, B).astype(np.int32)
-    rew = np.sign(rng.standard_normal(B)).astype(np.float32)
-    done = rng.random(B) < 0.1
-    y = orc.dqn_targets(q, qt, act, rew, done, 0.99, qo if double else None)
-    qq = torch.from_numpy(q).requires_grad_(True)
-    loss = ((qq - torch.from_numpy(y)) ** 2).mean(); loss.backward()
-    dq = torch.empty(B, A, device="cuda"); yo = torch.empty(B, device="cuda"); lo = torch.zeros(1, device="cuda")
-    xb["capi"].check(xb["lib"].xtb_dqn_loss_grad(_ptr(dev(q)), _ptr(dev(qt)), _ptr(dev(qo)) if double else None, _ptr(dev(act)), _ptr(dev(rew)),
-                                                _ptr(dev(done.view(np.uint8))), B, A, 0.99, 1.0 / (B * A), _ptr(dq), _ptr(yo), _ptr(lo), stream_ptr()))
-    assert rel_err(yo.cpu().numpy(), y[np.arange(B), act]) < 1e-6
-    assert rel_err(dq.cpu().numpy(), qq.grad.numpy()) < REL
-    assert abs(float(lo.cpu()[0]) - float(loss)) < REL * max(1.0, float(loss))
-
-
 # ------------------------------------------------------------------------------------------- Adam
 @pytest.mark.parametrize("mode", ["global", "per_tensor", "none"])
 def test_adam_clip_ten_steps(xb, mode):

@@ -141,7 +141,7 @@ _SIGS = {
     "xtb_dqn_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float,
                                     _P, _P, _P, _P]),
     "xtb_dqn_td_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
-                                      _P, _P, _P, _P]),
+                                      _P, _P, _P, _P, _P, _P]),
     "xtb_nstep_returns": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, _P, _P, _P]),
     "xtb_impala_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _P, C.c_int, _P]),
     "xtb_dqn_train": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, C.c_int, _P, _P, _P,
@@ -182,6 +182,7 @@ _SIGS = {
     "xtb_ppo_predict_host": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P, _P,
                                        C.c_int, _P]),
     "xtb_ppo_heads_plan": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "xtb_dqn_heads_plan": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "xtb_diag_gaussian_sample": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "xtb_ppo_gauss_loss_grad": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.POINTER(PpoHyper), C.c_float,
                                           _P, _P, _P, _P, _P]),

@@ -1677,19 +1677,19 @@ static int dqn_td_loss(const float* q, const float* q_next_target, const float* 
 }
 extern "C" int xtb_dqn_td_loss_grad(const float* q, const float* q_next_target, const float* q_next_online, const int32_t* idx,
                                     const int32_t* action, const float* reward, const uint8_t* done, const float* disc, int batch,
-                                    int adim, float gamma, float huber_delta, float inv_count, float* dq, float* y_out,
-                                    float* loss_out, void* stream) {
+                                    int adim, float gamma, float huber_delta, float inv_count, const float* wt, float* dq,
+                                    float* y_out, float* td_abs, float* loss_out, void* stream) {
   if (!q || !q_next_target || !action || !reward || !done || !dq || !loss_out) return fail(XTB_ERR_ARG, "xtb_dqn_td_loss_grad: null pointer");
   if (batch <= 0 || adim <= 0) return fail(XTB_ERR_ARG, "xtb_dqn_td_loss_grad: bad sizes");
   return dqn_td_loss(q, q_next_target, q_next_online, idx, action, reward, done, disc, batch, adim, gamma, huber_delta, inv_count,
-                     nullptr, dq, y_out, nullptr, loss_out, stream);
+                     wt, dq, y_out, td_abs, loss_out, stream);
 }
 extern "C" int xtb_dqn_loss_grad(const float* q, const float* q_next_target, const float* q_next_online,
                                  const int32_t* action, const float* reward, const uint8_t* done, int batch,
                                  int adim, float gamma, float inv_count, float* dq, float* y_out,
                                  float* loss_out, void* stream) {
   return xtb_dqn_td_loss_grad(q, q_next_target, q_next_online, nullptr, action, reward, done, nullptr, batch, adim, gamma, 0.f,
-                              inv_count, dq, y_out, loss_out, stream);
+                              inv_count, nullptr, dq, y_out, nullptr, loss_out, stream);
 }
 extern "C" int xtb_nstep_returns(const float* reward, const uint8_t* done, int n_env, int n_step, int n, float gamma, float* ret,
                                  float* disc, int32_t* last, uint8_t* done_n, void* stream) {
@@ -2087,7 +2087,7 @@ static int heads_fused(xtb_net* net, const void* obs, PpoHeadsArgs& a, int mb, i
   bool bh_pi_ok = net->L[lpi.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lpi.d.src) && !ext_pi;
   bool bh_v_ok = net->L[lv.d.src - 1].d.kind == XTB_DENSE && only_feeds_heads(lv.d.src) && !ext_v;
   a.B = mb; a.K = lpi.K; a.A = adim; a.act_pi = dgrad_act(lpi); a.act_v = dgrad_act(lv); a.shared = lpi.d.src == lv.d.src ? 1 : 0;
-  int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 1184 samples
+  int blocks = std::max(1, std::min(kSMs, (mb + 7) / 8));      // one sample per warp up to 8 * kSMs = 1056 samples
   const int HK = lpi.K, nacc = HK * adim + 3 * HK + adim + 2 + (LOSS::kLogStd ? adim : 0);
   a.part = (float*)(net->ws + net->heads_part_off); a.slab = (nacc + 3) & ~3;
   size_t shb = (size_t)8 * nacc * sizeof(float);
@@ -3754,6 +3754,19 @@ static bool dueling_fusable(const xtb_net* net, int q_tensor) {
   const LayerPlan& la = net->L[lq.d.k - 1];
   return lv.d.kind == XTB_DENSE && la.d.kind == XTB_DENSE && lv.d.act == 0 && la.d.act == 0 && lv.d.src != 0 &&
          lv.d.src == la.d.src && heads_fit(lv.K, lv.N) && !act_is_ext(lv.src_act);
+}
+
+// the heads_kernel<DuelingTdLoss> entry the DQN steps launch for q_tensor, (0, 0) when they run layer by layer
+extern "C" int xtb_dqn_heads_plan(const xtb_net* net, int q_tensor, int* kpl, int* amax) {
+  const char* fn = "xtb_dqn_heads_plan";
+  if (!net || !kpl || !amax) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
+  if (q_tensor < 1 || q_tensor > (int)net->L.size()) return fail(XTB_ERR_ARG, "%s: bad head tensor", fn);
+  *kpl = *amax = 0;
+  if (!dueling_fusable(net, q_tensor)) return XTB_OK;
+  const LayerPlan& lq = net->L[q_tensor - 1];
+  const auto* e = heads_pick(kHeadsKernels<DuelingTdLoss>, net->L[lq.d.src - 1].K, net->tsize[lq.d.src]);
+  *kpl = e->kpl; *amax = e->amax;
+  return XTB_OK;
 }
 
 // The online half of the dueling TD step in one heads_kernel launch (heads_fused with the value stream as the pi head

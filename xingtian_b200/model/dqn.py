@@ -1,4 +1,6 @@
 """DqnCnn / DqnMlp on the CUDA engine (xt/model/dqn/dqn_cnn.py:31-83, dqn_mlp.py:30-76)."""
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -76,6 +78,13 @@ class _DqnBase(XTModel):
         net.backward(b["obs"], n, [self.q_name])
         self.opt.step()
         return float(b["loss"].cpu()[0])
+
+    def heads_plan(self):
+        """(kpl, amax) of the fused dueling heads kernel the TD step launches for this model's Q head under the current
+        fused-heads mode; (0, 0) when the step runs layer by layer."""
+        kpl, amax = C.c_int(), C.c_int()
+        check(self.net.lib.xtb_dqn_heads_plan(self.net.handle, self.net.tid[self.q_name], C.byref(kpl), C.byref(amax)))
+        return kpl.value, amax.value
 
     def _td_scratch(self, target_model, n):
         self.net.ensure_batch(n)
