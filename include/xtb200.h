@@ -168,12 +168,14 @@ int xtb_net_backward(xtb_net* net, const void* obs, const int32_t* gather_idx, i
  * Philox4x32-10(seed, offset).  logp = log-softmax(logits)[action]. */
 int xtb_categorical_sample(const float* logits, int batch, int adim, const float* uniforms,
                            uint64_t seed, uint64_t offset, int32_t* action, float* logp, void* stream);
-/* argmax over the last axis (DQN greedy action, xt/algorithm/algorithm.py:124-135) */
+/* argmax over the last axis (DQN greedy action, xt/algorithm/algorithm.py:124-135): as np.argmax, the first maximum
+ * wins and the first NaN wins over any number */
 int xtb_argmax(const float* q, int batch, int adim, int32_t* action, void* stream);
 
 /* ---- GAE: replaces PPO.data_proc (xt/agent/ppo/ppo.py:77-106) ------------------- */
 /* value [E,T+1], reward [E,T], done [E,T] (uint8) -> adv, old_value, target_value [E,T].
- * sign_clip != 0 applies np.sign to rewards (xt/agent/ppo/atari_ppo.py:46). */
+ * sign_clip != 0 applies np.sign to rewards (xt/agent/ppo/atari_ppo.py:46), which keeps a NaN reward NaN.
+ * E = 0 or T = 0 is a no-op; a negative size is refused. */
 int xtb_gae(const float* value, const float* reward, const uint8_t* done, int n_env, int n_step,
             float gamma, float lam, int sign_clip, float* adv, float* old_value, float* target_value,
             void* stream);

@@ -500,6 +500,67 @@ def gae(value, reward, done, gamma=GAMMA, lam=LAM):
     return adv, value, adv + value
 
 
+def sign_clip_f32(reward):
+    """np.sign of float32 rewards written as the device clips them: +-1, +0 for either zero, NaN kept"""
+    r = np.asarray(reward, np.float32)
+    one = np.float32(1)
+    return np.where(r > 0, one, np.where(r < 0, -one, np.where(r == r, np.float32(0), r))).astype(np.float32)
+
+
+def gae_f32(value, reward, done, gamma=GAMMA, lam=LAM, sign_clip=False):
+    """gae's backward loop in plain float32 arithmetic, vectorised over rows: what fp32 rounding alone costs.
+
+    value [..., T+1] (a trailing unit axis is dropped), reward / done [..., T]; gamma and lam are rounded to float32 as a
+    C float argument carries them; sign_clip: rewards through sign_clip_f32 first.  Returns adv, old_value, target_value,
+    each float32 [..., T]."""
+    f = np.float32
+    value = np.asarray(value, f)
+    reward = np.asarray(reward, f)
+    if value.shape[-1] == 1 and value.ndim == reward.ndim + 1:
+        value = value[..., 0]
+    if sign_clip:
+        reward = sign_clip_f32(reward)
+    done = np.asarray(done, bool)
+    g, lm = f(gamma), f(lam)
+    disc = np.where(done, f(0), g)
+    delta = reward + disc * value[..., 1:] - value[..., :-1]
+    adv = np.empty_like(delta)
+    nxt = np.zeros(delta.shape[:-1], f)
+    for t in range(delta.shape[-1] - 1, -1, -1):
+        nxt = delta[..., t] + disc[..., t] * lm * nxt
+        adv[..., t] = nxt
+    return adv, value[..., :-1].copy(), adv + value[..., :-1]
+
+
+def nstep_returns(reward, done, n, gamma, dtype=np.float64):
+    """n-step returns of env-major segments [E, T] (or one segment [T]) in `dtype`, vectorised over rows: the window of
+    step t stops after its first terminal step (inclusive), after n steps or at the end of the segment, m steps in all.
+    Returns ret = sum_{k<m} gamma^k r_{t+k}, disc = gamma^m (0 when the window hit a terminal step), last = flat row index
+    e * T + t + m - 1 (the row whose next state bootstraps) and done_n (the window hit a terminal step)."""
+    f = np.dtype(dtype).type
+    r = np.asarray(reward, f)
+    d = np.asarray(done, bool)
+    shape = r.shape
+    r, d = r.reshape(-1, shape[-1]), d.reshape(-1, shape[-1])
+    E, T = r.shape
+    g = np.ones((E, T), f)
+    acc = np.zeros((E, T), f)
+    m = np.zeros((E, T), np.int64)
+    term = np.zeros((E, T), bool)
+    t = np.arange(T)
+    for k in range(min(n, T)):
+        live = ~term & (t + k < T)[None, :]          # windows still open at their k-th step
+        rk = np.zeros((E, T), f)
+        dk = np.zeros((E, T), bool)
+        rk[:, :T - k], dk[:, :T - k] = r[:, k:], d[:, k:]
+        acc = np.where(live, acc + g * rk, acc)
+        g = np.where(live, g * f(gamma), g)
+        m += live
+        term |= live & dk
+    last = np.arange(E)[:, None] * T + t[None, :] + m - 1
+    return (acc.reshape(shape), np.where(term, f(0), g).reshape(shape), last.reshape(shape), term.reshape(shape))
+
+
 # --------------------------------------------------------------------------- #
 # PPO loss / optimiser / train loop
 # --------------------------------------------------------------------------- #

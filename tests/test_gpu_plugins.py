@@ -375,22 +375,6 @@ def test_dqn_c4_config_size_step_matches_oracle():
     assert l2_rel(upd, rupd) < 5e-2
 
 
-def _nstep_ref(reward, done, n, gamma):
-    """numpy restatement of the n-step return (north_star extension; not in the reference): window stops at the first
-    terminal step (inclusive), after n steps, or at the end of the segment."""
-    T = len(reward)
-    ret = np.zeros(T, np.float64); disc = np.zeros(T, np.float64); last = np.zeros(T, np.int64); dn = np.zeros(T, bool)
-    for t in range(T):
-        acc, g, k, term = 0.0, 1.0, 0, False
-        while k < n and t + k < T:
-            acc += g * reward[t + k]; g *= gamma
-            if done[t + k]:
-                term = True; k += 1; break
-            k += 1
-        ret[t], disc[t], last[t], dn[t] = acc, (0.0 if term else g), t + k - 1, term
-    return ret, disc, last, dn
-
-
 @pytest.mark.parametrize("E,T,n", [(1, 64, 3), (5, 33, 1), (3, 40, 5)])
 def test_nstep_returns_kernel(E, T, n):
     from xingtian_b200 import capi
@@ -402,7 +386,7 @@ def test_nstep_returns_kernel(E, T, n):
     last = torch.empty(E, T, dtype=torch.int32, device="cuda"); dn = torch.empty(E, T, dtype=torch.uint8, device="cuda")
     capi.check(capi.lib().xtb_nstep_returns(_ptr(rd), _ptr(dd), E, T, n, 0.99, _ptr(ret), _ptr(disc), _ptr(last), _ptr(dn), stream_ptr()))
     for e in range(E):
-        r_ret, r_disc, r_last, r_dn = _nstep_ref(rew[e], done[e], n, 0.99)
+        r_ret, r_disc, r_last, r_dn = orc.nstep_returns(rew[e], done[e], n, 0.99)
         assert rel_err(ret[e].cpu().numpy(), r_ret) < 1e-5 and rel_err(disc[e].cpu().numpy(), r_disc, floor=1.0) < 1e-6
         np.testing.assert_array_equal(last[e].cpu().numpy() - e * T, r_last)
         np.testing.assert_array_equal(dn[e].cpu().numpy().astype(bool), r_dn)
@@ -424,7 +408,7 @@ def test_dqn_nstep_huber_step_matches_numpy():
     s = rng.integers(0, 256, (T, 84, 84, 4), dtype=np.uint8); s2 = rng.integers(0, 256, (T, 84, 84, 4), dtype=np.uint8)
     a = rng.integers(0, 4, T); r = rng.normal(0, 2, T).astype(np.float32); d = rng.random(T) < 0.1
     alg.prepare_data(dict(cur_state=s, action=a, reward=r, next_state=s2, done=d))
-    ret, disc, last, dn = _nstep_ref(r, d, 3, 0.99)
+    ret, disc, last, dn = orc.nstep_returns(r, d, 3, 0.99)
     random.seed(0)
     loss = alg.train()
     random.seed(0)

@@ -48,6 +48,10 @@ __device__ inline void block_atomic_add(float v, float* out) {
 // Each lane owns `chunk` consecutive steps; per-lane affine map (a,b): adv_in -> a*adv_in+b is
 // composed right-to-left, exclusive-scanned across lanes with shuffles, then replayed.
 // ------------------------------------------------------------------------------------------
+// np.sign of a reward, as the reference clips on the explorer: +-1, +0 for either zero, and NaN stays NaN (so a bad
+// reward reaches the advantages of its own and every earlier step, as in the reference's float64 GAE)
+__device__ __forceinline__ float sign_clip_reward(float r) { return r > 0.f ? 1.f : (r < 0.f ? -1.f : (r == r ? 0.f : r)); }
+
 __global__ void gae_kernel(const float* __restrict__ value, const float* __restrict__ reward,
                            const uint8_t* __restrict__ done, int n_env, int T, float gamma, float lam,
                            int sign_clip, float* __restrict__ adv, float* __restrict__ old_v,
@@ -68,7 +72,7 @@ __global__ void gae_kernel(const float* __restrict__ value, const float* __restr
   float a = 1.f, b = 0.f;
   for (int t = t1 - 1; t >= t0; --t) {
     float r = R[t];
-    if (sign_clip) r = (r > 0.f) ? 1.f : ((r < 0.f) ? -1.f : 0.f);
+    if (sign_clip) r = sign_clip_reward(r);
     float disc = D[t] ? 0.f : gamma;
     float delta = r + disc * V[t + 1] - V[t];
     float c = disc * lam;
@@ -94,7 +98,7 @@ __global__ void gae_kernel(const float* __restrict__ value, const float* __restr
   float nxt = incoming;
   for (int t = t1 - 1; t >= t0; --t) {
     float r = R[t];
-    if (sign_clip) r = (r > 0.f) ? 1.f : ((r < 0.f) ? -1.f : 0.f);
+    if (sign_clip) r = sign_clip_reward(r);
     float disc = D[t] ? 0.f : gamma;
     float v = V[t];
     float delta = r + disc * V[t + 1] - v;
@@ -174,7 +178,8 @@ __global__ void argmax_kernel(const float* __restrict__ q, int B, int A, int32_t
   if (b >= B) return;
   const float* l = q + (long long)b * A;
   float best = l[0]; int bi = 0;
-  for (int i = 1; i < A; i++) if (l[i] > best) { best = l[i]; bi = i; }
+  // the first maximum wins, and the first NaN over any number, as np.argmax
+  for (int i = 1; i < A; i++) if (l[i] > best || (l[i] != l[i] && best == best)) { best = l[i]; bi = i; }
   action[b] = bi;
 }
 

@@ -1596,8 +1596,8 @@ extern "C" int xtb_gae(const float* value, const float* reward, const uint8_t* d
                        float gamma, float lam, int sign_clip, float* adv, float* old_value, float* target_value,
                        void* stream) {
   if (!value || !reward || !done || !adv || !old_value || !target_value) return fail(XTB_ERR_ARG, "xtb_gae: null pointer");
-  if (n_env == 0 || n_step == 0) return XTB_OK;   // empty rollout: nothing to do
   if (n_env < 0 || n_step < 0) return fail(XTB_ERR_ARG, "xtb_gae: negative size");
+  if (n_env == 0 || n_step == 0) return XTB_OK;   // empty rollout: nothing to do
   int threads = 128;  // 4 envs per block
   int blocks = (n_env * 32 + threads - 1) / threads;
   XLAUNCH(gae_kernel, blocks, threads, 0, S(stream), value, reward, done, n_env, n_step, gamma, lam, sign_clip, adv,
