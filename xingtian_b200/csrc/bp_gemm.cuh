@@ -33,6 +33,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "bp_tables.cuh"
 #include "gemm_f32.cuh"
 
 #ifndef XTB_BP_WAIT_HINT
@@ -41,8 +42,6 @@
 
 namespace xtb {
 namespace bp {
-
-typedef __nv_bfloat16 bf16;
 
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -255,11 +254,6 @@ __device__ __forceinline__ void split8(const float v[8], uint4& hi, uint4& lo) {
 // ------------------------------------------------------------------------------------------
 // batch-planar tensor handle
 // ------------------------------------------------------------------------------------------
-struct BpT {
-  bf16* hi;            // hi plane; NULL = absent
-  long long lo_off;    // lo plane = hi + lo_off (elements)
-  int pitch;           // rows per feature chunk (multiple of 16)
-};
 __host__ __device__ inline long long bp_index(int pitch, int row, int f) { return ((long long)(f >> 3) * pitch + row) * 8 + (f & 7); }
 
 // Warp roles of both GEMM kernels: warps 0..7 are two consumer warpgroups (wgmma needs a warpgroup to start at a warp
@@ -295,12 +289,6 @@ __host__ __device__ inline int dgrad_epi_planes(int src_act, int accumulate) {
   return (src_act == 1 ? 1 : (src_act == 2 ? 2 : 0)) + (accumulate ? 2 : 0);
 }
 
-struct StageEnt {            // one K stage of a conv unit (8 bytes; the tables are copied to shared memory at kernel start)
-  uint32_t a_chunk;          // first operand feature chunk of the stage
-  uint16_t w_row;            // first weight-blob row of the stage (forward: k row; data gradient: tap * Cin)
-  uint16_t nch;              // feature chunks in this stage (even, <= 8)
-};
-typedef uint32_t UnitEnt;    // first stage index | stage count << 24
 struct StageDesc { uint32_t a_off, w_off, nch; };   // byte offsets inside a plane / blob plane
 
 struct RowsArgs {
@@ -753,12 +741,6 @@ constexpr int WG_STAGE = WG_STAGE_A + WG_STAGE_B;
 constexpr int WG_STAGES = 4;
 constexpr int WG_THREADS = BP_THREADS;
 
-struct WgEnt {               // conv: one (output pixel, accumulator) pair (8 bytes, copied to shared memory)
-  int32_t x_chunk;           // first X feature chunk of the M tile (may be negative at a padded border)
-  uint16_t okmask;           // bit c: chunk c of the tile lies inside the image and inside the filter row
-  uint16_t valid;            // the filter row exists for this pixel
-};
-
 struct WgradArgs {
   BpT x; int x_split; BpT g; const bf16* zeros;
   int mode;                                      // 0 conv, 1 dense
@@ -932,14 +914,6 @@ bp_wgrad_kernel(const __grid_constant__ WgradArgs a) {
 // ------------------------------------------------------------------------------------------
 // Ordered reduction of per-CTA partial sums into the flat gradient bucket (assignment, not accumulation).
 // ------------------------------------------------------------------------------------------
-struct RedSeg {
-  const float* part; int n_slabs; long long slab;   // slab stride (floats); element idx of the segment inside a slab
-  int count;                                         // elements of one slab that this segment covers
-  int kind;                                          // 0: conv weight partials [R][128][N]; 1: plain vector (bias)
-  int N, C, KW, mts, s2d_k4;                         // conv mapping
-  long long dst_off; float alpha;
-  float* dst_ptr;                                    // destination base instead of the gradient bucket (kind 1), or NULL
-};
 // real HWIO row of row k' = ((ty*k4 + tx)*16 + dy*4 + dx)*4 + c of the (k4 x k4, stride 1, 64 channel) conv over a
 // space-to-depth plane: ((4ty+dy)*4k4 + 4tx+dx)*4 + c of the (4k4 x 4k4, stride 4, 4 channel) conv
 __host__ __device__ inline int s2d_real_row(int m, int k4) {
@@ -1107,9 +1081,6 @@ __global__ void bp_splitk_finish_kernel(const float* __restrict__ part, int n_z,
   }
 }
 
-// Weight blobs: for every tensor-core layer the kernel matrix W[K, N] as batch-planar W^T planes
-// blob[((n >> 3) * K + k') * 8 + (n & 7)], k' = space-to-depth row order for a stride-4 first layer.
-struct BlobSeg { long long w_off, blob_off; int K, N, s2d_k4; };
 // inverse of s2d_real_row: real HWIO row -> row of the space-to-depth ordered blob
 __host__ __device__ inline int s2d_blob_row(int k, int k4) {
   const int c = k & 3, pix = k >> 2, x = pix % (4 * k4), y = pix / (4 * k4);

@@ -17,6 +17,8 @@
 
 namespace xtb {
 
+constexpr int MAX_ADIM = 32;   // widest action distribution (logits / Gaussian mean) of the RL kernels
+
 // keep the bf16 hi/lo planes of a tensor current (hi == NULL: tensor has no tensor-core consumer)
 __device__ __forceinline__ void f32_store_plane(__nv_bfloat16* hi, long long lo_off, long long e, float x) {
   if (!hi) return;
@@ -63,12 +65,18 @@ __device__ inline float act_grad_from_out(int act, float y) {
   return 1.f;
 }
 
+__device__ inline float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // ------------------------------------------------------------------------------------------
 // The activations past tanh (enum xtb_act, include/xtb200.h).  The GEMM epilogues above and in bp_gemm.cuh apply only
 // relu / tanh / linear: code for the others in their unrolled bodies slowed every network (instruction fetch, register
-// pressure).  A layer with one of these runs its GEMM linear into fp32 and act_fwd_kernel applies the activation; the
-// data gradients into its tensor are taken wrt its output y, and act_bwd_kernel turns their sum into the gradient wrt
-// the pre-activation before the layer's own backward.
+// pressure).  A layer with one of these runs its GEMM linear into fp32 and act_fwd_kernel (layer_kernels.cuh) applies
+// the activation; the data gradients into its tensor are taken wrt its output y, and act_bwd_kernel turns their sum
+// into the gradient wrt the pre-activation before the layer's own backward.
 // ------------------------------------------------------------------------------------------
 constexpr float kLeakyAlpha = 0.2f;
 constexpr float kSeluScale = 1.0507009873554805f, kSeluAlpha = 1.6732632423543772f;
@@ -109,44 +117,6 @@ __device__ inline float act_grad_ext(int act, float u) {
       return 0.5f * (1.f + t) + 0.5f * u * (1.f - t * t) * kGeluC * (1.f + 3.f * kGeluA * u * u);
     }
     default: return 1.f;
-  }
-}
-
-// y[i] = act(pre[i]) over n floats (pre may be y itself)
-__global__ void act_fwd_kernel(const float* pre, long long n, int act, float* y) {
-  pdl_wait(); pdl_trigger();
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    y[i] = act_apply_ext(act, pre[i]);
-}
-// g *= act'(u) over rows x N (u: z or y, act_grad_ext): the gradient wrt the output becomes the gradient wrt the
-// pre-activation.  Also the layer's bias gradient, without atomics: block b takes a fixed run of rows, its row lanes
-// add in a fixed order, and part[b][N] is left for the ordered reduction (bp::grad_reduce_kernel).
-constexpr int ACT_BWD_BLOCKS = 132, ACT_BWD_THREADS = 256;
-__global__ void __launch_bounds__(ACT_BWD_THREADS) act_bwd_kernel(float* __restrict__ g, const float* __restrict__ u, int rows,
-                                                                  int N, int act, float* __restrict__ part) {
-  pdl_wait(); pdl_trigger();
-  __shared__ float red[ACT_BWD_THREADS];
-  const int rpb = (rows + gridDim.x - 1) / gridDim.x, r0 = blockIdx.x * rpb, r1 = min(rows, r0 + rpb);
-  const int W = min(N, ACT_BWD_THREADS), R = ACT_BWD_THREADS / W;      // columns per pass, row lanes
-  const int rr = threadIdx.x / W;
-  for (int c0 = 0; c0 < N; c0 += W) {
-    const int c = c0 + threadIdx.x % W;
-    float s = 0.f;
-    if (rr < R && c < N)
-      for (int r = r0 + rr; r < r1; r += R) {
-        const long long e = (long long)r * N + c;
-        const float v = g[e] * act_grad_ext(act, u[e]);
-        g[e] = v;
-        s += v;
-      }
-    red[threadIdx.x] = s;
-    __syncthreads();
-    if (rr == 0 && c < N) {
-      float t = red[threadIdx.x];
-      for (int k = 1; k < R; k++) t += red[k * W + threadIdx.x];
-      part[(long long)blockIdx.x * N + c] = t;
-    }
-    __syncthreads();
   }
 }
 

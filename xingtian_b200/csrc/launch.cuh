@@ -14,7 +14,7 @@ namespace xtb {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-static int g_pdl = [] { const char* e = getenv("XTB_PDL"); return e ? atoi(e) : 1; }();
+inline int g_pdl = [] { const char* e = getenv("XTB_PDL"); return e ? atoi(e) : 1; }();
 
 template <class... KArgs, class... Args>
 static inline cudaError_t pdl_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {

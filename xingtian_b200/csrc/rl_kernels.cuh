@@ -8,7 +8,6 @@
 //   nstep_kernel              : n-step returns of a device-resident rollout buffer
 //   heads_kernel<LOSS>        : both dense heads + the per-sample loss of LOSS + their backward, one warp per sample
 //   infer_heads_kernel<DIST>  : both dense heads + the draw of DIST (rollout inference), one warp per sample
-//   dueling_fwd / dgrad       : the dueling combine layer
 //   IMPALA Keras, MuZero      : softmax_rows, impala_keras_*, mse_loss; mz_*
 // The per-sample rules (categorical_draw / gaussian_draw, ppo_categorical_row, ppo_gauss_row, dqn_td_target / td_loss)
 // are written once: the standalone kernels of the layer-by-layer path and the fused heads kernels both call them.
@@ -19,14 +18,6 @@
 #include "gemm_f32.cuh"
 
 namespace xtb {
-
-constexpr int MAX_ADIM = 32;
-
-__device__ inline float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // block-level sum -> one atomicAdd per block
 __device__ inline void block_atomic_add(float v, float* out) {
@@ -679,42 +670,6 @@ __global__ void __launch_bounds__(256) heads_kernel(PpoHeadsArgs a) {
     float t = sh_dw[e];
     for (int w = 1; w < nwarp; w++) t += sh_dw[(size_t)w * nacc + e];
     out[e] = t;
-  }
-}
-
-// Dueling combine layer (XTB_DUELING), one warp per sample: q = adv + (value - mean_a value) (xt/model/dqn/dqn_mlp.py:80-87)
-__global__ void __launch_bounds__(256) dueling_fwd_kernel(const float* __restrict__ value, const float* __restrict__ adv, int B, int A,
-                                                          float* __restrict__ q) {
-  pdl_wait(); pdl_trigger();
-  const int lane = threadIdx.x & 31, b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (b >= B) return;
-  const float* v = value + (long long)b * A;
-  float s = 0.f;
-  for (int i = lane; i < A; i += 32) s += v[i];
-  const float mean = warp_sum(s) / A, ad = adv[b];
-  for (int i = lane; i < A; i += 32) q[(long long)b * A + i] = ad + (v[i] - mean);
-}
-// Its data gradient, g = dloss/dq: gvalue = (g - mean_a g) * act'(value), gadv = sum_a g * act'(adv), written or, when
-// acc_v / acc_a is set, added to what another consumer of that tensor already wrote.
-__global__ void __launch_bounds__(256) dueling_dgrad_kernel(const float* __restrict__ g, const float* __restrict__ value,
-                                                            const float* __restrict__ adv, int B, int A, int act_v, int act_a,
-                                                            int acc_v, int acc_a, float* __restrict__ gvalue, float* __restrict__ gadv) {
-  pdl_wait(); pdl_trigger();
-  const int lane = threadIdx.x & 31, b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (b >= B) return;
-  const float* gr = g + (long long)b * A;
-  float s = 0.f;
-  for (int i = lane; i < A; i += 32) s += gr[i];
-  s = warp_sum(s);
-  const float mean = s / A;
-  for (int i = lane; i < A; i += 32) {
-    const long long e = (long long)b * A + i;
-    const float r = (gr[i] - mean) * act_grad_from_out(act_v, value[e]);
-    gvalue[e] = acc_v ? gvalue[e] + r : r;
-  }
-  if (lane == 0) {
-    const float r = s * act_grad_from_out(act_a, adv[b]);
-    gadv[b] = acc_a ? gadv[b] + r : r;
   }
 }
 
