@@ -648,6 +648,8 @@ typedef struct xtb_qmix_desc {
   int32_t use_double_q;
   float gamma;
   long long gru_off;      /* offset (floats) of gates/kernel in a weight set */
+  int32_t act_envs;       /* most environments one xtb_qmix_act call steps (0: one); fc1 and fc2 must hold act_envs
+                             n_agents rows */
 } xtb_qmix_desc;
 int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyper, const xtb_qmix_desc* desc, xtb_qmix** out);
 void xtb_qmix_destroy(xtb_qmix* q);
@@ -677,6 +679,25 @@ int xtb_qmix_train(xtb_qmix* q, xtb_adam* opt, const float* target, const xtb_qm
  * `explore` on obs [n_agents, obs_dim]; hidden [n_agents, H] is read as the state and overwritten with the new one;
  * q_out [n_agents, A]. */
 int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream);
+/* QMixAlg.predict_with_selector for n_envs environments at once (1 <= n_envs <= act_envs), as one launch sequence:
+ *   - the agent inputs of build_inputs for one step: obs [n_envs, n_agents, o] (o = fc1's width less n_actions with
+ *     obs_last_action, less n_agents with obs_agent_id), then the one-hot of last_action [n_envs, n_agents] (zeros for
+ *     a value < 0), then the one-hot of the agent;
+ *   - an environment whose reset [n_envs] flag is non-zero starts from zero hidden rows and no last action (its
+ *     last_action rows become -1 before the inputs are read);
+ *   - fc1 -> one GRU step -> fc2 of the weight set `explore` on the n_envs n_agents rows, hidden [n_envs, n_agents, H]
+ *     read and overwritten; the Q values stay in fc2's output tensor (rows e n_agents + a);
+ *   - EpsilonGreedyActionSelector.select_action per row: avail [n_envs, n_agents, A] int32 action weights (< 1e-6:
+ *     unavailable), epsilon [n_envs] float64; the action is np.random.choice(A, p=avail/sum) for u1 if u0 < epsilon,
+ *     else the first argmax of the masked Q (agent_act.cuh states the rule).  (u0, u1) = uniforms[e, 0, a] and
+ *     uniforms[e, 1, a] (float64 [n_envs, 2, n_agents]); with uniforms NULL they are 53-bit uniforms of Philox4x32-10
+ *     keyed by seed on counter (a, e, counter[e]), counter [n_envs] uint64 in device memory advancing by one per call.
+ * actions [n_envs, n_agents] int32 and last_action get the chosen actions.  Every array is a device array.  A row
+ * without a positive weight gets an action that means nothing.  XTB_ERR_ARG before any launch for a null pointer (counter
+ * only when uniforms is NULL), n_envs outside [1, act_envs] or no room for the observation in fc1's inputs. */
+int xtb_qmix_act(xtb_qmix* q, const float* explore, int n_envs, int obs_last_action, int obs_agent_id, const float* obs,
+                 const int32_t* avail, const int32_t* reset, const double* epsilon, const double* uniforms, unsigned long long seed,
+                 unsigned long long* counter, float* hidden, int32_t* last_action, int32_t* actions, int use_graph, void* stream);
 
 /* ---- SCC: replaces SCCModel's train and explore graphs (xt/model/scc/scc_tf.py:195-707) -----------------------------
  * The agent network and its explore step are QMIX's (above): fc1 / GRU / fc2 in the same layout, with the same limits
@@ -707,6 +728,7 @@ typedef struct xtb_scc_desc {
   float gamma;
   long long gru_off;        /* offset (floats) of gates/kernel in a weight set */
   long long head_off;       /* offset (floats) of the critic head's kernel */
+  int32_t act_envs;         /* as xtb_qmix_desc's */
 } xtb_scc_desc;
 /* critic: n_groups nets (1 when n_groups = 0) */
 int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic, const xtb_scc_desc* desc, xtb_scc** out);
@@ -740,6 +762,10 @@ int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_opt, const f
                   float* loss_out, int use_graph, void* stream);
 /* SCCModel.infer_actions: as xtb_qmix_infer. */
 int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream);
+/* SCC's acting: as xtb_qmix_act. */
+int xtb_scc_act(xtb_scc* q, const float* explore, int n_envs, int obs_last_action, int obs_agent_id, const float* obs,
+                const int32_t* avail, const int32_t* reset, const double* epsilon, const double* uniforms, unsigned long long seed,
+                unsigned long long* counter, float* hidden, int32_t* last_action, int32_t* actions, int use_graph, void* stream);
 /* SCCModel.get_mixer_output (scc_tf.py:500-503): v_out[r] = V_eval(states[r]) for states [rows, n_agents D], rows <= B L. */
 int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream);
 

@@ -364,6 +364,9 @@ class QMixAlg(Algorithm):
         }
         self.obs_shape = self._get_input_shape(alg_config, self.scheme)
         model_info["actor"]["model_config"]["obs_shape"] = self.obs_shape
+        # the model's acting assembles the inputs as build_inputs does
+        model_info["actor"]["model_config"]["obs_last_action"] = bool(alg_config["obs_last_action"])
+        model_info["actor"]["model_config"]["obs_agent_id"] = bool(alg_config["obs_agent_id"])
         model_info["actor"].update({"scene": kwargs.get("scene", "train")})
         super().__init__(alg_name="QMixAlg", model_info=model_info["actor"], alg_config=alg_config)
         self.async_flag = False
@@ -414,6 +417,31 @@ class QMixAlg(Algorithm):
         avail_actions = ep_batch["avail_actions"][:, t_ep]
         out_val = self.actor.infer_actions(self.build_inputs(ep_batch, t_ep))
         return self.selector.select_action(out_val, avail_actions, t_env, test_mode=test_mode)
+
+    def predict_with_selector_envs(self, obs, avail, reset, t_env, test_mode, uniforms=None):
+        """predict_with_selector for N environments in one device call (the model's act, environment e in slot e) ->
+        int32 actions [N, n_agents].  obs [N, n_agents, obs_shape] and avail [N, n_agents, n_actions] are the step's
+        observations and available actions; reset [N] marks the environments whose episode starts at this step (the
+        t_ep == 0 of build_inputs and reset_hidden_state).  Epsilon follows the selector's schedule per environment (t_env
+        a scalar or [N]), 0 in test mode; selector.epsilon is left as the host selector would leave it after the last
+        environment.  uniforms: [N, 2, n_agents] float64 (selector_uniforms draws the host selector's numbers), or None
+        for Philox draws on the device."""
+        N = np.shape(obs)[0]
+        t = np.broadcast_to(np.asarray(t_env), (N,))
+        eps = np.zeros(N) if test_mode else np.array([self.selector.schedule.eval(x) for x in t], np.float64)
+        self.selector.epsilon = 0.0 if test_mode else self.selector.schedule.eval(t[-1])
+        return self.actor.act(obs, avail, reset, eps, uniforms)
+
+    @staticmethod
+    def selector_uniforms(N, n_agents):
+        """The uniforms EpsilonGreedyActionSelector.select_action draws from the global np.random stream, one
+        environment after another -> float64 [N, 2, n_agents]: per environment n_agents rand values (the epsilon tests),
+        then one per agent row for np.random.choice (which draws one random_sample and inverts the CDF)."""
+        out = np.empty((N, 2, n_agents), np.float64)
+        for e in range(N):
+            out[e, 0] = np.random.rand(1, n_agents)[0]
+            out[e, 1] = [np.random.random_sample() for _ in range(n_agents)]
+        return out
 
     def save(self, model_path, model_index):
         """The explore agent's weights under model_path/actor<index>."""

@@ -72,7 +72,7 @@ class MuzeroReplayBatch(C.Structure):
 
 class QmixDesc(C.Structure):
     _fields_ = [("batch", C.c_int32), ("episode_limit", C.c_int32), ("n_agents", C.c_int32), ("use_double_q", C.c_int32),
-                ("gamma", C.c_float), ("gru_off", C.c_longlong)]
+                ("gamma", C.c_float), ("gru_off", C.c_longlong), ("act_envs", C.c_int32)]
 
 
 class QmixBatch(C.Structure):
@@ -83,7 +83,7 @@ class QmixBatch(C.Structure):
 class SccDesc(C.Structure):
     _fields_ = [("batch", C.c_int32), ("episode_limit", C.c_int32), ("n_agents", C.c_int32), ("n_groups", C.c_int32),
                 ("group", C.c_int32 * 8), ("channel_merge", C.c_int32), ("mc_sample_times", C.c_int32), ("gamma", C.c_float),
-                ("gru_off", C.c_longlong), ("head_off", C.c_longlong)]
+                ("gru_off", C.c_longlong), ("head_off", C.c_longlong), ("act_envs", C.c_int32)]
 
 
 class SccBatch(C.Structure):
@@ -207,10 +207,12 @@ _SIGS = {
     "xtb_qmix_destroy": (None, [_P]),
     "xtb_qmix_train": (C.c_int, [_P, _P, _P, C.POINTER(QmixBatch), _P, C.c_int, _P]),
     "xtb_qmix_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_qmix_act": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_scc_create": (C.c_int, [_P, _P, C.POINTER(_P), C.POINTER(SccDesc), C.POINTER(_P)]),
     "xtb_scc_destroy": (None, [_P]),
     "xtb_scc_train": (C.c_int, [_P, _P, _P, _P, C.POINTER(SccBatch), _P, C.c_int, _P]),
     "xtb_scc_infer": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P]),
+    "xtb_scc_act": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_uint64, _P, _P, _P, _P, C.c_int, _P]),
     "xtb_scc_critic": (C.c_int, [_P, _P, C.c_int, _P, C.c_int, _P]),
     "xtb_episode_replay_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "xtb_episode_replay_destroy": (None, [_P]),

@@ -252,7 +252,7 @@ struct StreamScope {
 enum GraphTag { kPpoTrain = 1, kImpalaTrain, kDqnTrain, kRolloutInfer, kImpalaKerasFit, kImpalaKerasTrain, kMuzeroTrain,
                 kMuzeroInitInfer, kMuzeroRecurInfer, kMuzeroSearch, kQmixTrain, kQmixInfer,
                 kSccTrain, kSccInfer, kSccCritic, kDqnTrainWeighted, kDqnPerTrain, kInfoflowTrain, kInfoflowPredict, kMuzeroReplayTrain,
-                kQmixReplayTrain, kSccReplayTrain };
+                kQmixReplayTrain, kSccReplayTrain, kQmixAct, kSccAct };
 struct CaptureKey {
   uint64_t tag;          // entry point
   const void* own[7];    // the objects the capture reads (nets, optimiser, ...) and the communicator (own[6]):

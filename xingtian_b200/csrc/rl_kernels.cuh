@@ -16,6 +16,7 @@
 #include <stdint.h>
 
 #include "gemm_f32.cuh"
+#include "philox.cuh"
 
 namespace xtb {
 
@@ -98,20 +99,6 @@ __global__ void gae_kernel(const float* __restrict__ value, const float* __restr
     OV[t] = v;
     TV[t] = ad + v;
     nxt = ad;
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Philox4x32-10
-// ------------------------------------------------------------------------------------------
-__device__ inline void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int i = 0; i < 10; i++) {
-    uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-    uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-    uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
 }
 

@@ -13,6 +13,7 @@
 #include "layer_kernels.cuh"
 #include "optim.cuh"
 #include "qmix.cuh"
+#include "agent_act.cuh"
 #include "scc.cuh"
 #include "episode_replay.cuh"
 #include "infoflow.cuh"
@@ -1601,14 +1602,16 @@ int learner_check(const char* fn, bool missing, const xtb_net* net, const xtb_ad
 // fc1 and fc2 are engine nets bound to the slices [fc1 | gru | fc2] at the front of their object's eval weight set, the
 // GRU's kernels and biases at o_gru; other weight sets are read through the nets' foreign-parameter forward.  A training
 // batch is B episodes of T = L + 1 steps of n agents: R = B T n agent rows, BL = B L steps and S = B n GRU sequences, G
-// of them per CTA of the GRU kernels with smem bytes of shared memory.
+// of them per CTA of the GRU kernels with smem bytes of shared memory.  Acting steps up to E environments at once (E n
+// rows of one step each, agent_act): the forward's scratch holds max(R, E n) rows.
 struct QmixAgent {
   xtb_net *fc1 = nullptr, *fc2 = nullptr;
-  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, R = 0, BL = 0, S = 0, G = 0;
+  int B = 0, L = 0, T = 0, n = 0, A = 0, H = 0, R = 0, BL = 0, S = 0, G = 0, E = 1;
   size_t smem = 0;
   long long o_gru = 0, o_fc2 = 0;
   float *xg = nullptr, *xc = nullptr, *hout = nullptr, *rh = nullptr, *dy = nullptr, *dag = nullptr, *dac = nullptr;
-  int32_t* ones = nullptr;   // [n] sequence lengths of the one-step inference
+  float* xin = nullptr;      // [E n, fc1 input width] the acting inputs
+  int32_t* ones = nullptr;   // [E n] sequence lengths of the one-step inference and of acting
 };
 
 // layer i of nt is a dense layer on tensor src with activation act
@@ -1617,10 +1620,19 @@ static bool dense_layer(const xtb_net* nt, int i, int src, int act) {
   return lp.d.kind == XTB_DENSE && lp.d.src == src && lp.d.act == act;
 }
 
+// Sequences per CTA of the GRU kernels for S sequences of width H: enough to cover S in one wave of CTAs, at most 8,
+// fewer while their shared memory would not fit
+static int gru_group(long long S, int H) {
+  int G = (int)std::max(1LL, std::min(8LL, (S + kSMs - 1) / kSMs));
+  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
+  return G;
+}
+
 // The agent's checks and sizes for `batch` episodes of `episode_limit` steps of `n_agents` agents with the GRU at gru_off,
-// into *a: all of them but the nets' row capacity (agent_capacity), which the caller checks after its own size bounds.
+// acting for up to act_envs environments (0: one), into *a: all of them but the nets' row capacity (agent_capacity),
+// which the caller checks after its own size bounds.
 static int agent_plan(const char* fn, xtb_net* fc1, xtb_net* fc2, int batch, int episode_limit, int n_agents, long long gru_off,
-                      QmixAgent* a) {
+                      int act_envs, QmixAgent* a) {
   for (xtb_net* nt : {fc1, fc2})
     if (!nt->ws || !nt->params || !nt->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
   if (fc1->L.size() != 1 || !dense_layer(fc1, 0, 0, XTB_ACT_RELU) || fc1->desc.input_u8 || fc1->desc.scale != 1.f)
@@ -1635,9 +1647,9 @@ static int agent_plan(const char* fn, xtb_net* fc1, xtb_net* fc2, int batch, int
   if (batch < 1 || episode_limit < 1) return fail(XTB_ERR_ARG, "%s: batch %d / episode_limit %d out of range", fn, batch, episode_limit);
   const long long T = episode_limit + 1LL, R = batch * T * n;
   if (R > (1LL << 30) / std::max(3 * H, 1)) return fail(XTB_ERR_ARG, "%s: batch too large", fn);
-  const int S = batch * n;
-  int G = std::max(1, std::min(8, (S + kSMs - 1) / kSMs));
-  while (G > 1 && qgru_smem_floats(H, G) * 4 > kMaxDynSmem) G--;
+  if (act_envs < 0 || (long long)act_envs * n > (1LL << 30) / std::max(3 * H, std::max(fc1->tsize[0], 1)))
+    return fail(XTB_ERR_ARG, "%s: act_envs %d out of range", fn, act_envs);
+  const int S = batch * n, G = gru_group(S, H);
   if (H < 1 || qgru_smem_floats(H, G) * 4 > kMaxDynSmem)
     return fail(XTB_ERR_ARG, "%s: rnn_hidden_dim %d: the GRU weights do not fit in shared memory", fn, H);
   // the gradients at the same offsets as the weights
@@ -1646,14 +1658,17 @@ static int agent_plan(const char* fn, xtb_net* fc1, xtb_net* fc2, int batch, int
     return fail(XTB_ERR_ARG, "%s: nets must be bound to slices [fc1 | gru | fc2] at the front of one buffer, in order", fn);
   a->fc1 = fc1; a->fc2 = fc2;
   a->B = batch; a->L = episode_limit; a->T = (int)T; a->n = n; a->A = A; a->H = H; a->R = (int)R; a->BL = batch * episode_limit;
-  a->S = S; a->G = G; a->smem = qgru_smem_floats(H, G) * 4;
+  a->S = S; a->G = G; a->smem = qgru_smem_floats(H, G) * 4; a->E = std::max(act_envs, 1);
   a->o_gru = gru_off; a->o_fc2 = o_fc2;
   return XTB_OK;
 }
 
-// fc1 and fc2 hold the R rows of a training batch
+// fc1 and fc2 hold the R rows of a training batch and the E n rows of acting
 static int agent_capacity(const char* fn, const QmixAgent& a) {
   if (a.fc1->max_batch < a.R || a.fc2->max_batch < a.R) return fail(XTB_ERR_ARG, "%s: fc1 / fc2 hold fewer rows than a batch (%d)", fn, a.R);
+  const long long act_rows = (long long)a.E * a.n;
+  if (a.fc1->max_batch < act_rows || a.fc2->max_batch < act_rows)
+    return fail(XTB_ERR_ARG, "%s: fc1 / fc2 hold fewer rows than act_envs x n_agents (%lld)", fn, act_rows);
   return XTB_OK;
 }
 
@@ -1668,13 +1683,14 @@ static int gru_kernel_attrs(const char* fn) {
 }
 
 // The GRU kernels' shared-memory opt-in, then the object's scratch in one carve_scratch into *buf: the agent's pieces,
-// with the one-step inference's sequence lengths, before the object's own `pieces`.  On failure nothing stays allocated.
+// with the acting inputs and the one-step sequence lengths, before the object's own `pieces`.  On failure nothing stays
+// allocated.
 static int agent_alloc(const char* fn, QmixAgent& a, void** buf, std::vector<Piece> pieces) {
   if (int rc = gru_kernel_attrs(fn)) return rc;
-  const long long R = a.R, H = a.H;
-  const std::vector<int32_t> ones(a.n, 1);
-  pieces.insert(pieces.begin(), {{&a.xg, R * 2 * H}, {&a.xc, R * H}, {&a.hout, R * H}, {&a.rh, R * H}, {&a.dy, R * H},
-                                 {&a.dag, R * 2 * H}, {&a.dac, R * H}, {&a.ones, a.n, ones.data()}});
+  const long long R = a.R, H = a.H, En = (long long)a.E * a.n, F = std::max(R, En);
+  const std::vector<int32_t> ones(En, 1);
+  pieces.insert(pieces.begin(), {{&a.xg, F * 2 * H}, {&a.xc, F * H}, {&a.hout, F * H}, {&a.rh, R * H}, {&a.dy, R * H},
+                                 {&a.dag, R * 2 * H}, {&a.dac, R * H}, {&a.xin, En * a.fc1->tsize[0]}, {&a.ones, En, ones.data()}});
   return carve_scratch(fn, buf, pieces);
 }
 
@@ -1757,6 +1773,39 @@ static int agent_infer(const char* fn, GraphTag tag, const void* const (&owners)
                    [&](void* st) { return qmix_agent_step(a, explore, obs, hidden, q_out, S(st)); });
 }
 
+// xtb_qmix_act and xtb_scc_act: one step of n_envs environments of object obj (agent_act.cuh), graph-replayed under the
+// object's tag and owners.  The GRU runs the n_envs n sequences with the sequences per CTA gru_group picks for them.
+template <size_t N>
+static int agent_act(const char* fn, GraphTag tag, const void* const (&owners)[N], const void* obj, QmixAgent& a, const float* explore,
+                     int n_envs, int last_on, int id_on, const float* obs, const int32_t* avail, const int32_t* reset, const double* eps,
+                     const double* uniforms, unsigned long long seed, unsigned long long* counter, float* hidden, int32_t* last_action,
+                     int32_t* actions, int use_graph, void* stream) {
+  const bool missing = !explore || !obs || !avail || !reset || !eps || !hidden || !last_action || !actions || (!uniforms && !counter);
+  if (int rc = learner_check(fn, missing, a.fc1, nullptr, 1, true)) return rc;
+  if (n_envs < 1 || n_envs > a.E) return fail(XTB_ERR_ARG, "%s: n_envs %d not in [1, %d] (act_envs)", fn, n_envs, a.E);
+  const int W = a.fc1->tsize[0], o = W - (last_on ? a.A : 0) - (id_on ? a.n : 0);
+  if (o < 1) return fail(XTB_ERR_ARG, "%s: fc1's %d inputs leave no room for the observation", fn, W);
+  last_on = last_on ? 1 : 0; id_on = id_on ? 1 : 0;
+  return run_graph(capture_key(tag, owners, obj, explore, n_envs, last_on, id_on, obs, avail, reset, eps, uniforms, seed, counter, hidden,
+                               last_action, actions),
+                   use_graph, stream, [&](void* sv) -> int {
+    cudaStream_t st = S(sv);
+    const int n = a.n, H = a.H, rows = n_envs * n;
+    const long long work = (long long)rows * std::max(W, H);
+    XLAUNCH(agent_act_inputs_kernel, (unsigned)std::min<long long>((work + AA_THREADS - 1) / AA_THREADS, 8LL * kSMs), AA_THREADS, 0, st,
+            obs, reset, last_action, hidden, uniforms ? nullptr : counter, a.xin, n_envs, n, o, a.A, H, last_on, id_on);
+    LAUNCH_CHECK();
+    QmixAgent b = a;
+    b.G = gru_group(rows, H);
+    b.smem = qgru_smem_floats(H, b.G) * 4;
+    if (int rc = qmix_agent_forward(b, explore, a.xin, rows, 1, a.ones, hidden, hidden, 0, st)) return rc;
+    XLAUNCH(agent_act_select_kernel, (rows + AA_THREADS - 1) / AA_THREADS, AA_THREADS, 0, st, (const float*)xtb_net_tensor(a.fc2, 1), avail,
+            eps, uniforms, seed, (const unsigned long long*)counter, actions, last_action, n_envs, n, a.A);
+    LAUNCH_CHECK();
+    return XTB_OK;
+  });
+}
+
 // ---- QMIX (xt/model/qmix/qmix_tf.py) ----------------------------------------------------------------------------------
 // The agent and the hypernetworks, an engine net bound to the slice after fc2 of the eval weight set; target and explore
 // sets are read through the nets' foreign-parameter forward.  The object owns the step's device scratch for the fixed
@@ -1778,7 +1827,7 @@ extern "C" int xtb_qmix_create(xtb_net* fc1, xtb_net* fc2, xtb_net* hyp, const x
   if (!fc1 || !fc2 || !hyp || !desc || !out) return fail(XTB_ERR_ARG, "%s: null pointer", fn);
   const xtb_qmix_desc& d = *desc;
   QmixAgent ag;
-  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, d.n_agents, d.gru_off, &ag)) return rc;
+  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, d.n_agents, d.gru_off, d.act_envs, &ag)) return rc;
   if (!hyp->ws || !hyp->params || !hyp->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
   if (hyp->L.size() != 7 || !dense_layer(hyp, 0, 0, XTB_ACT_RELU) || !dense_layer(hyp, 1, 1, XTB_ACT_NONE) ||
       !dense_layer(hyp, 2, 0, XTB_ACT_NONE) || !dense_layer(hyp, 3, 0, XTB_ACT_RELU) || !dense_layer(hyp, 4, 4, XTB_ACT_NONE) ||
@@ -1880,6 +1929,15 @@ extern "C" int xtb_qmix_infer(xtb_qmix* q, const float* explore, const float* ob
                      stream);
 }
 
+extern "C" int xtb_qmix_act(xtb_qmix* q, const float* explore, int n_envs, int obs_last_action, int obs_agent_id, const float* obs,
+                            const int32_t* avail, const int32_t* reset, const double* epsilon, const double* uniforms,
+                            unsigned long long seed, unsigned long long* counter, float* hidden, int32_t* last_action, int32_t* actions,
+                            int use_graph, void* stream) {
+  if (!q) return fail(XTB_ERR_ARG, "xtb_qmix_act: null object");
+  return agent_act("xtb_qmix_act", kQmixAct, {q->ag.fc1, q->ag.fc2, q->hyp, q}, q, q->ag, explore, n_envs, obs_last_action, obs_agent_id,
+                   obs, avail, reset, epsilon, uniforms, seed, counter, hidden, last_action, actions, use_graph, stream);
+}
+
 // ---- SCC (xt/model/scc/scc_tf.py) ------------------------------------------------------------------------------------
 // The agent is QMIX's; the critic's hidden layers are engine nets, one per agent group (multi-channel) or one over the
 // whole row, bound to slices of the eval set after fc2; the target critic is read through their foreign-parameter
@@ -1935,7 +1993,7 @@ extern "C" int xtb_scc_create(xtb_net* fc1, xtb_net* fc2, xtb_net* const* critic
     return fail(XTB_ERR_ARG, "%s: channel_merge %d is neither concat (0) nor add (1)", fn, d.channel_merge);
   if (n > 2 && d.mc_sample_times < 1) return fail(XTB_ERR_ARG, "%s: mc_sample_times %d < 1", fn, d.mc_sample_times);
   QmixAgent ag;
-  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, n, d.gru_off, &ag)) return rc;
+  if (int rc = agent_plan(fn, fc1, fc2, d.batch, d.episode_limit, n, d.gru_off, d.act_envs, &ag)) return rc;
   for (int j = 0; j < ncn; j++)
     if (!critic[j] || !critic[j]->ws || !critic[j]->params || !critic[j]->grads) return fail(XTB_ERR_STATE, "%s: every net must be bound", fn);
   const int A = ag.A;
@@ -2087,6 +2145,15 @@ extern "C" int xtb_scc_train(xtb_scc* q, xtb_adam* critic_opt, xtb_adam* actor_o
 extern "C" int xtb_scc_infer(xtb_scc* q, const float* explore, const float* obs, float* hidden, float* q_out, int use_graph, void* stream) {
   if (!q) return fail(XTB_ERR_ARG, "xtb_scc_infer: null object");
   return agent_infer("xtb_scc_infer", kSccInfer, {q->ag.fc1, q->ag.fc2, q}, q, q->ag, explore, obs, hidden, q_out, use_graph, stream);
+}
+
+extern "C" int xtb_scc_act(xtb_scc* q, const float* explore, int n_envs, int obs_last_action, int obs_agent_id, const float* obs,
+                           const int32_t* avail, const int32_t* reset, const double* epsilon, const double* uniforms,
+                           unsigned long long seed, unsigned long long* counter, float* hidden, int32_t* last_action, int32_t* actions,
+                           int use_graph, void* stream) {
+  if (!q) return fail(XTB_ERR_ARG, "xtb_scc_act: null object");
+  return agent_act("xtb_scc_act", kSccAct, {q->ag.fc1, q->ag.fc2, q}, q, q->ag, explore, n_envs, obs_last_action, obs_agent_id, obs,
+                   avail, reset, epsilon, uniforms, seed, counter, hidden, last_action, actions, use_graph, stream);
 }
 
 extern "C" int xtb_scc_critic(xtb_scc* q, const float* states, int rows, float* v_out, int use_graph, void* stream) {

@@ -4,8 +4,8 @@ The reference builds five TF sub-graphs: the explore agent (one step, hidden sta
 target agents over whole episodes, and the eval and target mixers.  Here a weight set is one flat buffer
 [fc1 | GRU | fc2 | mixer] in the TF variable order of the eval_agent and eval_mixer scopes: the eval set is the one the
 engine nets (fc1, fc2 and the hypernetworks) are bound to and the optimiser steps, the target set and the explore agent
-are buffers of the same layout.  The training step (xtb_qmix_train) and the one-step inference (xtb_qmix_infer) run in
-libxtb200."""
+are buffers of the same layout.  The training step (xtb_qmix_train), the one-step inference (xtb_qmix_infer) and the
+acting of up to act_envs environments per call (xtb_qmix_act) run in libxtb200."""
 import ctypes as C
 import math
 import os
@@ -36,7 +36,7 @@ class QMixModel(XTModel):
     SCCModel shares the agent: its config fields, nets and variable table, its weight sets, the explore step and the
     native object's lifetime (the entry points named by _native)."""
 
-    _native = "xtb_qmix"   # the native object's entry points: <_native>_infer and <_native>_destroy
+    _native = "xtb_qmix"   # the native object's entry points: <_native>_infer, <_native>_act and <_native>_destroy
 
     def __init__(self, model_info):
         model_config = self._agent_config(model_info)
@@ -62,6 +62,12 @@ class QMixModel(XTModel):
         self.avail_action_num = self.n_actions
         self.state_dim = int(np.prod(model_config["state_shape"]))
         self.g_type = model_info.get("scene", "explore")
+        # acting (act): environment slots, and which one-hots build_inputs appends to the observation
+        self.act_envs = int(model_config.get("act_envs", 1))
+        if self.act_envs < 1:
+            raise ValueError("act_envs must be >= 1, got {}".format(self.act_envs))
+        self.obs_last_action = bool(model_config.get("obs_last_action", False))
+        self.obs_agent_id = bool(model_config.get("obs_agent_id", False))
         return model_config
 
     # ---- construction ---------------------------------------------------------------------------------------------
@@ -95,6 +101,7 @@ class QMixModel(XTModel):
         desc = capi.QmixDesc()
         desc.batch, desc.episode_limit, desc.n_agents = B, L, n
         desc.use_double_q, desc.gamma, desc.gru_off = int(self.use_double_q), float(self.gamma), self.gru_off
+        desc.act_envs = self.act_envs
         self.handle = C.c_void_p()
         with torch.cuda.device(dev):
             check(capi.lib().xtb_qmix_create(self.fc1.handle, self.fc2.handle, self.hyper.handle, C.byref(desc), C.byref(self.handle)))
@@ -103,14 +110,16 @@ class QMixModel(XTModel):
 
     def _agent_nets(self, train):
         """fc1 and fc2 for the scene's training batch and the agent's variable table -> (batch, episode limit).  The
-        explore scene keeps a minimal training shape: only the one-step inference runs."""
+        explore scene keeps a minimal training shape: only the one-step inference and acting run.  Both nets also hold
+        the act_envs n_agents rows of acting."""
         H, A, n = self.rnn_hidden_dim, self.n_actions, self.n_agents
         B, L = (self.batch_size, self.fix_seq_length) if train else (1, 1)
         fc1_a = dict(input_dtype="float32", state_dim=(self.obs_shape,), scale=1.0,
                      layers=[("dense", "dense", "obs", dict(n=H, act="relu"))])
         fc2_a = dict(input_dtype="float32", state_dim=(H,), scale=1.0, layers=[("dense_1", "dense", "obs", dict(n=A, act=None))])
-        self.fc1 = Net(fc1_a, max_batch=B * (L + 1) * n, device=self.device)
-        self.fc2 = Net(fc2_a, max_batch=B * (L + 1) * n, device=self.device)
+        rows = max(B * (L + 1) * n, self.act_envs * n)
+        self.fc1 = Net(fc1_a, max_batch=rows, device=self.device)
+        self.fc2 = Net(fc2_a, max_batch=rows, device=self.device)
         gru = OrderedDict([("rnn/gru_cell/gates/kernel", (2 * H, 2 * H)), ("rnn/gru_cell/gates/bias", (2 * H,)),
                            ("rnn/gru_cell/candidate/kernel", (2 * H, H)), ("rnn/gru_cell/candidate/bias", (H,))])
         self.gru_off = _align(self.fc1.n_params)
@@ -152,13 +161,27 @@ class QMixModel(XTModel):
             net.params_changed()
 
     def _acting_state(self):
-        """The hidden state and the one-step inference's staging; the training buffers are made at first use."""
+        """The hidden state and the one-step inference's staging, the act_envs environment slots of act (hidden state,
+        last action, Philox step counter) and its staging; the training buffers are made at first use."""
         n, dev = self.n_agents, self.device
         self.hidden = torch.zeros(n, self.rnn_hidden_dim, dtype=torch.float32, device=dev)
         self._io = dict(obs1=torch.empty(n, self.obs_shape, dtype=torch.float32, device=dev),
                         q1=torch.empty(n, self.n_actions, dtype=torch.float32, device=dev))
+        N, A, i32 = self.act_envs, self.n_actions, dict(dtype=torch.int32, device=dev)
+        self.act_hidden = torch.zeros(N, n, self.rnn_hidden_dim, dtype=torch.float32, device=dev)
+        self.act_last = torch.full((N, n), -1, **i32)
+        self.act_counter = torch.zeros(N, dtype=torch.int64, device=dev)   # uint64 on the device
+        self._act_seed = None
+        self._act_io = dict(obs=torch.empty(N, n, self.act_obs_dim, dtype=torch.float32, device=dev), avail=torch.empty(N, n, A, **i32),
+                            reset=torch.empty(N, **i32), epsilon=torch.empty(N, dtype=torch.float64, device=dev),
+                            uniforms=torch.empty(N, 2, n, dtype=torch.float64, device=dev), actions=torch.empty(N, n, **i32))
         self._bufs = None
         self.net = self.fc1
+
+    @property
+    def act_obs_dim(self):
+        """The raw observation width act takes: obs_shape less the one-hots build_inputs appends."""
+        return self.obs_shape - (self.n_actions if self.obs_last_action else 0) - (self.n_agents if self.obs_agent_id else 0)
 
     def _init_set(self, flat, table):
         """TF 1.15 initialisers: glorot_uniform kernels (dense and GRUCell alike), zero biases except the GRU gates bias,
@@ -247,6 +270,87 @@ class QMixModel(XTModel):
         check(getattr(capi.lib(), self._native + "_infer")(self.handle, _ptr(self.explore), _ptr(io["obs1"]), _ptr(self.hidden),
                                                            _ptr(io["q1"]), 1 if self.use_graph else 0, stream_ptr()))
         return io["q1"].cpu().numpy().reshape(1, self.n_agents, self.n_actions)
+
+    def reset_act_state(self, envs=None):
+        """Zero hidden state and no last action for the environment slots `envs` (all when None); the Philox step counters
+        keep running, so a slot's next episode draws new numbers."""
+        idx = slice(None) if envs is None else torch.as_tensor(np.asarray(envs, np.int64).reshape(-1), device=self.device)
+        self.act_hidden[idx] = 0.0
+        self.act_last[idx] = -1
+
+    def _act_args(self, N, epsilon, uniforms):
+        """Checked n_envs, epsilon [N] and uniforms (None or [N, 2, n]) as host float64 arrays."""
+        if not 1 <= N <= self.act_envs:
+            raise ValueError("{} environments, act_envs is {}".format(N, self.act_envs))
+        eps = np.broadcast_to(np.asarray(epsilon, np.float64), (N,))
+        if uniforms is not None:
+            uniforms = np.asarray(uniforms, np.float64)
+            if uniforms.shape != (N, 2, self.n_agents):
+                raise ValueError("uniforms: shape {} != {}".format(uniforms.shape, (N, 2, self.n_agents)))
+        return eps, uniforms
+
+    def act(self, obs, avail, reset, epsilon, uniforms=None):
+        """One step of N <= act_envs environments (environment e in slot e) -> host int32 actions [N, n_agents]: obs
+        [N, n_agents, act_obs_dim], avail [N, n_agents, n_actions] integer action weights (0: unavailable), reset [N]
+        (True: the episode starts, zero hidden state and no last action), epsilon (scalar or [N]) and uniforms
+        ([N, 2, n_agents] float64, None: Philox draws on the device).  The agent inputs, the network and the selector run
+        on the device (act_device); ValueError before any launch for a wrong shape or dtype, a negative weight or a row
+        without an available action (the host selector's np.random.choice fails there too)."""
+        obs = np.asarray(obs)
+        N = obs.shape[0] if obs.ndim == 3 else -1
+        n, A = self.n_agents, self.n_actions
+        if obs.shape != (N, n, self.act_obs_dim):
+            raise ValueError("obs: shape {} is not [N, {}, {}]".format(obs.shape, n, self.act_obs_dim))
+        av = np.asarray(avail)
+        if av.shape != (N, n, A) or not (np.issubdtype(av.dtype, np.integer) or av.dtype == np.bool_):
+            raise ValueError("avail: integer [{}, {}, {}] expected, got {} {}".format(N, n, A, av.dtype, av.shape))
+        if np.any(av < 0) or np.any(av.astype(np.int64).sum(-1) <= 0):
+            raise ValueError("avail: every row needs non-negative weights and an available action")
+        if np.any(av > np.iinfo(np.int32).max):
+            raise ValueError("avail: weights must fit in int32")
+        rs = np.asarray(reset)
+        if rs.shape != (N,):
+            raise ValueError("reset: shape {} != ({},)".format(rs.shape, N))
+        eps, uniforms = self._act_args(N, epsilon, uniforms)
+        io = self._act_io
+        stage_h2d(io["obs"][:N], obs, np.float32)
+        stage_h2d(io["avail"][:N], av, np.int32)
+        stage_h2d(io["reset"][:N], rs.astype(bool), np.int32)
+        stage_h2d(io["epsilon"][:N], eps, np.float64)
+        if uniforms is not None:
+            stage_h2d(io["uniforms"][:N], uniforms, np.float64)
+        out = self.act_device(io["obs"][:N], io["avail"][:N], io["reset"][:N], io["epsilon"][:N],
+                              None if uniforms is None else io["uniforms"][:N], out=io["actions"][:N])
+        return out.cpu().numpy()
+
+    def act_device(self, obs, avail, reset, epsilon, uniforms=None, out=None):
+        """act on contiguous device tensors (obs float32 [N, n_agents, act_obs_dim], avail int32 [N, n_agents, n_actions],
+        reset int32 [N], epsilon float64 [N], uniforms float64 [N, 2, n_agents] or None) -> the int32 [N, n_agents] device
+        tensor `out` (default: the model's own, overwritten by the next call).  Shapes and dtypes are checked (ValueError);
+        the weights are not read on the host: a row without an available action gets an action that means nothing.  The
+        Q values stay in fc2's output tensor, rows e n_agents + a."""
+        N = obs.shape[0] if obs.dim() == 3 else -1
+        n, A = self.n_agents, self.n_actions
+        want = [("obs", obs, (N, n, self.act_obs_dim), torch.float32), ("avail", avail, (N, n, A), torch.int32),
+                ("reset", reset, (N,), torch.int32), ("epsilon", epsilon, (N,), torch.float64)]
+        if uniforms is not None:
+            want.append(("uniforms", uniforms, (N, 2, n), torch.float64))
+        if out is None:
+            out = self._act_io["actions"][:max(N, 0)]
+        want.append(("out", out, (N, n), torch.int32))
+        dev = self.act_hidden.device
+        for name, t, shape, dt in want:
+            if tuple(t.shape) != shape or t.dtype != dt or t.device != dev or not t.is_contiguous():
+                raise ValueError("{}: contiguous {} {} on {} expected, got {} {} on {}".format(name, dt, shape, dev, t.dtype,
+                                                                                           tuple(t.shape), t.device))
+        self._act_args(N, 0.0, None)
+        if uniforms is None and self._act_seed is None:
+            self._act_seed = int(self._init_rng.integers(0, 2 ** 63))
+        check(getattr(capi.lib(), self._native + "_act")(
+            self.handle, _ptr(self.explore), N, int(self.obs_last_action), int(self.obs_agent_id), _ptr(obs), _ptr(avail), _ptr(reset),
+            _ptr(epsilon), _ptr(uniforms), self._act_seed or 0, _ptr(self.act_counter), _ptr(self.act_hidden), _ptr(self.act_last),
+            _ptr(out), 1 if self.use_graph else 0, stream_ptr()))
+        return out
 
     # ---- training ---------------------------------------------------------------------------------------------------
     def _train_buffers(self):

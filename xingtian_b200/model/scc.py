@@ -92,6 +92,7 @@ class SCCModel(QMixModel):
         self.opt = self.critic_opt = None
         desc = capi.SccDesc()
         desc.batch, desc.episode_limit, desc.n_agents, desc.gamma, desc.gru_off = B, L, n, float(self.gamma), self.gru_off
+        desc.act_envs = self.act_envs
         if train:
             clip = self.actor_grad_norm_clip > 0      # scc_tf.py:421: both clips, or neither
             mode = capi.CLIP_PER_TENSOR if clip else capi.CLIP_NONE
@@ -148,6 +149,7 @@ class SCCModel(QMixModel):
         desc = capi.SccDesc()
         desc.batch, desc.episode_limit, desc.n_agents, desc.gru_off, desc.head_off = 1, 1, n, self.gru_off, head
         desc.n_groups, desc.group[0], desc.channel_merge, desc.mc_sample_times = 1, n, 1, 1
+        desc.act_envs = self.act_envs
         nets = (C.c_void_p * 1)(stub.handle.value)
         with torch.cuda.device(self.device):
             check(capi.lib().xtb_scc_create(self.fc1.handle, self.fc2.handle, nets, C.byref(desc), C.byref(self.handle)))
